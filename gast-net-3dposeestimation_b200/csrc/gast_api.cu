@@ -1017,7 +1017,7 @@ extern "C" size_t gast_train_workspace_bytes(gast_t* h, int32_t B, int32_t T, fl
   TrainState ts;
   ts.drop_p = dropout_p;
   if (train_forward(h, c, ts, nullptr, nullptr, B, T)) return 0;
-  if (train_backward(h, c, ts, nullptr)) return 0;
+  if (train_backward(h, c, ts, nullptr, nullptr)) return 0;
   return a.off + 512;
 }
 
@@ -1059,7 +1059,13 @@ extern "C" int gast_set_dropout_state(gast_t* h, void* dev_u64) {
 }
 
 extern "C" int gast_backward(gast_t* h, const float* dy, void* workspace, size_t workspace_bytes, void* stream) {
+  return gast_backward_input(h, dy, nullptr, 1, workspace, workspace_bytes, stream);
+}
+
+extern "C" int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_t param_grads, void* workspace,
+                                   size_t workspace_bytes, void* stream) {
   if (!h) return fail("gast_backward: null handle");
+  if (!dx && !param_grads) return fail("gast_backward_input: neither dx nor parameter gradients requested");
   size_t ti = h->trains.size();
   for (size_t i = 0; i < h->trains.size(); ++i)
     if (h->trains[i].first == workspace) ti = i;
@@ -1075,8 +1081,57 @@ extern "C" int gast_backward(gast_t* h, const float* dy, void* workspace, size_t
   Lookup L{h};
   TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
   c.tc_slot = 1024;                         // the backward's GEMMs follow the forward's in the operand-copy table
-  if (train_backward(h, c, ts, dy)) return 1;
+  c.pgrad = param_grads != 0;
+  if (train_backward(h, c, ts, dy, dx)) return 1;
   if (a.off > workspace_bytes) return fail("gast_backward: workspace overrun");
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---- eval-mode backward: a frozen-BatchNorm training forward recomputes the activations from x, then the training
+// backward runs on them.  The inference forward stays as it is; nothing is held between forward and backward.
+static size_t eval_backward_bytes(gast_handle* h, int B, int T, int strided_now, bool pgrad) {
+  if (!h || train_check(h)) return 0;
+  Arena a{nullptr, 0, 0, true};
+  Lookup L{h};
+  TCtx c{h, nullptr, &a, &L, h->cfg.num_joints, true};
+  c.pgrad = pgrad;
+  TrainState ts;
+  ts.frozen = true; ts.sn = strided_now ? 1 : 0;
+  if (train_forward(h, c, ts, nullptr, nullptr, B, T)) return 0;
+  if (train_backward(h, c, ts, nullptr, nullptr)) return 0;
+  return a.off + 512;
+}
+
+extern "C" size_t gast_eval_backward_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now) {
+  return eval_backward_bytes(h, B, T, strided_now, true);
+}
+
+extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads, int32_t B,
+                                  int32_t T, int32_t strided_now, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h) return fail("gast_eval_backward: null handle");
+  if (train_check(h)) return 1;
+  if (B <= 0 || T <= 0) return fail("gast_eval_backward: empty batch (B=%d T=%d)", B, T);
+  if (!x || !dy) return fail("gast_eval_backward: x and dy must be device pointers");
+  if (!dx && !param_grads) return fail("gast_eval_backward: neither dx nor parameter gradients requested");
+  const size_t need = eval_backward_bytes(h, B, T, strided_now, param_grads != 0);
+  if (need == 0) return 1;
+  if (!workspace || workspace_bytes < need)
+    return fail("gast_eval_backward: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CUDA_OK(cudaSetDevice(h->cfg.device));
+  uintptr_t wsb = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255;
+  Arena a{reinterpret_cast<char*>(wsb), workspace_bytes, 0, false};
+  Lookup L{h};
+  TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
+  c.pgrad = param_grads != 0;
+  TrainState ts;
+  ts.frozen = true; ts.sn = strided_now ? 1 : 0;
+  h->launches = 0;
+  if (train_forward(h, c, ts, x, nullptr, B, T)) return 1;
+  c.tc_slot = 1024;
+  if (train_backward(h, c, ts, dy, dx)) return 1;
+  if (a.off > workspace_bytes) return fail("gast_eval_backward: workspace overrun");
   CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -8,6 +8,9 @@
 // Dense contractions run on the FFMA GEMM kernel (exact fp32); the frame-mapped operands of the
 // temporal stages are gathered exactly as in inference.  Both schedules train: the strided one of
 // SpatioTemporalModelOptimized1f (main.py:166-170) and the dilated one of SpatioTemporalModel (main.py:171-175).
+// The same forward in frozen mode (TrainState::frozen: BatchNorm on the running statistics, no dropout, the inference
+// schedule) recomputes the activations for the eval-mode backward; the backward also writes dL/dx, and skips every
+// parameter-gradient kernel when only dL/dx is wanted (TCtx::pgrad).
 #pragma once
 
 // ---------------------------------------------------------------------------------------------
@@ -15,6 +18,9 @@ struct TCtx {
   gast_handle* h; cudaStream_t st; Arena* a; Lookup* L; int J;
   bool dry;   // sizing pass: no launches
   int tc_slot = 0;   // next slot of the handle's table of per-GEMM tensor-core operand copies (train_tcw)
+  // backward: false = input gradient only (every parameter frozen): no weight-gradient contraction, no parameter-
+  // gradient kernel, and no gradient buffer has to be bound
+  bool pgrad = true;
   float* fl(size_t n) { return a->take(n); }
   double* dbl(size_t n) { return reinterpret_cast<double*>(a->take(2 * n)); }
   unsigned char* bytes(size_t n) { return reinterpret_cast<unsigned char*>(a->take((n + 3) / 4)); }
@@ -25,6 +31,15 @@ static float* grad_ptr(gast_handle* h, const std::string& key, int64_t numel) {
   if (it == h->grads.end()) { fail("gradient buffer for '%s' is not bound", key.c_str()); return nullptr; }
   if (it->second.numel != numel) { fail("gradient buffer '%s' has the wrong size", key.c_str()); return nullptr; }
   return reinterpret_cast<float*>(it->second.ptr);
+}
+
+// *out = the bound gradient buffer of `key`, or null when no parameter gradient is computed (sizing pass, input-only
+// backward).  false: a wanted buffer is missing or has the wrong size.
+static bool want_grad(TCtx& c, const std::string& key, int64_t numel, float** out) {
+  *out = nullptr;
+  if (c.dry || !c.pgrad) return true;
+  *out = grad_ptr(c.h, key, numel);
+  return *out != nullptr;
 }
 
 // Tensor-core operand copies of one training GEMM's weight matrix (forward: the raw weights, backward: their transposes):
@@ -73,6 +88,7 @@ static long long pad32(long long m) { return (m + 31) / 32 * 32; }
 // dW[N][K] = dZ[M][N]^T . A[M][K]: split over the rows (wgrad_tn_kernel) + fixed-order reduction of the partials
 static int dense_tn(TCtx& c, const float* dZ, int lddz, const float* A, int lda, long long M, int N, int K, float* dW,
                     int lddw) {
+  if (!c.pgrad) return 0;   // every use is a parameter gradient
   const int tiles = (int)(cdiv(N, WG_T) * cdiv(K, WG_T));
   // enough CTAs for two waves of the machine, at least 256 rows per split
   long long S = std::max<long long>(1, std::min<long long>((M + 255) / 256, (2LL * c.h->sm_count + tiles - 1) / tiles));
@@ -107,12 +123,13 @@ static int dense_nn(TCtx& c, const float* dZ, int lddz, const float* W, int ldw,
   return dense_nt(c, dz, ld, Wt, M, K, Np, dA, ldda);
 }
 
-// ---- BatchNorm, training mode -----------------------------------------------------------------
+// ---- BatchNorm, training mode (batch statistics) or frozen (running statistics: ts.frozen) ----------------
 static int bn_fwd(TCtx& c, BnSave& s, const std::string& prefix, const float* Z, int ldz, long long M, int N, int relu,
                   float drop_p, TrainState& ts, const float* res, int ldres, RowMap rmap, float* Y, int ldy) {
-  s.prefix = prefix; s.Z = Z; s.ldz = ldz; s.M = M; s.N = N; s.relu = relu;
+  s.prefix = prefix; s.Z = Z; s.ldz = ldz; s.M = M; s.N = N; s.relu = relu; s.frozen = ts.frozen;
   s.mean = c.fl(N); s.invstd = c.fl(N);
-  double* sums = c.dbl(2 * (size_t)N);
+  double* sums = ts.frozen ? nullptr : c.dbl(2 * (size_t)N);
+  if (ts.frozen) drop_p = 0.f;   // eval semantics whatever the module's dropout
   unsigned char* keep = nullptr;
   s.kscale = 1.f;
   if (drop_p > 0.f) { keep = c.bytes((size_t)M * N); s.kscale = 1.f / (1.f - drop_p); }
@@ -122,10 +139,14 @@ static int bn_fwd(TCtx& c, BnSave& s, const std::string& prefix, const float* Z,
   float* rm = const_cast<float*>(c.L->get(prefix + "running_mean", N));
   float* rv = const_cast<float*>(c.L->get(prefix + "running_var", N));
   if (!c.L->ok) return 1;
-  cudaMemsetAsync(sums, 0, sizeof(double) * 2 * N, c.st);
-  dim3 grid(cdiv(N, 32), (unsigned)std::min<long long>(256, (M + 7) / 8));
-  col_stats_kernel<<<grid, 256, 0, c.st>>>(Z, M, N, ldz, sums, sums + N);
-  bn_finalize_kernel<<<cdiv(N, 128), 128, 0, c.st>>>(sums, sums + N, M, N, s.mean, s.invstd, rm, rv, 0.1f);
+  if (ts.frozen) {
+    bn_running_kernel<<<cdiv(N, 128), 128, 0, c.st>>>(rm, rv, N, s.mean, s.invstd);
+  } else {
+    cudaMemsetAsync(sums, 0, sizeof(double) * 2 * N, c.st);
+    dim3 grid(cdiv(N, 32), (unsigned)std::min<long long>(256, (M + 7) / 8));
+    col_stats_kernel<<<grid, 256, 0, c.st>>>(Z, M, N, ldz, sums, sums + N);
+    bn_finalize_kernel<<<cdiv(N, 128), 128, 0, c.st>>>(sums, sums + N, M, N, s.mean, s.invstd, rm, rv, 0.1f);
+  }
   if (keep) {
     dropout_mask_kernel<<<cdiv(M * N, 256), 256, 0, c.st>>>(keep, M * N, drop_p, ts.seed + 0x51ED270B * (++ts.drop_ctr), c.h->dropout_state);
   }
@@ -134,20 +155,29 @@ static int bn_fwd(TCtx& c, BnSave& s, const std::string& prefix, const float* Z,
   return 0;
 }
 
-// dZ from dY; writes the weight/bias gradients of this BatchNorm
+// dZ from dY; writes the weight/bias gradients of this BatchNorm (c.pgrad).  The column sums dgamma = sum dY'.xhat,
+// dbeta = sum dY' are those gradients; batch statistics also need them for dZ, running statistics do not.
 static int bn_bwd(TCtx& c, const BnSave& s, const float* dY, int lddy, float* dZ, int lddz) {
-  double* sums = c.dbl(2 * (size_t)s.N);
+  double* sums = (!s.frozen || c.pgrad) ? c.dbl(2 * (size_t)s.N) : nullptr;
+  float *gw, *gb;
+  if (!want_grad(c, s.prefix + "weight", s.N, &gw) || !want_grad(c, s.prefix + "bias", s.N, &gb)) return 1;
   if (c.dry) return 0;
-  float* gw = grad_ptr(c.h, s.prefix + "weight", s.N);
-  float* gb = grad_ptr(c.h, s.prefix + "bias", s.N);
-  if (!gw || !gb) return 1;
-  cudaMemsetAsync(sums, 0, sizeof(double) * 2 * s.N, c.st);
-  dim3 grid(cdiv(s.N, 32), (unsigned)std::min<long long>(256, (s.M + 7) / 8));
-  bn_bwd_reduce_kernel<<<grid, 256, 0, c.st>>>(dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma, s.beta, s.relu, s.keep,
-                                              s.kscale, s.M, s.N, sums, sums + s.N);
-  bn_bwd_apply_kernel<<<cdiv(s.M * s.N, 256), 256, 0, c.st>>>(dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma, s.beta,
-                                                            s.relu, s.keep, s.kscale, s.M, s.N, sums, sums + s.N, dZ,
-                                                            lddz, gw, gb);
+  if (sums) {
+    cudaMemsetAsync(sums, 0, sizeof(double) * 2 * s.N, c.st);
+    dim3 grid(cdiv(s.N, 32), (unsigned)std::min<long long>(256, (s.M + 7) / 8));
+    bn_bwd_reduce_kernel<<<grid, 256, 0, c.st>>>(dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma, s.beta, s.relu, s.keep,
+                                                s.kscale, s.M, s.N, sums, sums + s.N);
+  }
+  const double* dg = sums;
+  const double* db = sums ? sums + s.N : nullptr;
+  if (s.frozen)
+    bn_bwd_apply_kernel<true><<<cdiv(s.M * s.N, 256), 256, 0, c.st>>>(dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma,
+                                                                      s.beta, s.relu, s.keep, s.kscale, s.M, s.N, dg, db,
+                                                                      dZ, lddz, gw, gb);
+  else
+    bn_bwd_apply_kernel<false><<<cdiv(s.M * s.N, 256), 256, 0, c.st>>>(dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma,
+                                                                       s.beta, s.relu, s.keep, s.kscale, s.M, s.N, dg, db,
+                                                                       dZ, lddz, gw, gb);
   return 0;
 }
 
@@ -240,15 +270,15 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
   if (bn_bwd(c, b.bnbc, dOut, 2 * C, dZbc, 2 * C)) return 1;
   float* Acat = c.fl((size_t)M * 3 * C);
   float* dAcat = c.fl((size_t)M * 3 * C);
-  if (!c.dry) {
+  if (!c.dry && c.pgrad) {
     copy2d_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(b.X, C, Acat, 3 * C, M, C, 0);
     copy2d_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(b.L, C, Acat + C, 3 * C, M, C, 0);
     copy2d_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(b.Gl, C, Acat + 2 * C, 3 * C, M, C, 0);
   }
   {
     const float* w = c.dry ? nullptr : c.L->get(P + "cat_conv.weight", (int64_t)2 * C * 3 * C);
-    float* gw = c.dry ? nullptr : grad_ptr(h, P + "cat_conv.weight", (int64_t)2 * C * 3 * C);
-    if (!c.dry && (!c.L->ok || !gw)) return 1;
+    float* gw;
+    if (!want_grad(c, P + "cat_conv.weight", (int64_t)2 * C * 3 * C, &gw) || (!c.dry && !c.L->ok)) return 1;
     if (dense_tn(c, dZbc, 2 * C, Acat, 3 * C, M, 2 * C, 3 * C, gw, 3 * C)) return 1;
     if (dense_nn(c, dZbc, 2 * C, w, 3 * C, M, 2 * C, 3 * C, dAcat, 3 * C)) return 1;
   }
@@ -259,8 +289,8 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
   float* dY = c.fl((size_t)M * C);
   {
     const float* w = c.dry ? nullptr : c.L->get(gp + "cat_conv.weight", (int64_t)C * C);
-    float* gw = c.dry ? nullptr : grad_ptr(h, gp + "cat_conv.weight", (int64_t)C * C);
-    if (!c.dry && (!c.L->ok || !gw)) return 1;
+    float* gw;
+    if (!want_grad(c, gp + "cat_conv.weight", (int64_t)C * C, &gw) || (!c.dry && !c.L->ok)) return 1;
     if (dense_tn(c, dZgc, C, b.Y, C, M, C, C, gw, C)) return 1;
     if (dense_nn(c, dZgc, C, w, C, M, C, C, dY, C)) return 1;
   }
@@ -277,14 +307,16 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
   if (!c.dry) {
     att_mix_bwd_kernel<<<(unsigned)F, 256, sizeof(float) * 16 * J * J, c.st>>>(dY, C, b.G, C, b.AB, bc.Ck, J, 4, C / 4, dG,
                                                                                C, dab, dCkp);
-    col_sum_det_kernel<<<cdiv(4 * J * J, 32), 256, 0, c.st>>>(dCkp, F, 4 * J * J, dCk);
-    cudaMemsetAsync(dsum, 0, sizeof(double) * (C + 8), c.st);
-    dim3 g1(cdiv(C, 32), (unsigned)std::min<long long>(256, (M + 7) / 8));
-    col_sum_kernel<<<g1, 256, 0, c.st>>>(dG, M, C, C, dsum);
-    dim3 g2(1, (unsigned)std::min<long long>(256, (M + 7) / 8));
-    col_sum_kernel<<<g2, 256, 0, c.st>>>(dab, M, 8, 8, dsum + C);
-    d2f_kernel<<<cdiv(C, 128), 128, 0, c.st>>>(dsum, dbg, C);
-    d2f_kernel<<<1, 32, 0, c.st>>>(dsum + C, dcab, 8);
+    if (c.pgrad) {
+      col_sum_det_kernel<<<cdiv(4 * J * J, 32), 256, 0, c.st>>>(dCkp, F, 4 * J * J, dCk);
+      cudaMemsetAsync(dsum, 0, sizeof(double) * (C + 8), c.st);
+      dim3 g1(cdiv(C, 32), (unsigned)std::min<long long>(256, (M + 7) / 8));
+      col_sum_kernel<<<g1, 256, 0, c.st>>>(dG, M, C, C, dsum);
+      dim3 g2(1, (unsigned)std::min<long long>(256, (M + 7) / 8));
+      col_sum_kernel<<<g2, 256, 0, c.st>>>(dab, M, 8, 8, dsum + C);
+      d2f_kernel<<<cdiv(C, 128), 128, 0, c.st>>>(dsum, dbg, C);
+      d2f_kernel<<<1, 32, 0, c.st>>>(dsum + C, dcab, 8);
+    }
   }
   if (dense_tn(c, dG, C, b.X, C, M, C, C, dWg, C)) return 1;
   if (dense_nn(c, dG, C, bc.Wg, C, M, C, C, dXg, C)) return 1;
@@ -295,7 +327,7 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
     rowdot_bwd_x_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(dab, bc.U, 8, M, C, dXg, C);
     add_inplace_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(dX, dXg, M * C);
     const int Cg = C / 4;
-    for (int hd = 0; hd < 4; ++hd) {
+    for (int hd = 0; hd < (c.pgrad ? 4 : 0); ++hd) {
       const std::string hp = gp + "attentions." + std::to_string(hd) + ".";
       float* ggw = grad_ptr(h, hp + "g.weight", (int64_t)Cg * C);
       float* ggb = grad_ptr(h, hp + "g.bias", Cg);
@@ -324,8 +356,8 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
   float* dXY = c.fl((size_t)M * 2 * C);
   {
     const float* w = c.dry ? nullptr : c.L->get(lp + "cat_conv.weight", (int64_t)C * 2 * C);
-    float* gw = c.dry ? nullptr : grad_ptr(h, lp + "cat_conv.weight", (int64_t)C * 2 * C);
-    if (!c.dry && (!c.L->ok || !gw)) return 1;
+    float* gw;
+    if (!want_grad(c, lp + "cat_conv.weight", (int64_t)C * 2 * C, &gw) || (!c.dry && !c.L->ok)) return 1;
     if (dense_tn(c, dZlc, C, b.XY, 2 * C, M, C, 2 * C, gw, 2 * C)) return 1;
     if (dense_nn(c, dZlc, C, w, 2 * C, M, C, 2 * C, dXY, 2 * C)) return 1;
   }
@@ -339,13 +371,14 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
     float* dA = c.fl((size_t)h->nnz[m] * C);
     const int dsplit = (int)std::max<long long>(1, std::min<long long>(32, F / 32));   // frame ranges of semch_dcoef_kernel
     double* dpart = c.dbl((size_t)dsplit * h->nnz[m] * C);
-    if (c.dry) continue;
     const std::string g = lp + (m == 0 ? "gcn_sym." : "gcn_con.");
-    float* ge = grad_ptr(h, g + "e", (int64_t)C * h->nnz[m]);
-    if (!ge) return 1;
+    float* ge;
+    if (!want_grad(c, g + "e", (int64_t)C * h->nnz[m], &ge)) return 1;
+    if (c.dry) continue;
     NbrRows nr = nbr_rows(h->nbr[m], J);
     semch_mix_bwd_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(dS + m * C, 2 * C, b.coefA[m], h->nbr[m], nr, h->nnz[m], J, F,
                                                             C, dH + m * 2 * C, 4 * C);
+    if (!c.pgrad) continue;
     semch_dcoef_kernel<<<dim3(cdiv((long long)h->nnz[m] * C, 128), dsplit), 128, 0, c.st>>>(
         dS + m * C, 2 * C, b.H + m * 2 * C, 4 * C, h->nbr[m], nr, h->nnz[m], J, F, C, dpart);
     semch_dcoef_reduce_kernel<<<cdiv((long long)h->nnz[m] * C, 128), 128, 0, c.st>>>(dpart, dsplit, h->nnz[m] * C, dA);
@@ -355,7 +388,7 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
   if (dense_nn(c, dH, 4 * C, b.Wst, C, M, 4 * C, C, dXl, C)) return 1;
   if (!c.dry) {
     add_inplace_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(dX, dXl, M * C);
-    for (int m = 0; m < 2; ++m) {
+    for (int m = 0; m < (c.pgrad ? 2 : 0); ++m) {
       const std::string g = lp + (m == 0 ? "gcn_sym." : "gcn_con.");
       float* gW = grad_ptr(h, g + "W", (int64_t)2 * C * C);
       if (!gW) return 1;
@@ -366,14 +399,17 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
 }
 
 // ---- whole model ---------------------------------------------------------------------------------
+// y may be null (the eval backward recomputes the activations only)
 static int train_forward(gast_handle* h, TCtx& c, TrainState& ts, const float* x, float* y, int B, int T) {
   const gast_cfg& cf = h->cfg;
   const int J = c.J, C = cf.channels, L = cf.num_stages, Fin = cf.in_features, k0 = cf.filter_widths[0];
   // schedule = the handle's own: strided for SpatioTemporalModelOptimized1f (main.py:166-170), dilated (or the
   // dense ablation) for SpatioTemporalModel (main.py:171-175, `--disable-optimizations` / stride > 1).  Batch
   // statistics are taken over every position the reference computes, so a dilated model never runs the
-  // needed-only schedule in training.
-  const int sn = cf.strided ? 1 : 0;
+  // needed-only schedule in training.  Frozen BatchNorm makes the positions independent: the eval-mode forward
+  // takes the schedule gast_forward takes (ts.sn), and a dilated model fed one receptive field computes only
+  // the positions its output needs.
+  const int sn = ts.frozen ? ts.sn : (cf.strided ? 1 : 0);
   Geometry g;
   if (geometry(h, T, sn, &g)) return 1;
   ts.B = B; ts.T = T; ts.T0 = g.T0; ts.s0 = g.s0; ts.x = x;
@@ -445,7 +481,7 @@ static int train_forward(gast_handle* h, TCtx& c, TrainState& ts, const float* x
     F = Fn; Tp = Tn;
   }
   ts.last = cur; ts.Flast = F;
-  if (!c.dry) {
+  if (!c.dry && y) {
     const int Cl = C << L;
     const float* ws = c.L->get("shrink.weight", (int64_t)3 * Cl);
     if (!c.L->ok) return 1;
@@ -454,7 +490,8 @@ static int train_forward(gast_handle* h, TCtx& c, TrainState& ts, const float* x
   return 0;
 }
 
-static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* dy) {
+// dy -> the parameter gradients (c.pgrad) and dL/dx into dx (B,T,J,F; may be null)
+static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* dy, float* dx) {
   const gast_cfg& cf = h->cfg;
   const int J = c.J, C = cf.channels, L = cf.num_stages, Fin = cf.in_features, k0 = cf.filter_widths[0];
   const int Cl = C << L;
@@ -463,10 +500,10 @@ static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* 
   float* dcur = c.fl((size_t)F * J * Cl);
   if (!c.dry) {
     const float* ws = c.L->get("shrink.weight", (int64_t)3 * Cl);
-    float* gws = grad_ptr(h, "shrink.weight", (int64_t)3 * Cl);
-    if (!c.L->ok || !gws) return 1;
+    float* gws;
+    if (!want_grad(c, "shrink.weight", (int64_t)3 * Cl, &gws) || !c.L->ok) return 1;
     shrink_bwd_x_kernel<<<cdiv(F * J * Cl, 256), 256, 0, c.st>>>(dy, ws, F * J, Cl, dcur);
-    shrink_bwd_w_kernel<<<cdiv(Cl, 32), dim3(32, SBW_RG), 0, c.st>>>(dy, ts.last, F * J, Cl, gws);
+    if (gws) shrink_bwd_w_kernel<<<cdiv(Cl, 32), dim3(32, SBW_RG), 0, c.st>>>(dy, ts.last, F * J, Cl, gws);
   }
   for (int i = L - 1; i >= 1; --i) {
     StageSave& s = ts.stages[i - 1];
@@ -491,22 +528,22 @@ static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* 
     {
       const std::string k1s = "layers_conv." + std::to_string(2 * s.idx + 1) + ".weight";
       const float* w1 = c.dry ? nullptr : c.L->get(k1s, (int64_t)Cw * Cw);
-      float* gw1 = c.dry ? nullptr : grad_ptr(h, k1s, (int64_t)Cw * Cw);
-      if (!c.dry && (!c.L->ok || !gw1)) return 1;
+      float* gw1;
+      if (!want_grad(c, k1s, (int64_t)Cw * Cw, &gw1) || (!c.dry && !c.L->ok)) return 1;
       if (dense_tn(c, dZ2, Cw, s.Hh, Cw, Mn, Cw, Cw, gw1, Cw)) return 1;
       if (dense_nn(c, dZ2, Cw, w1, Cw, Mn, Cw, Cw, dHh, Cw)) return 1;
     }
     if (bn_bwd(c, s.bnA, dHh, Cw, dZ1, Cw)) return 1;
     ASeg sg; sg.base = s.X; sg.ld = Cw; sg.K = s.taps * Cw; sg.Kc = Cw; sg.tap_stride = (long long)s.dil * J * Cw;
     sg.map = s.tapmap;
-    if (!c.dry) seg_gather_kernel<<<cdiv(Mn * sg.K, 256), 256, 0, c.st>>>(sg, J, s.Fout, Xcol, s.taps * Cw, 0);
+    if (!c.dry && c.pgrad) seg_gather_kernel<<<cdiv(Mn * sg.K, 256), 256, 0, c.st>>>(sg, J, s.Fout, Xcol, s.taps * Cw, 0);
     if (dense_tn(c, dZ1, Cw, Xcol, s.taps * Cw, Mn, Cw, s.taps * Cw, dWt, s.taps * Cw)) return 1;
     if (dense_nn(c, dZ1, Cw, s.Wt, s.taps * Cw, Mn, Cw, s.taps * Cw, dXcol, s.taps * Cw)) return 1;
+    float* gw0;
+    if (!want_grad(c, "layers_conv." + std::to_string(2 * s.idx) + ".weight", (int64_t)Cw * Cw * s.taps, &gw0)) return 1;
     if (!c.dry) {
-      const std::string k0s = "layers_conv." + std::to_string(2 * s.idx) + ".weight";
-      float* gw0 = grad_ptr(h, k0s, (int64_t)Cw * Cw * s.taps);
-      if (!gw0) return 1;
-      conv_wgrad_relayout_kernel<<<cdiv((long long)Cw * Cw * s.taps, 256), 256, 0, c.st>>>(dWt, Cw, Cw, s.taps, s.taps * Cw, gw0);
+      if (gw0)
+        conv_wgrad_relayout_kernel<<<cdiv((long long)Cw * Cw * s.taps, 256), 256, 0, c.st>>>(dWt, Cw, Cw, s.taps, s.taps * Cw, gw0);
       ASeg dsg = sg; dsg.base = dXin;
       seg_scatter_add_kernel<<<cdiv(Mn * dsg.K, 256), 256, 0, c.st>>>(dsg, J, s.Fout, dXcol, s.taps * Cw, 0);
     }
@@ -528,15 +565,16 @@ static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* 
   float* dxin = c.fl((size_t)Min * Fin);
   if (dense_tn(c, dZ0, C, ts.Acol, KP, M0, C, KP, dWe8, KP)) return 1;
   if (dense_nn(c, dZ0, C, ts.We8, KP, M0, C, KP, dAcol, KP)) return 1;
+  float* gwe;
+  if (!want_grad(c, "expand_conv.weight", (int64_t)C * Fin * k0, &gwe)) return 1;
   if (!c.dry) {
-    float* gwe = grad_ptr(h, "expand_conv.weight", (int64_t)C * Fin * k0);
-    if (!gwe) return 1;
-    conv_wgrad_relayout_kernel<<<cdiv((long long)C * Fin * k0, 256), 256, 0, c.st>>>(dWe8, C, Fin, k0, KP, gwe);
+    if (gwe) conv_wgrad_relayout_kernel<<<cdiv((long long)C * Fin * k0, 256), 256, 0, c.st>>>(dWe8, C, Fin, k0, KP, gwe);
     cudaMemsetAsync(dxbn, 0, sizeof(float) * (size_t)Min * Fin, c.st);
     ASeg sg; sg.base = dxbn; sg.ld = Fin; sg.K = k0 * Fin; sg.Kc = Fin; sg.tap_stride = (long long)J * Fin;
     sg.map = RowMap{ts.T0, ts.T, ts.s0, 0};
     seg_scatter_add_kernel<<<cdiv(M0 * sg.K, 256), 256, 0, c.st>>>(sg, J, F0, dAcol, KP, 0);
   }
-  if (bn_bwd(c, ts.bnin, dxbn, Fin, dxin, Fin)) return 1;
+  // init_bn: dx = dxbn . gamma . invstd (frozen), the batch-statistics adjoint otherwise
+  if (bn_bwd(c, ts.bnin, dxbn, Fin, dx ? dx : dxin, Fin)) return 1;
   return 0;
 }

@@ -54,6 +54,15 @@ __global__ void bn_finalize_kernel(const double* __restrict__ sum, const double*
   }
 }
 
+// frozen (eval-mode) BatchNorm: mean / invstd from the running statistics, which are only read
+__global__ void bn_running_kernel(const float* __restrict__ running_mean, const float* __restrict__ running_var, int N,
+                                  float* __restrict__ mean, float* __restrict__ invstd) {
+  int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  mean[n] = running_mean[n];
+  invstd[n] = (float)(1.0 / sqrt((double)running_var[n] + (double)BN_EPS));
+}
+
 // Y = [res +] drop( relu( (Z-mean)*invstd*gamma + beta ) )      (relu / res / drop optional)
 // res rows follow a frame map (residual slice of the temporal stage, gast_net.py:243)
 __global__ void bn_apply_kernel(const float* __restrict__ Z, int ldz, const float* __restrict__ mean,
@@ -107,7 +116,10 @@ __global__ void bn_bwd_reduce_kernel(const float* __restrict__ dY, int lddy, con
   }
 }
 
-// dZ = gamma*invstd*(dYhat - dbeta/M - xhat*dgamma/M); also writes the float parameter grads
+// dZ = gamma*invstd*(dYhat - dbeta/M - xhat*dgamma/M); also writes the float parameter grads (when g_gamma / g_beta are
+// given).  FROZEN (running statistics, eval mode): mean / invstd do not depend on Z, so dZ = gamma*invstd*dYhat, and
+// dgamma / dbeta are read only for the parameter grads (null in an input-only backward).
+template <bool FROZEN>
 __global__ void bn_bwd_apply_kernel(const float* __restrict__ dY, int lddy, const float* __restrict__ Z, int ldz,
                                     const float* __restrict__ mean, const float* __restrict__ invstd,
                                     const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
@@ -124,8 +136,12 @@ __global__ void bn_bwd_apply_kernel(const float* __restrict__ dY, int lddy, cons
   float d = dY[m * lddy + n];
   if (keep) d = keep[idx] ? d * keep_scale : 0.f;
   if (relu && !(xh * ga + beta[n] > 0.f)) d = 0.f;
-  const float invM = 1.f / (float)M;
-  dZ[m * lddz + n] = ga * is * (d - (float)dbeta[n] * invM - xh * (float)dgamma[n] * invM);
+  if (FROZEN) {
+    dZ[m * lddz + n] = ga * is * d;
+  } else {
+    const float invM = 1.f / (float)M;
+    dZ[m * lddz + n] = ga * is * (d - (float)dbeta[n] * invM - xh * (float)dgamma[n] * invM);
+  }
   if (m == 0) {
     if (g_gamma) g_gamma[n] = (float)dgamma[n];
     if (g_beta) g_beta[n] = (float)dbeta[n];

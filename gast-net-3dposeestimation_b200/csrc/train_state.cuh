@@ -11,6 +11,7 @@ struct BnSave {
   float* mean = nullptr; float* invstd = nullptr;
   const float* gamma = nullptr; const float* beta = nullptr;
   int relu = 0; const unsigned char* keep = nullptr; float kscale = 1.f;
+  bool frozen = false;   // mean / invstd are the running statistics (eval-mode BatchNorm)
   std::string prefix;
 };
 
@@ -33,6 +34,9 @@ struct StageSave {
 
 struct TrainState {
   bool valid = false;
+  // frozen: the eval-mode forward (model.eval()) -- BatchNorm on the running statistics, which stay untouched, no
+  // dropout, and the schedule `sn` of gast_forward (strided_now); otherwise train mode on the handle's own schedule
+  bool frozen = false; int sn = 0;
   int B = 0, T = 0, T0 = 0, s0 = 1;   // s0: stride of the expand conv (filter width when strided, else 1)
   const float* x = nullptr;
   float *xbn = nullptr, *Acol = nullptr, *We8 = nullptr, *Z0 = nullptr, *act0 = nullptr;

@@ -18,7 +18,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_receptive_field', 'gast_workspace_bytes', 'gast_forward', 'gast_forward_mpjpe',
            'gast_last_launch_count', 'gast_last_tc_launch_count', 'gast_set_timing',
            'gast_get_timings', 'gast_set_gemm_core', 'gast_debug_gemm', 'gast_bind_grads',
-           'gast_train_workspace_bytes', 'gast_forward_train', 'gast_backward', 'gast_set_dropout_state', 'gast_tta_prepare', 'gast_tta_merge',
+           'gast_train_workspace_bytes', 'gast_forward_train', 'gast_backward', 'gast_backward_input',
+           'gast_eval_backward_workspace_bytes', 'gast_eval_backward', 'gast_set_dropout_state', 'gast_tta_prepare', 'gast_tta_merge',
            'gast_stream_state_bytes', 'gast_stream_workspace_bytes', 'gast_stream_push',
            'gast_chunk_gather', 'gast_keypoints_convert', 'gast_normalize_screen', 'gast_camera_to_world',
            'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_adam_chunk', 'gast_adam_step',
@@ -92,6 +93,12 @@ def load():
     lib.gast_forward_train.restype = C.c_int
     lib.gast_backward.argtypes = [vp, vp, vp, C.c_size_t, vp]
     lib.gast_backward.restype = C.c_int
+    lib.gast_backward_input.argtypes = [vp, vp, vp, C.c_int32, vp, C.c_size_t, vp]
+    lib.gast_backward_input.restype = C.c_int
+    lib.gast_eval_backward_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32]
+    lib.gast_eval_backward_workspace_bytes.restype = C.c_size_t
+    lib.gast_eval_backward.argtypes = [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.c_size_t, vp]
+    lib.gast_eval_backward.restype = C.c_int
     lib.gast_set_dropout_state.argtypes = [vp, vp]
     lib.gast_set_dropout_state.restype = C.c_int
     lib.gast_stream_state_bytes.argtypes = [vp, C.c_int32]

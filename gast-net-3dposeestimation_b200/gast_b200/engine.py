@@ -269,11 +269,9 @@ class _TrainFn(torch.autograd.Function):
     def backward(ctx, dy):
         handle, ws, names, params = ctx.handle, ctx.ws, ctx.names, ctx.params
         lib = handle.lib
-        total = sum(p.numel() for p in params)
         n = len(params)
-        keys = (C.c_char_p * n)()
-        ptrs = (C.c_void_p * n)()
-        numel = (C.c_int64 * n)()
+        need_x = ctx.needs_input_grad[2]
+        need_p = any(ctx.needs_input_grad[4:])
         # A trainer that owns the gradient buffers (module._gast_direct_grads, set by gast_b200.trainer: every .grad is
         # a view of its flat all-reduce buffer and one backward runs per step) gets the gradients WRITTEN straight into
         # them: autograd's AccumulateGrad would otherwise launch one add per parameter (166 per step at 27f/128ch,
@@ -281,25 +279,84 @@ class _TrainFn(torch.autograd.Function):
         direct = ctx.direct and all(p.is_leaf and p.grad is not None and p.grad.is_contiguous() and
                                     p.grad.dtype == torch.float32 and p.grad.device == p.device and
                                     p.grad.shape == p.shape for p in params)
-        flat = None if direct else torch.empty(total, dtype=torch.float32, device=ctx.dev)
-        views, off = [], 0
-        for i, (k, p) in enumerate(zip(names, params)):
-            v = p.grad if direct else flat[off:off + p.numel()].view_as(p)
-            views.append(v)
-            keys[i] = k.encode()
-            ptrs[i] = v.data_ptr()
-            numel[i] = p.numel()
-            off += p.numel()
         dy = dy.contiguous()
+        dx = torch.empty_like(ctx.x) if need_x else None
         with torch.cuda.device(ctx.dev):
-            _check(lib.gast_bind_grads(handle.h, n, keys, ptrs, numel), 'gast_bind_grads')
-            _check(lib.gast_backward(handle.h, C.c_void_p(dy.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
-                                     C.c_void_p(_stream(ctx.dev))), 'gast_backward')
+            views = _bind_grad_views(handle, names, params, direct, ctx.dev) if need_p else None
+            # no parameter needs a gradient (all frozen, only x is differentiated): the library skips every
+            # weight-gradient kernel
+            _check(lib.gast_backward_input(handle.h, C.c_void_p(dy.data_ptr()),
+                                           C.c_void_p(dx.data_ptr() if dx is not None else None), 1 if need_p else 0,
+                                           C.c_void_p(ws.data_ptr()), ws.numel(), C.c_void_p(_stream(ctx.dev))),
+                   'gast_backward')
         ctx.ws = None
         ctx.x = None
-        if direct:
-            return (None, None, None, None) + (None,) * n
-        return (None, None, None, None) + tuple(views)
+        if direct or views is None:
+            return (None, None, dx, None) + (None,) * n
+        return (None, None, dx, None) + tuple(views)
+
+
+def _bind_grad_views(handle, names, params, direct, dev):
+    """bind one gradient buffer per parameter (gast_bind_grads): the parameters' own .grad when `direct`, else views of
+    one fresh flat buffer, which are returned for autograd to accumulate"""
+    n = len(params)
+    keys = (C.c_char_p * n)()
+    ptrs = (C.c_void_p * n)()
+    numel = (C.c_int64 * n)()
+    flat = None if direct else torch.empty(sum(p.numel() for p in params), dtype=torch.float32, device=dev)
+    views, off = [], 0
+    for i, (k, p) in enumerate(zip(names, params)):
+        v = p.grad if direct else flat[off:off + p.numel()].view_as(p)
+        views.append(v)
+        keys[i] = k.encode()
+        ptrs[i] = v.data_ptr()
+        numel[i] = p.numel()
+        off += p.numel()
+    _check(handle.lib.gast_bind_grads(handle.h, n, keys, ptrs, numel), 'gast_bind_grads')
+    return views
+
+
+class _EvalFn(torch.autograd.Function):
+    """Eval-mode forward of the whole model with a backward (model.eval(): BatchNorm on the running statistics, no
+    dropout).  The forward is the inference forward, unchanged.  The backward (gast_eval_backward) recomputes the
+    activations from the saved x with a frozen-BatchNorm training forward, then runs the training backward: nothing is
+    held on the device between the two beyond x.  x, the parameters and the running statistics are saved with
+    save_for_backward, so an in-place change to any of them before the backward raises torch's version error, as
+    it does for the reference module."""
+
+    @staticmethod
+    def forward(ctx, module, handle, x, strided_now, names, *params):
+        y = _eval_forward(module, handle, x, strided_now)
+        stats = [v for k, v in named_tensors(module) if k.endswith('.running_mean') or k.endswith('.running_var')]
+        ctx.save_for_backward(x, *params, *stats)
+        ctx.module, ctx.handle, ctx.sn, ctx.names, ctx.n = module, handle, strided_now, names, len(params)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        saved = ctx.saved_tensors
+        x, params = saved[0], saved[1:1 + ctx.n]
+        module, h = ctx.module, ctx.handle
+        need_x = ctx.needs_input_grad[2]
+        need_p = any(ctx.needs_input_grad[5:])
+        dev = x.device
+        B, T = int(x.shape[0]), int(x.shape[1])
+        dy = dy.contiguous()
+        with torch.cuda.device(dev):
+            st = _stream(dev)
+            h.refresh(module, st)            # binds the current storage and GEMM-core choice (no work when unchanged)
+            lib = h.lib
+            need = lib.gast_eval_backward_workspace_bytes(h.h, B, T, ctx.sn)
+            if need == 0:
+                raise GastError('gast_eval_backward_workspace_bytes: %s' % L.last_error())
+            ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
+            dx = torch.empty_like(x) if need_x else None
+            views = _bind_grad_views(h, ctx.names, params, False, dev) if need_p else None
+            _check(lib.gast_eval_backward(h.h, C.c_void_p(x.data_ptr()), C.c_void_p(dy.data_ptr()),
+                                          C.c_void_p(dx.data_ptr() if dx is not None else None), 1 if need_p else 0,
+                                          B, T, ctx.sn, C.c_void_p(ws.data_ptr()), ws.numel(), C.c_void_p(st)),
+                   'gast_eval_backward')
+        return (None, None, dx, None, None) + (tuple(views) if views is not None else (None,) * ctx.n)
 
 
 def _no_train(module, what):
@@ -343,6 +400,20 @@ def run_model(module, x):
     # schedule computes (same arithmetic per output); skip the unused positions.
     strided_now = 1 if (module._gast_strided or
                         (T == module.receptive_field() and not module._gast_dense)) else 0
+    np_ = named_params(module) if torch.is_grad_enabled() else []
+    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for _, p in np_)):
+        # the reference's output would carry a grad_fn here: same forward, plus a backward
+        y = _EvalFn.apply(module, h, x, strided_now, [k for k, _ in np_], *[p for _, p in np_])
+    else:
+        y = _eval_forward(module, h, x, strided_now)
+    module.__dict__['_gast_last_launches'] = h.launches()
+    return y
+
+
+def _eval_forward(module, h, x, strided_now):
+    """the eval-mode forward (gast_forward) of x (B,T,J,F) -> (B,T_out,J,3)"""
+    dev = x.device
+    B, T = int(x.shape[0]), int(x.shape[1])
     with torch.cuda.device(dev):
         st = _stream(dev)
         h.refresh(module, st)
@@ -351,7 +422,6 @@ def run_model(module, x):
             raise GastError('forward: %s' % L.last_error())
         y = torch.empty((B, T_out, module.num_joints_in, 3), dtype=torch.float32, device=dev)
         h.forward(x, y, B, T, strided_now, st)
-    module.__dict__['_gast_last_launches'] = h.launches()
     return y
 
 

@@ -143,12 +143,31 @@ int gast_tta_merge(const float* pred, float* out, int32_t T, int32_t J, int32_t 
  *   needs in `workspace` (must stay untouched until gast_backward).  x (B,T,J,F) -> y (B,T_out,J,3).
  * gast_backward: dy (B,T_out,J,3) -> gradient of every parameter, WRITTEN (not accumulated) into the
  *   buffers bound with gast_bind_grads (same keys as gast_bind; buffers/running stats have none).
- * Only the strided schedule trains, like the reference (main.py:166-171). */
+ * gast_backward_input: the same backward, plus dL/dx (B,T,J,F) into dx when dx is not null.  param_grads = 0
+ *   computes no parameter gradient: no weight-gradient kernel runs and no gradient buffer need be bound.
+ *   gast_backward(h, dy, ws, n, st) is gast_backward_input(h, dy, NULL, 1, ws, n, st).
+ * Both models train on their own schedule (strided for Optimized1f, dilated or dense otherwise; main.py:166-175). */
 int gast_bind_grads(gast_t* h, int32_t n, const char* const* keys, void* const* dev_ptrs, const int64_t* numel);
 size_t gast_train_workspace_bytes(gast_t* h, int32_t B, int32_t T, float dropout_p);
 int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B, int32_t T, float dropout_p, uint64_t seed,
                        void* workspace, size_t workspace_bytes, void* stream);
 int gast_backward(gast_t* h, const float* dy, void* workspace, size_t workspace_bytes, void* stream);
+int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_t param_grads, void* workspace,
+                        size_t workspace_bytes, void* stream);
+
+/* ---- eval-mode gradients (model.eval(): BatchNorm on the running statistics, no dropout) ---------------------
+ * gast_eval_backward: backward of gast_forward(h, x, ..., B, T, strided_now) for the output gradient dy
+ *   (B,T_out,J,3).  Recomputes what it needs from x with a training-path forward whose BatchNorms use the running
+ *   statistics (same schedule as gast_forward: with strided_now a dilated model computes only the positions its
+ *   output needs), then writes the parameter gradients (param_grads != 0) into the buffers bound with
+ *   gast_bind_grads and dL/dx (B,T,J,F) into dx (may be null).  Running statistics are only read.  The eval
+ *   forward itself is unchanged; nothing is kept between it and this call.  Like gast_forward_train it rewrites
+ *   the attention constants gast_prepare derives, from the same parameters (so with the same values).
+ * gast_eval_backward_workspace_bytes: scratch for it with parameter gradients (the input-only call needs less).
+ * gast_last_launch_count afterwards: the GEMM and weight-gradient kernels this call enqueued. */
+size_t gast_eval_backward_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now);
+int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads, int32_t B, int32_t T,
+                       int32_t strided_now, void* workspace, size_t workspace_bytes, void* stream);
 /* Optional device-side dropout state: one uint64 on the device (caller-owned, may be null to unset) that is added to
  * `seed` by every dropout kernel and advanced once per gast_forward_train.  With it a CUDA graph that captured a
  * training step (frozen kernel arguments) draws a fresh mask at every replay. */
