@@ -99,8 +99,6 @@ struct gast_handle {
   int gemm_core = 0;                 // 0 auto (tensor cores where possible), 1 force FFMA
   // training: per-GEMM tensor-core operand copies (3xTF32), indexed by the GEMM's position in the step (train.cuh)
   std::vector<TcWeights> train_tc;
-  bool train_tc_on = true;
-  int block1_slabs = 1;              // clip slabs of the expand stage + first block (GAST_BLOCK1_SLABS)
   // optional per-launch device timing (bench.py roofline): event pairs around every launch
   bool timing = false;
   std::vector<cudaEvent_t> ev_pool;
@@ -210,8 +208,6 @@ extern "C" int gast_create(gast_t** out, const gast_cfg* cfg) {
   h->cfg = *cfg;
   h->sm_count = prop.multiProcessorCount;
   h->fpt = 128 / J;
-  if (const char* e = getenv("GAST_BLOCK1_SLABS")) h->block1_slabs = std::max(1, atoi(e));
-  if (const char* e = getenv("GAST_TRAIN_TC")) h->train_tc_on = atoi(e) != 0;   // 0: training GEMMs on the FFMA core (A/B runs)
   h->sym_r.assign(cfg->sym_rows, cfg->sym_rows + cfg->sym_nnz);
   h->sym_c.assign(cfg->sym_cols, cfg->sym_cols + cfg->sym_nnz);
   h->nnz[0] = cfg->sym_nnz;
@@ -422,7 +418,33 @@ static int prepare_block(gast_handle* h, Lookup& L, cudaStream_t st, BlockConsts
   return 0;
 }
 
-static int prepare_tc(gast_handle* h, cudaStream_t st);
+// ------------------------------------------------------------------------------------------
+// tensor-core weight copies
+// ------------------------------------------------------------------------------------------
+static int prep_one_tc(gast_handle* h, cudaStream_t st, TcWeights& t, const float* W, int N, int K) {
+  if (!W) return 0;
+  int rc = tc_prepare_weights(t, W, N, K, st, &h->owned);
+  if (rc) return fail("tensor-core weight preparation failed: %s", cudaGetErrorString((cudaError_t)rc));
+  return 0;
+}
+
+static int prepare_tc(gast_handle* h, cudaStream_t st) {
+  const int kind = h->cfg.kind;
+  for (BlockConsts& b : h->blocks) {
+    const int C = b.C;
+    const int nmask = (kind == GAST_KIND_SEMCH) ? 1 : 2;
+    if (prep_one_tc(h, st, b.tc_loc, b.Wloc, nmask * b.tpm * 128, C)) return 1;
+    if (prep_one_tc(h, st, b.tc_lc, b.Wlc, C, 2 * C)) return 1;
+    if (prep_one_tc(h, st, b.tc_g, b.Wg, b.heads * b.Cg, C)) return 1;
+    if (prep_one_tc(h, st, b.tc_gc, b.Wgc, C, C)) return 1;
+    if (prep_one_tc(h, st, b.tc_bc, b.Wbc, 2 * C, 3 * C)) return 1;
+  }
+  for (StageConsts& s : h->stages) {
+    if (prep_one_tc(h, st, s.tc_t, s.Wt, s.Cw, s.taps * s.Cw)) return 1;
+    if (prep_one_tc(h, st, s.tc_1, s.W1, s.Cw, s.Cw)) return 1;
+  }
+  return 0;
+}
 
 extern "C" int gast_prepare(gast_t* h, void* stream) {
   if (!h) return fail("gast_prepare: null handle");
@@ -551,6 +573,15 @@ struct Arena {
   }
 };
 
+// Caller buffers are used from their first 256-byte boundary; every *_bytes function adds at least that much slack.
+static char* align256(void* p) {
+  return reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(p) + 255) & ~(uintptr_t)255);
+}
+
+static Arena workspace_arena(void* workspace, size_t bytes, size_t off = 0) {
+  return Arena{align256(workspace), bytes, off, false};
+}
+
 struct BlockBufs { float *XY, *L, *AB, *Y, *Gl; };
 
 static void block_bufs(Arena& a, long long rows, int C, int Cout, int heads, int Cg, BlockBufs* b) {
@@ -564,23 +595,29 @@ static void block_bufs(Arena& a, long long rows, int C, int Cout, int heads, int
 // ------------------------------------------------------------------------------------------
 // launches
 // ------------------------------------------------------------------------------------------
-static ASeg seg_flat(const float* base, int ld, int K) {
-  ASeg s; s.base = base; s.ld = ld; s.K = K; s.Kc = K; s.tap_stride = 0; s.map = RowMap{1, 1, 1, 0};
+// A operand of `taps` K-segments of width Kc, tap_stride floats apart; output row r reads input row map(r)
+static ASeg seg_taps(const float* base, int ld, int Kc, int taps, long long tap_stride, RowMap map) {
+  ASeg s; s.base = base; s.ld = ld; s.K = taps * Kc; s.Kc = Kc; s.tap_stride = tap_stride; s.map = map;
   return s;
 }
 
-static void gemm_defaults(GemmP& p, const gast_handle* h, long long F) {
+static ASeg seg_flat(const float* base, int ld, int K) { return seg_taps(base, ld, K, 1, 0, RowMap{1, 1, 1, 0}); }
+
+// GEMM over M plain rows: "frames" of one joint, 128 per tile, no residual
+static void gemm_flat(GemmP& p, long long M) {
   memset(&p, 0, sizeof(p));
-  p.F = (int)F; p.J = h->cfg.num_joints; p.fpt = h->fpt;
+  p.F = (int)M; p.J = 1; p.fpt = 128;
   p.res_map = RowMap{1, 1, 1, 0};
+}
+
+static void gemm_defaults(GemmP& p, const gast_handle* h, long long F) {
+  gemm_flat(p, F);
+  p.J = h->cfg.num_joints; p.fpt = h->fpt;
 }
 
 // A 1x1 layer with flat operands and no joint mixing does not need frame-aligned tiles: run it as
 // F*J "frames" of one joint, so that every tile carries 128 rows instead of floor(128/J)*J (119 for J=17).
-static void gemm_defaults_flat(GemmP& p, const gast_handle* h, long long F) {
-  gemm_defaults(p, h, F);
-  p.F = (int)(F * h->cfg.num_joints); p.J = 1; p.fpt = 128;
-}
+static void gemm_defaults_flat(GemmP& p, const gast_handle* h, long long F) { gemm_flat(p, F * h->cfg.num_joints); }
 
 static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p, const TcWeights* tcw) {
   if (p.F <= 0) return 0;
@@ -666,27 +703,20 @@ static int run_global(gast_handle* h, cudaStream_t st, BlockConsts& b, const flo
   GemmP p;
   // tensor-core core, block / MultiGlobalGraph: plain `g` GEMM (flat 128-row tiles) into out_G as scratch, then the
   // attention mix as its own full-occupancy kernel into Y.  Measured faster than the mix fused into the GEMM
-  // epilogue (the fused form stays for the FFMA core and the single-head kind, and as GAST_GLOBAL_FUSED=1).
-  static const bool fused_env = getenv("GAST_GLOBAL_FUSED") && atoi(getenv("GAST_GLOBAL_FUSED")) != 0;
-  if (!fused_env && h->gemm_core == 0 && kind != GAST_KIND_GLOBAL_HEAD && b.tc_g.ready && Ng % 4 == 0 &&
-      b.Cg % 4 == 0 && J <= MIX_JMAX) {
+  // epilogue, which stays for the FFMA core, the single-head kind and the shapes the mix kernel does not take.
+  if (h->gemm_core == 0 && kind != GAST_KIND_GLOBAL_HEAD && b.tc_g.ready && Ng % 4 == 0 && b.Cg % 4 == 0 &&
+      J <= MIX_JMAX) {
     gemm_defaults_flat(p, h, F);
     p.nseg = 1; p.seg[0] = seg_flat(X, C, C);
     p.W = b.Wg; p.ldw = C; p.N = Ng; p.out = out_G; p.ld_out = Ng; p.bias = b.bg; p.relu = 0;
     if (launch_gemm(h, st, EPI_PLAIN, p, &b.tc_g)) return 1;
-    static const int mix_v = getenv("GAST_MIX_V") ? atoi(getenv("GAST_MIX_V")) : 4;   // channels per thread (4 or 2)
-    const int vn = (mix_v == 2 && b.Cg % 2 == 0) ? 2 : 4;
-    const int GV = Ng / vn;
-    const int nthr = (vn == 2) ? 2 * MIX_THREADS : MIX_THREADS;
-    int fpb = GV >= nthr ? 1 : nthr / GV;
+    const int GV = Ng / 4;   // threads per frame
+    int fpb = GV >= MIX_THREADS ? 1 : MIX_THREADS / GV;
     fpb = std::max(1, std::min(fpb, (int)(40 * 1024 / (sizeof(float) * b.heads * J * MIX_JP))));   // attention rows fit 40 KB
     const size_t smem = sizeof(float) * (size_t)fpb * b.heads * J * MIX_JP;
     {
       TimedLaunch tl(h, st, LK_GLOBAL_MIX);
-      if (vn == 2)
-        global_mix_kernel<float2, 2 * MIX_THREADS><<<cdiv(F, fpb), 2 * MIX_THREADS, smem, st>>>(out_G, Ng, w.AB, b.Ck, w.Y, Ng, F, J, b.heads, b.Cg, fpb);
-      else
-        global_mix_kernel<float4, MIX_THREADS><<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(out_G, Ng, w.AB, b.Ck, w.Y, Ng, F, J, b.heads, b.Cg, fpb);
+      global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(out_G, Ng, w.AB, b.Ck, w.Y, Ng, F, J, b.heads, b.Cg, fpb);
       h->launches++;
     }
     CUDA_OK(cudaGetLastError());
@@ -713,20 +743,73 @@ static int run_global(gast_handle* h, cudaStream_t st, BlockConsts& b, const flo
 static int run_block(gast_handle* h, cudaStream_t st, BlockConsts& b, const float* X, long long F,
                      const BlockBufs& w, float* out) {
   const int C = b.C;
-  static const bool global_first = getenv("GAST_BLOCK_ORDER") && atoi(getenv("GAST_BLOCK_ORDER")) != 0;   // experiment
-  if (global_first) {
-    if (run_global(h, st, b, X, F, w, w.Gl, GAST_KIND_BLOCK)) return 1;
-    if (run_local(h, st, b, X, F, w, w.L, GAST_KIND_BLOCK)) return 1;
-  } else {
-    if (run_local(h, st, b, X, F, w, w.L, GAST_KIND_BLOCK)) return 1;
-    if (run_global(h, st, b, X, F, w, w.Gl, GAST_KIND_BLOCK)) return 1;
-  }
+  if (run_local(h, st, b, X, F, w, w.L, GAST_KIND_BLOCK)) return 1;
+  if (run_global(h, st, b, X, F, w, w.Gl, GAST_KIND_BLOCK)) return 1;
   GemmP p;
   gemm_defaults_flat(p, h, F);
   p.nseg = 3;
   p.seg[0] = seg_flat(X, C, C); p.seg[1] = seg_flat(w.L, C, C); p.seg[2] = seg_flat(w.Gl, C, C);
   p.W = b.Wbc; p.ldw = 3 * C; p.N = 2 * C; p.out = out; p.ld_out = 2 * C; p.bias = b.bbc; p.relu = 1;
   return launch_gemm(h, st, EPI_PLAIN, p, &b.tc_bc);
+}
+
+// expand (gast_net.py:163-164): rows output positions, windows of x (clips of T frames, stride `stride`) -> out (rows, C)
+static int launch_expand(gast_handle* h, cudaStream_t st, const float* x, float* out, long long rows, int T, int T0,
+                         int stride) {
+  const gast_cfg& c = h->cfg;
+  const int k0 = c.filter_widths[0], Fin = c.in_features;
+  if (rows >= 0x7fffffffLL) return fail("expand: more than 2^31 positions in one call");
+  if (k0 * Fin > EXP_MAXKF) return fail("expand: filter_width*in_features > %d unsupported", EXP_MAXKF);
+  TimedLaunch tl(h, st, LK_EXPAND);
+  const dim3 grid(cdiv(rows, EXS_ROWS), cdiv(c.channels, EXS_CHUNK));
+  if (k0 * Fin <= 6)
+    expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, out, rows, c.num_joints, T, T0, stride, k0,
+                                                         Fin, c.channels);
+  else
+    expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, out, rows, c.num_joints, T, T0, stride,
+                                                                 k0, Fin, c.channels);
+  h->launches++;
+  return 0;
+}
+
+// temporal stage on F frames: conv over the taps of `taps` + BN + ReLU into tmp, then 1x1 conv + BN + ReLU (+Dropout =
+// identity in eval) + the residual rows res_map of `res` into out (gast_net.py:170,173-174 / :243,247)
+static int run_stage(gast_handle* h, cudaStream_t st, const StageConsts& s, long long F, const ASeg& taps,
+                     const float* Wt, const TcWeights* tc_t, float* tmp, const float* res, RowMap res_map, float* out) {
+  const int Cw = s.Cw;
+  GemmP p;
+  gemm_defaults(p, h, F);
+  p.nseg = 1; p.seg[0] = taps;
+  p.W = Wt; p.ldw = taps.K; p.N = Cw; p.out = tmp; p.ld_out = Cw; p.bias = s.bt; p.relu = 1;
+  if (launch_gemm(h, st, EPI_PLAIN, p, tc_t)) return 1;
+  gemm_defaults(p, h, F);
+  p.nseg = 1; p.seg[0] = seg_flat(tmp, Cw, Cw);
+  p.W = s.W1; p.ldw = Cw; p.N = Cw; p.out = out; p.ld_out = Cw; p.bias = s.b1; p.relu = 1;
+  p.res = res; p.res_ld = Cw; p.res_map = res_map;
+  return launch_gemm(h, st, EPI_PLAIN, p, &s.tc_1);
+}
+
+// shrink (gast_net.py:99): X (rows, C << L) -> y (rows, 3); with a target also the mpjpe of y into *loss
+static int launch_shrink(gast_handle* h, cudaStream_t st, const float* X, float* y, long long rows, const float* target,
+                         float* loss) {
+  Lookup Lk{h};
+  const int Cl = h->cfg.channels << h->cfg.num_stages;
+  const float* ws = Lk.get("shrink.weight", (int64_t)3 * Cl);
+  if (!Lk.ok) return 1;
+  if (target) {
+    static_assert(SHL_MAXBLOCKS == 1024, "loss_scratch is sized for 1024 block partials");
+    if (!h->loss_scratch) return fail("gast_forward_mpjpe: handle has no loss scratch");
+    double* partial = reinterpret_cast<double*>(h->loss_scratch);
+    unsigned* ticket = reinterpret_cast<unsigned*>(h->loss_scratch + 2 * SHL_MAXBLOCKS);
+    const unsigned nb = (unsigned)std::min<long long>(SHL_MAXBLOCKS, (rows + 7) / 8);
+    TimedLaunch tl(h, st, LK_SHRINK);
+    shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(X, Cl, ws, y, rows, Cl, target, partial, ticket, loss);
+  } else {
+    TimedLaunch tl(h, st, LK_SHRINK);
+    shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(X, Cl, ws, y, rows, Cl);
+  }
+  h->launches++;
+  return 0;
 }
 
 struct ModelBufs {
@@ -773,25 +856,6 @@ extern "C" size_t gast_workspace_bytes(const gast_t* h, int32_t B, int32_t T, in
 }
 
 static int forward_impl(gast_t* h, const float* x, float* y, int32_t B, int32_t T, int32_t strided_now,
-                        void* workspace, size_t workspace_bytes, void* stream, const float* target, float* loss);
-
-extern "C" int gast_forward(gast_t* h, const float* x, float* y, int32_t B, int32_t T, int32_t strided_now,
-                            void* workspace, size_t workspace_bytes, void* stream) {
-  return forward_impl(h, x, y, B, T, strided_now, workspace, workspace_bytes, stream, nullptr, nullptr);
-}
-
-// forward + mpjpe of the prediction against `target` (B, T_out, J, 3) in one call: the caller-side pair
-// `predicted = model(x); error = mpjpe(predicted, target)` of main.py:evaluate / train with the loss taken in the shrink
-// kernel's epilogue (SURVEY §8f N2)
-extern "C" int gast_forward_mpjpe(gast_t* h, const float* x, const float* target, float* y, float* loss, int32_t B, int32_t T,
-                                  int32_t strided_now, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h) return fail("gast_forward_mpjpe: null handle");
-  if (h->cfg.kind != GAST_KIND_MODEL) return fail("gast_forward_mpjpe: only the MODEL kind has a shrink layer");
-  if (!target || !loss) return fail("gast_forward_mpjpe: target and loss must be device pointers");
-  return forward_impl(h, x, y, B, T, strided_now, workspace, workspace_bytes, stream, target, loss);
-}
-
-static int forward_impl(gast_t* h, const float* x, float* y, int32_t B, int32_t T, int32_t strided_now,
                         void* workspace, size_t workspace_bytes, void* stream, const float* target, float* loss) {
   if (!h) return fail("gast_forward: null handle");
   if (!h->prepared) return fail("gast_forward: gast_prepare() has not run since the last gast_bind()");
@@ -806,8 +870,7 @@ static int forward_impl(gast_t* h, const float* x, float* y, int32_t B, int32_t 
   if (need == 0) return 1;
   if (workspace_bytes < need || !workspace)
     return fail("gast_forward: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
-  uintptr_t wsb = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255;
-  Arena a{reinterpret_cast<char*>(wsb), workspace_bytes, 0, false};
+  Arena a = workspace_arena(workspace, workspace_bytes);
   const int J = h->cfg.num_joints;
   const int kind = h->cfg.kind;
 
@@ -827,133 +890,51 @@ static int forward_impl(gast_t* h, const float* x, float* y, int32_t B, int32_t 
 
   ModelBufs mb; Geometry g;
   if (plan_model(h, B, T, strided_now, a, &mb, &g)) return 1;
-  const gast_cfg& c = h->cfg;
-  const int C = c.channels, L = c.num_stages;
-  // expand (gast_net.py:163-164) + first GraphAttentionBlock, optionally in SLABS of clips: the layers of block 1 are
-  // the HBM-bound ones (K = C GEMMs, row dots, attention mix, expand), and a slab whose intermediates fit the 50 MB L2
-  // hands them from producer to consumer on chip; the block temporaries are reused by every slab.
+  // expand (gast_net.py:163-164) + first GraphAttentionBlock
   long long F = (long long)B * g.T0;
-  if (F * J >= 0x7fffffffLL) return fail("expand: more than 2^31 positions in one call");
-  if (c.filter_widths[0] * c.in_features > EXP_MAXKF) return fail("expand: filter_width*in_features > %d unsupported", EXP_MAXKF);
-  const int nslab = std::max(1, std::min(h->block1_slabs, B));
-  const int Bs = (B + nslab - 1) / nslab;
-  for (int b0 = 0; b0 < B; b0 += Bs) {
-    const int nb = std::min(Bs, B - b0);
-    const long long Fs = (long long)nb * g.T0, rows = Fs * J;
-    const float* xs = x + (long long)b0 * T * J * c.in_features;
-    float* a0 = mb.act[0] + (long long)b0 * g.T0 * J * C;
-    float* a1 = mb.act[1] + (long long)b0 * g.T0 * J * 2 * C;
-    static const bool expand_staged = !(getenv("GAST_EXPAND_STAGED") && atoi(getenv("GAST_EXPAND_STAGED")) == 0);
-    if (expand_staged && expand_rows_ok(C)) {
-      // staged form (kernels_hbm.cuh): inputs of 128 rows gathered once into shared memory, weights in registers
-      TimedLaunch tl(h, st, LK_EXPAND);
-      const unsigned nblk = (unsigned)cdiv(rows, EXS_ROWS);
-      if (c.filter_widths[0] * c.in_features <= 6)
-        expand_rows_kernel<6><<<nblk, EXS_THREADS, 0, st>>>(xs, h->We, h->be, a0, rows, J, T, g.T0, g.s0,
-                                                            c.filter_widths[0], c.in_features, C);
-      else
-        expand_rows_kernel<EXP_MAXKF><<<nblk, EXS_THREADS, 0, st>>>(xs, h->We, h->be, a0, rows, J, T, g.T0, g.s0,
-                                                                    c.filter_widths[0], c.in_features, C);
-      h->launches++;
-    } else {
-      long long thr = ((rows + EXP_ROWS - 1) / EXP_ROWS) * (C / 4);
-      TimedLaunch tl(h, st, LK_EXPAND);
-      if (c.filter_widths[0] * c.in_features <= 6)
-        expand_kernel<6><<<cdiv(thr, 256), 256, 0, st>>>(xs, h->We, h->be, a0, rows, J, T, g.T0, g.s0,
-                                                        c.filter_widths[0], c.in_features, C);
-      else
-        expand_kernel<EXP_MAXKF><<<cdiv(thr, 256), 256, 0, st>>>(xs, h->We, h->be, a0, rows, J, T, g.T0, g.s0,
-                                                                c.filter_widths[0], c.in_features, C);
-      h->launches++;
-    }
-    if (run_block(h, st, h->blocks[0], a0, Fs, mb.bb, a1)) return 1;
-  }
+  if (launch_expand(h, st, x, mb.act[0], F * J, T, g.T0, g.s0)) return 1;
+  if (run_block(h, st, h->blocks[0], mb.act[0], F, mb.bb, mb.act[1])) return 1;
   int cur = 1;
   int Tp = g.T0;
-  for (int i = 1; i < L; ++i) {
+  for (int i = 1; i < h->cfg.num_stages; ++i) {
     StageConsts& s = h->stages[i - 1];
     Sched sc;
     stage_sched(h, i, strided_now, &sc);
     const int Cw = s.Cw, Tn = g.Ts[i - 1];
     const long long Fn = (long long)B * Tn;
     const float* xin = mb.act[cur];
-    // temporal conv + BN + ReLU (gast_net.py:173)
-    GemmP p;
-    gemm_defaults(p, h, Fn);
-    p.nseg = 1;
-    p.seg[0].base = xin; p.seg[0].ld = Cw; p.seg[0].K = sc.taps * Cw; p.seg[0].Kc = Cw;
-    p.seg[0].tap_stride = (long long)sc.dil * J * Cw;
-    p.seg[0].map = RowMap{Tn, Tp, sc.stride, 0};
-    p.W = s.Wt; p.ldw = sc.taps * Cw; p.N = Cw; p.out = mb.tmp; p.ld_out = Cw; p.bias = s.bt; p.relu = 1;
-    if (launch_gemm(h, st, EPI_PLAIN, p, &s.tc_t)) return 1;
-    // 1x1 conv + BN + ReLU (+Dropout = identity in eval) + residual slice (gast_net.py:170,174 / :243,247)
-    gemm_defaults(p, h, Fn);
-    p.nseg = 1; p.seg[0] = seg_flat(mb.tmp, Cw, Cw);
-    p.W = s.W1; p.ldw = Cw; p.N = Cw; p.out = mb.act[cur ^ 1]; p.ld_out = Cw; p.bias = s.b1; p.relu = 1;
-    p.res = xin; p.res_ld = Cw; p.res_map = RowMap{Tn, Tp, sc.res_mul, sc.res_off};
-    if (launch_gemm(h, st, EPI_PLAIN, p, &s.tc_1)) return 1;
+    const ASeg taps = seg_taps(xin, Cw, Cw, sc.taps, (long long)sc.dil * J * Cw, RowMap{Tn, Tp, sc.stride, 0});
+    if (run_stage(h, st, s, Fn, taps, s.Wt, &s.tc_t, mb.tmp, xin, RowMap{Tn, Tp, sc.res_mul, sc.res_off},
+                  mb.act[cur ^ 1])) return 1;
     cur ^= 1;
     if (run_block(h, st, h->blocks[i], mb.act[cur], Fn, mb.bb, mb.act[cur ^ 1])) return 1;
     cur ^= 1;
     Tp = Tn;
     F = Fn;
   }
-  // shrink (gast_net.py:99) ; output is already (B, T_out, J, 3)
-  {
-    Lookup Lk{h};
-    const int Cl = C << L;
-    const float* ws = Lk.get("shrink.weight", (int64_t)3 * Cl);
-    if (!Lk.ok) return 1;
-    long long rows = F * J;
-    if (target) {
-      static_assert(SHL_MAXBLOCKS == 1024, "loss_scratch is sized for 1024 block partials");
-      if (!h->loss_scratch) return fail("gast_forward_mpjpe: handle has no loss scratch");
-      double* partial = reinterpret_cast<double*>(h->loss_scratch);
-      unsigned* ticket = reinterpret_cast<unsigned*>(h->loss_scratch + 2 * SHL_MAXBLOCKS);
-      const unsigned nb = (unsigned)std::min<long long>(SHL_MAXBLOCKS, (rows + 7) / 8);
-      TimedLaunch tl(h, st, LK_SHRINK);
-      shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(mb.act[cur], Cl, ws, y, rows, Cl, target, partial, ticket, loss);
-      h->launches++;
-    } else {
-    TimedLaunch tl(h, st, LK_SHRINK);
-    shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(mb.act[cur], Cl, ws, y, rows, Cl);
-    h->launches++;
-    }
-  }
+  // output is already (B, T_out, J, 3)
+  if (launch_shrink(h, st, mb.act[cur], y, F * J, target, loss)) return 1;
   CUDA_OK(cudaGetLastError());
   return 0;
 }
 
-static int prep_one_tc(gast_handle* h, cudaStream_t st, TcWeights& t, const float* W, int N, int K);
+extern "C" int gast_forward(gast_t* h, const float* x, float* y, int32_t B, int32_t T, int32_t strided_now,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+  return forward_impl(h, x, y, B, T, strided_now, workspace, workspace_bytes, stream, nullptr, nullptr);
+}
+
+// forward + mpjpe of the prediction against `target` (B, T_out, J, 3) in one call: the caller-side pair
+// `predicted = model(x); error = mpjpe(predicted, target)` of main.py:evaluate / train with the loss taken in the shrink
+// kernel's epilogue (SURVEY §8f N2)
+extern "C" int gast_forward_mpjpe(gast_t* h, const float* x, const float* target, float* y, float* loss, int32_t B, int32_t T,
+                                  int32_t strided_now, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h) return fail("gast_forward_mpjpe: null handle");
+  if (h->cfg.kind != GAST_KIND_MODEL) return fail("gast_forward_mpjpe: only the MODEL kind has a shrink layer");
+  if (!target || !loss) return fail("gast_forward_mpjpe: target and loss must be device pointers");
+  return forward_impl(h, x, y, B, T, strided_now, workspace, workspace_bytes, stream, target, loss);
+}
+
 #include "stream.cuh"
-
-// ------------------------------------------------------------------------------------------
-// tensor-core weight copies
-// ------------------------------------------------------------------------------------------
-static int prep_one_tc(gast_handle* h, cudaStream_t st, TcWeights& t, const float* W, int N, int K) {
-  if (!W) return 0;
-  int rc = tc_prepare_weights(t, W, N, K, st, &h->owned);
-  if (rc) return fail("tensor-core weight preparation failed: %s", cudaGetErrorString((cudaError_t)rc));
-  return 0;
-}
-
-static int prepare_tc(gast_handle* h, cudaStream_t st) {
-  const int kind = h->cfg.kind;
-  for (BlockConsts& b : h->blocks) {
-    const int C = b.C;
-    const int nmask = (kind == GAST_KIND_SEMCH) ? 1 : 2;
-    if (prep_one_tc(h, st, b.tc_loc, b.Wloc, nmask * b.tpm * 128, C)) return 1;
-    if (prep_one_tc(h, st, b.tc_lc, b.Wlc, C, 2 * C)) return 1;
-    if (prep_one_tc(h, st, b.tc_g, b.Wg, b.heads * b.Cg, C)) return 1;
-    if (prep_one_tc(h, st, b.tc_gc, b.Wgc, C, C)) return 1;
-    if (prep_one_tc(h, st, b.tc_bc, b.Wbc, 2 * C, 3 * C)) return 1;
-  }
-  for (StageConsts& s : h->stages) {
-    if (prep_one_tc(h, st, s.tc_t, s.Wt, s.Cw, s.taps * s.Cw)) return 1;
-    if (prep_one_tc(h, st, s.tc_1, s.W1, s.Cw, s.Cw)) return 1;
-  }
-  return 0;
-}
 
 // ------------------------------------------------------------------------------------------
 // test-time augmentation around the forward (SURVEY.md §8f N1)
@@ -1009,16 +990,22 @@ static int train_check(gast_handle* h) {
   return 0;
 }
 
-extern "C" size_t gast_train_workspace_bytes(gast_t* h, int32_t B, int32_t T, float dropout_p) {
+// workspace of a training forward + backward of the mode `ts` describes, by a dry run of both (no launches); 0 on error
+static size_t train_dry_run_bytes(gast_handle* h, int B, int T, TrainState ts, bool pgrad) {
   if (!h || train_check(h)) return 0;
   Arena a{nullptr, 0, 0, true};
   Lookup L{h};
   TCtx c{h, nullptr, &a, &L, h->cfg.num_joints, true};
-  TrainState ts;
-  ts.drop_p = dropout_p;
+  c.pgrad = pgrad;
   if (train_forward(h, c, ts, nullptr, nullptr, B, T)) return 0;
   if (train_backward(h, c, ts, nullptr, nullptr)) return 0;
   return a.off + 512;
+}
+
+extern "C" size_t gast_train_workspace_bytes(gast_t* h, int32_t B, int32_t T, float dropout_p) {
+  TrainState ts;
+  ts.drop_p = dropout_p;
+  return train_dry_run_bytes(h, B, T, ts, true);
 }
 
 extern "C" int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B, int32_t T, float dropout_p,
@@ -1028,8 +1015,7 @@ extern "C" int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B
   if (dropout_p < 0.f || dropout_p >= 1.f) return fail("gast_forward_train: dropout_p out of range");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CUDA_OK(cudaSetDevice(h->cfg.device));
-  uintptr_t wsb = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255;
-  Arena a{reinterpret_cast<char*>(wsb), workspace_bytes, 0, false};
+  Arena a = workspace_arena(workspace, workspace_bytes);
   Lookup L{h};
   TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
   const size_t need = gast_train_workspace_bytes(h, B, T, dropout_p);
@@ -1074,10 +1060,9 @@ extern "C" int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_
                 "or more than %d forwards were outstanding)", GAST_MAX_PENDING_TRAIN);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CUDA_OK(cudaSetDevice(h->cfg.device));
-  uintptr_t wsb = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255;
   TrainState ts = h->trains[ti].second;
   h->trains.erase(h->trains.begin() + ti);
-  Arena a{reinterpret_cast<char*>(wsb), workspace_bytes, ts.arena_off, false};
+  Arena a = workspace_arena(workspace, workspace_bytes, ts.arena_off);
   Lookup L{h};
   TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
   c.tc_slot = 1024;                         // the backward's GEMMs follow the forward's in the operand-copy table
@@ -1090,21 +1075,14 @@ extern "C" int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_
 
 // ---- eval-mode backward: a frozen-BatchNorm training forward recomputes the activations from x, then the training
 // backward runs on them.  The inference forward stays as it is; nothing is held between forward and backward.
-static size_t eval_backward_bytes(gast_handle* h, int B, int T, int strided_now, bool pgrad) {
-  if (!h || train_check(h)) return 0;
-  Arena a{nullptr, 0, 0, true};
-  Lookup L{h};
-  TCtx c{h, nullptr, &a, &L, h->cfg.num_joints, true};
-  c.pgrad = pgrad;
+static TrainState eval_state(int strided_now) {
   TrainState ts;
   ts.frozen = true; ts.sn = strided_now ? 1 : 0;
-  if (train_forward(h, c, ts, nullptr, nullptr, B, T)) return 0;
-  if (train_backward(h, c, ts, nullptr, nullptr)) return 0;
-  return a.off + 512;
+  return ts;
 }
 
 extern "C" size_t gast_eval_backward_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now) {
-  return eval_backward_bytes(h, B, T, strided_now, true);
+  return train_dry_run_bytes(h, B, T, eval_state(strided_now), true);
 }
 
 extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads, int32_t B,
@@ -1114,19 +1092,17 @@ extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, fl
   if (B <= 0 || T <= 0) return fail("gast_eval_backward: empty batch (B=%d T=%d)", B, T);
   if (!x || !dy) return fail("gast_eval_backward: x and dy must be device pointers");
   if (!dx && !param_grads) return fail("gast_eval_backward: neither dx nor parameter gradients requested");
-  const size_t need = eval_backward_bytes(h, B, T, strided_now, param_grads != 0);
+  TrainState ts = eval_state(strided_now);
+  const size_t need = train_dry_run_bytes(h, B, T, ts, param_grads != 0);
   if (need == 0) return 1;
   if (!workspace || workspace_bytes < need)
     return fail("gast_eval_backward: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CUDA_OK(cudaSetDevice(h->cfg.device));
-  uintptr_t wsb = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255;
-  Arena a{reinterpret_cast<char*>(wsb), workspace_bytes, 0, false};
+  Arena a = workspace_arena(workspace, workspace_bytes);
   Lookup L{h};
   TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
   c.pgrad = param_grads != 0;
-  TrainState ts;
-  ts.frozen = true; ts.sn = strided_now ? 1 : 0;
   h->launches = 0;
   if (train_forward(h, c, ts, x, nullptr, B, T)) return 1;
   c.tc_slot = 1024;
@@ -1146,12 +1122,8 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
   if (M <= 0 || N <= 0 || K <= 0 || N % 4 || K % 4) return fail("gast_debug_gemm: bad shape");
   if (core < 0 || core > 1 || tc_mode != 0) return fail("gast_debug_gemm: core must be 0 (tensor cores) or 1 (FFMA), tc_mode 0");
   GemmP p;
-  memset(&p, 0, sizeof(p));
-  p.F = M; p.J = 1; p.fpt = 128;
-  p.res_map = RowMap{1, 1, 1, 0};
-  p.nseg = 1;
-  p.seg[0].base = A; p.seg[0].ld = K; p.seg[0].K = K; p.seg[0].Kc = K; p.seg[0].tap_stride = 0;
-  p.seg[0].map = RowMap{1, 1, 1, 0};
+  gemm_flat(p, M);
+  p.nseg = 1; p.seg[0] = seg_flat(A, K, K);
   p.W = W; p.ldw = K; p.N = N; p.out = out; p.ld_out = N;
   int rc = 0;
   std::vector<void*> owned;

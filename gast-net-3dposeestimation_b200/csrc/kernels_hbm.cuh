@@ -1,6 +1,5 @@
-// HBM-bound kernels of the lifting path, round 2: the expand stage staged through shared memory (replaces the
-// latency-bound expand_kernel of kernels_misc.cuh, which stays as the fallback for shapes this one does not cover and
-// behind GAST_EXPAND_STAGED=0) and the shrink layer with mpjpe in its epilogue (gast_forward_mpjpe).
+// HBM-bound kernels of the lifting path: the expand stage staged through shared memory (every width, the forward and the
+// streaming push) and the shrink layer with mpjpe in its epilogue (gast_forward_mpjpe).
 //
 // Measured (on the earlier B200 build) and NOT kept: persistent bulk-copy
 // (cp.async.bulk + mbarrier ring) forms of the attention mix -- register-resident g and g kept in shared memory with
@@ -14,16 +13,19 @@
 namespace gast {
 
 // ---------------------------------------------------------------------------------------
-// expand stage (gast_net.py:163-164), staged: a block owns EXS_ROWS consecutive output rows.  Their taps*Fin input
-// values are gathered ONCE into shared memory (expand_kernel has every one of the C/4 threads of a row request them
+// expand stage (gast_net.py:163-164): ReLU(BN(Conv_{(k,1), F->C}(BN_in(x)))) with both BNs folded into We/be.
+// x: (B,T,J,Fin) ; out: (rows = B*T0*J, C).  A block owns EXS_ROWS consecutive output rows.  Their taps*Fin input
+// values are gathered ONCE into shared memory (a first version had every one of the C/4 threads of a row request them
 // again through L1: 48 loads in flight per thread, 126 registers, 16 warps per SM, 1.7 TB/s of output); a thread then
 // keeps the folded weights of its 4 channels in registers and walks the block's rows: 2 broadcast shared-memory reads,
-// 4*KF FMAs and one coalesced 16-byte store per row, ~50 registers, full occupancy.  Same FMA order as expand_kernel
-// (bias first, then k ascending), so the two are bit-identical.
+// 4*KF FMAs (bias first, then k ascending) and one coalesced 16-byte store per row, full occupancy.
+// A block covers at most EXS_CHUNK channels; wider layers take more chunks along blockIdx.y, each staging the same rows.
 // ---------------------------------------------------------------------------------------
 constexpr int EXS_ROWS = 128;
 constexpr int EXS_THREADS = 256;
-template <int KFT>
+constexpr int EXS_CHUNK = 4 * EXS_THREADS;               // channels per block: 4 per thread
+constexpr int EXP_MAXKF = 10;   // taps * in_features supported by the register path (3*2 = 6; 5*2 = 10)
+template <int KFT>   // register-resident K = taps * in_features rounded up: 6 (3 taps x 2) or EXP_MAXKF
 __global__ void __launch_bounds__(EXS_THREADS)
 expand_rows_kernel(const float* __restrict__ x, const float* __restrict__ We, const float* __restrict__ be,
                    float* __restrict__ out, long long rows, int J, int T, int T0, int stride, int taps, int Fin, int C) {
@@ -45,10 +47,11 @@ expand_rows_kernel(const float* __restrict__ x, const float* __restrict__ We, co
     }
     xs[e] = v;
   }
-  const int cq = C >> 2;                                  // channel groups (threads) per row
+  const int c0 = blockIdx.y * EXS_CHUNK;                  // first channel of this block's chunk
+  const int cq = min(C - c0, EXS_CHUNK) >> 2;             // channel groups (threads) per row
   const int rpp = EXS_THREADS / cq;                       // rows per pass of the block
   const int cg = tid % cq, rsub = tid / cq;
-  const int c = cg * 4;
+  const int c = c0 + cg * 4;
   float w[4][KFT];
 #pragma unroll
   for (int k = 0; k < KFT; ++k) {
@@ -78,9 +81,6 @@ expand_rows_kernel(const float* __restrict__ x, const float* __restrict__ We, co
     *reinterpret_cast<float4*>(op) = make_float4(fmaxf(v0, 0.f), fmaxf(v1, 0.f), fmaxf(v2, 0.f), fmaxf(v3, 0.f));
   }
 }
-
-// true when expand_rows_kernel covers the shape (else the caller keeps expand_kernel)
-static inline bool expand_rows_ok(int C) { return C % 4 == 0 && C / 4 >= 1 && C / 4 <= EXS_THREADS; }
 
 // ---------------------------------------------------------------------------------------
 // shrink (gast_net.py:60,99) with mpjpe (common/loss.py:5-11) in its epilogue: the warp that produced the 3 coordinates

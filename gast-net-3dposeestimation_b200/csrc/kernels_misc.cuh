@@ -1,86 +1,9 @@
-// Small kernels of the lifting path: expand stage, collapsed theta/phi row dots, shrink,
+// Small kernels of the lifting path: collapsed theta/phi row dots, attention mix, shrink,
 // and the parameter-preparation kernels (BN folding, adjacency softmax, weight packing).
 #pragma once
 #include "gast_common.cuh"
 
 namespace gast {
-
-// ---------------------------------------------------------------------------------------
-// expand stage (gast_net.py:163-164): ReLU(BN(Conv_{(k,1), F->C}(BN_in(x)))) with both BNs
-// folded into We/be.  x: (B,T,J,Fin) ; out: (B*T0*J, C).   One thread = one row x 4 channels.
-// ---------------------------------------------------------------------------------------
-// One thread = 4 channels x EXP_ROWS rows: the 4 x (taps*Fin) folded weights and the bias stay in
-// registers, the x values are broadcast loads (all C/4 threads of a row group read the same
-// addresses), so the kernel is bound by its output stream (C*4 B per row) instead of by ~30
-// load instructions per output float4 (first version: 0.50 ms for 321 MB, 10x off the HBM bound).
-constexpr int EXP_ROWS = 8;
-constexpr int EXP_MAXKF = 10;   // taps * in_features supported by the register path (3*2 = 6; 5*2 = 10)
-template <int KFT>   // register-resident K = taps * in_features rounded up: 6 (3 taps x 2) or EXP_MAXKF
-__global__ void expand_kernel(const float* __restrict__ x, const float* __restrict__ We,
-                              const float* __restrict__ be, float* __restrict__ out,
-                              long long rows, int J, int T, int T0, int stride, int taps,
-                              int Fin, int C) {
-  const int cq = C >> 2;
-  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long groups = (rows + EXP_ROWS - 1) / EXP_ROWS;
-  if (idx >= groups * cq) return;
-  const long long grp = idx / cq;
-  const int c = (int)(idx - grp * cq) * 4;
-  const int KF = taps * Fin;
-  // folded weights are stored [k][C]: one coalesced float4 (4 channels) per k (the [C][k] layout made every lane
-  // of 24 scalar loads hit a different sector; measured 0.309 -> 0.286 ms)
-  float w[4][KFT];
-#pragma unroll
-  for (int k = 0; k < KFT; ++k) {
-    float4 wk = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (k < KF) wk = ldg4(We + (long long)k * C + c);
-    w[0][k] = wk.x; w[1][k] = wk.y; w[2][k] = wk.z; w[3][k] = wk.w;
-  }
-  const float4 b4 = ldg4(be + c);
-  const long long r0 = grp * EXP_ROWS;
-  // All EXP_ROWS x KF input values are requested before the first FMA (rows past the end re-read the
-  // last row): with the loads issued row by row the kernel ran at 1/3 of its output-stream bound.
-  float xv[EXP_ROWS][KFT];
-  // (clip, frame, joint) of the first row by division (32-bit: the host checks rows < 2^31), the following rows by
-  // increment: the 16 integer divisions per thread of the first version were a third of its instructions
-  int f = (int)r0 / J;
-  int j = (int)r0 - f * J;
-  int b = f / T0;
-  int t = f - b * T0;
-  // offset of (tap kk, feature i) = element k of the folded K axis, by increment as well (`k / Fin` with a
-  // runtime Fin inside the unrolled loops was 48 divisions per thread: half of the kernel's stall samples)
-  int xoff[KFT];
-  {
-    int kk = 0, i = 0;
-#pragma unroll
-    for (int k = 0; k < KFT; ++k) {
-      xoff[k] = kk * J * Fin + i;
-      if (++i == Fin) { i = 0; ++kk; }
-    }
-  }
-#pragma unroll
-  for (int rr = 0; rr < EXP_ROWS; ++rr) {
-    const float* xin = x + (((long long)b * T + (long long)t * stride) * J + j) * Fin;
-#pragma unroll
-    for (int k = 0; k < KFT; ++k) xv[rr][k] = (k < KF) ? __ldg(xin + xoff[k]) : 0.f;
-    if (r0 + rr + 1 < rows) {                 // rows past the end re-read the last row
-      if (++j == J) { j = 0; if (++t == T0) { t = 0; ++b; } }
-    }
-  }
-#pragma unroll
-  for (int rr = 0; rr < EXP_ROWS; ++rr) {
-    const long long row = r0 + rr;
-    float v0 = b4.x, v1 = b4.y, v2 = b4.z, v3 = b4.w;
-#pragma unroll
-    for (int k = 0; k < KFT; ++k) {
-      v0 = fmaf(w[0][k], xv[rr][k], v0); v1 = fmaf(w[1][k], xv[rr][k], v1);
-      v2 = fmaf(w[2][k], xv[rr][k], v2); v3 = fmaf(w[3][k], xv[rr][k], v3);
-    }
-    if (row < rows)
-      *reinterpret_cast<float4*>(out + row * C + c) =
-          make_float4(fmaxf(v0, 0.f), fmaxf(v1, 0.f), fmaxf(v2, 0.f), fmaxf(v3, 0.f));
-  }
-}
 
 // ---------------------------------------------------------------------------------------
 // ab[row][q] = X[row,:] . U[q,:] + cab[q],  q < Q (= 2*heads <= 8).   Warp per row.
@@ -246,27 +169,8 @@ constexpr int MIX_THREADS = 128;
 constexpr int MIX_JMAX = 20;
 constexpr int MIX_JP = 20;        // padded row length of an attention row in shared memory (float4 reads)
 
-template <typename V> struct MixVec;
-template <> struct MixVec<float4> {
-  static constexpr int N = 4;
-  __device__ static float4 zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-  __device__ static float4 load(const float* p) { return ldg4(p); }
-  __device__ static void fma(float a, const float4& g, float4& o) {
-    o.x = fmaf(a, g.x, o.x); o.y = fmaf(a, g.y, o.y); o.z = fmaf(a, g.z, o.z); o.w = fmaf(a, g.w, o.w);
-  }
-};
-template <> struct MixVec<float2> {
-  static constexpr int N = 2;
-  __device__ static float2 zero() { return make_float2(0.f, 0.f); }
-  __device__ static float2 load(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
-  __device__ static void fma(float a, const float2& g, float2& o) { o.x = fmaf(a, g.x, o.x); o.y = fmaf(a, g.y, o.y); }
-};
-
-// V = float4: one thread = (frame, 4 channels), 17 float4 of g in registers (120 registers, 16 warps per SM);
-// V = float2: (frame, 2 channels), half the registers per thread and twice the warps in flight per SM -- the kernel
-// is latency-bound (25-30 % of the issue slots, 43 % of the HBM rate with float4), so occupancy is what it lacks.
-template <typename V, int NT>
-__global__ void __launch_bounds__(NT, (MixVec<V>::N == 2) ? 4 : 1)
+// 17 float4 of g in registers per thread: 116 registers, 16 warps per SM.
+__global__ void __launch_bounds__(MIX_THREADS, 1)
 global_mix_kernel(const float* __restrict__ G, int ldg, const float* __restrict__ ab, const float* __restrict__ ck,
                   float* __restrict__ Y, int ldy, long long F, int J, int heads, int Cg, int fpb) {
   extern __shared__ __align__(16) float att_s[];            // [fpb][heads][J][MIX_JP]
@@ -275,7 +179,7 @@ global_mix_kernel(const float* __restrict__ G, int ldg, const float* __restrict_
   const long long f0 = (long long)blockIdx.x * fpb;
   // ---- attention rows of this block's frames
   const int nrow = fpb * heads * J;
-  for (int e = tid; e < nrow; e += NT) {
+  for (int e = tid; e < nrow; e += MIX_THREADS) {
     const int i = e % J, h = (e / J) % heads, fs = e / (J * heads);
     const long long f = f0 + fs;
     float* dst = att_s + (size_t)e * MIX_JP;
@@ -306,19 +210,18 @@ global_mix_kernel(const float* __restrict__ G, int ldg, const float* __restrict_
     }
   }
   __syncthreads();
-  // ---- mix: thread = (frame slot, group of V::N channels)
-  constexpr int VN = MixVec<V>::N;
-  const int GV = (heads * Cg) / VN;
-  for (int w = tid; w < fpb * GV; w += NT) {
-    const int fs = w / GV, c = (w - fs * GV) * VN;
+  // ---- mix: thread = (frame slot, group of 4 channels)
+  const int GV = (heads * Cg) / 4;
+  for (int w = tid; w < fpb * GV; w += MIX_THREADS) {
+    const int fs = w / GV, c = (w - fs * GV) * 4;
     const long long f = f0 + fs;
     if (f >= F) continue;
     const int h = c / Cg;
-    V g[MIX_JMAX];
+    float4 g[MIX_JMAX];
     const float* gp = G + (f * J) * (long long)ldg + c;
 #pragma unroll
     for (int j = 0; j < MIX_JMAX; ++j)
-      if (j < J) g[j] = MixVec<V>::load(gp + (long long)j * ldg);
+      if (j < J) g[j] = ldg4(gp + (long long)j * ldg);
     const float* arow = att_s + (size_t)((fs * heads + h) * J) * MIX_JP;
     float* yp = Y + (f * J) * (long long)ldy + c;
     for (int i = 0; i < J; ++i) {
@@ -328,11 +231,14 @@ global_mix_kernel(const float* __restrict__ G, int ldg, const float* __restrict_
         const float4 t = *reinterpret_cast<const float4*>(arow + i * MIX_JP + q * 4);
         a[q * 4] = t.x; a[q * 4 + 1] = t.y; a[q * 4 + 2] = t.z; a[q * 4 + 3] = t.w;
       }
-      V o = MixVec<V>::zero();
+      float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
       for (int j = 0; j < MIX_JMAX; ++j)
-        if (j < J) MixVec<V>::fma(a[j], g[j], o);
-      *reinterpret_cast<V*>(yp + (long long)i * ldy) = o;
+        if (j < J) {
+          o.x = fmaf(a[j], g[j].x, o.x); o.y = fmaf(a[j], g[j].y, o.y);
+          o.z = fmaf(a[j], g[j].z, o.z); o.w = fmaf(a[j], g[j].w, o.w);
+        }
+      *reinterpret_cast<float4*>(yp + (long long)i * ldy) = o;
     }
   }
 }

@@ -81,6 +81,9 @@ static int stream_check(const gast_handle* h) {
   if (!h->cfg.causal) return fail("streaming needs a causal model (gen_skes.py:59: causal=True): a non-causal network "
                                   "has no output for the newest frame");
   if (h->cfg.dense) return fail("the dense ablation has no streaming form");
+  // checked before a push touches the stream state (launch_expand checks it again for the forward)
+  if (h->cfg.filter_widths[0] * h->cfg.in_features > EXP_MAXKF)
+    return fail("expand: filter_width*in_features > %d unsupported", EXP_MAXKF);
   return 0;
 }
 
@@ -173,25 +176,16 @@ extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const floa
   h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
   const gast_cfg& c = h->cfg;
   const int n = n_streams, J = c.num_joints, C = c.channels, L = c.num_stages, k0 = c.filter_widths[0], Fin = c.in_features;
-  float* sbase = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(state) + 255) & ~(uintptr_t)255);
-  uintptr_t wsb = (reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255;
-  Arena a{reinterpret_cast<char*>(wsb), workspace_bytes, 0, false};
+  float* sbase = reinterpret_cast<float*>(align256(state));
+  Arena a = workspace_arena(workspace, workspace_bytes);
   StreamBufs sb;
   stream_bufs(h, n, a, &sb);
   const long long rows = (long long)n * J;
-  if (k0 * Fin > EXP_MAXKF) return fail("expand: filter_width*in_features > %d unsupported", EXP_MAXKF);
   // input history + expand (gast_net.py:163-164) on the last k0 frames
   float* xhist = sbase + sp.xhist_off;
   stream_xpush_kernel<<<cdiv((long long)n * J * Fin, 256), 256, 0, st>>>(xhist, x, fresh, n, k0, J * Fin);
   h->launches++;
-  {
-    long long thr = ((rows + EXP_ROWS - 1) / EXP_ROWS) * (C / 4);
-    if (k0 * Fin <= 6)
-      expand_kernel<6><<<cdiv(thr, 256), 256, 0, st>>>(xhist, h->We, h->be, sb.E, rows, J, k0, 1, 1, k0, Fin, C);
-    else
-      expand_kernel<EXP_MAXKF><<<cdiv(thr, 256), 256, 0, st>>>(xhist, h->We, h->be, sb.E, rows, J, k0, 1, 1, k0, Fin, C);
-    h->launches++;
-  }
+  if (launch_expand(h, st, xhist, sb.E, rows, k0, 1, 1)) return 1;
   auto slot_ptr = [&](int i /*stage 1..L-1*/) {
     const int R = sp.R[i - 1], Cw = C << i;
     return sbase + sp.ring_off[i - 1] + (size_t)(step % R) * n * J * Cw;
@@ -209,33 +203,16 @@ extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const floa
       stream_fill_fresh_kernel<<<g, 256, 0, st>>>(ring, R, hs, n, (long long)J * Cw, fresh);
       h->launches++;
     }
+    // taps = slots p0 + k d with the weights rotated to slot order; residual = the newest slot (causal_shift = pad)
     const int p0 = hs % d, r = hs / d;
-    // temporal conv + BN + ReLU: taps = slots p0 + k d, weights rotated to slot order (gast_net.py:173)
-    GemmP p;
-    gemm_defaults(p, h, n);
-    p.nseg = 1;
-    p.seg[0].base = ring + (long long)p0 * slot_floats; p.seg[0].ld = Cw; p.seg[0].K = fw * Cw; p.seg[0].Kc = Cw;
-    p.seg[0].tap_stride = (long long)d * slot_floats;
-    p.seg[0].map = RowMap{n, n, 1, 0};
-    p.W = s.Wrot[r]; p.ldw = fw * Cw; p.N = Cw; p.out = sb.tmp; p.ld_out = Cw; p.bias = s.bt; p.relu = 1;
-    if (launch_gemm(h, st, EPI_PLAIN, p, &s.tc_rot[r])) return 1;
-    // 1x1 conv + BN + ReLU + residual = the newest slot (gast_net.py:170,174 with causal_shift = pad)
-    gemm_defaults(p, h, n);
-    p.nseg = 1; p.seg[0] = seg_flat(sb.tmp, Cw, Cw);
-    p.W = s.W1; p.ldw = Cw; p.N = Cw; p.out = sb.act; p.ld_out = Cw; p.bias = s.b1; p.relu = 1;
-    p.res = ring + (long long)hs * slot_floats; p.res_ld = Cw; p.res_map = RowMap{n, n, 1, 0};
-    if (launch_gemm(h, st, EPI_PLAIN, p, &s.tc_1)) return 1;
+    const RowMap same{n, n, 1, 0};
+    const ASeg taps = seg_taps(ring + (long long)p0 * slot_floats, Cw, Cw, fw, (long long)d * slot_floats, same);
+    if (run_stage(h, st, s, n, taps, s.Wrot[r], &s.tc_rot[r], sb.tmp, ring + (long long)hs * slot_floats, same, sb.act))
+      return 1;
     bout = (i < L - 1) ? slot_ptr(i + 1) : sb.fin;
     if (run_block(h, st, h->blocks[i], sb.act, n, sb.bb, bout)) return 1;
   }
-  {
-    Lookup Lk{h};
-    const int Cl = C << L;
-    const float* ws = Lk.get("shrink.weight", (int64_t)3 * Cl);
-    if (!Lk.ok) return 1;
-    shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(bout, Cl, ws, y, rows, Cl);
-    h->launches++;
-  }
+  if (launch_shrink(h, st, bout, y, rows, nullptr, nullptr)) return 1;
   CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -49,7 +49,7 @@ static bool want_grad(TCtx& c, const std::string& key, int64_t numel, float** ou
 // (K % 16: the expand conv) stay on FFMA.
 static const TcWeights* train_tcw(TCtx& c, const float* W, int N, int K) {
   const size_t slot = (size_t)c.tc_slot++;
-  if (c.h->gemm_core != 0 || !c.h->train_tc_on) return nullptr;
+  if (c.h->gemm_core != 0) return nullptr;
   if (c.h->train_tc.size() <= slot) c.h->train_tc.resize(slot + 1);
   TcWeights& t = c.h->train_tc[slot];
   if (tc_prepare_weights(t, W, N, K, c.st, &c.h->owned)) return nullptr;
@@ -61,12 +61,8 @@ static int dense_nt(TCtx& c, const float* A, int lda, const float* W, long long 
                     const float* bias = nullptr) {
   if (c.dry || M <= 0) return 0;
   GemmP p;
-  memset(&p, 0, sizeof(p));
-  p.F = (int)M; p.J = 1; p.fpt = 128;
-  p.res_map = RowMap{1, 1, 1, 0};
-  p.nseg = 1;
-  p.seg[0].base = A; p.seg[0].ld = lda; p.seg[0].K = K; p.seg[0].Kc = K; p.seg[0].tap_stride = 0;
-  p.seg[0].map = RowMap{1, 1, 1, 0};
+  gemm_flat(p, M);
+  p.nseg = 1; p.seg[0] = seg_flat(A, lda, K);
   p.W = W; p.ldw = K; p.N = N; p.out = out; p.ld_out = ldo; p.bias = bias;
   return launch_gemm(c.h, c.st, EPI_PLAIN, p, train_tcw(c, W, N, K));
 }
@@ -430,8 +426,7 @@ static int train_forward(gast_handle* h, TCtx& c, TrainState& ts, const float* x
     if (!c.L->ok) return 1;
     cudaMemsetAsync(ts.Acol, 0, sizeof(float) * (size_t)M0 * KP, c.st);
     cudaMemsetAsync(ts.We8, 0, sizeof(float) * (size_t)C * KP, c.st);
-    ASeg sg; sg.base = ts.xbn; sg.ld = Fin; sg.K = k0 * Fin; sg.Kc = Fin; sg.tap_stride = (long long)J * Fin;
-    sg.map = RowMap{g.T0, T, g.s0, 0};
+    const ASeg sg = seg_taps(ts.xbn, Fin, Fin, k0, (long long)J * Fin, RowMap{g.T0, T, g.s0, 0});
     seg_gather_kernel<<<cdiv(M0 * sg.K, 256), 256, 0, c.st>>>(sg, J, F0, ts.Acol, KP, 0);
     BnP none{nullptr, nullptr, nullptr, nullptr};
     // We8[c][tap*Fin + i] = w[c][i][tap]  (fold_conv_kernel with no BN is exactly this re-layout)
@@ -468,8 +463,7 @@ static int train_forward(gast_handle* h, TCtx& c, TrainState& ts, const float* x
       BnP none{nullptr, nullptr, nullptr, nullptr};
       fold_conv_kernel<<<cdiv((long long)Cw * Cw * sc.taps, 256), 256, 0, c.st>>>(s.Wt, nullptr, w0, Cw, Cw, sc.taps, none);
     }
-    ASeg sg; sg.base = cur; sg.ld = Cw; sg.K = sc.taps * Cw; sg.Kc = Cw; sg.tap_stride = (long long)sc.dil * J * Cw;
-    sg.map = s.tapmap;
+    const ASeg sg = seg_taps(cur, Cw, Cw, sc.taps, (long long)sc.dil * J * Cw, s.tapmap);
     if (seg_gemm(c, &sg, 1, s.Wt, sc.taps * Cw, Fn, Cw, s.Z1, Cw)) return 1;
     if (bn_fwd(c, s.bnA, "layers_bn." + std::to_string(2 * (i - 1)) + ".", s.Z1, Cw, Mn, Cw, 1, 0.f, ts, nullptr, 0, id,
                s.Hh, Cw)) return 1;
@@ -521,7 +515,7 @@ static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* 
     float* dWt = c.fl((size_t)Cw * s.taps * Cw);
     if (!c.dry) {
       cudaMemsetAsync(dXin, 0, sizeof(float) * (size_t)Mi * Cw, c.st);
-      ASeg rs; rs.base = dXin; rs.ld = Cw; rs.K = Cw; rs.Kc = Cw; rs.tap_stride = 0; rs.map = s.resmap;
+      const ASeg rs = seg_taps(dXin, Cw, Cw, 1, 0, s.resmap);
       seg_scatter_add_kernel<<<cdiv(Mn * Cw, 256), 256, 0, c.st>>>(rs, J, s.Fout, dSout, Cw, 0);
     }
     if (bn_bwd(c, s.bnB, dSout, Cw, dZ2, Cw)) return 1;
@@ -534,8 +528,7 @@ static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* 
       if (dense_nn(c, dZ2, Cw, w1, Cw, Mn, Cw, Cw, dHh, Cw)) return 1;
     }
     if (bn_bwd(c, s.bnA, dHh, Cw, dZ1, Cw)) return 1;
-    ASeg sg; sg.base = s.X; sg.ld = Cw; sg.K = s.taps * Cw; sg.Kc = Cw; sg.tap_stride = (long long)s.dil * J * Cw;
-    sg.map = s.tapmap;
+    const ASeg sg = seg_taps(s.X, Cw, Cw, s.taps, (long long)s.dil * J * Cw, s.tapmap);
     if (!c.dry && c.pgrad) seg_gather_kernel<<<cdiv(Mn * sg.K, 256), 256, 0, c.st>>>(sg, J, s.Fout, Xcol, s.taps * Cw, 0);
     if (dense_tn(c, dZ1, Cw, Xcol, s.taps * Cw, Mn, Cw, s.taps * Cw, dWt, s.taps * Cw)) return 1;
     if (dense_nn(c, dZ1, Cw, s.Wt, s.taps * Cw, Mn, Cw, s.taps * Cw, dXcol, s.taps * Cw)) return 1;
@@ -570,8 +563,7 @@ static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* 
   if (!c.dry) {
     if (gwe) conv_wgrad_relayout_kernel<<<cdiv((long long)C * Fin * k0, 256), 256, 0, c.st>>>(dWe8, C, Fin, k0, KP, gwe);
     cudaMemsetAsync(dxbn, 0, sizeof(float) * (size_t)Min * Fin, c.st);
-    ASeg sg; sg.base = dxbn; sg.ld = Fin; sg.K = k0 * Fin; sg.Kc = Fin; sg.tap_stride = (long long)J * Fin;
-    sg.map = RowMap{ts.T0, ts.T, ts.s0, 0};
+    const ASeg sg = seg_taps(dxbn, Fin, Fin, k0, (long long)J * Fin, RowMap{ts.T0, ts.T, ts.s0, 0});
     seg_scatter_add_kernel<<<cdiv(M0 * sg.K, 256), 256, 0, c.st>>>(sg, J, F0, dAcol, KP, 0);
   }
   // init_bn: dx = dxbn . gamma . invstd (frozen), the batch-statistics adjoint otherwise

@@ -129,13 +129,17 @@ class _Handle(object):
         except Exception:
             pass
 
+    def apply_core(self):
+        """hand the set_gemm_core() choice to the library handle (every forward, training or eval)"""
+        if _FORCE_CORE['core'] != self.core:
+            _check(self.lib.gast_set_gemm_core(self.h, _FORCE_CORE['core']), 'gast_set_gemm_core')
+            self.core = _FORCE_CORE['core']
+
     def refresh(self, module, stream):
         """(re)bind + prepare when any parameter/buffer moved or changed."""
         items = named_tensors(module)
         sig = tuple((v.data_ptr(), v._version) for _, v in items)
-        if _FORCE_CORE['core'] != self.core:
-            _check(self.lib.gast_set_gemm_core(self.h, _FORCE_CORE['core']), 'gast_set_gemm_core')
-            self.core = _FORCE_CORE['core']
+        self.apply_core()
         if sig == self.sig:
             return
         n = len(items)
@@ -157,6 +161,7 @@ class _Handle(object):
 
     def bind_only(self, module):
         """bind parameter/buffer storage without the eval-mode prepare (training path)"""
+        self.apply_core()
         items = named_tensors(module)
         n = len(items)
         keys = (C.c_char_p * n)()

@@ -117,7 +117,8 @@ def test_against_oracle_random_shapes(core):
             (17, [3, 3, 3], 32, 1, 33, False, False),
             (19, [3, 3], 32, 3, 11, False, True),
             (15, [3, 3, 3], 16, 2, 27, True, True),
-            (17, [3, 3, 3], 64, 9, 27, False, False)]:
+            (17, [3, 3, 3], 64, 9, 27, False, False),
+            (17, [3, 3], 1056, 3, 9, True, False)]:        # > 1024 channels: two channel chunks in the expand
         meta = dict(J=J, filter_widths=fw, channels=ch, strided=strided, causal=causal, dense=False, seed=11)
         from model.gast_net import SpatioTemporalModel, SpatioTemporalModelOptimized1f
         cls = SpatioTemporalModelOptimized1f if strided else SpatioTemporalModel

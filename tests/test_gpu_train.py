@@ -182,6 +182,26 @@ def test_one_adam_amsgrad_step_matches_reference_port():
     assert checked > 100000
 
 
+def test_gemm_core_choice_reaches_training():
+    """engine.set_gemm_core(1) puts the training GEMMs on the FFMA core, as it does those of the eval forward"""
+    from gast_b200 import engine
+    from model.gast_net import SpatioTemporalModelOptimized1f
+    x = torch.from_numpy(synth.synth_input(4, 27, 17, 2, seed=3)).cuda()
+    tc = {}
+    try:
+        for core in (0, 1):
+            engine.set_gemm_core(core)
+            m = SpatioTemporalModelOptimized1f(_adj(17), 17, 2, 17, [3, 3, 3], dropout=0.0, channels=32)
+            synth.randomize_module(m, 5)
+            m = m.cuda().train()
+            m(x).sum().backward()
+            h = list(m.__dict__['_gast_handles'].values())[0]
+            tc[core] = int(h.lib.gast_last_tc_launch_count(h.h))     # counted since the handle was created
+    finally:
+        engine.set_gemm_core(0)
+    assert tc[0] > 0 and tc[1] == 0, tc
+
+
 def test_dropout_and_mode_errors():
     from model.gast_net import SpatioTemporalModel, SpatioTemporalModelOptimized1f
     m = SpatioTemporalModelOptimized1f(_adj(17), 17, 2, 17, [3, 3, 3], dropout=0.25, channels=32).cuda().train()

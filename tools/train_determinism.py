@@ -1,6 +1,8 @@
 """GPU diagnostic: run-to-run determinism of the training gradients (same weights, same batch, two runs) and the
 fraction of parameter entries that differ after three Adam(amsgrad) steps between two identically-seeded trainers
-(eager vs eager, eager vs CUDA graph).  Run once with GAST_TRAIN_TC=1 and once with GAST_TRAIN_TC=0."""
+(eager vs eager, eager vs CUDA graph), on one GEMM core.
+
+    python tools/train_determinism.py [channels] [core]     core: 0 = tensor cores where possible (default), 1 = FFMA"""
 import os
 import sys
 import torch
@@ -8,7 +10,7 @@ import torch
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(REPO, 'gast-net-3dposeestimation_b200'))
 sys.path.insert(0, REPO)
-from gast_b200 import synth  # noqa: E402
+from gast_b200 import engine, synth  # noqa: E402
 from gast_b200.trainer import DataParallelTrainer, GraphedTrainer  # noqa: E402
 from gast_b200.pipeline import FusedAdam  # noqa: E402
 from common.skeleton import Skeleton  # noqa: E402
@@ -35,15 +37,24 @@ def grads_once(m, x, y):
     return {k: p.grad.detach().clone() for k, p in m.named_parameters()}, float(loss)
 
 
+def tc_launches(m):
+    """tensor-core GEMM launches the model's handle has counted (0 when every training GEMM ran on FFMA)"""
+    h = list(m.__dict__['_gast_handles'].values())[0]
+    return int(h.lib.gast_last_tc_launch_count(h.h))
+
+
 def main():
     ch = int(sys.argv[1]) if len(sys.argv) > 1 else 32
+    core = int(sys.argv[2]) if len(sys.argv) > 2 else 0
+    engine.set_gemm_core(core)
     B = 16
-    print('GAST_TRAIN_TC=%s channels=%d' % (os.environ.get('GAST_TRAIN_TC', '1'), ch))
+    print('gemm core %d channels=%d' % (core, ch))
     x = torch.from_numpy(synth.synth_input(B, 27, J, 2, seed=40)).cuda()
     y = torch.from_numpy(synth.synth_target(B, J, seed=50)).cuda()
     m = make(ch)
     sd = {k: v.clone() for k, v in m.state_dict().items()}
     g1, l1 = grads_once(m, x, y)
+    print('tensor-core GEMM launches in the first training step: %d' % tc_launches(m))
     m.load_state_dict(sd)
     g2, l2 = grads_once(m, x, y)
     nd = [(k, float((g1[k] - g2[k]).abs().max()), float(g1[k].abs().max())) for k in g1 if not torch.equal(g1[k], g2[k])]
