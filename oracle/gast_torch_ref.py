@@ -31,6 +31,13 @@ def _bn(x, p, prefix, training, stats):
                         p[prefix + 'weight'], p[prefix + 'bias'], training, BN_MOMENTUM, BN_EPS)
 
 
+def _relu(h, tap, name):
+    """F.relu, first showing its input to `tap(name, input)` when one is given (name: the BatchNorm's prefix)"""
+    if tap is not None:
+        tap(name, h)
+    return F.relu(h)
+
+
 def semch(x, W, e, mask, bias=None):
     """SemCHGraphConv.forward (model/local_attention.py:35-53)."""
     Cout = W.shape[2]
@@ -46,20 +53,21 @@ def semch(x, W, e, mask, bias=None):
     return out if bias is None else out + bias.view(1, 1, -1)
 
 
-def local_graph(x, p, prefix, masks, training=False, stats=None, drop=0.0):
+def local_graph(x, p, prefix, masks, training=False, stats=None, drop=0.0, tap=None):
     """LocalGraph.forward (model/local_attention.py:130-151)."""
     sym, con = masks
     a = semch(x, p[prefix + 'gcn_sym.W'], p[prefix + 'gcn_sym.e'], sym).permute(0, 3, 1, 2)
     b = semch(x, p[prefix + 'gcn_con.W'], p[prefix + 'gcn_con.e'], con).permute(0, 3, 1, 2)
-    a = F.relu(_bn(a, p, prefix + 'bn_1.', training, stats))
-    b = F.relu(_bn(b, p, prefix + 'bn_2.', training, stats))
+    a = _relu(_bn(a, p, prefix + 'bn_1.', training, stats), tap, prefix + 'bn_1.')
+    b = _relu(_bn(b, p, prefix + 'bn_2.', training, stats), tap, prefix + 'bn_2.')
     o = torch.cat((a, b), dim=1)
-    o = F.relu(_bn(F.conv2d(o, p[prefix + 'cat_conv.weight']), p, prefix + 'cat_bn.', training, stats))
+    o = _relu(_bn(F.conv2d(o, p[prefix + 'cat_conv.weight']), p, prefix + 'cat_bn.', training, stats), tap,
+              prefix + 'cat_bn.')
     o = F.dropout(o, drop, training)
     return o.permute(0, 2, 3, 1)
 
 
-def global_graph(x, p, prefix):
+def global_graph(x, p, prefix, tap=None):
     """GlobalGraph.forward (model/global_attention.py:52-82); x: (BT, C, N)."""
     bsz = x.size(0)
     g_x = F.conv1d(x, p[prefix + 'g.weight'], p[prefix + 'g.bias']).permute(0, 2, 1)
@@ -69,40 +77,47 @@ def global_graph(x, p, prefix):
     theta_x = theta.view(bsz, Ci, -1, 1).expand(-1, -1, -1, N)
     phi_x = phi.view(bsz, Ci, 1, -1).expand(-1, -1, N, -1)
     concat = torch.cat([theta_x, phi_x], dim=1)                        # :71 (materialised)
-    f = F.conv2d(concat, p[prefix + 'concat_project.0.weight'])        # :72
-    att = F.leaky_relu(f.view(bsz, N, N), 0.2)                         # :74
+    f = F.conv2d(concat, p[prefix + 'concat_project.0.weight']).view(bsz, N, N)   # :72
+    if tap is not None:
+        tap(prefix, f)                                                 # the LeakyReLU input (the logits)
+    att = F.leaky_relu(f, 0.2)                                         # :74
     att = torch.add(F.softmax(att, dim=-1), p[prefix + 'C_k'])         # :76
     y = torch.matmul(att, g_x).permute(0, 2, 1).contiguous()           # :78-79
     return y
 
 
-def multi_global_graph(x, p, prefix, training=False, stats=None, drop=0.0):
+def multi_global_graph(x, p, prefix, training=False, stats=None, drop=0.0, tap=None):
     """MultiGlobalGraph.forward (model/global_attention.py:103-130)."""
     B, T, J, C = x.shape
     xf = x.contiguous().view(-1, J, C).permute(0, 2, 1)
     heads = 0
     while (prefix + 'attentions.%d.C_k' % heads) in p:
         heads += 1
-    y = torch.cat([global_graph(xf, p, prefix + 'attentions.%d.' % h) for h in range(heads)], dim=1)
+    y = torch.cat([global_graph(xf, p, prefix + 'attentions.%d.' % h, tap) for h in range(heads)], dim=1)
     y = y.permute(0, 2, 1).contiguous().view(B, T, J, C).permute(0, 3, 1, 2)
-    y = F.relu(_bn(F.conv2d(y, p[prefix + 'cat_conv.weight']), p, prefix + 'cat_bn.', training, stats))
+    y = _relu(_bn(F.conv2d(y, p[prefix + 'cat_conv.weight']), p, prefix + 'cat_bn.', training, stats), tap,
+              prefix + 'cat_bn.')
     y = F.dropout(y, drop, training)
     return y.permute(0, 2, 3, 1)
 
 
-def graph_attention_block(x, p, prefix, masks, training=False, stats=None, drop=0.0):
+def graph_attention_block(x, p, prefix, masks, training=False, stats=None, drop=0.0, tap=None):
     """GraphAttentionBlock.forward (model/gast_net.py:22-33); x: (B,C,T,N)."""
     xl = x.permute(0, 2, 3, 1)
-    a = local_graph(xl, p, prefix + 'local_graph_layer.', masks, training, stats, drop)
-    g = multi_global_graph(xl, p, prefix + 'global_graph_layer.', training, stats, drop)
+    a = local_graph(xl, p, prefix + 'local_graph_layer.', masks, training, stats, drop, tap)
+    g = multi_global_graph(xl, p, prefix + 'global_graph_layer.', training, stats, drop, tap)
     cat = torch.cat((xl, a, g), dim=-1).permute(0, 3, 1, 2)
-    return F.relu(_bn(F.conv2d(cat, p[prefix + 'cat_conv.weight']), p, prefix + 'cat_bn.', training, stats))
+    return _relu(_bn(F.conv2d(cat, p[prefix + 'cat_conv.weight']), p, prefix + 'cat_bn.', training, stats), tap,
+                 prefix + 'cat_bn.')
 
 
 def forward(x, p, masks, filter_widths, causal=False, strided=False, dense=False,
-            training=False, stats=None, drop=0.0):
+            training=False, stats=None, drop=0.0, tap=None):
     """SpatioTemporalModel / SpatioTemporalModelOptimized1f forward (model/gast_net.py:84-104,
-    159-177, 236-251).  x: (B,T,J,F) -> (B,T_out,J,3)."""
+    159-177, 236-251).  x: (B,T,J,F) -> (B,T_out,J,3).
+    `tap(name, h)`, when given, sees every kink input in forward order without changing anything: each ReLU input
+    (name: the prefix of the BatchNorm in front of it) and each head's attention logits before the LeakyReLU (name:
+    the head's prefix, h of shape (BT, J, J))."""
     fw = filter_widths
     pad = [fw[0] // 2]
     shift = [(fw[0] // 2) if causal else 0]
@@ -120,19 +135,19 @@ def forward(x, p, masks, filter_widths, causal=False, strided=False, dense=False
     h = x.permute(0, 3, 1, 2)
     h = _bn(h, p, 'init_bn.', training, stats)
     h = F.conv2d(h, p['expand_conv.weight'], stride=(fw[0], 1) if strided else (1, 1))
-    h = F.relu(_bn(h, p, 'expand_bn.', training, stats))
-    h = graph_attention_block(h, p, 'layers_graph_conv.0.', masks, training, stats, drop)
+    h = _relu(_bn(h, p, 'expand_bn.', training, stats), tap, 'expand_bn.')
+    h = graph_attention_block(h, p, 'layers_graph_conv.0.', masks, training, stats, drop, tap)
     for i, g in enumerate(geo):
         if strided:
             res = h[:, :, shift[i + 1] + fw[i + 1] // 2:: fw[i + 1]]
         else:
             res = h[:, :, pad[i + 1] + shift[i + 1]: h.shape[2] - pad[i + 1] + shift[i + 1]]
-        h = F.relu(_bn(F.conv2d(h, p['layers_conv.%d.weight' % (2 * i)], **g), p, 'layers_bn.%d.' % (2 * i),
-                       training, stats))
-        h = F.relu(_bn(F.conv2d(h, p['layers_conv.%d.weight' % (2 * i + 1)]), p, 'layers_bn.%d.' % (2 * i + 1),
-                       training, stats))
+        h = _relu(_bn(F.conv2d(h, p['layers_conv.%d.weight' % (2 * i)], **g), p, 'layers_bn.%d.' % (2 * i),
+                      training, stats), tap, 'layers_bn.%d.' % (2 * i))
+        h = _relu(_bn(F.conv2d(h, p['layers_conv.%d.weight' % (2 * i + 1)]), p, 'layers_bn.%d.' % (2 * i + 1),
+                      training, stats), tap, 'layers_bn.%d.' % (2 * i + 1))
         h = res + F.dropout(h, drop, training)
-        h = graph_attention_block(h, p, 'layers_graph_conv.%d.' % (i + 1), masks, training, stats, drop)
+        h = graph_attention_block(h, p, 'layers_graph_conv.%d.' % (i + 1), masks, training, stats, drop, tap)
     y = F.conv2d(h, p['shrink.weight'])
     return y.permute(0, 2, 3, 1)
 
