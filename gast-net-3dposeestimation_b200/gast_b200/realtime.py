@@ -7,6 +7,12 @@ ring of that stage's past inputs for all streams (`csrc/stream.cuh`, C ABI `gast
 computes one new position per layer.  A stream's first frame stands for its whole (edge-padded) history exactly
 like `UnchunkedGenerator(pad, causal_shift=pad)` does (`common/generators.py:210-221`).
 
+The rings hold activations computed with the weights of the pushes that wrote them.  Any change to the model's
+parameters or buffers (`load_state_dict`, an optimiser step, a training forward, which moves the BatchNorm running
+statistics) therefore invalidates the history of every stream: the next push raises `GastError` unless `reset()`
+(every stream) was called after the change.  Switching the GEMM core (`engine.set_gemm_core`) changes no weight and
+keeps the streams.
+
 `WindowStream` is the generic form for any callable network: a device ring of the last `rf` input frames and one
 window forward per pushed frame (what the reference does; used for non-GAST callables and as the cross-check).
 """
@@ -39,6 +45,8 @@ class CausalStream(object):
         self.step = 0
         self.fresh = torch.ones(self.n, dtype=torch.int32, device=self.device)     # every stream starts anew
         self._any_fresh = True
+        self._all_fresh = True           # host-side: every stream starts anew at the next push (no device sync)
+        self._sig = None                 # the handle's parameter signature at the last push
         self._state = None
         self._ws = None
 
@@ -46,6 +54,7 @@ class CausalStream(object):
         """Forget the history of all (or the listed) streams: their next frame starts a new sequence."""
         if streams is None:
             self.fresh.fill_(1)
+            self._all_fresh = True
         else:
             self.fresh[torch.as_tensor(streams, device=self.device, dtype=torch.long)] = 1
         self._any_fresh = True
@@ -64,6 +73,10 @@ class CausalStream(object):
         with torch.cuda.device(self.device):
             st = torch.cuda.current_stream(self.device).cuda_stream
             h.refresh(self.model, st)
+            if self._sig is not None and h.sig != self._sig and not self._all_fresh:
+                raise eng.GastError('CausalStream: the model\'s parameters or buffers changed since the last push '
+                                    '(load_state_dict, an optimiser step or a training forward); the streams\' history '
+                                    'was computed with the old weights -- call reset() before pushing again')
             if self._state is None:
                 nb = lib.gast_stream_state_bytes(h.h, self.n)
                 wb = lib.gast_stream_workspace_bytes(h.h, self.n)
@@ -81,6 +94,8 @@ class CausalStream(object):
             if self._any_fresh:
                 self.fresh.zero_()                       # (stream-ordered after the push that read it)
                 self._any_fresh = False
+                self._all_fresh = False
+            self._sig = h.sig
         self.step += 1
         self.last_launches = int(lib.gast_last_launch_count(h.h))
         return y

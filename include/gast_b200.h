@@ -183,7 +183,11 @@ int gast_set_dropout_state(gast_t* h, void* dev_u64);
  *   replicating the stream's first frame (UnchunkedGenerator(pad, causal_shift=pad), common/generators.py:210-221).
  *   step = number of frames pushed into `state` before this one (0, 1, 2, ...; the caller counts).
  *   fresh (n_streams) int32 on the device, or null: non-zero = this frame starts a new sequence on that stream
- *   (must be non-zero for every stream at step 0).  MODEL handles with causal = 1 only; all work on `stream`. */
+ *   (must be non-zero for every stream at step 0).  MODEL handles with causal = 1 only; all work on `stream`.
+ *   The rings hold layer inputs computed with the weights of the pushes that wrote them.  A gast_prepare (after
+ *   new weights or BatchNorm statistics were bound) therefore invalidates `state`: unless the next push marks
+ *   every stream fresh, it mixes old and new weights for up to receptive_field - 1 pushes.  Nothing checks this
+ *   here; gast_b200.realtime.CausalStream refuses such a push.  gast_set_gemm_core does not invalidate `state`. */
 size_t gast_stream_state_bytes(gast_t* h, int32_t n_streams);
 size_t gast_stream_workspace_bytes(gast_t* h, int32_t n_streams);
 int gast_stream_push(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,

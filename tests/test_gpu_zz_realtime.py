@@ -8,9 +8,17 @@ import torch
 from conftest import load_golden
 from gast_b200 import synth
 from gast_b200.realtime import CausalStream, WindowStream
-from test_gpu_parity import build_model, TOL
+from test_gpu_parity import build_model
 
 pytestmark = pytest.mark.gpu
+
+# Absolute bars, about 4x the worst over both GEMM cores measured on an H100 80GB HBM3 (400 W power limit): stream
+# against the whole-sequence forward 1.0e-6, against the stream_* goldens 5.0e-6 (the goldens' own fp32 rounding is
+# about 2e-6 of max |y|, tests/test_streamref_cpu.py), O(1) rings against window recomputation 3.6e-6 (max |y| 3.1).
+# tests/test_gpu_zz_stream_exact.py holds every push to fp64.
+WHOLE_TOL = 5e-6
+GOLDEN_TOL = 2e-5
+WINDOW_TOL = 1.5e-5
 
 
 def test_causal_stream_equals_full_sequence_forward():
@@ -28,7 +36,7 @@ def test_causal_stream_equals_full_sequence_forward():
     with torch.no_grad():
         want = mfull(torch.from_numpy(padded).cuda())
     assert want.shape == got.shape == (n, T, 17, 3)
-    assert (got - want).abs().max().item() < TOL
+    assert (got - want).abs().max().item() < WHOLE_TOL
 
 
 @pytest.mark.parametrize('name', ['stream_17_333_c32_causal', 'stream_17_333_c128_causal', 'stream_17_3333_c64_causal'])
@@ -48,11 +56,11 @@ def test_causal_stream_vs_reference_golden(name):
     cs = CausalStream(m, n_streams=x.shape[0])
     got = torch.stack([cs.push(torch.from_numpy(x[:, t]).cuda()) for t in range(x.shape[1])], dim=1).cpu().numpy()
     err = float(np.abs(got - y).max())
-    assert err < TOL, err
+    assert err < GOLDEN_TOL, err
     # a stream that restarts: same outputs again
     cs.reset()
     again = torch.stack([cs.push(torch.from_numpy(x[:, t]).cuda()) for t in range(5)], dim=1).cpu().numpy()
-    assert np.abs(again - y[:, :5]).max() < TOL
+    assert np.abs(again - y[:, :5]).max() < GOLDEN_TOL
 
 
 def test_o1_stream_matches_window_recompute_with_staggered_resets():
@@ -77,7 +85,7 @@ def test_o1_stream_matches_window_recompute_with_staggered_resets():
             a.reset([0]); b.reset([0])
         ya, yb = a.push(seqs[:, t]), b.push(seqs[:, t])
         worst = max(worst, (ya - yb).abs().max().item())
-    assert worst < 2e-5, worst
+    assert worst < WINDOW_TOL, worst
     assert a.last_launches < 60                       # one position per layer: ~40 launches per frame, any n
     with pytest.raises(RuntimeError, match='causal'):
         CausalStream(SpatioTemporalModelOptimized1f(_adj(17), 17, 2, 17, [3, 3, 3], channels=32).cuda().eval(), 2)
