@@ -1,4 +1,4 @@
-// O(1)-per-frame causal streaming of the lifting network (SURVEY.md §8f N4; the reference's real-time path is a
+// O(1)-per-frame streaming of the lifting network (SURVEY.md §8f N4; the reference's real-time path is a
 // causal SpatioTemporalModelOptimized1f re-run on the last `receptive_field` frames for every new frame,
 // gen_skes.py:43-69, tools/inference.py:19-110).  Included by gast_api.cu (uses its helpers).
 //
@@ -7,6 +7,20 @@
 // (gast_net.py:139-143,167-174: with causal_shift = pad the residual slice and the last tap are both the newest
 // position), and the blocks are pointwise in time.  So a pushed frame needs ONE new position per layer, given the
 // layer inputs of the past: per stage a ring of R_i = w_i d_i slots holding G_{i-1}, slot = frame index mod R_i.
+//
+// Non-causal models (causal_shift = 0, gast_net.py:167-174,242-247).  Index every layer by the push that completes
+// its window instead of by the frame it is centred on.  Then the taps are the same w_i positions t - (w_i-1) d_i ... t
+// and the only change is the residual: the centre tap t - (w_i/2) d_i instead of the newest one.  So the rings, the
+// tap rotation and the weights are shared with the causal form.  The one exception is the residual slot,
+// (hs + R_i - (w_i/2) d_i) mod R_i.  The lags add up: the output of push t is the pose of frame t - pad, where
+// pad = (rf-1)/2 (the latency).  The generator (common/generators.py:210-221) pads a sequence with pad copies of its
+// first frame on the left and pad copies of its last frame on the right.
+//   * Left: fill-fresh (below) gives a stream an infinite history of copies of its first frame.  The window of
+//     frame t >= 0 reaches back to frame t - pad >= -pad, and that is all the left padding it sees.  The first `pad`
+//     outputs after a start belong to frames before 0 and are dropped by the caller.
+//   * Right: a HELD stream (`hold` mask) re-appends its own newest input frame instead of reading x.  After the last
+//     frame, `pad` held pushes are exactly the right padding and return the last `pad` poses.  This also holds for
+//     a sequence shorter than pad: a window then sees only padding beyond the sequence, as in the generator.
 //
 // Layout: rings are SLOT-major, ring_i[slot][stream][joint][channel], so that
 //   * a slot is an ordinary contiguous (n_streams*J, C) activation matrix: the producing block writes it directly;
@@ -24,14 +38,17 @@
 namespace gast {
 
 // xhist (n, k0, J, F): the last k0 input frames of every stream, oldest first.  One thread per (stream, joint, feature).
+// A held stream (hold[b] != 0, fresh[b] == 0) appends its own newest frame again and ignores x.
 __global__ void stream_xpush_kernel(float* __restrict__ xhist, const float* __restrict__ x,
-                                    const int32_t* __restrict__ fresh, int n, int k0, int JF) {
+                                    const int32_t* __restrict__ fresh, const int32_t* __restrict__ hold, int n, int k0,
+                                    int JF) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n * JF) return;
   const int b = idx / JF, e = idx - b * JF;
   float* hrow = xhist + (long long)b * k0 * JF + e;
-  const float v = x[idx];
-  if (fresh && fresh[b]) {
+  const bool is_fresh = fresh && fresh[b];
+  const float v = (hold && hold[b] && !is_fresh) ? hrow[(long long)(k0 - 1) * JF] : x[idx];
+  if (is_fresh) {
     for (int k = 0; k < k0; ++k) hrow[(long long)k * JF] = v;
   } else {
     for (int k = 0; k + 1 < k0; ++k) hrow[(long long)k * JF] = hrow[(long long)(k + 1) * JF];
@@ -78,8 +95,6 @@ struct StreamPlan {
 
 static int stream_check(const gast_handle* h) {
   if (h->cfg.kind != GAST_KIND_MODEL) return fail("streaming is implemented for the MODEL kind only");
-  if (!h->cfg.causal) return fail("streaming needs a causal model (gen_skes.py:59: causal=True): a non-causal network "
-                                  "has no output for the newest frame");
   if (h->cfg.dense) return fail("the dense ablation has no streaming form");
   // checked before a push touches the stream state (launch_expand checks it again for the forward)
   if (h->cfg.filter_widths[0] * h->cfg.in_features > EXP_MAXKF)
@@ -160,11 +175,17 @@ static int stream_prepare(gast_handle* h, cudaStream_t st) {
   return 0;
 }
 
-extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
-                                const int32_t* fresh, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h) return fail("gast_stream_push: null handle");
-  if (!h->prepared) return fail("gast_stream_push: gast_prepare() has not run since the last gast_bind()");
-  if (step < 0 || !state || !x || !y) return fail("gast_stream_push: bad arguments");
+extern "C" int32_t gast_stream_latency(const gast_t* h) {
+  if (!h || stream_check(h)) return -1;
+  return h->cfg.causal ? 0 : (gast_receptive_field(h) - 1) / 2;
+}
+
+extern "C" int gast_stream_push_ex(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
+                                   const int32_t* fresh, const int32_t* hold, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+  if (!h) return fail("gast_stream_push_ex: null handle");
+  if (!h->prepared) return fail("gast_stream_push_ex: gast_prepare() has not run since the last gast_bind()");
+  if (step < 0 || !state || !x || !y) return fail("gast_stream_push_ex: bad arguments");
   StreamPlan sp;
   if (stream_plan(h, n_streams, &sp)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -172,7 +193,7 @@ extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const floa
   if (!h->stream_ready && stream_prepare(h, st)) return 1;
   const size_t need = gast_stream_workspace_bytes(h, n_streams);
   if (!workspace || workspace_bytes < need)
-    return fail("gast_stream_push: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+    return fail("gast_stream_push_ex: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
   h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
   const gast_cfg& c = h->cfg;
   const int n = n_streams, J = c.num_joints, C = c.channels, L = c.num_stages, k0 = c.filter_widths[0], Fin = c.in_features;
@@ -183,7 +204,7 @@ extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const floa
   const long long rows = (long long)n * J;
   // input history + expand (gast_net.py:163-164) on the last k0 frames
   float* xhist = sbase + sp.xhist_off;
-  stream_xpush_kernel<<<cdiv((long long)n * J * Fin, 256), 256, 0, st>>>(xhist, x, fresh, n, k0, J * Fin);
+  stream_xpush_kernel<<<cdiv((long long)n * J * Fin, 256), 256, 0, st>>>(xhist, x, fresh, hold, n, k0, J * Fin);
   h->launches++;
   if (launch_expand(h, st, xhist, sb.E, rows, k0, 1, 1)) return 1;
   auto slot_ptr = [&](int i /*stage 1..L-1*/) {
@@ -204,10 +225,12 @@ extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const floa
       h->launches++;
     }
     // taps = slots p0 + k d with the weights rotated to slot order; residual = the newest slot (causal_shift = pad)
+    // or the centre tap (causal_shift = 0)
     const int p0 = hs % d, r = hs / d;
+    const int rs = c.causal ? hs : (hs + R - (fw / 2) * d) % R;
     const RowMap same{n, n, 1, 0};
     const ASeg taps = seg_taps(ring + (long long)p0 * slot_floats, Cw, Cw, fw, (long long)d * slot_floats, same);
-    if (run_stage(h, st, s, n, taps, s.Wrot[r], &s.tc_rot[r], sb.tmp, ring + (long long)hs * slot_floats, same, sb.act))
+    if (run_stage(h, st, s, n, taps, s.Wrot[r], &s.tc_rot[r], sb.tmp, ring + (long long)rs * slot_floats, same, sb.act))
       return 1;
     bout = (i < L - 1) ? slot_ptr(i + 1) : sb.fin;
     if (run_block(h, st, h->blocks[i], sb.act, n, sb.bb, bout)) return 1;
@@ -215,4 +238,13 @@ extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const floa
   if (launch_shrink(h, st, bout, y, rows, nullptr, nullptr)) return 1;
   CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
+                                const int32_t* fresh, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h) return fail("gast_stream_push: null handle");
+  if (h->cfg.kind == GAST_KIND_MODEL && !h->cfg.causal)
+    return fail("gast_stream_push needs a causal model (gen_skes.py:59: causal=True): a non-causal network has no "
+                "output for the newest frame (gast_stream_push_ex returns it `latency` pushes later)");
+  return gast_stream_push_ex(h, state, step, x, y, n_streams, fresh, nullptr, workspace, workspace_bytes, stream);
 }

@@ -1,11 +1,19 @@
-"""Frame-by-frame causal lifting of many concurrent keypoint streams (SURVEY.md §8f N4).
+"""Frame-by-frame lifting of many concurrent keypoint streams (SURVEY.md §8f N4).
 
 The reference's real-time model is a causal `SpatioTemporalModelOptimized1f` fed the last `receptive_field`
 frames of one stream for every new frame (`gen_skes.py:43-69`, `tools/inference.py:19-110`): O(rf) work per
-frame.  `CausalStream` produces the same poses with O(1) work per frame: the library keeps, per temporal stage, a
-ring of that stage's past inputs for all streams (`csrc/stream.cuh`, C ABI `gast_stream_push`), so a pushed frame
+frame.  `PoseStream` produces the same poses with O(1) work per frame: the library keeps, per temporal stage, a
+ring of that stage's past inputs for all streams (`csrc/stream.cuh`, C ABI `gast_stream_push_ex`), so a pushed frame
 computes one new position per layer.  A stream's first frame stands for its whole (edge-padded) history exactly
-like `UnchunkedGenerator(pad, causal_shift=pad)` does (`common/generators.py:210-221`).
+like `UnchunkedGenerator` does (`common/generators.py:210-221`).
+
+`PoseStream` takes causal and non-causal models.  A non-causal model returns the pose of frame t - pad when frame t
+is pushed (`latency` = pad = (rf - 1) // 2; 0 for a causal model).  `end()` closes a stream's sequence: its next
+`latency` pushes repeat the last frame (the generator's right padding) and return the remaining poses.  With
+`augment=True` every push also runs the mirrored twin and averages it back, as every inference helper of the
+reference does (`tools/inference.py:19-110`).  The poses of a sequence then equal
+`UnchunkedGenerator([seq], pad, causal_shift, augment)` + `tools/inference.evaluate`.  `CausalStream` is the causal,
+un-augmented restriction that returns the pose of the newest frame.
 
 The rings hold activations computed with the weights of the pushes that wrote them.  Any change to the model's
 parameters or buffers (`load_state_dict`, an optimiser step, a training forward, which moves the BatchNorm running
@@ -17,88 +25,218 @@ keeps the streams.
 window forward per pushed frame (what the reference does; used for non-GAST callables and as the cross-check).
 """
 import ctypes as C
+import numpy as np
 import torch
 
 from . import _lib as L
 
+# left/right keypoint and joint lists of the reference's inference helpers (tools/inference.py:14-15) and of
+# reconstruction.py:get_joints_info for 19 joints (reconstruction.py:185 uses the same lists for the keypoints)
+SYMMETRY = {
+    17: ([4, 5, 6, 11, 12, 13], [1, 2, 3, 14, 15, 16]),
+    19: ([5, 6, 7, 8, 13, 14, 15], [1, 2, 3, 4, 16, 17, 18]),
+}
 
-class CausalStream(object):
-    """O(1)-per-frame lifting of `n_streams` concurrent streams with a causal model of the drop-in classes
-    (`SpatioTemporalModelOptimized1f(causal=True)` as gen_skes.load_model_realtime builds it, or the dilated
-    `SpatioTemporalModel(causal=True)`: the weights are interchangeable)."""
 
-    def __init__(self, model_pos, n_streams, device=None):
+class SequenceBook(object):
+    """Host-side sequence bookkeeping of `n` streams with output latency `latency` (no CUDA, no device sync).
+
+    A stream is LIVE (its pushes append frames to its current sequence), ENDING (`end` was called: its next pushes
+    are held and return the sequence's last poses) or IDLE (held, nothing due).  `advance()` is called once per push
+    and returns the fresh and hold masks of that push and, per stream, the position within the current sequence of
+    the frame whose pose that push returns (-1 where nothing is due)."""
+
+    def __init__(self, n, latency):
+        self.n, self.latency = int(n), int(latency)
+        self.fresh = np.ones(self.n, dtype=bool)            # the next push starts a new sequence
+        self.length = np.zeros(self.n, dtype=np.int64)      # frames in the current sequence
+        self.left = np.full(self.n, -1, dtype=np.int64)     # -1 live; k >= 0: k held pushes left (0 = idle)
+
+    def _sel(self, streams):
+        if streams is None:
+            return slice(None)
+        return np.asarray(streams, dtype=np.int64).reshape(-1)
+
+    def reset(self, streams=None):
+        s = self._sel(streams)
+        self.fresh[s] = True
+        self.length[s] = 0
+        self.left[s] = -1
+
+    def end(self, streams=None):
+        s = np.arange(self.n)[self._sel(streams)]
+        s = s[self.left[s] < 0]                           # already ending or idle: nothing to do
+        empty = self.fresh[s]                             # reset but nothing pushed since: an empty sequence
+        self.fresh[s[empty]] = False
+        self.left[s[empty]] = 0
+        self.left[s[~empty]] = self.latency
+
+    def all_restarting(self):
+        """every stream either starts anew at the next push or is idle (its history is never read again)"""
+        return bool(np.all(self.fresh | (self.left == 0)))
+
+    def advance(self):
+        """-> (fresh, hold, index) of the next push; updates the state as that push does"""
+        fresh = self.fresh.copy()
+        self.length[fresh] = 0
+        self.left[fresh] = -1
+        live = self.left < 0
+        hold = ~live
+        index = np.full(self.n, -1, dtype=np.int64)
+        index[live] = self.length[live] - self.latency
+        self.length[live] += 1
+        ending = self.left > 0
+        # the k-th held push (k = latency - left + 1) returns frame length - 1 + k - latency
+        index[ending] = self.length[ending] - self.left[ending]
+        self.left[ending] -= 1
+        index[index < 0] = -1
+        self.fresh[:] = False
+        return fresh, hold, index
+
+
+class PoseStream(object):
+    """O(1)-per-frame lifting of `n_streams` concurrent streams with any non-dense model of the drop-in classes
+    (`SpatioTemporalModel` or `SpatioTemporalModelOptimized1f`, causal or not: the weights are interchangeable).
+
+    push(frame (n, J, F)) -> (poses (n, J, 3) CUDA, index (n,) CPU int64): poses[s] is the pose of frame index[s] of
+    stream s's current sequence, or unspecified where index[s] == -1.  The kps/joints lists default to the
+    reference's for J = 17 and J = 19; `augment=True` with another J needs all four."""
+
+    def __init__(self, model_pos, n_streams, augment=False, kps_left=None, kps_right=None, joints_left=None,
+                 joints_right=None, device=None):
         from . import engine
-        if not getattr(model_pos, '_gast_causal', False):
-            raise engine.GastError('CausalStream needs a causal model (gen_skes.py:59 builds it with causal=True)')
+        name = type(self).__name__
+        if not hasattr(model_pos, '_gast_causal'):
+            raise engine.GastError('%s needs a model of the drop-in classes (model/gast_net.py)' % name)
+        if getattr(model_pos, '_gast_dense', False):
+            raise engine.GastError('%s: the dense ablation has no streaming form' % name)
         if device is None:
             device = next(model_pos.parameters()).device
         self.device = torch.device(device)
         if self.device.type != 'cuda':
-            raise engine.GastError('CausalStream: the model must be on a CUDA device (there is no CPU path)')
+            raise engine.GastError('%s: the model must be on a CUDA device (there is no CPU path)' % name)
         self.model = model_pos
         self.engine = engine
         self.rf = int(model_pos.receptive_field())
         self.n = int(n_streams)
         self.J = int(model_pos.num_joints_in)
         self.F = int(model_pos.in_features)
+        self.causal = bool(model_pos._gast_causal)
+        self.latency = 0 if self.causal else (self.rf - 1) // 2
+        self.augment = bool(augment)
+        if self.augment:
+            lists = [kps_left, kps_right, joints_left, joints_right]
+            if any(v is None for v in lists):
+                if self.J not in SYMMETRY:
+                    raise engine.GastError('%s: augment=True with %d joints needs kps_left, kps_right, joints_left and '
+                                           'joints_right (defaults exist for 17 and 19 joints)' % (name, self.J))
+                left, right = SYMMETRY[self.J]
+                lists = [d if v is None else v for v, d in zip(lists, [left, right, left, right])]
+            self.kps_left, self.kps_right, self.joints_left, self.joints_right = [[int(i) for i in v] for v in lists]
+            if len(self.kps_left) != len(self.kps_right) or len(self.joints_left) != len(self.joints_right):
+                raise engine.GastError('%s: left and right lists differ in length' % name)
+            arr = lambda v: (C.c_int32 * len(v))(*v)   # noqa: E731
+            self._kl, self._kr = arr(self.kps_left), arr(self.kps_right)
+            self._jl, self._jr = arr(self.joints_left), arr(self.joints_right)
+        self.copies = 2 if self.augment else 1      # streams the library runs: [original | mirrored]
+        self.book = SequenceBook(self.n, self.latency)
         self.step = 0
-        self.fresh = torch.ones(self.n, dtype=torch.int32, device=self.device)     # every stream starts anew
-        self._any_fresh = True
-        self._all_fresh = True           # host-side: every stream starts anew at the next push (no device sync)
+        self._masks = torch.zeros((2, self.copies * self.n), dtype=torch.int32, device=self.device)
         self._sig = None                 # the handle's parameter signature at the last push
         self._state = None
         self._ws = None
 
     def reset(self, streams=None):
-        """Forget the history of all (or the listed) streams: their next frame starts a new sequence."""
-        if streams is None:
-            self.fresh.fill_(1)
-            self._all_fresh = True
-        else:
-            self.fresh[torch.as_tensor(streams, device=self.device, dtype=torch.long)] = 1
-        self._any_fresh = True
+        """Start new sequences on all (or the listed) streams with the next pushed frame; drop any pending tail."""
+        self.book.reset(streams)
+
+    def end(self, streams=None):
+        """The current sequences of all (or the listed) streams ended with their last pushed frame.  Their next
+        `latency` pushes ignore the caller's rows and return the remaining poses; then they are idle until reset."""
+        self.book.end(streams)
+
+    def _upload(self, fresh, hold):
+        """-> device pointers of the fresh and hold masks of this push (None where no stream is set)"""
+        any_f, any_h = bool(fresh.any()), bool(hold.any())
+        if not (any_f or any_h):
+            return None, None
+        mk = np.tile(np.stack([fresh, hold]).astype(np.int32), (1, self.copies))
+        # pinned + non_blocking: no device sync; the caching host allocator keeps the buffer until the copy ran
+        self._masks.copy_(torch.from_numpy(mk).pin_memory(), non_blocking=True)
+        return (self._masks[0].data_ptr() if any_f else None), (self._masks[1].data_ptr() if any_h else None)
 
     def push(self, frame):
         """frame (n_streams, J, in_features): the newest 2D keypoints of every stream (normalised screen
-        coordinates).  Returns the 3D pose of that frame, (n_streams, J, 3)."""
+        coordinates; rows of held streams are ignored) -> (poses (n, J, 3), index (n,) CPU int64)."""
         eng = self.engine
+        name = type(self).__name__
         frame = torch.as_tensor(frame, dtype=torch.float32, device=self.device).contiguous()
         assert frame.shape == (self.n, self.J, self.F), frame.shape
         if self.model.training:
-            raise eng.GastError('CausalStream: call .eval() on the model (streaming is inference)')
+            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
         h = eng.model_handle(self.model, self.device)
         lib = h.lib
+        m = self.copies * self.n
         y = torch.empty((self.n, self.J, 3), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             st = torch.cuda.current_stream(self.device).cuda_stream
             h.refresh(self.model, st)
-            if self._sig is not None and h.sig != self._sig and not self._all_fresh:
-                raise eng.GastError('CausalStream: the model\'s parameters or buffers changed since the last push '
+            if self._sig is not None and h.sig != self._sig and not self.book.all_restarting():
+                raise eng.GastError('%s: the model\'s parameters or buffers changed since the last push '
                                     '(load_state_dict, an optimiser step or a training forward); the streams\' history '
-                                    'was computed with the old weights -- call reset() before pushing again')
+                                    'was computed with the old weights -- call reset() before pushing again' % name)
             if self._state is None:
-                nb = lib.gast_stream_state_bytes(h.h, self.n)
-                wb = lib.gast_stream_workspace_bytes(h.h, self.n)
+                if lib.gast_stream_latency(h.h) != self.latency:
+                    raise eng.GastError('gast_stream_latency: %s' % L.last_error())
+                nb = lib.gast_stream_state_bytes(h.h, m)
+                wb = lib.gast_stream_workspace_bytes(h.h, m)
                 if nb == 0 or wb == 0:
                     raise eng.GastError('gast_stream_state_bytes: %s' % L.last_error())
                 self._state = torch.empty(int(nb), dtype=torch.uint8, device=self.device)
                 self._ws = torch.empty(int(wb), dtype=torch.uint8, device=self.device)
-            fresh = self.fresh.data_ptr() if self._any_fresh else None
-            rc = lib.gast_stream_push(h.h, C.c_void_p(self._state.data_ptr()), C.c_int64(self.step),
-                                      C.c_void_p(frame.data_ptr()), C.c_void_p(y.data_ptr()), self.n,
-                                      C.c_void_p(fresh), C.c_void_p(self._ws.data_ptr()), self._ws.numel(),
-                                      C.c_void_p(st))
+            fresh, hold, index = self.book.advance()
+            fresh_p, hold_p = self._upload(fresh, hold)
+            x, out = frame, y
+            if self.augment:
+                x = torch.empty((2, self.n, self.J, self.F), dtype=torch.float32, device=self.device)
+                if lib.gast_tta_prepare(C.c_void_p(frame.data_ptr()), C.c_void_p(x.data_ptr()), self.n, self.J, self.F,
+                                        0, 0, len(self.kps_left), self._kl, self._kr, C.c_void_p(st)) != 0:
+                    raise eng.GastError('gast_tta_prepare: %s' % L.last_error())
+                out = torch.empty((2, self.n, self.J, 3), dtype=torch.float32, device=self.device)
+            rc = lib.gast_stream_push_ex(h.h, C.c_void_p(self._state.data_ptr()), C.c_int64(self.step),
+                                         C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), m, C.c_void_p(fresh_p),
+                                         C.c_void_p(hold_p), C.c_void_p(self._ws.data_ptr()), self._ws.numel(),
+                                         C.c_void_p(st))
             if rc != 0:
-                raise eng.GastError('gast_stream_push: %s' % L.last_error())
-            if self._any_fresh:
-                self.fresh.zero_()                       # (stream-ordered after the push that read it)
-                self._any_fresh = False
-                self._all_fresh = False
+                raise eng.GastError('gast_stream_push_ex: %s' % L.last_error())
+            launches = int(lib.gast_last_launch_count(h.h))
+            if self.augment:
+                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(y.data_ptr()), self.n, self.J,
+                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
+                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
+                launches += 2
             self._sig = h.sig
         self.step += 1
-        self.last_launches = int(lib.gast_last_launch_count(h.h))
-        return y
+        self.last_launches = launches
+        return y, torch.from_numpy(index)
+
+
+class CausalStream(PoseStream):
+    """O(1)-per-frame lifting of `n_streams` concurrent streams with a causal model of the drop-in classes
+    (`SpatioTemporalModelOptimized1f(causal=True)` as gen_skes.load_model_realtime builds it, or the dilated
+    `SpatioTemporalModel(causal=True)`: the weights are interchangeable).  `push` returns the pose of the pushed
+    frame of every stream: `PoseStream` without augmentation, poses only."""
+
+    def __init__(self, model_pos, n_streams, device=None):
+        from . import engine
+        if not getattr(model_pos, '_gast_causal', False):
+            raise engine.GastError('CausalStream needs a causal model (gen_skes.py:59 builds it with causal=True)')
+        super(CausalStream, self).__init__(model_pos, n_streams, device=device)
+
+    def push(self, frame):
+        """frame (n_streams, J, in_features): the newest 2D keypoints of every stream (normalised screen
+        coordinates).  Returns the 3D pose of that frame, (n_streams, J, 3)."""
+        return super(CausalStream, self).push(frame)[0]
 
 
 class WindowStream(object):

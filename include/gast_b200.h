@@ -173,11 +173,12 @@ int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, in
  * training step (frozen kernel arguments) draws a fresh mask at every replay. */
 int gast_set_dropout_state(gast_t* h, void* dev_u64);
 
-/* ---- real-time causal streams (SURVEY.md 8f N4; gen_skes.py:43-69, tools/inference.py:19-110) -------------
+/* ---- real-time streams (SURVEY.md 8f N4; gen_skes.py:43-69, tools/inference.py:19-110) -------------------
  * The reference's real-time model is a causal SpatioTemporalModelOptimized1f re-run on the last
  * receptive_field frames for every new frame.  Here a pushed frame costs ONE new position per layer: `state`
  * (caller-owned device memory, gast_stream_state_bytes, contents irrelevant before the first push) holds per
- * temporal stage a ring of that stage's past inputs for n_streams concurrent streams.
+ * temporal stage a ring of that stage's past inputs for n_streams concurrent streams.  State and workspace
+ * sizes are the same for causal and non-causal handles of one architecture.
  * gast_stream_push: x (n_streams, J, in_features) = the newest frame of every stream -> y (n_streams, J, 3) =
  *   its 3D pose, identical to the whole-sequence causal forward on the sequence so far, left-padded by
  *   replicating the stream's first frame (UnchunkedGenerator(pad, causal_shift=pad), common/generators.py:210-221).
@@ -192,6 +193,27 @@ size_t gast_stream_state_bytes(gast_t* h, int32_t n_streams);
 size_t gast_stream_workspace_bytes(gast_t* h, int32_t n_streams);
 int gast_stream_push(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
                      const int32_t* fresh, void* workspace, size_t workspace_bytes, void* stream);
+/* gast_stream_push_ex: gast_stream_push for causal AND non-causal MODEL handles (not dense), with a hold mask.
+ *   y[s] is the pose of the frame pushed gast_stream_latency(h) pushes earlier on stream s: 0 for a causal
+ *   model, pad = (receptive_field - 1) / 2 for a non-causal one.  A sequence's poses equal the reference's
+ *   UnchunkedGenerator([seq], pad, causal_shift = causal ? pad : 0) + model forward when the caller
+ *     - marks the sequence's first frame fresh (left padding: copies of the first frame), and
+ *     - after its last frame makes `latency` more pushes with hold[s] != 0 (right padding: copies of the last
+ *       frame).  Those pushes return the sequence's last `latency` poses.
+ *   The first `latency` outputs after a fresh frame belong to frames before the sequence and are meaningless.
+ *   hold (n_streams) int32 on the device, or null: non-zero = stream s re-appends its own newest frame and
+ *   ignores x[s]; fresh wins over hold.  gast_stream_push(...) is gast_stream_push_ex(..., hold = NULL, ...)
+ *   after refusing non-causal handles.  Same step / fresh / weight-change rules as gast_stream_push.
+ *   Test-time augmentation (tools/inference.py:19-110: augment=True, un-flip and average) composes from the TTA
+ *   entries with T = n_streams: gast_tta_prepare(x, x2, n, J, F, pad = 0, shift = 0, kps lists) writes
+ *   x2 (2, n, J, F) = [original | mirrored]; push x2 as 2n streams into a state sized for 2n streams, with the
+ *   fresh and hold masks repeated for both halves; gast_tta_merge(y2, y, n, J, joints lists) averages
+ *   y2 (2n, J, 3) into y (n, J, 3).
+ * gast_stream_latency: 0 (causal), (receptive_field - 1) / 2 (non-causal), -1 for a handle that cannot stream. */
+int32_t gast_stream_latency(const gast_t* h);
+int gast_stream_push_ex(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
+                        const int32_t* fresh, const int32_t* hold, void* workspace, size_t workspace_bytes,
+                        void* stream);
 
 /* ---- either side of the forward, on the device (SURVEY.md 8f N1-N3) --------------------------------
  * All pointers are device pointers unless marked (host).  Work is enqueued on `stream`.
