@@ -39,6 +39,10 @@ __host__ __device__ inline size_t ffma_smem_bytes(int epi, int J, int fpt, int h
   return f * sizeof(float) + 3 * 128 * sizeof(long long);
 }
 
+// The epilogues run on 256 threads: the whole block of the FFMA core, the two consumer warpgroups of the
+// tensor-core core (whose producer warpgroup has left by then), so they synchronise on named barrier 1 over 256.
+__device__ __forceinline__ void epi_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
 // Fused epilogues shared by both GEMM cores.  `acc` holds the 128 x 128 tile product in the FFMA thread layout:
 // thread tid (of 256) owns rows {ty*4+i, 64+ty*4+i} (i<4) and cols {tx*4+j, 64+tx*4+j} (j<4), ty = tid/16,
 // tx = tid%16.  `smem` is free scratch of at least ffma_smem_bytes() - 3*128*8 bytes; callers synchronise before.
@@ -82,14 +86,14 @@ __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)
   } else if (EPI == EPI_SEMCH) {
     // tile = 64 channels of one mask: cols [0,64) = X.W0 (self), cols [64,128) = X.W1 (neighbours)
     float* Hs = smem;  // [128][64]
-    // main loop finished with a __syncthreads(): smem is free
+    // the caller synchronised after its main loop: smem is free
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       int r = (i < 4) ? (ty * 4 + i) : (64 + ty * 4 + i - 4);
       *reinterpret_cast<float4*>(Hs + r * 64 + tx * 4) =
           make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
     }
-    __syncthreads();
+    epi_sync();
     const int mask = blockIdx.y / p.tiles_per_mask;
     const int c0 = (blockIdx.y - mask * p.tiles_per_mask) * 64 + tx * 4;
     if (c0 < p.C) {
@@ -144,7 +148,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)
       int r = i / H2, q = i - r * H2;
       abs_[r * H2 + q] = p.ab[((long long)f0 * J + r) * H2 + q];
     }
-    __syncthreads();
+    epi_sync();
     // attention rows: softmax_j(LeakyReLU_0.2(a_i + b_j)) + C_k[i,j]   (global_attention.py:72-76)
     for (int i = tid; i < nf * hpt * J; i += FF_THREADS) {
       int ji = i % J;
@@ -166,7 +170,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)
       const float* ck = p.ck + ((long long)h * J + ji) * J;
       for (int j = 0; j < J; ++j) row[j] = row[j] * inv + ck[j];
     }
-    __syncthreads();
+    epi_sync();
     const bool vec = (p.Cg % 4) == 0;
     for (int i = tid; i < vrows * 32; i += FF_THREADS) {
       int r = i >> 5, nl = (i & 31) * 4;

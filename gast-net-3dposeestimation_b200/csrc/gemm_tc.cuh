@@ -11,17 +11,27 @@
 // fresh register tile (6 wgmmas) and added into the fp32 tile sum with round-to-nearest (32 K per partial sum
 // roughly doubled the error and pushed single training gradients past their bar).
 //
-// Per CTA (256 threads = 2 warpgroups, one CTA per SM): a 3-stage shared-memory ring of 32-wide K stages.
-//   B (weights): the hi and lo copies are stored [K/4][N][4] (tc_prepare_weights), so one 3D TMA box per operand
+// Per CTA (384 threads = 3 warpgroups, one CTA per SM), warp-specialised around a 3-slot shared-memory ring of
+// 32-wide K stages (slot = B_hi | B_lo | A):
+//   producer (warpgroup 0, 40 registers after setmaxnreg): waits for a slot's `empty` mbarrier, then fills it.
+//     B (weights): the hi and lo copies are stored [K/4][N][4] (tc_prepare_weights), so one 3D TMA box per operand
 //                lands in the no-swizzle K-major core-matrix layout wgmma reads from shared memory (8 rows x 16 B
-//                core matrices, 128 B apart along N, 2048 B apart along K); completion on the stage's mbarrier.
-//   A (activations): rows are gathered per frame (dilated / strided taps, residual slices, concatenations), so they
-//                arrive by cp.async (16 B per row and k-quad, zero-filled outside the tile); each warp loads its
-//                m64 fragment rows from shared memory into registers and splits them into tf32 hi / lo there.
-//   MMA: warpgroup w owns rows 64w .. 64w+63 and all 128 columns: wgmma.m64n128k8 tf32, A from registers,
-//                B from the shared-memory descriptor.
-// Tiles (fpt whole frames per 128-row tile) and the fused epilogues (gemm_epilogue) are the FFMA core's, so both
-// cores are interchangeable per launch.
+//                core matrices, 128 B apart along N, 2048 B apart along K); one elected thread issues both boxes.
+//     A (activations): rows are gathered per frame (dilated / strided taps, residual slices, concatenations), so
+//                they arrive by cp.async (16 B per row and k-quad, zero-filled outside the tile) from all 128
+//                producer threads.  A stage never straddles a tap (Kc % 32 == 0), so segment, tap and column are
+//                advanced once per stage.
+//     The slot's `full` mbarrier completes when the TMA bytes (expect_tx) and every producer thread's cp.asyncs
+//     (cp.async.mbarrier.arrive.noinc) have landed: 1 + 128 arrivals.
+//   consumers (warpgroups 1 and 2, 232 registers): warpgroup 1 + w owns rows 64w .. 64w+63 and all 128 columns:
+//     wgmma.m64n128k8 tf32, A from registers (loaded from the slot and split into tf32 hi / lo there), B from the
+//     shared-memory descriptor.  A stage's two 16-K partials (6 wgmmas each) go into two register tiles back to back;
+//     the first is added into the tile sum while the second runs (wgmma.wait_group 1), then the second is retired
+//     and added, and the slot is released (its `empty` mbarrier, one arrival per consumer warp, 8 in all).  No
+//     partial stays in flight across the loop's back edge: ptxas then serialises every wgmma of the kernel (C7514).
+//     The two consumers do not synchronise with each other inside the K loop, so one's MMAs fill the other's drain.
+// Tiles (fpt whole frames per 128-row tile) and the fused epilogues (gemm_epilogue, run by the 256 consumer threads)
+// are the FFMA core's, so both cores are interchangeable per launch.
 #pragma once
 #include <cuda.h>
 #include <vector>
@@ -40,9 +50,10 @@ struct TcWeights {
 
 constexpr int TC_BM = 128, TC_BN = 128;
 constexpr int TC_KS = 32;                            // K per ring stage; segment widths must be multiples of it
-constexpr int TC_STAGES = 3;
+constexpr int TC_STAGES = 3;                         // a fourth slot measured slower (DESIGN.md §4.1)
 constexpr int TC_KP = 16;                            // K per partial sum (6 wgmmas), added into the tile sum with RN
-constexpr int TC_THREADS = 256;
+constexpr int TC_THREADS = 384;                      // warpgroup 0 produces, warpgroups 1 and 2 consume
+constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;   // 128 * 40 + 256 * 232 <= 64K registers of the SM
 constexpr int TC_ALD = TC_KS + 4;                    // A stage row stride (floats): conflict-free fragment loads
 constexpr int TC_B_BYTES = TC_BN * TC_KS * 4;        // one of B_hi / B_lo in a stage
 constexpr int TC_A_BYTES = TC_BM * TC_ALD * 4;
@@ -54,7 +65,7 @@ constexpr int TC_SMEM_MAX = 200 * 1024;
 static_assert(TC_SLOT % 1024 == 0, "ring slots stay 1024-byte aligned");
 
 __host__ __device__ inline size_t tc_smem_bytes(int epi, int J, int fpt, int hpt) {
-  size_t m = (size_t)TC_RING + 8 * TC_STAGES;
+  size_t m = (size_t)TC_RING + 16 * TC_STAGES;       // + a full and an empty mbarrier per slot
   const size_t stg = (size_t)TC_BM * TC_STG_LD * 4;
   const size_t e = ffma_smem_bytes(epi, J, fpt, hpt) - TC_ROWBASE_BYTES;
   if (stg > m) m = stg;
@@ -76,6 +87,9 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   asm volatile(
       "{\n\t"
@@ -96,9 +110,11 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+// arrive on `bar` once every cp.async this thread has issued so far has landed (counted in the barrier's init count)
+__device__ __forceinline__ void cp_async_arrive(uint32_t bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // shared-memory matrix descriptor of a no-swizzle K-major operand: core matrices 128 B apart along N (SBO),
 // 2048 B apart along K (LBO)
@@ -107,7 +123,18 @@ __device__ __forceinline__ uint64_t tc_bdesc(uint32_t addr) {
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// pins a register tile at this point of the program, so that the compiler does not move its reads or writes across
+// the wgmma fence / commit / wait around it
+__device__ __forceinline__ void tile_fence(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // d (+)= a . B, m64n128k8, tf32 operands (A from registers, B from shared memory), fp32 accumulate;
 // scale_d == 0 overwrites d
@@ -119,6 +146,45 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], const uint32_t (&a)[4
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(scale_d), "l"(bdesc));
 }
 
+// One 16-K partial of a consumer: d = sum over the k8 steps s0, s0 + 1 of the slot at sb of
+// A_lo.B_hi + A_hi.B_lo + A_hi.B_hi (small products first), issued as one wgmma group
+__device__ __forceinline__ void tc_partial(float (&d)[64], const uint32_t (&ah)[2][4], const uint32_t (&al)[2][4],
+                                           uint32_t sb, int s0) {
+  tile_fence(d);
+  wgmma_fence();
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {   // k8 step s = core matrices 2s, 2s+1
+    const int s = s0 + i;
+    const uint64_t dh = tc_bdesc(sb + s * 4096), dl = tc_bdesc(sb + TC_B_BYTES + s * 4096);
+    wgmma_tf32(d, al[i], dh, i);
+    wgmma_tf32(d, ah[i], dl, 1);
+    wgmma_tf32(d, ah[i], dh, 1);
+  }
+  wgmma_commit();
+}
+
+// A fragment rows r0, r0 + 8 of the k8 steps s0, s0 + 1 of a slot's A (row stride TC_ALD), split into tf32 hi / lo
+__device__ __forceinline__ void tc_load_a(const float* A, int r0, int t, int s0, uint32_t (&ah)[2][4],
+                                          uint32_t (&al)[2][4]) {
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int k = 8 * (s0 + i) + t;
+    const float x[4] = {A[r0 * TC_ALD + k], A[(r0 + 8) * TC_ALD + k], A[r0 * TC_ALD + k + 4],
+                        A[(r0 + 8) * TC_ALD + k + 4]};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      ah[i][q] = tf32_bits(x[q]);
+      al[i][q] = tf32_bits(x[q] - __uint_as_float(ah[i][q]));
+    }
+  }
+}
+
+__device__ __forceinline__ void tc_add(float (&acc)[64], float (&part)[64]) {
+  tile_fence(part);
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] += part[i];
+}
+
 template <int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensorMap mhi,
@@ -128,7 +194,8 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t rb = (raw + TC_ROWBASE_BYTES + 1023) & ~1023u;        // ring base (shared address)
   unsigned char* ring = smem_raw + (rb - raw);
-  const uint32_t bar0 = rb + TC_RING;                                   // one mbarrier per ring slot
+  const uint32_t full0 = rb + TC_RING;                                  // per ring slot: stage landed
+  const uint32_t empty0 = full0 + 8 * TC_STAGES;                        // per ring slot: both consumers done with it
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int J = p.J;
@@ -138,7 +205,10 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   const int n0 = blockIdx.y * TC_BN;
 
   if (tid == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) mbar_init(bar0 + 8 * s, 1);
+    for (int s = 0; s < TC_STAGES; ++s) {
+      mbar_init(full0 + 8 * s, 1 + 128);
+      mbar_init(empty0 + 8 * s, 8);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
@@ -157,85 +227,66 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   int nstages = 0;
   for (int s = 0; s < p.nseg; ++s) nstages += p.seg[s].K / TC_KS;
 
-  // producer: stage c into ring slot c % TC_STAGES (B by TMA, A by cp.async); one cp.async group per stage
-  int pseg = 0, pk0 = 0, pkcol = 0;
-  auto issue = [&](int c) {
-    if (c < nstages) {
+  if (warp < 4) {
+    // producer: stage c into ring slot c % TC_STAGES once both consumers have released the slot's previous stage
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    const int q = tid & 7, rq = tid >> 3;                               // k-quad q of rows rq + 16 i
+    int seg = 0, k0 = 0, kcol = 0, tap = 0, kin = 0;                    // stage start: segment, K in it, W column, tap
+    for (int c = 0; c < nstages; ++c) {
       const int slot = c % TC_STAGES;
-      const uint32_t sb = rb + slot * TC_SLOT;
+      if (c >= TC_STAGES) mbar_wait(empty0 + 8 * slot, (c / TC_STAGES - 1) & 1);
+      const uint32_t sb = rb + slot * TC_SLOT, full = full0 + 8 * slot;
       if (tid == 0) {
-        const uint32_t bar = bar0 + 8 * slot;
-        mbar_arrive_expect_tx(bar, 2 * TC_B_BYTES);
-        const int kq = (pkcol + pk0) >> 2;
-        tma_load_3d(sb, &mhi, bar, 0, n0, kq);
-        tma_load_3d(sb + TC_B_BYTES, &mlo, bar, 0, n0, kq);
+        mbar_arrive_expect_tx(full, 2 * TC_B_BYTES);
+        const int kq = (kcol + k0) >> 2;
+        tma_load_3d(sb, &mhi, full, 0, n0, kq);
+        tma_load_3d(sb + TC_B_BYTES, &mlo, full, 0, n0, kq);
       }
-      const ASeg& sg = p.seg[pseg];
+      const ASeg& sg = p.seg[seg];
+      const float* src = sg.base + tap * sg.tap_stride + kin + q * 4;
 #pragma unroll
-      for (int i = 0; i < (TC_BM * TC_KS / 4) / TC_THREADS; ++i) {
-        const int id = tid + i * TC_THREADS, r = id >> 3, q = id & 7;
-        const int k = pk0 + q * 4;
-        const long long off = rowbase[pseg * 128 + r];
-        const float* src = sg.base;
-        int bytes = 0;
-        if (off >= 0) {
-          const int tap = k / sg.Kc;
-          src = sg.base + off + tap * sg.tap_stride + (k - tap * sg.Kc);
-          bytes = 16;
-        }
-        cp_async16(sb + 2 * TC_B_BYTES + (r * TC_ALD + q * 4) * 4, src, bytes);
+      for (int i = 0; i < TC_BM / 16; ++i) {
+        const int r = rq + 16 * i;
+        const long long off = rowbase[seg * 128 + r];
+        cp_async16(sb + 2 * TC_B_BYTES + (r * TC_ALD + q * 4) * 4, off >= 0 ? src + off : sg.base, off >= 0 ? 16 : 0);
       }
-      pk0 += TC_KS;
-      if (pk0 >= sg.K) { pkcol += sg.K; pk0 = 0; ++pseg; }
+      cp_async_arrive(full);
+      k0 += TC_KS;
+      kin += TC_KS;
+      if (kin == sg.Kc) { kin = 0; ++tap; }
+      if (k0 == sg.K) { kcol += sg.K; k0 = 0; tap = 0; ++seg; }
     }
-    cp_async_commit();
-  };
+    cp_async_wait_all();
+    return;
+  }
 
-  const int wg = warp >> 2, wq = warp & 3;
+  // consumers
+  setmaxnreg_inc<TC_CONSUMER_REGS>();
+  const int ct = tid - 128;                                             // 0 .. 255: the epilogue's thread index
+  const int wg = ct >> 7, wq = (ct >> 5) & 3;
   const int g = lane >> 2, t = lane & 3;
   const int r0 = wg * 64 + wq * 16 + g;                                 // fragment rows r0 and r0 + 8
-  float acc[64], part[64];
+  float acc[64], part0[64], part1[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 
-  for (int c = 0; c < TC_STAGES - 1; ++c) issue(c);
   for (int c = 0; c < nstages; ++c) {
-    issue(c + TC_STAGES - 1);                   // its slot was released by the barrier that ended stage c - 1
-    cp_async_wait<TC_STAGES - 1>();             // this thread's A rows of stage c have landed
-    __syncthreads();                            // ... and every other thread's
     const int slot = c % TC_STAGES;
-    mbar_wait(bar0 + 8 * slot, (c / TC_STAGES) & 1);
+    mbar_wait(full0 + 8 * slot, (c / TC_STAGES) & 1);
     const uint32_t sb = rb + slot * TC_SLOT;
     const float* A = reinterpret_cast<const float*>(ring + slot * TC_SLOT + 2 * TC_B_BYTES);
-    uint32_t ah[TC_KS / 8][4], al[TC_KS / 8][4];
-#pragma unroll
-    for (int s = 0; s < TC_KS / 8; ++s) {
-      const float x[4] = {A[r0 * TC_ALD + 8 * s + t], A[(r0 + 8) * TC_ALD + 8 * s + t],
-                          A[r0 * TC_ALD + 8 * s + t + 4], A[(r0 + 8) * TC_ALD + 8 * s + t + 4]};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        ah[s][q] = tf32_bits(x[q]);
-        al[s][q] = tf32_bits(x[q] - __uint_as_float(ah[s][q]));
-      }
-    }
-#pragma unroll
-    for (int h = 0; h < TC_KS / TC_KP; ++h) {
-      wgmma_fence();
-#pragma unroll
-      for (int s = h * (TC_KP / 8); s < (h + 1) * (TC_KP / 8); ++s) {   // small products first; k8 step s = core
-        const uint64_t dh = tc_bdesc(sb + s * 4096), dl = tc_bdesc(sb + TC_B_BYTES + s * 4096);   // matrices 2s, 2s+1
-        wgmma_tf32(part, al[s], dh, s != h * (TC_KP / 8));
-        wgmma_tf32(part, ah[s], dl, 1);
-        wgmma_tf32(part, ah[s], dh, 1);
-      }
-      wgmma_commit();
-      wgmma_wait0();
-#pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] += part[i];
-    }
-    __syncthreads();
+    uint32_t ah[2][4], al[2][4];
+    tc_load_a(A, r0, t, 0, ah, al);
+    tc_partial(part0, ah, al, sb, 0);
+    tc_load_a(A, r0, t, 2, ah, al);
+    tc_partial(part1, ah, al, sb, 2);
+    wgmma_wait<1>();                            // the first partial has retired ...
+    tc_add(acc, part0);                         // ... and is summed while the second runs
+    wgmma_wait<0>();
+    tc_add(acc, part1);
+    if (lane == 0) mbar_arrive(empty0 + 8 * slot);
   }
-  cp_async_wait<0>();
+  epi_sync();                                   // both consumers are done with the ring
 
   // hand the tile over in the FFMA thread layout the shared epilogues expect
   float* S = reinterpret_cast<float*>(ring);   // [128][TC_STG_LD]
@@ -245,8 +296,8 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
     *reinterpret_cast<float2*>(S + r0 * TC_STG_LD + col) = make_float2(acc[4 * i], acc[4 * i + 1]);
     *reinterpret_cast<float2*>(S + (r0 + 8) * TC_STG_LD + col) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
   }
-  __syncthreads();
-  const int ty = tid >> 4, tx = tid & 15;
+  epi_sync();
+  const int ty = ct >> 4, tx = ct & 15;
   float out[8][8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -256,8 +307,8 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
     out[i][0] = u.x; out[i][1] = u.y; out[i][2] = u.z; out[i][3] = u.w;
     out[i][4] = v.x; out[i][5] = v.y; out[i][6] = v.z; out[i][7] = v.w;
   }
-  __syncthreads();
-  gemm_epilogue<EPI>(p, out, reinterpret_cast<float*>(ring), tid, f0, nf, vrows, n0);
+  epi_sync();
+  gemm_epilogue<EPI>(p, out, reinterpret_cast<float*>(ring), ct, f0, nf, vrows, n0);
 }
 
 // W [N][K] -> hi / lo in the TMA-friendly layout [K/4][N][4]
