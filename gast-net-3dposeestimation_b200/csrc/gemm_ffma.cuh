@@ -46,9 +46,10 @@ __device__ __forceinline__ void epi_sync() { asm volatile("bar.sync 1, 256;" :::
 // Fused epilogues shared by both GEMM cores.  `acc` holds the 128 x 128 tile product in the FFMA thread layout:
 // thread tid (of 256) owns rows {ty*4+i, 64+ty*4+i} (i<4) and cols {tx*4+j, 64+tx*4+j} (j<4), ty = tid/16,
 // tx = tid%16.  `smem` is free scratch of at least ffma_smem_bytes() - 3*128*8 bytes; callers synchronise before.
+// The tile is frames f0 .. f0 + nf - 1 (vrows rows) x columns n0 .. n0 + 127, column tile `ctile` (n0 = 128 ctile).
 template <int EPI>
 __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)[8][8], float* smem, int tid,
-                                              int f0, int nf, int vrows, int n0) {
+                                              int f0, int nf, int vrows, int n0, int ctile) {
   const int J = p.J;
   const int ty = tid >> 4, tx = tid & 15;
   if (EPI == EPI_PLAIN) {
@@ -94,8 +95,8 @@ __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)
           make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
     }
     epi_sync();
-    const int mask = blockIdx.y / p.tiles_per_mask;
-    const int c0 = (blockIdx.y - mask * p.tiles_per_mask) * 64 + tx * 4;
+    const int mask = ctile / p.tiles_per_mask;
+    const int c0 = (ctile - mask * p.tiles_per_mask) * 64 + tx * 4;
     if (c0 < p.C) {
       const NbrTable& nb = p.nbr[mask];
       const float* coef = p.coef[mask];
@@ -322,7 +323,7 @@ gemm_ffma_kernel(const __grid_constant__ GemmP p) {
     __syncthreads();
   }
 
-  gemm_epilogue<EPI>(p, acc, smem, tid, f0, nf, vrows, n0);
+  gemm_epilogue<EPI>(p, acc, smem, tid, f0, nf, vrows, n0, blockIdx.y);
 }
 
 }  // namespace gast

@@ -32,6 +32,10 @@
 //     The two consumers do not synchronise with each other inside the K loop, so one's MMAs fill the other's drain.
 // Tiles (fpt whole frames per 128-row tile) and the fused epilogues (gemm_epilogue, run by the 256 consumer threads)
 // are the FFMA core's, so both cores are interchangeable per launch.
+//
+// One tile per CTA, on a 1D grid in which the column tile is the fast index (tc_launch): the CTAs dispatched together
+// cover a row tile's column tiles side by side, so its A rows come from HBM once and its other column tiles find them
+// in L2.  (Every layer's A is larger than the L2; with the row tile fast, A was read from HBM once per column tile.)
 #pragma once
 #include <cuda.h>
 #include <vector>
@@ -185,6 +189,16 @@ __device__ __forceinline__ void tc_add(float (&acc)[64], float (&part)[64]) {
   for (int i = 0; i < 64; ++i) acc[i] += part[i];
 }
 
+// This CTA's row tile and column tile.  %ctaid is read with a volatile move, so that the consumers can recompute the
+// tile after their K loop instead of keeping it in registers through it (that spilled in the SemCH instantiation).
+__device__ __forceinline__ void tc_tile(const GemmP& p, int& rt, int& ctile) {
+  uint32_t b;
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(b));
+  const int col_tiles = (p.N + TC_BN - 1) / TC_BN;
+  rt = (int)b / col_tiles;
+  ctile = (int)b - rt * col_tiles;
+}
+
 template <int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensorMap mhi,
@@ -199,10 +213,12 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int J = p.J;
-  const int f0 = blockIdx.x * p.fpt;
+  int rt, ctile;
+  tc_tile(p, rt, ctile);
+  const int f0 = rt * p.fpt;
   const int nf = min(p.fpt, p.F - f0);
   const int vrows = nf * J;
-  const int n0 = blockIdx.y * TC_BN;
+  const int n0 = ctile * TC_BN;
 
   if (tid == 0) {
     for (int s = 0; s < TC_STAGES; ++s) {
@@ -287,6 +303,8 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
     if (lane == 0) mbar_arrive(empty0 + 8 * slot);
   }
   epi_sync();                                   // both consumers are done with the ring
+  tc_tile(p, rt, ctile);
+  const int fe = rt * p.fpt, nfe = min(p.fpt, p.F - fe);
 
   // hand the tile over in the FFMA thread layout the shared epilogues expect
   float* S = reinterpret_cast<float*>(ring);   // [128][TC_STG_LD]
@@ -308,7 +326,7 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
     out[i][4] = v.x; out[i][5] = v.y; out[i][6] = v.z; out[i][7] = v.w;
   }
   epi_sync();
-  gemm_epilogue<EPI>(p, out, reinterpret_cast<float*>(ring), ct, f0, nf, vrows, n0);
+  gemm_epilogue<EPI>(p, out, reinterpret_cast<float*>(ring), ct, fe, nfe, nfe * J, ctile * TC_BN, ctile);
 }
 
 // W [N][K] -> hi / lo in the TMA-friendly layout [K/4][N][4]
@@ -385,8 +403,9 @@ inline bool tc_supported(const GemmP& p, int epi, const TcWeights& t) {
   return true;
 }
 
+// One CTA per tile, tile = row tile * column tiles + column tile (the column tile fastest, see gemm_tc_kernel).
 inline int tc_launch(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t) {
-  const dim3 grid((unsigned)((p.F + p.fpt - 1) / p.fpt), (unsigned)((p.N + TC_BN - 1) / TC_BN));
+  const dim3 grid((unsigned)(((p.F + p.fpt - 1) / p.fpt) * ((p.N + TC_BN - 1) / TC_BN)));
   const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
   const size_t smem = tc_smem_bytes(epi, p.J, p.fpt, hpt);
   static bool attr_set[64][3];              // the shared-memory opt-in is per device
