@@ -72,6 +72,87 @@ __global__ void stream_fill_fresh_kernel(float* __restrict__ ring, int R, int sr
   }
 }
 
+// ---- chunks of K frames per stream (gast_stream_push_chunk, below) ----
+constexpr int CHUNK_XIN_THREADS = 256;
+
+// xin (n, k0-1+K, J, F) = the last k0-1 frames of xhist followed by the K new frames x (n, K, J, F); then xhist = the
+// last k0 frames of xin.  One block per stream.  hold (n, K) or null: a held frame (not fresh frame 0) repeats the
+// stream's newest frame, which may be an earlier held frame of the chunk, so frame k takes x[b, src[k]] with src[k] the
+// latest frame <= k that is not held (a block-wide max scan), or the newest frame of xhist when there is none.  A fresh
+// stream's history is copies of its frame 0.  x rows of held frames are never read.
+__global__ void __launch_bounds__(CHUNK_XIN_THREADS)
+stream_chunk_xin_kernel(float* __restrict__ xhist, const float* __restrict__ x, float* __restrict__ xin,
+                        const int32_t* __restrict__ fresh, const int32_t* __restrict__ hold, int k0, int K, int JF) {
+  __shared__ int src[CHUNK_XIN_THREADS];
+  __shared__ int wmax[CHUNK_XIN_THREADS / 32];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const bool is_fresh = fresh && fresh[b];
+  float* hrow = xhist + (long long)b * k0 * JF;
+  float* irow = xin + (long long)b * (k0 - 1 + K) * JF;
+  const float* xrow = x + (long long)b * K * JF;
+  const int32_t* hb = hold ? hold + (long long)b * K : nullptr;
+  int carry = -1;                                          // latest frame not held before this tile
+  for (int t0 = 0; t0 < K; t0 += CHUNK_XIN_THREADS) {
+    const int k = t0 + tid;
+    const bool held = k >= K || (hb && hb[k] && !(k == 0 && is_fresh));
+    int v = held ? -1 : k;
+    for (int o = 1; o < 32; o <<= 1) {                    // inclusive max scan: warp, then across warps
+      const int u = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v = max(v, u);
+    }
+    if (lane == 31) wmax[warp] = v;
+    __syncthreads();
+    for (int w = 0; w < warp; ++w) v = max(v, wmax[w]);
+    src[tid] = max(v, carry);
+    __syncthreads();
+    carry = src[CHUNK_XIN_THREADS - 1];
+    const int nk = min(CHUNK_XIN_THREADS, K - t0);
+    for (int e = tid; e < nk * JF; e += CHUNK_XIN_THREADS) {
+      const int kk = e / JF, c = e - kk * JF, s = src[kk];
+      irow[(long long)(k0 - 1 + t0 + kk) * JF + c] = s >= 0 ? xrow[(long long)s * JF + c] : hrow[(long long)(k0 - 1) * JF + c];
+    }
+    __syncthreads();                                       // src and wmax are rewritten by the next tile
+  }
+  for (int e = tid; e < (k0 - 1) * JF; e += CHUNK_XIN_THREADS)
+    irow[e] = is_fresh ? xrow[e % JF] : hrow[e + JF];
+  __syncthreads();                                         // every read of hrow is done; irow is visible to the block
+  for (int e = tid; e < k0 * JF; e += CHUNK_XIN_THREADS) hrow[e] = irow[(long long)(K - 1) * JF + e];
+}
+
+// G (n, H+K, rowlen) = stage input at times step-H .. step+K-1: the head (positions p < H) from the ring slots
+// (step - H + p) mod R, the tail (p >= H) from the previous block's K outputs tail (n, K, rowlen).  A fresh stream's head
+// is copies of its tail position 0 (its history is constant, as stream_fill_fresh_kernel makes it).  hs = step mod R.
+__global__ void stream_chunk_gather_kernel(float4* __restrict__ G, const float4* __restrict__ ring,
+                                           const float4* __restrict__ tail, const int32_t* __restrict__ fresh, int n,
+                                           int R, int hs, int H, int K, long long row4) {
+  const long long total = (long long)n * (H + K) * row4;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long q = i % row4, f = i / row4;
+    const int b = (int)(f / (H + K)), p = (int)(f - (long long)b * (H + K));
+    float4 v;
+    if (p >= H) v = tail[((long long)b * K + (p - H)) * row4 + q];
+    else if (fresh && fresh[b]) v = tail[(long long)b * K * row4 + q];
+    else v = ring[((long long)((hs - H + p + R) % R) * n + b) * row4 + q];
+    G[i] = v;
+  }
+}
+
+// Ring write-back after a chunk: slot p gets the stage input at the latest time t <= step+K-1 with t = p (mod R), from
+// the tail of G when t falls in the chunk, copies of tail position 0 for a fresh stream, else the slot keeps its value.
+// ek = (step + K - 1) mod R.  Launched after stream_chunk_gather_kernel, which reads slots this kernel overwrites.
+__global__ void stream_chunk_ring_kernel(float4* __restrict__ ring, const float4* __restrict__ G,
+                                         const int32_t* __restrict__ fresh, int n, int R, int ek, int H, int K,
+                                         long long row4) {
+  const long long total = (long long)R * n * row4;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long q = i % row4, f = i / row4;
+    const int p = (int)(f / n), b = (int)(f - (long long)p * n);
+    const int k = K - 1 - (ek - p + R) % R;               // chunk position of time t
+    if (k < 0 && !(fresh && fresh[b])) continue;
+    ring[i] = G[((long long)b * (H + K) + H + max(k, 0)) * row4 + q];
+  }
+}
+
 // dst[n][k*Cw + c] = src[n][j*Cw + c],  j = (k - r - 1) mod taps: slot order -> time order of the taps
 __global__ void rotate_taps_kernel(float* __restrict__ dst, const float* __restrict__ src, int N, int Cw, int taps, int r) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -247,4 +328,99 @@ extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const floa
     return fail("gast_stream_push needs a causal model (gen_skes.py:59: causal=True): a non-causal network has no "
                 "output for the newest frame (gast_stream_push_ex returns it `latency` pushes later)");
   return gast_stream_push_ex(h, state, step, x, y, n_streams, fresh, nullptr, workspace, workspace_bytes, stream);
+}
+
+// ---- K frames per stream in one call ---------------------------------------------------------------------------
+// gast_stream_push_chunk is gast_stream_push_ex at steps step .. step+K-1 with x[:, k], fresh at k = 0 only and
+// hold[:, k], run as ONE forward over n*K positions on the dilated schedule's kernels.  Temporal stage i (width w,
+// dilation d, ring R = w d) needs its last H = (w-1) d inputs before the chunk plus the K new ones: they are gathered
+// into G (n, H+K, J, Cw) (head from the ring, tail from the previous block), the stage runs on G with the time-ordered
+// weights Wt and the row map of the whole-sequence forward (taps d*J*Cw floats apart, residual at the newest or the
+// centre tap), and every ring slot is then given the input of the latest time it stands for, so that the next push
+// (single or chunk) finds the history it expects.  The blocks are pointwise in time and run on n*K frames.
+struct ChunkBufs { float *xin, *G; StreamBufs sb; };
+
+static int chunk_bufs(const gast_handle* h, const StreamPlan& sp, int K, Arena& a, ChunkBufs* cb) {
+  const gast_cfg& c = h->cfg;
+  const int n = sp.n, J = c.num_joints, k0 = c.filter_widths[0];
+  if (K < 1) return fail("gast_stream_push_chunk: K must be at least 1 (got %d)", K);
+  if ((long long)n * K * J >= 0x7fffffffLL) return fail("expand: more than 2^31 positions in one call");
+  size_t g = 0;
+  for (int i = 1; i < c.num_stages; ++i)
+    g = std::max(g, (size_t)n * ((c.filter_widths[i] - 1) * sp.dil[i - 1] + K) * J * (c.channels << i));
+  cb->xin = a.take((size_t)n * (k0 - 1 + K) * J * c.in_features);
+  cb->G = a.take(g);
+  stream_bufs(h, n * K, a, &cb->sb);
+  return 0;
+}
+
+extern "C" size_t gast_stream_chunk_workspace_bytes(gast_t* h, int32_t n_streams, int32_t K) {
+  if (!h) return 0;
+  StreamPlan sp;
+  if (stream_plan(h, n_streams, &sp)) return 0;
+  Arena a{nullptr, 0, 0, true};
+  ChunkBufs cb;
+  if (chunk_bufs(h, sp, K, a, &cb)) return 0;
+  return a.off + 256;
+}
+
+extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
+                                      int32_t K, const int32_t* fresh, const int32_t* hold, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  if (!h) return fail("gast_stream_push_chunk: null handle");
+  if (!h->prepared) return fail("gast_stream_push_chunk: gast_prepare() has not run since the last gast_bind()");
+  if (step < 0 || !state || !x || !y) return fail("gast_stream_push_chunk: bad arguments");
+  StreamPlan sp;
+  if (stream_plan(h, n_streams, &sp)) return 1;
+  {
+    Arena dry{nullptr, 0, 0, true};
+    ChunkBufs cb;
+    if (chunk_bufs(h, sp, K, dry, &cb)) return 1;
+    const size_t need = dry.off + 256;
+    if (!workspace || workspace_bytes < need)
+      return fail("gast_stream_push_chunk: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CUDA_OK(cudaSetDevice(h->cfg.device));
+  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
+  const gast_cfg& c = h->cfg;
+  const int n = n_streams, J = c.num_joints, L = c.num_stages, k0 = c.filter_widths[0], Fin = c.in_features;
+  const long long F = (long long)n * K;                  // frames of the chunk, in (stream, frame) order
+  float* sbase = reinterpret_cast<float*>(align256(state));
+  Arena a = workspace_arena(workspace, workspace_bytes);
+  ChunkBufs cb;
+  if (chunk_bufs(h, sp, K, a, &cb)) return 1;
+  const StreamBufs& sb = cb.sb;
+  stream_chunk_xin_kernel<<<n, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K, J * Fin);
+  h->launches++;
+  if (launch_expand(h, st, cb.xin, sb.E, F * J, k0 - 1 + K, K, 1)) return 1;
+  if (run_block(h, st, h->blocks[0], sb.E, F, sb.bb, sb.fin)) return 1;
+  const unsigned grid_cap = (unsigned)h->sm_count * 16;
+  for (int i = 1; i < L; ++i) {
+    const StageConsts& s = h->stages[i - 1];
+    const int Cw = s.Cw, fw = c.filter_widths[i], d = sp.dil[i - 1], R = sp.R[i - 1], H = (fw - 1) * d;
+    if (s.taps != fw) return fail("streaming: stage %d has %d taps, expected %d", i - 1, s.taps, fw);
+    if ((J * Cw) % 4) return fail("gast_stream_push_chunk: J*channels of stage %d is not a multiple of 4", i);
+    float* ring = sbase + sp.ring_off[i - 1];
+    const long long row4 = (long long)J * Cw / 4;
+    const long long g4 = (long long)n * (H + K) * row4, r4 = (long long)R * n * row4;
+    stream_chunk_gather_kernel<<<(unsigned)std::min<long long>(cdiv(g4, 256), grid_cap), 256, 0, st>>>(
+        reinterpret_cast<float4*>(cb.G), reinterpret_cast<const float4*>(ring),
+        reinterpret_cast<const float4*>(sb.fin), fresh, n, R, (int)(step % R), H, K, row4);
+    h->launches++;
+    stream_chunk_ring_kernel<<<(unsigned)std::min<long long>(cdiv(r4, 256), grid_cap), 256, 0, st>>>(
+        reinterpret_cast<float4*>(ring), reinterpret_cast<const float4*>(cb.G), fresh, n, R,
+        (int)((step + K - 1) % R), H, K, row4);
+    h->launches++;
+    // output frame (b, t) = time step+t: taps at G positions t, t+d, ..., t+H; residual at the newest tap (causal)
+    // or the centre tap t + H - (w/2) d (non-causal), as in the whole-sequence forward
+    const ASeg taps = seg_taps(cb.G, Cw, Cw, fw, (long long)d * J * Cw, RowMap{K, H + K, 1, 0});
+    const RowMap res{K, H + K, 1, c.causal ? H : H - (fw / 2) * d};
+    if (run_stage(h, st, s, F, taps, s.Wt, &s.tc_t, sb.tmp, cb.G, res, sb.act)) return 1;
+    if (run_block(h, st, h->blocks[i], sb.act, F, sb.bb, sb.fin)) return 1;
+  }
+  // rows of fin are already in (stream, frame, joint) order
+  if (launch_shrink(h, st, sb.fin, y, F * J, nullptr, nullptr)) return 1;
+  CUDA_OK(cudaGetLastError());
+  return 0;
 }

@@ -93,6 +93,40 @@ class SequenceBook(object):
         self.fresh[:] = False
         return fresh, hold, index
 
+    def advance_many(self, K, valid=None):
+        """-> (fresh (n,), hold (n, K), index (n, K)) of K consecutive pushes, as K calls of `advance()` return them,
+        with `end([s])` before push valid[s] of every live stream s whose valid[s] < K (0 <= valid[s] <= K; None:
+        no end).  Vectorised over the pushes: every stream is live up to its end and held from then on."""
+        K = int(K)
+        if K < 1:
+            raise ValueError('advance_many: K must be at least 1 (got %d)' % K)
+        if valid is None:
+            e = np.full(self.n, K, dtype=np.int64)
+        else:
+            e = np.asarray(valid, dtype=np.int64).reshape(-1)
+            if e.shape != (self.n,) or (e < 0).any() or (e > K).any():
+                raise ValueError('advance_many: valid must hold %d values in [0, %d]' % (self.n, K))
+        live = self.left < 0                               # live at the first push (a fresh stream is live)
+        ends = live & (e < K)
+        empty = ends & self.fresh & (e == 0)               # ended before its first frame: idle at once
+        # the held part of every stream starts at push kh with `left0` pushes left and a sequence of `lh` frames
+        kh = np.where(live, e, 0)
+        left0 = np.where(live, np.where(empty, 0, self.latency), self.left)
+        len0 = np.where(self.fresh, 0, self.length)
+        lh = np.where(live, len0 + kh, self.length)
+        k = np.arange(K, dtype=np.int64)[None, :]
+        hold = k >= kh[:, None]
+        index = np.where(hold, -1, len0[:, None] + k - self.latency)
+        left_k = left0[:, None] - (k - kh[:, None])        # pushes left before each held push
+        due = hold & (left_k > 0)
+        index[due] = (lh[:, None] - left_k)[due]
+        index[index < 0] = -1
+        fresh = self.fresh & ~empty
+        self.length = lh
+        self.left = np.where(live & ~ends, -1, np.maximum(left0 - (K - kh), 0))
+        self.fresh[:] = False
+        return fresh, hold, index
+
 
 class PoseStream(object):
     """O(1)-per-frame lifting of `n_streams` concurrent streams with any non-dense model of the drop-in classes
@@ -145,6 +179,8 @@ class PoseStream(object):
         self._sig = None                 # the handle's parameter signature at the last push
         self._state = None
         self._ws = None
+        self._chunk_ws = None            # push_frames: workspace of the largest K so far
+        self._chunk_masks = None
 
     def reset(self, streams=None):
         """Start new sequences on all (or the listed) streams with the next pushed frame; drop any pending tail."""
@@ -165,6 +201,26 @@ class PoseStream(object):
         self._masks.copy_(torch.from_numpy(mk).pin_memory(), non_blocking=True)
         return (self._masks[0].data_ptr() if any_f else None), (self._masks[1].data_ptr() if any_h else None)
 
+    def _begin(self, h, st):
+        """refresh the handle, refuse a push over history computed with other weights, allocate the state"""
+        eng, lib = self.engine, h.lib
+        h.refresh(self.model, st)
+        if self._sig is not None and h.sig != self._sig and not self.book.all_restarting():
+            raise eng.GastError('%s: the model\'s parameters or buffers changed since the last push '
+                                '(load_state_dict, an optimiser step or a training forward); the streams\' history '
+                                'was computed with the old weights -- call reset() before pushing again'
+                                % type(self).__name__)
+        if self._state is None:
+            m = self.copies * self.n
+            if lib.gast_stream_latency(h.h) != self.latency:
+                raise eng.GastError('gast_stream_latency: %s' % L.last_error())
+            nb = lib.gast_stream_state_bytes(h.h, m)
+            wb = lib.gast_stream_workspace_bytes(h.h, m)
+            if nb == 0 or wb == 0:
+                raise eng.GastError('gast_stream_state_bytes: %s' % L.last_error())
+            self._state = torch.empty(int(nb), dtype=torch.uint8, device=self.device)
+            self._ws = torch.empty(int(wb), dtype=torch.uint8, device=self.device)
+
     def push(self, frame):
         """frame (n_streams, J, in_features): the newest 2D keypoints of every stream (normalised screen
         coordinates; rows of held streams are ignored) -> (poses (n, J, 3), index (n,) CPU int64)."""
@@ -180,20 +236,7 @@ class PoseStream(object):
         y = torch.empty((self.n, self.J, 3), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             st = torch.cuda.current_stream(self.device).cuda_stream
-            h.refresh(self.model, st)
-            if self._sig is not None and h.sig != self._sig and not self.book.all_restarting():
-                raise eng.GastError('%s: the model\'s parameters or buffers changed since the last push '
-                                    '(load_state_dict, an optimiser step or a training forward); the streams\' history '
-                                    'was computed with the old weights -- call reset() before pushing again' % name)
-            if self._state is None:
-                if lib.gast_stream_latency(h.h) != self.latency:
-                    raise eng.GastError('gast_stream_latency: %s' % L.last_error())
-                nb = lib.gast_stream_state_bytes(h.h, m)
-                wb = lib.gast_stream_workspace_bytes(h.h, m)
-                if nb == 0 or wb == 0:
-                    raise eng.GastError('gast_stream_state_bytes: %s' % L.last_error())
-                self._state = torch.empty(int(nb), dtype=torch.uint8, device=self.device)
-                self._ws = torch.empty(int(wb), dtype=torch.uint8, device=self.device)
+            self._begin(h, st)
             fresh, hold, index = self.book.advance()
             fresh_p, hold_p = self._upload(fresh, hold)
             x, out = frame, y
@@ -220,6 +263,80 @@ class PoseStream(object):
         self.last_launches = launches
         return y, torch.from_numpy(index)
 
+    def push_frames(self, frames, valid=None):
+        """frames (n_streams, K, J, in_features): the next K frames of every stream -> (poses (n, K, J, 3) CUDA,
+        index (n, K) CPU int64), what K calls of `push` with frames[:, k] return, in one library call
+        (gast_stream_push_chunk).  valid (n,) or None: only the first valid[s] frames of stream s belong to its
+        sequence; a smaller value than K ends the sequence there (as `end([s])` before frame valid[s] would) and the
+        rest of the chunk returns its tail.  Rows of held frames are ignored.  `reset()` / `end()` take effect at
+        frame 0 of the call, as for `push`."""
+        eng = self.engine
+        name = type(self).__name__
+        frames = torch.as_tensor(frames, dtype=torch.float32, device=self.device).contiguous()
+        assert frames.dim() == 4 and frames.shape[0] == self.n and frames.shape[1] >= 1 and \
+            tuple(frames.shape[2:]) == (self.J, self.F), frames.shape
+        K = int(frames.shape[1])
+        if K == 1 and valid is None:
+            y, index = self.push(frames[:, 0])
+            return y.view(self.n, 1, self.J, 3), index.view(self.n, 1)
+        if self.model.training:
+            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
+        h = eng.model_handle(self.model, self.device)
+        lib = h.lib
+        m = self.copies * self.n
+        y = torch.empty((self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device).cuda_stream
+            self._begin(h, st)
+            wb = int(lib.gast_stream_chunk_workspace_bytes(h.h, m, K))
+            if wb == 0:
+                raise eng.GastError('gast_stream_chunk_workspace_bytes: %s' % L.last_error())
+            if self._chunk_ws is None or self._chunk_ws.numel() < wb:   # grows with K: serves every smaller K
+                self._chunk_ws = None
+                self._chunk_ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
+            fresh, hold, index = self.book.advance_many(K, valid)
+            fresh_p, hold_p = self._upload_chunk(fresh, hold)
+            x, out = frames, y
+            if self.augment:
+                # (2, n*K, J, F) = 2n streams of K frames: [original | mirrored]
+                x = torch.empty((2, self.n, K, self.J, self.F), dtype=torch.float32, device=self.device)
+                if lib.gast_tta_prepare(C.c_void_p(frames.data_ptr()), C.c_void_p(x.data_ptr()), self.n * K, self.J,
+                                        self.F, 0, 0, len(self.kps_left), self._kl, self._kr, C.c_void_p(st)) != 0:
+                    raise eng.GastError('gast_tta_prepare: %s' % L.last_error())
+                out = torch.empty((2, self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
+            rc = lib.gast_stream_push_chunk(h.h, C.c_void_p(self._state.data_ptr()), C.c_int64(self.step),
+                                            C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), m, K,
+                                            C.c_void_p(fresh_p), C.c_void_p(hold_p),
+                                            C.c_void_p(self._chunk_ws.data_ptr()), self._chunk_ws.numel(),
+                                            C.c_void_p(st))
+            if rc != 0:
+                raise eng.GastError('gast_stream_push_chunk: %s' % L.last_error())
+            launches = int(lib.gast_last_launch_count(h.h))
+            if self.augment:
+                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(y.data_ptr()), self.n * K, self.J,
+                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
+                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
+                launches += 2
+            self._sig = h.sig
+        self.step += K
+        self.last_launches = launches
+        return y, torch.from_numpy(index)
+
+    def _upload_chunk(self, fresh, hold):
+        """-> device pointers of the fresh (n) and hold (n, K) masks of a chunk, repeated for the mirrored half
+        (None where no stream is set)"""
+        any_f, any_h = bool(fresh.any()), bool(hold.any())
+        if not (any_f or any_h):
+            return None, None
+        m = self.copies * self.n
+        mk = np.concatenate([np.tile(fresh.astype(np.int32), self.copies),
+                             np.tile(hold.astype(np.int32), (self.copies, 1)).reshape(-1)])
+        # kept until the next chunk, so that no allocation of this one reuses it before the push read it
+        self._chunk_masks = dev = torch.empty(mk.size, dtype=torch.int32, device=self.device)
+        # pinned + non_blocking: no device sync; the caching host allocator keeps the buffer until the copy ran
+        dev.copy_(torch.from_numpy(mk).pin_memory(), non_blocking=True)
+        return (dev.data_ptr() if any_f else None), (dev[m:].data_ptr() if any_h else None)
+
 
 class CausalStream(PoseStream):
     """O(1)-per-frame lifting of `n_streams` concurrent streams with a causal model of the drop-in classes
@@ -237,6 +354,75 @@ class CausalStream(PoseStream):
         """frame (n_streams, J, in_features): the newest 2D keypoints of every stream (normalised screen
         coordinates).  Returns the 3D pose of that frame, (n_streams, J, 3)."""
         return super(CausalStream, self).push(frame)[0]
+
+    def push_frames(self, frames):
+        """frames (n_streams, K, J, in_features): the next K frames of every stream -> their 3D poses
+        (n_streams, K, J, 3), what K calls of `push` return, in one library call."""
+        return super(CausalStream, self).push_frames(frames)[0]
+
+
+def lift_sequences(model_pos, sequences, n_streams=64, chunk=256, augment=False, kps_left=None, kps_right=None,
+                   joints_left=None, joints_right=None):
+    """Whole-sequence lifting in bounded memory: sequences [(T_i, J, in_features)] -> [(T_i, J, 3) CUDA tensors],
+    the poses `UnchunkedGenerator` + the model forward (+ the TTA merge with `augment=True`) compute for each
+    sequence, i.e. what `tta.evaluate_sequence` returns.  The sequences are packed onto `n_streams` streams of a
+    `PoseStream` and pushed `chunk` frames at a time; a stream starts its next sequence at the first chunk after the
+    last pose of its previous one.  The library's scratch memory depends on (n_streams, chunk), not on T_i."""
+    from . import engine
+    dev = next(model_pos.parameters()).device
+    seqs = [torch.as_tensor(s, dtype=torch.float32).to(dev) for s in sequences]
+    J, F = int(model_pos.num_joints_in), int(model_pos.in_features)
+    for s in seqs:
+        if s.dim() != 3 or tuple(s.shape[1:]) != (J, F):
+            raise engine.GastError('lift_sequences: every sequence must be (T, %d, %d), got %s' % (J, F, tuple(s.shape)))
+    lengths = [int(s.shape[0]) for s in seqs]
+    starts = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
+    out = torch.empty((int(starts[-1]), J, 3), dtype=torch.float32, device=dev)
+    todo = [q for q, T in enumerate(lengths) if T > 0]
+    if todo:
+        model_pos.eval()
+        allx = torch.cat([seqs[q] for q in todo])                 # every frame, for one gather per chunk
+        base = np.zeros(len(lengths), dtype=np.int64)             # first row of sequence q in allx
+        base[todo] = np.concatenate([[0], np.cumsum([lengths[q] for q in todo])[:-1]])
+        n = max(1, min(int(n_streams), len(todo)))
+        ps = PoseStream(model_pos, n, augment=augment, kps_left=kps_left, kps_right=kps_right,
+                        joints_left=joints_left, joints_right=joints_right, device=dev)
+        lat = ps.latency
+        T = np.array(lengths, dtype=np.int64)
+        cur = np.full(n, -1, dtype=np.int64)                      # sequence on each stream (-1: none)
+        pushed = np.zeros(n, dtype=np.int64)                      # its frames pushed so far
+        steps = np.zeros(n, dtype=np.int64)                       # pushes since it started: T + latency in all
+        queue = list(reversed(todo))
+        with torch.no_grad():
+            while True:
+                for s in range(n):
+                    if cur[s] < 0 or steps[s] == T[cur[s]] + lat:
+                        cur[s] = -1
+                        if queue:
+                            cur[s], pushed[s], steps[s] = queue.pop(), 0, 0
+                            ps.reset([s])
+                active = cur >= 0
+                if not active.any():
+                    break
+                Ta = T[cur[active]]
+                K = int(min(chunk, (Ta + lat - steps[active]).max()))
+                valid = np.zeros(n, dtype=np.int64)
+                valid[active] = np.minimum(K, Ta - pushed[active])
+                k = np.arange(K)[None, :]
+                rows = np.where(k < valid[:, None], (base[cur.clip(min=0)] + pushed)[:, None] + k, 0)
+                frames = allx[torch.from_numpy(rows).to(dev)]       # rows of held frames: any frame, not read
+                y, index = ps.push_frames(frames, valid=valid)
+                index = index.numpy()
+                for s in np.flatnonzero(active):
+                    sel = np.flatnonzero(index[s] >= 0)           # one run of consecutive poses of the sequence
+                    if sel.size:
+                        a, c, q = int(index[s, sel[0]]), sel.size, cur[s]
+                        out[starts[q] + a:starts[q] + a + c] = y[s, sel[0]:sel[0] + c]
+                    pushed[s] += valid[s]
+                    steps[s] = min(steps[s] + K, T[cur[s]] + lat)
+                    if pushed[s] == T[cur[s]] and valid[s] == K:
+                        ps.end([s])                               # the sequence ended with the chunk's last frame
+    return [out[starts[q]:starts[q + 1]] for q in range(len(lengths))]
 
 
 class WindowStream(object):

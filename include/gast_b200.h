@@ -214,6 +214,24 @@ int32_t gast_stream_latency(const gast_t* h);
 int gast_stream_push_ex(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
                         const int32_t* fresh, const int32_t* hold, void* workspace, size_t workspace_bytes,
                         void* stream);
+/* gast_stream_push_chunk: K frames per stream in one call.  x (n_streams, K, J, in_features) -> y (n_streams, K, J, 3),
+ *   equal up to float rounding to K calls of gast_stream_push_ex at steps step, step+1, ..., step+K-1 with x[:, k],
+ *   fresh at k = 0 only and hold[:, k]; it also leaves `state` as those K pushes would.  So single pushes and chunks
+ *   can be mixed freely on one state, and step advances by K.  Same state (gast_stream_state_bytes), handles (causal
+ *   or not, not dense) and step / fresh / weight-change rules as gast_stream_push_ex.  The launch count does not
+ *   depend on n_streams or K: the work is one forward over n_streams*K positions, so frames that are already
+ *   available (a burst, catching up, a recorded sequence) cost far less than K single pushes.
+ *   fresh (n_streams) int32 or null: applies to frame 0 of the chunk (start sequences only at chunk boundaries).
+ *   hold (n_streams, K) int32 or null: hold[s, k] != 0 = frame k of stream s repeats that stream's newest frame
+ *   (which may be a held frame earlier in the chunk) and x[s, k] is not read; fresh wins over hold at k = 0.
+ *   K >= 1 and n_streams*K*J < 2^31.  The workspace is gast_stream_chunk_workspace_bytes(h, n_streams, K) bytes
+ *   (0 for invalid arguments; it grows with K, so a workspace sized for K serves every smaller K).
+ *   With test-time augmentation: gast_tta_prepare / gast_tta_merge with T = n_streams*K: the (2, n*K, J, F) layout is
+ *   2n streams of K frames, with the masks repeated for both halves. */
+size_t gast_stream_chunk_workspace_bytes(gast_t* h, int32_t n_streams, int32_t K);
+int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
+                           int32_t K, const int32_t* fresh, const int32_t* hold, void* workspace,
+                           size_t workspace_bytes, void* stream);
 
 /* ---- either side of the forward, on the device (SURVEY.md 8f N1-N3) --------------------------------
  * All pointers are device pointers unless marked (host).  Work is enqueued on `stream`.
