@@ -97,6 +97,7 @@ struct gast_handle {
   int launches = 0;
   int tc_launches = 0;
   int gemm_core = 0;                 // 0 auto (tensor cores where possible), 1 force FFMA
+  int precision = 0;                 // 0 fp32-grade (3xTF32 on the tensor cores), 1 single-pass TF32 (inference only)
   // training: per-GEMM tensor-core operand copies (3xTF32), indexed by the GEMM's position in the step (train.cuh)
   std::vector<TcWeights> train_tc;
   // optional per-launch device timing (bench.py roofline): event pairs around every launch
@@ -293,6 +294,13 @@ extern "C" int gast_set_gemm_core(gast_t* h, int32_t core) {
   if (!h) return fail("null handle");
   if (core != 0 && core != 1) return fail("gast_set_gemm_core: core must be 0 (auto) or 1 (ffma)");
   h->gemm_core = core;
+  return 0;
+}
+
+extern "C" int gast_set_precision(gast_t* h, int32_t mode) {
+  if (!h) return fail("null handle");
+  if (mode != 0 && mode != 1) return fail("gast_set_precision: mode must be 0 (fp32-grade) or 1 (tf32), got %d", mode);
+  h->precision = mode;
   return 0;
 }
 
@@ -627,7 +635,7 @@ static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p,
   if (p.N % 4 || p.ld_out % 4) return fail("internal: N/ld_out must be multiples of 4");
   if (h->gemm_core == 0 && tcw && tc_supported(p, epi, *tcw)) {
     TimedLaunch tl(h, st, LK_TC_PLAIN + epi);
-    int rc = tc_launch(st, epi, p, *tcw);
+    int rc = tc_launch(st, epi, p, *tcw, h->precision == 1 ? TC_1XTF32 : TC_3XTF32);
     if (rc) return fail("tensor-core gemm launch failed: %s", cudaGetErrorString((cudaError_t)rc));
     h->launches++;
     h->tc_launches++;
@@ -985,14 +993,22 @@ extern "C" int gast_bind_grads(gast_t* h, int32_t n, const char* const* keys, vo
   return 0;
 }
 
-static int train_check(gast_handle* h) {
-  if (h->cfg.kind != GAST_KIND_MODEL) return fail("training is implemented for the MODEL kind only");
+// reduced precision is for inference: training and every gradient run at fp32 grade, and nothing falls back silently
+static int precision_check(gast_handle* h, const char* what) {
+  if (h->precision != 0)
+    return fail("%s: reduced precision is inference-only; call gast_set_precision(h, 0) before training or "
+                "differentiating (precision is %d)", what, h->precision);
   return 0;
 }
 
+static int train_check(gast_handle* h, const char* what) {
+  if (h->cfg.kind != GAST_KIND_MODEL) return fail("training is implemented for the MODEL kind only");
+  return precision_check(h, what);
+}
+
 // workspace of a training forward + backward of the mode `ts` describes, by a dry run of both (no launches); 0 on error
-static size_t train_dry_run_bytes(gast_handle* h, int B, int T, TrainState ts, bool pgrad) {
-  if (!h || train_check(h)) return 0;
+static size_t train_dry_run_bytes(gast_handle* h, int B, int T, TrainState ts, bool pgrad, const char* what) {
+  if (!h || train_check(h, what)) return 0;
   Arena a{nullptr, 0, 0, true};
   Lookup L{h};
   TCtx c{h, nullptr, &a, &L, h->cfg.num_joints, true};
@@ -1005,13 +1021,13 @@ static size_t train_dry_run_bytes(gast_handle* h, int B, int T, TrainState ts, b
 extern "C" size_t gast_train_workspace_bytes(gast_t* h, int32_t B, int32_t T, float dropout_p) {
   TrainState ts;
   ts.drop_p = dropout_p;
-  return train_dry_run_bytes(h, B, T, ts, true);
+  return train_dry_run_bytes(h, B, T, ts, true, "gast_train_workspace_bytes");
 }
 
 extern "C" int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B, int32_t T, float dropout_p,
                                   uint64_t seed, void* workspace, size_t workspace_bytes, void* stream) {
   if (!h) return fail("gast_forward_train: null handle");
-  if (train_check(h)) return 1;
+  if (train_check(h, "gast_forward_train")) return 1;
   if (dropout_p < 0.f || dropout_p >= 1.f) return fail("gast_forward_train: dropout_p out of range");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CUDA_OK(cudaSetDevice(h->cfg.device));
@@ -1051,6 +1067,7 @@ extern "C" int gast_backward(gast_t* h, const float* dy, void* workspace, size_t
 extern "C" int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_t param_grads, void* workspace,
                                    size_t workspace_bytes, void* stream) {
   if (!h) return fail("gast_backward: null handle");
+  if (precision_check(h, "gast_backward")) return 1;
   if (!dx && !param_grads) return fail("gast_backward_input: neither dx nor parameter gradients requested");
   size_t ti = h->trains.size();
   for (size_t i = 0; i < h->trains.size(); ++i)
@@ -1082,18 +1099,18 @@ static TrainState eval_state(int strided_now) {
 }
 
 extern "C" size_t gast_eval_backward_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now) {
-  return train_dry_run_bytes(h, B, T, eval_state(strided_now), true);
+  return train_dry_run_bytes(h, B, T, eval_state(strided_now), true, "gast_eval_backward_workspace_bytes");
 }
 
 extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads, int32_t B,
                                   int32_t T, int32_t strided_now, void* workspace, size_t workspace_bytes, void* stream) {
   if (!h) return fail("gast_eval_backward: null handle");
-  if (train_check(h)) return 1;
+  if (train_check(h, "gast_eval_backward")) return 1;
   if (B <= 0 || T <= 0) return fail("gast_eval_backward: empty batch (B=%d T=%d)", B, T);
   if (!x || !dy) return fail("gast_eval_backward: x and dy must be device pointers");
   if (!dx && !param_grads) return fail("gast_eval_backward: neither dx nor parameter gradients requested");
   TrainState ts = eval_state(strided_now);
-  const size_t need = train_dry_run_bytes(h, B, T, ts, param_grads != 0);
+  const size_t need = train_dry_run_bytes(h, B, T, ts, param_grads != 0, "gast_eval_backward");
   if (need == 0) return 1;
   if (!workspace || workspace_bytes < need)
     return fail("gast_eval_backward: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
@@ -1114,13 +1131,15 @@ extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, fl
 
 // ------------------------------------------------------------------------------------------
 // debug / probe entry: out[M,N] = A[M,K] . W[N,K]^T on a chosen GEMM core (test infrastructure
-// for the numerics of the tensor-core path; not used by the forward).
+// for the numerics of the tensor-core path; not used by the forward).  tc_mode: the tensor-core core's precision
+// (0 3xTF32, 1 single-pass TF32).
 // ------------------------------------------------------------------------------------------
 extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32_t N, int32_t K,
                                int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (M <= 0 || N <= 0 || K <= 0 || N % 4 || K % 4) return fail("gast_debug_gemm: bad shape");
-  if (core < 0 || core > 1 || tc_mode != 0) return fail("gast_debug_gemm: core must be 0 (tensor cores) or 1 (FFMA), tc_mode 0");
+  if (core < 0 || core > 1 || tc_mode < 0 || tc_mode > 1 || (core == 1 && tc_mode != 0))
+    return fail("gast_debug_gemm: core must be 0 (tensor cores, tc_mode 0 = 3xTF32 or 1 = TF32) or 1 (FFMA, tc_mode 0)");
   GemmP p;
   gemm_flat(p, M);
   p.nseg = 1; p.seg[0] = seg_flat(A, K, K);
@@ -1138,7 +1157,7 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
     cudaFuncSetAttribute((const void*)gemm_ffma_kernel<EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   }
   auto launch = [&]() -> int {
-    if (core == 0) return tc_launch(st, EPI_PLAIN, p, t);
+    if (core == 0) return tc_launch(st, EPI_PLAIN, p, t, tc_mode == 1 ? TC_1XTF32 : TC_3XTF32);
     dim3 grid(cdiv(M, 128), cdiv(N, FF_BN));
     gemm_ffma_kernel<EPI_PLAIN><<<grid, FF_THREADS, ffma_smem_bytes(EPI_PLAIN, 1, 128, 1), st>>>(p);
     return (int)cudaGetLastError();

@@ -1,22 +1,27 @@
-// Tensor-core GEMM core of the lifting path (sm_90a): error-compensated TF32 (3xTF32) on wgmma.
+// Tensor-core GEMM core of the lifting path (sm_90a): TF32 on wgmma, in two precisions (template PREC).
 //
-//   D[128 rows, 128 cols] = A_hi.B_hi + A_lo.B_hi + A_hi.B_lo
+//   TC_3XTF32 (default, fp32-grade):  D[128 rows, 128 cols] = A_hi.B_hi + A_lo.B_hi + A_hi.B_lo
+//   TC_1XTF32 (opt-in, gast_set_precision(h, 1)):  D = A_hi.B_hi
 //
-// where x_hi = tf32(x) and x_lo = tf32(x - x_hi).  The dropped A_lo.B_lo term is 2^-22 of the result, so
-// D matches an fp32 FFMA GEMM to ~1e-7 relative (the parity bar is 1e-4 abs; a single TF32 pass would
-// not reach it, SURVEY.md §7).
+// where x_hi = tf32(x) and x_lo = tf32(x - x_hi).  The dropped A_lo.B_lo term is 2^-22 of the result, so the
+// 3xTF32 D matches an fp32 FFMA GEMM to ~1e-7 relative (the parity bar is 1e-4 abs; a single TF32 pass does
+// not reach it, SURVEY.md §7).  The single pass is a third of the tensor work per multiply-add; its operands are
+// rounded to 10 mantissa bits, and it is offered for inference only (DESIGN.md §4.1).
+//
+// The two forms share everything below except the slot contents (B_lo is not staged in 1xTF32), the ring depth
+// and the number of wgmmas per k8 step (3 or 1).
 //
 // Two-level accumulation: the tensor core aligns and truncates its addends, so a long chain of MMAs
 // into one accumulator is biased towards zero by ~0.5 ulp per MMA.  Every 16 K are therefore accumulated in a
-// fresh register tile (6 wgmmas) and added into the fp32 tile sum with round-to-nearest (32 K per partial sum
+// fresh register tile (6 wgmmas in 3xTF32, 2 in 1xTF32) and added into the fp32 tile sum with round-to-nearest (32 K per partial sum
 // roughly doubled the error and pushed single training gradients past their bar).
 //
-// Per CTA (384 threads = 3 warpgroups, one CTA per SM), warp-specialised around a 3-slot shared-memory ring of
-// 32-wide K stages (slot = B_hi | B_lo | A):
+// Per CTA (384 threads = 3 warpgroups, one CTA per SM), warp-specialised around a shared-memory ring of
+// 32-wide K stages (3xTF32: 3 slots of B_hi | B_lo | A; 1xTF32: tc_stages(TC_1XTF32) slots of B_hi | A):
 //   producer (warpgroup 0, 40 registers after setmaxnreg): waits for a slot's `empty` mbarrier, then fills it.
 //     B (weights): the hi and lo copies are stored [K/4][N][4] (tc_prepare_weights), so one 3D TMA box per operand
 //                lands in the no-swizzle K-major core-matrix layout wgmma reads from shared memory (8 rows x 16 B
-//                core matrices, 128 B apart along N, 2048 B apart along K); one elected thread issues both boxes.
+//                core matrices, 128 B apart along N, 2048 B apart along K); one elected thread issues the boxes.
 //     A (activations): rows are gathered per frame (dilated / strided taps, residual slices, concatenations), so
 //                they arrive by cp.async (16 B per row and k-quad, zero-filled outside the tile) from all 128
 //                producer threads.  A stage never straddles a tap (Kc % 32 == 0), so segment, tap and column are
@@ -24,8 +29,8 @@
 //     The slot's `full` mbarrier completes when the TMA bytes (expect_tx) and every producer thread's cp.asyncs
 //     (cp.async.mbarrier.arrive.noinc) have landed: 1 + 128 arrivals.
 //   consumers (warpgroups 1 and 2, 232 registers): warpgroup 1 + w owns rows 64w .. 64w+63 and all 128 columns:
-//     wgmma.m64n128k8 tf32, A from registers (loaded from the slot and split into tf32 hi / lo there), B from the
-//     shared-memory descriptor.  A stage's two 16-K partials (6 wgmmas each) go into two register tiles back to back;
+//     wgmma.m64n128k8 tf32, A from registers (loaded from the slot and converted to tf32 there, split into hi / lo in
+//     3xTF32), B from the shared-memory descriptor.  A stage's two 16-K partials go into two register tiles back to back;
 //     the first is added into the tile sum while the second runs (wgmma.wait_group 1), then the second is retired
 //     and added, and the slot is released (its `empty` mbarrier, one arrival per consumer warp, 8 in all).  No
 //     partial stays in flight across the loop's back edge: ptxas then serialises every wgmma of the kernel (C7514).
@@ -52,24 +57,35 @@ struct TcWeights {
   bool ready = false;
 };
 
+enum { TC_3XTF32 = 0, TC_1XTF32 = 1 };               // precision of the core: gast_set_precision's mode
+
+#ifndef GAST_TC1_STAGES
+#define GAST_TC1_STAGES 3                             // ring depth of the 1xTF32 form: 4 and 5 measured slower (DESIGN.md §4.1)
+#endif
+
 constexpr int TC_BM = 128, TC_BN = 128;
 constexpr int TC_KS = 32;                            // K per ring stage; segment widths must be multiples of it
-constexpr int TC_STAGES = 3;                         // a fourth slot measured slower (DESIGN.md §4.1)
-constexpr int TC_KP = 16;                            // K per partial sum (6 wgmmas), added into the tile sum with RN
+constexpr int TC_KP = 16;                            // K per partial sum, added into the tile sum with RN
 constexpr int TC_THREADS = 384;                      // warpgroup 0 produces, warpgroups 1 and 2 consume
 constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;   // 128 * 40 + 256 * 232 <= 64K registers of the SM
 constexpr int TC_ALD = TC_KS + 4;                    // A stage row stride (floats): conflict-free fragment loads
 constexpr int TC_B_BYTES = TC_BN * TC_KS * 4;        // one of B_hi / B_lo in a stage
 constexpr int TC_A_BYTES = TC_BM * TC_ALD * 4;
-constexpr int TC_SLOT = 2 * TC_B_BYTES + TC_A_BYTES; // B_hi | B_lo | A
-constexpr int TC_RING = TC_STAGES * TC_SLOT;
+// B copies per slot, slot size and ring depth of each precision.  3xTF32: a fourth slot measured slower
+// (DESIGN.md §4.1).
+__host__ __device__ constexpr int tc_nb(int prec) { return prec == TC_1XTF32 ? 1 : 2; }
+__host__ __device__ constexpr int tc_slot(int prec) { return tc_nb(prec) * TC_B_BYTES + TC_A_BYTES; }   // B_hi [| B_lo] | A
+__host__ __device__ constexpr int tc_stages(int prec) { return prec == TC_1XTF32 ? GAST_TC1_STAGES : 3; }
+__host__ __device__ constexpr int tc_ring(int prec) { return tc_stages(prec) * tc_slot(prec); }
 constexpr int TC_STG_LD = 136;                       // [row][col] stride of the accumulator hand-over to the epilogue
 constexpr int TC_ROWBASE_BYTES = 3 * 128 * sizeof(long long);
 constexpr int TC_SMEM_MAX = 200 * 1024;
-static_assert(TC_SLOT % 1024 == 0, "ring slots stay 1024-byte aligned");
+static_assert(tc_slot(TC_3XTF32) % 1024 == 0 && tc_slot(TC_1XTF32) % 1024 == 0, "ring slots stay 1024-byte aligned");
+static_assert(tc_ring(TC_1XTF32) + 16 * tc_stages(TC_1XTF32) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX,
+              "the 1xTF32 ring fits the shared memory the 3xTF32 form may use");
 
-__host__ __device__ inline size_t tc_smem_bytes(int epi, int J, int fpt, int hpt) {
-  size_t m = (size_t)TC_RING + 16 * TC_STAGES;       // + a full and an empty mbarrier per slot
+__host__ __device__ inline size_t tc_smem_bytes(int prec, int epi, int J, int fpt, int hpt) {
+  size_t m = (size_t)tc_ring(prec) + 16 * tc_stages(prec);   // + a full and an empty mbarrier per slot
   const size_t stg = (size_t)TC_BM * TC_STG_LD * 4;
   const size_t e = ffma_smem_bytes(epi, J, fpt, hpt) - TC_ROWBASE_BYTES;
   if (stg > m) m = stg;
@@ -151,7 +167,8 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], const uint32_t (&a)[4
 }
 
 // One 16-K partial of a consumer: d = sum over the k8 steps s0, s0 + 1 of the slot at sb of
-// A_lo.B_hi + A_hi.B_lo + A_hi.B_hi (small products first), issued as one wgmma group
+// A_lo.B_hi + A_hi.B_lo + A_hi.B_hi (3xTF32, small products first) or A_hi.B_hi (1xTF32), issued as one wgmma group
+template <int PREC>
 __device__ __forceinline__ void tc_partial(float (&d)[64], const uint32_t (&ah)[2][4], const uint32_t (&al)[2][4],
                                            uint32_t sb, int s0) {
   tile_fence(d);
@@ -159,15 +176,22 @@ __device__ __forceinline__ void tc_partial(float (&d)[64], const uint32_t (&ah)[
 #pragma unroll
   for (int i = 0; i < 2; ++i) {   // k8 step s = core matrices 2s, 2s+1
     const int s = s0 + i;
-    const uint64_t dh = tc_bdesc(sb + s * 4096), dl = tc_bdesc(sb + TC_B_BYTES + s * 4096);
-    wgmma_tf32(d, al[i], dh, i);
-    wgmma_tf32(d, ah[i], dl, 1);
-    wgmma_tf32(d, ah[i], dh, 1);
+    const uint64_t dh = tc_bdesc(sb + s * 4096);
+    if (PREC == TC_3XTF32) {
+      const uint64_t dl = tc_bdesc(sb + TC_B_BYTES + s * 4096);
+      wgmma_tf32(d, al[i], dh, i);
+      wgmma_tf32(d, ah[i], dl, 1);
+      wgmma_tf32(d, ah[i], dh, 1);
+    } else {
+      wgmma_tf32(d, ah[i], dh, i);
+    }
   }
   wgmma_commit();
 }
 
-// A fragment rows r0, r0 + 8 of the k8 steps s0, s0 + 1 of a slot's A (row stride TC_ALD), split into tf32 hi / lo
+// A fragment rows r0, r0 + 8 of the k8 steps s0, s0 + 1 of a slot's A (row stride TC_ALD), rounded to tf32 (hi) and,
+// in 3xTF32, the rounding error split off as lo
+template <int PREC>
 __device__ __forceinline__ void tc_load_a(const float* A, int r0, int t, int s0, uint32_t (&ah)[2][4],
                                           uint32_t (&al)[2][4]) {
 #pragma unroll
@@ -178,7 +202,7 @@ __device__ __forceinline__ void tc_load_a(const float* A, int r0, int t, int s0,
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       ah[i][q] = tf32_bits(x[q]);
-      al[i][q] = tf32_bits(x[q] - __uint_as_float(ah[i][q]));
+      if (PREC == TC_3XTF32) al[i][q] = tf32_bits(x[q] - __uint_as_float(ah[i][q]));
     }
   }
 }
@@ -199,17 +223,19 @@ __device__ __forceinline__ void tc_tile(const GemmP& p, int& rt, int& ctile) {
   ctile = (int)b - rt * col_tiles;
 }
 
-template <int EPI>
+// mlo is not read in 1xTF32
+template <int EPI, int PREC>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensorMap mhi,
                const __grid_constant__ CUtensorMap mlo) {
+  constexpr int STAGES = tc_stages(PREC), SLOT = tc_slot(PREC), NB = tc_nb(PREC);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   long long* rowbase = reinterpret_cast<long long*>(smem_raw);          // [3][128]
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t rb = (raw + TC_ROWBASE_BYTES + 1023) & ~1023u;        // ring base (shared address)
   unsigned char* ring = smem_raw + (rb - raw);
-  const uint32_t full0 = rb + TC_RING;                                  // per ring slot: stage landed
-  const uint32_t empty0 = full0 + 8 * TC_STAGES;                        // per ring slot: both consumers done with it
+  const uint32_t full0 = rb + tc_ring(PREC);                            // per ring slot: stage landed
+  const uint32_t empty0 = full0 + 8 * STAGES;                           // per ring slot: both consumers done with it
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int J = p.J;
@@ -221,7 +247,7 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   const int n0 = ctile * TC_BN;
 
   if (tid == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) {
+    for (int s = 0; s < STAGES; ++s) {
       mbar_init(full0 + 8 * s, 1 + 128);
       mbar_init(empty0 + 8 * s, 8);
     }
@@ -244,19 +270,19 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   for (int s = 0; s < p.nseg; ++s) nstages += p.seg[s].K / TC_KS;
 
   if (warp < 4) {
-    // producer: stage c into ring slot c % TC_STAGES once both consumers have released the slot's previous stage
+    // producer: stage c into ring slot c % STAGES once both consumers have released the slot's previous stage
     setmaxnreg_dec<TC_PRODUCER_REGS>();
     const int q = tid & 7, rq = tid >> 3;                               // k-quad q of rows rq + 16 i
     int seg = 0, k0 = 0, kcol = 0, tap = 0, kin = 0;                    // stage start: segment, K in it, W column, tap
     for (int c = 0; c < nstages; ++c) {
-      const int slot = c % TC_STAGES;
-      if (c >= TC_STAGES) mbar_wait(empty0 + 8 * slot, (c / TC_STAGES - 1) & 1);
-      const uint32_t sb = rb + slot * TC_SLOT, full = full0 + 8 * slot;
+      const int slot = c % STAGES;
+      if (c >= STAGES) mbar_wait(empty0 + 8 * slot, (c / STAGES - 1) & 1);
+      const uint32_t sb = rb + slot * SLOT, full = full0 + 8 * slot;
       if (tid == 0) {
-        mbar_arrive_expect_tx(full, 2 * TC_B_BYTES);
+        mbar_arrive_expect_tx(full, NB * TC_B_BYTES);
         const int kq = (kcol + k0) >> 2;
         tma_load_3d(sb, &mhi, full, 0, n0, kq);
-        tma_load_3d(sb + TC_B_BYTES, &mlo, full, 0, n0, kq);
+        if (NB == 2) tma_load_3d(sb + TC_B_BYTES, &mlo, full, 0, n0, kq);
       }
       const ASeg& sg = p.seg[seg];
       const float* src = sg.base + tap * sg.tap_stride + kin + q * 4;
@@ -264,7 +290,7 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
       for (int i = 0; i < TC_BM / 16; ++i) {
         const int r = rq + 16 * i;
         const long long off = rowbase[seg * 128 + r];
-        cp_async16(sb + 2 * TC_B_BYTES + (r * TC_ALD + q * 4) * 4, off >= 0 ? src + off : sg.base, off >= 0 ? 16 : 0);
+        cp_async16(sb + NB * TC_B_BYTES + (r * TC_ALD + q * 4) * 4, off >= 0 ? src + off : sg.base, off >= 0 ? 16 : 0);
       }
       cp_async_arrive(full);
       k0 += TC_KS;
@@ -287,15 +313,15 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 
   for (int c = 0; c < nstages; ++c) {
-    const int slot = c % TC_STAGES;
-    mbar_wait(full0 + 8 * slot, (c / TC_STAGES) & 1);
-    const uint32_t sb = rb + slot * TC_SLOT;
-    const float* A = reinterpret_cast<const float*>(ring + slot * TC_SLOT + 2 * TC_B_BYTES);
+    const int slot = c % STAGES;
+    mbar_wait(full0 + 8 * slot, (c / STAGES) & 1);
+    const uint32_t sb = rb + slot * SLOT;
+    const float* A = reinterpret_cast<const float*>(ring + slot * SLOT + NB * TC_B_BYTES);
     uint32_t ah[2][4], al[2][4];
-    tc_load_a(A, r0, t, 0, ah, al);
-    tc_partial(part0, ah, al, sb, 0);
-    tc_load_a(A, r0, t, 2, ah, al);
-    tc_partial(part1, ah, al, sb, 2);
+    tc_load_a<PREC>(A, r0, t, 0, ah, al);
+    tc_partial<PREC>(part0, ah, al, sb, 0);
+    tc_load_a<PREC>(A, r0, t, 2, ah, al);
+    tc_partial<PREC>(part1, ah, al, sb, 2);
     wgmma_wait<1>();                            // the first partial has retired ...
     tc_add(acc, part0);                         // ... and is summed while the second runs
     wgmma_wait<0>();
@@ -329,7 +355,7 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   gemm_epilogue<EPI>(p, out, reinterpret_cast<float*>(ring), ct, fe, nfe, nfe * J, ctile * TC_BN, ctile);
 }
 
-// W [N][K] -> hi / lo in the TMA-friendly layout [K/4][N][4]
+// W [N][K] -> hi / lo in the TMA-friendly layout [K/4][N][4] (both precisions read hi = tf32(W))
 __global__ void tc_split_kernel(const float* __restrict__ w, float* __restrict__ hi, float* __restrict__ lo, int N, int K) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)N * K) return;
@@ -392,6 +418,7 @@ inline int tc_prepare_weights(TcWeights& t, const float* W, int N, int K, cudaSt
   return 0;
 }
 
+// The shapes the core takes are the same in both precisions (the 1xTF32 ring is no larger than the bound below).
 inline bool tc_supported(const GemmP& p, int epi, const TcWeights& t) {
   if (!t.ready || t.K != p.ldw || t.N < p.N || p.N % 4) return false;
   for (int s = 0; s < p.nseg; ++s) {
@@ -399,30 +426,38 @@ inline bool tc_supported(const GemmP& p, int epi, const TcWeights& t) {
     if (sg.K % TC_KS || sg.Kc % TC_KS || sg.ld % 4 || sg.tap_stride % 4) return false;
     if (reinterpret_cast<uintptr_t>(sg.base) & 15) return false;
   }
-  if (tc_smem_bytes(epi, p.J, p.fpt, epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1) > TC_SMEM_MAX) return false;
+  const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
+  if (tc_smem_bytes(TC_3XTF32, epi, p.J, p.fpt, hpt) > TC_SMEM_MAX) return false;
+  if (tc_smem_bytes(TC_1XTF32, epi, p.J, p.fpt, hpt) > TC_SMEM_MAX) return false;
   return true;
 }
 
-// One CTA per tile, tile = row tile * column tiles + column tile (the column tile fastest, see gemm_tc_kernel).
-inline int tc_launch(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t) {
+template <int PREC>
+inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t) {
   const dim3 grid((unsigned)(((p.F + p.fpt - 1) / p.fpt) * ((p.N + TC_BN - 1) / TC_BN)));
   const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
-  const size_t smem = tc_smem_bytes(epi, p.J, p.fpt, hpt);
+  const size_t smem = tc_smem_bytes(PREC, epi, p.J, p.fpt, hpt);
   static bool attr_set[64][3];              // the shared-memory opt-in is per device
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr_set[dev & 63][epi]) {
-    const void* fn = epi == EPI_PLAIN ? (const void*)gemm_tc_kernel<EPI_PLAIN>
-                   : epi == EPI_SEMCH ? (const void*)gemm_tc_kernel<EPI_SEMCH>
-                                      : (const void*)gemm_tc_kernel<EPI_GLOBAL>;
+    const void* fn = epi == EPI_PLAIN ? (const void*)gemm_tc_kernel<EPI_PLAIN, PREC>
+                   : epi == EPI_SEMCH ? (const void*)gemm_tc_kernel<EPI_SEMCH, PREC>
+                                      : (const void*)gemm_tc_kernel<EPI_GLOBAL, PREC>;
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX);
     if (e != cudaSuccess) return (int)e;
     attr_set[dev & 63][epi] = true;
   }
-  if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN><<<grid, TC_THREADS, smem, st>>>(p, t.map_hi, t.map_lo);
-  else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH><<<grid, TC_THREADS, smem, st>>>(p, t.map_hi, t.map_lo);
-  else gemm_tc_kernel<EPI_GLOBAL><<<grid, TC_THREADS, smem, st>>>(p, t.map_hi, t.map_lo);
+  if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN, PREC><<<grid, TC_THREADS, smem, st>>>(p, t.map_hi, t.map_lo);
+  else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH, PREC><<<grid, TC_THREADS, smem, st>>>(p, t.map_hi, t.map_lo);
+  else gemm_tc_kernel<EPI_GLOBAL, PREC><<<grid, TC_THREADS, smem, st>>>(p, t.map_hi, t.map_lo);
   return (int)cudaGetLastError();
+}
+
+// One CTA per tile, tile = row tile * column tiles + column tile (the column tile fastest, see gemm_tc_kernel).
+// prec: TC_3XTF32 or TC_1XTF32.
+inline int tc_launch(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t, int prec) {
+  return prec == TC_1XTF32 ? tc_launch_prec<TC_1XTF32>(st, epi, p, t) : tc_launch_prec<TC_3XTF32>(st, epi, p, t);
 }
 
 }  // namespace gast

@@ -25,6 +25,34 @@ class GastError(RuntimeError):
     pass
 
 
+_PRECISIONS = {'fp32': 0, 'tf32': 1}
+
+
+def set_precision(module, mode):
+    """Arithmetic of the tensor-core GEMMs of `module` and all of its sub-modules, like torch's `allow_tf32`:
+    'fp32' (default) is fp32-grade (3xTF32, the reference's numbers to ~1e-7 relative); 'tf32' is one TF32 product
+    per multiply-add with fp32 accumulation, faster and about 1e-3 relative off (DESIGN.md §4.1).  'tf32' is for
+    inference: forward under no_grad, run_model_mpjpe, the streams, lift_sequences, tta.evaluate_sequence; a
+    train-mode forward or one that builds an autograd graph raises.  The setting lives in each module's __dict__
+    (DataParallel replicas and deepcopies keep it, state_dict does not).  Returns the module."""
+    if mode not in _PRECISIONS:
+        raise GastError("set_precision: mode must be 'fp32' or 'tf32' (got %r)" % (mode,))
+    for m in module.modules():
+        m.__dict__['_gast_precision'] = mode
+    return module
+
+
+def get_precision(module):
+    """'fp32' or 'tf32' (set_precision)"""
+    return module.__dict__.get('_gast_precision', 'fp32')
+
+
+def _fp32_only(module, what):
+    if get_precision(module) != 'fp32':
+        raise GastError("%s: the model is set to TF32, which is inference-only; call "
+                        "engine.set_precision(model, 'fp32') to train or differentiate it" % what)
+
+
 def _check(rc, what):
     if rc != 0:
         raise GastError('%s: %s' % (what, L.last_error()))
@@ -120,6 +148,7 @@ class _Handle(object):
         self.sig = None
         self.ws = None
         self.core = None
+        self.precision = 0
 
     def __del__(self):
         try:
@@ -129,17 +158,22 @@ class _Handle(object):
         except Exception:
             pass
 
-    def apply_core(self):
-        """hand the set_gemm_core() choice to the library handle (every forward, training or eval)"""
+    def apply_core(self, module):
+        """hand the set_gemm_core() choice and the module's set_precision() to the library handle (every forward,
+        training or eval, and every stream push)"""
         if _FORCE_CORE['core'] != self.core:
             _check(self.lib.gast_set_gemm_core(self.h, _FORCE_CORE['core']), 'gast_set_gemm_core')
             self.core = _FORCE_CORE['core']
+        prec = _PRECISIONS[get_precision(module)]
+        if prec != self.precision:
+            _check(self.lib.gast_set_precision(self.h, prec), 'gast_set_precision')
+            self.precision = prec
 
     def refresh(self, module, stream):
         """(re)bind + prepare when any parameter/buffer moved or changed."""
         items = named_tensors(module)
         sig = tuple((v.data_ptr(), v._version) for _, v in items)
-        self.apply_core()
+        self.apply_core(module)
         if sig == self.sig:
             return
         n = len(items)
@@ -161,7 +195,7 @@ class _Handle(object):
 
     def bind_only(self, module):
         """bind parameter/buffer storage without the eval-mode prepare (training path)"""
-        self.apply_core()
+        self.apply_core(module)
         items = named_tensors(module)
         n = len(items)
         keys = (C.c_char_p * n)()
@@ -393,6 +427,7 @@ def run_model(module, x):
     x = x.contiguous()
     B, T = int(x.shape[0]), int(x.shape[1])
     if module.training:
+        _fp32_only(module, 'SpatioTemporalModel.forward in train mode')
         # both of the reference's training models: Optimized1f (main.py:166-170) and, with
         # --disable-optimizations / stride > 1, the dilated SpatioTemporalModel (main.py:171-175)
         np_ = named_params(module)
@@ -408,6 +443,7 @@ def run_model(module, x):
     np_ = named_params(module) if torch.is_grad_enabled() else []
     if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for _, p in np_)):
         # the reference's output would carry a grad_fn here: same forward, plus a backward
+        _fp32_only(module, 'SpatioTemporalModel.forward with autograd (requires_grad input or parameters)')
         y = _EvalFn.apply(module, h, x, strided_now, [k for k, _ in np_], *[p for _, p in np_])
     else:
         y = _eval_forward(module, h, x, strided_now)
@@ -602,6 +638,7 @@ def profile_forward(module, x, reps=5):
     gemm = sum(v for k, v in per.items() if fam(k))
     ng = sum(v for k, v in n_launch.items() if fam(k))
     tc = int(lib.gast_last_tc_launch_count(h.h))
+    tc_name = 'wgmma-1xtf32' if get_precision(module) == 'tf32' else 'wgmma-3xtf32'
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     with torch.no_grad():
         e0.record()
@@ -610,5 +647,5 @@ def profile_forward(module, x, reps=5):
     torch.cuda.synchronize(dev)
     return {'per_kernel_ms': per, 'launches': n_launch, 'gemm_ms_per_step': gemm, 'gemm_launches': ng,
             'step_ms': e0.elapsed_time(e1), 'workspace_bytes': int(h.ws.numel()) if h.ws is not None else 0,
-            'gemm_core': ('wgmma-3xtf32 x%d + ffma x%d + attention-mix x%d'
-                          % (tc, ng - tc - n_launch.get('global_mix', 0), n_launch.get('global_mix', 0))) if tc else 'ffma-fp32'}
+            'gemm_core': ('%s x%d + ffma x%d + attention-mix x%d'
+                          % (tc_name, tc, ng - tc - n_launch.get('global_mix', 0), n_launch.get('global_mix', 0))) if tc else 'ffma-fp32'}

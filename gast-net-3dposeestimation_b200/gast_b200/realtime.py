@@ -18,8 +18,8 @@ un-augmented restriction that returns the pose of the newest frame.
 The rings hold activations computed with the weights of the pushes that wrote them.  Any change to the model's
 parameters or buffers (`load_state_dict`, an optimiser step, a training forward, which moves the BatchNorm running
 statistics) therefore invalidates the history of every stream: the next push raises `GastError` unless `reset()`
-(every stream) was called after the change.  Switching the GEMM core (`engine.set_gemm_core`) changes no weight and
-keeps the streams.
+(every stream) was called after the change.  Switching the GEMM core (`engine.set_gemm_core`) or the precision
+(`engine.set_precision`, which the streams follow like every forward) changes no weight and keeps the streams.
 
 `WindowStream` is the generic form for any callable network: a device ring of the last `rf` input frames and one
 window forward per pushed frame (what the reference does; used for non-GAST callables and as the cross-check).

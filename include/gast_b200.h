@@ -110,7 +110,7 @@ int gast_forward_mpjpe(gast_t* h, const float* x, const float* target, float* y,
 /* Number of kernels the last gast_forward enqueued (for bench.py's gpu_launches). */
 int32_t gast_last_launch_count(const gast_t* h);
 
-/* Number of those that ran on the tensor-core (wgmma 3xTF32) GEMM core. */
+/* Number of those that ran on the tensor-core (wgmma) GEMM core, in either precision (gast_set_precision). */
 int32_t gast_last_tc_launch_count(const gast_t* h);
 
 /* Per-launch device timing for the roofline report: when on, gast_forward brackets every
@@ -122,8 +122,21 @@ int gast_set_timing(gast_t* h, int32_t on);
 int32_t gast_get_timings(gast_t* h, int32_t max_n, float* ms, int32_t* kinds);
 
 /* GEMM core selection for A/B checks on the GPU: 0 = auto (tensor cores where the shape
- * allows), 1 = force the FP32 FFMA core.  Not a fallback switch: both are CUDA paths. */
+ * allows; 3xTF32 or single-pass TF32 as gast_set_precision says), 1 = force the FP32 FFMA core (fp32 in either
+ * precision).  Not a fallback switch: both are CUDA paths. */
 int gast_set_gemm_core(gast_t* h, int32_t core);
+
+/* Arithmetic of the GEMMs the tensor-core core runs, for every handle kind and for gast_forward,
+ * gast_forward_mpjpe and the gast_stream_push* calls:
+ *   0 = fp32-grade (default): 3xTF32, within ~1e-7 relative of an fp32 GEMM.
+ *   1 = TF32: tf32(A) . tf32(W) with fp32 accumulation, one tensor-core product per multiply-add.  Operands are
+ *       rounded to 10 mantissa bits (round to nearest, ties away), so outputs move by ~1e-3 relative
+ *       (DESIGN.md §4.1).  Inference only: gast_forward_train, gast_backward(_input), gast_eval_backward and their
+ *       workspace queries fail while it is set.
+ * Any other value fails.  Everything else (expand, row-dots, the attention mix, shrink, GEMMs the tensor-core core
+ * does not take, every GEMM under gast_set_gemm_core(h, 1)) stays fp32.  Like a core switch it needs no
+ * gast_prepare, costs nothing and does not invalidate stream `state`. */
+int gast_set_precision(gast_t* h, int32_t mode);
 
 /* ---- test-time augmentation around the forward (the caller-side steps of reconstruction.evaluate /
  * main.evaluate, kept on the device) -----------------------------------------------------------------
@@ -188,7 +201,8 @@ int gast_set_dropout_state(gast_t* h, void* dev_u64);
  *   The rings hold layer inputs computed with the weights of the pushes that wrote them.  A gast_prepare (after
  *   new weights or BatchNorm statistics were bound) therefore invalidates `state`: unless the next push marks
  *   every stream fresh, it mixes old and new weights for up to receptive_field - 1 pushes.  Nothing checks this
- *   here; gast_b200.realtime.CausalStream refuses such a push.  gast_set_gemm_core does not invalidate `state`. */
+ *   here; gast_b200.realtime.CausalStream refuses such a push.  gast_set_gemm_core and gast_set_precision do not
+ *   invalidate `state`. */
 size_t gast_stream_state_bytes(gast_t* h, int32_t n_streams);
 size_t gast_stream_workspace_bytes(gast_t* h, int32_t n_streams);
 int gast_stream_push(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
@@ -281,7 +295,7 @@ int gast_adam_step(const int64_t* table, int32_t n_chunks, float* exp_avg, float
                    double lr, double beta1, double beta2, double eps, double weight_decay, int64_t step, void* stream);
 
 /* Test/probe entry (not on the forward path): out[M,N] = A[M,K] . W[N,K]^T on one GEMM core
- * (core 0 = tensor cores, 3xTF32; 1 = FFMA); tc_mode must be 0.  Runs once, then `reps` timed launches
+ * (core 0 = tensor cores, tc_mode 0 = 3xTF32 or 1 = single-pass TF32; core 1 = FFMA, tc_mode 0).  Runs once, then `reps` timed launches
  * (CUDA events) whose mean duration is written to *ms_out (host).  Synchronises the stream. */
 int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32_t N, int32_t K,
                     int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream);
