@@ -153,6 +153,19 @@ __global__ void stream_chunk_ring_kernel(float4* __restrict__ ring, const float4
   }
 }
 
+// xin (n, k0-1+K, J, F) = the last k0-1 frames of xhist followed by K copies of its newest frame: the input of K held
+// pushes (gast_stream_peek, below).  xhist is only read.  Grid-stride over the elements of xin.
+__global__ void stream_peek_xin_kernel(const float* __restrict__ xhist, float* __restrict__ xin, int n, int k0, int K,
+                                       int JF) {
+  const int T = k0 - 1 + K;
+  const long long total = (long long)n * T * JF;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long f = i / JF;
+    const int e = (int)(i - f * JF), b = (int)(f / T), p = (int)(f - (long long)b * T);
+    xin[i] = xhist[((long long)b * k0 + min(p + 1, k0 - 1)) * JF + e];
+  }
+}
+
 // dst[n][k*Cw + c] = src[n][j*Cw + c],  j = (k - r - 1) mod taps: slot order -> time order of the taps
 __global__ void rotate_taps_kernel(float* __restrict__ dst, const float* __restrict__ src, int N, int Cw, int taps, int r) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -364,35 +377,25 @@ extern "C" size_t gast_stream_chunk_workspace_bytes(gast_t* h, int32_t n_streams
   return a.off + 256;
 }
 
-extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
-                                      int32_t K, const int32_t* fresh, const int32_t* hold, void* workspace,
-                                      size_t workspace_bytes, void* stream) {
-  if (!h) return fail("gast_stream_push_chunk: null handle");
-  if (!h->prepared) return fail("gast_stream_push_chunk: gast_prepare() has not run since the last gast_bind()");
-  if (step < 0 || !state || !x || !y) return fail("gast_stream_push_chunk: bad arguments");
-  StreamPlan sp;
-  if (stream_plan(h, n_streams, &sp)) return 1;
-  {
-    Arena dry{nullptr, 0, 0, true};
-    ChunkBufs cb;
-    if (chunk_bufs(h, sp, K, dry, &cb)) return 1;
-    const size_t need = dry.off + 256;
-    if (!workspace || workspace_bytes < need)
-      return fail("gast_stream_push_chunk: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
-  }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
-  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
-  const gast_cfg& c = h->cfg;
-  const int n = n_streams, J = c.num_joints, L = c.num_stages, k0 = c.filter_widths[0], Fin = c.in_features;
-  const long long F = (long long)n * K;                  // frames of the chunk, in (stream, frame) order
-  float* sbase = reinterpret_cast<float*>(align256(state));
-  Arena a = workspace_arena(workspace, workspace_bytes);
+static int chunk_check_workspace(gast_handle* h, const StreamPlan& sp, int K, const void* workspace,
+                                 size_t workspace_bytes, const char* who) {
+  Arena dry{nullptr, 0, 0, true};
   ChunkBufs cb;
-  if (chunk_bufs(h, sp, K, a, &cb)) return 1;
+  if (chunk_bufs(h, sp, K, dry, &cb)) return 1;
+  const size_t need = dry.off + 256;
+  if (!workspace || workspace_bytes < need)
+    return fail("%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
+  return 0;
+}
+
+// The chunk forward after its input frames are in cb.xin: expand, block 0, the temporal stages on their gathered
+// history (ring write-back when write_rings), shrink into y (n, K, J, 3).
+static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, float* sbase, int64_t step, int K,
+                         const int32_t* fresh, bool write_rings, const ChunkBufs& cb, float* y) {
+  const gast_cfg& c = h->cfg;
+  const int n = sp.n, J = c.num_joints, L = c.num_stages, k0 = c.filter_widths[0];
+  const long long F = (long long)n * K;                  // frames of the chunk, in (stream, frame) order
   const StreamBufs& sb = cb.sb;
-  stream_chunk_xin_kernel<<<n, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K, J * Fin);
-  h->launches++;
   if (launch_expand(h, st, cb.xin, sb.E, F * J, k0 - 1 + K, K, 1)) return 1;
   if (run_block(h, st, h->blocks[0], sb.E, F, sb.bb, sb.fin)) return 1;
   const unsigned grid_cap = (unsigned)h->sm_count * 16;
@@ -400,7 +403,7 @@ extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, cons
     const StageConsts& s = h->stages[i - 1];
     const int Cw = s.Cw, fw = c.filter_widths[i], d = sp.dil[i - 1], R = sp.R[i - 1], H = (fw - 1) * d;
     if (s.taps != fw) return fail("streaming: stage %d has %d taps, expected %d", i - 1, s.taps, fw);
-    if ((J * Cw) % 4) return fail("gast_stream_push_chunk: J*channels of stage %d is not a multiple of 4", i);
+    if ((J * Cw) % 4) return fail("streaming chunk: J*channels of stage %d is not a multiple of 4", i);
     float* ring = sbase + sp.ring_off[i - 1];
     const long long row4 = (long long)J * Cw / 4;
     const long long g4 = (long long)n * (H + K) * row4, r4 = (long long)R * n * row4;
@@ -408,10 +411,12 @@ extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, cons
         reinterpret_cast<float4*>(cb.G), reinterpret_cast<const float4*>(ring),
         reinterpret_cast<const float4*>(sb.fin), fresh, n, R, (int)(step % R), H, K, row4);
     h->launches++;
-    stream_chunk_ring_kernel<<<(unsigned)std::min<long long>(cdiv(r4, 256), grid_cap), 256, 0, st>>>(
-        reinterpret_cast<float4*>(ring), reinterpret_cast<const float4*>(cb.G), fresh, n, R,
-        (int)((step + K - 1) % R), H, K, row4);
-    h->launches++;
+    if (write_rings) {
+      stream_chunk_ring_kernel<<<(unsigned)std::min<long long>(cdiv(r4, 256), grid_cap), 256, 0, st>>>(
+          reinterpret_cast<float4*>(ring), reinterpret_cast<const float4*>(cb.G), fresh, n, R,
+          (int)((step + K - 1) % R), H, K, row4);
+      h->launches++;
+    }
     // output frame (b, t) = time step+t: taps at G positions t, t+d, ..., t+H; residual at the newest tap (causal)
     // or the centre tap t + H - (w/2) d (non-causal), as in the whole-sequence forward
     const ASeg taps = seg_taps(cb.G, Cw, Cw, fw, (long long)d * J * Cw, RowMap{K, H + K, 1, 0});
@@ -423,4 +428,64 @@ extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, cons
   if (launch_shrink(h, st, sb.fin, y, F * J, nullptr, nullptr)) return 1;
   CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
+                                      int32_t K, const int32_t* fresh, const int32_t* hold, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  if (!h) return fail("gast_stream_push_chunk: null handle");
+  if (!h->prepared) return fail("gast_stream_push_chunk: gast_prepare() has not run since the last gast_bind()");
+  if (step < 0 || !state || !x || !y) return fail("gast_stream_push_chunk: bad arguments");
+  StreamPlan sp;
+  if (stream_plan(h, n_streams, &sp)) return 1;
+  if (chunk_check_workspace(h, sp, K, workspace, workspace_bytes, "gast_stream_push_chunk")) return 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CUDA_OK(cudaSetDevice(h->cfg.device));
+  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
+  const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0];
+  float* sbase = reinterpret_cast<float*>(align256(state));
+  Arena a = workspace_arena(workspace, workspace_bytes);
+  ChunkBufs cb;
+  if (chunk_bufs(h, sp, K, a, &cb)) return 1;
+  stream_chunk_xin_kernel<<<n_streams, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K,
+                                                                   J * h->cfg.in_features);
+  h->launches++;
+  return chunk_forward(h, st, sp, sbase, step, K, fresh, true, cb, y);
+}
+
+// ---- peek: the poses K held pushes would return, without pushing ------------------------------------------------
+// gast_stream_peek is gast_stream_push_chunk with fresh = null and every frame held, minus every write to the state:
+// stream_peek_xin_kernel builds the chunk input from the input history without updating it, and the stages gather
+// their ring history but write no slot back.  Row k of stream s is the pose the (k+1)-th held push would return: for a
+// sequence of l pushed frames, the pose of frame l - latency + k with the generator's right padding applied after
+// frame l - 1.
+extern "C" int gast_stream_peek(gast_t* h, const void* state, int64_t step, float* y, int32_t n_streams, int32_t K,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h) return fail("gast_stream_peek: null handle");
+  if (!h->prepared) return fail("gast_stream_peek: gast_prepare() has not run since the last gast_bind()");
+  const int32_t lat = gast_stream_latency(h);
+  if (lat < 0) return 1;
+  if (lat == 0)
+    return fail("gast_stream_peek needs a non-causal model: a causal model returns the pose of the pushed frame, so "
+                "none is ever pending");
+  if (K < 1 || K > lat) return fail("gast_stream_peek: K must be in [1, latency = %d] (got %d)", lat, K);
+  if (step < 1) return fail("gast_stream_peek: step must be at least 1 (the state holds no pushed frame)");
+  if (!state || !y) return fail("gast_stream_peek: bad arguments");
+  StreamPlan sp;
+  if (stream_plan(h, n_streams, &sp)) return 1;
+  if (chunk_check_workspace(h, sp, K, workspace, workspace_bytes, "gast_stream_peek")) return 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CUDA_OK(cudaSetDevice(h->cfg.device));
+  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
+  const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0];
+  // only read: chunk_forward writes no ring back when write_rings is false
+  float* sbase = reinterpret_cast<float*>(align256(const_cast<void*>(state)));
+  Arena a = workspace_arena(workspace, workspace_bytes);
+  ChunkBufs cb;
+  if (chunk_bufs(h, sp, K, a, &cb)) return 1;
+  const long long xe = (long long)n_streams * (k0 - 1 + K) * J * h->cfg.in_features;
+  stream_peek_xin_kernel<<<(unsigned)std::min<long long>(cdiv(xe, 256), (long long)h->sm_count * 16), 256, 0, st>>>(
+      sbase + sp.xhist_off, cb.xin, n_streams, k0, K, J * h->cfg.in_features);
+  h->launches++;
+  return chunk_forward(h, st, sp, sbase, step, K, nullptr, false, cb, y);
 }

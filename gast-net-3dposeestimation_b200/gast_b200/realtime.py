@@ -12,7 +12,9 @@ is pushed (`latency` = pad = (rf - 1) // 2; 0 for a causal model).  `end()` clos
 `latency` pushes repeat the last frame (the generator's right padding) and return the remaining poses.  With
 `augment=True` every push also runs the mirrored twin and averages it back, as every inference helper of the
 reference does (`tools/inference.py:19-110`).  The poses of a sequence then equal
-`UnchunkedGenerator([seq], pad, causal_shift, augment)` + `tools/inference.evaluate`.  `CausalStream` is the causal,
+`UnchunkedGenerator([seq], pad, causal_shift, augment)` + `tools/inference.evaluate`.  Until then `peek()` returns
+provisional poses of the pending frames, those of the sequence cut at its newest frame, without changing any stream.
+`CausalStream` is the causal,
 un-augmented restriction that returns the pose of the newest frame.
 
 The rings hold activations computed with the weights of the pushes that wrote them.  Any change to the model's
@@ -24,6 +26,7 @@ statistics) therefore invalidates the history of every stream: the next push rai
 `WindowStream` is the generic form for any callable network: a device ring of the last `rf` input frames and one
 window forward per pushed frame (what the reference does; used for non-GAST callables and as the cross-check).
 """
+import copy
 import ctypes as C
 import numpy as np
 import torch
@@ -126,6 +129,13 @@ class SequenceBook(object):
         self.left = np.where(live & ~ends, -1, np.maximum(left0 - (K - kh), 0))
         self.fresh[:] = False
         return fresh, hold, index
+
+    def peek(self, K):
+        """-> index (n, K) of a peek of K pushes: what `advance_many(K)` returns after `end()` of every live stream,
+        computed on a copy; this book is unchanged"""
+        book = copy.deepcopy(self)
+        book.end()
+        return book.advance_many(K)[2]
 
 
 class PoseStream(object):
@@ -288,12 +298,7 @@ class PoseStream(object):
         with torch.cuda.device(self.device):
             st = torch.cuda.current_stream(self.device).cuda_stream
             self._begin(h, st)
-            wb = int(lib.gast_stream_chunk_workspace_bytes(h.h, m, K))
-            if wb == 0:
-                raise eng.GastError('gast_stream_chunk_workspace_bytes: %s' % L.last_error())
-            if self._chunk_ws is None or self._chunk_ws.numel() < wb:   # grows with K: serves every smaller K
-                self._chunk_ws = None
-                self._chunk_ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
+            ws = self._chunk_workspace(h, m, K)
             fresh, hold, index = self.book.advance_many(K, valid)
             fresh_p, hold_p = self._upload_chunk(fresh, hold)
             x, out = frames, y
@@ -306,9 +311,8 @@ class PoseStream(object):
                 out = torch.empty((2, self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
             rc = lib.gast_stream_push_chunk(h.h, C.c_void_p(self._state.data_ptr()), C.c_int64(self.step),
                                             C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), m, K,
-                                            C.c_void_p(fresh_p), C.c_void_p(hold_p),
-                                            C.c_void_p(self._chunk_ws.data_ptr()), self._chunk_ws.numel(),
-                                            C.c_void_p(st))
+                                            C.c_void_p(fresh_p), C.c_void_p(hold_p), C.c_void_p(ws.data_ptr()),
+                                            ws.numel(), C.c_void_p(st))
             if rc != 0:
                 raise eng.GastError('gast_stream_push_chunk: %s' % L.last_error())
             launches = int(lib.gast_last_launch_count(h.h))
@@ -321,6 +325,70 @@ class PoseStream(object):
         self.step += K
         self.last_launches = launches
         return y, torch.from_numpy(index)
+
+    def peek(self, K=None):
+        """Provisional poses of the frames a non-causal model has not returned yet, without pushing -> (poses
+        (n, K, J, 3) CUDA, index (n, K) CPU int64): what K more pushes would return if every stream's sequence ended
+        at its newest frame (`end()` and K held pushes), in one library call (gast_stream_peek).  Nothing changes:
+        not the library state, not `step`, not the sequences.  Those poses are the reference's for the sequence cut
+        at its newest frame (UnchunkedGenerator pads it with copies of that frame); the pushes still return the final
+        poses `latency` pushes later.  K defaults to `latency`, 1 <= K <= latency.
+
+        Lookahead: for a stream that pushed frames 0 .. l-1 of its sequence, row k is the pose of frame
+        l - latency + k, so with K = latency the last row is the newest frame.  To show poses L frames behind the
+        newest (0 <= L < latency), peek K = latency - L and take row K - 1: a smaller K costs less.  index[s, k] is
+        the frame's position in stream s's sequence, -1 where nothing is due (ending streams with fewer poses left,
+        idle or freshly reset streams, frames before the sequence's start); when no stream has a pose due the call
+        launches nothing."""
+        eng = self.engine
+        name = type(self).__name__
+        if self.causal:
+            raise eng.GastError('%s.peek needs a non-causal model: a causal model returns the pose of every pushed '
+                                'frame at once, so none is ever pending' % name)
+        K = self.latency if K is None else int(K)
+        if not 1 <= K <= self.latency:
+            raise eng.GastError('%s.peek: K must be in [1, latency = %d] (got %d)' % (name, self.latency, K))
+        if self.model.training:
+            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
+        index = self.book.peek(K)
+        y = torch.empty((self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
+        if not (index >= 0).any():
+            self.last_launches = 0
+            return y, torch.from_numpy(index)
+        h = eng.model_handle(self.model, self.device)
+        lib = h.lib
+        m = self.copies * self.n
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device).cuda_stream
+            self._begin(h, st)
+            ws = self._chunk_workspace(h, m, K)
+            out = y
+            if self.augment:
+                out = torch.empty((2, self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
+            rc = lib.gast_stream_peek(h.h, C.c_void_p(self._state.data_ptr()), C.c_int64(self.step),
+                                      C.c_void_p(out.data_ptr()), m, K, C.c_void_p(ws.data_ptr()), ws.numel(),
+                                      C.c_void_p(st))
+            if rc != 0:
+                raise eng.GastError('gast_stream_peek: %s' % L.last_error())
+            launches = int(lib.gast_last_launch_count(h.h))
+            if self.augment:
+                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(y.data_ptr()), self.n * K, self.J,
+                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
+                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
+                launches += 2
+        self.last_launches = launches
+        return y, torch.from_numpy(index)
+
+    def _chunk_workspace(self, h, m, K):
+        """the workspace of a chunk (or peek) of K frames over m library streams; grows with K and serves every
+        smaller K"""
+        wb = int(h.lib.gast_stream_chunk_workspace_bytes(h.h, m, K))
+        if wb == 0:
+            raise self.engine.GastError('gast_stream_chunk_workspace_bytes: %s' % L.last_error())
+        if self._chunk_ws is None or self._chunk_ws.numel() < wb:
+            self._chunk_ws = None
+            self._chunk_ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
+        return self._chunk_ws
 
     def _upload_chunk(self, fresh, hold):
         """-> device pointers of the fresh (n) and hold (n, K) masks of a chunk, repeated for the mirrored half

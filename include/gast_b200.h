@@ -246,6 +246,22 @@ size_t gast_stream_chunk_workspace_bytes(gast_t* h, int32_t n_streams, int32_t K
 int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
                            int32_t K, const int32_t* fresh, const int32_t* hold, void* workspace,
                            size_t workspace_bytes, void* stream);
+/* gast_stream_peek: provisional poses of the frames a non-causal stream has not returned yet, without pushing.
+ *   y (n_streams, K, J, 3) is what K calls of gast_stream_push_ex at steps step, step+1, ..., step+K-1 would return
+ *   with fresh = NULL and hold[s] = 1 for every stream; `state` is not modified (byte for byte), and step does not
+ *   advance.  So, for a stream that pushed frames 0 .. l-1 of its current sequence, row k is the pose of frame
+ *   l - latency + k as the reference computes it for the sequence cut at frame l - 1 (UnchunkedGenerator's right
+ *   padding by copies of the newest frame).  The final poses still come from the pushes, latency pushes later.
+ *   Lookahead: for poses L frames behind the newest (0 <= L < latency) peek K = latency - L and take row K-1; with
+ *   K = latency the last row is the newest frame.
+ *   1 <= K <= gast_stream_latency(h) (so a causal handle, whose latency is 0, is refused) and step >= 1.  Same
+ *   handles, state and weight-change rule as gast_stream_push_chunk; the workspace is
+ *   gast_stream_chunk_workspace_bytes(h, n_streams, K) bytes.  The cost is that of a chunk of K frames; the launch
+ *   count does not depend on n_streams or K.
+ *   Test-time augmentation: peek the 2n-stream state (no gast_tta_prepare: a peek has no new input), then
+ *   gast_tta_merge(y2, y, n * K, J, ...) with y2 (2, n, K, J, 3). */
+int gast_stream_peek(gast_t* h, const void* state, int64_t step, float* y, int32_t n_streams, int32_t K,
+                     void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- either side of the forward, on the device (SURVEY.md 8f N1-N3) --------------------------------
  * All pointers are device pointers unless marked (host).  Work is enqueued on `stream`.
