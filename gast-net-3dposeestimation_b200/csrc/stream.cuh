@@ -79,15 +79,17 @@ constexpr int CHUNK_XIN_THREADS = 256;
 // last k0 frames of xin.  One block per stream.  hold (n, K) or null: a held frame (not fresh frame 0) repeats the
 // stream's newest frame, which may be an earlier held frame of the chunk, so frame k takes x[b, src[k]] with src[k] the
 // latest frame <= k that is not held (a block-wide max scan), or the newest frame of xhist when there is none.  A fresh
-// stream's history is copies of its frame 0.  x rows of held frames are never read.
+// stream's history is copies of its frame 0.  x rows of held frames are never read.  sidx (m) or null: row b of x / xin
+// / fresh / hold belongs to state stream sidx[b] (a subset push, gast_stream_push_subset); null = stream b.
 __global__ void __launch_bounds__(CHUNK_XIN_THREADS)
 stream_chunk_xin_kernel(float* __restrict__ xhist, const float* __restrict__ x, float* __restrict__ xin,
-                        const int32_t* __restrict__ fresh, const int32_t* __restrict__ hold, int k0, int K, int JF) {
+                        const int32_t* __restrict__ fresh, const int32_t* __restrict__ hold, int k0, int K, int JF,
+                        const int32_t* __restrict__ sidx) {
   __shared__ int src[CHUNK_XIN_THREADS];
   __shared__ int wmax[CHUNK_XIN_THREADS / 32];
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool is_fresh = fresh && fresh[b];
-  float* hrow = xhist + (long long)b * k0 * JF;
+  float* hrow = xhist + (long long)(sidx ? sidx[b] : b) * k0 * JF;
   float* irow = xin + (long long)b * (k0 - 1 + K) * JF;
   const float* xrow = x + (long long)b * K * JF;
   const int32_t* hb = hold ? hold + (long long)b * K : nullptr;
@@ -119,20 +121,26 @@ stream_chunk_xin_kernel(float* __restrict__ xhist, const float* __restrict__ x, 
   for (int e = tid; e < k0 * JF; e += CHUNK_XIN_THREADS) hrow[e] = irow[(long long)(K - 1) * JF + e];
 }
 
-// G (n, H+K, rowlen) = stage input at times step-H .. step+K-1: the head (positions p < H) from the ring slots
-// (step - H + p) mod R, the tail (p >= H) from the previous block's K outputs tail (n, K, rowlen).  A fresh stream's head
-// is copies of its tail position 0 (its history is constant, as stream_fill_fresh_kernel makes it).  hs = step mod R.
+// G (m, H+K, rowlen) = stage input at times step-H .. step+K-1: the head (positions p < H) from the ring slots
+// (step - H + p) mod R, the tail (p >= H) from the previous block's K outputs tail (m, K, rowlen).  A fresh stream's head
+// is copies of its tail position 0 (its history is constant, as stream_fill_fresh_kernel makes it).  The ring holds n
+// streams per slot.  tab null: m = n, row b is stream b and hs = step mod R for all; else row b is state stream tab[b]
+// at its own phase tab[m + b] (its step mod R_max, which R divides) and hs is unused.
 __global__ void stream_chunk_gather_kernel(float4* __restrict__ G, const float4* __restrict__ ring,
-                                           const float4* __restrict__ tail, const int32_t* __restrict__ fresh, int n,
-                                           int R, int hs, int H, int K, long long row4) {
-  const long long total = (long long)n * (H + K) * row4;
+                                           const float4* __restrict__ tail, const int32_t* __restrict__ fresh, int m,
+                                           int n, int R, int hs, int H, int K, long long row4,
+                                           const int32_t* __restrict__ tab) {
+  const long long total = (long long)m * (H + K) * row4;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long q = i % row4, f = i / row4;
     const int b = (int)(f / (H + K)), p = (int)(f - (long long)b * (H + K));
     float4 v;
     if (p >= H) v = tail[((long long)b * K + (p - H)) * row4 + q];
     else if (fresh && fresh[b]) v = tail[(long long)b * K * row4 + q];
-    else v = ring[((long long)((hs - H + p + R) % R) * n + b) * row4 + q];
+    else {
+      const int sb = tab ? tab[b] : b, h = tab ? tab[m + b] % R : hs;
+      v = ring[((long long)((h - H + p + R) % R) * n + sb) * row4 + q];
+    }
     G[i] = v;
   }
 }
@@ -140,29 +148,33 @@ __global__ void stream_chunk_gather_kernel(float4* __restrict__ G, const float4*
 // Ring write-back after a chunk: slot p gets the stage input at the latest time t <= step+K-1 with t = p (mod R), from
 // the tail of G when t falls in the chunk, copies of tail position 0 for a fresh stream, else the slot keeps its value.
 // ek = (step + K - 1) mod R.  Launched after stream_chunk_gather_kernel, which reads slots this kernel overwrites.
+// Grid over the R*m rows (slot, listed stream); tab as in stream_chunk_gather_kernel (null: m = n, ek for all; else
+// ek = (tab[m + b] + K - 1) mod R per stream and slot p of stream tab[b] is written).
 __global__ void stream_chunk_ring_kernel(float4* __restrict__ ring, const float4* __restrict__ G,
-                                         const int32_t* __restrict__ fresh, int n, int R, int ek, int H, int K,
-                                         long long row4) {
-  const long long total = (long long)R * n * row4;
+                                         const int32_t* __restrict__ fresh, int m, int n, int R, int ek, int H, int K,
+                                         long long row4, const int32_t* __restrict__ tab) {
+  const long long total = (long long)R * m * row4;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long q = i % row4, f = i / row4;
-    const int p = (int)(f / n), b = (int)(f - (long long)p * n);
-    const int k = K - 1 - (ek - p + R) % R;               // chunk position of time t
+    const int p = (int)(f / m), b = (int)(f - (long long)p * m);
+    const int e = tab ? (int)(((long long)tab[m + b] + K - 1) % R) : ek;
+    const int k = K - 1 - (e - p + R) % R;                // chunk position of time t
     if (k < 0 && !(fresh && fresh[b])) continue;
-    ring[i] = G[((long long)b * (H + K) + H + max(k, 0)) * row4 + q];
+    ring[tab ? ((long long)p * n + tab[b]) * row4 + q : i] = G[((long long)b * (H + K) + H + max(k, 0)) * row4 + q];
   }
 }
 
 // xin (n, k0-1+K, J, F) = the last k0-1 frames of xhist followed by K copies of its newest frame: the input of K held
-// pushes (gast_stream_peek, below).  xhist is only read.  Grid-stride over the elements of xin.
-__global__ void stream_peek_xin_kernel(const float* __restrict__ xhist, float* __restrict__ xin, int n, int k0, int K,
-                                       int JF) {
+// pushes (gast_stream_peek, below).  xhist is only read.  Grid-stride over the elements of xin.  sidx (m) or null: row b
+// of xin is state stream sidx[b] (gast_stream_peek_subset); null = stream b.
+__global__ void stream_peek_xin_kernel(const float* __restrict__ xhist, float* __restrict__ xin, int m, int k0, int K,
+                                       int JF, const int32_t* __restrict__ sidx) {
   const int T = k0 - 1 + K;
-  const long long total = (long long)n * T * JF;
+  const long long total = (long long)m * T * JF;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long f = i / JF;
     const int e = (int)(i - f * JF), b = (int)(f / T), p = (int)(f - (long long)b * T);
-    xin[i] = xhist[((long long)b * k0 + min(p + 1, k0 - 1)) * JF + e];
+    xin[i] = xhist[((long long)(sidx ? sidx[b] : b) * k0 + min(p + 1, k0 - 1)) * JF + e];
   }
 }
 
@@ -389,12 +401,14 @@ static int chunk_check_workspace(gast_handle* h, const StreamPlan& sp, int K, co
 }
 
 // The chunk forward after its input frames are in cb.xin: expand, block 0, the temporal stages on their gathered
-// history (ring write-back when write_rings), shrink into y (n, K, J, 3).
-static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, float* sbase, int64_t step, int K,
-                         const int32_t* fresh, bool write_rings, const ChunkBufs& cb, float* y) {
+// history (ring write-back when write_rings), shrink into y (m, K, J, 3).  tab null: all m = sp.n streams at `step`;
+// else the device table of a subset call (stream_chunk_gather_kernel): m listed streams, each at its own phase.
+static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, float* sbase, int64_t step, int m,
+                         int K, const int32_t* fresh, bool write_rings, const ChunkBufs& cb, float* y,
+                         const int32_t* tab) {
   const gast_cfg& c = h->cfg;
   const int n = sp.n, J = c.num_joints, L = c.num_stages, k0 = c.filter_widths[0];
-  const long long F = (long long)n * K;                  // frames of the chunk, in (stream, frame) order
+  const long long F = (long long)m * K;                  // frames of the chunk, in (stream, frame) order
   const StreamBufs& sb = cb.sb;
   if (launch_expand(h, st, cb.xin, sb.E, F * J, k0 - 1 + K, K, 1)) return 1;
   if (run_block(h, st, h->blocks[0], sb.E, F, sb.bb, sb.fin)) return 1;
@@ -406,15 +420,15 @@ static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, 
     if ((J * Cw) % 4) return fail("streaming chunk: J*channels of stage %d is not a multiple of 4", i);
     float* ring = sbase + sp.ring_off[i - 1];
     const long long row4 = (long long)J * Cw / 4;
-    const long long g4 = (long long)n * (H + K) * row4, r4 = (long long)R * n * row4;
+    const long long g4 = (long long)m * (H + K) * row4, r4 = (long long)R * m * row4;
     stream_chunk_gather_kernel<<<(unsigned)std::min<long long>(cdiv(g4, 256), grid_cap), 256, 0, st>>>(
         reinterpret_cast<float4*>(cb.G), reinterpret_cast<const float4*>(ring),
-        reinterpret_cast<const float4*>(sb.fin), fresh, n, R, (int)(step % R), H, K, row4);
+        reinterpret_cast<const float4*>(sb.fin), fresh, m, n, R, (int)(step % R), H, K, row4, tab);
     h->launches++;
     if (write_rings) {
       stream_chunk_ring_kernel<<<(unsigned)std::min<long long>(cdiv(r4, 256), grid_cap), 256, 0, st>>>(
-          reinterpret_cast<float4*>(ring), reinterpret_cast<const float4*>(cb.G), fresh, n, R,
-          (int)((step + K - 1) % R), H, K, row4);
+          reinterpret_cast<float4*>(ring), reinterpret_cast<const float4*>(cb.G), fresh, m, n, R,
+          (int)((step + K - 1) % R), H, K, row4, tab);
       h->launches++;
     }
     // output frame (b, t) = time step+t: taps at G positions t, t+d, ..., t+H; residual at the newest tap (causal)
@@ -448,9 +462,9 @@ extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, cons
   ChunkBufs cb;
   if (chunk_bufs(h, sp, K, a, &cb)) return 1;
   stream_chunk_xin_kernel<<<n_streams, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K,
-                                                                   J * h->cfg.in_features);
+                                                                   J * h->cfg.in_features, nullptr);
   h->launches++;
-  return chunk_forward(h, st, sp, sbase, step, K, fresh, true, cb, y);
+  return chunk_forward(h, st, sp, sbase, step, n_streams, K, fresh, true, cb, y, nullptr);
 }
 
 // ---- peek: the poses K held pushes would return, without pushing ------------------------------------------------
@@ -485,7 +499,126 @@ extern "C" int gast_stream_peek(gast_t* h, const void* state, int64_t step, floa
   if (chunk_bufs(h, sp, K, a, &cb)) return 1;
   const long long xe = (long long)n_streams * (k0 - 1 + K) * J * h->cfg.in_features;
   stream_peek_xin_kernel<<<(unsigned)std::min<long long>(cdiv(xe, 256), (long long)h->sm_count * 16), 256, 0, st>>>(
-      sbase + sp.xhist_off, cb.xin, n_streams, k0, K, J * h->cfg.in_features);
+      sbase + sp.xhist_off, cb.xin, n_streams, k0, K, J * h->cfg.in_features, nullptr);
   h->launches++;
-  return chunk_forward(h, st, sp, sbase, step, K, nullptr, false, cb, y);
+  return chunk_forward(h, st, sp, sbase, step, n_streams, K, nullptr, false, cb, y, nullptr);
+}
+
+// ---- any subset of the streams, each at its own frame count -------------------------------------------------------
+// A subset call runs the chunk (or peek) forward over the m listed streams only: the four copy kernels read and write
+// the state rows of stream streams[i] at that stream's own ring phase, and everything between them (expand, blocks,
+// stages on the time-ordered weights Wt, shrink) works on the m*K gathered frames as for a chunk.  Every ring size R_i
+// divides the largest one, R_max = w_0 w_1 ... w_{L-1} (R_i = w_i d_i and d_{i+1} = R_i), so one phase per stream,
+// steps[i] mod R_max, gives its slot in every ring.  The (stream, phase) table goes to the workspace in one copy.
+static int subset_bufs(const gast_handle* h, int m, int K, Arena& a, ChunkBufs* cb, int32_t** tab) {
+  StreamPlan spm;                                          // the chunk buffers of m streams
+  if (stream_plan(h, m, &spm) || chunk_bufs(h, spm, K, a, cb)) return 1;
+  *tab = reinterpret_cast<int32_t*>(a.take((size_t)2 * m));
+  return 0;
+}
+
+extern "C" size_t gast_stream_subset_workspace_bytes(gast_t* h, int32_t m, int32_t K) {
+  if (!h || m < 1) return 0;
+  Arena a{nullptr, 0, 0, true};
+  ChunkBufs cb;
+  int32_t* tab;
+  if (subset_bufs(h, m, K, a, &cb, &tab)) return 0;
+  return a.off + 256;
+}
+
+// Host-side checks of a subset call and its table: {streams[i]} then {steps[i] mod R_max}.  *lockstep = the call lists
+// every stream in order at one step (the chunk path's own call, no table needed).
+static int subset_table(const StreamPlan& sp, const int32_t* streams, const int64_t* steps,
+                        int m, int64_t min_step, const char* who, std::vector<int32_t>* tab, bool* lockstep) {
+  const int n = sp.n;
+  if (!streams || !steps) return fail("%s: null streams or steps", who);
+  if (m < 1 || m > n) return fail("%s: m must be in [1, n_streams = %d] (got %d)", who, n, m);
+  const int64_t Rmax = sp.R.empty() ? 1 : sp.R.back();
+  std::vector<char> seen(n, 0);
+  tab->resize((size_t)2 * m);
+  *lockstep = m == n;
+  for (int i = 0; i < m; ++i) {
+    const int32_t s = streams[i];
+    if (s < 0 || s >= n) return fail("%s: streams[%d] = %d is outside [0, %d)", who, i, s, n);
+    if (seen[s]) return fail("%s: stream %d is listed twice", who, s);
+    seen[s] = 1;
+    if (steps[i] < min_step) return fail("%s: steps[%d] = %lld must be at least %lld", who, i, (long long)steps[i],
+                                         (long long)min_step);
+    (*tab)[i] = s;
+    (*tab)[m + i] = (int32_t)(steps[i] % Rmax);
+    *lockstep = *lockstep && s == i && steps[i] == steps[0];
+  }
+  return 0;
+}
+
+extern "C" int gast_stream_push_subset(gast_t* h, void* state, int32_t n_streams, const int32_t* streams,
+                                       const int64_t* steps, int32_t m, int32_t K, const float* x, float* y,
+                                       const int32_t* fresh, const int32_t* hold, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  const char* who = "gast_stream_push_subset";
+  if (!h) return fail("%s: null handle", who);
+  if (!h->prepared) return fail("%s: gast_prepare() has not run since the last gast_bind()", who);
+  if (!state || !x || !y) return fail("%s: bad arguments", who);
+  StreamPlan sp;
+  if (stream_plan(h, n_streams, &sp)) return 1;
+  std::vector<int32_t> tab;
+  bool lockstep;
+  if (subset_table(sp, streams, steps, m, 0, who, &tab, &lockstep)) return 1;
+  const size_t need = gast_stream_subset_workspace_bytes(h, m, K);
+  if (need == 0) return 1;
+  if (!workspace || workspace_bytes < need) return fail("%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CUDA_OK(cudaSetDevice(h->cfg.device));
+  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
+  const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0];
+  float* sbase = reinterpret_cast<float*>(align256(state));
+  Arena a = workspace_arena(workspace, workspace_bytes);
+  ChunkBufs cb;
+  int32_t* dtab;
+  if (subset_bufs(h, m, K, a, &cb, &dtab)) return 1;
+  if (lockstep) dtab = nullptr;
+  else CUDA_OK(cudaMemcpyAsync(dtab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  stream_chunk_xin_kernel<<<m, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K,
+                                                           J * h->cfg.in_features, dtab);
+  h->launches++;
+  return chunk_forward(h, st, sp, sbase, steps[0], m, K, fresh, true, cb, y, dtab);
+}
+
+extern "C" int gast_stream_peek_subset(gast_t* h, const void* state, int32_t n_streams, const int32_t* streams,
+                                       const int64_t* steps, int32_t m, int32_t K, float* y, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  const char* who = "gast_stream_peek_subset";
+  if (!h) return fail("%s: null handle", who);
+  if (!h->prepared) return fail("%s: gast_prepare() has not run since the last gast_bind()", who);
+  const int32_t lat = gast_stream_latency(h);
+  if (lat < 0) return 1;
+  if (lat == 0)
+    return fail("%s needs a non-causal model: a causal model returns the pose of the pushed frame, so none is ever "
+                "pending", who);
+  if (K < 1 || K > lat) return fail("%s: K must be in [1, latency = %d] (got %d)", who, lat, K);
+  if (!state || !y) return fail("%s: bad arguments", who);
+  StreamPlan sp;
+  if (stream_plan(h, n_streams, &sp)) return 1;
+  std::vector<int32_t> tab;
+  bool lockstep;
+  if (subset_table(sp, streams, steps, m, 1, who, &tab, &lockstep)) return 1;
+  const size_t need = gast_stream_subset_workspace_bytes(h, m, K);
+  if (need == 0) return 1;
+  if (!workspace || workspace_bytes < need) return fail("%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CUDA_OK(cudaSetDevice(h->cfg.device));
+  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
+  const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0];
+  float* sbase = reinterpret_cast<float*>(align256(const_cast<void*>(state)));   // only read (write_rings = false)
+  Arena a = workspace_arena(workspace, workspace_bytes);
+  ChunkBufs cb;
+  int32_t* dtab;
+  if (subset_bufs(h, m, K, a, &cb, &dtab)) return 1;
+  if (lockstep) dtab = nullptr;
+  else CUDA_OK(cudaMemcpyAsync(dtab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  const long long xe = (long long)m * (k0 - 1 + K) * J * h->cfg.in_features;
+  stream_peek_xin_kernel<<<(unsigned)std::min<long long>(cdiv(xe, 256), (long long)h->sm_count * 16), 256, 0, st>>>(
+      sbase + sp.xhist_off, cb.xin, m, k0, K, J * h->cfg.in_features, dtab);
+  h->launches++;
+  return chunk_forward(h, st, sp, sbase, steps[0], m, K, nullptr, false, cb, y, dtab);
 }

@@ -22,7 +22,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_eval_backward_workspace_bytes', 'gast_eval_backward', 'gast_set_dropout_state', 'gast_tta_prepare', 'gast_tta_merge',
            'gast_stream_state_bytes', 'gast_stream_workspace_bytes', 'gast_stream_push',
            'gast_stream_latency', 'gast_stream_push_ex', 'gast_stream_chunk_workspace_bytes', 'gast_stream_push_chunk',
-           'gast_stream_peek', 'gast_chunk_gather', 'gast_keypoints_convert', 'gast_normalize_screen', 'gast_camera_to_world',
+           'gast_stream_peek', 'gast_stream_subset_workspace_bytes', 'gast_stream_push_subset', 'gast_stream_peek_subset',
+           'gast_chunk_gather', 'gast_keypoints_convert', 'gast_normalize_screen', 'gast_camera_to_world',
            'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_adam_chunk', 'gast_adam_step',
            'gast_last_error', 'gast_version']
 
@@ -118,6 +119,13 @@ def load():
     lib.gast_stream_push_chunk.restype = C.c_int
     lib.gast_stream_peek.argtypes = [vp, vp, C.c_int64, vp, C.c_int32, C.c_int32, vp, C.c_size_t, vp]
     lib.gast_stream_peek.restype = C.c_int
+    lib.gast_stream_subset_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32]
+    lib.gast_stream_subset_workspace_bytes.restype = C.c_size_t
+    lib.gast_stream_push_subset.argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp,
+                                            C.c_size_t, vp]
+    lib.gast_stream_push_subset.restype = C.c_int
+    lib.gast_stream_peek_subset.argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, C.c_int32, vp, vp, C.c_size_t, vp]
+    lib.gast_stream_peek_subset.restype = C.c_int
     lib.gast_stream_latency.argtypes = [vp]
     lib.gast_stream_latency.restype = C.c_int32
     ip = C.POINTER(C.c_int32)

@@ -47,7 +47,8 @@ class SequenceBook(object):
     A stream is LIVE (its pushes append frames to its current sequence), ENDING (`end` was called: its next pushes
     are held and return the sequence's last poses) or IDLE (held, nothing due).  `advance()` is called once per push
     and returns the fresh and hold masks of that push and, per stream, the position within the current sequence of
-    the frame whose pose that push returns (-1 where nothing is due)."""
+    the frame whose pose that push returns (-1 where nothing is due).  With `streams` (distinct indices), `advance`,
+    `advance_many` and `peek` act on those streams only, in that order, as a book of those streams alone would."""
 
     def __init__(self, n, latency):
         self.n, self.latency = int(n), int(latency)
@@ -59,6 +60,25 @@ class SequenceBook(object):
         if streams is None:
             return slice(None)
         return np.asarray(streams, dtype=np.int64).reshape(-1)
+
+    def check_streams(self, streams):
+        """-> streams as an int64 array; ValueError unless they are 1 to n distinct indices in [0, n)"""
+        s = np.asarray(streams).reshape(-1)
+        if s.size and not np.issubdtype(s.dtype, np.integer):
+            raise ValueError('streams must be integer stream indices (got %s)' % s.dtype)
+        s = s.astype(np.int64)
+        if s.size < 1 or (s < 0).any() or (s >= self.n).any() or np.unique(s).size != s.size:
+            raise ValueError('streams must be 1 to %d distinct indices in [0, %d) (got %s)' % (self.n, self.n, s.tolist()))
+        return s
+
+    def _subset(self, streams, fn):
+        """fn(book of the listed streams alone), then its state written back to those streams"""
+        s = self.check_streams(streams)
+        sub = copy.copy(self)
+        sub.n, sub.fresh, sub.length, sub.left = s.size, self.fresh[s], self.length[s], self.left[s]
+        out = fn(sub)
+        self.fresh[s], self.length[s], self.left[s] = sub.fresh, sub.length, sub.left
+        return out
 
     def reset(self, streams=None):
         s = self._sel(streams)
@@ -78,8 +98,10 @@ class SequenceBook(object):
         """every stream either starts anew at the next push or is idle (its history is never read again)"""
         return bool(np.all(self.fresh | (self.left == 0)))
 
-    def advance(self):
+    def advance(self, streams=None):
         """-> (fresh, hold, index) of the next push; updates the state as that push does"""
+        if streams is not None:
+            return self._subset(streams, lambda b: b.advance())
         fresh = self.fresh.copy()
         self.length[fresh] = 0
         self.left[fresh] = -1
@@ -96,10 +118,12 @@ class SequenceBook(object):
         self.fresh[:] = False
         return fresh, hold, index
 
-    def advance_many(self, K, valid=None):
+    def advance_many(self, K, valid=None, streams=None):
         """-> (fresh (n,), hold (n, K), index (n, K)) of K consecutive pushes, as K calls of `advance()` return them,
         with `end([s])` before push valid[s] of every live stream s whose valid[s] < K (0 <= valid[s] <= K; None:
         no end).  Vectorised over the pushes: every stream is live up to its end and held from then on."""
+        if streams is not None:
+            return self._subset(streams, lambda b: b.advance_many(K, valid))
         K = int(K)
         if K < 1:
             raise ValueError('advance_many: K must be at least 1 (got %d)' % K)
@@ -130,9 +154,11 @@ class SequenceBook(object):
         self.fresh[:] = False
         return fresh, hold, index
 
-    def peek(self, K):
+    def peek(self, K, streams=None):
         """-> index (n, K) of a peek of K pushes: what `advance_many(K)` returns after `end()` of every live stream,
         computed on a copy; this book is unchanged"""
+        if streams is not None:
+            return copy.deepcopy(self)._subset(streams, lambda b: b.peek(K))
         book = copy.deepcopy(self)
         book.end()
         return book.advance_many(K)[2]
@@ -144,7 +170,13 @@ class PoseStream(object):
 
     push(frame (n, J, F)) -> (poses (n, J, 3) CUDA, index (n,) CPU int64): poses[s] is the pose of frame index[s] of
     stream s's current sequence, or unspecified where index[s] == -1.  The kps/joints lists default to the
-    reference's for J = 17 and J = 19; `augment=True` with another J needs all four."""
+    reference's for J = 17 and J = 19; `augment=True` with another J needs all four.
+
+    `push`, `push_frames` and `peek` take `streams`, a list of distinct stream indices: only those streams take part
+    (their rows come in and go out in that order), the others sit the call out untouched.  Each stream then has its
+    own frame count (`counts`); `step` is the smallest of them.  Calls without `streams` while every count is equal
+    use the lockstep library entries (gast_stream_push_ex / _push_chunk / _peek at `step`), all others the subset
+    entries (gast_stream_push_subset / _peek_subset), whose cost follows the listed streams, not n_streams."""
 
     def __init__(self, model_pos, n_streams, augment=False, kps_left=None, kps_right=None, joints_left=None,
                  joints_right=None, device=None):
@@ -185,12 +217,37 @@ class PoseStream(object):
         self.copies = 2 if self.augment else 1      # streams the library runs: [original | mirrored]
         self.book = SequenceBook(self.n, self.latency)
         self.step = 0
+        self._delta = np.zeros(self.n, dtype=np.int64)   # counts - step (>= 0; all 0 while the streams are in step)
         self._masks = torch.zeros((2, self.copies * self.n), dtype=torch.int32, device=self.device)
         self._sig = None                 # the handle's parameter signature at the last push
         self._state = None
         self._ws = None
         self._chunk_ws = None            # push_frames: workspace of the largest K so far
         self._chunk_masks = None
+        self._subset_ws = None           # subset calls: workspace of the largest (streams, K) so far
+
+    @property
+    def counts(self):
+        """(n,) int64: the frames pushed into each stream so far (held frames included)"""
+        return self.step + self._delta
+
+    def _select(self, streams):
+        """-> None for a lockstep call, else the int64 stream indices of a subset call (every stream, in order, for
+        streams=None once the counts differ)"""
+        if streams is None:
+            return np.arange(self.n, dtype=np.int64) if self._delta.any() else None
+        try:
+            return self.book.check_streams(streams)
+        except ValueError as e:
+            raise self.engine.GastError('%s: %s' % (type(self).__name__, e))
+
+    def _advanced(self, sel, K):
+        """the listed streams pushed K frames: counts[sel] += K, with `step` kept at the smallest count"""
+        delta = self._delta.copy()
+        delta[sel] += K
+        low = int(delta.min())
+        self.step += low
+        self._delta = delta - low
 
     def reset(self, streams=None):
         """Start new sequences on all (or the listed) streams with the next pushed frame; drop any pending tail."""
@@ -231,12 +288,19 @@ class PoseStream(object):
             self._state = torch.empty(int(nb), dtype=torch.uint8, device=self.device)
             self._ws = torch.empty(int(wb), dtype=torch.uint8, device=self.device)
 
-    def push(self, frame):
+    def push(self, frame, streams=None):
         """frame (n_streams, J, in_features): the newest 2D keypoints of every stream (normalised screen
-        coordinates; rows of held streams are ignored) -> (poses (n, J, 3), index (n,) CPU int64)."""
+        coordinates; rows of held streams are ignored) -> (poses (n, J, 3), index (n,) CPU int64).  With `streams`
+        (m distinct indices): frame (m, J, F) -> (poses (m, J, 3), index (m,)) of those streams, in that order;
+        the other streams are unchanged."""
         eng = self.engine
         name = type(self).__name__
         frame = torch.as_tensor(frame, dtype=torch.float32, device=self.device).contiguous()
+        sel = self._select(streams)
+        if sel is not None:
+            assert frame.shape == (sel.size, self.J, self.F), frame.shape
+            y, index = self._push_subset(frame[:, None], None, sel)
+            return y[:, 0], index[:, 0]
         assert frame.shape == (self.n, self.J, self.F), frame.shape
         if self.model.training:
             raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
@@ -273,16 +337,23 @@ class PoseStream(object):
         self.last_launches = launches
         return y, torch.from_numpy(index)
 
-    def push_frames(self, frames, valid=None):
+    def push_frames(self, frames, valid=None, streams=None):
         """frames (n_streams, K, J, in_features): the next K frames of every stream -> (poses (n, K, J, 3) CUDA,
         index (n, K) CPU int64), what K calls of `push` with frames[:, k] return, in one library call
         (gast_stream_push_chunk).  valid (n,) or None: only the first valid[s] frames of stream s belong to its
         sequence; a smaller value than K ends the sequence there (as `end([s])` before frame valid[s] would) and the
         rest of the chunk returns its tail.  Rows of held frames are ignored.  `reset()` / `end()` take effect at
-        frame 0 of the call, as for `push`."""
+        frame 0 of the call, as for `push`.  With `streams` (m distinct indices) frames, valid, poses and index have m
+        rows, those streams' in that order, and only those streams advance (gast_stream_push_subset).  A stream's
+        flush is `push_frames(nan frames (1, latency, J, F), valid=[0], streams=[s])`."""
         eng = self.engine
         name = type(self).__name__
         frames = torch.as_tensor(frames, dtype=torch.float32, device=self.device).contiguous()
+        sel = self._select(streams)
+        if sel is not None:
+            assert frames.dim() == 4 and frames.shape[0] == sel.size and frames.shape[1] >= 1 and \
+                tuple(frames.shape[2:]) == (self.J, self.F), frames.shape
+            return self._push_subset(frames, valid, sel)
         assert frames.dim() == 4 and frames.shape[0] == self.n and frames.shape[1] >= 1 and \
             tuple(frames.shape[2:]) == (self.J, self.F), frames.shape
         K = int(frames.shape[1])
@@ -326,7 +397,7 @@ class PoseStream(object):
         self.last_launches = launches
         return y, torch.from_numpy(index)
 
-    def peek(self, K=None):
+    def peek(self, K=None, streams=None):
         """Provisional poses of the frames a non-causal model has not returned yet, without pushing -> (poses
         (n, K, J, 3) CUDA, index (n, K) CPU int64): what K more pushes would return if every stream's sequence ended
         at its newest frame (`end()` and K held pushes), in one library call (gast_stream_peek).  Nothing changes:
@@ -339,7 +410,8 @@ class PoseStream(object):
         newest (0 <= L < latency), peek K = latency - L and take row K - 1: a smaller K costs less.  index[s, k] is
         the frame's position in stream s's sequence, -1 where nothing is due (ending streams with fewer poses left,
         idle or freshly reset streams, frames before the sequence's start); when no stream has a pose due the call
-        launches nothing."""
+        launches nothing.  With `streams` (m distinct indices) poses and index have m rows, those streams' in that
+        order, each stream peeked at its own frame count (gast_stream_peek_subset)."""
         eng = self.engine
         name = type(self).__name__
         if self.causal:
@@ -350,6 +422,9 @@ class PoseStream(object):
             raise eng.GastError('%s.peek: K must be in [1, latency = %d] (got %d)' % (name, self.latency, K))
         if self.model.training:
             raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
+        sel = self._select(streams)
+        if sel is not None:
+            return self._peek_subset(K, sel)
         index = self.book.peek(K)
         y = torch.empty((self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
         if not (index >= 0).any():
@@ -379,6 +454,106 @@ class PoseStream(object):
         self.last_launches = launches
         return y, torch.from_numpy(index)
 
+    def _subset_args(self, sel, counts):
+        """-> (library stream indices, their counts) as host arrays: [sel | sel + n] with augment"""
+        lib_streams = np.concatenate([sel + c * self.n for c in range(self.copies)]).astype(np.int32)
+        lib_steps = np.tile(counts, self.copies).astype(np.int64)
+        return lib_streams, lib_steps
+
+    def _subset_workspace(self, h, m, K):
+        """the workspace of a subset call of m library streams and K frames; serves every smaller m and K"""
+        wb = int(h.lib.gast_stream_subset_workspace_bytes(h.h, m, K))
+        if wb == 0:
+            raise self.engine.GastError('gast_stream_subset_workspace_bytes: %s' % L.last_error())
+        if self._subset_ws is None or self._subset_ws.numel() < wb:
+            self._subset_ws = None
+            self._subset_ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
+        return self._subset_ws
+
+    def _push_subset(self, frames, valid, sel):
+        """push_frames of the streams `sel` (frames (m, K, J, F)) through gast_stream_push_subset"""
+        eng = self.engine
+        name = type(self).__name__
+        if self.model.training:
+            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
+        h = eng.model_handle(self.model, self.device)
+        lib = h.lib
+        m, K = int(sel.size), int(frames.shape[1])
+        mm = self.copies * m
+        y = torch.empty((m, K, self.J, 3), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device).cuda_stream
+            self._begin(h, st)
+            ws = self._subset_workspace(h, mm, K)
+            lib_streams, lib_steps = self._subset_args(sel, self.counts[sel])
+            fresh, hold, index = self.book.advance_many(K, valid, streams=sel)
+            fresh_p, hold_p = self._upload_chunk(fresh, hold)
+            x, out = frames, y
+            if self.augment:
+                x = torch.empty((2, m, K, self.J, self.F), dtype=torch.float32, device=self.device)
+                if lib.gast_tta_prepare(C.c_void_p(frames.data_ptr()), C.c_void_p(x.data_ptr()), m * K, self.J,
+                                        self.F, 0, 0, len(self.kps_left), self._kl, self._kr, C.c_void_p(st)) != 0:
+                    raise eng.GastError('gast_tta_prepare: %s' % L.last_error())
+                out = torch.empty((2, m, K, self.J, 3), dtype=torch.float32, device=self.device)
+            rc = lib.gast_stream_push_subset(h.h, C.c_void_p(self._state.data_ptr()), self.copies * self.n,
+                                             C.c_void_p(lib_streams.ctypes.data), C.c_void_p(lib_steps.ctypes.data), mm,
+                                             K, C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
+                                             C.c_void_p(fresh_p), C.c_void_p(hold_p), C.c_void_p(ws.data_ptr()),
+                                             ws.numel(), C.c_void_p(st))
+            if rc != 0:
+                raise eng.GastError('gast_stream_push_subset: %s' % L.last_error())
+            launches = int(lib.gast_last_launch_count(h.h))
+            if self.augment:
+                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(y.data_ptr()), m * K, self.J,
+                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
+                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
+                launches += 2
+            self._sig = h.sig
+        self._advanced(sel, K)
+        self.last_launches = launches
+        return y, torch.from_numpy(index)
+
+    def _peek_subset(self, K, sel):
+        """peek of the streams `sel` through gast_stream_peek_subset; streams that never pushed a frame (nothing due)
+        are left out of the library call and their rows are unspecified"""
+        eng = self.engine
+        index = self.book.peek(K, streams=sel)
+        m = int(sel.size)
+        y = torch.empty((m, K, self.J, 3), dtype=torch.float32, device=self.device)
+        counts = self.counts[sel]
+        rows = np.flatnonzero(counts >= 1)
+        if not (index >= 0).any():
+            self.last_launches = 0
+            return y, torch.from_numpy(index)
+        h = eng.model_handle(self.model, self.device)
+        lib = h.lib
+        r = int(rows.size)
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device).cuda_stream
+            self._begin(h, st)
+            ws = self._subset_workspace(h, self.copies * r, K)
+            lib_streams, lib_steps = self._subset_args(sel[rows], counts[rows])
+            yr = y if r == m else torch.empty((r, K, self.J, 3), dtype=torch.float32, device=self.device)
+            out = yr
+            if self.augment:
+                out = torch.empty((2, r, K, self.J, 3), dtype=torch.float32, device=self.device)
+            rc = lib.gast_stream_peek_subset(h.h, C.c_void_p(self._state.data_ptr()), self.copies * self.n,
+                                             C.c_void_p(lib_streams.ctypes.data), C.c_void_p(lib_steps.ctypes.data),
+                                             self.copies * r, K, C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()),
+                                             ws.numel(), C.c_void_p(st))
+            if rc != 0:
+                raise eng.GastError('gast_stream_peek_subset: %s' % L.last_error())
+            launches = int(lib.gast_last_launch_count(h.h))
+            if self.augment:
+                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(yr.data_ptr()), r * K, self.J,
+                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
+                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
+                launches += 2
+            if r < m:
+                y[torch.from_numpy(rows).to(self.device)] = yr
+        self.last_launches = launches
+        return y, torch.from_numpy(index)
+
     def _chunk_workspace(self, h, m, K):
         """the workspace of a chunk (or peek) of K frames over m library streams; grows with K and serves every
         smaller K"""
@@ -396,7 +571,7 @@ class PoseStream(object):
         any_f, any_h = bool(fresh.any()), bool(hold.any())
         if not (any_f or any_h):
             return None, None
-        m = self.copies * self.n
+        m = self.copies * len(fresh)
         mk = np.concatenate([np.tile(fresh.astype(np.int32), self.copies),
                              np.tile(hold.astype(np.int32), (self.copies, 1)).reshape(-1)])
         # kept until the next chunk, so that no allocation of this one reuses it before the push read it
@@ -418,15 +593,16 @@ class CausalStream(PoseStream):
             raise engine.GastError('CausalStream needs a causal model (gen_skes.py:59 builds it with causal=True)')
         super(CausalStream, self).__init__(model_pos, n_streams, device=device)
 
-    def push(self, frame):
+    def push(self, frame, streams=None):
         """frame (n_streams, J, in_features): the newest 2D keypoints of every stream (normalised screen
-        coordinates).  Returns the 3D pose of that frame, (n_streams, J, 3)."""
-        return super(CausalStream, self).push(frame)[0]
+        coordinates).  Returns the 3D pose of that frame, (n_streams, J, 3).  With `streams` (m distinct indices):
+        the frames and poses of those streams only, (m, J, F) -> (m, J, 3)."""
+        return super(CausalStream, self).push(frame, streams=streams)[0]
 
-    def push_frames(self, frames):
+    def push_frames(self, frames, streams=None):
         """frames (n_streams, K, J, in_features): the next K frames of every stream -> their 3D poses
-        (n_streams, K, J, 3), what K calls of `push` return, in one library call."""
-        return super(CausalStream, self).push_frames(frames)[0]
+        (n_streams, K, J, 3), what K calls of `push` return, in one library call.  `streams` as for `push`."""
+        return super(CausalStream, self).push_frames(frames, streams=streams)[0]
 
 
 def lift_sequences(model_pos, sequences, n_streams=64, chunk=256, augment=False, kps_left=None, kps_right=None,

@@ -262,6 +262,33 @@ int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, const float* x,
  *   gast_tta_merge(y2, y, n * K, J, ...) with y2 (2, n, K, J, 3). */
 int gast_stream_peek(gast_t* h, const void* state, int64_t step, float* y, int32_t n_streams, int32_t K,
                      void* workspace, size_t workspace_bytes, void* stream);
+/* gast_stream_push_subset / gast_stream_peek_subset: any subset of the streams, each at its own frame count.
+ *   The lockstep entries above advance every stream of `state` by the same frames.  These take m distinct streams
+ *   streams[0..m) (host array, indices into [0, n_streams)) with their own counts steps[0..m) (host array: the frames
+ *   pushed into that stream so far; the caller keeps the counts, as it keeps `step` for the lockstep entries).
+ *   Row i of x (m, K, J, in_features), y (m, K, J, 3), fresh (m) and hold (m, K) (device, null as for
+ *   gast_stream_push_chunk) belongs to stream streams[i].  A subset push returns, and leaves stream streams[i]'s part
+ *   of `state` as, what gast_stream_push_chunk returns and leaves on a state holding that stream alone at step
+ *   steps[i].  Every byte of an unlisted stream (its input history and every ring slot of its rows) is unchanged.
+ *   A stream whose own count is 0 must be fresh.  gast_stream_peek_subset is gast_stream_peek for the listed streams
+ *   on the same terms: 1 <= K <= gast_stream_latency(h), steps[i] >= 1, nothing written to `state`.
+ *   Refused (gast_last_error) before any launch: m outside [1, n_streams], a stream outside [0, n_streams) or listed
+ *   twice, a negative step (peek: a step below 1).  The work is one chunk forward over m*K positions, so it costs
+ *   what the listed streams cost, not what n_streams cost; the launch count depends on neither n_streams, m nor K.
+ *   The workspace is gast_stream_subset_workspace_bytes(h, m, K) bytes (it grows with m and K; 0 for bad arguments),
+ *   independent of n_streams.  Listing every stream in order at one step runs exactly gast_stream_push_chunk's (or
+ *   gast_stream_peek's) kernels on the same rows.
+ *   Mixing with the lockstep entries: gast_stream_push(_ex), _push_chunk and _peek remain valid on the same state
+ *   only while every stream's own count equals their `step`; after counts diverge, use the subset entries.
+ *   Test-time augmentation: list 2m library streams [streams, streams + n] of the 2n-stream state with the steps
+ *   repeated for both halves, gast_tta_prepare / gast_tta_merge with T = m*K, masks repeated for both halves. */
+size_t gast_stream_subset_workspace_bytes(gast_t* h, int32_t m, int32_t K);
+int gast_stream_push_subset(gast_t* h, void* state, int32_t n_streams, const int32_t* streams, const int64_t* steps,
+                            int32_t m, int32_t K, const float* x, float* y, const int32_t* fresh, const int32_t* hold,
+                            void* workspace, size_t workspace_bytes, void* stream);
+int gast_stream_peek_subset(gast_t* h, const void* state, int32_t n_streams, const int32_t* streams,
+                            const int64_t* steps, int32_t m, int32_t K, float* y, void* workspace,
+                            size_t workspace_bytes, void* stream);
 
 /* ---- either side of the forward, on the device (SURVEY.md 8f N1-N3) --------------------------------
  * All pointers are device pointers unless marked (host).  Work is enqueued on `stream`.
