@@ -44,7 +44,9 @@ static int fail(const char* fmt, ...) {
   } while (0)
 
 extern "C" const char* gast_last_error(void) { return g_err; }
-extern "C" const char* gast_version(void) { return "gast_b200 0.4 (sm_90a; wgmma 3xTF32)"; }
+extern "C" const char* gast_version(void) {
+  return "gast_b200 0.5 (sm_90a; wgmma 3xFP16 on power-of-two-scaled operands, training 3xTF32)";
+}
 
 // ------------------------------------------------------------------------------------------
 // handle
@@ -97,7 +99,8 @@ struct gast_handle {
   int launches = 0;
   int tc_launches = 0;
   int gemm_core = 0;                 // 0 auto (tensor cores where possible), 1 force FFMA
-  int precision = 0;                 // 0 fp32-grade (3xTF32 on the tensor cores), 1 single-pass TF32 (inference only)
+  int precision = 0;                 // 0 fp32-grade (3xFP16 on scaled operands in inference, 3xTF32 in training),
+                                     // 1 single-pass TF32 (inference only)
   // training: per-GEMM tensor-core operand copies (3xTF32), indexed by the GEMM's position in the step (train.cuh)
   std::vector<TcWeights> train_tc;
   // optional per-launch device timing (bench.py roofline): event pairs around every launch
@@ -431,7 +434,7 @@ static int prepare_block(gast_handle* h, Lookup& L, cudaStream_t st, BlockConsts
 // ------------------------------------------------------------------------------------------
 static int prep_one_tc(gast_handle* h, cudaStream_t st, TcWeights& t, const float* W, int N, int K) {
   if (!W) return 0;
-  int rc = tc_prepare_weights(t, W, N, K, st, &h->owned);
+  int rc = tc_prepare_weights(t, W, N, K, st, &h->owned, true);   // inference: F16X3 at fp32 grade
   if (rc) return fail("tensor-core weight preparation failed: %s", cudaGetErrorString((cudaError_t)rc));
   return 0;
 }
@@ -635,7 +638,7 @@ static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p,
   if (p.N % 4 || p.ld_out % 4) return fail("internal: N/ld_out must be multiples of 4");
   if (h->gemm_core == 0 && tcw && tc_supported(p, epi, *tcw)) {
     TimedLaunch tl(h, st, LK_TC_PLAIN + epi);
-    int rc = tc_launch(st, epi, p, *tcw, h->precision == 1 ? TC_1XTF32 : TC_3XTF32);
+    int rc = tc_launch(st, epi, p, *tcw, tc_prec(*tcw, h->precision));
     if (rc) return fail("tensor-core gemm launch failed: %s", cudaGetErrorString((cudaError_t)rc));
     h->launches++;
     h->tc_launches++;
@@ -1132,14 +1135,14 @@ extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, fl
 // ------------------------------------------------------------------------------------------
 // debug / probe entry: out[M,N] = A[M,K] . W[N,K]^T on a chosen GEMM core (test infrastructure
 // for the numerics of the tensor-core path; not used by the forward).  tc_mode: the tensor-core core's precision
-// (0 3xTF32, 1 single-pass TF32).
+// (0 fp32-grade as inference runs it, three fp16 products on scaled operands; 1 single-pass TF32).
 // ------------------------------------------------------------------------------------------
 extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32_t N, int32_t K,
                                int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (M <= 0 || N <= 0 || K <= 0 || N % 4 || K % 4) return fail("gast_debug_gemm: bad shape");
   if (core < 0 || core > 1 || tc_mode < 0 || tc_mode > 1 || (core == 1 && tc_mode != 0))
-    return fail("gast_debug_gemm: core must be 0 (tensor cores, tc_mode 0 = 3xTF32 or 1 = TF32) or 1 (FFMA, tc_mode 0)");
+    return fail("gast_debug_gemm: core must be 0 (tensor cores, tc_mode 0 = fp32-grade or 1 = TF32) or 1 (FFMA, tc_mode 0)");
   GemmP p;
   gemm_flat(p, M);
   p.nseg = 1; p.seg[0] = seg_flat(A, K, K);
@@ -1148,7 +1151,7 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
   std::vector<void*> owned;
   TcWeights t;
   if (core == 0) {
-    rc = tc_prepare_weights(t, W, N, K, st, &owned);
+    rc = tc_prepare_weights(t, W, N, K, st, &owned, true);
     if (rc || !t.ready || !tc_supported(p, EPI_PLAIN, t)) {
       for (void* q : owned) cudaFree(q);
       return fail("gast_debug_gemm: shape not supported by the tensor-core core (rc=%d)", rc);
@@ -1157,7 +1160,7 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
     cudaFuncSetAttribute((const void*)gemm_ffma_kernel<EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   }
   auto launch = [&]() -> int {
-    if (core == 0) return tc_launch(st, EPI_PLAIN, p, t, tc_mode == 1 ? TC_1XTF32 : TC_3XTF32);
+    if (core == 0) return tc_launch(st, EPI_PLAIN, p, t, tc_prec(t, tc_mode));
     dim3 grid(cdiv(M, 128), cdiv(N, FF_BN));
     gemm_ffma_kernel<EPI_PLAIN><<<grid, FF_THREADS, ffma_smem_bytes(EPI_PLAIN, 1, 128, 1), st>>>(p);
     return (int)cudaGetLastError();

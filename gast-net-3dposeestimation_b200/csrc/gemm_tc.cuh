@@ -1,27 +1,38 @@
-// Tensor-core GEMM core of the lifting path (sm_90a): TF32 on wgmma, in two precisions (template PREC).
+// Tensor-core GEMM core of the lifting path (sm_90a): wgmma in three precisions (template PREC).
 //
-//   TC_3XTF32 (default, fp32-grade):  D[128 rows, 128 cols] = A_hi.B_hi + A_lo.B_hi + A_hi.B_lo
-//   TC_1XTF32 (opt-in, gast_set_precision(h, 1)):  D = A_hi.B_hi
+//   TC_F16X3 (inference at fp32 grade, gast_set_precision(h, 0)):
+//       D[128 rows, 128 cols] = 2^-(s_r + s_W) (A_lo.B_hi + A_hi.B_lo + A_hi.B_hi), fp16 operands
+//   TC_3XTF32 (training and every gradient, fp32 grade):  D = A_hi.B_hi + A_lo.B_hi + A_hi.B_lo, tf32 operands
+//   TC_1XTF32 (opt-in, gast_set_precision(h, 1)):  D = A_hi.B_hi, tf32 operands
 //
-// where x_hi = tf32(x) and x_lo = tf32(x - x_hi).  The dropped A_lo.B_lo term is 2^-22 of the result, so the
-// 3xTF32 D matches an fp32 FFMA GEMM to ~1e-7 relative (the parity bar is 1e-4 abs; a single TF32 pass does
-// not reach it, SURVEY.md §7).  The single pass is a third of the tensor work per multiply-add; its operands are
-// rounded to 10 mantissa bits, and it is offered for inference only (DESIGN.md §4.1).
+// 3xTF32 / 1xTF32: x_hi = tf32(x) and x_lo = tf32(x - x_hi).  F16X3: x is first scaled by an exact power of two,
+// 2^s_W per weight matrix (max |W| 2^s_W in [2^14, 2^15), tc_prepare_weights) and 2^s_r per A row and 32-K stage
+// (chosen the same way from the row's 32 values, in the consumers), then x_hi = fp16(x 2^s) and
+// x_lo = fp16(x 2^s - x_hi).  fp16 and tf32 both carry 11 significant bits, so both splits carry 22 and the dropped
+// A_lo.B_lo term is 2^-22 of the result in either: D matches an fp32 FFMA GEMM to ~1e-7 relative (the parity bar is
+// 1e-4 abs; a single TF32 pass does not reach it, SURVEY.md §7).  The scales keep fp32's range (no activation
+// saturates at fp16's 65504) and add no rounding; 2^-(s_r + s_W) is applied when a 16-K partial is added into the
+// tile sum, in the same single rounding as an add.  An fp16 product runs at twice the TF32 rate and stages half the
+// weight bytes, so F16X3 costs half of 3xTF32 in tensor time and a third less in staged bytes.  The single TF32
+// pass is a third of the 3xTF32 tensor work; its operands are rounded to 10 mantissa bits, and it is offered for
+// inference only (DESIGN.md §4.1).
 //
-// The two forms share everything below except the slot contents (B_lo is not staged in 1xTF32), the ring depth
-// and the number of wgmmas per k8 step (3 or 1).
+// The three forms share everything below except the slot contents (B_lo is not staged in 1xTF32; F16X3 stages
+// fp16 B copies and pads A rows to 40 floats), the ring depth and the wgmmas per 16-K partial (3xTF32 6 m64n128k8,
+// 1xTF32 2, F16X3 3 m64n128k16).
 //
 // Two-level accumulation: the tensor core aligns and truncates its addends, so a long chain of MMAs
 // into one accumulator is biased towards zero by ~0.5 ulp per MMA.  Every 16 K are therefore accumulated in a
-// fresh register tile (6 wgmmas in 3xTF32, 2 in 1xTF32) and added into the fp32 tile sum with round-to-nearest (32 K per partial sum
+// fresh register tile and added into the fp32 tile sum with round-to-nearest (32 K per partial sum
 // roughly doubled the error and pushed single training gradients past their bar).
 //
 // Per CTA (384 threads = 3 warpgroups, one CTA per SM), warp-specialised around a shared-memory ring of
-// 32-wide K stages (3xTF32: 3 slots of B_hi | B_lo | A; 1xTF32: tc_stages(TC_1XTF32) slots of B_hi | A):
+// 32-wide K stages (tc_stages(PREC) slots of B_hi | B_lo | A, B_hi | A in 1xTF32):
 //   producer (warpgroup 0, 40 registers after setmaxnreg): waits for a slot's `empty` mbarrier, then fills it.
-//     B (weights): the hi and lo copies are stored [K/4][N][4] (tc_prepare_weights), so one 3D TMA box per operand
-//                lands in the no-swizzle K-major core-matrix layout wgmma reads from shared memory (8 rows x 16 B
-//                core matrices, 128 B apart along N, 2048 B apart along K); one elected thread issues the boxes.
+//     B (weights): the hi and lo copies are stored [K/4][N][4] floats ([K/8][N][8] halves in F16X3,
+//                tc_prepare_weights), so one 3D TMA box per operand lands in the no-swizzle K-major core-matrix
+//                layout wgmma reads from shared memory (8 rows x 16 B core matrices, 128 B apart along N, 2048 B
+//                apart along K); one elected thread issues the boxes.
 //     A (activations): rows are gathered per frame (dilated / strided taps, residual slices, concatenations), so
 //                they arrive by cp.async (16 B per row and k-quad, zero-filled outside the tile) from all 128
 //                producer threads.  A stage never straddles a tap (Kc % 32 == 0), so segment, tap and column are
@@ -29,8 +40,10 @@
 //     The slot's `full` mbarrier completes when the TMA bytes (expect_tx) and every producer thread's cp.asyncs
 //     (cp.async.mbarrier.arrive.noinc) have landed: 1 + 128 arrivals.
 //   consumers (warpgroups 1 and 2, 232 registers): warpgroup 1 + w owns rows 64w .. 64w+63 and all 128 columns:
-//     wgmma.m64n128k8 tf32, A from registers (loaded from the slot and converted to tf32 there, split into hi / lo in
-//     3xTF32), B from the shared-memory descriptor.  A stage's two 16-K partials go into two register tiles back to back;
+//     wgmma.m64n128k8 tf32 or m64n128k16 f16, A from registers (loaded from the slot and converted there: to tf32,
+//     split into hi / lo in 3xTF32; in F16X3 the four threads of a quad find their rows' max |a| over the stage's
+//     32 K with two shuffles, scale and split into fp16 hi / lo), B from the shared-memory descriptor.  A stage's
+//     two 16-K partials go into two register tiles back to back;
 //     the first is added into the tile sum while the second runs (wgmma.wait_group 1), then the second is retired
 //     and added, and the slot is released (its `empty` mbarrier, one arrival per consumer warp, 8 in all).  No
 //     partial stays in flight across the loop's back edge: ptxas then serialises every wgmma of the kernel (C7514).
@@ -43,24 +56,35 @@
 // in L2.  (Every layer's A is larger than the L2; with the row tile fast, A was read from HBM once per column tile.)
 #pragma once
 #include <cuda.h>
+#include <cuda_fp16.h>
 #include <vector>
 #include "gast_common.cuh"
 #include "gemm_ffma.cuh"
 
 namespace gast {
 
+// f16 == false (training's copies): hi and lo, for 3xTF32 and 1xTF32.  f16 == true (inference's copies): hi for
+// 1xTF32 and the F16X3 pair h16 with its exponent s_W.
 struct TcWeights {
   float* hi = nullptr;   // tf32(W), stored [K/4][N][4]
-  float* lo = nullptr;   // tf32(W - tf32(W)), same layout
-  CUtensorMap map_hi, map_lo;
+  float* lo = nullptr;   // tf32(W - tf32(W)), same layout; not allocated when f16
+  __half* h16 = nullptr; // fp16(W 2^s_W) then fp16(W 2^s_W - hi), each stored [K/8][N][8]
+  int* sw = nullptr;     // s_W (device)
+  CUtensorMap map_hi, map_lo, map_h16hi, map_h16lo;
   int N = 0, K = 0;
+  bool f16 = false;
   bool ready = false;
 };
 
-enum { TC_3XTF32 = 0, TC_1XTF32 = 1 };               // precision of the core: gast_set_precision's mode
+// precision of the core: TC_3XTF32 and TC_F16X3 are gast_set_precision's mode 0 (training and inference), TC_1XTF32
+// its mode 1
+enum { TC_3XTF32 = 0, TC_1XTF32 = 1, TC_F16X3 = 2 };
 
 #ifndef GAST_TC1_STAGES
 #define GAST_TC1_STAGES 3                             // ring depth of the 1xTF32 form: 4 and 5 measured slower (DESIGN.md §4.1)
+#endif
+#ifndef GAST_TC16_STAGES
+#define GAST_TC16_STAGES 3                            // ring depth of the F16X3 form: 4 and 5 measured no faster (DESIGN.md §4.1)
 #endif
 
 constexpr int TC_BM = 128, TC_BN = 128;
@@ -69,20 +93,30 @@ constexpr int TC_KP = 16;                            // K per partial sum, added
 constexpr int TC_THREADS = 384;                      // warpgroup 0 produces, warpgroups 1 and 2 consume
 constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;   // 128 * 40 + 256 * 232 <= 64K registers of the SM
 constexpr int TC_ALD = TC_KS + 4;                    // A stage row stride (floats): conflict-free fragment loads
+constexpr int TC_ALD16 = TC_KS + 8;                  // the same for F16X3's 64-bit k-pair loads
 constexpr int TC_B_BYTES = TC_BN * TC_KS * 4;        // one of B_hi / B_lo in a stage
+constexpr int TC_B16_BYTES = TC_BN * TC_KS * 2;      // the same in F16X3
 constexpr int TC_A_BYTES = TC_BM * TC_ALD * 4;
-// B copies per slot, slot size and ring depth of each precision.  3xTF32: a fourth slot measured slower
-// (DESIGN.md §4.1).
+// A row stride, B copy bytes, B copies per slot, slot size and ring depth of each precision.  3xTF32: a fourth slot
+// measured slower (DESIGN.md §4.1).
+__host__ __device__ constexpr int tc_ald(int prec) { return prec == TC_F16X3 ? TC_ALD16 : TC_ALD; }
+__host__ __device__ constexpr int tc_bbytes(int prec) { return prec == TC_F16X3 ? TC_B16_BYTES : TC_B_BYTES; }
 __host__ __device__ constexpr int tc_nb(int prec) { return prec == TC_1XTF32 ? 1 : 2; }
-__host__ __device__ constexpr int tc_slot(int prec) { return tc_nb(prec) * TC_B_BYTES + TC_A_BYTES; }   // B_hi [| B_lo] | A
-__host__ __device__ constexpr int tc_stages(int prec) { return prec == TC_1XTF32 ? GAST_TC1_STAGES : 3; }
+__host__ __device__ constexpr int tc_slot(int prec) {                       // B_hi [| B_lo] | A
+  return tc_nb(prec) * tc_bbytes(prec) + TC_BM * tc_ald(prec) * 4;
+}
+__host__ __device__ constexpr int tc_stages(int prec) {
+  return prec == TC_1XTF32 ? GAST_TC1_STAGES : prec == TC_F16X3 ? GAST_TC16_STAGES : 3;
+}
 __host__ __device__ constexpr int tc_ring(int prec) { return tc_stages(prec) * tc_slot(prec); }
 constexpr int TC_STG_LD = 136;                       // [row][col] stride of the accumulator hand-over to the epilogue
 constexpr int TC_ROWBASE_BYTES = 3 * 128 * sizeof(long long);
 constexpr int TC_SMEM_MAX = 200 * 1024;
-static_assert(tc_slot(TC_3XTF32) % 1024 == 0 && tc_slot(TC_1XTF32) % 1024 == 0, "ring slots stay 1024-byte aligned");
-static_assert(tc_ring(TC_1XTF32) + 16 * tc_stages(TC_1XTF32) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX,
-              "the 1xTF32 ring fits the shared memory the 3xTF32 form may use");
+static_assert(tc_slot(TC_3XTF32) % 1024 == 0 && tc_slot(TC_1XTF32) % 1024 == 0 && tc_slot(TC_F16X3) % 1024 == 0,
+              "ring slots stay 1024-byte aligned");
+static_assert(tc_ring(TC_1XTF32) + 16 * tc_stages(TC_1XTF32) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX &&
+              tc_ring(TC_F16X3) + 16 * tc_stages(TC_F16X3) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX,
+              "every ring fits the shared memory the core may use");
 
 __host__ __device__ inline size_t tc_smem_bytes(int prec, int epi, int J, int fpt, int hpt) {
   size_t m = (size_t)tc_ring(prec) + 16 * tc_stages(prec);   // + a full and an empty mbarrier per slot
@@ -213,6 +247,93 @@ __device__ __forceinline__ void tc_add(float (&acc)[64], float (&part)[64]) {
   for (int i = 0; i < 64; ++i) acc[i] += part[i];
 }
 
+// d (+)= a . B, m64n128k16, fp16 operands (A from registers, B K-major from shared memory), fp32 accumulate
+__device__ __forceinline__ void wgmma_f16(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %68, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %69, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(scale_d), "l"(bdesc));
+}
+
+// One F16X3 16-K partial: d = A_lo.B_hi + A_hi.B_lo + A_hi.B_hi (small products first) of the k16 step s of the slot
+// at sb, issued as one wgmma group
+__device__ __forceinline__ void tc_partial16(float (&d)[64], const uint32_t (&ah)[4], const uint32_t (&al)[4],
+                                             uint32_t sb, int s) {
+  tile_fence(d);
+  wgmma_fence();
+  const uint64_t dh = tc_bdesc(sb + s * 4096), dl = tc_bdesc(sb + TC_B16_BYTES + s * 4096);
+  wgmma_f16(d, al, dh, 0);
+  wgmma_f16(d, ah, dl, 1);
+  wgmma_f16(d, ah, dh, 1);
+  wgmma_commit();
+}
+
+__device__ __forceinline__ float exp2i(int e) { return __int_as_float((e + 127) << 23); }   // 2^e, e in [-126, 127]
+
+// s_r of a row whose max |a| is m: m 2^s_r in [2^14, 2^15) from m's exponent bits, 0 for m == 0 or not finite,
+// clamped to [smin, smax] (tc_scale_bounds)
+__device__ __forceinline__ int tc_row_exp(float m, int smin, int smax) {
+  const int eb = __float_as_int(m) >> 23;                                // m >= 0: the biased exponent
+  const int s = (m == 0.f || eb == 255) ? 0 : 141 - eb;                  // m in [2^(eb-127), 2^(eb-126))
+  return min(max(s, smin), smax);
+}
+
+// s_r's range: 2^s_r and 2^-(s_r + s_W) both normal fp32
+__device__ __forceinline__ void tc_scale_bounds(int sw, int& smin, int& smax) {
+  smin = max(-126, -127 - sw);
+  smax = min(127, 126 - sw);
+}
+
+// The F16X3 A fragments of both k16 steps of a slot's A (row stride TC_ALD16): rows r0, r0 + 8 at k pairs
+// 16 s + 2t and 16 s + 2t + 8, scaled per row by 2^s_r and split into fp16 hi / lo; u0, u1 = 2^-(s_r + s_W) of the
+// two rows.  The quad's four threads hold a row's 32 values of the stage between them.
+__device__ __forceinline__ void tc_load_a16(const float* A, int r0, int t, int sw, int smin, int smax,
+                                            uint32_t (&ah)[2][4], uint32_t (&al)[2][4], float& u0, float& u1) {
+  float2 x[2][4];
+#pragma unroll
+  for (int s = 0; s < 2; ++s) {
+    const int k = 16 * s + 2 * t;
+    x[s][0] = *reinterpret_cast<const float2*>(A + r0 * TC_ALD16 + k);
+    x[s][1] = *reinterpret_cast<const float2*>(A + (r0 + 8) * TC_ALD16 + k);
+    x[s][2] = *reinterpret_cast<const float2*>(A + r0 * TC_ALD16 + k + 8);
+    x[s][3] = *reinterpret_cast<const float2*>(A + (r0 + 8) * TC_ALD16 + k + 8);
+  }
+  float m[2] = {0.f, 0.f};
+#pragma unroll
+  for (int s = 0; s < 2; ++s)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) m[q & 1] = fmaxf(m[q & 1], fmaxf(fabsf(x[s][q].x), fabsf(x[s][q].y)));
+  float v[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
+    m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
+    const int e = tc_row_exp(m[h], smin, smax);
+    v[h] = exp2i(e);
+    (h ? u1 : u0) = exp2i(-(e + sw));
+  }
+#pragma unroll
+  for (int s = 0; s < 2; ++s)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float2 y = make_float2(x[s][q].x * v[q & 1], x[s][q].y * v[q & 1]);
+      const __half2 hi = __float22half2_rn(y);
+      const float2 hf = __half22float2(hi);
+      const __half2 lo = __float22half2_rn(make_float2(y.x - hf.x, y.y - hf.y));
+      ah[s][q] = *reinterpret_cast<const uint32_t*>(&hi);
+      al[s][q] = *reinterpret_cast<const uint32_t*>(&lo);
+    }
+}
+
+// acc += 2^-(s_r + s_W) part, one rounding per element (the multiplier is a power of two); u0 scales the fragment's
+// row r0, u1 its row r0 + 8
+__device__ __forceinline__ void tc_add_scaled(float (&acc)[64], float (&part)[64], float u0, float u1) {
+  tile_fence(part);
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = fmaf(part[i], (i & 2) ? u1 : u0, acc[i]);
+}
+
 // This CTA's row tile and column tile.  %ctaid is read with a volatile move, so that the consumers can recompute the
 // tile after their K loop instead of keeping it in registers through it (that spilled in the SemCH instantiation).
 __device__ __forceinline__ void tc_tile(const GemmP& p, int& rt, int& ctile) {
@@ -223,12 +344,14 @@ __device__ __forceinline__ void tc_tile(const GemmP& p, int& rt, int& ctile) {
   ctile = (int)b - rt * col_tiles;
 }
 
-// mlo is not read in 1xTF32
+// mlo is not read in 1xTF32, sw (s_W) only in F16X3
 template <int EPI, int PREC>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensorMap mhi,
-               const __grid_constant__ CUtensorMap mlo) {
+               const __grid_constant__ CUtensorMap mlo, const int* __restrict__ sw) {
   constexpr int STAGES = tc_stages(PREC), SLOT = tc_slot(PREC), NB = tc_nb(PREC);
+  constexpr int BBYTES = tc_bbytes(PREC), ALD = tc_ald(PREC);
+  constexpr int KSH = PREC == TC_F16X3 ? 3 : 2;                         // log2 of the k's per 16-byte row of a B copy
   extern __shared__ __align__(16) unsigned char smem_raw[];
   long long* rowbase = reinterpret_cast<long long*>(smem_raw);          // [3][128]
   const uint32_t raw = smem_u32(smem_raw);
@@ -279,10 +402,10 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
       if (c >= STAGES) mbar_wait(empty0 + 8 * slot, (c / STAGES - 1) & 1);
       const uint32_t sb = rb + slot * SLOT, full = full0 + 8 * slot;
       if (tid == 0) {
-        mbar_arrive_expect_tx(full, NB * TC_B_BYTES);
-        const int kq = (kcol + k0) >> 2;
+        mbar_arrive_expect_tx(full, NB * BBYTES);
+        const int kq = (kcol + k0) >> KSH;
         tma_load_3d(sb, &mhi, full, 0, n0, kq);
-        if (NB == 2) tma_load_3d(sb + TC_B_BYTES, &mlo, full, 0, n0, kq);
+        if (NB == 2) tma_load_3d(sb + BBYTES, &mlo, full, 0, n0, kq);
       }
       const ASeg& sg = p.seg[seg];
       const float* src = sg.base + tap * sg.tap_stride + kin + q * 4;
@@ -290,7 +413,7 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
       for (int i = 0; i < TC_BM / 16; ++i) {
         const int r = rq + 16 * i;
         const long long off = rowbase[seg * 128 + r];
-        cp_async16(sb + NB * TC_B_BYTES + (r * TC_ALD + q * 4) * 4, off >= 0 ? src + off : sg.base, off >= 0 ? 16 : 0);
+        cp_async16(sb + NB * BBYTES + (r * ALD + q * 4) * 4, off >= 0 ? src + off : sg.base, off >= 0 ? 16 : 0);
       }
       cp_async_arrive(full);
       k0 += TC_KS;
@@ -312,21 +435,43 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 
-  for (int c = 0; c < nstages; ++c) {
-    const int slot = c % STAGES;
-    mbar_wait(full0 + 8 * slot, (c / STAGES) & 1);
-    const uint32_t sb = rb + slot * SLOT;
-    const float* A = reinterpret_cast<const float*>(ring + slot * SLOT + NB * TC_B_BYTES);
-    uint32_t ah[2][4], al[2][4];
-    tc_load_a<PREC>(A, r0, t, 0, ah, al);
-    tc_partial<PREC>(part0, ah, al, sb, 0);
-    tc_load_a<PREC>(A, r0, t, 2, ah, al);
-    tc_partial<PREC>(part1, ah, al, sb, 2);
-    wgmma_wait<1>();                            // the first partial has retired ...
-    tc_add(acc, part0);                         // ... and is summed while the second runs
-    wgmma_wait<0>();
-    tc_add(acc, part1);
-    if (lane == 0) mbar_arrive(empty0 + 8 * slot);
+  if constexpr (PREC == TC_F16X3) {
+    const int s_w = *sw;
+    int smin, smax;
+    tc_scale_bounds(s_w, smin, smax);
+    for (int c = 0; c < nstages; ++c) {
+      const int slot = c % STAGES;
+      mbar_wait(full0 + 8 * slot, (c / STAGES) & 1);
+      const uint32_t sb = rb + slot * SLOT;
+      const float* A = reinterpret_cast<const float*>(ring + slot * SLOT + NB * BBYTES);
+      uint32_t ah[2][4], al[2][4];
+      float u0, u1;
+      tc_load_a16(A, r0, t, s_w, smin, smax, ah, al, u0, u1);   // one scale per row and stage
+      tc_partial16(part0, ah[0], al[0], sb, 0);
+      tc_partial16(part1, ah[1], al[1], sb, 1);
+      wgmma_wait<1>();
+      tc_add_scaled(acc, part0, u0, u1);
+      wgmma_wait<0>();
+      tc_add_scaled(acc, part1, u0, u1);
+      if (lane == 0) mbar_arrive(empty0 + 8 * slot);
+    }
+  } else {
+    for (int c = 0; c < nstages; ++c) {
+      const int slot = c % STAGES;
+      mbar_wait(full0 + 8 * slot, (c / STAGES) & 1);
+      const uint32_t sb = rb + slot * SLOT;
+      const float* A = reinterpret_cast<const float*>(ring + slot * SLOT + NB * TC_B_BYTES);
+      uint32_t ah[2][4], al[2][4];
+      tc_load_a<PREC>(A, r0, t, 0, ah, al);
+      tc_partial<PREC>(part0, ah, al, sb, 0);
+      tc_load_a<PREC>(A, r0, t, 2, ah, al);
+      tc_partial<PREC>(part1, ah, al, sb, 2);
+      wgmma_wait<1>();                            // the first partial has retired ...
+      tc_add(acc, part0);                         // ... and is summed while the second runs
+      wgmma_wait<0>();
+      tc_add(acc, part1);
+      if (lane == 0) mbar_arrive(empty0 + 8 * slot);
+    }
   }
   epi_sync();                                   // both consumers are done with the ring
   tc_tile(p, rt, ctile);
@@ -355,7 +500,7 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   gemm_epilogue<EPI>(p, out, reinterpret_cast<float*>(ring), ct, fe, nfe, nfe * J, ctile * TC_BN, ctile);
 }
 
-// W [N][K] -> hi / lo in the TMA-friendly layout [K/4][N][4] (both precisions read hi = tf32(W))
+// W [N][K] -> hi / lo in the TMA-friendly layout [K/4][N][4] (both TF32 forms read hi = tf32(W)); lo may be null
 __global__ void tc_split_kernel(const float* __restrict__ w, float* __restrict__ hi, float* __restrict__ lo, int N, int K) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)N * K) return;
@@ -364,7 +509,35 @@ __global__ void tc_split_kernel(const float* __restrict__ w, float* __restrict__
   const float h = __uint_as_float(tf32_bits(x));
   const long long o = ((long long)(k >> 2) * N + n) * 4 + (k & 3);
   hi[o] = h;
-  lo[o] = __uint_as_float(tf32_bits(x - h));
+  if (lo) lo[o] = __uint_as_float(tf32_bits(x - h));
+}
+
+// s_W of W [n]: max |W| 2^s_W in [2^14, 2^15), 0 for an all-zero or non-finite W.  One block.
+__global__ void tc_wscale_kernel(const float* __restrict__ w, long long n, int* __restrict__ sw) {
+  __shared__ float red[32];
+  float m = 0.f;
+  for (long long i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(w[i]));
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    m = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if (threadIdx.x == 0) *sw = (m == 0.f || !isfinite(m)) ? 0 : 14 - ilogbf(m);   // ilogbf: subnormals too
+  }
+}
+
+// W [N][K] -> fp16(W 2^s_W) and fp16(W 2^s_W - hi), each in the TMA-friendly layout [K/8][N][8]
+__global__ void tc_split16_kernel(const float* __restrict__ w, const int* __restrict__ sw, __half* __restrict__ hi,
+                                  __half* __restrict__ lo, int N, int K) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)N * K) return;
+  const int n = (int)(i / K), k = (int)(i - (long long)n * K);
+  const float x = scalbnf(w[i], *sw);
+  const __half h = __float2half_rn(x);
+  const long long o = ((long long)(k >> 3) * N + n) * 8 + (k & 7);
+  hi[o] = h;
+  lo[o] = __float2half_rn(x - __half2float(h));
 }
 
 typedef CUresult (*tc_encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -383,42 +556,64 @@ inline tc_encode_fn tc_get_encode() {
   return fn;
 }
 
-// W: [N][K] fp32 K-major (device).  Allocates hi / lo once per shape, encodes their TMA maps and splits W into them.
-// Returns 0 on success (t.ready says whether the core takes the shape), a cudaError_t or -1 otherwise.
-inline int tc_prepare_weights(TcWeights& t, const float* W, int N, int K, cudaStream_t st, std::vector<void*>* owned) {
+// W: [N][K] fp32 K-major (device).  Allocates the copies once per shape and form, encodes their TMA maps and splits W
+// into them: f16 == false, tf32 hi / lo (training: 3xTF32); f16 == true, tf32 hi (1xTF32) and the F16X3 pair with
+// s_W (inference).  Returns 0 on success (t.ready says whether the core takes the shape), a cudaError_t or -1
+// otherwise.
+inline int tc_prepare_weights(TcWeights& t, const float* W, int N, int K, cudaStream_t st, std::vector<void*>* owned,
+                              bool f16) {
   t.ready = false;
   if (K % TC_KS != 0 || N % 4 != 0) return 0;            // shape not taken by this core (FFMA runs it)
-  if (!t.hi || t.N != N || t.K != K) {
+  if (!t.hi || t.N != N || t.K != K || t.f16 != f16) {
     tc_encode_fn enc = tc_get_encode();
     if (!enc) return -1;
     void* a = nullptr; void* b = nullptr;
+    const size_t nb = f16 ? sizeof(__half) * 2 * (size_t)N * K + 256 : sizeof(float) * (size_t)N * K;
     cudaError_t e = cudaMalloc(&a, sizeof(float) * (size_t)N * K);
     if (e != cudaSuccess) return (int)e;
-    e = cudaMalloc(&b, sizeof(float) * (size_t)N * K);
+    e = cudaMalloc(&b, nb);
     if (e != cudaSuccess) { cudaFree(a); return (int)e; }
     owned->push_back(a); owned->push_back(b);
-    t.hi = (float*)a; t.lo = (float*)b; t.N = N; t.K = K;
+    t.hi = (float*)a; t.N = N; t.K = K; t.f16 = f16;
+    t.lo = f16 ? nullptr : (float*)b;
+    t.h16 = f16 ? (__half*)b : nullptr;
+    t.sw = f16 ? (int*)(t.h16 + 2 * (size_t)N * K) : nullptr;
     // dims {4 k's, N rows, K/4 k-quads}; box {4, 128, TC_KS/4}: rows past N read as zero
     cuuint64_t dims[3] = {4, (cuuint64_t)N, (cuuint64_t)(K / 4)};
     cuuint64_t strides[2] = {16, (cuuint64_t)N * 16};
     cuuint32_t box[3] = {4, (cuuint32_t)TC_BN, (cuuint32_t)(TC_KS / 4)};
     cuuint32_t estr[3] = {1, 1, 1};
-    for (int m = 0; m < 2; ++m) {
+    for (int m = 0; m < (f16 ? 1 : 2); ++m) {
       CUresult r = enc(m ? &t.map_lo : &t.map_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, m ? t.lo : t.hi, dims, strides, box,
                        estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) { t.hi = nullptr; return -1; }
     }
+    if (f16) {
+      // dims {8 k's, N rows, K/8 k-octets}; box {8, 128, TC_KS/8}: the same 16-byte rows as the fp32 copies
+      cuuint64_t d16[3] = {8, (cuuint64_t)N, (cuuint64_t)(K / 8)};
+      cuuint32_t b16[3] = {8, (cuuint32_t)TC_BN, (cuuint32_t)(TC_KS / 8)};
+      for (int m = 0; m < 2; ++m) {
+        CUresult r = enc(m ? &t.map_h16lo : &t.map_h16hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, t.h16 + (size_t)m * N * K,
+                         d16, strides, b16, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) { t.hi = nullptr; return -1; }
+      }
+    }
   }
   const long long n = (long long)N * K;
   tc_split_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, t.hi, t.lo, N, K);
+  if (f16) {
+    tc_wscale_kernel<<<1, 1024, 0, st>>>(W, n, t.sw);
+    tc_split16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, t.sw, t.h16, t.h16 + n, N, K);
+  }
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
   t.ready = true;
   return 0;
 }
 
-// The shapes the core takes are the same in both precisions (the 1xTF32 ring is no larger than the bound below).
+// The shapes the core takes are the same in every precision (each ring is no larger than the bound below).
 inline bool tc_supported(const GemmP& p, int epi, const TcWeights& t) {
   if (!t.ready || t.K != p.ldw || t.N < p.N || p.N % 4) return false;
   for (int s = 0; s < p.nseg; ++s) {
@@ -429,6 +624,7 @@ inline bool tc_supported(const GemmP& p, int epi, const TcWeights& t) {
   const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
   if (tc_smem_bytes(TC_3XTF32, epi, p.J, p.fpt, hpt) > TC_SMEM_MAX) return false;
   if (tc_smem_bytes(TC_1XTF32, epi, p.J, p.fpt, hpt) > TC_SMEM_MAX) return false;
+  if (tc_smem_bytes(TC_F16X3, epi, p.J, p.fpt, hpt) > TC_SMEM_MAX) return false;
   return true;
 }
 
@@ -448,16 +644,25 @@ inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeig
     if (e != cudaSuccess) return (int)e;
     attr_set[dev & 63][epi] = true;
   }
-  if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN, PREC><<<grid, TC_THREADS, smem, st>>>(p, t.map_hi, t.map_lo);
-  else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH, PREC><<<grid, TC_THREADS, smem, st>>>(p, t.map_hi, t.map_lo);
-  else gemm_tc_kernel<EPI_GLOBAL, PREC><<<grid, TC_THREADS, smem, st>>>(p, t.map_hi, t.map_lo);
+  const CUtensorMap& mhi = PREC == TC_F16X3 ? t.map_h16hi : t.map_hi;
+  const CUtensorMap& mlo = PREC == TC_F16X3 ? t.map_h16lo : t.map_lo;
+  if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, t.sw);
+  else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, t.sw);
+  else gemm_tc_kernel<EPI_GLOBAL, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, t.sw);
   return (int)cudaGetLastError();
 }
 
 // One CTA per tile, tile = row tile * column tiles + column tile (the column tile fastest, see gemm_tc_kernel).
-// prec: TC_3XTF32 or TC_1XTF32.
+// prec: TC_3XTF32 (needs t.f16 false), TC_1XTF32 or TC_F16X3 (needs t.f16).
 inline int tc_launch(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t, int prec) {
-  return prec == TC_1XTF32 ? tc_launch_prec<TC_1XTF32>(st, epi, p, t) : tc_launch_prec<TC_3XTF32>(st, epi, p, t);
+  if (prec == TC_1XTF32) return tc_launch_prec<TC_1XTF32>(st, epi, p, t);
+  if (prec == TC_F16X3) return t.f16 ? tc_launch_prec<TC_F16X3>(st, epi, p, t) : -1;
+  return t.f16 ? -1 : tc_launch_prec<TC_3XTF32>(st, epi, p, t);
+}
+
+// The fp32-grade form of a weight copy: F16X3 for inference's copies, 3xTF32 for training's
+inline int tc_prec(const TcWeights& t, int precision) {
+  return precision == 1 ? TC_1XTF32 : t.f16 ? TC_F16X3 : TC_3XTF32;
 }
 
 }  // namespace gast

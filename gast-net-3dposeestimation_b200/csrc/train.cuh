@@ -44,15 +44,15 @@ static bool want_grad(TCtx& c, const std::string& key, int64_t numel, float** ou
 
 // Tensor-core operand copies of one training GEMM's weight matrix (forward: the raw weights, backward: their transposes):
 // the weights change every step, so the hi/lo split runs per call; buffers live in a per-handle table indexed by the
-// GEMM's position in the step (the sequence of GEMMs of a model is fixed).  3xTF32 arithmetic (gemm_tc.cuh), the same
-// as inference, so the gradient-noise bars of tests/test_gpu_train.py hold unchanged.  Shapes the core does not take
-// (K % 16: the expand conv) stay on FFMA.
+// GEMM's position in the step (the sequence of GEMMs of a model is fixed).  3xTF32 arithmetic (gemm_tc.cuh; inference
+// runs the equally precise F16X3 form), the arithmetic the gradient-noise bars of tests/test_gpu_train.py were set
+// against.  Shapes the core does not take (K % 16: the expand conv) stay on FFMA.
 static const TcWeights* train_tcw(TCtx& c, const float* W, int N, int K) {
   const size_t slot = (size_t)c.tc_slot++;
   if (c.h->gemm_core != 0) return nullptr;
   if (c.h->train_tc.size() <= slot) c.h->train_tc.resize(slot + 1);
   TcWeights& t = c.h->train_tc[slot];
-  if (tc_prepare_weights(t, W, N, K, c.st, &c.h->owned)) return nullptr;
+  if (tc_prepare_weights(t, W, N, K, c.st, &c.h->owned, false)) return nullptr;
   return t.ready ? &t : nullptr;
 }
 

@@ -638,7 +638,8 @@ def profile_forward(module, x, reps=5):
     gemm = sum(v for k, v in per.items() if fam(k))
     ng = sum(v for k, v in n_launch.items() if fam(k))
     tc = int(lib.gast_last_tc_launch_count(h.h))
-    tc_name = 'wgmma-1xtf32' if get_precision(module) == 'tf32' else 'wgmma-3xtf32'
+    # fp32 grade: three fp16 products on scaled operands, as precise as 3xTF32 (gemm_tc.cuh)
+    tc_name = 'wgmma-1xtf32' if get_precision(module) == 'tf32' else 'wgmma-3xtf32-grade-3xfp16'
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     with torch.no_grad():
         e0.record()

@@ -122,13 +122,15 @@ int gast_set_timing(gast_t* h, int32_t on);
 int32_t gast_get_timings(gast_t* h, int32_t max_n, float* ms, int32_t* kinds);
 
 /* GEMM core selection for A/B checks on the GPU: 0 = auto (tensor cores where the shape
- * allows; 3xTF32 or single-pass TF32 as gast_set_precision says), 1 = force the FP32 FFMA core (fp32 in either
+ * allows; fp32-grade or single-pass TF32 as gast_set_precision says), 1 = force the FP32 FFMA core (fp32 in either
  * precision).  Not a fallback switch: both are CUDA paths. */
 int gast_set_gemm_core(gast_t* h, int32_t core);
 
 /* Arithmetic of the GEMMs the tensor-core core runs, for every handle kind and for gast_forward,
  * gast_forward_mpjpe and the gast_stream_push* calls:
- *   0 = fp32-grade (default): 3xTF32, within ~1e-7 relative of an fp32 GEMM.
+ *   0 = fp32-grade (default), within ~1e-7 relative of an fp32 GEMM: three fp16 products on operands scaled by
+ *       exact powers of two (per weight matrix, and per row and 32-K stage of A), fp32's full range; training and
+ *       every gradient run the equally precise 3xTF32.
  *   1 = TF32: tf32(A) . tf32(W) with fp32 accumulation, one tensor-core product per multiply-add.  Operands are
  *       rounded to 10 mantissa bits (round to nearest, ties away), so outputs move by ~1e-3 relative
  *       (DESIGN.md §4.1).  Inference only: gast_forward_train, gast_backward(_input), gast_eval_backward and their
@@ -338,7 +340,8 @@ int gast_adam_step(const int64_t* table, int32_t n_chunks, float* exp_avg, float
                    double lr, double beta1, double beta2, double eps, double weight_decay, int64_t step, void* stream);
 
 /* Test/probe entry (not on the forward path): out[M,N] = A[M,K] . W[N,K]^T on one GEMM core
- * (core 0 = tensor cores, tc_mode 0 = 3xTF32 or 1 = single-pass TF32; core 1 = FFMA, tc_mode 0).  Runs once, then `reps` timed launches
+ * (core 0 = tensor cores, tc_mode 0 = fp32-grade as inference runs it, three scaled fp16 products, or
+ * 1 = single-pass TF32; core 1 = FFMA, tc_mode 0).  Runs once, then `reps` timed launches
  * (CUDA events) whose mean duration is written to *ms_out (host).  Synchronises the stream. */
 int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32_t N, int32_t K,
                     int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream);
