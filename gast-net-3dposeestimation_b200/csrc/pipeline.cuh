@@ -216,8 +216,12 @@ __global__ void mpjpe_final_kernel(const double* __restrict__ partial, int nb, l
 // ------------------------------------------------------------------------------------------
 // N2: p_mpjpe (common/loss.py:14-53): per frame, similarity-Procrustes alignment of the prediction to
 // the target (3x3 SVD), then the mean joint distance.  One warp per frame, lanes over joints; the 3x3
-// decomposition runs in double (Jacobi on H^T H) on every lane redundantly.
+// decomposition runs in double (Jacobi on H^T H) on every lane redundantly.  R is a proper rotation for every rank of
+// H (planar and collinear frames included); a frame with zero spread divides by a zero norm and gives NaN, as the
+// reference does.
 // ------------------------------------------------------------------------------------------
+constexpr double PM_NOISE = 1e-12;                        // |H v| below PM_NOISE s0 is rounding noise, not a direction
+
 __device__ __forceinline__ double warp_sum_d(double v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
@@ -277,22 +281,41 @@ __global__ void p_mpjpe_kernel(const float* __restrict__ pred, const float* __re
   int ord[3] = {0, 1, 2};                                 // descending eigenvalues (numpy's singular-value order)
   for (int i = 0; i < 2; ++i) for (int j = 0; j < 2 - i; ++j)
     if (lam[ord[j]] < lam[ord[j + 1]]) { int tq = ord[j]; ord[j] = ord[j + 1]; ord[j + 1] = tq; }
-  double Vs[3][3], U[3][3], s[3];
-  for (int k = 0; k < 3; ++k) {
-    s[k] = sqrt(fmax(lam[ord[k]], 0.0));
+  double Vs[3][3], U[3][3], s[3], w[3][3];                // w[:,k] = H v_k
+  for (int k = 0; k < 3; ++k)
     for (int i = 0; i < 3; ++i) Vs[i][k] = V[i][ord[k]];
+  for (int k = 0; k < 3; ++k)
+    for (int i = 0; i < 3; ++i) w[i][k] = H[i][0] * Vs[0][k] + H[i][1] * Vs[1][k] + H[i][2] * Vs[2][k];
+  // U from H v_k by Gram-Schmidt, orthonormal at every rank of H.  sqrt(lambda_k) cannot be the divisor: H^T H carries
+  // rounding of ~1e-16 s0^2, so for a planar or collinear frame the "zero" singular values come out near 1e-8 s0 and
+  // H v_k / sqrt(lambda_k) is noise of no particular length.  s_k = u_k^T H v_k.
+  const double n0 = sqrt(w[0][0] * w[0][0] + w[1][0] * w[1][0] + w[2][0] * w[2][0]);
+  for (int i = 0; i < 3; ++i) U[i][0] = n0 > 0.0 ? w[i][0] / n0 : (i == 0 ? 1.0 : 0.0);
+  double u1[3] = {w[0][1], w[1][1], w[2][1]};
+  for (int pass = 0; pass < 2; ++pass) {                  // twice: orthogonal to rounding even when H v1 is mostly u0
+    const double p = U[0][0] * u1[0] + U[1][0] * u1[1] + U[2][0] * u1[2];
+    for (int i = 0; i < 3; ++i) u1[i] -= p * U[i][0];
   }
-  for (int k = 0; k < 2; ++k)
-    for (int i = 0; i < 3; ++i)
-      U[i][k] = (H[i][0] * Vs[0][k] + H[i][1] * Vs[1][k] + H[i][2] * Vs[2][k]) / fmax(s[k], 1e-300);
-  {
-    double u2[3] = {H[0][0] * Vs[0][2] + H[0][1] * Vs[1][2] + H[0][2] * Vs[2][2],
-                    H[1][0] * Vs[0][2] + H[1][1] * Vs[1][2] + H[1][2] * Vs[2][2],
-                    H[2][0] * Vs[0][2] + H[2][1] * Vs[1][2] + H[2][2] * Vs[2][2]};
-    const double cr[3] = {U[1][0] * U[2][1] - U[2][0] * U[1][1], U[2][0] * U[0][1] - U[0][0] * U[2][1],
-                          U[0][0] * U[1][1] - U[1][0] * U[0][1]};
-    if (s[2] > 1e-9 * s[0]) { for (int i = 0; i < 3; ++i) U[i][2] = u2[i] / s[2]; }
-    else { for (int i = 0; i < 3; ++i) U[i][2] = cr[i]; }   // rank-deficient H: any unit vector completing the basis
+  const double n1 = sqrt(u1[0] * u1[0] + u1[1] * u1[1] + u1[2] * u1[2]);
+  if (n1 > PM_NOISE * n0) {
+    for (int i = 0; i < 3; ++i) U[i][1] = u1[i] / n1;
+  } else {                                                // rank(H) <= 1: any unit vector orthogonal to u0 (u0 x e_m,
+    int m = 0;                                            // e_m the axis of u0's smallest component)
+    for (int i = 1; i < 3; ++i) if (fabs(U[i][0]) < fabs(U[m][0])) m = i;
+    const double e[3] = {m == 0 ? 1.0 : 0.0, m == 1 ? 1.0 : 0.0, m == 2 ? 1.0 : 0.0};
+    const double c[3] = {U[1][0] * e[2] - U[2][0] * e[1], U[2][0] * e[0] - U[0][0] * e[2], U[0][0] * e[1] - U[1][0] * e[0]};
+    const double nc = sqrt(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]);
+    for (int i = 0; i < 3; ++i) U[i][1] = c[i] / nc;
+  }
+  {                                                       // u2 = +-(u0 x u1), the sign of (H v2).(u0 x u1); + at noise
+    const double c[3] = {U[1][0] * U[2][1] - U[2][0] * U[1][1], U[2][0] * U[0][1] - U[0][0] * U[2][1],
+                         U[0][0] * U[1][1] - U[1][0] * U[0][1]};
+    const double d = w[0][2] * c[0] + w[1][2] * c[1] + w[2][2] * c[2];
+    const double sg = (d < 0.0 && -d > PM_NOISE * n0) ? -1.0 : 1.0;
+    for (int i = 0; i < 3; ++i) U[i][2] = sg * c[i];
+    s[0] = n0;
+    s[1] = U[0][1] * w[0][1] + U[1][1] * w[1][1] + U[2][1] * w[2][1];
+    s[2] = sg * d;
   }
   auto det3 = [](double m[3][3]) {
     return m[0][0] * (m[1][1] * m[2][2] - m[1][2] * m[2][1]) - m[0][1] * (m[1][0] * m[2][2] - m[1][2] * m[2][0]) +

@@ -146,12 +146,16 @@ def mpjpe(pred, tgt):
 
 
 def p_mpjpe_per_frame(pred, tgt):
-    """loss.py:14-53 frame by frame (float64): Procrustes (scale, rotation, translation) then mean distance."""
+    """loss.py:14-53 frame by frame (float64): Procrustes (scale, rotation, translation) then mean distance.  A frame
+    with zero spread gives NaN (loss.py:30-31 divide by its zero norm; numpy's SVD then raises on the NaN matrix)."""
     out = []
     for Y, X in zip(np.asarray(pred, np.float64), np.asarray(tgt, np.float64)):
         muX, muY = X.mean(0), Y.mean(0)
         X0, Y0 = X - muX, Y - muY
         nX, nY = np.sqrt((X0 ** 2).sum()), np.sqrt((Y0 ** 2).sum())
+        if nX == 0 or nY == 0:
+            out.append(np.nan)
+            continue
         U, s, Vt = np.linalg.svd((X0 / nX).T @ (Y0 / nY))
         V = Vt.T
         if np.linalg.det(V @ U.T) < 0:                                   # :39-43
@@ -164,10 +168,19 @@ def p_mpjpe_per_frame(pred, tgt):
     return np.array(out)
 
 
-def adam_amsgrad_step(p, g, m, v, vmax, step, lr, b1=0.9, b2=0.999, eps=1e-8):
-    """torch/optim/adam.py single-tensor update with amsgrad=True (what trainval.py:78 constructs); float64."""
+def adam_step(p, g, m, v, vmax, step, lr, b1=0.9, b2=0.999, eps=1e-8, weight_decay=0.0, amsgrad=True):
+    """torch/optim/adam.py single-tensor update, in place, float64; amsgrad=True is what trainval.py:78 constructs.
+    weight_decay adds weight_decay * p to the gradient (L2, not decoupled); vmax is unused without amsgrad."""
+    if weight_decay != 0:
+        g = g + weight_decay * p
     m[:] = m + (1 - b1) * (g - m)
     v[:] = b2 * v + (1 - b2) * g * g
-    np.maximum(vmax, v, out=vmax)
+    if amsgrad:
+        np.maximum(vmax, v, out=vmax)
     bc1, bc2 = 1 - b1 ** step, 1 - b2 ** step
-    p[:] = p - (lr / bc1) * m / (np.sqrt(vmax) / np.sqrt(bc2) + eps)
+    p[:] = p - (lr / bc1) * m / (np.sqrt(vmax if amsgrad else v) / np.sqrt(bc2) + eps)
+
+
+def adam_amsgrad_step(p, g, m, v, vmax, step, lr, b1=0.9, b2=0.999, eps=1e-8):
+    """adam_step with amsgrad=True and no weight decay: what trainval.py:78 constructs."""
+    adam_step(p, g, m, v, vmax, step, lr, b1, b2, eps)

@@ -92,6 +92,27 @@ def test_adam_amsgrad(G):
         assert np.abs(p - G['adam_p%d' % i]).max() < 2e-6, i
 
 
+@pytest.mark.parametrize('wd', [0.0, 1e-2])
+@pytest.mark.parametrize('amsgrad', [True, False])
+def test_adam_step_matches_torch_adam(amsgrad, wd):
+    """the fp64 oracle against torch.optim.Adam itself (float64, CPU) with and without amsgrad and weight decay"""
+    import torch
+    rs = np.random.RandomState(5)
+    p0 = rs.standard_normal(300)
+    grads = [rs.standard_normal(300) * (10.0 if s == 1 else 0.1) for s in range(6)]
+    tp = torch.nn.Parameter(torch.from_numpy(p0.copy()))
+    opt = torch.optim.Adam([tp], lr=1e-3, weight_decay=wd, amsgrad=amsgrad)
+    p, m, v, vm = p0.copy(), np.zeros(300), np.zeros(300), np.zeros(300)
+    lr = 1e-3
+    for s, g in enumerate(grads):
+        tp.grad = torch.from_numpy(g.copy())
+        opt.step()
+        opt.param_groups[0]['lr'] *= 0.95
+        PO.adam_step(p, g, m, v, vm, s + 1, lr, weight_decay=wd, amsgrad=amsgrad)
+        lr *= 0.95
+    assert np.abs(tp.detach().numpy() - p).max() < 1e-13
+
+
 def test_oracle_vs_reference_random_configs():
     """The reference's own ChunkedGenerator / converters on random configurations (short videos, long chunks, causal
     shifts, ragged last batch), stored by tests/golden/make_golden_live.py: the oracle must match them bit for bit."""
