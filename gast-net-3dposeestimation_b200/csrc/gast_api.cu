@@ -19,6 +19,7 @@
 #include "gemm_tc.cuh"
 #include "kernels_hbm.cuh"
 #include "train_kernels.cuh"
+#include "wgrad_tc.cuh"
 #include "train_state.cuh"
 
 using namespace gast;
@@ -101,6 +102,9 @@ struct gast_handle {
   int gemm_core = 0;                 // 0 auto (tensor cores where possible), 1 force FFMA
   int precision = 0;                 // 0 fp32-grade (3xFP16 on scaled operands in inference, 3xTF32 in training),
                                      // 1 single-pass TF32 (inference only)
+  int train_precision = 0;           // training and every gradient: 0 fp32-grade, 1 single-pass TF32 (forward and
+                                     // input-gradient GEMMs) with the TF32 weight-gradient kernel (wgrad_tc.cuh)
+  int wgrad_tc_launches = 0;         // weight gradients of the last training call that ran on wgrad_tc_kernel
   // training: per-GEMM tensor-core operand copies (3xTF32), indexed by the GEMM's position in the step (train.cuh)
   std::vector<TcWeights> train_tc;
   // optional per-launch device timing (bench.py roofline): event pairs around every launch
@@ -307,7 +311,16 @@ extern "C" int gast_set_precision(gast_t* h, int32_t mode) {
   return 0;
 }
 
+extern "C" int gast_set_train_precision(gast_t* h, int32_t mode) {
+  if (!h) return fail("null handle");
+  if (mode != 0 && mode != 1)
+    return fail("gast_set_train_precision: mode must be 0 (fp32-grade) or 1 (tf32), got %d", mode);
+  h->train_precision = mode;
+  return 0;
+}
+
 extern "C" int32_t gast_last_launch_count(const gast_t* h) { return h ? h->launches : -1; }
+extern "C" int32_t gast_last_wgrad_tc_launch_count(const gast_t* h) { return h ? h->wgrad_tc_launches : -1; }
 extern "C" int32_t gast_last_tc_launch_count(const gast_t* h) { return h ? h->tc_launches : -1; }
 
 extern "C" int gast_set_timing(gast_t* h, int32_t on) {
@@ -638,7 +651,8 @@ static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p,
   if (p.N % 4 || p.ld_out % 4) return fail("internal: N/ld_out must be multiples of 4");
   if (h->gemm_core == 0 && tcw && tc_supported(p, epi, *tcw)) {
     TimedLaunch tl(h, st, LK_TC_PLAIN + epi);
-    int rc = tc_launch(st, epi, p, *tcw, tc_prec(*tcw, h->precision));
+    // training's operand copies (train_tcw, the only ones without the fp16 pair) run at the training precision
+    int rc = tc_launch(st, epi, p, *tcw, tc_prec(*tcw, tcw->f16 ? h->precision : h->train_precision));
     if (rc) return fail("tensor-core gemm launch failed: %s", cudaGetErrorString((cudaError_t)rc));
     h->launches++;
     h->tc_launches++;
@@ -996,9 +1010,10 @@ extern "C" int gast_bind_grads(gast_t* h, int32_t n, const char* const* keys, vo
   return 0;
 }
 
-// reduced precision is for inference: training and every gradient run at fp32 grade, and nothing falls back silently
+// The inference precision alone does not reach training: a handle at inference TF32 trains and differentiates only
+// once the training precision is TF32 too (gast_set_train_precision), and nothing falls back silently
 static int precision_check(gast_handle* h, const char* what) {
-  if (h->precision != 0)
+  if (h->precision != 0 && h->train_precision == 0)
     return fail("%s: reduced precision is inference-only; call gast_set_precision(h, 0) before training or "
                 "differentiating (precision is %d)", what, h->precision);
   return 0;
@@ -1041,6 +1056,7 @@ extern "C" int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B
   if (need == 0) return 1;
   if (!workspace || workspace_bytes < need) return fail("gast_forward_train: workspace too small (%zu < %zu)", workspace_bytes, need);
   h->launches = 0;
+  h->wgrad_tc_launches = 0;
   for (size_t i = 0; i < h->trains.size(); ++i)      // a workspace reused by the caller: its old state is dead
     if (h->trains[i].first == workspace) { h->trains.erase(h->trains.begin() + i); break; }
   if (h->trains.size() >= GAST_MAX_PENDING_TRAIN) h->trains.erase(h->trains.begin());   // forwards never differentiated
@@ -1124,6 +1140,7 @@ extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, fl
   TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
   c.pgrad = param_grads != 0;
   h->launches = 0;
+  h->wgrad_tc_launches = 0;
   if (train_forward(h, c, ts, x, nullptr, B, T)) return 1;
   c.tc_slot = 1024;
   if (train_backward(h, c, ts, dy, dx)) return 1;
@@ -1184,6 +1201,54 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
   cudaEventDestroy(e1);
   for (void* q : owned) cudaFree(q);
   if (rc || e != cudaSuccess) return fail("gast_debug_gemm: %s", cudaGetErrorString(rc ? (cudaError_t)rc : e));
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// debug / probe entry: dW[N,K] = dZ[M,N]^T . A[M,K] (dense leading dimensions) as the training backward computes a
+// weight gradient: dense_tn's row splits on this device, one kernel over them, the fixed-order reduction.  core 1:
+// wgrad_tn_kernel (FFMA, exact fp32; tc_mode 0).  core 0 with tc_mode 1: the kernel the TF32 training precision
+// picks, wgrad_tc_kernel where it takes the shape and wgrad_tn_kernel elsewhere.  There is no fp32-grade tensor-core
+// weight gradient, so core 0 with tc_mode 0 is refused.  reps > 0 times reps more runs of both kernels into *ms_out
+// (ms per run).
+// ------------------------------------------------------------------------------------------
+extern "C" int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int32_t M, int32_t N, int32_t K,
+                                int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (M <= 0 || N <= 0 || K <= 0) return fail("gast_debug_wgrad: bad shape");
+  if (core == 0 && tc_mode == 0)
+    return fail("gast_debug_wgrad: there is no fp32-grade tensor-core weight gradient (core 0 needs tc_mode 1)");
+  if (core < 0 || core > 1 || tc_mode < 0 || tc_mode > 1 || (core == 1 && tc_mode != 0))
+    return fail("gast_debug_wgrad: core must be 0 (tensor cores, tc_mode 1 = TF32) or 1 (FFMA, tc_mode 0)");
+  int dev = 0;
+  CUDA_OK(cudaGetDevice(&dev));
+  int sms = 0;
+  CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  long long S, rps;
+  wgrad_split(M, N, K, sms, &S, &rps);
+  float* part = nullptr;
+  CUDA_OK(cudaMalloc(&part, sizeof(float) * (size_t)S * N * K));
+  bool on_tc = false;
+  auto launch = [&]() { return wgrad_run(st, dZ, N, A, K, M, N, K, S, rps, part, dW, K, core == 0, &on_tc); };
+  cudaEvent_t e0, e1;
+  cudaEventCreate(&e0);
+  cudaEventCreate(&e1);
+  int rc = launch();
+  if (!rc && reps > 0) {
+    cudaEventRecord(e0, st);
+    for (int i = 0; i < reps && !rc; ++i) rc = launch();
+    cudaEventRecord(e1, st);
+  }
+  cudaError_t e = cudaStreamSynchronize(st);
+  if (!rc && e == cudaSuccess && reps > 0 && ms_out) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e0, e1);
+    *ms_out = ms / reps;
+  }
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  cudaFree(part);
+  if (rc || e != cudaSuccess) return fail("gast_debug_wgrad: %s", cudaGetErrorString(rc ? (cudaError_t)rc : e));
   return 0;
 }
 

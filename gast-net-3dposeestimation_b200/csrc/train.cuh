@@ -46,7 +46,8 @@ static bool want_grad(TCtx& c, const std::string& key, int64_t numel, float** ou
 // the weights change every step, so the hi/lo split runs per call; buffers live in a per-handle table indexed by the
 // GEMM's position in the step (the sequence of GEMMs of a model is fixed).  3xTF32 arithmetic (gemm_tc.cuh; inference
 // runs the equally precise F16X3 form), the arithmetic the gradient-noise bars of tests/test_gpu_train.py were set
-// against.  Shapes the core does not take (K % 16: the expand conv) stay on FFMA.
+// against; one TF32 product in the TF32 training precision (launch_gemm picks it from h->train_precision).  Shapes
+// the core does not take (K % 16: the expand conv) stay on FFMA.
 static const TcWeights* train_tcw(TCtx& c, const float* W, int N, int K) {
   const size_t slot = (size_t)c.tc_slot++;
   if (c.h->gemm_core != 0) return nullptr;
@@ -81,22 +82,48 @@ static int seg_gemm(TCtx& c, const ASeg* segs, int nseg, const float* W, int ldw
 
 static long long pad32(long long m) { return (m + 31) / 32 * 32; }
 
-// dW[N][K] = dZ[M][N]^T . A[M][K]: split over the rows (wgrad_tn_kernel) + fixed-order reduction of the partials
+// row splits *S of *rps rows each of the weight-gradient contraction over M rows: enough CTAs for two waves of the
+// machine, at least 256 rows per split
+static void wgrad_split(long long M, int N, int K, int sm_count, long long* S, long long* rps) {
+  const int tiles = (int)(cdiv(N, WG_T) * cdiv(K, WG_T));
+  long long s = std::max<long long>(1, std::min<long long>((M + 255) / 256, (2LL * sm_count + tiles - 1) / tiles));
+  const long long r = ((M + s - 1) / s + WG_M - 1) / WG_M * WG_M;
+  s = r > 0 ? (M + r - 1) / r : 1;
+  *S = s < 1 ? 1 : s;
+  *rps = r;
+}
+
+// the split contraction into part (S * N * K floats) and the fixed-order reduction of the partials into dW.  tf32:
+// wgrad_tc_kernel where it takes the shape (*on_tc = true), wgrad_tn_kernel (exact fp32) otherwise.  0 or a cudaError_t.
+static int wgrad_run(cudaStream_t st, const float* dZ, int lddz, const float* A, int lda, long long M, int N, int K,
+                     long long S, long long rps, float* part, float* dW, int lddw, bool tf32, bool* on_tc) {
+  *on_tc = tf32 && wgrad_tc_takes(dZ, lddz, N, K);
+  if (*on_tc) {
+    const int rc = wgrad_tc_launch(st, dZ, lddz, A, lda, M, N, K, rps, S, part);
+    if (rc) return rc;
+  } else {
+    dim3 grid(cdiv(N, WG_T), cdiv(K, WG_T), (unsigned)S);
+    wgrad_tn_kernel<<<grid, 256, 0, st>>>(dZ, lddz, A, lda, M, N, K, rps, part);
+  }
+  wgrad_reduce_kernel<<<cdiv((long long)N * K, 256), 256, 0, st>>>(part, (int)S, N, K, dW, lddw);
+  return (int)cudaGetLastError();
+}
+
+// dW[N][K] = dZ[M][N]^T . A[M][K]: split over the rows + fixed-order reduction of the partials (wgrad_run); on the
+// TF32 tensor-core kernel in the TF32 training precision on the tensor-core core
 static int dense_tn(TCtx& c, const float* dZ, int lddz, const float* A, int lda, long long M, int N, int K, float* dW,
                     int lddw) {
   if (!c.pgrad) return 0;   // every use is a parameter gradient
-  const int tiles = (int)(cdiv(N, WG_T) * cdiv(K, WG_T));
-  // enough CTAs for two waves of the machine, at least 256 rows per split
-  long long S = std::max<long long>(1, std::min<long long>((M + 255) / 256, (2LL * c.h->sm_count + tiles - 1) / tiles));
-  long long rps = ((M + S - 1) / S + WG_M - 1) / WG_M * WG_M;
-  S = (M + rps - 1) / rps;
-  if (S < 1) S = 1;
+  long long S, rps;
+  wgrad_split(M, N, K, c.h->sm_count, &S, &rps);
   float* part = c.fl((size_t)S * N * K);
   if (c.dry || M <= 0) return 0;
-  dim3 grid(cdiv(N, WG_T), cdiv(K, WG_T), (unsigned)S);
-  wgrad_tn_kernel<<<grid, 256, 0, c.st>>>(dZ, lddz, A, lda, M, N, K, rps, part);
-  wgrad_reduce_kernel<<<cdiv((long long)N * K, 256), 256, 0, c.st>>>(part, (int)S, N, K, dW, lddw);
+  bool on_tc = false;
+  const int rc = wgrad_run(c.st, dZ, lddz, A, lda, M, N, K, S, rps, part, dW, lddw,
+                           c.h->gemm_core == 0 && c.h->train_precision == 1, &on_tc);
+  if (rc) return fail("weight-gradient launch failed: %s", cudaGetErrorString((cudaError_t)rc));
   c.h->launches += 2;
+  if (on_tc) c.h->wgrad_tc_launches++;
   return 0;
 }
 

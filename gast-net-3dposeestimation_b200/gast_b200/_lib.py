@@ -17,7 +17,8 @@ KIND_MODEL, KIND_BLOCK, KIND_LOCAL, KIND_MGLOBAL, KIND_SEMCH, KIND_GLOBAL_HEAD =
 SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out_frames',
            'gast_receptive_field', 'gast_workspace_bytes', 'gast_forward', 'gast_forward_mpjpe',
            'gast_last_launch_count', 'gast_last_tc_launch_count', 'gast_set_timing',
-           'gast_get_timings', 'gast_set_gemm_core', 'gast_set_precision', 'gast_debug_gemm', 'gast_bind_grads',
+           'gast_get_timings', 'gast_set_gemm_core', 'gast_set_precision', 'gast_set_train_precision',
+           'gast_last_wgrad_tc_launch_count', 'gast_debug_gemm', 'gast_debug_wgrad', 'gast_bind_grads',
            'gast_train_workspace_bytes', 'gast_forward_train', 'gast_backward', 'gast_backward_input',
            'gast_eval_backward_workspace_bytes', 'gast_eval_backward', 'gast_set_dropout_state', 'gast_tta_prepare', 'gast_tta_merge',
            'gast_stream_state_bytes', 'gast_stream_workspace_bytes', 'gast_stream_push',
@@ -86,9 +87,16 @@ def load():
     lib.gast_set_gemm_core.restype = C.c_int
     lib.gast_set_precision.argtypes = [vp, C.c_int32]
     lib.gast_set_precision.restype = C.c_int
+    lib.gast_set_train_precision.argtypes = [vp, C.c_int32]
+    lib.gast_set_train_precision.restype = C.c_int
+    lib.gast_last_wgrad_tc_launch_count.argtypes = [vp]
+    lib.gast_last_wgrad_tc_launch_count.restype = C.c_int32
     lib.gast_debug_gemm.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                     C.POINTER(C.c_float), vp]
     lib.gast_debug_gemm.restype = C.c_int
+    lib.gast_debug_wgrad.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                     C.POINTER(C.c_float), vp]
+    lib.gast_debug_wgrad.restype = C.c_int
     lib.gast_bind_grads.argtypes = [vp, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(vp), C.POINTER(C.c_int64)]
     lib.gast_bind_grads.restype = C.c_int
     lib.gast_train_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32, C.c_float]

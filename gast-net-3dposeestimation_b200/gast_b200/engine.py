@@ -47,8 +47,30 @@ def get_precision(module):
     return module.__dict__.get('_gast_precision', 'fp32')
 
 
+def set_training_precision(module, mode):
+    """Arithmetic of training and of every gradient of `module` and its sub-modules: 'fp32' (default) is fp32-grade;
+    'tf32' runs every tensor-core GEMM of a train-mode forward, of the backward and of the eval-mode backward's
+    recompute as one TF32 product, and the weight gradients whose N and K are multiples of 32 on a TF32 tensor-core
+    kernel (DESIGN.md §4.3).  BatchNorm statistics, dropout and the remaining parameter gradients stay fp32; the
+    results repeat bit for bit run to run and across CUDA-graph replays in either mode.  With 'tf32' the model trains
+    and differentiates whatever set_precision says.  An eval-mode forward that builds an autograd graph is still the
+    inference forward, at the inference precision (set_precision); its backward recomputes the activations at this
+    precision.  Stored in each module's __dict__ like set_precision (DataParallel replicas and deepcopies keep it,
+    state_dict does not).  Returns the module."""
+    if mode not in _PRECISIONS:
+        raise GastError("set_training_precision: mode must be 'fp32' or 'tf32' (got %r)" % (mode,))
+    for m in module.modules():
+        m.__dict__['_gast_train_precision'] = mode
+    return module
+
+
+def get_training_precision(module):
+    """'fp32' or 'tf32' (set_training_precision)"""
+    return module.__dict__.get('_gast_train_precision', 'fp32')
+
+
 def _fp32_only(module, what):
-    if get_precision(module) != 'fp32':
+    if get_precision(module) != 'fp32' and get_training_precision(module) == 'fp32':
         raise GastError("%s: the model is set to TF32, which is inference-only; call "
                         "engine.set_precision(model, 'fp32') to train or differentiate it" % what)
 
@@ -149,6 +171,7 @@ class _Handle(object):
         self.ws = None
         self.core = None
         self.precision = 0
+        self.train_precision = 0
 
     def __del__(self):
         try:
@@ -159,8 +182,8 @@ class _Handle(object):
             pass
 
     def apply_core(self, module):
-        """hand the set_gemm_core() choice and the module's set_precision() to the library handle (every forward,
-        training or eval, and every stream push)"""
+        """hand the set_gemm_core() choice and the module's set_precision() and set_training_precision() to the
+        library handle (every forward, training or eval, and every stream push)"""
         if _FORCE_CORE['core'] != self.core:
             _check(self.lib.gast_set_gemm_core(self.h, _FORCE_CORE['core']), 'gast_set_gemm_core')
             self.core = _FORCE_CORE['core']
@@ -168,6 +191,10 @@ class _Handle(object):
         if prec != self.precision:
             _check(self.lib.gast_set_precision(self.h, prec), 'gast_set_precision')
             self.precision = prec
+        tprec = _PRECISIONS[get_training_precision(module)]
+        if tprec != self.train_precision:
+            _check(self.lib.gast_set_train_precision(self.h, tprec), 'gast_set_train_precision')
+            self.train_precision = tprec
 
     def refresh(self, module, stream):
         """(re)bind + prepare when any parameter/buffer moved or changed."""
@@ -237,6 +264,10 @@ class _Handle(object):
 
     def launches(self):
         return int(self.lib.gast_last_launch_count(self.h))
+
+    def wgrad_tc_launches(self):
+        """weight gradients of the last training step or eval backward that ran on the TF32 tensor-core kernel"""
+        return int(self.lib.gast_last_wgrad_tc_launch_count(self.h))
 
 
 def _require_cuda(x, what):

@@ -134,11 +134,29 @@ int gast_set_gemm_core(gast_t* h, int32_t core);
  *   1 = TF32: tf32(A) . tf32(W) with fp32 accumulation, one tensor-core product per multiply-add.  Operands are
  *       rounded to 10 mantissa bits (round to nearest, ties away), so outputs move by ~1e-3 relative
  *       (DESIGN.md §4.1).  Inference only: gast_forward_train, gast_backward(_input), gast_eval_backward and their
- *       workspace queries fail while it is set.
+ *       workspace queries fail while it is set, unless the training precision is TF32 too (gast_set_train_precision).
  * Any other value fails.  Everything else (expand, row-dots, the attention mix, shrink, GEMMs the tensor-core core
  * does not take, every GEMM under gast_set_gemm_core(h, 1)) stays fp32.  Like a core switch it needs no
  * gast_prepare, costs nothing and does not invalidate stream `state`. */
 int gast_set_precision(gast_t* h, int32_t mode);
+
+/* Arithmetic of training and of every gradient: gast_forward_train, gast_backward, gast_backward_input and
+ * gast_eval_backward (its recompute of the activations included):
+ *   0 = fp32-grade (default): 3xTF32 tensor-core GEMMs, weight gradients in exact fp32 (FFMA).
+ *   1 = TF32: every tensor-core GEMM (forward and input-gradient) is one TF32 product per multiply-add, and every
+ *       weight gradient whose N and K are multiples of 32 runs on a TF32 tensor-core kernel (wgrad_tc.cuh): operands
+ *       rounded to nearest tf32, fp32 accumulation, the same row splits and fixed-order reduction, so results repeat
+ *       bit for bit.  Gradients move by ~1e-3 relative (DESIGN.md §4.3).  The other weight gradients (the 8-wide
+ *       row-dot one, the expand conv's), BatchNorm statistics, dropout, the SemCH / attention parameter gradients, the
+ *       shrink and the expand stay fp32.
+ * Under gast_set_gemm_core(h, 1) everything stays fp32 FFMA in either mode.  While it is 0, a handle whose inference
+ * precision (gast_set_precision) is 1 refuses training; at 1 training runs whatever the inference precision.  Any
+ * other value fails.  Needs no gast_prepare, leaves no state behind and does not touch stream `state`. */
+int gast_set_train_precision(gast_t* h, int32_t mode);
+
+/* Number of weight gradients of the last gast_forward_train + gast_backward(_input) pair, or of the last
+ * gast_eval_backward, that ran on the TF32 tensor-core weight-gradient kernel. */
+int32_t gast_last_wgrad_tc_launch_count(const gast_t* h);
 
 /* ---- test-time augmentation around the forward (the caller-side steps of reconstruction.evaluate /
  * main.evaluate, kept on the device) -----------------------------------------------------------------
@@ -345,6 +363,16 @@ int gast_adam_step(const int64_t* table, int32_t n_chunks, float* exp_avg, float
  * (CUDA events) whose mean duration is written to *ms_out (host).  Synchronises the stream. */
 int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32_t N, int32_t K,
                     int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream);
+
+/* Test/probe entry (not on the training path): dW[N,K] = dZ[M,N]^T . A[M,K] (dense row-major operands) as the
+ * training backward computes a weight gradient: the same row splits on this device, one contraction kernel over
+ * them, the fixed-order reduction of the partials.  core 1 = the FFMA kernel (exact fp32, tc_mode 0); core 0 with
+ * tc_mode 1 = the kernel TF32 training runs: the TF32 tensor-core kernel where N % 32 == 0, K % 32 == 0 and dZ is
+ * 16-byte aligned, the FFMA kernel elsewhere.
+ * core 0 with tc_mode 0 fails: there is no fp32-grade tensor-core weight gradient.  Runs once, then `reps` timed
+ * runs whose mean duration (contraction + reduction) is written to *ms_out (host).  Synchronises the stream. */
+int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int32_t M, int32_t N, int32_t K,
+                     int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream);
 
 const char* gast_last_error(void);
 const char* gast_version(void);
