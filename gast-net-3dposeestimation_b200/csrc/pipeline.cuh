@@ -146,6 +146,203 @@ __global__ void kpt_convert_kernel(const float* __restrict__ kp, float* __restri
   if (valid) valid[t] = (np_pairwise_sum(o, Jo * 2) != 0.f) ? 1 : 0;
 }
 
+// ------------------------------------------------------------------------------------------
+// The video demo's keypoint repair and placement of the lifted persons (tools/preprocess.py), float32 in the
+// reference's order of operations, so results are bit-identical for float32 input.
+// ------------------------------------------------------------------------------------------
+constexpr int PREP_BLOCK = 256;
+__device__ __forceinline__ float np_minf(float a, float b) { return (isnan(a) || a < b) ? a : b; }   // np.amin: NaN wins
+
+// h36m_coco_format (preprocess.py:47-75): one thread per (person, frame).  Keypoints and valid mask as
+// kpt_convert_kernel mode 0; the scores remapped (:65-69); keep[p] = 1 once any coordinate of person p is non-zero
+// (keep is zeroed by the caller; every writer stores the same value).
+__global__ void h36m_coco_format_kernel(const float* __restrict__ kp, const float* __restrict__ sc, float* __restrict__ out,
+                                        float* __restrict__ sout, int* __restrict__ valid, int* __restrict__ keep, int P,
+                                        int T) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)P * T) return;
+  const float* k = kp + i * 34;
+  bool any = false;
+  for (int c = 0; c < 34; ++c) any |= (k[c] != 0.f);
+  if (any) keep[i / T] = 1;
+  float o[34];
+  coco_to_h36m_frame(k, 2, o);
+  float* op = out + i * 34;
+  for (int c = 0; c < 34; ++c) op[c] = o[c];
+  valid[i] = (np_pairwise_sum(o, 34) != 0.f) ? 1 : 0;
+  const float* s = sc + i * 17;
+  float n[17];
+  const int h36m_coco_order[13] = {9, 11, 14, 12, 15, 13, 16, 4, 1, 5, 2, 6, 3};
+  const int coco_order[13] = {0, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16};
+#pragma unroll
+  for (int q = 0; q < 13; ++q) n[h36m_coco_order[q]] = s[coco_order[q]];
+  n[0] = __fdiv_rn(__fadd_rn(s[11], s[12]), 2.f);
+  n[8] = __fdiv_rn(__fadd_rn(s[5], s[6]), 2.f);
+  n[7] = __fdiv_rn(__fadd_rn(n[0], n[8]), 2.f);
+  n[10] = __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(s[1], s[2]), s[3]), s[4]), 4.f);
+  float* so = sout + i * 17;
+#pragma unroll
+  for (int q = 0; q < 17; ++q) so[q] = n[q];
+}
+
+// revise_kpts (preprocess.py:78-112): one thread per (person, frame).  Zero outside the valid frames; at a valid
+// frame the pose, with the low-confidence limb joints replaced by the first matching case of :94-109 (every right-hand
+// side read before the assignment, as numpy's fancy indexing does).  low joints: score < float32(0.3).
+__global__ void revise_kpts_kernel(const float* __restrict__ kp, const float* __restrict__ sc, const int* __restrict__ mask,
+                                   float* __restrict__ out, long long PT, int J) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= PT) return;
+  const float2* k = reinterpret_cast<const float2*>(kp) + i * J;
+  float2* o = reinterpret_cast<float2*>(out) + i * J;
+  if (!mask[i]) {
+    for (int j = 0; j < J; ++j) o[j] = make_float2(0.f, 0.f);
+    return;
+  }
+  for (int j = 0; j < J; ++j) o[j] = k[j];
+  const float* s = sc + i * J;
+  const int low = (s[2] < 0.3f ? 1 : 0) | (s[3] < 0.3f ? 2 : 0) | (s[5] < 0.3f ? 4 : 0) | (s[6] < 0.3f ? 8 : 0);
+  const float2 k1 = k[1], k2 = k[2], k4 = k[4], k5 = k[5];
+  switch (low) {
+    case 15: o[2] = k1; o[3] = k1; o[5] = k4; o[6] = k4; break;   // [2, 3, 5, 6] <- [1, 1, 4, 4]
+    case 11: o[2] = k1; o[3] = k1; o[6] = k5; break;              // [2, 3, 6] <- [1, 1, 5]
+    case 14: o[3] = k2; o[5] = k4; o[6] = k4; break;              // [3, 5, 6] <- [2, 4, 4]
+    case 10: o[3] = k2; o[6] = k5; break;                         // [3, 6] <- [2, 5]
+    case 2: o[3] = k2; break;                                     // 3 <- 2
+    case 8: o[6] = k5; break;                                     // 6 <- 5
+    default: break;                                               // any other combination: unchanged
+  }
+}
+
+// mean over joints [1, 4, 11, 14] of (a - b) (b may be null = 0), channel c of rows with D floats per joint:
+// float32, left to right, then / 4 (np.mean over a 4-row axis)
+__device__ __forceinline__ float limb_mean(const float* a, const float* b, int D, int c) {
+  const int jj[4] = {1, 4, 11, 14};
+  float s = 0.f;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float v = b ? __fsub_rn(a[jj[q] * D + c], b[jj[q] * D + c]) : a[jj[q] * D + c];
+    s = q == 0 ? v : __fadd_rn(s, v);
+  }
+  return __fdiv_rn(s, 4.f);
+}
+
+// revise_skes, two persons (:138-141): the first entry k of person 0's frames that person 1 also has (mask1 = person
+// 1's valid mask); per block the smallest such k, INT_MAX when none.
+__global__ void first_common_kernel(const long long* __restrict__ frames0, int F0, const int* __restrict__ mask1,
+                                    int* __restrict__ part) {
+  int best = INT_MAX;
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < F0; k += gridDim.x * blockDim.x)
+    if (mask1[frames0[k]]) best = min(best, k);
+  for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+  __shared__ int sh[PREP_BLOCK / 32];
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = best;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 0; w < PREP_BLOCK / 32; ++w) best = min(best, sh[w]);
+    part[blockIdx.x] = best;
+  }
+}
+
+__global__ void mask_scatter_kernel(const long long* __restrict__ frames, int F, int* __restrict__ mask) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < F) mask[frames[k]] = 1;
+}
+
+// revise_skes (:123-147): grid.y = person; one thread per (packed row, joint) of that person.  Scatters the packed
+// prediction row k to frame frames[k]; rows after the first move by the limb-mean 2D displacement from the first
+// valid frame / 500 (:130-133); with two persons both move by half their limb-mean distance at the first common frame
+// (:138-147; ncommon_part blocks of first_common_kernel partials, NaN poses when there is no common frame).
+// out must be zero.
+__global__ void revise_skes_kernel(const float* __restrict__ pred, const long long* __restrict__ frames,
+                                   const long long* __restrict__ off, const float* __restrict__ kp, float* __restrict__ out,
+                                   int T, int J, int D, const int* __restrict__ common_part, int ncommon_part) {
+  const int p = blockIdx.y;
+  const long long o0 = off[p], F = off[p + 1] - o0;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= F * J) return;
+  const long long k = i / J;
+  const int j = (int)(i - k * J);
+  const float* r = pred + ((o0 + k) * J + j) * 3;
+  float x = r[0], y = r[1];
+  const float z = r[2];
+  const long long t = frames[o0 + k];
+  const float* kpp = kp + (long long)p * T * J * D;
+  if (k > 0) {
+    const float* a = kpp + t * J * D;
+    const float* b = kpp + frames[o0] * J * D;
+    x = __fsub_rn(x, __fdiv_rn(limb_mean(a, b, D, 0), 500.f));
+    y = __fadd_rn(y, __fdiv_rn(limb_mean(a, b, D, 1), 500.f));
+  }
+  if (common_part) {
+    int kc = INT_MAX;
+    for (int q = 0; q < ncommon_part; ++q) kc = min(kc, common_part[q]);
+    if (kc == INT_MAX) {
+      x = y = __int_as_float(0x7fc00000);
+    } else {
+      const long long tc = frames[off[0] + kc];
+      const float* a = kp + tc * J * D;                       // person 0
+      const float* b = kp + ((long long)T + tc) * J * D;      // person 1
+      const float ax = __fdiv_rn(__fdiv_rn(limb_mean(a, b, D, 0), 2.f), 500.f);
+      const float ay = __fdiv_rn(__fdiv_rn(limb_mean(a, b, D, 1), 2.f), 500.f);
+      x = p == 0 ? __fsub_rn(x, ax) : __fadd_rn(x, ax);
+      y = p == 0 ? __fadd_rn(y, ay) : __fsub_rn(y, ay);
+    }
+  }
+  float* w = out + (((long long)p * T + t) * J + j) * 3;
+  w[0] = x; w[1] = y; w[2] = z;
+}
+
+// pass 1 of z -= amin(z): per block the NaN-propagating minimum of x[3 i + 2], i < n
+__global__ void zmin_partial_kernel(const float* __restrict__ x, long long n, float* __restrict__ part) {
+  float m = INFINITY;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    m = np_minf(x[3 * i + 2], m);
+  for (int o = 16; o > 0; o >>= 1) m = np_minf(__shfl_xor_sync(0xffffffffu, m, o), m);
+  __shared__ float sh[PREP_BLOCK / 32];
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 0; w < PREP_BLOCK / 32; ++w) m = np_minf(sh[w], m);
+    part[blockIdx.x] = m;
+  }
+}
+
+// pass 2: every block finishes the minimum from the nb partials in the same order, then x[3 i + 2] -= min
+__global__ void zmin_subtract_kernel(float* __restrict__ x, long long n, const float* __restrict__ part, int nb) {
+  __shared__ float zmin;
+  if (threadIdx.x == 0) {
+    float m = part[0];
+    for (int q = 1; q < nb; ++q) m = np_minf(part[q], m);
+    zmin = m;
+  }
+  __syncthreads();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    x[3 * i + 2] = __fsub_rn(x[3 * i + 2], zmin);
+}
+
+// revise_skes_real_time (:158-172), one thread per (person, joint): x -= (m_x - cx) / r, y += (m_y - cy) / r with m the
+// limb mean of the person's 2D keypoints (J = 17, D floats per keypoint), and the per-block minimum of z
+__global__ void revise_rt_kernel(const float* __restrict__ pred, const float* __restrict__ kp, float* __restrict__ out, int M,
+                                 int D, float cx, float cy, float r, float* __restrict__ part) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  float z = INFINITY;
+  if (i < M * 17) {
+    const float* a = kp + (long long)(i / 17) * 17 * D;
+    const float x = __fsub_rn(pred[3 * i], __fdiv_rn(__fsub_rn(limb_mean(a, nullptr, D, 0), cx), r));
+    const float y = __fadd_rn(pred[3 * i + 1], __fdiv_rn(__fsub_rn(limb_mean(a, nullptr, D, 1), cy), r));
+    z = pred[3 * i + 2];
+    out[3 * i] = x; out[3 * i + 1] = y; out[3 * i + 2] = z;
+  }
+  for (int o = 16; o > 0; o >>= 1) z = np_minf(__shfl_xor_sync(0xffffffffu, z, o), z);
+  __shared__ float sh[PREP_BLOCK / 32];
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = z;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 0; w < PREP_BLOCK / 32; ++w) z = np_minf(sh[w], z);
+    part[blockIdx.x] = z;
+  }
+}
+
 // normalize_screen_coordinates (common/camera.py:8-12): X/w*2 - [1, h/w].  numpy evaluates X/w*2 in
 // float32 and the subtraction of the Python-float list in float64; the result is rounded to float32
 // here (callers cast it: reconstruction.py:143, main.py:46).   image_coordinates (:15-19) is the inverse.
@@ -462,6 +659,107 @@ extern "C" int gast_adam_step(const int64_t* table, int32_t n_chunks, float* exp
   adam_multi_kernel<<<n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const long long*>(table), exp_avg, exp_avg_sq, max_exp_avg_sq, (float)(1.0 - beta1), (float)beta2,
       (float)(1.0 - beta2), (float)(lr / bc1), (float)sqrt(bc2), (float)eps, (float)weight_decay);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gast_h36m_coco_format(const float* kpts, const float* scores, int32_t P, int32_t T, float* out_kpts,
+                                     float* out_scores, int32_t* valid, int32_t* keep, void* stream) {
+  if (!kpts || !scores || !out_kpts || !out_scores || !valid || !keep || P <= 0 || T <= 0)
+    return fail("gast_h36m_coco_format: bad arguments");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CUDA_OK(cudaMemsetAsync(keep, 0, sizeof(int32_t) * P, st));
+  h36m_coco_format_kernel<<<cdiv((long long)P * T, 128), 128, 0, st>>>(kpts, scores, out_kpts, out_scores, valid, keep, P, T);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gast_revise_kpts(const float* kpts, const float* scores, const int32_t* valid, int32_t P, int32_t T, int32_t J,
+                                float* out, void* stream) {
+  if (!kpts || !scores || !valid || !out || P <= 0 || T <= 0 || J < 7) return fail("gast_revise_kpts: bad arguments (J >= 7)");
+  const long long PT = (long long)P * T;
+  revise_kpts_kernel<<<cdiv(PT, 128), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(kpts, scores, valid, out, PT, J);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+namespace gast {
+constexpr int PREP_COMMON_BLOCKS = 64, PREP_ZMIN_BLOCKS = 512;
+static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+}  // namespace gast
+
+extern "C" size_t gast_revise_skes_workspace_bytes(int32_t P, int32_t T) {
+  if (P <= 0 || T <= 0) return 0;
+  return align256(sizeof(int64_t) * (P + 1)) + align256(sizeof(int32_t) * (size_t)T) +
+         align256(sizeof(int32_t) * PREP_COMMON_BLOCKS) + align256(sizeof(float) * PREP_ZMIN_BLOCKS);
+}
+
+extern "C" int gast_revise_skes(const float* pred, const int64_t* frames, const int64_t* offsets, int32_t P, int32_t T,
+                                int32_t J, int32_t D, const float* kpts, float* out, void* workspace, size_t workspace_bytes,
+                                void* stream) {
+  if (!pred || !frames || !offsets || !kpts || !out || !workspace || P <= 0 || T <= 0 || J < 15 || D < 2)
+    return fail("gast_revise_skes: bad arguments (J >= 15, D >= 2)");
+  if (workspace_bytes < gast_revise_skes_workspace_bytes(P, T))
+    return fail("gast_revise_skes: workspace of %zu bytes, %zu needed", workspace_bytes, gast_revise_skes_workspace_bytes(P, T));
+  long long maxF = 0;
+  for (int p = 0; p < P; ++p) {
+    const long long F = offsets[p + 1] - offsets[p];
+    if (offsets[0] != 0 || F < 0 || F > T) return fail("gast_revise_skes: person %d has %lld frames, T = %d", p, F, T);
+    maxF = std::max(maxF, F);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  char* ws = reinterpret_cast<char*>(workspace);
+  long long* doff = reinterpret_cast<long long*>(ws);
+  ws += align256(sizeof(int64_t) * (P + 1));
+  int* mask1 = reinterpret_cast<int*>(ws);
+  ws += align256(sizeof(int32_t) * (size_t)T);
+  int* cpart = reinterpret_cast<int*>(ws);
+  ws += align256(sizeof(int32_t) * PREP_COMMON_BLOCKS);
+  float* zpart = reinterpret_cast<float*>(ws);
+  CUDA_OK(cudaMemcpyAsync(doff, offsets, sizeof(int64_t) * (P + 1), cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)P * T * J * 3, st));
+  const long long* fr = reinterpret_cast<const long long*>(frames);
+  const int* common = nullptr;
+  int ncommon = 0;
+  if (P == 2) {                                           // preprocess.py:138-141
+    const long long F0 = offsets[1], F1 = offsets[2] - offsets[1];
+    CUDA_OK(cudaMemsetAsync(mask1, 0, sizeof(int32_t) * (size_t)T, st));
+    if (F1 > 0) mask_scatter_kernel<<<cdiv(F1, 256), 256, 0, st>>>(fr + F0, (int)F1, mask1);
+    ncommon = (int)std::max<long long>(1, std::min<long long>(PREP_COMMON_BLOCKS, cdiv(F0, PREP_BLOCK)));
+    first_common_kernel<<<ncommon, PREP_BLOCK, 0, st>>>(fr, (int)F0, mask1, cpart);
+    common = cpart;
+  }
+  if (maxF > 0) {
+    dim3 grid(cdiv(maxF * J, 128), P);
+    revise_skes_kernel<<<grid, 128, 0, st>>>(pred, fr, doff, kpts, out, T, J, D, common, ncommon);
+  }
+  const long long n = (long long)P * T * J;                // preprocess.py:153, over the whole output
+  const int nb = (int)std::min<long long>(PREP_ZMIN_BLOCKS, cdiv(n, PREP_BLOCK));
+  zmin_partial_kernel<<<nb, PREP_BLOCK, 0, st>>>(out, n, zpart);
+  zmin_subtract_kernel<<<nb, PREP_BLOCK, 0, st>>>(out, n, zpart, nb);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" size_t gast_revise_skes_real_time_workspace_bytes(int32_t M) {
+  return M > 0 ? sizeof(float) * cdiv((long long)M * 17, PREP_BLOCK) : 0;
+}
+
+extern "C" int gast_revise_skes_real_time(const float* pred, const float* kpts, int32_t M, int32_t J, int32_t D, double width,
+                                          float* out, void* workspace, size_t workspace_bytes, void* stream) {
+  if (J != 17) return fail("gast_revise_skes_real_time: the reference places 17 joints, got %d", J);
+  if (!pred || !kpts || !out || !workspace || M <= 0 || D < 2) return fail("gast_revise_skes_real_time: bad arguments");
+  if (workspace_bytes < gast_revise_skes_real_time_workspace_bytes(M))
+    return fail("gast_revise_skes_real_time: workspace of %zu bytes, %zu needed", workspace_bytes,
+                gast_revise_skes_real_time_workspace_bytes(M));
+  // preprocess.py:159,167-168 under NumPy 2's promotion: the Python-float constants are rounded to float32 and every
+  // operation is float32
+  const float cx = (float)(3.0 * width / 5.0), cy = (float)(width / 5.0), r = (float)(500.0 * (width / 1920.0));
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int nb = (int)cdiv((long long)M * 17, PREP_BLOCK);
+  float* part = reinterpret_cast<float*>(workspace);
+  revise_rt_kernel<<<nb, PREP_BLOCK, 0, st>>>(pred, kpts, out, M, D, cx, cy, r, part);
+  zmin_subtract_kernel<<<nb, PREP_BLOCK, 0, st>>>(out, (long long)M * 17, part, nb);
   CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -24,7 +24,9 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_stream_state_bytes', 'gast_stream_workspace_bytes', 'gast_stream_push',
            'gast_stream_latency', 'gast_stream_push_ex', 'gast_stream_chunk_workspace_bytes', 'gast_stream_push_chunk',
            'gast_stream_peek', 'gast_stream_subset_workspace_bytes', 'gast_stream_push_subset', 'gast_stream_peek_subset',
-           'gast_chunk_gather', 'gast_keypoints_convert', 'gast_normalize_screen', 'gast_camera_to_world',
+           'gast_chunk_gather', 'gast_keypoints_convert', 'gast_h36m_coco_format', 'gast_revise_kpts',
+           'gast_revise_skes_workspace_bytes', 'gast_revise_skes', 'gast_revise_skes_real_time_workspace_bytes',
+           'gast_revise_skes_real_time', 'gast_normalize_screen', 'gast_camera_to_world',
            'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_adam_chunk', 'gast_adam_step',
            'gast_last_error', 'gast_version']
 
@@ -148,6 +150,19 @@ def load():
     lib.gast_chunk_gather.restype = C.c_int
     lib.gast_keypoints_convert.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp]
     lib.gast_keypoints_convert.restype = C.c_int
+    lib.gast_h36m_coco_format.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp]
+    lib.gast_h36m_coco_format.restype = C.c_int
+    lib.gast_revise_kpts.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp]
+    lib.gast_revise_kpts.restype = C.c_int
+    lib.gast_revise_skes_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
+    lib.gast_revise_skes_workspace_bytes.restype = C.c_size_t
+    lib.gast_revise_skes.argtypes = [vp, vp, C.POINTER(C.c_int64), C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp,
+                                     C.c_size_t, vp]
+    lib.gast_revise_skes.restype = C.c_int
+    lib.gast_revise_skes_real_time_workspace_bytes.argtypes = [C.c_int32]
+    lib.gast_revise_skes_real_time_workspace_bytes.restype = C.c_size_t
+    lib.gast_revise_skes_real_time.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, vp, vp, C.c_size_t, vp]
+    lib.gast_revise_skes_real_time.restype = C.c_int
     lib.gast_normalize_screen.argtypes = [vp, vp, C.c_int64, C.c_float, C.c_float, C.c_int32, vp]
     lib.gast_normalize_screen.restype = C.c_int
     lib.gast_camera_to_world.argtypes = [vp, vp, C.c_int64, fp, fp, vp]

@@ -129,6 +129,98 @@ def camera_to_world(x, R, t=0):
 
 
 # ------------------------------------------------------------------------------------------------
+# The video demo's keypoint repair and placement of the lifted persons (tools/preprocess.py)
+# ------------------------------------------------------------------------------------------------
+_PREP_WS = {}
+
+
+def _prep_ws(dev, nbytes):
+    """scratch for the placement minima, grown on demand and kept per device"""
+    ws = _PREP_WS.get(dev)
+    if ws is None or ws.numel() < nbytes:
+        ws = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
+        _PREP_WS[dev] = ws
+    return ws
+
+
+def h36m_coco_format(kpts, scores):
+    """preprocess.py:47-75 over every person slot: kpts (P,T,17,2), scores (P,T,17) -> (H36M keypoints (P,T,17,2),
+    H36M scores (P,T,17), valid mask (P,T) int32, keep (P,) int32).  The caller drops the slots whose keep is 0."""
+    k = _cuda_f32(kpts, 'h36m_coco_format')
+    s = _cuda_f32(scores, 'h36m_coco_format')
+    if k.dim() != 4 or tuple(k.shape[2:]) != (17, 2) or tuple(s.shape) != tuple(k.shape[:3]):
+        raise GastError('h36m_coco_format: kpts (P,T,17,2) and scores (P,T,17) expected, got %s and %s'
+                        % (tuple(k.shape), tuple(s.shape)))
+    P, T = int(k.shape[0]), int(k.shape[1])
+    dev = k.device
+    out = torch.empty_like(k)
+    sout = torch.empty_like(s)
+    valid = torch.empty((P, T), dtype=torch.int32, device=dev)
+    keep = torch.empty((P,), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _check(L.load().gast_h36m_coco_format(_p(k), _p(s), P, T, _p(out), _p(sout), _p(valid), _p(keep),
+                                              C.c_void_p(_stream(dev))), 'gast_h36m_coco_format')
+    return out, sout, valid, keep
+
+
+def revise_kpts(kpts, scores, valid):
+    """preprocess.py:78-112: kpts (P,T,J,2), scores (P,T,J), valid (P,T) int32 mask -> repaired kpts (P,T,J,2)."""
+    k = _cuda_f32(kpts, 'revise_kpts')
+    s = _cuda_f32(scores, 'revise_kpts')
+    if k.dim() != 4 or k.shape[-1] != 2 or tuple(s.shape) != tuple(k.shape[:3]) or tuple(valid.shape) != tuple(k.shape[:2]):
+        raise GastError('revise_kpts: kpts (P,T,J,2), scores (P,T,J) and valid (P,T) expected')
+    v = valid.to(torch.int32).contiguous()
+    P, T, J = (int(d) for d in k.shape[:3])
+    out = torch.empty_like(k)
+    with torch.cuda.device(k.device):
+        _check(L.load().gast_revise_kpts(_p(k), _p(s), _p(v), P, T, J, _p(out), C.c_void_p(_stream(k.device))),
+               'gast_revise_kpts')
+    return out
+
+
+def revise_skes(pred, frames, offsets, kpts):
+    """preprocess.py:123-155: pred (N,J,3) every person's prediction packed (person p at rows offsets[p] ..
+    offsets[p+1]-1; offsets a host sequence of P+1 ints), frames (N,) CUDA int64 the frame of each row, kpts (P,T,J,D)
+    -> (P,T,J,3).  Two persons without a common frame get NaN x and y (the caller checks host frame lists)."""
+    pr = _cuda_f32(pred, 'revise_skes')
+    k = _cuda_f32(kpts, 'revise_skes')
+    fr = frames.contiguous()
+    off = np.ascontiguousarray(offsets, dtype=np.int64)
+    if k.dim() != 4 or pr.dim() != 3 or pr.shape[-1] != 3 or pr.shape[1] != k.shape[2] or fr.dtype != torch.int64 \
+            or not fr.is_cuda or off.shape != (k.shape[0] + 1,) or int(off[-1]) != pr.shape[0] or fr.numel() != pr.shape[0]:
+        raise GastError('revise_skes: pred (N,J,3), frames (N,) CUDA int64, offsets (P+1,) and kpts (P,T,J,D) expected')
+    P, T, J, D = (int(d) for d in k.shape)
+    dev = k.device
+    out = torch.empty((P, T, J, 3), dtype=torch.float32, device=dev)
+    lib = L.load()
+    wb = int(lib.gast_revise_skes_workspace_bytes(P, T))
+    with torch.cuda.device(dev):
+        ws = _prep_ws(dev, wb)
+        _check(lib.gast_revise_skes(_p(pr), _p(fr), off.ctypes.data_as(C.POINTER(C.c_int64)), P, T, J, D, _p(k), _p(out),
+                                    _p(ws), ws.numel(), C.c_void_p(_stream(dev))), 'gast_revise_skes')
+    return out
+
+
+def revise_skes_real_time(pred, kpts, width):
+    """preprocess.py:158-172: pred (M,17,3), kpts (M,17,D) of one tick, image width -> placed poses (M,17,3)."""
+    pr = _cuda_f32(pred, 'revise_skes_real_time')
+    k = _cuda_f32(kpts, 'revise_skes_real_time')
+    if pr.dim() != 3 or pr.shape[-1] != 3 or k.dim() != 3 or k.shape[0] != pr.shape[0] or k.shape[1] != pr.shape[1]:
+        raise GastError('revise_skes_real_time: pred (M,17,3) and kpts (M,17,D) expected, got %s and %s'
+                        % (tuple(pr.shape), tuple(k.shape)))
+    M, J, D = int(pr.shape[0]), int(pr.shape[1]), int(k.shape[2])
+    dev = pr.device
+    out = torch.empty_like(pr)
+    lib = L.load()
+    wb = int(lib.gast_revise_skes_real_time_workspace_bytes(M))
+    with torch.cuda.device(dev):
+        ws = _prep_ws(dev, wb)
+        _check(lib.gast_revise_skes_real_time(_p(pr), _p(k), M, J, D, float(width), _p(out), _p(ws), ws.numel(),
+                                              C.c_void_p(_stream(dev))), 'gast_revise_skes_real_time')
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # N2: losses and the optimiser step
 # ------------------------------------------------------------------------------------------------
 _WS = {}

@@ -331,6 +331,46 @@ int gast_chunk_gather(const float* poses_2d, const float* poses_3d, const float*
 int gast_keypoints_convert(const float* kpts, float* out, int32_t* valid, int32_t T, int32_t J_in, int32_t mode,
                            void* stream);
 
+/* The video demo's keypoint repair and placement of the lifted persons (tools/preprocess.py), float32 in the
+ * reference's order of operations: bit-identical to it for float32 input.  Minima are taken in two deterministic
+ * passes (per-block partials, then a fixed-order finish), so results repeat bit for bit.
+ *
+ * gast_h36m_coco_format (preprocess.py:47-75): kpts (P,T,17,2) COCO keypoints and scores (P,T,17) of P person slots ->
+ *   out_kpts (P,T,17,2) H36M keypoints and valid (P,T) as gast_keypoints_convert mode 0 (:61), out_scores (P,T,17) the
+ *   H36M scores (:65-69), keep (P) = 1 where the slot holds a person.  The reference keeps a slot when np.sum(kpts) != 0
+ *   (:60); here when some coordinate is non-zero.  The two differ only when non-zero coordinates cancel to exactly 0,
+ *   which needs negative pixel coordinates.  The caller drops the slots with keep = 0. */
+int gast_h36m_coco_format(const float* kpts, const float* scores, int32_t P, int32_t T, float* out_kpts, float* out_scores,
+                          int32_t* valid, int32_t* keep, void* stream);
+
+/* gast_revise_kpts (preprocess.py:78-112): kpts (P,T,J,2), scores (P,T,J), valid (P,T) int32 mask of each person's
+ *   valid frames -> out (P,T,J,2): zero outside the valid frames; at a valid frame the pose with the low-confidence
+ *   joints among [2, 3, 5, 6] (score < float32(0.3)) replaced as :96-107 do. */
+int gast_revise_kpts(const float* kpts, const float* scores, const int32_t* valid, int32_t P, int32_t T, int32_t J,
+                     float* out, void* stream);
+
+/* gast_revise_skes (preprocess.py:123-155): pred (sum F_p, J, 3) = every person's prediction packed, person p at rows
+ *   offsets[p] .. offsets[p+1]-1 (offsets (host), P+1 entries, offsets[0] = 0); frames (sum F_p) int64 = the frame of
+ *   each row (the reference's valid_frames, concatenated); kpts (P,T,J,D) the repaired 2D keypoints (D >= 2, J >= 15)
+ *   -> out (P,T,J,3): zero, each row scattered to its frame, moved in x/y by the joint [1,4,11,14] mean displacement
+ *   from the person's first frame / 500 (:130-133); with P = 2 both persons moved apart by half their mean distance at
+ *   the first frame of person 0 that person 1 also has (:138-147); then z -= min z over the whole output (:153), zero
+ *   rows of missing frames included (so the minimum is <= 0 as soon as a person misses a frame, as in the reference).
+ *   The first and common frames are found on the device.  Two persons without a common frame, where the reference
+ *   raises ValueError, get NaN x and y.  workspace: gast_revise_skes_workspace_bytes(P, T) bytes. */
+size_t gast_revise_skes_workspace_bytes(int32_t P, int32_t T);
+int gast_revise_skes(const float* pred, const int64_t* frames, const int64_t* offsets, int32_t P, int32_t T, int32_t J,
+                     int32_t D, const float* kpts, float* out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* gast_revise_skes_real_time (preprocess.py:158-172): pred (M,17,3) and kpts (M,17,D) of one tick -> out (M,17,3):
+ *   x -= (m_x - 3 width/5) / r, y += (m_y - width/5) / r with m the joint [1,4,11,14] mean of the person's keypoints and
+ *   r = 500 width/1920, then z -= min z over all M persons.  The constants are computed in double and rounded to
+ *   float32, every other step is float32 (NumPy 2 promotion of the reference's Python-float constants).  J != 17 fails,
+ *   as the reference hard-codes 17 joints.  workspace: gast_revise_skes_real_time_workspace_bytes(M) bytes. */
+size_t gast_revise_skes_real_time_workspace_bytes(int32_t M);
+int gast_revise_skes_real_time(const float* pred, const float* kpts, int32_t M, int32_t J, int32_t D, double width, float* out,
+                               void* workspace, size_t workspace_bytes, void* stream);
+
 /* common/camera.py:8-19: normalize_screen_coordinates (inverse = 0) / image_coordinates (inverse = 1) on
  * n_points (x,y) pairs. */
 int gast_normalize_screen(const float* x, float* out, int64_t n_points, float w, float h, int32_t inverse, void* stream);
