@@ -286,21 +286,30 @@ extern "C" int32_t gast_stream_latency(const gast_t* h) {
   return h->cfg.causal ? 0 : (gast_receptive_field(h) - 1) / 2;
 }
 
+// The start of every streaming call once its own checks passed: the handle's weights must be prepared; then its device
+// is made current and the launch counters restart for this call.
+static int stream_call_begin(gast_handle* h, const char* who) {
+  if (!h->prepared) return fail("%s: gast_prepare() has not run since the last gast_bind()", who);
+  CUDA_OK(cudaSetDevice(h->cfg.device));
+  h->launches = h->tc_launches = 0;
+  h->ev_used = 0;
+  h->ev_kind.clear();
+  return 0;
+}
+
 extern "C" int gast_stream_push_ex(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
                                    const int32_t* fresh, const int32_t* hold, void* workspace, size_t workspace_bytes,
                                    void* stream) {
   if (!h) return fail("gast_stream_push_ex: null handle");
-  if (!h->prepared) return fail("gast_stream_push_ex: gast_prepare() has not run since the last gast_bind()");
   if (step < 0 || !state || !x || !y) return fail("gast_stream_push_ex: bad arguments");
   StreamPlan sp;
   if (stream_plan(h, n_streams, &sp)) return 1;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
-  if (!h->stream_ready && stream_prepare(h, st)) return 1;
   const size_t need = gast_stream_workspace_bytes(h, n_streams);
   if (!workspace || workspace_bytes < need)
     return fail("gast_stream_push_ex: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
-  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
+  if (stream_call_begin(h, "gast_stream_push_ex")) return 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (!h->stream_ready && stream_prepare(h, st)) return 1;
   const gast_cfg& c = h->cfg;
   const int n = n_streams, J = c.num_joints, C = c.channels, L = c.num_stages, k0 = c.filter_widths[0], Fin = c.in_features;
   float* sbase = reinterpret_cast<float*>(align256(state));
@@ -363,41 +372,38 @@ extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const floa
 // weights Wt and the row map of the whole-sequence forward (taps d*J*Cw floats apart, residual at the newest or the
 // centre tap), and every ring slot is then given the input of the latest time it stands for, so that the next push
 // (single or chunk) finds the history it expects.  The blocks are pointwise in time and run on n*K frames.
-struct ChunkBufs { float *xin, *G; StreamBufs sb; };
+struct ChunkBufs { float *xin, *G; StreamBufs sb; int32_t* tab; };
 
-static int chunk_bufs(const gast_handle* h, const StreamPlan& sp, int K, Arena& a, ChunkBufs* cb) {
+// The workspace of a chunk call over m streams of K frames: the chunk buffers, then the (stream, phase) table of a
+// subset call (2m ints, gast_stream_push_subset below) when `table`.  sp gives the dilations only.
+static int chunk_bufs(const gast_handle* h, const StreamPlan& sp, int m, int K, bool table, const char* who, Arena& a,
+                      ChunkBufs* cb) {
   const gast_cfg& c = h->cfg;
-  const int n = sp.n, J = c.num_joints, k0 = c.filter_widths[0];
-  if (K < 1) return fail("gast_stream_push_chunk: K must be at least 1 (got %d)", K);
-  if ((long long)n * K * J >= 0x7fffffffLL) return fail("expand: more than 2^31 positions in one call");
+  const int J = c.num_joints, k0 = c.filter_widths[0];
+  if (K < 1) return fail("%s: K must be at least 1 (got %d)", who, K);
+  if ((long long)m * K * J >= 0x7fffffffLL) return fail("expand: more than 2^31 positions in one call");
   size_t g = 0;
   for (int i = 1; i < c.num_stages; ++i)
-    g = std::max(g, (size_t)n * ((c.filter_widths[i] - 1) * sp.dil[i - 1] + K) * J * (c.channels << i));
-  cb->xin = a.take((size_t)n * (k0 - 1 + K) * J * c.in_features);
+    g = std::max(g, (size_t)m * ((c.filter_widths[i] - 1) * sp.dil[i - 1] + K) * J * (c.channels << i));
+  cb->xin = a.take((size_t)m * (k0 - 1 + K) * J * c.in_features);
   cb->G = a.take(g);
-  stream_bufs(h, n * K, a, &cb->sb);
+  stream_bufs(h, m * K, a, &cb->sb);
+  cb->tab = table ? reinterpret_cast<int32_t*>(a.take((size_t)2 * m)) : nullptr;
   return 0;
+}
+
+// Bytes that chunk_bufs takes (0 after a refusal): what the workspace of the call must hold.
+static size_t chunk_workspace_bytes(const gast_handle* h, const StreamPlan& sp, int m, int K, bool table,
+                                    const char* who) {
+  Arena dry{nullptr, 0, 0, true};
+  ChunkBufs cb;
+  return chunk_bufs(h, sp, m, K, table, who, dry, &cb) ? 0 : dry.off + 256;
 }
 
 extern "C" size_t gast_stream_chunk_workspace_bytes(gast_t* h, int32_t n_streams, int32_t K) {
-  if (!h) return 0;
   StreamPlan sp;
-  if (stream_plan(h, n_streams, &sp)) return 0;
-  Arena a{nullptr, 0, 0, true};
-  ChunkBufs cb;
-  if (chunk_bufs(h, sp, K, a, &cb)) return 0;
-  return a.off + 256;
-}
-
-static int chunk_check_workspace(gast_handle* h, const StreamPlan& sp, int K, const void* workspace,
-                                 size_t workspace_bytes, const char* who) {
-  Arena dry{nullptr, 0, 0, true};
-  ChunkBufs cb;
-  if (chunk_bufs(h, sp, K, dry, &cb)) return 1;
-  const size_t need = dry.off + 256;
-  if (!workspace || workspace_bytes < need)
-    return fail("%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
-  return 0;
+  if (!h || stream_plan(h, n_streams, &sp)) return 0;
+  return chunk_workspace_bytes(h, sp, n_streams, K, false, "gast_stream_chunk_workspace_bytes");
 }
 
 // The chunk forward after its input frames are in cb.xin: expand, block 0, the temporal stages on their gathered
@@ -444,86 +450,16 @@ static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, 
   return 0;
 }
 
-extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
-                                      int32_t K, const int32_t* fresh, const int32_t* hold, void* workspace,
-                                      size_t workspace_bytes, void* stream) {
-  if (!h) return fail("gast_stream_push_chunk: null handle");
-  if (!h->prepared) return fail("gast_stream_push_chunk: gast_prepare() has not run since the last gast_bind()");
-  if (step < 0 || !state || !x || !y) return fail("gast_stream_push_chunk: bad arguments");
-  StreamPlan sp;
-  if (stream_plan(h, n_streams, &sp)) return 1;
-  if (chunk_check_workspace(h, sp, K, workspace, workspace_bytes, "gast_stream_push_chunk")) return 1;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
-  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
-  const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0];
-  float* sbase = reinterpret_cast<float*>(align256(state));
-  Arena a = workspace_arena(workspace, workspace_bytes);
-  ChunkBufs cb;
-  if (chunk_bufs(h, sp, K, a, &cb)) return 1;
-  stream_chunk_xin_kernel<<<n_streams, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K,
-                                                                   J * h->cfg.in_features, nullptr);
-  h->launches++;
-  return chunk_forward(h, st, sp, sbase, step, n_streams, K, fresh, true, cb, y, nullptr);
-}
-
-// ---- peek: the poses K held pushes would return, without pushing ------------------------------------------------
-// gast_stream_peek is gast_stream_push_chunk with fresh = null and every frame held, minus every write to the state:
-// stream_peek_xin_kernel builds the chunk input from the input history without updating it, and the stages gather
-// their ring history but write no slot back.  Row k of stream s is the pose the (k+1)-th held push would return: for a
-// sequence of l pushed frames, the pose of frame l - latency + k with the generator's right padding applied after
-// frame l - 1.
-extern "C" int gast_stream_peek(gast_t* h, const void* state, int64_t step, float* y, int32_t n_streams, int32_t K,
-                                void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h) return fail("gast_stream_peek: null handle");
-  if (!h->prepared) return fail("gast_stream_peek: gast_prepare() has not run since the last gast_bind()");
-  const int32_t lat = gast_stream_latency(h);
-  if (lat < 0) return 1;
-  if (lat == 0)
-    return fail("gast_stream_peek needs a non-causal model: a causal model returns the pose of the pushed frame, so "
-                "none is ever pending");
-  if (K < 1 || K > lat) return fail("gast_stream_peek: K must be in [1, latency = %d] (got %d)", lat, K);
-  if (step < 1) return fail("gast_stream_peek: step must be at least 1 (the state holds no pushed frame)");
-  if (!state || !y) return fail("gast_stream_peek: bad arguments");
-  StreamPlan sp;
-  if (stream_plan(h, n_streams, &sp)) return 1;
-  if (chunk_check_workspace(h, sp, K, workspace, workspace_bytes, "gast_stream_peek")) return 1;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
-  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
-  const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0];
-  // only read: chunk_forward writes no ring back when write_rings is false
-  float* sbase = reinterpret_cast<float*>(align256(const_cast<void*>(state)));
-  Arena a = workspace_arena(workspace, workspace_bytes);
-  ChunkBufs cb;
-  if (chunk_bufs(h, sp, K, a, &cb)) return 1;
-  const long long xe = (long long)n_streams * (k0 - 1 + K) * J * h->cfg.in_features;
-  stream_peek_xin_kernel<<<(unsigned)std::min<long long>(cdiv(xe, 256), (long long)h->sm_count * 16), 256, 0, st>>>(
-      sbase + sp.xhist_off, cb.xin, n_streams, k0, K, J * h->cfg.in_features, nullptr);
-  h->launches++;
-  return chunk_forward(h, st, sp, sbase, step, n_streams, K, nullptr, false, cb, y, nullptr);
-}
-
 // ---- any subset of the streams, each at its own frame count -------------------------------------------------------
 // A subset call runs the chunk (or peek) forward over the m listed streams only: the four copy kernels read and write
 // the state rows of stream streams[i] at that stream's own ring phase, and everything between them (expand, blocks,
 // stages on the time-ordered weights Wt, shrink) works on the m*K gathered frames as for a chunk.  Every ring size R_i
 // divides the largest one, R_max = w_0 w_1 ... w_{L-1} (R_i = w_i d_i and d_{i+1} = R_i), so one phase per stream,
 // steps[i] mod R_max, gives its slot in every ring.  The (stream, phase) table goes to the workspace in one copy.
-static int subset_bufs(const gast_handle* h, int m, int K, Arena& a, ChunkBufs* cb, int32_t** tab) {
-  StreamPlan spm;                                          // the chunk buffers of m streams
-  if (stream_plan(h, m, &spm) || chunk_bufs(h, spm, K, a, cb)) return 1;
-  *tab = reinterpret_cast<int32_t*>(a.take((size_t)2 * m));
-  return 0;
-}
-
 extern "C" size_t gast_stream_subset_workspace_bytes(gast_t* h, int32_t m, int32_t K) {
-  if (!h || m < 1) return 0;
-  Arena a{nullptr, 0, 0, true};
-  ChunkBufs cb;
-  int32_t* tab;
-  if (subset_bufs(h, m, K, a, &cb, &tab)) return 0;
-  return a.off + 256;
+  StreamPlan sp;                                           // the chunk buffers of m streams
+  if (!h || m < 1 || stream_plan(h, m, &sp)) return 0;
+  return chunk_workspace_bytes(h, sp, m, K, true, "gast_stream_subset_workspace_bytes");
 }
 
 // Host-side checks of a subset call and its table: {streams[i]} then {steps[i] mod R_max}.  *lockstep = the call lists
@@ -531,7 +467,6 @@ extern "C" size_t gast_stream_subset_workspace_bytes(gast_t* h, int32_t m, int32
 static int subset_table(const StreamPlan& sp, const int32_t* streams, const int64_t* steps,
                         int m, int64_t min_step, const char* who, std::vector<int32_t>* tab, bool* lockstep) {
   const int n = sp.n;
-  if (!streams || !steps) return fail("%s: null streams or steps", who);
   if (m < 1 || m > n) return fail("%s: m must be in [1, n_streams = %d] (got %d)", who, n, m);
   const int64_t Rmax = sp.R.empty() ? 1 : sp.R.back();
   std::vector<char> seen(n, 0);
@@ -551,74 +486,99 @@ static int subset_table(const StreamPlan& sp, const int32_t* streams, const int6
   return 0;
 }
 
+// ---- the four chunk entries ---------------------------------------------------------------------------------------
+// One chunk call over m streams of K frames.  x null: a peek (below), every frame held and the state only read, its
+// input built by stream_peek_xin_kernel; else a push of x through stream_chunk_xin_kernel.  streams null: the lockstep
+// form, all m = n_streams streams at `step`; else the subset form, stream streams[i] at steps[i], which takes the
+// lockstep addressing (no table) when it lists every stream in order at one step.  Every refusal comes before the
+// first launch.
+static int chunk_call(const char* who, gast_handle* h, void* state, int n_streams, const int32_t* streams,
+                      const int64_t* steps, int64_t step, int m, int K, const float* x, float* y,
+                      const int32_t* fresh, const int32_t* hold, void* workspace, size_t workspace_bytes,
+                      void* stream) {
+  if (!h) return fail("%s: null handle", who);
+  const bool peek = !x;
+  if (peek) {
+    const int32_t lat = gast_stream_latency(h);
+    if (lat < 0) return 1;
+    if (lat == 0)
+      return fail("%s needs a non-causal model: a causal model returns the pose of the pushed frame, so none is ever "
+                  "pending", who);
+    if (K < 1 || K > lat) return fail("%s: K must be in [1, latency = %d] (got %d)", who, lat, K);
+    if (!streams && step < 1) return fail("%s: step must be at least 1 (the state holds no pushed frame)", who);
+  }
+  if ((!streams && step < 0) || !state || !y) return fail("%s: bad arguments", who);
+  StreamPlan sp;
+  if (stream_plan(h, n_streams, &sp)) return 1;
+  std::vector<int32_t> tab;
+  bool lockstep = true;
+  if (streams && subset_table(sp, streams, steps, m, peek ? 1 : 0, who, &tab, &lockstep)) return 1;
+  const size_t need = chunk_workspace_bytes(h, sp, m, K, streams != nullptr, who);
+  if (need == 0) return 1;
+  if (!workspace || workspace_bytes < need)
+    return fail("%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
+  if (stream_call_begin(h, who)) return 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0], JF = J * h->cfg.in_features;
+  float* sbase = reinterpret_cast<float*>(align256(state));
+  Arena a = workspace_arena(workspace, workspace_bytes);
+  ChunkBufs cb;
+  chunk_bufs(h, sp, m, K, streams != nullptr, who, a, &cb);      // sized above: cannot fail
+  const int32_t* dtab = nullptr;
+  if (!lockstep) {
+    CUDA_OK(cudaMemcpyAsync(cb.tab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    dtab = cb.tab;
+  }
+  if (streams) step = steps[0];                                  // read by the lockstep addressing only
+  if (peek) {
+    const long long xe = (long long)m * (k0 - 1 + K) * JF;
+    stream_peek_xin_kernel<<<(unsigned)std::min<long long>(cdiv(xe, 256), (long long)h->sm_count * 16), 256, 0, st>>>(
+        sbase + sp.xhist_off, cb.xin, m, k0, K, JF, dtab);
+  } else {
+    stream_chunk_xin_kernel<<<m, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K, JF,
+                                                             dtab);
+  }
+  h->launches++;
+  return chunk_forward(h, st, sp, sbase, step, m, K, fresh, !peek, cb, y, dtab);
+}
+
+extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
+                                      int32_t K, const int32_t* fresh, const int32_t* hold, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  if (!x) return fail("gast_stream_push_chunk: bad arguments");   // a null x would make the call a peek
+  return chunk_call("gast_stream_push_chunk", h, state, n_streams, nullptr, nullptr, step, n_streams, K, x, y, fresh,
+                    hold, workspace, workspace_bytes, stream);
+}
+
+// ---- peek: the poses K held pushes would return, without pushing ------------------------------------------------
+// gast_stream_peek is gast_stream_push_chunk with fresh = null and every frame held, minus every write to the state:
+// stream_peek_xin_kernel builds the chunk input from the input history without updating it, and the stages gather
+// their ring history but write no slot back.  Row k of stream s is the pose the (k+1)-th held push would return: for a
+// sequence of l pushed frames, the pose of frame l - latency + k with the generator's right padding applied after
+// frame l - 1.
+extern "C" int gast_stream_peek(gast_t* h, const void* state, int64_t step, float* y, int32_t n_streams, int32_t K,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  // only read: chunk_forward writes no ring back for a peek
+  return chunk_call("gast_stream_peek", h, const_cast<void*>(state), n_streams, nullptr, nullptr, step, n_streams, K,
+                    nullptr, y, nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
 extern "C" int gast_stream_push_subset(gast_t* h, void* state, int32_t n_streams, const int32_t* streams,
                                        const int64_t* steps, int32_t m, int32_t K, const float* x, float* y,
                                        const int32_t* fresh, const int32_t* hold, void* workspace,
                                        size_t workspace_bytes, void* stream) {
   const char* who = "gast_stream_push_subset";
-  if (!h) return fail("%s: null handle", who);
-  if (!h->prepared) return fail("%s: gast_prepare() has not run since the last gast_bind()", who);
-  if (!state || !x || !y) return fail("%s: bad arguments", who);
-  StreamPlan sp;
-  if (stream_plan(h, n_streams, &sp)) return 1;
-  std::vector<int32_t> tab;
-  bool lockstep;
-  if (subset_table(sp, streams, steps, m, 0, who, &tab, &lockstep)) return 1;
-  const size_t need = gast_stream_subset_workspace_bytes(h, m, K);
-  if (need == 0) return 1;
-  if (!workspace || workspace_bytes < need) return fail("%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
-  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
-  const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0];
-  float* sbase = reinterpret_cast<float*>(align256(state));
-  Arena a = workspace_arena(workspace, workspace_bytes);
-  ChunkBufs cb;
-  int32_t* dtab;
-  if (subset_bufs(h, m, K, a, &cb, &dtab)) return 1;
-  if (lockstep) dtab = nullptr;
-  else CUDA_OK(cudaMemcpyAsync(dtab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  stream_chunk_xin_kernel<<<m, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K,
-                                                           J * h->cfg.in_features, dtab);
-  h->launches++;
-  return chunk_forward(h, st, sp, sbase, steps[0], m, K, fresh, true, cb, y, dtab);
+  if (!streams || !steps) return fail("%s: null streams or steps", who);   // null streams is the lockstep form
+  if (!x) return fail("%s: bad arguments", who);
+  return chunk_call(who, h, state, n_streams, streams, steps, 0, m, K, x, y, fresh, hold, workspace, workspace_bytes,
+                    stream);
 }
 
 extern "C" int gast_stream_peek_subset(gast_t* h, const void* state, int32_t n_streams, const int32_t* streams,
                                        const int64_t* steps, int32_t m, int32_t K, float* y, void* workspace,
                                        size_t workspace_bytes, void* stream) {
   const char* who = "gast_stream_peek_subset";
-  if (!h) return fail("%s: null handle", who);
-  if (!h->prepared) return fail("%s: gast_prepare() has not run since the last gast_bind()", who);
-  const int32_t lat = gast_stream_latency(h);
-  if (lat < 0) return 1;
-  if (lat == 0)
-    return fail("%s needs a non-causal model: a causal model returns the pose of the pushed frame, so none is ever "
-                "pending", who);
-  if (K < 1 || K > lat) return fail("%s: K must be in [1, latency = %d] (got %d)", who, lat, K);
-  if (!state || !y) return fail("%s: bad arguments", who);
-  StreamPlan sp;
-  if (stream_plan(h, n_streams, &sp)) return 1;
-  std::vector<int32_t> tab;
-  bool lockstep;
-  if (subset_table(sp, streams, steps, m, 1, who, &tab, &lockstep)) return 1;
-  const size_t need = gast_stream_subset_workspace_bytes(h, m, K);
-  if (need == 0) return 1;
-  if (!workspace || workspace_bytes < need) return fail("%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
-  h->launches = 0; h->tc_launches = 0; h->ev_used = 0; h->ev_kind.clear();
-  const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0];
-  float* sbase = reinterpret_cast<float*>(align256(const_cast<void*>(state)));   // only read (write_rings = false)
-  Arena a = workspace_arena(workspace, workspace_bytes);
-  ChunkBufs cb;
-  int32_t* dtab;
-  if (subset_bufs(h, m, K, a, &cb, &dtab)) return 1;
-  if (lockstep) dtab = nullptr;
-  else CUDA_OK(cudaMemcpyAsync(dtab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  const long long xe = (long long)m * (k0 - 1 + K) * J * h->cfg.in_features;
-  stream_peek_xin_kernel<<<(unsigned)std::min<long long>(cdiv(xe, 256), (long long)h->sm_count * 16), 256, 0, st>>>(
-      sbase + sp.xhist_off, cb.xin, m, k0, K, J * h->cfg.in_features, dtab);
-  h->launches++;
-  return chunk_forward(h, st, sp, sbase, steps[0], m, K, nullptr, false, cb, y, dtab);
+  if (!streams || !steps) return fail("%s: null streams or steps", who);
+  return chunk_call(who, h, const_cast<void*>(state), n_streams, streams, steps, 0, m, K, nullptr, y, nullptr,
+                    nullptr, workspace, workspace_bytes, stream);
 }

@@ -3,9 +3,11 @@
 The reference's real-time model is a causal `SpatioTemporalModelOptimized1f` fed the last `receptive_field`
 frames of one stream for every new frame (`gen_skes.py:43-69`, `tools/inference.py:19-110`): O(rf) work per
 frame.  `PoseStream` produces the same poses with O(1) work per frame: the library keeps, per temporal stage, a
-ring of that stage's past inputs for all streams (`csrc/stream.cuh`, C ABI `gast_stream_push_ex`), so a pushed frame
-computes one new position per layer.  A stream's first frame stands for its whole (edge-padded) history exactly
-like `UnchunkedGenerator` does (`common/generators.py:210-221`).
+ring of that stage's past inputs for all streams (`csrc/stream.cuh`), so a pushed frame computes one new position per
+layer.  A single-frame push of every stream runs the C ABI's `gast_stream_push_ex`; lockstep multi-frame and peek
+calls go through the subset entries `gast_stream_push_subset` / `_peek_subset` on their null-table branch, and
+calls on some of the streams or at unequal counts through the same entries with a table.  A stream's first frame
+stands for its whole (edge-padded) history exactly like `UnchunkedGenerator` does (`common/generators.py:210-221`).
 
 `PoseStream` takes causal and non-causal models.  A non-causal model returns the pose of frame t - pad when frame t
 is pushed (`latency` = pad = (rf - 1) // 2; 0 for a causal model).  `end()` closes a stream's sequence: its next
@@ -174,9 +176,11 @@ class PoseStream(object):
 
     `push`, `push_frames` and `peek` take `streams`, a list of distinct stream indices: only those streams take part
     (their rows come in and go out in that order), the others sit the call out untouched.  Each stream then has its
-    own frame count (`counts`); `step` is the smallest of them.  Calls without `streams` while every count is equal
-    use the lockstep library entries (gast_stream_push_ex / _push_chunk / _peek at `step`), all others the subset
-    entries (gast_stream_push_subset / _peek_subset), whose cost follows the listed streams, not n_streams."""
+    own frame count (`counts`); `step` is the smallest of them.  A `push` without `streams` while every count is
+    equal runs the single-frame library entry gast_stream_push_ex at `step`.  Every other call runs the subset entries
+    (gast_stream_push_subset / _peek_subset), whose cost follows the listed streams, not n_streams; a multi-frame or
+    peek call without `streams` at equal counts lists every stream in order at `step`, which the library runs on the
+    chunk path's plain lockstep addressing."""
 
     def __init__(self, model_pos, n_streams, augment=False, kps_left=None, kps_right=None, joints_left=None,
                  joints_right=None, device=None):
@@ -218,13 +222,10 @@ class PoseStream(object):
         self.book = SequenceBook(self.n, self.latency)
         self.step = 0
         self._delta = np.zeros(self.n, dtype=np.int64)   # counts - step (>= 0; all 0 while the streams are in step)
-        self._masks = torch.zeros((2, self.copies * self.n), dtype=torch.int32, device=self.device)
         self._sig = None                 # the handle's parameter signature at the last push
         self._state = None
-        self._ws = None
-        self._chunk_ws = None            # push_frames: workspace of the largest K so far
-        self._chunk_masks = None
-        self._subset_ws = None           # subset calls: workspace of the largest (streams, K) so far
+        self._ws = None                  # library workspace of the largest call so far
+        self._masks = None               # device [fresh | hold] masks of the largest push so far
 
     @property
     def counts(self):
@@ -259,14 +260,20 @@ class PoseStream(object):
         self.book.end(streams)
 
     def _upload(self, fresh, hold):
-        """-> device pointers of the fresh and hold masks of this push (None where no stream is set)"""
+        """-> device pointers of the fresh (m,) and hold (m, K) masks of a push, repeated for the mirrored half (None
+        where no stream is set).  Every push reuses one buffer [fresh | hold]: the copy into it and the kernels that
+        read it are ordered on the one stream the calls run on."""
         any_f, any_h = bool(fresh.any()), bool(hold.any())
         if not (any_f or any_h):
             return None, None
-        mk = np.tile(np.stack([fresh, hold]).astype(np.int32), (1, self.copies))
+        mk = np.concatenate([np.tile(fresh.astype(np.int32), self.copies),
+                             np.tile(hold.astype(np.int32), (self.copies, 1)).reshape(-1)])
+        if self._masks is None or self._masks.numel() < mk.size:
+            self._masks = torch.empty(mk.size, dtype=torch.int32, device=self.device)
         # pinned + non_blocking: no device sync; the caching host allocator keeps the buffer until the copy ran
-        self._masks.copy_(torch.from_numpy(mk).pin_memory(), non_blocking=True)
-        return (self._masks[0].data_ptr() if any_f else None), (self._masks[1].data_ptr() if any_h else None)
+        self._masks[:mk.size].copy_(torch.from_numpy(mk).pin_memory(), non_blocking=True)
+        mm = self.copies * fresh.size
+        return (self._masks.data_ptr() if any_f else None), (self._masks[mm:].data_ptr() if any_h else None)
 
     def _begin(self, h, st):
         """refresh the handle, refuse a push over history computed with other weights, allocate the state"""
@@ -278,132 +285,46 @@ class PoseStream(object):
                                 'was computed with the old weights -- call reset() before pushing again'
                                 % type(self).__name__)
         if self._state is None:
-            m = self.copies * self.n
             if lib.gast_stream_latency(h.h) != self.latency:
                 raise eng.GastError('gast_stream_latency: %s' % L.last_error())
-            nb = lib.gast_stream_state_bytes(h.h, m)
-            wb = lib.gast_stream_workspace_bytes(h.h, m)
-            if nb == 0 or wb == 0:
+            nb = lib.gast_stream_state_bytes(h.h, self.copies * self.n)
+            if nb == 0:
                 raise eng.GastError('gast_stream_state_bytes: %s' % L.last_error())
             self._state = torch.empty(int(nb), dtype=torch.uint8, device=self.device)
-            self._ws = torch.empty(int(wb), dtype=torch.uint8, device=self.device)
 
     def push(self, frame, streams=None):
         """frame (n_streams, J, in_features): the newest 2D keypoints of every stream (normalised screen
         coordinates; rows of held streams are ignored) -> (poses (n, J, 3), index (n,) CPU int64).  With `streams`
         (m distinct indices): frame (m, J, F) -> (poses (m, J, 3), index (m,)) of those streams, in that order;
         the other streams are unchanged."""
-        eng = self.engine
-        name = type(self).__name__
         frame = torch.as_tensor(frame, dtype=torch.float32, device=self.device).contiguous()
         sel = self._select(streams)
-        if sel is not None:
-            assert frame.shape == (sel.size, self.J, self.F), frame.shape
-            y, index = self._push_subset(frame[:, None], None, sel)
-            return y[:, 0], index[:, 0]
-        assert frame.shape == (self.n, self.J, self.F), frame.shape
-        if self.model.training:
-            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
-        h = eng.model_handle(self.model, self.device)
-        lib = h.lib
-        m = self.copies * self.n
-        y = torch.empty((self.n, self.J, 3), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device).cuda_stream
-            self._begin(h, st)
-            fresh, hold, index = self.book.advance()
-            fresh_p, hold_p = self._upload(fresh, hold)
-            x, out = frame, y
-            if self.augment:
-                x = torch.empty((2, self.n, self.J, self.F), dtype=torch.float32, device=self.device)
-                if lib.gast_tta_prepare(C.c_void_p(frame.data_ptr()), C.c_void_p(x.data_ptr()), self.n, self.J, self.F,
-                                        0, 0, len(self.kps_left), self._kl, self._kr, C.c_void_p(st)) != 0:
-                    raise eng.GastError('gast_tta_prepare: %s' % L.last_error())
-                out = torch.empty((2, self.n, self.J, 3), dtype=torch.float32, device=self.device)
-            rc = lib.gast_stream_push_ex(h.h, C.c_void_p(self._state.data_ptr()), C.c_int64(self.step),
-                                         C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), m, C.c_void_p(fresh_p),
-                                         C.c_void_p(hold_p), C.c_void_p(self._ws.data_ptr()), self._ws.numel(),
-                                         C.c_void_p(st))
-            if rc != 0:
-                raise eng.GastError('gast_stream_push_ex: %s' % L.last_error())
-            launches = int(lib.gast_last_launch_count(h.h))
-            if self.augment:
-                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(y.data_ptr()), self.n, self.J,
-                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
-                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
-                launches += 2
-            self._sig = h.sig
-        self.step += 1
-        self.last_launches = launches
-        return y, torch.from_numpy(index)
+        assert frame.shape == (self.n if sel is None else sel.size, self.J, self.F), frame.shape
+        y, index = self._call(frame[:, None], 1, sel)
+        return y[:, 0], index[:, 0]
 
     def push_frames(self, frames, valid=None, streams=None):
         """frames (n_streams, K, J, in_features): the next K frames of every stream -> (poses (n, K, J, 3) CUDA,
         index (n, K) CPU int64), what K calls of `push` with frames[:, k] return, in one library call
-        (gast_stream_push_chunk).  valid (n,) or None: only the first valid[s] frames of stream s belong to its
+        (gast_stream_push_subset).  valid (n,) or None: only the first valid[s] frames of stream s belong to its
         sequence; a smaller value than K ends the sequence there (as `end([s])` before frame valid[s] would) and the
         rest of the chunk returns its tail.  Rows of held frames are ignored.  `reset()` / `end()` take effect at
         frame 0 of the call, as for `push`.  With `streams` (m distinct indices) frames, valid, poses and index have m
-        rows, those streams' in that order, and only those streams advance (gast_stream_push_subset).  A stream's
-        flush is `push_frames(nan frames (1, latency, J, F), valid=[0], streams=[s])`."""
-        eng = self.engine
-        name = type(self).__name__
+        rows, those streams' in that order, and only those streams advance.  A stream's flush is
+        `push_frames(nan frames (1, latency, J, F), valid=[0], streams=[s])`."""
         frames = torch.as_tensor(frames, dtype=torch.float32, device=self.device).contiguous()
         sel = self._select(streams)
-        if sel is not None:
-            assert frames.dim() == 4 and frames.shape[0] == sel.size and frames.shape[1] >= 1 and \
-                tuple(frames.shape[2:]) == (self.J, self.F), frames.shape
-            return self._push_subset(frames, valid, sel)
-        assert frames.dim() == 4 and frames.shape[0] == self.n and frames.shape[1] >= 1 and \
-            tuple(frames.shape[2:]) == (self.J, self.F), frames.shape
-        K = int(frames.shape[1])
-        if K == 1 and valid is None:
-            y, index = self.push(frames[:, 0])
-            return y.view(self.n, 1, self.J, 3), index.view(self.n, 1)
-        if self.model.training:
-            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
-        h = eng.model_handle(self.model, self.device)
-        lib = h.lib
-        m = self.copies * self.n
-        y = torch.empty((self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device).cuda_stream
-            self._begin(h, st)
-            ws = self._chunk_workspace(h, m, K)
-            fresh, hold, index = self.book.advance_many(K, valid)
-            fresh_p, hold_p = self._upload_chunk(fresh, hold)
-            x, out = frames, y
-            if self.augment:
-                # (2, n*K, J, F) = 2n streams of K frames: [original | mirrored]
-                x = torch.empty((2, self.n, K, self.J, self.F), dtype=torch.float32, device=self.device)
-                if lib.gast_tta_prepare(C.c_void_p(frames.data_ptr()), C.c_void_p(x.data_ptr()), self.n * K, self.J,
-                                        self.F, 0, 0, len(self.kps_left), self._kl, self._kr, C.c_void_p(st)) != 0:
-                    raise eng.GastError('gast_tta_prepare: %s' % L.last_error())
-                out = torch.empty((2, self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
-            rc = lib.gast_stream_push_chunk(h.h, C.c_void_p(self._state.data_ptr()), C.c_int64(self.step),
-                                            C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), m, K,
-                                            C.c_void_p(fresh_p), C.c_void_p(hold_p), C.c_void_p(ws.data_ptr()),
-                                            ws.numel(), C.c_void_p(st))
-            if rc != 0:
-                raise eng.GastError('gast_stream_push_chunk: %s' % L.last_error())
-            launches = int(lib.gast_last_launch_count(h.h))
-            if self.augment:
-                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(y.data_ptr()), self.n * K, self.J,
-                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
-                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
-                launches += 2
-            self._sig = h.sig
-        self.step += K
-        self.last_launches = launches
-        return y, torch.from_numpy(index)
+        assert frames.dim() == 4 and frames.shape[0] == (self.n if sel is None else sel.size) and \
+            frames.shape[1] >= 1 and tuple(frames.shape[2:]) == (self.J, self.F), frames.shape
+        return self._call(frames, int(frames.shape[1]), sel, valid)
 
     def peek(self, K=None, streams=None):
         """Provisional poses of the frames a non-causal model has not returned yet, without pushing -> (poses
         (n, K, J, 3) CUDA, index (n, K) CPU int64): what K more pushes would return if every stream's sequence ended
-        at its newest frame (`end()` and K held pushes), in one library call (gast_stream_peek).  Nothing changes:
-        not the library state, not `step`, not the sequences.  Those poses are the reference's for the sequence cut
-        at its newest frame (UnchunkedGenerator pads it with copies of that frame); the pushes still return the final
-        poses `latency` pushes later.  K defaults to `latency`, 1 <= K <= latency.
+        at its newest frame (`end()` and K held pushes), in one library call (gast_stream_peek_subset).  Nothing
+        changes: not the library state, not `step`, not the sequences.  Those poses are the reference's for the
+        sequence cut at its newest frame (UnchunkedGenerator pads it with copies of that frame); the pushes still
+        return the final poses `latency` pushes later.  K defaults to `latency`, 1 <= K <= latency.
 
         Lookahead: for a stream that pushed frames 0 .. l-1 of its sequence, row k is the pose of frame
         l - latency + k, so with K = latency the last row is the newest frame.  To show poses L frames behind the
@@ -411,174 +332,95 @@ class PoseStream(object):
         the frame's position in stream s's sequence, -1 where nothing is due (ending streams with fewer poses left,
         idle or freshly reset streams, frames before the sequence's start); when no stream has a pose due the call
         launches nothing.  With `streams` (m distinct indices) poses and index have m rows, those streams' in that
-        order, each stream peeked at its own frame count (gast_stream_peek_subset)."""
-        eng = self.engine
+        order, each stream peeked at its own frame count."""
         name = type(self).__name__
         if self.causal:
-            raise eng.GastError('%s.peek needs a non-causal model: a causal model returns the pose of every pushed '
-                                'frame at once, so none is ever pending' % name)
+            raise self.engine.GastError('%s.peek needs a non-causal model: a causal model returns the pose of every '
+                                        'pushed frame at once, so none is ever pending' % name)
         K = self.latency if K is None else int(K)
         if not 1 <= K <= self.latency:
-            raise eng.GastError('%s.peek: K must be in [1, latency = %d] (got %d)' % (name, self.latency, K))
-        if self.model.training:
-            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
-        sel = self._select(streams)
-        if sel is not None:
-            return self._peek_subset(K, sel)
-        index = self.book.peek(K)
-        y = torch.empty((self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
-        if not (index >= 0).any():
-            self.last_launches = 0
-            return y, torch.from_numpy(index)
-        h = eng.model_handle(self.model, self.device)
-        lib = h.lib
-        m = self.copies * self.n
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device).cuda_stream
-            self._begin(h, st)
-            ws = self._chunk_workspace(h, m, K)
-            out = y
-            if self.augment:
-                out = torch.empty((2, self.n, K, self.J, 3), dtype=torch.float32, device=self.device)
-            rc = lib.gast_stream_peek(h.h, C.c_void_p(self._state.data_ptr()), C.c_int64(self.step),
-                                      C.c_void_p(out.data_ptr()), m, K, C.c_void_p(ws.data_ptr()), ws.numel(),
-                                      C.c_void_p(st))
-            if rc != 0:
-                raise eng.GastError('gast_stream_peek: %s' % L.last_error())
-            launches = int(lib.gast_last_launch_count(h.h))
-            if self.augment:
-                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(y.data_ptr()), self.n * K, self.J,
-                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
-                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
-                launches += 2
-        self.last_launches = launches
-        return y, torch.from_numpy(index)
+            raise self.engine.GastError('%s.peek: K must be in [1, latency = %d] (got %d)' % (name, self.latency, K))
+        return self._call(None, K, self._select(streams))
 
-    def _subset_args(self, sel, counts):
-        """-> (library stream indices, their counts) as host arrays: [sel | sel + n] with augment"""
-        lib_streams = np.concatenate([sel + c * self.n for c in range(self.copies)]).astype(np.int32)
-        lib_steps = np.tile(counts, self.copies).astype(np.int64)
-        return lib_streams, lib_steps
-
-    def _subset_workspace(self, h, m, K):
-        """the workspace of a subset call of m library streams and K frames; serves every smaller m and K"""
-        wb = int(h.lib.gast_stream_subset_workspace_bytes(h.h, m, K))
-        if wb == 0:
-            raise self.engine.GastError('gast_stream_subset_workspace_bytes: %s' % L.last_error())
-        if self._subset_ws is None or self._subset_ws.numel() < wb:
-            self._subset_ws = None
-            self._subset_ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
-        return self._subset_ws
-
-    def _push_subset(self, frames, valid, sel):
-        """push_frames of the streams `sel` (frames (m, K, J, F)) through gast_stream_push_subset"""
+    def _call(self, frames, K, sel, valid=None):
+        """The library call of a push of frames (m, K, J, F), or for frames None of a peek of K frames, over every
+        stream (sel None: a lockstep call at `step`) or over the streams `sel`, each at its own count -> (poses
+        (m, K, J, 3) CUDA, index (m, K) CPU int64).  A lockstep push of one frame without `valid` runs
+        gast_stream_push_ex; every other call runs gast_stream_push_subset / _peek_subset, which run a lockstep call
+        (every library stream listed in order at `step`) on the chunk path's own addressing.  A peek launches nothing
+        when no pose is due, and leaves out the streams that never pushed a frame (their rows are unspecified)."""
         eng = self.engine
-        name = type(self).__name__
         if self.model.training:
-            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
+            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % type(self).__name__)
+        rows = np.arange(self.n, dtype=np.int64) if sel is None else sel
+        y = torch.empty((rows.size, K, self.J, 3), dtype=torch.float32, device=self.device)
+        if frames is None:
+            index = self.book.peek(K, streams=sel)
+            if not (index >= 0).any():
+                self.last_launches = 0
+                return y, torch.from_numpy(index)
+            keep = self.counts[rows] >= 1
+        else:
+            keep = np.ones(rows.size, dtype=bool)
+        single = sel is None and frames is not None and K == 1 and valid is None
+        r = int(keep.sum())
+        mm = self.copies * r
         h = eng.model_handle(self.model, self.device)
         lib = h.lib
-        m, K = int(sel.size), int(frames.shape[1])
-        mm = self.copies * m
-        y = torch.empty((m, K, self.J, 3), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             st = torch.cuda.current_stream(self.device).cuda_stream
             self._begin(h, st)
-            ws = self._subset_workspace(h, mm, K)
-            lib_streams, lib_steps = self._subset_args(sel, self.counts[sel])
-            fresh, hold, index = self.book.advance_many(K, valid, streams=sel)
-            fresh_p, hold_p = self._upload_chunk(fresh, hold)
-            x, out = frames, y
+            if single:
+                fn, wb = 'gast_stream_workspace_bytes', lib.gast_stream_workspace_bytes(h.h, mm)
+            else:
+                fn, wb = 'gast_stream_subset_workspace_bytes', lib.gast_stream_subset_workspace_bytes(h.h, mm, K)
+            if wb == 0:
+                raise eng.GastError('%s: %s' % (fn, L.last_error()))
+            if self._ws is None or self._ws.numel() < wb:
+                self._ws = None
+                self._ws = torch.empty(int(wb), dtype=torch.uint8, device=self.device)
+            fresh_p = hold_p = None
+            if frames is not None:
+                fresh, hold, index = self.book.advance_many(K, valid, streams=sel)
+                fresh_p, hold_p = self._upload(fresh, hold)
+            yr = y if r == rows.size else torch.empty((r, K, self.J, 3), dtype=torch.float32, device=self.device)
+            x, out = frames, yr
             if self.augment:
-                x = torch.empty((2, m, K, self.J, self.F), dtype=torch.float32, device=self.device)
-                if lib.gast_tta_prepare(C.c_void_p(frames.data_ptr()), C.c_void_p(x.data_ptr()), m * K, self.J,
-                                        self.F, 0, 0, len(self.kps_left), self._kl, self._kr, C.c_void_p(st)) != 0:
-                    raise eng.GastError('gast_tta_prepare: %s' % L.last_error())
-                out = torch.empty((2, m, K, self.J, 3), dtype=torch.float32, device=self.device)
-            rc = lib.gast_stream_push_subset(h.h, C.c_void_p(self._state.data_ptr()), self.copies * self.n,
-                                             C.c_void_p(lib_streams.ctypes.data), C.c_void_p(lib_steps.ctypes.data), mm,
-                                             K, C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
-                                             C.c_void_p(fresh_p), C.c_void_p(hold_p), C.c_void_p(ws.data_ptr()),
-                                             ws.numel(), C.c_void_p(st))
-            if rc != 0:
-                raise eng.GastError('gast_stream_push_subset: %s' % L.last_error())
-            launches = int(lib.gast_last_launch_count(h.h))
-            if self.augment:
-                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(y.data_ptr()), m * K, self.J,
-                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
-                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
-                launches += 2
-            self._sig = h.sig
-        self._advanced(sel, K)
-        self.last_launches = launches
-        return y, torch.from_numpy(index)
-
-    def _peek_subset(self, K, sel):
-        """peek of the streams `sel` through gast_stream_peek_subset; streams that never pushed a frame (nothing due)
-        are left out of the library call and their rows are unspecified"""
-        eng = self.engine
-        index = self.book.peek(K, streams=sel)
-        m = int(sel.size)
-        y = torch.empty((m, K, self.J, 3), dtype=torch.float32, device=self.device)
-        counts = self.counts[sel]
-        rows = np.flatnonzero(counts >= 1)
-        if not (index >= 0).any():
-            self.last_launches = 0
-            return y, torch.from_numpy(index)
-        h = eng.model_handle(self.model, self.device)
-        lib = h.lib
-        r = int(rows.size)
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device).cuda_stream
-            self._begin(h, st)
-            ws = self._subset_workspace(h, self.copies * r, K)
-            lib_streams, lib_steps = self._subset_args(sel[rows], counts[rows])
-            yr = y if r == m else torch.empty((r, K, self.J, 3), dtype=torch.float32, device=self.device)
-            out = yr
-            if self.augment:
+                if frames is not None:
+                    # (2, m, K, J, F) = 2m library streams of K frames: [original | mirrored]
+                    x = torch.empty((2,) + tuple(frames.shape), dtype=torch.float32, device=self.device)
+                    if lib.gast_tta_prepare(frames.data_ptr(), x.data_ptr(), r * K, self.J, self.F, 0, 0,
+                                            len(self.kps_left), self._kl, self._kr, st) != 0:
+                        raise eng.GastError('gast_tta_prepare: %s' % L.last_error())
                 out = torch.empty((2, r, K, self.J, 3), dtype=torch.float32, device=self.device)
-            rc = lib.gast_stream_peek_subset(h.h, C.c_void_p(self._state.data_ptr()), self.copies * self.n,
-                                             C.c_void_p(lib_streams.ctypes.data), C.c_void_p(lib_steps.ctypes.data),
-                                             self.copies * r, K, C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()),
-                                             ws.numel(), C.c_void_p(st))
-            if rc != 0:
-                raise eng.GastError('gast_stream_peek_subset: %s' % L.last_error())
+            state = self._state.data_ptr()
+            if single:
+                fn, args = 'gast_stream_push_ex', (state, C.c_int64(self.step), x.data_ptr(), out.data_ptr(), mm,
+                                                   fresh_p, hold_p)
+            else:
+                # library streams [rows | rows + n] with augment, at their counts
+                lib_streams = np.concatenate([rows[keep] + c * self.n for c in range(self.copies)]).astype(np.int32)
+                lib_steps = np.tile(self.counts[rows[keep]], self.copies).astype(np.int64)
+                table = (state, self.copies * self.n, lib_streams.ctypes.data, lib_steps.ctypes.data, mm, K)
+                if frames is None:
+                    fn, args = 'gast_stream_peek_subset', table + (out.data_ptr(),)
+                else:
+                    fn, args = 'gast_stream_push_subset', table + (x.data_ptr(), out.data_ptr(), fresh_p, hold_p)
+            if getattr(lib, fn)(h.h, *args, self._ws.data_ptr(), self._ws.numel(), st) != 0:
+                raise eng.GastError('%s: %s' % (fn, L.last_error()))
             launches = int(lib.gast_last_launch_count(h.h))
             if self.augment:
-                if lib.gast_tta_merge(C.c_void_p(out.data_ptr()), C.c_void_p(yr.data_ptr()), r * K, self.J,
-                                      len(self.joints_left), self._jl, self._jr, C.c_void_p(st)) != 0:
+                if lib.gast_tta_merge(out.data_ptr(), yr.data_ptr(), r * K, self.J, len(self.joints_left), self._jl,
+                                      self._jr, st) != 0:
                     raise eng.GastError('gast_tta_merge: %s' % L.last_error())
                 launches += 2
-            if r < m:
-                y[torch.from_numpy(rows).to(self.device)] = yr
+            if r < rows.size:
+                y[torch.from_numpy(np.flatnonzero(keep)).to(self.device)] = yr
+        if frames is not None:
+            self._sig = h.sig
+            self._advanced(rows, K)
         self.last_launches = launches
         return y, torch.from_numpy(index)
-
-    def _chunk_workspace(self, h, m, K):
-        """the workspace of a chunk (or peek) of K frames over m library streams; grows with K and serves every
-        smaller K"""
-        wb = int(h.lib.gast_stream_chunk_workspace_bytes(h.h, m, K))
-        if wb == 0:
-            raise self.engine.GastError('gast_stream_chunk_workspace_bytes: %s' % L.last_error())
-        if self._chunk_ws is None or self._chunk_ws.numel() < wb:
-            self._chunk_ws = None
-            self._chunk_ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
-        return self._chunk_ws
-
-    def _upload_chunk(self, fresh, hold):
-        """-> device pointers of the fresh (n) and hold (n, K) masks of a chunk, repeated for the mirrored half
-        (None where no stream is set)"""
-        any_f, any_h = bool(fresh.any()), bool(hold.any())
-        if not (any_f or any_h):
-            return None, None
-        m = self.copies * len(fresh)
-        mk = np.concatenate([np.tile(fresh.astype(np.int32), self.copies),
-                             np.tile(hold.astype(np.int32), (self.copies, 1)).reshape(-1)])
-        # kept until the next chunk, so that no allocation of this one reuses it before the push read it
-        self._chunk_masks = dev = torch.empty(mk.size, dtype=torch.int32, device=self.device)
-        # pinned + non_blocking: no device sync; the caching host allocator keeps the buffer until the copy ran
-        dev.copy_(torch.from_numpy(mk).pin_memory(), non_blocking=True)
-        return (dev.data_ptr() if any_f else None), (dev[m:].data_ptr() if any_h else None)
 
 
 class CausalStream(PoseStream):

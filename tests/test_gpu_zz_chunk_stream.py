@@ -287,13 +287,14 @@ def test_dilated_handle_chunks_bitwise_like_optimized1f(augment, core):
 
 
 def test_causal_stream_push_frames():
-    """CausalStream.push_frames returns the poses of its frames, close to single pushes"""
+    """CausalStream.push_frames returns the poses of its frames, close to single pushes, for one frame too"""
     case = Case(17, (3, 3, 3), 32, 3, 20, 0, (), 51, True, False)
     m = D.module(case).cuda()
     x = torch.from_numpy(D.frames(case)).cuda()
     a, b = CausalStream(m, case.n), CausalStream(m, case.n)
     ya = torch.stack([a.push(x[t]) for t in range(case.T)], 1)
-    yb = torch.cat([b.push_frames(x[0:9].transpose(0, 1)), b.push_frames(x[9:20].transpose(0, 1))], 1)
+    yb = torch.cat([b.push_frames(x[0:9].transpose(0, 1)), b.push_frames(x[9:10].transpose(0, 1)),
+                    b.push_frames(x[10:20].transpose(0, 1))], 1)
     assert yb.shape == ya.shape
     mx, l2 = S.errors(yb.cpu().numpy(), ya.cpu().double().numpy())
     assert mx <= DS.MAX_BAR and l2 <= DS.L2_BAR, (mx, l2)

@@ -115,7 +115,7 @@ def clone(ps):
     c = copy.copy(ps)
     c.book = copy.deepcopy(ps.book)
     c._state = ps._state.clone()
-    c._chunk_ws = None
+    c._ws = None
     return c
 
 

@@ -1,7 +1,8 @@
-"""GPU: K frames per stream in one call (PoseStream.push_frames, gast_stream_push_chunk) against one push per frame
-(K = 1 is `push`), and bounded-memory whole-sequence lifting (lift_sequences) against the whole-sequence forward
-(tta.evaluate_sequence): time, peak device memory and the largest difference of their poses.  Prints one JSON line per
-measurement, the first with the card's name and power limit read in the same run.  CUDA events after a warm-up.
+"""GPU: K frames per stream in one call (PoseStream.push_frames, the kernels of gast_stream_push_chunk) against one
+push per frame (K = 1 is `push`), and bounded-memory whole-sequence lifting (lift_sequences) against the
+whole-sequence forward (tta.evaluate_sequence): time, peak device memory and the largest difference of their poses.
+Prints one JSON line per measurement, the first with the card's name and power limit read in the same run.  CUDA
+events after a warm-up.
 
     python tools/chunk_stream_bench.py [--quick] [--frames 20000]
 """

@@ -1,6 +1,7 @@
 """GPU: what a provisional pose costs a live caller.  ms per `PoseStream.push` and per `push` followed by `peek(K)`
-(gast_stream_peek) for the 27-frame/128ch and 81-frame/64ch non-causal models, n = 1, 64, 1024 streams, K = 1,
-latency/2 and latency, with and without augmentation.  Prints one JSON line per measurement, the first with the card's
+(gast_stream_peek_subset on its lockstep branch: the kernels of gast_stream_peek) for the 27-frame/128ch and
+81-frame/64ch non-causal models, n = 1, 64, 1024 streams, K = 1, latency/2 and latency, with and without
+augmentation.  Prints one JSON line per measurement, the first with the card's
 name, power limit and SM clock read in the same run.  CUDA events after a warm-up; each stream has pushed more than
 `latency` frames, so that every peek has poses due.
 
