@@ -880,27 +880,37 @@ extern "C" size_t gast_workspace_bytes(const gast_t* h, int32_t B, int32_t T, in
   return a.off + 256;
 }
 
+// The start of every model and streaming call once its own checks passed: a null or short workspace is refused, the
+// handle's device is made current and the launch counters and timing events restart for this call.  A backward
+// (restart_counts false) continues the counts of its training forward instead.
+static int call_begin(gast_handle* h, const char* who, size_t need, void* workspace, size_t workspace_bytes,
+                      bool restart_counts = true) {
+  if (!workspace || workspace_bytes < need)
+    return fail("%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
+  CUDA_OK(cudaSetDevice(h->cfg.device));
+  if (restart_counts) {
+    h->launches = h->tc_launches = h->wgrad_tc_launches = 0;
+    h->ev_used = 0;
+    h->ev_kind.clear();
+  }
+  return 0;
+}
+
 static int forward_impl(gast_t* h, const float* x, float* y, int32_t B, int32_t T, int32_t strided_now,
                         void* workspace, size_t workspace_bytes, void* stream, const float* target, float* loss) {
   if (!h) return fail("gast_forward: null handle");
   if (!h->prepared) return fail("gast_forward: gast_prepare() has not run since the last gast_bind()");
   if (B <= 0 || T <= 0) return fail("gast_forward: empty batch (B=%d T=%d)", B, T);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
-  h->launches = 0;
-  h->tc_launches = 0;
-  h->ev_used = 0;
-  h->ev_kind.clear();
+  const int kind = h->cfg.kind;
+  if (kind != GAST_KIND_MODEL && T != 1) return fail("gast_forward: module kinds take T == 1 (frames in B)");
   const size_t need = gast_workspace_bytes(h, B, T, strided_now);
   if (need == 0) return 1;
-  if (workspace_bytes < need || !workspace)
-    return fail("gast_forward: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+  if (call_begin(h, "gast_forward", need, workspace, workspace_bytes)) return 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   Arena a = workspace_arena(workspace, workspace_bytes);
   const int J = h->cfg.num_joints;
-  const int kind = h->cfg.kind;
 
   if (kind != GAST_KIND_MODEL) {
-    if (T != 1) return fail("gast_forward: module kinds take T == 1 (frames in B)");
     BlockConsts& b = h->blocks[0];
     BlockBufs bb;
     block_bufs(a, (long long)B * J, b.C, b.Cout, b.heads ? b.heads : 4, b.Cg ? b.Cg : b.C / 4, &bb);
@@ -1046,17 +1056,16 @@ extern "C" int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B
                                   uint64_t seed, void* workspace, size_t workspace_bytes, void* stream) {
   if (!h) return fail("gast_forward_train: null handle");
   if (train_check(h, "gast_forward_train")) return 1;
+  if (B <= 0 || T <= 0) return fail("gast_forward_train: empty batch (B=%d T=%d)", B, T);
+  if (!x || !y) return fail("gast_forward_train: x and y must be device pointers");
   if (dropout_p < 0.f || dropout_p >= 1.f) return fail("gast_forward_train: dropout_p out of range");
+  const size_t need = gast_train_workspace_bytes(h, B, T, dropout_p);
+  if (need == 0) return 1;
+  if (call_begin(h, "gast_forward_train", need, workspace, workspace_bytes)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
   Arena a = workspace_arena(workspace, workspace_bytes);
   Lookup L{h};
   TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
-  const size_t need = gast_train_workspace_bytes(h, B, T, dropout_p);
-  if (need == 0) return 1;
-  if (!workspace || workspace_bytes < need) return fail("gast_forward_train: workspace too small (%zu < %zu)", workspace_bytes, need);
-  h->launches = 0;
-  h->wgrad_tc_launches = 0;
   for (size_t i = 0; i < h->trains.size(); ++i)      // a workspace reused by the caller: its old state is dead
     if (h->trains[i].first == workspace) { h->trains.erase(h->trains.begin() + i); break; }
   if (h->trains.size() >= GAST_MAX_PENDING_TRAIN) h->trains.erase(h->trains.begin());   // forwards never differentiated
@@ -1064,6 +1073,7 @@ extern "C" int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B
   TrainState& ts = h->trains.back().second;
   ts.drop_p = dropout_p;
   ts.seed = seed;
+  ts.workspace_bytes = need;
   if (train_forward(h, c, ts, x, y, B, T)) { h->trains.pop_back(); return 1; }
   ts.arena_off = a.off;
   ts.valid = true;
@@ -1087,6 +1097,7 @@ extern "C" int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_
                                    size_t workspace_bytes, void* stream) {
   if (!h) return fail("gast_backward: null handle");
   if (precision_check(h, "gast_backward")) return 1;
+  if (!dy) return fail("gast_backward: dy must be a device pointer");
   if (!dx && !param_grads) return fail("gast_backward_input: neither dx nor parameter gradients requested");
   size_t ti = h->trains.size();
   for (size_t i = 0; i < h->trains.size(); ++i)
@@ -1094,8 +1105,8 @@ extern "C" int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_
   if (ti == h->trains.size() || !h->trains[ti].second.valid)
     return fail("gast_backward: no training forward is saved in this workspace (already differentiated, "
                 "or more than %d forwards were outstanding)", GAST_MAX_PENDING_TRAIN);
+  if (call_begin(h, "gast_backward", h->trains[ti].second.workspace_bytes, workspace, workspace_bytes, false)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
   TrainState ts = h->trains[ti].second;
   h->trains.erase(h->trains.begin() + ti);
   Arena a = workspace_arena(workspace, workspace_bytes, ts.arena_off);
@@ -1104,7 +1115,6 @@ extern "C" int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_
   c.tc_slot = 1024;                         // the backward's GEMMs follow the forward's in the operand-copy table
   c.pgrad = param_grads != 0;
   if (train_backward(h, c, ts, dy, dx)) return 1;
-  if (a.off > workspace_bytes) return fail("gast_backward: workspace overrun");
   CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -1131,22 +1141,43 @@ extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, fl
   TrainState ts = eval_state(strided_now);
   const size_t need = train_dry_run_bytes(h, B, T, ts, param_grads != 0, "gast_eval_backward");
   if (need == 0) return 1;
-  if (!workspace || workspace_bytes < need)
-    return fail("gast_eval_backward: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+  if (call_begin(h, "gast_eval_backward", need, workspace, workspace_bytes)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
   Arena a = workspace_arena(workspace, workspace_bytes);
   Lookup L{h};
   TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
   c.pgrad = param_grads != 0;
-  h->launches = 0;
-  h->wgrad_tc_launches = 0;
   if (train_forward(h, c, ts, x, nullptr, B, T)) return 1;
   c.tc_slot = 1024;
   if (train_backward(h, c, ts, dy, dx)) return 1;
-  if (a.off > workspace_bytes) return fail("gast_eval_backward: workspace overrun");
   CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+// Timing of the debug entries: `launch` once, then `reps` more times between two events on `st`; waits for the stream
+// and, when all of it succeeded and reps > 0, stores the ms per rep in *ms_out.  Returns 0, the first failing launch's
+// code or the stream's error.
+template <class Launch>
+static int timed_reps(cudaStream_t st, int reps, float* ms_out, Launch launch) {
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  int rc = (int)cudaEventCreate(&e0);
+  if (!rc) rc = (int)cudaEventCreate(&e1);
+  if (!rc) rc = launch();
+  if (!rc && reps > 0) {
+    cudaEventRecord(e0, st);
+    for (int i = 0; i < reps && !rc; ++i) rc = launch();
+    cudaEventRecord(e1, st);
+  }
+  const cudaError_t e = cudaStreamSynchronize(st);
+  if (!rc) rc = (int)e;
+  if (!rc && reps > 0 && ms_out) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e0, e1);
+    *ms_out = ms / reps;
+  }
+  if (e0) cudaEventDestroy(e0);
+  if (e1) cudaEventDestroy(e1);
+  return rc;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1176,31 +1207,14 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
   } else {
     cudaFuncSetAttribute((const void*)gemm_ffma_kernel<EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   }
-  auto launch = [&]() -> int {
+  rc = timed_reps(st, reps, ms_out, [&]() -> int {
     if (core == 0) return tc_launch(st, EPI_PLAIN, p, t, tc_prec(t, tc_mode));
     dim3 grid(cdiv(M, 128), cdiv(N, FF_BN));
     gemm_ffma_kernel<EPI_PLAIN><<<grid, FF_THREADS, ffma_smem_bytes(EPI_PLAIN, 1, 128, 1), st>>>(p);
     return (int)cudaGetLastError();
-  };
-  cudaEvent_t e0, e1;
-  CUDA_OK(cudaEventCreate(&e0));
-  CUDA_OK(cudaEventCreate(&e1));
-  rc = launch();
-  if (!rc && reps > 0) {
-    cudaEventRecord(e0, st);
-    for (int i = 0; i < reps && !rc; ++i) rc = launch();
-    cudaEventRecord(e1, st);
-  }
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (!rc && e == cudaSuccess && reps > 0 && ms_out) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    *ms_out = ms / reps;
-  }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
+  });
   for (void* q : owned) cudaFree(q);
-  if (rc || e != cudaSuccess) return fail("gast_debug_gemm: %s", cudaGetErrorString(rc ? (cudaError_t)rc : e));
+  if (rc) return fail("gast_debug_gemm: %s", cudaGetErrorString((cudaError_t)rc));
   return 0;
 }
 
@@ -1229,26 +1243,10 @@ extern "C" int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int3
   float* part = nullptr;
   CUDA_OK(cudaMalloc(&part, sizeof(float) * (size_t)S * N * K));
   bool on_tc = false;
-  auto launch = [&]() { return wgrad_run(st, dZ, N, A, K, M, N, K, S, rps, part, dW, K, core == 0, &on_tc); };
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0);
-  cudaEventCreate(&e1);
-  int rc = launch();
-  if (!rc && reps > 0) {
-    cudaEventRecord(e0, st);
-    for (int i = 0; i < reps && !rc; ++i) rc = launch();
-    cudaEventRecord(e1, st);
-  }
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (!rc && e == cudaSuccess && reps > 0 && ms_out) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    *ms_out = ms / reps;
-  }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
+  const int rc = timed_reps(st, reps, ms_out,
+                            [&]() { return wgrad_run(st, dZ, N, A, K, M, N, K, S, rps, part, dW, K, core == 0, &on_tc); });
   cudaFree(part);
-  if (rc || e != cudaSuccess) return fail("gast_debug_wgrad: %s", cudaGetErrorString(rc ? (cudaError_t)rc : e));
+  if (rc) return fail("gast_debug_wgrad: %s", cudaGetErrorString((cudaError_t)rc));
   return 0;
 }
 

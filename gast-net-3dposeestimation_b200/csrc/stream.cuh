@@ -286,17 +286,6 @@ extern "C" int32_t gast_stream_latency(const gast_t* h) {
   return h->cfg.causal ? 0 : (gast_receptive_field(h) - 1) / 2;
 }
 
-// The start of every streaming call once its own checks passed: the handle's weights must be prepared; then its device
-// is made current and the launch counters restart for this call.
-static int stream_call_begin(gast_handle* h, const char* who) {
-  if (!h->prepared) return fail("%s: gast_prepare() has not run since the last gast_bind()", who);
-  CUDA_OK(cudaSetDevice(h->cfg.device));
-  h->launches = h->tc_launches = 0;
-  h->ev_used = 0;
-  h->ev_kind.clear();
-  return 0;
-}
-
 extern "C" int gast_stream_push_ex(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
                                    const int32_t* fresh, const int32_t* hold, void* workspace, size_t workspace_bytes,
                                    void* stream) {
@@ -304,10 +293,9 @@ extern "C" int gast_stream_push_ex(gast_t* h, void* state, int64_t step, const f
   if (step < 0 || !state || !x || !y) return fail("gast_stream_push_ex: bad arguments");
   StreamPlan sp;
   if (stream_plan(h, n_streams, &sp)) return 1;
-  const size_t need = gast_stream_workspace_bytes(h, n_streams);
-  if (!workspace || workspace_bytes < need)
-    return fail("gast_stream_push_ex: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
-  if (stream_call_begin(h, "gast_stream_push_ex")) return 1;
+  if (!h->prepared) return fail("gast_stream_push_ex: gast_prepare() has not run since the last gast_bind()");
+  if (call_begin(h, "gast_stream_push_ex", gast_stream_workspace_bytes(h, n_streams), workspace, workspace_bytes))
+    return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (!h->stream_ready && stream_prepare(h, st)) return 1;
   const gast_cfg& c = h->cfg;
@@ -515,9 +503,8 @@ static int chunk_call(const char* who, gast_handle* h, void* state, int n_stream
   if (streams && subset_table(sp, streams, steps, m, peek ? 1 : 0, who, &tab, &lockstep)) return 1;
   const size_t need = chunk_workspace_bytes(h, sp, m, K, streams != nullptr, who);
   if (need == 0) return 1;
-  if (!workspace || workspace_bytes < need)
-    return fail("%s: workspace too small (%zu < %zu bytes)", who, workspace_bytes, need);
-  if (stream_call_begin(h, who)) return 1;
+  if (!h->prepared) return fail("%s: gast_prepare() has not run since the last gast_bind()", who);
+  if (call_begin(h, who, need, workspace, workspace_bytes)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0], JF = J * h->cfg.in_features;
   float* sbase = reinterpret_cast<float*>(align256(state));

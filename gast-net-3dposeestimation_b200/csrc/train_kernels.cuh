@@ -591,17 +591,6 @@ __global__ void rowdot_bwd_x_kernel(const float* __restrict__ dab, const float* 
   dX[m * ldx + k] += s;
 }
 
-// dU[q][k] = sum_m dab[m][q] X[m][k]   (thread per (q,k); rows in double)
-__global__ void rowdot_bwd_u_kernel(const float* __restrict__ dab, const float* __restrict__ X, int ldx, int Q,
-                                    long long M, int K, float* __restrict__ dU) {
-  int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= Q * K) return;
-  int q = idx / K, k = idx - q * K;
-  double s = 0.0;
-  for (long long m = 0; m < M; ++m) s += (double)dab[m * Q + q] * (double)X[m * ldx + k];
-  dU[idx] = (float)s;
-}
-
 // parameter gradients of one head from dU (2 rows) and dcab (2 values); see global_collapse_kernel
 __global__ void global_collapse_bwd_kernel(const float* __restrict__ dU, const float* __restrict__ dcab, int h, int C,
                                            int Ci, const float* __restrict__ tw, const float* __restrict__ tb,

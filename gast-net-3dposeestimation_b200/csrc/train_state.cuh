@@ -47,5 +47,7 @@ struct TrainState {
   long long Flast = 0;
   float drop_p = 0.f; unsigned long long seed = 0; unsigned long long drop_ctr = 0;
   size_t arena_off = 0;          // workspace used by the forward (backward temporaries go after it)
+  size_t workspace_bytes = 0;    // what the forward checked: its own dry run plus a backward with parameter gradients,
+                                 // which bounds every backward of it
 };
 

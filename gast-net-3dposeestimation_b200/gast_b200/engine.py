@@ -9,6 +9,8 @@ a cached workspace from the caching allocator) and the current CUDA stream -- pl
 No fallback: CPU tensors, a missing library or an unsupported mode raise.
 """
 import ctypes as C
+import math
+
 import torch
 
 from . import _lib as L
@@ -93,28 +95,16 @@ def _m2d(m):
 
 
 def named_tensors(module):
-    """(key, tensor) pairs under the names `module.state_dict()` uses, in its order.  Unlike state_dict() this
-    also works on the per-forward replicas of nn.DataParallel (trainval.py:56-61), whose weights are broadcast
-    views kept as plain attributes (`_former_parameters`) instead of in `_parameters`."""
-    out = []
-    for prefix, mod in module.named_modules():
-        pre = prefix + '.' if prefix else ''
-        former = getattr(mod, '_former_parameters', None) or {}
-        for k, v in mod._parameters.items():
-            if v is not None:
-                out.append((pre + k, v))
-        for k, v in former.items():
-            if v is not None and mod._parameters.get(k) is None:
-                out.append((pre + k, v))
-        for k, v in mod._buffers.items():
-            if v is not None and k not in mod._non_persistent_buffers_set:
-                out.append((pre + k, v))
-    return out
+    """(key, tensor) pairs under the names `module.state_dict()` uses, in its order: named_params with the persistent
+    buffers.  Unlike state_dict() this also works on the per-forward replicas of nn.DataParallel (trainval.py:56-61),
+    whose weights are broadcast views kept as plain attributes (`_former_parameters`) instead of in `_parameters`."""
+    return named_params(module, buffers=True)
 
 
-def named_params(module):
+def named_params(module, buffers=False):
     """named_parameters() that also sees the broadcast parameter views of a DataParallel replica
-    (they are non-leaf tensors connected to the real parameters, so autograd routes the gradients)."""
+    (they are non-leaf tensors connected to the real parameters, so autograd routes the gradients); with `buffers`
+    each module's persistent buffers follow its parameters."""
     out = []
     for prefix, mod in module.named_modules():
         pre = prefix + '.' if prefix else ''
@@ -125,6 +115,10 @@ def named_params(module):
         for k, v in former.items():
             if v is not None and mod._parameters.get(k) is None:
                 out.append((pre + k, v))
+        if buffers:
+            for k, v in mod._buffers.items():
+                if v is not None and k not in mod._non_persistent_buffers_set:
+                    out.append((pre + k, v))
     return out
 
 
@@ -203,64 +197,30 @@ class _Handle(object):
         self.apply_core(module)
         if sig == self.sig:
             return
-        n = len(items)
-        keys = (C.c_char_p * n)()
-        ptrs = (C.c_void_p * n)()
-        numel = (C.c_int64 * n)()
-        for i, (k, v) in enumerate(items):
-            if not v.is_cuda or v.device != self.device:
-                raise GastError('parameter %r is on %s, expected %s (call .cuda() on the module)'
-                                % (k, v.device, self.device))
-            if v.dtype == torch.float32 and not v.is_contiguous():
-                raise GastError('parameter %r is not contiguous' % k)
-            keys[i] = k.encode()
-            ptrs[i] = v.data_ptr()
-            numel[i] = v.numel()
-        _check(self.lib.gast_bind(self.h, n, keys, ptrs, numel), 'gast_bind')
+        _bind(self, 'gast_bind', items)
         _check(self.lib.gast_prepare(self.h, C.c_void_p(stream)), 'gast_prepare')
         self.sig = sig
 
     def bind_only(self, module):
         """bind parameter/buffer storage without the eval-mode prepare (training path)"""
         self.apply_core(module)
-        items = named_tensors(module)
-        n = len(items)
-        keys = (C.c_char_p * n)()
-        ptrs = (C.c_void_p * n)()
-        numel = (C.c_int64 * n)()
-        for i, (k, v) in enumerate(items):
-            if not v.is_cuda or v.device != self.device:
-                raise GastError('parameter %r is on %s, expected %s' % (k, v.device, self.device))
-            if not v.is_contiguous():
-                raise GastError('parameter %r is not contiguous' % k)
-            keys[i] = k.encode()
-            ptrs[i] = v.data_ptr()
-            numel[i] = v.numel()
-        _check(self.lib.gast_bind(self.h, n, keys, ptrs, numel), 'gast_bind')
+        _bind(self, 'gast_bind', named_tensors(module))
         self.sig = None
 
-    def forward(self, x, y, B, T, strided_now, stream):
+    def forward(self, x, y, B, T, strided_now, stream, target=None, loss=None):
+        """gast_forward, or with a target gast_forward_mpjpe, on the handle's grow-only workspace self.ws"""
         need = self.lib.gast_workspace_bytes(self.h, B, T, strided_now)
         if need == 0:
             raise GastError('gast_workspace_bytes: %s' % L.last_error())
         if self.ws is None or self.ws.numel() < need:
             self.ws = None
             self.ws = torch.empty(int(need), dtype=torch.uint8, device=self.device)
-        _check(self.lib.gast_forward(self.h, C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), B, T,
-                                     strided_now, C.c_void_p(self.ws.data_ptr()), self.ws.numel(),
-                                     C.c_void_p(stream)), 'gast_forward')
-
-    def forward_mpjpe(self, x, target, y, loss, B, T, strided_now, stream):
-        need = self.lib.gast_workspace_bytes(self.h, B, T, strided_now)
-        if need == 0:
-            raise GastError('gast_workspace_bytes: %s' % L.last_error())
-        if self.ws is None or self.ws.numel() < need:
-            self.ws = None
-            self.ws = torch.empty(int(need), dtype=torch.uint8, device=self.device)
-        _check(self.lib.gast_forward_mpjpe(self.h, C.c_void_p(x.data_ptr()), C.c_void_p(target.data_ptr()),
-                                           C.c_void_p(y.data_ptr()), C.c_void_p(loss.data_ptr()), B, T, strided_now,
-                                           C.c_void_p(self.ws.data_ptr()), self.ws.numel(), C.c_void_p(stream)),
-               'gast_forward_mpjpe')
+        tail = (B, T, strided_now, _p(self.ws), self.ws.numel(), C.c_void_p(stream))
+        if target is None:
+            _check(self.lib.gast_forward(self.h, _p(x), _p(y), *tail), 'gast_forward')
+        else:
+            _check(self.lib.gast_forward_mpjpe(self.h, _p(x), _p(target), _p(y), _p(loss), *tail),
+                   'gast_forward_mpjpe')
 
     def launches(self):
         return int(self.lib.gast_last_launch_count(self.h))
@@ -270,11 +230,42 @@ class _Handle(object):
         return int(self.lib.gast_last_wgrad_tc_launch_count(self.h))
 
 
-def _require_cuda(x, what):
+def _bind(handle, entry, items):
+    """hand (key, tensor) pairs to the library entry `entry` (gast_bind or gast_bind_grads) of `handle`"""
+    n = len(items)
+    keys = (C.c_char_p * n)()
+    ptrs = (C.c_void_p * n)()
+    numel = (C.c_int64 * n)()
+    for i, (k, v) in enumerate(items):
+        if not v.is_cuda or v.device != handle.device:
+            raise GastError('parameter %r is on %s, expected %s (call .cuda() on the module)'
+                            % (k, v.device, handle.device))
+        if not v.is_contiguous():
+            raise GastError('parameter %r is not contiguous' % k)
+        keys[i] = k.encode()
+        ptrs[i] = v.data_ptr()
+        numel[i] = v.numel()
+    _check(getattr(handle.lib, entry)(handle.h, n, keys, ptrs, numel), entry)
+
+
+def _p(t):
+    """a tensor's device pointer for the C ABI (None: null)"""
+    return C.c_void_p(t.data_ptr() if t is not None else None)
+
+
+def _cuda_f32(x, what):
+    """x as a contiguous CUDA float32 tensor; anything else raises (there is no CPU path)"""
     if not isinstance(x, torch.Tensor) or not x.is_cuda:
         raise GastError('%s: input must be a CUDA tensor -- this implementation has no CPU path' % what)
     if x.dtype != torch.float32:
         raise GastError('%s: input must be float32 (got %s)' % (what, x.dtype))
+    return x.contiguous()
+
+
+def _ilist(v):
+    """a host int32 array of the indices `v` (None: none) for the C ABI, and their count"""
+    v = [] if v is None else list(v)
+    return (C.c_int32 * max(len(v), 1))(*[int(i) for i in v]), len(v)
 
 
 def _handle_for(module, device, factory):
@@ -309,19 +300,14 @@ class _TrainFn(torch.autograd.Function):
             if need == 0:
                 raise GastError('gast_train_workspace_bytes: %s' % L.last_error())
             ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
-            T_out = lib.gast_out_frames(handle.h, T, 1 if module._gast_strided else 0)
-            if T_out <= 0:
-                raise GastError('forward: %s' % L.last_error())
-            y = torch.empty((B, T_out, module.num_joints_in, 3), dtype=torch.float32, device=dev)
+            y = _new_output(module, handle, B, T, 1 if module._gast_strided else 0, dev)
             p = float(module._gast_dropout)
             seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if p > 0 else 0
             # device-side dropout counter (set by a graph-capturing trainer): keeps the masks fresh across replays
             ds = module.__dict__.get('_gast_dropout_state')
-            _check(lib.gast_set_dropout_state(handle.h, C.c_void_p(ds.data_ptr() if ds is not None else None)),
-                   'gast_set_dropout_state')
-            _check(lib.gast_forward_train(handle.h, C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), B, T,
-                                          C.c_float(p), C.c_uint64(seed), C.c_void_p(ws.data_ptr()), ws.numel(),
-                                          C.c_void_p(st)), 'gast_forward_train')
+            _check(lib.gast_set_dropout_state(handle.h, _p(ds)), 'gast_set_dropout_state')
+            _check(lib.gast_forward_train(handle.h, _p(x), _p(y), B, T, C.c_float(p), C.c_uint64(seed), _p(ws),
+                                          ws.numel(), C.c_void_p(st)), 'gast_forward_train')
         # BatchNorm bookkeeping that torch does in Python: num_batches_tracked (this also bumps the
         # buffers' versions, so the eval-mode constants are refreshed on the next eval forward)
         with torch.no_grad():
@@ -355,10 +341,8 @@ class _TrainFn(torch.autograd.Function):
             views = _bind_grad_views(handle, names, params, direct, ctx.dev) if need_p else None
             # no parameter needs a gradient (all frozen, only x is differentiated): the library skips every
             # weight-gradient kernel
-            _check(lib.gast_backward_input(handle.h, C.c_void_p(dy.data_ptr()),
-                                           C.c_void_p(dx.data_ptr() if dx is not None else None), 1 if need_p else 0,
-                                           C.c_void_p(ws.data_ptr()), ws.numel(), C.c_void_p(_stream(ctx.dev))),
-                   'gast_backward')
+            _check(lib.gast_backward_input(handle.h, _p(dy), _p(dx), 1 if need_p else 0, _p(ws), ws.numel(),
+                                           C.c_void_p(_stream(ctx.dev))), 'gast_backward')
         ctx.ws = None
         ctx.x = None
         if direct or views is None:
@@ -369,20 +353,12 @@ class _TrainFn(torch.autograd.Function):
 def _bind_grad_views(handle, names, params, direct, dev):
     """bind one gradient buffer per parameter (gast_bind_grads): the parameters' own .grad when `direct`, else views of
     one fresh flat buffer, which are returned for autograd to accumulate"""
-    n = len(params)
-    keys = (C.c_char_p * n)()
-    ptrs = (C.c_void_p * n)()
-    numel = (C.c_int64 * n)()
     flat = None if direct else torch.empty(sum(p.numel() for p in params), dtype=torch.float32, device=dev)
     views, off = [], 0
-    for i, (k, p) in enumerate(zip(names, params)):
-        v = p.grad if direct else flat[off:off + p.numel()].view_as(p)
-        views.append(v)
-        keys[i] = k.encode()
-        ptrs[i] = v.data_ptr()
-        numel[i] = p.numel()
+    for p in params:
+        views.append(p.grad if direct else flat[off:off + p.numel()].view_as(p))
         off += p.numel()
-    _check(handle.lib.gast_bind_grads(handle.h, n, keys, ptrs, numel), 'gast_bind_grads')
+    _bind(handle, 'gast_bind_grads', list(zip(names, views)))
     return views
 
 
@@ -422,10 +398,8 @@ class _EvalFn(torch.autograd.Function):
             ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
             dx = torch.empty_like(x) if need_x else None
             views = _bind_grad_views(h, ctx.names, params, False, dev) if need_p else None
-            _check(lib.gast_eval_backward(h.h, C.c_void_p(x.data_ptr()), C.c_void_p(dy.data_ptr()),
-                                          C.c_void_p(dx.data_ptr() if dx is not None else None), 1 if need_p else 0,
-                                          B, T, ctx.sn, C.c_void_p(ws.data_ptr()), ws.numel(), C.c_void_p(st)),
-                   'gast_eval_backward')
+            _check(lib.gast_eval_backward(h.h, _p(x), _p(dy), _p(dx), 1 if need_p else 0, B, T, ctx.sn, _p(ws),
+                                          ws.numel(), C.c_void_p(st)), 'gast_eval_backward')
         return (None, None, dx, None, None) + (tuple(views) if views is not None else (None,) * ctx.n)
 
 
@@ -450,185 +424,130 @@ def model_handle(module, dev):
     return _handle_for(module, dev, make)
 
 
+def _strided_now(module, T):
+    """1 when the strided schedule runs: always for Optimized1f, and for a dilated model fed exactly one receptive
+    field, which computes only what the strided schedule computes (same arithmetic per output), so the unused
+    positions are skipped"""
+    return 1 if (module._gast_strided or (T == module.receptive_field() and not module._gast_dense)) else 0
+
+
 def run_model(module, x):
     """SpatioTemporalModelBase.forward (gast_net.py:84-104) on the CUDA library."""
-    _require_cuda(x, 'SpatioTemporalModel.forward')
-    dev = x.device
-    h = model_handle(module, dev)
-    x = x.contiguous()
-    B, T = int(x.shape[0]), int(x.shape[1])
+    x = _cuda_f32(x, 'SpatioTemporalModel.forward')
+    h = model_handle(module, x.device)
     if module.training:
         _fp32_only(module, 'SpatioTemporalModel.forward in train mode')
         # both of the reference's training models: Optimized1f (main.py:166-170) and, with
         # --disable-optimizations / stride > 1, the dilated SpatioTemporalModel (main.py:171-175)
         np_ = named_params(module)
-        names = [k for k, _ in np_]
-        params = [p for _, p in np_]
-        y = _TrainFn.apply(module, h, x, names, *params)
-        module.__dict__['_gast_last_launches'] = h.launches()
-        return y
-    # A dilated model fed exactly one receptive field computes only what the strided
-    # schedule computes (same arithmetic per output); skip the unused positions.
-    strided_now = 1 if (module._gast_strided or
-                        (T == module.receptive_field() and not module._gast_dense)) else 0
-    np_ = named_params(module) if torch.is_grad_enabled() else []
-    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for _, p in np_)):
-        # the reference's output would carry a grad_fn here: same forward, plus a backward
-        _fp32_only(module, 'SpatioTemporalModel.forward with autograd (requires_grad input or parameters)')
-        y = _EvalFn.apply(module, h, x, strided_now, [k for k, _ in np_], *[p for _, p in np_])
+        y = _TrainFn.apply(module, h, x, [k for k, _ in np_], *[p for _, p in np_])
     else:
-        y = _eval_forward(module, h, x, strided_now)
+        strided_now = _strided_now(module, int(x.shape[1]))
+        np_ = named_params(module) if torch.is_grad_enabled() else []
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for _, p in np_)):
+            # the reference's output would carry a grad_fn here: same forward, plus a backward
+            _fp32_only(module, 'SpatioTemporalModel.forward with autograd (requires_grad input or parameters)')
+            y = _EvalFn.apply(module, h, x, strided_now, [k for k, _ in np_], *[p for _, p in np_])
+        else:
+            y = _eval_forward(module, h, x, strided_now)
     module.__dict__['_gast_last_launches'] = h.launches()
     return y
 
 
-def _eval_forward(module, h, x, strided_now):
-    """the eval-mode forward (gast_forward) of x (B,T,J,F) -> (B,T_out,J,3)"""
+def _eval_forward(module, h, x, strided_now, target=None):
+    """the eval-mode forward (gast_forward) of x (B,T,J,F) -> y (B,T_out,J,3); with a target of y's shape it returns
+    (y, loss), loss the mpjpe of y against it as a 0-d tensor (gast_forward_mpjpe)"""
     dev = x.device
     B, T = int(x.shape[0]), int(x.shape[1])
     with torch.cuda.device(dev):
         st = _stream(dev)
         h.refresh(module, st)
-        T_out = h.lib.gast_out_frames(h.h, T, strided_now)
-        if T_out <= 0:
-            raise GastError('forward: %s' % L.last_error())
-        y = torch.empty((B, T_out, module.num_joints_in, 3), dtype=torch.float32, device=dev)
-        h.forward(x, y, B, T, strided_now, st)
-    return y
+        y = _new_output(module, h, B, T, strided_now, dev)
+        if target is None:
+            h.forward(x, y, B, T, strided_now, st)
+            return y
+        if target.shape != y.shape or target.device != dev:
+            raise GastError('run_model_mpjpe: target must be %s on %s (got %s on %s)'
+                            % (tuple(y.shape), dev, tuple(target.shape), target.device))
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        h.forward(x, y, B, T, strided_now, st, target, loss)
+    return y, loss
+
+
+def _new_output(module, h, B, T, strided_now, dev):
+    """an empty (B, T_out, J, 3) model output for an input of T frames on the schedule `strided_now`"""
+    T_out = h.lib.gast_out_frames(h.h, T, strided_now)
+    if T_out <= 0:
+        raise GastError('forward: %s' % L.last_error())
+    return torch.empty((B, T_out, module.num_joints_in, 3), dtype=torch.float32, device=dev)
 
 
 def run_model_mpjpe(module, x, target):
     """`predicted = model(x); error = mpjpe(predicted, target)` (main.py:270-300, common/loss.py:5-11) as ONE library
     call: the loss is taken in the shrink kernel's epilogue.  Eval mode; returns (predicted, loss) with loss a 0-d
     CUDA tensor.  (The training loss goes through gast_b200.pipeline.mpjpe, which also produces the gradient.)"""
-    _require_cuda(x, 'run_model_mpjpe')
-    _require_cuda(target, 'run_model_mpjpe (target)')
+    x = _cuda_f32(x, 'run_model_mpjpe')
+    target = _cuda_f32(target, 'run_model_mpjpe (target)')
     _no_train(module, 'run_model_mpjpe')
-    dev = x.device
-    h = model_handle(module, dev)
-    x = x.contiguous()
-    B, T = int(x.shape[0]), int(x.shape[1])
-    strided_now = 1 if (module._gast_strided or
-                        (T == module.receptive_field() and not module._gast_dense)) else 0
-    with torch.cuda.device(dev):
-        st = _stream(dev)
-        h.refresh(module, st)
-        T_out = h.lib.gast_out_frames(h.h, T, strided_now)
-        if T_out <= 0:
-            raise GastError('forward: %s' % L.last_error())
-        shape = (B, T_out, module.num_joints_in, 3)
-        if tuple(target.shape) != shape or target.device != dev:
-            raise GastError('run_model_mpjpe: target must be %s on %s (got %s on %s)'
-                            % (shape, dev, tuple(target.shape), target.device))
-        target = target.contiguous()
-        y = torch.empty(shape, dtype=torch.float32, device=dev)
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        h.forward_mpjpe(x, target, y, loss, B, T, strided_now, st)
+    h = model_handle(module, x.device)
+    y, loss = _eval_forward(module, h, x, _strided_now(module, int(x.shape[1])), target)
     module.__dict__['_gast_last_launches'] = h.launches()
     return y, loss
 
 
-def run_block(module, x):
-    """GraphAttentionBlock.forward: x (B,C,T,N) -> (B,2C,T,N) (gast_net.py:22-33)."""
-    _require_cuda(x, 'GraphAttentionBlock.forward')
-    _no_train(module, 'GraphAttentionBlock.forward')
+def _run_module(module, x, what, kind, cfg, width_out, masks=None, train_ok=False):
+    """The forward of a sub-module on its own, channels-last: x (..., J, C) -> (..., J, width_out), all leading rows in
+    one library call.  Only a sub-module without BatchNorm or dropout (train_ok) also runs in train mode."""
+    x = _cuda_f32(x, what)
+    if not train_ok:
+        _no_train(module, what)
     dev = x.device
-    lg = module.local_graph_layer
-    Bn, Cc, T, N = x.shape
-
-    def make():
-        return _Handle(module, L.KIND_BLOCK, dev, dict(num_joints=N, channels=Cc, heads=4),
-                       sym=lg.gcn_sym.m, con=lg.gcn_con.m)
-    h = _handle_for(module, dev, make)
-    xl = x.permute(0, 2, 3, 1).contiguous()
+    *lead, N, Cc = x.shape
+    h = _handle_for(module, dev, lambda: _Handle(module, kind, dev, dict(num_joints=N, channels=Cc, **cfg),
+                                                 **(masks or {})))
     with torch.cuda.device(dev):
         st = _stream(dev)
         h.refresh(module, st)
-        y = torch.empty((Bn, T, N, 2 * Cc), dtype=torch.float32, device=dev)
-        h.forward(xl, y, Bn * T, 1, 0, st)
-    return y.permute(0, 3, 1, 2)
+        y = torch.empty((*lead, N, width_out), dtype=torch.float32, device=dev)
+        h.forward(x, y, math.prod(lead), 1, 0, st)
+    return y
+
+
+def run_block(module, x):
+    """GraphAttentionBlock.forward: x (B,C,T,N) -> (B,2C,T,N) (gast_net.py:22-33)."""
+    lg = module.local_graph_layer
+    return _run_module(module, x.permute(0, 2, 3, 1), 'GraphAttentionBlock.forward', L.KIND_BLOCK, dict(heads=4),
+                       2 * x.shape[1], dict(sym=lg.gcn_sym.m, con=lg.gcn_con.m)).permute(0, 3, 1, 2)
 
 
 def run_local(module, x):
     """LocalGraph.forward: (B,T,J,C) -> (B,T,J,C) (local_attention.py:130-151)."""
-    _require_cuda(x, 'LocalGraph.forward')
-    _no_train(module, 'LocalGraph.forward')
-    dev = x.device
-    Bn, T, N, Cc = x.shape
-
-    def make():
-        return _Handle(module, L.KIND_LOCAL, dev, dict(num_joints=N, channels=Cc),
-                       sym=module.gcn_sym.m, con=module.gcn_con.m)
-    h = _handle_for(module, dev, make)
-    xl = x.contiguous()
-    with torch.cuda.device(dev):
-        st = _stream(dev)
-        h.refresh(module, st)
-        y = torch.empty((Bn, T, N, Cc), dtype=torch.float32, device=dev)
-        h.forward(xl, y, Bn * T, 1, 0, st)
-    return y
+    return _run_module(module, x, 'LocalGraph.forward', L.KIND_LOCAL, {}, x.shape[-1],
+                       dict(sym=module.gcn_sym.m, con=module.gcn_con.m))
 
 
 def run_semch(module, x):
     """SemCHGraphConv.forward / SemGraphConv.forward: (B,T,J,Cin) -> (B,T,J,Cout)."""
-    _require_cuda(x, 'SemCHGraphConv.forward')
-    dev = x.device
-    Bn, T, N, Cc = x.shape
     shared = 1 if module.e.shape[0] == 1 and module.out_features != 1 else 0
-
-    def make():
-        return _Handle(module, L.KIND_SEMCH, dev, dict(
-            num_joints=N, channels=Cc, channels_out=module.out_features, semch_shared_e=shared,
-            semch_bias=1 if module.bias is not None else 0), sym=module.m)
-    h = _handle_for(module, dev, make)
-    xl = x.contiguous()
-    with torch.cuda.device(dev):
-        st = _stream(dev)
-        h.refresh(module, st)
-        y = torch.empty((Bn, T, N, module.out_features), dtype=torch.float32, device=dev)
-        h.forward(xl, y, Bn * T, 1, 0, st)
-    return y
+    return _run_module(module, x, 'SemCHGraphConv.forward', L.KIND_SEMCH,
+                       dict(channels_out=module.out_features, semch_shared_e=shared,
+                            semch_bias=1 if module.bias is not None else 0),
+                       module.out_features, dict(sym=module.m), train_ok=True)
 
 
 def run_multi_global(module, x):
     """MultiGlobalGraph.forward: (B,T,J,C) -> (B,T,J,C) (global_attention.py:103-130)."""
-    _require_cuda(x, 'MultiGlobalGraph.forward')
-    _no_train(module, 'MultiGlobalGraph.forward')
-    dev = x.device
-    Bn, T, N, Cc = x.shape
-
-    def make():
-        return _Handle(module, L.KIND_MGLOBAL, dev, dict(num_joints=N, channels=Cc,
-                                                         heads=module.num_non_local))
-    h = _handle_for(module, dev, make)
-    xl = x.contiguous()
-    with torch.cuda.device(dev):
-        st = _stream(dev)
-        h.refresh(module, st)
-        y = torch.empty((Bn, T, N, Cc), dtype=torch.float32, device=dev)
-        h.forward(xl, y, Bn * T, 1, 0, st)
-    return y
+    return _run_module(module, x, 'MultiGlobalGraph.forward', L.KIND_MGLOBAL, dict(heads=module.num_non_local),
+                       x.shape[-1])
 
 
 def run_global_head(module, x):
     """GlobalGraph.forward: (B*T, C, N) -> (B*T, Cg, N) (global_attention.py:52-82)."""
-    _require_cuda(x, 'GlobalGraph.forward')
-    dev = x.device
-    BT, Cc, N = x.shape
     if module.g_channels != module.inter_channels:
         raise GastError('GlobalGraph with inter_channels == in_channels//2 is not on the lifting path')
-
-    def make():
-        return _Handle(module, L.KIND_GLOBAL_HEAD, dev, dict(num_joints=N, channels=Cc,
-                                                             channels_out=module.inter_channels, heads=1))
-    h = _handle_for(module, dev, make)
-    xl = x.permute(0, 2, 1).contiguous()
-    with torch.cuda.device(dev):
-        st = _stream(dev)
-        h.refresh(module, st)
-        y = torch.empty((BT, N, module.g_channels), dtype=torch.float32, device=dev)
-        h.forward(xl, y, BT, 1, 0, st)
-    return y.permute(0, 2, 1)
+    return _run_module(module, x.permute(0, 2, 1), 'GlobalGraph.forward', L.KIND_GLOBAL_HEAD,
+                       dict(channels_out=module.inter_channels, heads=1), module.g_channels,
+                       train_ok=True).permute(0, 2, 1)
 
 
 LAUNCH_KINDS = ['expand', 'gemm_ffma_plain', 'gemm_ffma_semch', 'gemm_ffma_global', 'rowdot', 'shrink',

@@ -10,26 +10,9 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .engine import GastError, _check, _stream
+from .engine import GastError, _check, _cuda_f32, _ilist, _p, _stream
 
 KPT_COCO_H36M, KPT_MPII_H36M, KPT_COCO_H36M_TOE = 0, 1, 2
-
-
-def _ilist(v):
-    v = [] if v is None else list(v)
-    return (C.c_int32 * max(len(v), 1))(*[int(i) for i in v]), len(v)
-
-
-def _cuda_f32(x, what):
-    if not isinstance(x, torch.Tensor) or not x.is_cuda:
-        raise GastError('%s: a CUDA tensor is required (there is no CPU path)' % what)
-    if x.dtype != torch.float32:
-        raise GastError('%s: float32 expected, got %s' % (what, x.dtype))
-    return x.contiguous()
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -10,38 +10,35 @@ import ctypes as C
 import torch
 
 from . import _lib as L
-from .engine import GastError, _check, _stream
-
-
-def _ilist(v):
-    return (C.c_int32 * len(v))(*[int(i) for i in v])
+from .engine import GastError, _check, _cuda_f32, _ilist, _stream
 
 
 def tta_prepare(seq, pad, causal_shift, kps_left, kps_right):
     """seq (T,J,F) CUDA float32 -> (2, T+2*pad, J, F)."""
-    if not seq.is_cuda or seq.dtype != torch.float32:
-        raise GastError('tta_prepare: CUDA float32 tensor expected')
-    seq = seq.contiguous()
+    seq = _cuda_f32(seq, 'tta_prepare')
     T, J, F = (int(s) for s in seq.shape)
     out = torch.empty((2, T + 2 * pad, J, F), dtype=torch.float32, device=seq.device)
+    kl, n = _ilist(kps_left)
+    kr, _ = _ilist(kps_right)
     with torch.cuda.device(seq.device):
         _check(L.load().gast_tta_prepare(C.c_void_p(seq.data_ptr()), C.c_void_p(out.data_ptr()), T, J, F, int(pad),
-                                         int(causal_shift), len(kps_left), _ilist(kps_left), _ilist(kps_right),
-                                         C.c_void_p(_stream(seq.device))), 'gast_tta_prepare')
+                                         int(causal_shift), n, kl, kr, C.c_void_p(_stream(seq.device))),
+               'gast_tta_prepare')
     return out
 
 
 def tta_merge(pred, joints_left, joints_right):
     """pred (2,T,J,3) -> (T,J,3): mean of the prediction and the un-flipped prediction of the twin."""
-    if not pred.is_cuda or pred.dtype != torch.float32 or pred.shape[0] != 2 or pred.shape[-1] != 3:
-        raise GastError('tta_merge: (2,T,J,3) CUDA float32 tensor expected')
-    pred = pred.contiguous()
+    pred = _cuda_f32(pred, 'tta_merge')
+    if pred.shape[0] != 2 or pred.shape[-1] != 3:
+        raise GastError('tta_merge: (2,T,J,3) tensor expected')
     T, J = int(pred.shape[1]), int(pred.shape[2])
     out = torch.empty((T, J, 3), dtype=torch.float32, device=pred.device)
+    jl, n = _ilist(joints_left)
+    jr, _ = _ilist(joints_right)
     with torch.cuda.device(pred.device):
-        _check(L.load().gast_tta_merge(C.c_void_p(pred.data_ptr()), C.c_void_p(out.data_ptr()), T, J, len(joints_left),
-                                       _ilist(joints_left), _ilist(joints_right), C.c_void_p(_stream(pred.device))),
-               'gast_tta_merge')
+        _check(L.load().gast_tta_merge(C.c_void_p(pred.data_ptr()), C.c_void_p(out.data_ptr()), T, J, n, jl, jr,
+                                       C.c_void_p(_stream(pred.device))), 'gast_tta_merge')
     return out
 
 

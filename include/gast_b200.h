@@ -107,7 +107,11 @@ int gast_forward(gast_t* h, const float* x, float* y, int32_t B, int32_t T,
 int gast_forward_mpjpe(gast_t* h, const float* x, const float* target, float* y, float* loss, int32_t B, int32_t T,
                        int32_t strided_now, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Number of kernels the last gast_forward enqueued (for bench.py's gpu_launches). */
+/* Launch counters.  Every forward-type call (gast_forward, gast_forward_mpjpe, gast_forward_train,
+ * gast_eval_backward and each gast_stream_* push or peek) starts this count, the two below and the timing events at
+ * zero once its checks pass; gast_backward(_input) continues the counts of its training forward, so after a training
+ * step they cover the whole step.
+ * gast_last_launch_count: number of kernels the last such call enqueued (for bench.py's gpu_launches). */
 int32_t gast_last_launch_count(const gast_t* h);
 
 /* Number of those that ran on the tensor-core (wgmma) GEMM core, in either precision (gast_set_precision). */
@@ -155,7 +159,8 @@ int gast_set_precision(gast_t* h, int32_t mode);
 int gast_set_train_precision(gast_t* h, int32_t mode);
 
 /* Number of weight gradients of the last gast_forward_train + gast_backward(_input) pair, or of the last
- * gast_eval_backward, that ran on the TF32 tensor-core weight-gradient kernel. */
+ * gast_eval_backward, that ran on the TF32 tensor-core weight-gradient kernel; 0 after any other forward-type call
+ * (counted like gast_last_launch_count). */
 int32_t gast_last_wgrad_tc_launch_count(const gast_t* h);
 
 /* ---- test-time augmentation around the forward (the caller-side steps of reconstruction.evaluate /
@@ -178,7 +183,9 @@ int gast_tta_merge(const float* pred, float* out, int32_t T, int32_t J, int32_t 
  *   buffers bound with gast_bind_grads (same keys as gast_bind; buffers/running stats have none).
  * gast_backward_input: the same backward, plus dL/dx (B,T,J,F) into dx when dx is not null.  param_grads = 0
  *   computes no parameter gradient: no weight-gradient kernel runs and no gradient buffer need be bound.
- *   gast_backward(h, dy, ws, n, st) is gast_backward_input(h, dy, NULL, 1, ws, n, st).
+ *   gast_backward(h, dy, ws, n, st) is gast_backward_input(h, dy, NULL, 1, ws, n, st).  The backward is refused
+ *   before any launch unless workspace_bytes is at least gast_train_workspace_bytes of its forward's B, T and
+ *   dropout_p: the size that forward checked, which bounds every backward of it.
  * Both models train on their own schedule (strided for Optimized1f, dilated or dense otherwise; main.py:166-175). */
 int gast_bind_grads(gast_t* h, int32_t n, const char* const* keys, void* const* dev_ptrs, const int64_t* numel);
 size_t gast_train_workspace_bytes(gast_t* h, int32_t B, int32_t T, float dropout_p);

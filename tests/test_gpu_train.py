@@ -196,7 +196,7 @@ def test_gemm_core_choice_reaches_training():
             m = m.cuda().train()
             m(x).sum().backward()
             h = list(m.__dict__['_gast_handles'].values())[0]
-            tc[core] = int(h.lib.gast_last_tc_launch_count(h.h))     # counted since the handle was created
+            tc[core] = int(h.lib.gast_last_tc_launch_count(h.h))     # the tensor-core launches of this training step
     finally:
         engine.set_gemm_core(0)
     assert tc[0] > 0 and tc[1] == 0, tc
