@@ -346,19 +346,26 @@ extern "C" int32_t gast_get_timings(gast_t* h, int32_t max_n, float* ms, int32_t
 // ------------------------------------------------------------------------------------------
 // prepare
 // ------------------------------------------------------------------------------------------
+// Finds the parameters (or, with grads, the gradient buffers) bound on a handle by state_dict key.  The first failed
+// lookup sets the error and is kept in `err`; ok stays false from then on.
 struct Lookup {
-  gast_handle* h;
+  const std::unordered_map<std::string, Binding>& m;
+  const char* what;
   bool ok = true;
-  const float* get(const std::string& key, int64_t numel) {
-    auto it = h->bound.find(key);
-    if (it == h->bound.end()) { if (ok) fail("parameter '%s' is not bound", key.c_str()); ok = false; return nullptr; }
-    if (numel >= 0 && it->second.numel != numel) {
-      if (ok) fail("parameter '%s' has %lld elements, expected %lld", key.c_str(), (long long)it->second.numel, (long long)numel);
-      ok = false; return nullptr;
+  std::string err;
+  explicit Lookup(gast_handle* h, bool grads = false)
+      : m(grads ? h->grads : h->bound), what(grads ? "gradient buffer" : "parameter") {}
+  float* get(const std::string& key, int64_t numel) {
+    auto it = m.find(key);
+    if (it != m.end() && (numel < 0 || it->second.numel == numel)) return reinterpret_cast<float*>(it->second.ptr);
+    if (ok) {
+      if (it == m.end()) fail("%s '%s' is not bound", what, key.c_str());
+      else fail("%s '%s' has %lld elements, expected %lld", what, key.c_str(), (long long)it->second.numel, (long long)numel);
+      err = g_err;
     }
-    return reinterpret_cast<const float*>(it->second.ptr);
+    ok = false;
+    return nullptr;
   }
-  bool has(const std::string& key) { return h->bound.count(key) != 0; }
   BnP bn(const std::string& prefix, int C) {
     BnP b;
     b.w = get(prefix + "weight", C); b.b = get(prefix + "bias", C);
@@ -402,38 +409,52 @@ static int prepare_local(gast_handle* h, Lookup& L, cudaStream_t st, BlockConsts
   return 0;
 }
 
-static int prepare_global(gast_handle* h, Lookup& L, cudaStream_t st, BlockConsts& b, const std::string& gp, int kind) {
+struct GlobalParams {   // what prepare_global reads: each head's parameters, then the cat conv and its BatchNorm
+  const float *gw[4], *gb[4], *tw[4], *tb[4], *pw[4], *pb[4], *wc[4], *ck[4];
+  const float* cat_w = nullptr;
+  BnP cat_bn = {nullptr, nullptr, nullptr, nullptr};
+};
+
+static void global_params(const gast_handle* h, Lookup& L, const BlockConsts& b, const std::string& gp, int kind,
+                          GlobalParams* p) {
   const int C = b.C, J = h->cfg.num_joints, Cg = b.Cg;
   for (int hd = 0; hd < b.heads; ++hd) {
     std::string hp = (kind == GAST_KIND_GLOBAL_HEAD) ? gp : gp + "attentions." + std::to_string(hd) + ".";
-    // inter_channels: theta/phi width.  In a block inter == Cg (global_attention.py:21-24).
-    const int Ci = Cg;
-    const float* gw = L.get(hp + "g.weight", (int64_t)Cg * C);
-    const float* gb = L.get(hp + "g.bias", Cg);
-    const float* tw = L.get(hp + "theta.weight", (int64_t)Ci * C);
-    const float* tb = L.get(hp + "theta.bias", Ci);
-    const float* pw = L.get(hp + "phi.weight", (int64_t)Ci * C);
-    const float* pb = L.get(hp + "phi.bias", Ci);
-    const float* wc = L.get(hp + "concat_project.0.weight", 2 * Ci);
-    const float* ck = L.get(hp + "C_k", (int64_t)J * J);
-    if (!L.ok) return 1;
-    CUDA_OK(cudaMemcpyAsync(b.Wg + (size_t)hd * Cg * C, gw, sizeof(float) * Cg * C, cudaMemcpyDeviceToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(b.bg + (size_t)hd * Cg, gb, sizeof(float) * Cg, cudaMemcpyDeviceToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(b.Ck + (size_t)hd * J * J, ck, sizeof(float) * J * J, cudaMemcpyDeviceToDevice, st));
-    global_collapse_kernel<<<cdiv(C, 32), 256, 0, st>>>(b.U, b.cab, tw, tb, pw, pb, wc, hd, C, Ci);
+    // theta / phi are inter_channels wide; in a block inter == Cg (global_attention.py:21-24)
+    p->gw[hd] = L.get(hp + "g.weight", (int64_t)Cg * C);
+    p->gb[hd] = L.get(hp + "g.bias", Cg);
+    p->tw[hd] = L.get(hp + "theta.weight", (int64_t)Cg * C);
+    p->tb[hd] = L.get(hp + "theta.bias", Cg);
+    p->pw[hd] = L.get(hp + "phi.weight", (int64_t)Cg * C);
+    p->pb[hd] = L.get(hp + "phi.bias", Cg);
+    p->wc[hd] = L.get(hp + "concat_project.0.weight", 2 * Cg);
+    p->ck[hd] = L.get(hp + "C_k", (int64_t)J * J);
   }
   if (kind != GAST_KIND_GLOBAL_HEAD) {
-    const float* w = L.get(gp + "cat_conv.weight", (int64_t)C * C);
-    BnP bn = L.bn(gp + "cat_bn.", C);
-    if (!L.ok) return 1;
-    prep_conv(st, b.Wgc, b.bgc, w, C, C, 1, bn);
+    p->cat_w = L.get(gp + "cat_conv.weight", (int64_t)C * C);
+    p->cat_bn = L.bn(gp + "cat_bn.", C);
   }
+}
+
+// the eval constants of a global layer from the parameters global_params found
+static int prepare_global(const gast_handle* h, cudaStream_t st, BlockConsts& b, const GlobalParams& p, int kind) {
+  const int C = b.C, J = h->cfg.num_joints, Cg = b.Cg;
+  for (int hd = 0; hd < b.heads; ++hd) {
+    CUDA_OK(cudaMemcpyAsync(b.Wg + (size_t)hd * Cg * C, p.gw[hd], sizeof(float) * Cg * C, cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(b.bg + (size_t)hd * Cg, p.gb[hd], sizeof(float) * Cg, cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(b.Ck + (size_t)hd * J * J, p.ck[hd], sizeof(float) * J * J, cudaMemcpyDeviceToDevice, st));
+    global_collapse_kernel<<<cdiv(C, 32), 256, 0, st>>>(b.U, b.cab, p.tw[hd], p.tb[hd], p.pw[hd], p.pb[hd], p.wc[hd], hd,
+                                                        C, Cg);
+  }
+  if (kind != GAST_KIND_GLOBAL_HEAD) prep_conv(st, b.Wgc, b.bgc, p.cat_w, C, C, 1, p.cat_bn);
   return 0;
 }
 
 static int prepare_block(gast_handle* h, Lookup& L, cudaStream_t st, BlockConsts& b, const std::string& P) {
   if (prepare_local(h, L, st, b, P + "local_graph_layer.", GAST_KIND_BLOCK)) return 1;
-  if (prepare_global(h, L, st, b, P + "global_graph_layer.", GAST_KIND_BLOCK)) return 1;
+  GlobalParams gpar;
+  global_params(h, L, b, P + "global_graph_layer.", GAST_KIND_BLOCK, &gpar);
+  if (!L.ok || prepare_global(h, st, b, gpar, GAST_KIND_BLOCK)) return 1;
   const int C = b.C;
   const float* w = L.get(P + "cat_conv.weight", (int64_t)2 * C * 3 * C);
   BnP bn = L.bn(P + "cat_bn.", 2 * C);
@@ -501,7 +522,9 @@ extern "C" int gast_prepare(gast_t* h, void* stream) {
   } else if (kind == GAST_KIND_LOCAL || kind == GAST_KIND_SEMCH) {
     if (prepare_local(h, L, st, h->blocks[0], "", kind)) return 1;
   } else if (kind == GAST_KIND_MGLOBAL || kind == GAST_KIND_GLOBAL_HEAD) {
-    if (prepare_global(h, L, st, h->blocks[0], "", kind)) return 1;
+    GlobalParams gpar;
+    global_params(h, L, h->blocks[0], "", kind, &gpar);
+    if (!L.ok || prepare_global(h, st, h->blocks[0], gpar, kind)) return 1;
   } else {
     return fail("gast_prepare: unknown kind %d", kind);
   }
@@ -515,37 +538,9 @@ extern "C" int gast_prepare(gast_t* h, void* stream) {
 // ------------------------------------------------------------------------------------------
 // forward planning
 // ------------------------------------------------------------------------------------------
-struct Geometry {          // frames per clip after each layer
-  int T0 = 0;              // after expand
-  std::vector<int> Ts;     // after stage i (index i-1)
-  int s0 = 1;
-  int T_out = 0;
-};
-
-// schedule actually run: the handle's own (cfg.strided) or, for a dilated model on a
-// receptive-field-long clip, the equivalent strided one (same arithmetic per output, see
-// SURVEY.md §7 "dense vs needed-only work").
-struct Sched {
-  int taps, stride, dil, res_mul, res_off;
-};
-
-static int stage_sched(const gast_handle* h, int i /*1-based*/, int strided_now, Sched* s) {
-  const gast_cfg& c = h->cfg;
-  const int fw = c.filter_widths[i];
-  if (strided_now) {
-    // gast_net.py:222-224,243 ; causal shift of the strided form is fw//2 (:220)
-    s->taps = fw; s->stride = fw; s->dil = 1;
-    s->res_mul = fw;
-    s->res_off = (c.causal ? fw / 2 : 0) + fw / 2;
-  } else {
-    const StageConsts& sc = h->stages[i - 1];
-    s->taps = sc.taps; s->stride = 1; s->dil = sc.dil;
-    s->res_mul = 1;
-    s->res_off = h->pad[i] + h->shift[i];   // gast_net.py:170
-  }
-  return 0;
-}
-
+// The schedule of a forward on clips of T frames.  It is the handle's own (cfg.strided) or, for a dilated model on a
+// receptive-field-long clip, the equivalent strided one (same arithmetic per output, see SURVEY.md §7 "dense vs
+// needed-only work").
 static int geometry(const gast_handle* h, int T, int strided_now, Geometry* g) {
   const gast_cfg& c = h->cfg;
   if (strided_now && !c.strided && c.dense) return fail("dense model has no strided schedule");
@@ -555,16 +550,31 @@ static int geometry(const gast_handle* h, int T, int strided_now, Geometry* g) {
   if (T < k0) return fail("input has %d frames, fewer than the first filter width %d", T, k0);
   g->T0 = (T - k0) / g->s0 + 1;
   int Tp = g->T0;
-  g->Ts.clear();
+  g->stages.clear();
   for (int i = 1; i < c.num_stages; ++i) {
-    Sched s;
-    stage_sched(h, i, strided_now, &s);
+    const int fw = c.filter_widths[i];
+    StageGeo s;
+    int res_mul, res_off;
+    if (strided_now) {
+      // gast_net.py:222-224,243 ; causal shift of the strided form is fw//2 (:220)
+      s.taps = fw; s.stride = fw; s.dil = 1;
+      res_mul = fw;
+      res_off = (c.causal ? fw / 2 : 0) + fw / 2;
+    } else {
+      const StageConsts& sc = h->stages[i - 1];
+      s.taps = sc.taps; s.stride = 1; s.dil = sc.dil;
+      res_mul = 1;
+      res_off = h->pad[i] + h->shift[i];   // gast_net.py:170
+    }
     const int span = (s.taps - 1) * s.dil + 1;
     if (Tp < span) return fail("input of %d frames is shorter than the receptive field", T);
-    int Tn = (Tp - span) / s.stride + 1;
+    const int Tn = (Tp - span) / s.stride + 1;
     // residual slice must cover the conv output (the reference would raise on the add otherwise)
-    if (s.res_off + (long long)(Tn - 1) * s.res_mul >= Tp) return fail("residual slice out of range for T=%d", T);
-    g->Ts.push_back(Tn);
+    if (res_off + (long long)(Tn - 1) * res_mul >= Tp) return fail("residual slice out of range for T=%d", T);
+    s.Tin = Tp; s.Tout = Tn;
+    s.tapmap = RowMap{Tn, Tp, s.stride, 0};
+    s.resmap = RowMap{Tn, Tp, res_mul, res_off};
+    g->stages.push_back(s);
     Tp = Tn;
   }
   g->T_out = Tp;
@@ -852,7 +862,7 @@ static int plan_model(const gast_handle* h, int B, int T, int strided_now, Arena
   for (int i = 0; i < L; ++i) {
     const int Cw = C << i;
     if (i > 0) {
-      rows = (long long)B * g->Ts[i - 1] * J;
+      rows = (long long)B * g->stages[i - 1].Tout * J;
       tmp = std::max(tmp, (size_t)rows * Cw);
     }
     act = std::max(act, (size_t)rows * 2 * Cw);
@@ -930,21 +940,17 @@ static int forward_impl(gast_t* h, const float* x, float* y, int32_t B, int32_t 
   if (launch_expand(h, st, x, mb.act[0], F * J, T, g.T0, g.s0)) return 1;
   if (run_block(h, st, h->blocks[0], mb.act[0], F, mb.bb, mb.act[1])) return 1;
   int cur = 1;
-  int Tp = g.T0;
   for (int i = 1; i < h->cfg.num_stages; ++i) {
     StageConsts& s = h->stages[i - 1];
-    Sched sc;
-    stage_sched(h, i, strided_now, &sc);
-    const int Cw = s.Cw, Tn = g.Ts[i - 1];
-    const long long Fn = (long long)B * Tn;
+    const StageGeo& sg = g.stages[i - 1];
+    const int Cw = s.Cw;
+    const long long Fn = (long long)B * sg.Tout;
     const float* xin = mb.act[cur];
-    const ASeg taps = seg_taps(xin, Cw, Cw, sc.taps, (long long)sc.dil * J * Cw, RowMap{Tn, Tp, sc.stride, 0});
-    if (run_stage(h, st, s, Fn, taps, s.Wt, &s.tc_t, mb.tmp, xin, RowMap{Tn, Tp, sc.res_mul, sc.res_off},
-                  mb.act[cur ^ 1])) return 1;
+    const ASeg taps = seg_taps(xin, Cw, Cw, sg.taps, (long long)sg.dil * J * Cw, sg.tapmap);
+    if (run_stage(h, st, s, Fn, taps, s.Wt, &s.tc_t, mb.tmp, xin, sg.resmap, mb.act[cur ^ 1])) return 1;
     cur ^= 1;
     if (run_block(h, st, h->blocks[i], mb.act[cur], Fn, mb.bb, mb.act[cur ^ 1])) return 1;
     cur ^= 1;
-    Tp = Tn;
     F = Fn;
   }
   // output is already (B, T_out, J, 3)
@@ -1034,22 +1040,21 @@ static int train_check(gast_handle* h, const char* what) {
   return precision_check(h, what);
 }
 
-// workspace of a training forward + backward of the mode `ts` describes, by a dry run of both (no launches); 0 on error
-static size_t train_dry_run_bytes(gast_handle* h, int B, int T, TrainState ts, bool pgrad, const char* what) {
-  if (!h || train_check(h, what)) return 0;
-  Arena a{nullptr, 0, 0, true};
-  Lookup L{h};
-  TCtx c{h, nullptr, &a, &L, h->cfg.num_joints, true};
-  c.pgrad = pgrad;
-  if (train_forward(h, c, ts, nullptr, nullptr, B, T)) return 0;
-  if (train_backward(h, c, ts, nullptr, nullptr)) return 0;
-  return a.off + 512;
+static Arena sizing_arena(size_t off = 0) { return Arena{nullptr, 0, off, true}; }
+
+// The workspace of a training forward + backward of the mode `ts` describes, by their sizing pass in c; 0 on error.
+// c keeps the pass's lookups for the caller to refuse on.
+static size_t train_sizing(TCtx& c, int B, int T, TrainState ts) {
+  if (train_forward(c.h, c, ts, nullptr, nullptr, B, T) || train_backward(c.h, c, ts, nullptr, nullptr)) return 0;
+  return c.a.off + 512;
 }
 
 extern "C" size_t gast_train_workspace_bytes(gast_t* h, int32_t B, int32_t T, float dropout_p) {
+  if (!h || train_check(h, "gast_train_workspace_bytes")) return 0;
   TrainState ts;
   ts.drop_p = dropout_p;
-  return train_dry_run_bytes(h, B, T, ts, true, "gast_train_workspace_bytes");
+  TCtx c(h, nullptr, sizing_arena(), true);
+  return train_sizing(c, B, T, ts);
 }
 
 extern "C" int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B, int32_t T, float dropout_p,
@@ -1059,13 +1064,15 @@ extern "C" int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B
   if (B <= 0 || T <= 0) return fail("gast_forward_train: empty batch (B=%d T=%d)", B, T);
   if (!x || !y) return fail("gast_forward_train: x and y must be device pointers");
   if (dropout_p < 0.f || dropout_p >= 1.f) return fail("gast_forward_train: dropout_p out of range");
-  const size_t need = gast_train_workspace_bytes(h, B, T, dropout_p);
-  if (need == 0) return 1;
+  TrainState sized;
+  sized.drop_p = dropout_p;
+  TCtx dry(h, nullptr, sizing_arena(), true);
+  const size_t need = train_sizing(dry, B, T, sized);
+  // gradient buffers are only read by the backward, which checks them itself
+  if (need == 0 || dry.refuse(false)) return 1;
   if (call_begin(h, "gast_forward_train", need, workspace, workspace_bytes)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  Arena a = workspace_arena(workspace, workspace_bytes);
-  Lookup L{h};
-  TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
+  TCtx c(h, st, workspace_arena(workspace, workspace_bytes), true);
   for (size_t i = 0; i < h->trains.size(); ++i)      // a workspace reused by the caller: its old state is dead
     if (h->trains[i].first == workspace) { h->trains.erase(h->trains.begin() + i); break; }
   if (h->trains.size() >= GAST_MAX_PENDING_TRAIN) h->trains.erase(h->trains.begin());   // forwards never differentiated
@@ -1075,7 +1082,7 @@ extern "C" int gast_forward_train(gast_t* h, const float* x, float* y, int32_t B
   ts.seed = seed;
   ts.workspace_bytes = need;
   if (train_forward(h, c, ts, x, y, B, T)) { h->trains.pop_back(); return 1; }
-  ts.arena_off = a.off;
+  ts.arena_off = c.a.off;
   ts.valid = true;
   if (h->dropout_state && dropout_p > 0.f) dropout_bump_kernel<<<1, 1, 0, st>>>(h->dropout_state);
   h->prepared = false;      // running statistics changed: eval constants are stale
@@ -1106,14 +1113,13 @@ extern "C" int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_
     return fail("gast_backward: no training forward is saved in this workspace (already differentiated, "
                 "or more than %d forwards were outstanding)", GAST_MAX_PENDING_TRAIN);
   if (call_begin(h, "gast_backward", h->trains[ti].second.workspace_bytes, workspace, workspace_bytes, false)) return 1;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   TrainState ts = h->trains[ti].second;
+  TCtx dry(h, nullptr, sizing_arena(ts.arena_off), param_grads != 0);
+  if (train_backward(h, dry, ts, nullptr, nullptr) || dry.refuse(true)) return 1;   // the saved forward stays
   h->trains.erase(h->trains.begin() + ti);
-  Arena a = workspace_arena(workspace, workspace_bytes, ts.arena_off);
-  Lookup L{h};
-  TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
+  TCtx c(h, reinterpret_cast<cudaStream_t>(stream), workspace_arena(workspace, workspace_bytes, ts.arena_off),
+         param_grads != 0);
   c.tc_slot = 1024;                         // the backward's GEMMs follow the forward's in the operand-copy table
-  c.pgrad = param_grads != 0;
   if (train_backward(h, c, ts, dy, dx)) return 1;
   CUDA_OK(cudaGetLastError());
   return 0;
@@ -1128,7 +1134,9 @@ static TrainState eval_state(int strided_now) {
 }
 
 extern "C" size_t gast_eval_backward_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now) {
-  return train_dry_run_bytes(h, B, T, eval_state(strided_now), true, "gast_eval_backward_workspace_bytes");
+  if (!h || train_check(h, "gast_eval_backward_workspace_bytes")) return 0;
+  TCtx c(h, nullptr, sizing_arena(), true);
+  return train_sizing(c, B, T, eval_state(strided_now));
 }
 
 extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads, int32_t B,
@@ -1139,14 +1147,11 @@ extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, fl
   if (!x || !dy) return fail("gast_eval_backward: x and dy must be device pointers");
   if (!dx && !param_grads) return fail("gast_eval_backward: neither dx nor parameter gradients requested");
   TrainState ts = eval_state(strided_now);
-  const size_t need = train_dry_run_bytes(h, B, T, ts, param_grads != 0, "gast_eval_backward");
-  if (need == 0) return 1;
+  TCtx dry(h, nullptr, sizing_arena(), param_grads != 0);
+  const size_t need = train_sizing(dry, B, T, ts);
+  if (need == 0 || dry.refuse(true)) return 1;
   if (call_begin(h, "gast_eval_backward", need, workspace, workspace_bytes)) return 1;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  Arena a = workspace_arena(workspace, workspace_bytes);
-  Lookup L{h};
-  TCtx c{h, st, &a, &L, h->cfg.num_joints, false};
-  c.pgrad = param_grads != 0;
+  TCtx c(h, reinterpret_cast<cudaStream_t>(stream), workspace_arena(workspace, workspace_bytes), param_grads != 0);
   if (train_forward(h, c, ts, x, nullptr, B, T)) return 1;
   c.tc_slot = 1024;
   if (train_backward(h, c, ts, dy, dx)) return 1;

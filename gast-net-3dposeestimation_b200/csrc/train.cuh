@@ -11,36 +11,47 @@
 // The same forward in frozen mode (TrainState::frozen: BatchNorm on the running statistics, no dropout, the inference
 // schedule) recomputes the activations for the eval-mode backward; the backward also writes dL/dx, and skips every
 // parameter-gradient kernel when only dL/dx is wanted (TCtx::pgrad).
+//
+// Every function here runs in two passes of one TCtx.  The sizing pass (an arena without memory) walks the same code
+// as the launch pass and enqueues nothing: its arena takes give the workspace size, and it makes every parameter and
+// gradient-buffer lookup the launch pass makes.  A failed lookup is recorded there, and each call refuses on that
+// record (TCtx::refuse) before its first launch.
 #pragma once
 
 // ---------------------------------------------------------------------------------------------
 struct TCtx {
-  gast_handle* h; cudaStream_t st; Arena* a; Lookup* L; int J;
-  bool dry;   // sizing pass: no launches
-  int tc_slot = 0;   // next slot of the handle's table of per-GEMM tensor-core operand copies (train_tcw)
+  gast_handle* h; cudaStream_t st; Arena a; int J;
+  bool dry;      // sizing pass: arena takes and lookups only, nothing is enqueued
   // backward: false = input gradient only (every parameter frozen): no weight-gradient contraction, no parameter-
   // gradient kernel, and no gradient buffer has to be bound
-  bool pgrad = true;
-  float* fl(size_t n) { return a->take(n); }
-  double* dbl(size_t n) { return reinterpret_cast<double*>(a->take(2 * n)); }
-  unsigned char* bytes(size_t n) { return reinterpret_cast<unsigned char*>(a->take((n + 3) / 4)); }
+  bool pgrad;
+  int tc_slot = 0;   // next slot of the handle's table of per-GEMM tensor-core operand copies (train_tcw)
+  Lookup params, grad_bufs;
+  TCtx(gast_handle* h_, cudaStream_t st_, Arena a_, bool pgrad_)
+      : h(h_), st(st_), a(a_), J(h_->cfg.num_joints), dry(a_.dry), pgrad(pgrad_), params(h_), grad_bufs(h_, true) {}
+  float* fl(size_t n) { return a.take(n); }
+  double* dbl(size_t n) { return reinterpret_cast<double*>(a.take(2 * n)); }
+  unsigned char* bytes(size_t n) { return reinterpret_cast<unsigned char*>(a.take((n + 3) / 4)); }
+  float* param(const std::string& key, int64_t numel) { return params.get(key, numel); }
+  // the gradient buffer bound for `key`, null when no parameter gradient is computed
+  float* grad(const std::string& key, int64_t numel) { return pgrad ? grad_bufs.get(key, numel) : nullptr; }
+  // nonzero with the error set when a lookup of this context failed: a parameter, or with grads a gradient buffer
+  int refuse(bool grads) const {
+    if (!params.ok) return fail("%s", params.err.c_str());
+    if (grads && !grad_bufs.ok) return fail("%s", grad_bufs.err.c_str());
+    return 0;
+  }
+  template <class... KP, class... A>
+  void launch(void (*kernel)(KP...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+    if (!dry) kernel<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+  }
+  void zero(void* p, size_t n) { if (!dry) cudaMemsetAsync(p, 0, n, st); }
+  void copy(void* dst, const void* src, size_t n) {
+    if (!dry) cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToDevice, st);
+  }
+  // f() in the launch pass only: the counted launches of the inference code
+  template <class F> int live(F f) { return dry ? 0 : f(); }
 };
-
-static float* grad_ptr(gast_handle* h, const std::string& key, int64_t numel) {
-  auto it = h->grads.find(key);
-  if (it == h->grads.end()) { fail("gradient buffer for '%s' is not bound", key.c_str()); return nullptr; }
-  if (it->second.numel != numel) { fail("gradient buffer '%s' has the wrong size", key.c_str()); return nullptr; }
-  return reinterpret_cast<float*>(it->second.ptr);
-}
-
-// *out = the bound gradient buffer of `key`, or null when no parameter gradient is computed (sizing pass, input-only
-// backward).  false: a wanted buffer is missing or has the wrong size.
-static bool want_grad(TCtx& c, const std::string& key, int64_t numel, float** out) {
-  *out = nullptr;
-  if (c.dry || !c.pgrad) return true;
-  *out = grad_ptr(c.h, key, numel);
-  return *out != nullptr;
-}
 
 // Tensor-core operand copies of one training GEMM's weight matrix (forward: the raw weights, backward: their transposes):
 // the weights change every step, so the hi/lo split runs per call; buffers live in a per-handle table indexed by the
@@ -60,24 +71,24 @@ static const TcWeights* train_tcw(TCtx& c, const float* W, int N, int K) {
 // dense out[M][N] = A[M][K] . W[N][K]^T (+bias), rows are plain (no frame structure)
 static int dense_nt(TCtx& c, const float* A, int lda, const float* W, long long M, int N, int K, float* out, int ldo,
                     const float* bias = nullptr) {
-  if (c.dry || M <= 0) return 0;
+  if (M <= 0) return 0;
   GemmP p;
   gemm_flat(p, M);
   p.nseg = 1; p.seg[0] = seg_flat(A, lda, K);
   p.W = W; p.ldw = K; p.N = N; p.out = out; p.ld_out = ldo; p.bias = bias;
-  return launch_gemm(c.h, c.st, EPI_PLAIN, p, train_tcw(c, W, N, K));
+  return c.live([&] { return launch_gemm(c.h, c.st, EPI_PLAIN, p, train_tcw(c, W, N, K)); });
 }
 
 // frame-structured forward GEMM with gathered segments (same kernel as inference), raw weights
 static int seg_gemm(TCtx& c, const ASeg* segs, int nseg, const float* W, int ldw, long long F, int N, float* out,
                     int ldo, const float* bias = nullptr) {
-  if (c.dry || F <= 0) return 0;
+  if (F <= 0) return 0;
   GemmP p;
   gemm_defaults(p, c.h, F);
   p.nseg = nseg;
   for (int i = 0; i < nseg; ++i) p.seg[i] = segs[i];
   p.W = W; p.ldw = ldw; p.N = N; p.out = out; p.ld_out = ldo; p.bias = bias;
-  return launch_gemm(c.h, c.st, EPI_PLAIN, p, train_tcw(c, W, N, ldw));
+  return c.live([&] { return launch_gemm(c.h, c.st, EPI_PLAIN, p, train_tcw(c, W, N, ldw)); });
 }
 
 static long long pad32(long long m) { return (m + 31) / 32 * 32; }
@@ -117,14 +128,16 @@ static int dense_tn(TCtx& c, const float* dZ, int lddz, const float* A, int lda,
   long long S, rps;
   wgrad_split(M, N, K, c.h->sm_count, &S, &rps);
   float* part = c.fl((size_t)S * N * K);
-  if (c.dry || M <= 0) return 0;
-  bool on_tc = false;
-  const int rc = wgrad_run(c.st, dZ, lddz, A, lda, M, N, K, S, rps, part, dW, lddw,
-                           c.h->gemm_core == 0 && c.h->train_precision == 1, &on_tc);
-  if (rc) return fail("weight-gradient launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-  c.h->launches += 2;
-  if (on_tc) c.h->wgrad_tc_launches++;
-  return 0;
+  if (M <= 0) return 0;
+  return c.live([&] {
+    bool on_tc = false;
+    const int rc = wgrad_run(c.st, dZ, lddz, A, lda, M, N, K, S, rps, part, dW, lddw,
+                             c.h->gemm_core == 0 && c.h->train_precision == 1, &on_tc);
+    if (rc) return fail("weight-gradient launch failed: %s", cudaGetErrorString((cudaError_t)rc));
+    c.h->launches += 2;
+    if (on_tc) c.h->wgrad_tc_launches++;
+    return 0;
+  });
 }
 
 // dA[M][K] = dZ[M][N] . W[N][K]   (W transposed on the fly)
@@ -132,18 +145,21 @@ static int dense_nn(TCtx& c, const float* dZ, int lddz, const float* W, int ldw,
                     int ldda) {
   const int Np = (int)pad32(N);
   float* Wt = c.fl((size_t)K * Np);
-  float* dZp = nullptr;
-  if (Np != N) dZp = c.fl((size_t)M * Np);
-  if (c.dry) return 0;
-  cudaMemsetAsync(Wt, 0, sizeof(float) * (size_t)K * Np, c.st);
-  transpose_kernel<<<dim3(cdiv(N, 32), cdiv(K, 32)), dim3(32, 8), 0, c.st>>>(W, N, K, ldw, Wt, Np);
-  const float* dz = dZ; int ld = lddz;
-  if (dZp) {
-    cudaMemsetAsync(dZp, 0, sizeof(float) * (size_t)M * Np, c.st);
-    copy2d_kernel<<<cdiv(M * N, 256), 256, 0, c.st>>>(dZ, lddz, dZp, Np, M, N, 0);
-    dz = dZp; ld = Np;
-  }
-  return dense_nt(c, dz, ld, Wt, M, K, Np, dA, ldda);
+  c.zero(Wt, sizeof(float) * (size_t)K * Np);
+  c.launch(transpose_kernel, dim3(cdiv(N, 32), cdiv(K, 32)), dim3(32, 8), 0, W, N, K, ldw, Wt, Np);
+  if (Np == N) return dense_nt(c, dZ, lddz, Wt, M, K, Np, dA, ldda);
+  float* dZp = c.fl((size_t)M * Np);
+  c.zero(dZp, sizeof(float) * (size_t)M * Np);
+  c.launch(copy2d_kernel, cdiv(M * N, 256), 256, 0, dZ, lddz, dZp, Np, M, N, 0);
+  return dense_nt(c, dZp, Np, Wt, M, K, Np, dA, ldda);
+}
+
+// backward of the 1x1 conv Z[M][N] = A[M][K] . W^T whose weight W[N][K] is bound as `key`: its weight gradient into
+// the gradient buffer of `key` (c.pgrad), then dA = dZ . W
+static int conv1x1_bwd(TCtx& c, const std::string& key, const float* dZ, const float* A, long long M, int N, int K,
+                       float* dA) {
+  if (dense_tn(c, dZ, N, A, K, M, N, K, c.grad(key, (int64_t)N * K), K)) return 1;
+  return dense_nn(c, dZ, N, c.param(key, (int64_t)N * K), K, M, N, K, dA, K);
 }
 
 // ---- BatchNorm, training mode (batch statistics) or frozen (running statistics: ts.frozen) ----------------
@@ -157,24 +173,23 @@ static int bn_fwd(TCtx& c, BnSave& s, const std::string& prefix, const float* Z,
   s.kscale = 1.f;
   if (drop_p > 0.f) { keep = c.bytes((size_t)M * N); s.kscale = 1.f / (1.f - drop_p); }
   s.keep = keep;
-  if (c.dry) return 0;
-  s.gamma = c.L->get(prefix + "weight", N); s.beta = c.L->get(prefix + "bias", N);
-  float* rm = const_cast<float*>(c.L->get(prefix + "running_mean", N));
-  float* rv = const_cast<float*>(c.L->get(prefix + "running_var", N));
-  if (!c.L->ok) return 1;
+  s.gamma = c.param(prefix + "weight", N); s.beta = c.param(prefix + "bias", N);
+  float* rm = c.param(prefix + "running_mean", N);
+  float* rv = c.param(prefix + "running_var", N);
   if (ts.frozen) {
-    bn_running_kernel<<<cdiv(N, 128), 128, 0, c.st>>>(rm, rv, N, s.mean, s.invstd);
+    c.launch(bn_running_kernel, cdiv(N, 128), 128, 0, rm, rv, N, s.mean, s.invstd);
   } else {
-    cudaMemsetAsync(sums, 0, sizeof(double) * 2 * N, c.st);
+    c.zero(sums, sizeof(double) * 2 * N);
     dim3 grid(cdiv(N, 32), (unsigned)std::min<long long>(256, (M + 7) / 8));
-    col_stats_kernel<<<grid, 256, 0, c.st>>>(Z, M, N, ldz, sums, sums + N);
-    bn_finalize_kernel<<<cdiv(N, 128), 128, 0, c.st>>>(sums, sums + N, M, N, s.mean, s.invstd, rm, rv, 0.1f);
+    c.launch(col_stats_kernel, grid, 256, 0, Z, M, N, ldz, sums, sums + N);
+    c.launch(bn_finalize_kernel, cdiv(N, 128), 128, 0, sums, sums + N, M, N, s.mean, s.invstd, rm, rv, 0.1f);
   }
   if (keep) {
-    dropout_mask_kernel<<<cdiv(M * N, 256), 256, 0, c.st>>>(keep, M * N, drop_p, ts.seed + 0x51ED270B * (++ts.drop_ctr), c.h->dropout_state);
+    const unsigned long long seed = ts.seed + 0x51ED270B * (++ts.drop_ctr);
+    c.launch(dropout_mask_kernel, cdiv(M * N, 256), 256, 0, keep, M * N, drop_p, seed, c.h->dropout_state);
   }
-  bn_apply_kernel<<<cdiv(M * N, 256), 256, 0, c.st>>>(Z, ldz, s.mean, s.invstd, s.gamma, s.beta, relu, res, ldres, rmap,
-                                                    c.J, keep, s.kscale, Y, ldy, M, N);
+  c.launch(bn_apply_kernel, cdiv(M * N, 256), 256, 0, Z, ldz, s.mean, s.invstd, s.gamma, s.beta, relu, res, ldres, rmap,
+           c.J, keep, s.kscale, Y, ldy, M, N);
   return 0;
 }
 
@@ -182,25 +197,18 @@ static int bn_fwd(TCtx& c, BnSave& s, const std::string& prefix, const float* Z,
 // dbeta = sum dY' are those gradients; batch statistics also need them for dZ, running statistics do not.
 static int bn_bwd(TCtx& c, const BnSave& s, const float* dY, int lddy, float* dZ, int lddz) {
   double* sums = (!s.frozen || c.pgrad) ? c.dbl(2 * (size_t)s.N) : nullptr;
-  float *gw, *gb;
-  if (!want_grad(c, s.prefix + "weight", s.N, &gw) || !want_grad(c, s.prefix + "bias", s.N, &gb)) return 1;
-  if (c.dry) return 0;
+  float* gw = c.grad(s.prefix + "weight", s.N);
+  float* gb = c.grad(s.prefix + "bias", s.N);
   if (sums) {
-    cudaMemsetAsync(sums, 0, sizeof(double) * 2 * s.N, c.st);
+    c.zero(sums, sizeof(double) * 2 * s.N);
     dim3 grid(cdiv(s.N, 32), (unsigned)std::min<long long>(256, (s.M + 7) / 8));
-    bn_bwd_reduce_kernel<<<grid, 256, 0, c.st>>>(dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma, s.beta, s.relu, s.keep,
-                                                s.kscale, s.M, s.N, sums, sums + s.N);
+    c.launch(bn_bwd_reduce_kernel, grid, 256, 0, dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma, s.beta, s.relu, s.keep,
+             s.kscale, s.M, s.N, sums, sums + s.N);
   }
   const double* dg = sums;
   const double* db = sums ? sums + s.N : nullptr;
-  if (s.frozen)
-    bn_bwd_apply_kernel<true><<<cdiv(s.M * s.N, 256), 256, 0, c.st>>>(dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma,
-                                                                      s.beta, s.relu, s.keep, s.kscale, s.M, s.N, dg, db,
-                                                                      dZ, lddz, gw, gb);
-  else
-    bn_bwd_apply_kernel<false><<<cdiv(s.M * s.N, 256), 256, 0, c.st>>>(dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma,
-                                                                       s.beta, s.relu, s.keep, s.kscale, s.M, s.N, dg, db,
-                                                                       dZ, lddz, gw, gb);
+  c.launch(s.frozen ? bn_bwd_apply_kernel<true> : bn_bwd_apply_kernel<false>, cdiv(s.M * s.N, 256), 256, 0, dY, lddy,
+           s.Z, s.ldz, s.mean, s.invstd, s.gamma, s.beta, s.relu, s.keep, s.kscale, s.M, s.N, dg, db, dZ, lddz, gw, gb);
   return 0;
 }
 
@@ -230,59 +238,42 @@ static int block_fwd(TCtx& c, TrainState& ts, BlockSave& b, BlockConsts& bc, con
   b.Zgc = c.fl((size_t)M * C); b.Gl = c.fl((size_t)M * C);
   b.Zbc = c.fl((size_t)M * 2 * C); b.Out = c.fl((size_t)M * 2 * C);
   // ---- local
-  if (!c.dry) {
-    for (int m = 0; m < 2; ++m) {
-      const std::string g = lp + (m == 0 ? "gcn_sym." : "gcn_con.");
-      const float* W = c.L->get(g + "W", (int64_t)2 * C * C);
-      const float* e = c.L->get(g + "e", (int64_t)C * h->nnz[m]);
-      if (!c.L->ok) return 1;
-      semch_wstack_kernel<<<cdiv((long long)2 * C * C, 256), 256, 0, c.st>>>(W, C, C, b.Wst + (size_t)m * 2 * C * C);
-      BnP none{nullptr, nullptr, nullptr, nullptr};
-      semch_coef_kernel<<<cdiv((long long)C * J, 128), 128, 0, c.st>>>(b.coefA[m], nullptr, e, h->nnz[m], h->nbr[m],
-                                                                      h->nnz[m], C, J, none, nullptr);
-    }
+  for (int m = 0; m < 2; ++m) {
+    const std::string g = lp + (m == 0 ? "gcn_sym." : "gcn_con.");
+    const float* W = c.param(g + "W", (int64_t)2 * C * C);
+    const float* e = c.param(g + "e", (int64_t)C * h->nnz[m]);
+    c.launch(semch_wstack_kernel, cdiv((long long)2 * C * C, 256), 256, 0, W, C, C, b.Wst + (size_t)m * 2 * C * C);
+    BnP none{nullptr, nullptr, nullptr, nullptr};
+    c.launch(semch_coef_kernel, cdiv((long long)C * J, 128), 128, 0, b.coefA[m], nullptr, e, h->nnz[m], h->nbr[m],
+             h->nnz[m], C, J, none, nullptr);
   }
   if (dense_nt(c, X, C, b.Wst, M, 4 * C, C, b.H, 4 * C)) return 1;
-  if (!c.dry)
-    for (int m = 0; m < 2; ++m)
-      semch_mix_fwd_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(b.H + m * 2 * C, 4 * C, b.coefA[m], h->nbr[m], J, F, C,
-                                                              b.S + m * C, 2 * C);
+  for (int m = 0; m < 2; ++m)
+    c.launch(semch_mix_fwd_kernel, cdiv(M * C, 256), 256, 0, b.H + m * 2 * C, 4 * C, b.coefA[m], h->nbr[m], J, F, C,
+             b.S + m * C, 2 * C);
   if (bn_fwd(c, b.bn1, lp + "bn_1.", b.S, 2 * C, M, C, 1, 0.f, ts, nullptr, 0, id, b.XY, 2 * C)) return 1;
   if (bn_fwd(c, b.bn2, lp + "bn_2.", b.S + C, 2 * C, M, C, 1, 0.f, ts, nullptr, 0, id, b.XY + C, 2 * C)) return 1;
-  {
-    const float* w = c.dry ? nullptr : c.L->get(lp + "cat_conv.weight", (int64_t)C * 2 * C);
-    if (!c.dry && !c.L->ok) return 1;
-    if (dense_nt(c, b.XY, 2 * C, w, M, C, 2 * C, b.Zlc, C)) return 1;
-  }
+  if (dense_nt(c, b.XY, 2 * C, c.param(lp + "cat_conv.weight", (int64_t)C * 2 * C), M, C, 2 * C, b.Zlc, C)) return 1;
   if (bn_fwd(c, b.bnlc, lp + "cat_bn.", b.Zlc, C, M, C, 1, ts.drop_p, ts, nullptr, 0, id, b.L, C)) return 1;
   // ---- global (stacked g / collapsed theta,phi constants are refreshed here, they follow the weights)
-  if (!c.dry) {
-    if (prepare_global(h, *c.L, c.st, bc, gp, GAST_KIND_MGLOBAL)) return 1;
-  }
+  GlobalParams gpar;
+  global_params(h, c.params, bc, gp, GAST_KIND_MGLOBAL, &gpar);
+  if (c.live([&] { return prepare_global(h, c.st, bc, gpar, GAST_KIND_MGLOBAL); })) return 1;
   if (dense_nt(c, X, C, bc.Wg, M, C, C, b.G, C, bc.bg)) return 1;
-  if (!c.dry) {
-    if (launch_rowdot(h, c.st, X, C, bc, b.AB, M)) return 1;
-    att_mix_fwd_kernel<<<(unsigned)F, 256, sizeof(float) * 4 * J * J, c.st>>>(b.G, C, b.AB, bc.Ck, J, 4, C / 4, b.Y, C);
-  }
-  {
-    const float* w = c.dry ? nullptr : c.L->get(gp + "cat_conv.weight", (int64_t)C * C);
-    if (!c.dry && !c.L->ok) return 1;
-    if (dense_nt(c, b.Y, C, w, M, C, C, b.Zgc, C)) return 1;
-  }
+  if (c.live([&] { return launch_rowdot(h, c.st, X, C, bc, b.AB, M); })) return 1;
+  c.launch(att_mix_fwd_kernel, (unsigned)F, 256, sizeof(float) * 4 * J * J, b.G, C, b.AB, bc.Ck, J, 4, C / 4, b.Y, C);
+  if (dense_nt(c, b.Y, C, c.param(gp + "cat_conv.weight", (int64_t)C * C), M, C, C, b.Zgc, C)) return 1;
   if (bn_fwd(c, b.bngc, gp + "cat_bn.", b.Zgc, C, M, C, 1, ts.drop_p, ts, nullptr, 0, id, b.Gl, C)) return 1;
   // ---- cat[x, local, global] -> 1x1 -> BN -> ReLU
-  {
-    const float* w = c.dry ? nullptr : c.L->get(P + "cat_conv.weight", (int64_t)2 * C * 3 * C);
-    if (!c.dry && !c.L->ok) return 1;
-    ASeg segs[3] = {seg_flat(X, C, C), seg_flat(b.L, C, C), seg_flat(b.Gl, C, C)};
-    if (seg_gemm(c, segs, 3, w, 3 * C, F, 2 * C, b.Zbc, 2 * C)) return 1;
-  }
+  const ASeg segs[3] = {seg_flat(X, C, C), seg_flat(b.L, C, C), seg_flat(b.Gl, C, C)};
+  if (seg_gemm(c, segs, 3, c.param(P + "cat_conv.weight", (int64_t)2 * C * 3 * C), 3 * C, F, 2 * C, b.Zbc, 2 * C))
+    return 1;
   if (bn_fwd(c, b.bnbc, P + "cat_bn.", b.Zbc, 2 * C, M, 2 * C, 1, 0.f, ts, nullptr, 0, id, b.Out, 2 * C)) return 1;
   return 0;
 }
 
 // ---- GraphAttentionBlock, backward: dOut (M x 2C) -> dX (M x C, overwritten) ----------------------------
-static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, float* dX) {
+static int block_bwd(TCtx& c, const BlockSave& b, BlockConsts& bc, const float* dOut, float* dX) {
   gast_handle* h = c.h;
   const int C = b.C, J = c.J;
   const long long F = b.F, M = F * J;
@@ -293,30 +284,18 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
   if (bn_bwd(c, b.bnbc, dOut, 2 * C, dZbc, 2 * C)) return 1;
   float* Acat = c.fl((size_t)M * 3 * C);
   float* dAcat = c.fl((size_t)M * 3 * C);
-  if (!c.dry && c.pgrad) {
-    copy2d_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(b.X, C, Acat, 3 * C, M, C, 0);
-    copy2d_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(b.L, C, Acat + C, 3 * C, M, C, 0);
-    copy2d_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(b.Gl, C, Acat + 2 * C, 3 * C, M, C, 0);
+  if (c.pgrad) {
+    c.launch(copy2d_kernel, cdiv(M * C, 256), 256, 0, b.X, C, Acat, 3 * C, M, C, 0);
+    c.launch(copy2d_kernel, cdiv(M * C, 256), 256, 0, b.L, C, Acat + C, 3 * C, M, C, 0);
+    c.launch(copy2d_kernel, cdiv(M * C, 256), 256, 0, b.Gl, C, Acat + 2 * C, 3 * C, M, C, 0);
   }
-  {
-    const float* w = c.dry ? nullptr : c.L->get(P + "cat_conv.weight", (int64_t)2 * C * 3 * C);
-    float* gw;
-    if (!want_grad(c, P + "cat_conv.weight", (int64_t)2 * C * 3 * C, &gw) || (!c.dry && !c.L->ok)) return 1;
-    if (dense_tn(c, dZbc, 2 * C, Acat, 3 * C, M, 2 * C, 3 * C, gw, 3 * C)) return 1;
-    if (dense_nn(c, dZbc, 2 * C, w, 3 * C, M, 2 * C, 3 * C, dAcat, 3 * C)) return 1;
-  }
-  if (!c.dry) copy2d_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(dAcat, 3 * C, dX, C, M, C, 0);
+  if (conv1x1_bwd(c, P + "cat_conv.weight", dZbc, Acat, M, 2 * C, 3 * C, dAcat)) return 1;
+  c.launch(copy2d_kernel, cdiv(M * C, 256), 256, 0, dAcat, 3 * C, dX, C, M, C, 0);
   // (b) global branch
   float* dZgc = c.fl((size_t)M * C);
   if (bn_bwd(c, b.bngc, dAcat + 2 * C, 3 * C, dZgc, C)) return 1;
   float* dY = c.fl((size_t)M * C);
-  {
-    const float* w = c.dry ? nullptr : c.L->get(gp + "cat_conv.weight", (int64_t)C * C);
-    float* gw;
-    if (!want_grad(c, gp + "cat_conv.weight", (int64_t)C * C, &gw) || (!c.dry && !c.L->ok)) return 1;
-    if (dense_tn(c, dZgc, C, b.Y, C, M, C, C, gw, C)) return 1;
-    if (dense_nn(c, dZgc, C, w, C, M, C, C, dY, C)) return 1;
-  }
+  if (conv1x1_bwd(c, gp + "cat_conv.weight", dZgc, b.Y, M, C, C, dY)) return 1;
   float* dG = c.fl((size_t)M * C);
   float* dab = c.fl((size_t)M * 8);
   float* dCk = c.fl((size_t)4 * J * J);
@@ -327,63 +306,48 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
   float* dbg = c.fl(C);
   float* dcab = c.fl(8);
   float* dXg = c.fl((size_t)M * C);
-  if (!c.dry) {
-    att_mix_bwd_kernel<<<(unsigned)F, 256, sizeof(float) * 16 * J * J, c.st>>>(dY, C, b.G, C, b.AB, bc.Ck, J, 4, C / 4, dG,
-                                                                               C, dab, dCkp);
-    if (c.pgrad) {
-      col_sum_det_kernel<<<cdiv(4 * J * J, 32), 256, 0, c.st>>>(dCkp, F, 4 * J * J, dCk);
-      cudaMemsetAsync(dsum, 0, sizeof(double) * (C + 8), c.st);
-      dim3 g1(cdiv(C, 32), (unsigned)std::min<long long>(256, (M + 7) / 8));
-      col_sum_kernel<<<g1, 256, 0, c.st>>>(dG, M, C, C, dsum);
-      dim3 g2(1, (unsigned)std::min<long long>(256, (M + 7) / 8));
-      col_sum_kernel<<<g2, 256, 0, c.st>>>(dab, M, 8, 8, dsum + C);
-      d2f_kernel<<<cdiv(C, 128), 128, 0, c.st>>>(dsum, dbg, C);
-      d2f_kernel<<<1, 32, 0, c.st>>>(dsum + C, dcab, 8);
-    }
+  c.launch(att_mix_bwd_kernel, (unsigned)F, 256, sizeof(float) * 16 * J * J, dY, C, b.G, C, b.AB, bc.Ck, J, 4, C / 4,
+           dG, C, dab, dCkp);
+  if (c.pgrad) {
+    c.launch(col_sum_det_kernel, cdiv(4 * J * J, 32), 256, 0, dCkp, F, 4 * J * J, dCk);
+    c.zero(dsum, sizeof(double) * (C + 8));
+    dim3 g1(cdiv(C, 32), (unsigned)std::min<long long>(256, (M + 7) / 8));
+    c.launch(col_sum_kernel, g1, 256, 0, dG, M, C, C, dsum);
+    dim3 g2(1, (unsigned)std::min<long long>(256, (M + 7) / 8));
+    c.launch(col_sum_kernel, g2, 256, 0, dab, M, 8, 8, dsum + C);
+    c.launch(d2f_kernel, cdiv(C, 128), 128, 0, dsum, dbg, C);
+    c.launch(d2f_kernel, 1, 32, 0, dsum + C, dcab, 8);
   }
   if (dense_tn(c, dG, C, b.X, C, M, C, C, dWg, C)) return 1;
   if (dense_nn(c, dG, C, bc.Wg, C, M, C, C, dXg, C)) return 1;
   // dU[8][C] = dab[M][8]^T . X[M][C]: the same row-contraction as a weight gradient (a one-thread-per-output
   // kernel took 3.4 ms per block at b = 128)
   if (dense_tn(c, dab, 8, b.X, C, M, 8, C, dU, C)) return 1;
-  if (!c.dry) {
-    rowdot_bwd_x_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(dab, bc.U, 8, M, C, dXg, C);
-    add_inplace_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(dX, dXg, M * C);
-    const int Cg = C / 4;
-    for (int hd = 0; hd < (c.pgrad ? 4 : 0); ++hd) {
-      const std::string hp = gp + "attentions." + std::to_string(hd) + ".";
-      float* ggw = grad_ptr(h, hp + "g.weight", (int64_t)Cg * C);
-      float* ggb = grad_ptr(h, hp + "g.bias", Cg);
-      float* gck = grad_ptr(h, hp + "C_k", (int64_t)J * J);
-      float* gtw = grad_ptr(h, hp + "theta.weight", (int64_t)Cg * C);
-      float* gtb = grad_ptr(h, hp + "theta.bias", Cg);
-      float* gpw = grad_ptr(h, hp + "phi.weight", (int64_t)Cg * C);
-      float* gpb = grad_ptr(h, hp + "phi.bias", Cg);
-      float* gwc = grad_ptr(h, hp + "concat_project.0.weight", 2 * Cg);
-      if (!ggw || !ggb || !gck || !gtw || !gtb || !gpw || !gpb || !gwc) return 1;
-      cudaMemcpyAsync(ggw, dWg + (size_t)hd * Cg * C, sizeof(float) * Cg * C, cudaMemcpyDeviceToDevice, c.st);
-      cudaMemcpyAsync(ggb, dbg + hd * Cg, sizeof(float) * Cg, cudaMemcpyDeviceToDevice, c.st);
-      cudaMemcpyAsync(gck, dCk + hd * J * J, sizeof(float) * J * J, cudaMemcpyDeviceToDevice, c.st);
-      const float* tw = c.L->get(hp + "theta.weight", (int64_t)Cg * C);
-      const float* tb = c.L->get(hp + "theta.bias", Cg);
-      const float* pw = c.L->get(hp + "phi.weight", (int64_t)Cg * C);
-      const float* pb = c.L->get(hp + "phi.bias", Cg);
-      const float* wc = c.L->get(hp + "concat_project.0.weight", 2 * Cg);
-      if (!c.L->ok) return 1;
-      global_collapse_bwd_kernel<<<Cg, 128, 0, c.st>>>(dU, dcab, hd, C, Cg, tw, tb, pw, pb, wc, gtw, gtb, gpw, gpb, gwc);
-    }
+  c.launch(rowdot_bwd_x_kernel, cdiv(M * C, 256), 256, 0, dab, bc.U, 8, M, C, dXg, C);
+  c.launch(add_inplace_kernel, cdiv(M * C, 256), 256, 0, dX, dXg, M * C);
+  const int Cg = C / 4;
+  for (int hd = 0; hd < (c.pgrad ? 4 : 0); ++hd) {
+    const std::string hp = gp + "attentions." + std::to_string(hd) + ".";
+    c.copy(c.grad(hp + "g.weight", (int64_t)Cg * C), dWg + (size_t)hd * Cg * C, sizeof(float) * Cg * C);
+    c.copy(c.grad(hp + "g.bias", Cg), dbg + hd * Cg, sizeof(float) * Cg);
+    c.copy(c.grad(hp + "C_k", (int64_t)J * J), dCk + hd * J * J, sizeof(float) * J * J);
+    const float* tw = c.param(hp + "theta.weight", (int64_t)Cg * C);
+    const float* tb = c.param(hp + "theta.bias", Cg);
+    const float* pw = c.param(hp + "phi.weight", (int64_t)Cg * C);
+    const float* pb = c.param(hp + "phi.bias", Cg);
+    const float* wc = c.param(hp + "concat_project.0.weight", 2 * Cg);
+    float* gtw = c.grad(hp + "theta.weight", (int64_t)Cg * C);
+    float* gtb = c.grad(hp + "theta.bias", Cg);
+    float* gpw = c.grad(hp + "phi.weight", (int64_t)Cg * C);
+    float* gpb = c.grad(hp + "phi.bias", Cg);
+    float* gwc = c.grad(hp + "concat_project.0.weight", 2 * Cg);
+    c.launch(global_collapse_bwd_kernel, Cg, 128, 0, dU, dcab, hd, C, Cg, tw, tb, pw, pb, wc, gtw, gtb, gpw, gpb, gwc);
   }
   // (c) local branch
   float* dZlc = c.fl((size_t)M * C);
   if (bn_bwd(c, b.bnlc, dAcat + C, 3 * C, dZlc, C)) return 1;
   float* dXY = c.fl((size_t)M * 2 * C);
-  {
-    const float* w = c.dry ? nullptr : c.L->get(lp + "cat_conv.weight", (int64_t)C * 2 * C);
-    float* gw;
-    if (!want_grad(c, lp + "cat_conv.weight", (int64_t)C * 2 * C, &gw) || (!c.dry && !c.L->ok)) return 1;
-    if (dense_tn(c, dZlc, C, b.XY, 2 * C, M, C, 2 * C, gw, 2 * C)) return 1;
-    if (dense_nn(c, dZlc, C, w, 2 * C, M, C, 2 * C, dXY, 2 * C)) return 1;
-  }
+  if (conv1x1_bwd(c, lp + "cat_conv.weight", dZlc, b.XY, M, C, 2 * C, dXY)) return 1;
   float* dS = c.fl((size_t)M * 2 * C);
   if (bn_bwd(c, b.bn1, dXY, 2 * C, dS, 2 * C)) return 1;
   if (bn_bwd(c, b.bn2, dXY + C, 2 * C, dS + C, 2 * C)) return 1;
@@ -394,30 +358,22 @@ static int block_bwd(TCtx& c, BlockSave& b, BlockConsts& bc, const float* dOut, 
     float* dA = c.fl((size_t)h->nnz[m] * C);
     const int dsplit = (int)std::max<long long>(1, std::min<long long>(32, F / 32));   // frame ranges of semch_dcoef_kernel
     double* dpart = c.dbl((size_t)dsplit * h->nnz[m] * C);
-    const std::string g = lp + (m == 0 ? "gcn_sym." : "gcn_con.");
-    float* ge;
-    if (!want_grad(c, g + "e", (int64_t)C * h->nnz[m], &ge)) return 1;
-    if (c.dry) continue;
-    NbrRows nr = nbr_rows(h->nbr[m], J);
-    semch_mix_bwd_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(dS + m * C, 2 * C, b.coefA[m], h->nbr[m], nr, h->nnz[m], J, F,
-                                                            C, dH + m * 2 * C, 4 * C);
+    float* ge = c.grad(lp + (m == 0 ? "gcn_sym.e" : "gcn_con.e"), (int64_t)C * h->nnz[m]);
+    const NbrRows nr = nbr_rows(h->nbr[m], J);
+    c.launch(semch_mix_bwd_kernel, cdiv(M * C, 256), 256, 0, dS + m * C, 2 * C, b.coefA[m], h->nbr[m], nr, h->nnz[m], J,
+             F, C, dH + m * 2 * C, 4 * C);
     if (!c.pgrad) continue;
-    semch_dcoef_kernel<<<dim3(cdiv((long long)h->nnz[m] * C, 128), dsplit), 128, 0, c.st>>>(
-        dS + m * C, 2 * C, b.H + m * 2 * C, 4 * C, h->nbr[m], nr, h->nnz[m], J, F, C, dpart);
-    semch_dcoef_reduce_kernel<<<cdiv((long long)h->nnz[m] * C, 128), 128, 0, c.st>>>(dpart, dsplit, h->nnz[m] * C, dA);
-    semch_de_kernel<<<cdiv((long long)C * J, 128), 128, 0, c.st>>>(b.coefA[m], dA, h->nbr[m], h->nnz[m], J, C, ge);
+    c.launch(semch_dcoef_kernel, dim3(cdiv((long long)h->nnz[m] * C, 128), dsplit), 128, 0, dS + m * C, 2 * C,
+             b.H + m * 2 * C, 4 * C, h->nbr[m], nr, h->nnz[m], J, F, C, dpart);
+    c.launch(semch_dcoef_reduce_kernel, cdiv((long long)h->nnz[m] * C, 128), 128, 0, dpart, dsplit, h->nnz[m] * C, dA);
+    c.launch(semch_de_kernel, cdiv((long long)C * J, 128), 128, 0, b.coefA[m], dA, h->nbr[m], h->nnz[m], J, C, ge);
   }
   if (dense_tn(c, dH, 4 * C, b.X, C, M, 4 * C, C, dWst, C)) return 1;
   if (dense_nn(c, dH, 4 * C, b.Wst, C, M, 4 * C, C, dXl, C)) return 1;
-  if (!c.dry) {
-    add_inplace_kernel<<<cdiv(M * C, 256), 256, 0, c.st>>>(dX, dXl, M * C);
-    for (int m = 0; m < (c.pgrad ? 2 : 0); ++m) {
-      const std::string g = lp + (m == 0 ? "gcn_sym." : "gcn_con.");
-      float* gW = grad_ptr(h, g + "W", (int64_t)2 * C * C);
-      if (!gW) return 1;
-      semch_wgrad_relayout_kernel<<<cdiv((long long)2 * C * C, 256), 256, 0, c.st>>>(dWst + (size_t)m * 2 * C * C, C, C, C, gW);
-    }
-  }
+  c.launch(add_inplace_kernel, cdiv(M * C, 256), 256, 0, dX, dXl, M * C);
+  for (int m = 0; m < (c.pgrad ? 2 : 0); ++m)
+    c.launch(semch_wgrad_relayout_kernel, cdiv((long long)2 * C * C, 256), 256, 0, dWst + (size_t)m * 2 * C * C, C, C,
+             C, c.grad(lp + (m == 0 ? "gcn_sym.W" : "gcn_con.W"), (int64_t)2 * C * C));
   return 0;
 }
 
@@ -433,9 +389,9 @@ static int train_forward(gast_handle* h, TCtx& c, TrainState& ts, const float* x
   // takes the schedule gast_forward takes (ts.sn), and a dilated model fed one receptive field computes only
   // the positions its output needs.
   const int sn = ts.frozen ? ts.sn : (cf.strided ? 1 : 0);
-  Geometry g;
-  if (geometry(h, T, sn, &g)) return 1;
-  ts.B = B; ts.T = T; ts.T0 = g.T0; ts.s0 = g.s0; ts.x = x;
+  if (geometry(h, T, sn, &ts.geo)) return 1;
+  const Geometry& g = ts.geo;
+  ts.B = B; ts.T = T; ts.x = x;
   ts.blocks.assign(L, BlockSave());
   ts.stages.assign(L - 1, StageSave());
   const RowMap id{1, 1, 1, 0};
@@ -448,88 +404,67 @@ static int train_forward(gast_handle* h, TCtx& c, TrainState& ts, const float* x
   ts.Z0 = c.fl((size_t)M0 * C);
   ts.act0 = c.fl((size_t)M0 * C);
   if (bn_fwd(c, ts.bnin, "init_bn.", x, Fin, Min, Fin, 0, 0.f, ts, nullptr, 0, id, ts.xbn, Fin)) return 1;
-  if (!c.dry) {
-    const float* we = c.L->get("expand_conv.weight", (int64_t)C * Fin * k0);
-    if (!c.L->ok) return 1;
-    cudaMemsetAsync(ts.Acol, 0, sizeof(float) * (size_t)M0 * KP, c.st);
-    cudaMemsetAsync(ts.We8, 0, sizeof(float) * (size_t)C * KP, c.st);
-    const ASeg sg = seg_taps(ts.xbn, Fin, Fin, k0, (long long)J * Fin, RowMap{g.T0, T, g.s0, 0});
-    seg_gather_kernel<<<cdiv(M0 * sg.K, 256), 256, 0, c.st>>>(sg, J, F0, ts.Acol, KP, 0);
-    BnP none{nullptr, nullptr, nullptr, nullptr};
-    // We8[c][tap*Fin + i] = w[c][i][tap]  (fold_conv_kernel with no BN is exactly this re-layout)
-    float* tmp = c.fl((size_t)C * k0 * Fin);
-    fold_conv_kernel<<<cdiv((long long)C * Fin * k0, 256), 256, 0, c.st>>>(tmp, nullptr, we, C, Fin, k0, none);
-    copy2d_kernel<<<cdiv((long long)C * k0 * Fin, 256), 256, 0, c.st>>>(tmp, k0 * Fin, ts.We8, KP, C, k0 * Fin, 0);
-  } else {
-    c.fl((size_t)C * k0 * Fin);
-  }
+  const float* we = c.param("expand_conv.weight", (int64_t)C * Fin * k0);
+  float* tmp = c.fl((size_t)C * k0 * Fin);
+  c.zero(ts.Acol, sizeof(float) * (size_t)M0 * KP);
+  c.zero(ts.We8, sizeof(float) * (size_t)C * KP);
+  const ASeg sg = seg_taps(ts.xbn, Fin, Fin, k0, (long long)J * Fin, RowMap{g.T0, T, g.s0, 0});
+  c.launch(seg_gather_kernel, cdiv(M0 * sg.K, 256), 256, 0, sg, J, F0, ts.Acol, KP, 0);
+  BnP none{nullptr, nullptr, nullptr, nullptr};
+  // We8[c][tap*Fin + i] = w[c][i][tap]  (fold_conv_kernel with no BN is exactly this re-layout)
+  c.launch(fold_conv_kernel, cdiv((long long)C * Fin * k0, 256), 256, 0, tmp, nullptr, we, C, Fin, k0, none);
+  c.launch(copy2d_kernel, cdiv((long long)C * k0 * Fin, 256), 256, 0, tmp, k0 * Fin, ts.We8, KP, C, k0 * Fin, 0);
   if (dense_nt(c, ts.Acol, KP, ts.We8, M0, C, KP, ts.Z0, C)) return 1;
   if (bn_fwd(c, ts.bnex, "expand_bn.", ts.Z0, C, M0, C, 1, 0.f, ts, nullptr, 0, id, ts.act0, C)) return 1;
   if (block_fwd(c, ts, ts.blocks[0], h->blocks[0], "layers_graph_conv.0.", ts.act0, F0)) return 1;
   const float* cur = ts.blocks[0].Out;
-  long long F = F0;
-  int Tp = g.T0;
   for (int i = 1; i < L; ++i) {
     StageSave& s = ts.stages[i - 1];
-    Sched sc;
-    stage_sched(h, i, sn, &sc);
-    const int Cw = C << i, Tn = g.Ts[i - 1];
-    const long long Fn = (long long)B * Tn, Mn = Fn * J;
-    s.Cw = Cw; s.taps = sc.taps; s.Fin = F; s.Fout = Fn; s.Tin = Tp; s.Tout = Tn; s.X = cur; s.idx = i - 1; s.dil = sc.dil;
-    s.tapmap = RowMap{Tn, Tp, sc.stride, 0};
-    s.resmap = RowMap{Tn, Tp, sc.res_mul, sc.res_off};
-    s.Wt = c.fl((size_t)Cw * sc.taps * Cw);
+    const StageGeo& sgeo = g.stages[i - 1];
+    const int Cw = C << i;
+    const long long Fn = (long long)B * sgeo.Tout, Mn = Fn * J;
+    s.g = sgeo; s.Cw = Cw; s.X = cur; s.idx = i - 1;
+    s.Wt = c.fl((size_t)Cw * sgeo.taps * Cw);
     s.Z1 = c.fl((size_t)Mn * Cw); s.Hh = c.fl((size_t)Mn * Cw); s.Z2 = c.fl((size_t)Mn * Cw); s.Out = c.fl((size_t)Mn * Cw);
-    const std::string k0s = "layers_conv." + std::to_string(2 * (i - 1)) + ".weight";
-    const std::string k1s = "layers_conv." + std::to_string(2 * (i - 1) + 1) + ".weight";
-    const float* w1 = nullptr;
-    if (!c.dry) {
-      const float* w0 = c.L->get(k0s, (int64_t)Cw * Cw * sc.taps);
-      w1 = c.L->get(k1s, (int64_t)Cw * Cw);
-      if (!c.L->ok) return 1;
-      BnP none{nullptr, nullptr, nullptr, nullptr};
-      fold_conv_kernel<<<cdiv((long long)Cw * Cw * sc.taps, 256), 256, 0, c.st>>>(s.Wt, nullptr, w0, Cw, Cw, sc.taps, none);
-    }
-    const ASeg sg = seg_taps(cur, Cw, Cw, sc.taps, (long long)sc.dil * J * Cw, s.tapmap);
-    if (seg_gemm(c, &sg, 1, s.Wt, sc.taps * Cw, Fn, Cw, s.Z1, Cw)) return 1;
+    const float* w0 = c.param("layers_conv." + std::to_string(2 * (i - 1)) + ".weight", (int64_t)Cw * Cw * sgeo.taps);
+    const float* w1 = c.param("layers_conv." + std::to_string(2 * (i - 1) + 1) + ".weight", (int64_t)Cw * Cw);
+    c.launch(fold_conv_kernel, cdiv((long long)Cw * Cw * sgeo.taps, 256), 256, 0, s.Wt, nullptr, w0, Cw, Cw, sgeo.taps,
+             none);
+    const ASeg taps = seg_taps(cur, Cw, Cw, sgeo.taps, (long long)sgeo.dil * J * Cw, sgeo.tapmap);
+    if (seg_gemm(c, &taps, 1, s.Wt, sgeo.taps * Cw, Fn, Cw, s.Z1, Cw)) return 1;
     if (bn_fwd(c, s.bnA, "layers_bn." + std::to_string(2 * (i - 1)) + ".", s.Z1, Cw, Mn, Cw, 1, 0.f, ts, nullptr, 0, id,
                s.Hh, Cw)) return 1;
     if (dense_nt(c, s.Hh, Cw, w1, Mn, Cw, Cw, s.Z2, Cw)) return 1;
     if (bn_fwd(c, s.bnB, "layers_bn." + std::to_string(2 * (i - 1) + 1) + ".", s.Z2, Cw, Mn, Cw, 1, ts.drop_p, ts, cur, Cw,
-               s.resmap, s.Out, Cw)) return 1;
+               sgeo.resmap, s.Out, Cw)) return 1;
     if (block_fwd(c, ts, ts.blocks[i], h->blocks[i], "layers_graph_conv." + std::to_string(i) + ".", s.Out, Fn)) return 1;
     cur = ts.blocks[i].Out;
-    F = Fn; Tp = Tn;
   }
-  ts.last = cur; ts.Flast = F;
-  if (!c.dry && y) {
-    const int Cl = C << L;
-    const float* ws = c.L->get("shrink.weight", (int64_t)3 * Cl);
-    if (!c.L->ok) return 1;
-    shrink_kernel<<<cdiv(F * J * 32, 256), 256, 0, c.st>>>(cur, Cl, ws, y, F * J, Cl);
-  }
+  ts.last = cur;
+  const int Cl = C << L;
+  const long long M = (long long)B * g.T_out * J;
+  const float* ws = c.param("shrink.weight", (int64_t)3 * Cl);
+  if (y) c.launch(shrink_kernel, cdiv(M * 32, 256), 256, 0, cur, Cl, ws, y, M, Cl);
   return 0;
 }
 
 // dy -> the parameter gradients (c.pgrad) and dL/dx into dx (B,T,J,F; may be null)
-static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* dy, float* dx) {
+static int train_backward(gast_handle* h, TCtx& c, const TrainState& ts, const float* dy, float* dx) {
   const gast_cfg& cf = h->cfg;
   const int J = c.J, C = cf.channels, L = cf.num_stages, Fin = cf.in_features, k0 = cf.filter_widths[0];
   const int Cl = C << L;
-  long long F = ts.Flast;
+  const Geometry& g = ts.geo;
   // shrink
-  float* dcur = c.fl((size_t)F * J * Cl);
-  if (!c.dry) {
-    const float* ws = c.L->get("shrink.weight", (int64_t)3 * Cl);
-    float* gws;
-    if (!want_grad(c, "shrink.weight", (int64_t)3 * Cl, &gws) || !c.L->ok) return 1;
-    shrink_bwd_x_kernel<<<cdiv(F * J * Cl, 256), 256, 0, c.st>>>(dy, ws, F * J, Cl, dcur);
-    if (gws) shrink_bwd_w_kernel<<<cdiv(Cl, 32), dim3(32, SBW_RG), 0, c.st>>>(dy, ts.last, F * J, Cl, gws);
-  }
+  const long long M = (long long)ts.B * g.T_out * J;
+  float* dcur = c.fl((size_t)M * Cl);
+  const float* ws = c.param("shrink.weight", (int64_t)3 * Cl);
+  float* gws = c.grad("shrink.weight", (int64_t)3 * Cl);
+  c.launch(shrink_bwd_x_kernel, cdiv(M * Cl, 256), 256, 0, dy, ws, M, Cl, dcur);
+  if (gws) c.launch(shrink_bwd_w_kernel, cdiv(Cl, 32), dim3(32, SBW_RG), 0, dy, ts.last, M, Cl, gws);
   for (int i = L - 1; i >= 1; --i) {
-    StageSave& s = ts.stages[i - 1];
-    const int Cw = s.Cw;
-    const long long Mn = s.Fout * J, Mi = s.Fin * J;
+    const StageSave& s = ts.stages[i - 1];
+    const int Cw = s.Cw, taps = s.g.taps;
+    const long long Fout = (long long)ts.B * s.g.Tout, Mn = Fout * J, Mi = (long long)ts.B * s.g.Tin * J;
     float* dSout = c.fl((size_t)Mn * Cw);
     if (block_bwd(c, ts.blocks[i], h->blocks[i], dcur, dSout)) return 1;
     // stage: out = res + drop(relu(bn(conv1x1(h))));  h = relu(bn(conv_taps(x)))
@@ -537,41 +472,28 @@ static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* 
     float* dZ2 = c.fl((size_t)Mn * Cw);
     float* dHh = c.fl((size_t)Mn * Cw);
     float* dZ1 = c.fl((size_t)Mn * Cw);
-    float* Xcol = c.fl((size_t)Mn * s.taps * Cw);
-    float* dXcol = c.fl((size_t)Mn * s.taps * Cw);
-    float* dWt = c.fl((size_t)Cw * s.taps * Cw);
-    if (!c.dry) {
-      cudaMemsetAsync(dXin, 0, sizeof(float) * (size_t)Mi * Cw, c.st);
-      const ASeg rs = seg_taps(dXin, Cw, Cw, 1, 0, s.resmap);
-      seg_scatter_add_kernel<<<cdiv(Mn * Cw, 256), 256, 0, c.st>>>(rs, J, s.Fout, dSout, Cw, 0);
-    }
+    float* Xcol = c.fl((size_t)Mn * taps * Cw);
+    float* dXcol = c.fl((size_t)Mn * taps * Cw);
+    float* dWt = c.fl((size_t)Cw * taps * Cw);
+    c.zero(dXin, sizeof(float) * (size_t)Mi * Cw);
+    const ASeg rs = seg_taps(dXin, Cw, Cw, 1, 0, s.g.resmap);
+    c.launch(seg_scatter_add_kernel, cdiv(Mn * Cw, 256), 256, 0, rs, J, Fout, dSout, Cw, 0);
     if (bn_bwd(c, s.bnB, dSout, Cw, dZ2, Cw)) return 1;
-    {
-      const std::string k1s = "layers_conv." + std::to_string(2 * s.idx + 1) + ".weight";
-      const float* w1 = c.dry ? nullptr : c.L->get(k1s, (int64_t)Cw * Cw);
-      float* gw1;
-      if (!want_grad(c, k1s, (int64_t)Cw * Cw, &gw1) || (!c.dry && !c.L->ok)) return 1;
-      if (dense_tn(c, dZ2, Cw, s.Hh, Cw, Mn, Cw, Cw, gw1, Cw)) return 1;
-      if (dense_nn(c, dZ2, Cw, w1, Cw, Mn, Cw, Cw, dHh, Cw)) return 1;
-    }
+    if (conv1x1_bwd(c, "layers_conv." + std::to_string(2 * s.idx + 1) + ".weight", dZ2, s.Hh, Mn, Cw, Cw, dHh)) return 1;
     if (bn_bwd(c, s.bnA, dHh, Cw, dZ1, Cw)) return 1;
-    const ASeg sg = seg_taps(s.X, Cw, Cw, s.taps, (long long)s.dil * J * Cw, s.tapmap);
-    if (!c.dry && c.pgrad) seg_gather_kernel<<<cdiv(Mn * sg.K, 256), 256, 0, c.st>>>(sg, J, s.Fout, Xcol, s.taps * Cw, 0);
-    if (dense_tn(c, dZ1, Cw, Xcol, s.taps * Cw, Mn, Cw, s.taps * Cw, dWt, s.taps * Cw)) return 1;
-    if (dense_nn(c, dZ1, Cw, s.Wt, s.taps * Cw, Mn, Cw, s.taps * Cw, dXcol, s.taps * Cw)) return 1;
-    float* gw0;
-    if (!want_grad(c, "layers_conv." + std::to_string(2 * s.idx) + ".weight", (int64_t)Cw * Cw * s.taps, &gw0)) return 1;
-    if (!c.dry) {
-      if (gw0)
-        conv_wgrad_relayout_kernel<<<cdiv((long long)Cw * Cw * s.taps, 256), 256, 0, c.st>>>(dWt, Cw, Cw, s.taps, s.taps * Cw, gw0);
-      ASeg dsg = sg; dsg.base = dXin;
-      seg_scatter_add_kernel<<<cdiv(Mn * dsg.K, 256), 256, 0, c.st>>>(dsg, J, s.Fout, dXcol, s.taps * Cw, 0);
-    }
+    const ASeg sg = seg_taps(s.X, Cw, Cw, taps, (long long)s.g.dil * J * Cw, s.g.tapmap);
+    if (c.pgrad) c.launch(seg_gather_kernel, cdiv(Mn * sg.K, 256), 256, 0, sg, J, Fout, Xcol, taps * Cw, 0);
+    if (dense_tn(c, dZ1, Cw, Xcol, taps * Cw, Mn, Cw, taps * Cw, dWt, taps * Cw)) return 1;
+    if (dense_nn(c, dZ1, Cw, s.Wt, taps * Cw, Mn, Cw, taps * Cw, dXcol, taps * Cw)) return 1;
+    float* gw0 = c.grad("layers_conv." + std::to_string(2 * s.idx) + ".weight", (int64_t)Cw * Cw * taps);
+    if (gw0)
+      c.launch(conv_wgrad_relayout_kernel, cdiv((long long)Cw * Cw * taps, 256), 256, 0, dWt, Cw, Cw, taps, taps * Cw, gw0);
+    ASeg dsg = sg; dsg.base = dXin;
+    c.launch(seg_scatter_add_kernel, cdiv(Mn * dsg.K, 256), 256, 0, dsg, J, Fout, dXcol, taps * Cw, 0);
     dcur = dXin;
-    F = s.Fin;
   }
   // first block
-  const long long F0 = (long long)ts.B * ts.T0, M0 = F0 * J;
+  const long long F0 = (long long)ts.B * g.T0, M0 = F0 * J;
   float* dAct0 = c.fl((size_t)M0 * C);
   if (block_bwd(c, ts.blocks[0], h->blocks[0], dcur, dAct0)) return 1;
   // expand
@@ -585,14 +507,11 @@ static int train_backward(gast_handle* h, TCtx& c, TrainState& ts, const float* 
   float* dxin = c.fl((size_t)Min * Fin);
   if (dense_tn(c, dZ0, C, ts.Acol, KP, M0, C, KP, dWe8, KP)) return 1;
   if (dense_nn(c, dZ0, C, ts.We8, KP, M0, C, KP, dAcol, KP)) return 1;
-  float* gwe;
-  if (!want_grad(c, "expand_conv.weight", (int64_t)C * Fin * k0, &gwe)) return 1;
-  if (!c.dry) {
-    if (gwe) conv_wgrad_relayout_kernel<<<cdiv((long long)C * Fin * k0, 256), 256, 0, c.st>>>(dWe8, C, Fin, k0, KP, gwe);
-    cudaMemsetAsync(dxbn, 0, sizeof(float) * (size_t)Min * Fin, c.st);
-    const ASeg sg = seg_taps(dxbn, Fin, Fin, k0, (long long)J * Fin, RowMap{ts.T0, ts.T, ts.s0, 0});
-    seg_scatter_add_kernel<<<cdiv(M0 * sg.K, 256), 256, 0, c.st>>>(sg, J, F0, dAcol, KP, 0);
-  }
+  float* gwe = c.grad("expand_conv.weight", (int64_t)C * Fin * k0);
+  if (gwe) c.launch(conv_wgrad_relayout_kernel, cdiv((long long)C * Fin * k0, 256), 256, 0, dWe8, C, Fin, k0, KP, gwe);
+  c.zero(dxbn, sizeof(float) * (size_t)Min * Fin);
+  const ASeg sg = seg_taps(dxbn, Fin, Fin, k0, (long long)J * Fin, RowMap{g.T0, ts.T, g.s0, 0});
+  c.launch(seg_scatter_add_kernel, cdiv(M0 * sg.K, 256), 256, 0, sg, J, F0, dAcol, KP, 0);
   // init_bn: dx = dxbn . gamma . invstd (frozen), the batch-statistics adjoint otherwise
   if (bn_bwd(c, ts.bnin, dxbn, Fin, dx ? dx : dxin, Fin)) return 1;
   return 0;

@@ -186,6 +186,10 @@ int gast_tta_merge(const float* pred, float* out, int32_t T, int32_t J, int32_t 
  *   gast_backward(h, dy, ws, n, st) is gast_backward_input(h, dy, NULL, 1, ws, n, st).  The backward is refused
  *   before any launch unless workspace_bytes is at least gast_train_workspace_bytes of its forward's B, T and
  *   dropout_p: the size that forward checked, which bounds every backward of it.
+ * A missing or wrong-sized parameter binding, and for a backward with param_grads a missing or wrong-sized gradient
+ *   buffer, is refused before any launch, and the error names the key.  A refused gast_forward_train leaves the
+ *   running statistics untouched; a refused backward keeps the saved forward, so the caller can fix the binding and
+ *   call it again.  gast_train_workspace_bytes needs nothing bound.
  * Both models train on their own schedule (strided for Optimized1f, dilated or dense otherwise; main.py:166-175). */
 int gast_bind_grads(gast_t* h, int32_t n, const char* const* keys, void* const* dev_ptrs, const int64_t* numel);
 size_t gast_train_workspace_bytes(gast_t* h, int32_t B, int32_t T, float dropout_p);
@@ -203,7 +207,9 @@ int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_t param_gra
  *   gast_bind_grads and dL/dx (B,T,J,F) into dx (may be null).  Running statistics are only read.  The eval
  *   forward itself is unchanged; nothing is kept between it and this call.  Like gast_forward_train it rewrites
  *   the attention constants gast_prepare derives, from the same parameters (so with the same values).
- * gast_eval_backward_workspace_bytes: scratch for it with parameter gradients (the input-only call needs less).
+ *   A bad parameter binding, or with param_grads a bad gradient buffer, is refused before any launch.
+ * gast_eval_backward_workspace_bytes: scratch for it with parameter gradients (the input-only call needs less); it
+ *   needs nothing bound.
  * gast_last_launch_count afterwards: the GEMM and weight-gradient kernels this call enqueued. */
 size_t gast_eval_backward_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now);
 int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads, int32_t B, int32_t T,
