@@ -80,15 +80,18 @@ constexpr int CHUNK_XIN_THREADS = 256;
 // stream's newest frame, which may be an earlier held frame of the chunk, so frame k takes x[b, src[k]] with src[k] the
 // latest frame <= k that is not held (a block-wide max scan), or the newest frame of xhist when there is none.  A fresh
 // stream's history is copies of its frame 0.  x rows of held frames are never read.  sidx (m) or null: row b of x / xin
-// / fresh / hold belongs to state stream sidx[b] (a subset push, gast_stream_push_subset); null = stream b.
+// / fresh / hold belongs to state stream sidx[b] (a subset push, gast_stream_push_subset); null = stream b.  act (m) or
+// null (all active): a row with act[b] == 0 sits the call out: its xin is built as if every frame were held (x is not
+// read) and its input history is not written.
 __global__ void __launch_bounds__(CHUNK_XIN_THREADS)
 stream_chunk_xin_kernel(float* __restrict__ xhist, const float* __restrict__ x, float* __restrict__ xin,
                         const int32_t* __restrict__ fresh, const int32_t* __restrict__ hold, int k0, int K, int JF,
-                        const int32_t* __restrict__ sidx) {
+                        const int32_t* __restrict__ sidx, const int32_t* __restrict__ act) {
   __shared__ int src[CHUNK_XIN_THREADS];
   __shared__ int wmax[CHUNK_XIN_THREADS / 32];
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool is_fresh = fresh && fresh[b];
+  const bool on = !act || act[b];
+  const bool is_fresh = on && fresh && fresh[b];
   float* hrow = xhist + (long long)(sidx ? sidx[b] : b) * k0 * JF;
   float* irow = xin + (long long)b * (k0 - 1 + K) * JF;
   const float* xrow = x + (long long)b * K * JF;
@@ -96,7 +99,7 @@ stream_chunk_xin_kernel(float* __restrict__ xhist, const float* __restrict__ x, 
   int carry = -1;                                          // latest frame not held before this tile
   for (int t0 = 0; t0 < K; t0 += CHUNK_XIN_THREADS) {
     const int k = t0 + tid;
-    const bool held = k >= K || (hb && hb[k] && !(k == 0 && is_fresh));
+    const bool held = k >= K || !on || (hb && hb[k] && !(k == 0 && is_fresh));
     int v = held ? -1 : k;
     for (int o = 1; o < 32; o <<= 1) {                    // inclusive max scan: warp, then across warps
       const int u = __shfl_up_sync(0xffffffffu, v, o);
@@ -117,6 +120,7 @@ stream_chunk_xin_kernel(float* __restrict__ xhist, const float* __restrict__ x, 
   }
   for (int e = tid; e < (k0 - 1) * JF; e += CHUNK_XIN_THREADS)
     irow[e] = is_fresh ? xrow[e % JF] : hrow[e + JF];
+  if (!on) return;                                         // the whole block: b is the block's row
   __syncthreads();                                         // every read of hrow is done; irow is visible to the block
   for (int e = tid; e < k0 * JF; e += CHUNK_XIN_THREADS) hrow[e] = irow[(long long)(K - 1) * JF + e];
 }
@@ -149,14 +153,17 @@ __global__ void stream_chunk_gather_kernel(float4* __restrict__ G, const float4*
 // the tail of G when t falls in the chunk, copies of tail position 0 for a fresh stream, else the slot keeps its value.
 // ek = (step + K - 1) mod R.  Launched after stream_chunk_gather_kernel, which reads slots this kernel overwrites.
 // Grid over the R*m rows (slot, listed stream); tab as in stream_chunk_gather_kernel (null: m = n, ek for all; else
-// ek = (tab[m + b] + K - 1) mod R per stream and slot p of stream tab[b] is written).
+// ek = (tab[m + b] + K - 1) mod R per stream and slot p of stream tab[b] is written).  act (m) or null (all active):
+// nothing is written for a row with act[b] == 0.
 __global__ void stream_chunk_ring_kernel(float4* __restrict__ ring, const float4* __restrict__ G,
                                          const int32_t* __restrict__ fresh, int m, int n, int R, int ek, int H, int K,
-                                         long long row4, const int32_t* __restrict__ tab) {
+                                         long long row4, const int32_t* __restrict__ tab,
+                                         const int32_t* __restrict__ act) {
   const long long total = (long long)R * m * row4;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long q = i % row4, f = i / row4;
     const int p = (int)(f / m), b = (int)(f - (long long)p * m);
+    if (act && !act[b]) continue;
     const int e = tab ? (int)(((long long)tab[m + b] + K - 1) % R) : ek;
     const int k = K - 1 - (e - p + R) % R;                // chunk position of time t
     if (k < 0 && !(fresh && fresh[b])) continue;
@@ -175,6 +182,23 @@ __global__ void stream_peek_xin_kernel(const float* __restrict__ xhist, float* _
     const long long f = i / JF;
     const int e = (int)(i - f * JF), b = (int)(f / T), p = (int)(f - (long long)b * T);
     xin[i] = xhist[((long long)(sidx ? sidx[b] : b) * k0 + min(p + 1, k0 - 1)) * JF + e];
+  }
+}
+
+// The table of a call driven by device-resident counts (gast_stream_push_device / _peek_device), over all n streams:
+// tab[b] = b, tab[n + b] = phase = count mod rmax, tab[2n + b] = the effective fresh mask fresh[b] || count == 0 (a
+// stream that never pushed starts a sequence: its ring is never read).  A negative count is taken as 0.  advance > 0 (a
+// push) then sets the count of every active stream (act null: all) to count + advance.  Every value read here only
+// selects a phase in [0, rmax) or a flag, so no content of counts, act or fresh can send a later kernel out of bounds.
+__global__ void stream_device_table_kernel(int64_t* __restrict__ counts, const int32_t* __restrict__ act,
+                                           const int32_t* __restrict__ fresh, int32_t* __restrict__ tab, int n,
+                                           int64_t rmax, int advance) {
+  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < n; b += gridDim.x * blockDim.x) {
+    const int64_t c = counts[b] > 0 ? counts[b] : 0;
+    tab[b] = b;
+    tab[n + b] = (int32_t)(c % rmax);
+    tab[2 * n + b] = (fresh && fresh[b]) || c == 0;
+    if (advance && (!act || act[b])) counts[b] = c + advance;
   }
 }
 
@@ -362,9 +386,10 @@ extern "C" int gast_stream_push(gast_t* h, void* state, int64_t step, const floa
 // (single or chunk) finds the history it expects.  The blocks are pointwise in time and run on n*K frames.
 struct ChunkBufs { float *xin, *G; StreamBufs sb; int32_t* tab; };
 
-// The workspace of a chunk call over m streams of K frames: the chunk buffers, then the (stream, phase) table of a
-// subset call (2m ints, gast_stream_push_subset below) when `table`.  sp gives the dilations only.
-static int chunk_bufs(const gast_handle* h, const StreamPlan& sp, int m, int K, bool table, const char* who, Arena& a,
+// The workspace of a chunk call over m streams of K frames: the chunk buffers, then `table` ints per stream: 0 for a
+// lockstep call, 2 for the (stream, phase) table of a subset call (gast_stream_push_subset below), 3 for the (stream,
+// phase, fresh) table of a device-counts call (gast_stream_push_device).  sp gives the dilations only.
+static int chunk_bufs(const gast_handle* h, const StreamPlan& sp, int m, int K, int table, const char* who, Arena& a,
                       ChunkBufs* cb) {
   const gast_cfg& c = h->cfg;
   const int J = c.num_joints, k0 = c.filter_widths[0];
@@ -376,12 +401,12 @@ static int chunk_bufs(const gast_handle* h, const StreamPlan& sp, int m, int K, 
   cb->xin = a.take((size_t)m * (k0 - 1 + K) * J * c.in_features);
   cb->G = a.take(g);
   stream_bufs(h, m * K, a, &cb->sb);
-  cb->tab = table ? reinterpret_cast<int32_t*>(a.take((size_t)2 * m)) : nullptr;
+  cb->tab = table ? reinterpret_cast<int32_t*>(a.take((size_t)table * m)) : nullptr;
   return 0;
 }
 
 // Bytes that chunk_bufs takes (0 after a refusal): what the workspace of the call must hold.
-static size_t chunk_workspace_bytes(const gast_handle* h, const StreamPlan& sp, int m, int K, bool table,
+static size_t chunk_workspace_bytes(const gast_handle* h, const StreamPlan& sp, int m, int K, int table,
                                     const char* who) {
   Arena dry{nullptr, 0, 0, true};
   ChunkBufs cb;
@@ -391,15 +416,16 @@ static size_t chunk_workspace_bytes(const gast_handle* h, const StreamPlan& sp, 
 extern "C" size_t gast_stream_chunk_workspace_bytes(gast_t* h, int32_t n_streams, int32_t K) {
   StreamPlan sp;
   if (!h || stream_plan(h, n_streams, &sp)) return 0;
-  return chunk_workspace_bytes(h, sp, n_streams, K, false, "gast_stream_chunk_workspace_bytes");
+  return chunk_workspace_bytes(h, sp, n_streams, K, 0, "gast_stream_chunk_workspace_bytes");
 }
 
 // The chunk forward after its input frames are in cb.xin: expand, block 0, the temporal stages on their gathered
 // history (ring write-back when write_rings), shrink into y (m, K, J, 3).  tab null: all m = sp.n streams at `step`;
-// else the device table of a subset call (stream_chunk_gather_kernel): m listed streams, each at its own phase.
+// else the device table of a subset call (stream_chunk_gather_kernel): m listed streams, each at its own phase.  act
+// (m) or null: the write-back skips the rows with act[b] == 0.
 static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, float* sbase, int64_t step, int m,
                          int K, const int32_t* fresh, bool write_rings, const ChunkBufs& cb, float* y,
-                         const int32_t* tab) {
+                         const int32_t* tab, const int32_t* act) {
   const gast_cfg& c = h->cfg;
   const int n = sp.n, J = c.num_joints, L = c.num_stages, k0 = c.filter_widths[0];
   const long long F = (long long)m * K;                  // frames of the chunk, in (stream, frame) order
@@ -422,7 +448,7 @@ static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, 
     if (write_rings) {
       stream_chunk_ring_kernel<<<(unsigned)std::min<long long>(cdiv(r4, 256), grid_cap), 256, 0, st>>>(
           reinterpret_cast<float4*>(ring), reinterpret_cast<const float4*>(cb.G), fresh, m, n, R,
-          (int)((step + K - 1) % R), H, K, row4, tab);
+          (int)((step + K - 1) % R), H, K, row4, tab, act);
       h->launches++;
     }
     // output frame (b, t) = time step+t: taps at G positions t, t+d, ..., t+H; residual at the newest tap (causal)
@@ -447,7 +473,7 @@ static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, 
 extern "C" size_t gast_stream_subset_workspace_bytes(gast_t* h, int32_t m, int32_t K) {
   StreamPlan sp;                                           // the chunk buffers of m streams
   if (!h || m < 1 || stream_plan(h, m, &sp)) return 0;
-  return chunk_workspace_bytes(h, sp, m, K, true, "gast_stream_subset_workspace_bytes");
+  return chunk_workspace_bytes(h, sp, m, K, 2, "gast_stream_subset_workspace_bytes");
 }
 
 // Host-side checks of a subset call and its table: {streams[i]} then {steps[i] mod R_max}.  *lockstep = the call lists
@@ -478,14 +504,17 @@ static int subset_table(const StreamPlan& sp, const int32_t* streams, const int6
 // One chunk call over m streams of K frames.  x null: a peek (below), every frame held and the state only read, its
 // input built by stream_peek_xin_kernel; else a push of x through stream_chunk_xin_kernel.  streams null: the lockstep
 // form, all m = n_streams streams at `step`; else the subset form, stream streams[i] at steps[i], which takes the
-// lockstep addressing (no table) when it lists every stream in order at one step.  Every refusal comes before the
-// first launch.
+// lockstep addressing (no table) when it lists every stream in order at one step.  counts (device) instead of streams:
+// the device-counts form, all m = n_streams streams at their own counts, the ones with active[b] == 0 (active null:
+// none) sitting the call out; its table is built on the device by stream_device_table_kernel.  Every refusal comes
+// before the first launch.
 static int chunk_call(const char* who, gast_handle* h, void* state, int n_streams, const int32_t* streams,
-                      const int64_t* steps, int64_t step, int m, int K, const float* x, float* y,
-                      const int32_t* fresh, const int32_t* hold, void* workspace, size_t workspace_bytes,
-                      void* stream) {
+                      const int64_t* steps, int64_t* counts, const int32_t* active, int64_t step, int m, int K,
+                      const float* x, float* y, const int32_t* fresh, const int32_t* hold, void* workspace,
+                      size_t workspace_bytes, void* stream) {
   if (!h) return fail("%s: null handle", who);
   const bool peek = !x;
+  const int table = streams ? 2 : counts ? 3 : 0;                // ints per stream in the workspace table
   if (peek) {
     const int32_t lat = gast_stream_latency(h);
     if (lat < 0) return 1;
@@ -493,15 +522,15 @@ static int chunk_call(const char* who, gast_handle* h, void* state, int n_stream
       return fail("%s needs a non-causal model: a causal model returns the pose of the pushed frame, so none is ever "
                   "pending", who);
     if (K < 1 || K > lat) return fail("%s: K must be in [1, latency = %d] (got %d)", who, lat, K);
-    if (!streams && step < 1) return fail("%s: step must be at least 1 (the state holds no pushed frame)", who);
+    if (!table && step < 1) return fail("%s: step must be at least 1 (the state holds no pushed frame)", who);
   }
-  if ((!streams && step < 0) || !state || !y) return fail("%s: bad arguments", who);
+  if ((!table && step < 0) || !state || !y) return fail("%s: bad arguments", who);
   StreamPlan sp;
   if (stream_plan(h, n_streams, &sp)) return 1;
   std::vector<int32_t> tab;
-  bool lockstep = true;
+  bool lockstep = !counts;
   if (streams && subset_table(sp, streams, steps, m, peek ? 1 : 0, who, &tab, &lockstep)) return 1;
-  const size_t need = chunk_workspace_bytes(h, sp, m, K, streams != nullptr, who);
+  const size_t need = chunk_workspace_bytes(h, sp, m, K, table, who);
   if (need == 0) return 1;
   if (!h->prepared) return fail("%s: gast_prepare() has not run since the last gast_bind()", who);
   if (call_begin(h, who, need, workspace, workspace_bytes)) return 1;
@@ -510,9 +539,15 @@ static int chunk_call(const char* who, gast_handle* h, void* state, int n_stream
   float* sbase = reinterpret_cast<float*>(align256(state));
   Arena a = workspace_arena(workspace, workspace_bytes);
   ChunkBufs cb;
-  chunk_bufs(h, sp, m, K, streams != nullptr, who, a, &cb);      // sized above: cannot fail
+  chunk_bufs(h, sp, m, K, table, who, a, &cb);                   // sized above: cannot fail
   const int32_t* dtab = nullptr;
-  if (!lockstep) {
+  if (counts) {                                                  // the table and the effective fresh mask
+    stream_device_table_kernel<<<(unsigned)std::min<long long>(cdiv(m, 256), h->sm_count), 256, 0, st>>>(
+        counts, active, fresh, cb.tab, m, sp.R.empty() ? 1 : sp.R.back(), peek ? 0 : K);
+    h->launches++;
+    dtab = cb.tab;
+    fresh = cb.tab + 2 * m;
+  } else if (!lockstep) {
     CUDA_OK(cudaMemcpyAsync(cb.tab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     dtab = cb.tab;
   }
@@ -523,18 +558,18 @@ static int chunk_call(const char* who, gast_handle* h, void* state, int n_stream
         sbase + sp.xhist_off, cb.xin, m, k0, K, JF, dtab);
   } else {
     stream_chunk_xin_kernel<<<m, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K, JF,
-                                                             dtab);
+                                                             dtab, active);
   }
   h->launches++;
-  return chunk_forward(h, st, sp, sbase, step, m, K, fresh, !peek, cb, y, dtab);
+  return chunk_forward(h, st, sp, sbase, step, m, K, fresh, !peek, cb, y, dtab, active);
 }
 
 extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
                                       int32_t K, const int32_t* fresh, const int32_t* hold, void* workspace,
                                       size_t workspace_bytes, void* stream) {
   if (!x) return fail("gast_stream_push_chunk: bad arguments");   // a null x would make the call a peek
-  return chunk_call("gast_stream_push_chunk", h, state, n_streams, nullptr, nullptr, step, n_streams, K, x, y, fresh,
-                    hold, workspace, workspace_bytes, stream);
+  return chunk_call("gast_stream_push_chunk", h, state, n_streams, nullptr, nullptr, nullptr, nullptr, step, n_streams,
+                    K, x, y, fresh, hold, workspace, workspace_bytes, stream);
 }
 
 // ---- peek: the poses K held pushes would return, without pushing ------------------------------------------------
@@ -546,8 +581,8 @@ extern "C" int gast_stream_push_chunk(gast_t* h, void* state, int64_t step, cons
 extern "C" int gast_stream_peek(gast_t* h, const void* state, int64_t step, float* y, int32_t n_streams, int32_t K,
                                 void* workspace, size_t workspace_bytes, void* stream) {
   // only read: chunk_forward writes no ring back for a peek
-  return chunk_call("gast_stream_peek", h, const_cast<void*>(state), n_streams, nullptr, nullptr, step, n_streams, K,
-                    nullptr, y, nullptr, nullptr, workspace, workspace_bytes, stream);
+  return chunk_call("gast_stream_peek", h, const_cast<void*>(state), n_streams, nullptr, nullptr, nullptr, nullptr, step,
+                    n_streams, K, nullptr, y, nullptr, nullptr, workspace, workspace_bytes, stream);
 }
 
 extern "C" int gast_stream_push_subset(gast_t* h, void* state, int32_t n_streams, const int32_t* streams,
@@ -557,8 +592,8 @@ extern "C" int gast_stream_push_subset(gast_t* h, void* state, int32_t n_streams
   const char* who = "gast_stream_push_subset";
   if (!streams || !steps) return fail("%s: null streams or steps", who);   // null streams is the lockstep form
   if (!x) return fail("%s: bad arguments", who);
-  return chunk_call(who, h, state, n_streams, streams, steps, 0, m, K, x, y, fresh, hold, workspace, workspace_bytes,
-                    stream);
+  return chunk_call(who, h, state, n_streams, streams, steps, nullptr, nullptr, 0, m, K, x, y, fresh, hold, workspace,
+                    workspace_bytes, stream);
 }
 
 extern "C" int gast_stream_peek_subset(gast_t* h, const void* state, int32_t n_streams, const int32_t* streams,
@@ -566,6 +601,39 @@ extern "C" int gast_stream_peek_subset(gast_t* h, const void* state, int32_t n_s
                                        size_t workspace_bytes, void* stream) {
   const char* who = "gast_stream_peek_subset";
   if (!streams || !steps) return fail("%s: null streams or steps", who);
-  return chunk_call(who, h, const_cast<void*>(state), n_streams, streams, steps, 0, m, K, nullptr, y, nullptr,
-                    nullptr, workspace, workspace_bytes, stream);
+  return chunk_call(who, h, const_cast<void*>(state), n_streams, streams, steps, nullptr, nullptr, 0, m, K, nullptr, y,
+                    nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
+// ---- the frame counts on the device: calls a CUDA graph can capture ----------------------------------------------
+// The subset entries read the streams and their counts on the host and copy the table from host memory, so a captured
+// call would replay the phases of the tick it was captured at.  These keep the counts on the device: one small kernel
+// (stream_device_table_kernel) turns counts and the active mask into the subset table of all n streams, then the chunk
+// path runs as for a subset call listing every stream, with the inactive rows built as held rows and left out of every
+// state write.  No argument depends on the step, and every check is on the host, before the first launch.
+extern "C" size_t gast_stream_device_workspace_bytes(gast_t* h, int32_t n_streams, int32_t K) {
+  StreamPlan sp;
+  if (!h || stream_plan(h, n_streams, &sp)) return 0;
+  return chunk_workspace_bytes(h, sp, n_streams, K, 3, "gast_stream_device_workspace_bytes");
+}
+
+extern "C" int gast_stream_push_device(gast_t* h, void* state, int32_t n_streams, int64_t* counts,
+                                       const int32_t* active, int32_t K, const float* x, float* y,
+                                       const int32_t* fresh, const int32_t* hold, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  const char* who = "gast_stream_push_device";
+  if (!counts) return fail("%s: null counts", who);
+  if (!x) return fail("%s: bad arguments", who);                 // a null x would make the call a peek
+  return chunk_call(who, h, state, n_streams, nullptr, nullptr, counts, active, 0, n_streams, K, x, y, fresh, hold,
+                    workspace, workspace_bytes, stream);
+}
+
+extern "C" int gast_stream_peek_device(gast_t* h, const void* state, int32_t n_streams, const int64_t* counts,
+                                       const int32_t* active, int32_t K, float* y, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  const char* who = "gast_stream_peek_device";
+  if (!counts) return fail("%s: null counts", who);
+  // only read: the table kernel advances no count for a peek, and chunk_forward writes no ring back
+  return chunk_call(who, h, const_cast<void*>(state), n_streams, nullptr, nullptr, const_cast<int64_t*>(counts), active,
+                    0, n_streams, K, nullptr, y, nullptr, nullptr, workspace, workspace_bytes, stream);
 }

@@ -447,6 +447,192 @@ class CausalStream(PoseStream):
         return super(CausalStream, self).push_frames(frames, streams=streams)[0]
 
 
+class GraphedPoseStream(PoseStream):
+    """`PoseStream` ticks replayed from one CUDA graph: a fixed pool of `n_streams` streams and K frames per stream.
+
+    An eager push costs far more host time (Python bookkeeping and ~30-40 kernel launches) than device time at a
+    few streams, and its time swings from call to call.  Here the launches of one tick,
+    `[gast_tta_prepare] -> gast_stream_push_device -> [gast_stream_peek_device] -> [gast_tta_merge]`, are captured once
+    over static buffers (input, poses, masks, the per-stream frame counts on the device, the state and the workspace)
+    and replayed per tick; the library builds each stream's ring phase from the device counts, so the graph is right
+    at every count.  The constructor takes `PoseStream`'s arguments plus K (frames per stream and tick) and `peek`: 0
+    for none, else the tick also returns provisional poses of `peek` frames (1 <= peek <= latency), what
+    `PoseStream.peek(peek)` returns right after the push.  The tick runs the chunk path, so it pays off for a few
+    streams, most with a peek (one tick instead of two eager calls); hundreds of streams that all push every tick
+    are faster with the eager lockstep push (DESIGN.md §8).
+
+    push(frames (n, K, J, F), streams=None) -> (poses (n, K, J, 3), index (n, K) CPU int64) [+ (peek poses
+    (n, peek, J, 3), peek index (n, peek))]: what `PoseStream.push_frames(frames[streams], streams=streams)` (and
+    then `.peek(peek, streams=streams)`) returns, bit for bit, in the rows of the listed streams; the other streams sit
+    the tick out unchanged, their rows of `frames` are not read and their index is -1.  The poses are views of static
+    buffers that the next tick overwrites: copy them to keep them.  `reset()` / `end()` and `counts` are
+    `PoseStream`'s; `counts` mirrors the device counts without any synchronisation.  `push_frames` and `peek` are
+    refused: the ticks are the graph's.
+
+    Refused with GastError before any replay: a model in training mode, an `engine.set_precision` or
+    `engine.set_gemm_core` change since the capture, and a change of the model's parameters or buffers since the
+    capture unless every stream is restarting (`PoseStream`'s rule after `reset()`), in which case the handle is
+    refreshed and the tick captured again: a graph is never replayed over weights a later `gast_prepare` replaced."""
+
+    def __init__(self, model_pos, n_streams, augment=False, kps_left=None, kps_right=None, joints_left=None,
+                 joints_right=None, device=None, K=1, peek=0):
+        super(GraphedPoseStream, self).__init__(model_pos, n_streams, augment=augment, kps_left=kps_left,
+                                                kps_right=kps_right, joints_left=joints_left,
+                                                joints_right=joints_right, device=device)
+        name = type(self).__name__
+        self.K, self.P = int(K), int(peek)
+        if self.K < 1:
+            raise self.engine.GastError('%s: K must be at least 1 (got %d)' % (name, self.K))
+        if self.P and not 1 <= self.P <= self.latency:
+            raise self.engine.GastError('%s: peek must be 0 or in [1, latency = %d] (got %d)'
+                                        % (name, self.latency, self.P))
+        n, N, J, dev = self.n, self.copies * self.n, self.J, self.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        self._x = torch.zeros((n, self.K, J, self.F), **f32)
+        self._y = torch.zeros((n, self.K, J, 3), **f32)
+        self._py = torch.zeros((n, self.P, J, 3), **f32) if self.P else None
+        # the library's [original | mirrored] twins of x, y and the peek poses
+        self._x2 = torch.zeros((2, n, self.K, J, self.F), **f32) if self.augment else None
+        self._y2 = torch.zeros((2, n, self.K, J, 3), **f32) if self.augment else None
+        self._py2 = torch.zeros((2, n, self.P, J, 3), **f32) if self.augment and self.P else None
+        # [fresh (N) | active (N) | hold (N, K)] on the device, and the pinned buffer every tick stages them in
+        self._mask_dev = torch.zeros(N * (2 + self.K), dtype=torch.int32, device=dev)
+        self._mask_host = torch.zeros(N * (2 + self.K), dtype=torch.int32).pin_memory()
+        self._uploaded = torch.cuda.Event()     # recorded after the last copy out of _mask_host
+        self._counts_dev = torch.zeros(N, dtype=torch.int64, device=dev)
+        self.graph = None
+        self._h = None
+        self._mode = None                       # (GEMM core, precision) at the capture
+        self._launches = 0
+
+    def push_frames(self, frames, valid=None, streams=None):
+        raise self.engine.GastError('%s: call push(); its ticks are replayed from the graph' % type(self).__name__)
+
+    def peek(self, K=None, streams=None):
+        raise self.engine.GastError('%s: construct it with peek=K; every tick then returns the peek'
+                                    % type(self).__name__)
+
+    def _mode_now(self):
+        return (self.engine._FORCE_CORE['core'], self.engine.get_precision(self.model))
+
+    def _tick(self, h, st):
+        """enqueue one tick's library calls on stream `st` -> their launch count"""
+        eng, lib = self.engine, h.lib
+        n, N, K, P, J = self.n, self.copies * self.n, self.K, self.P, self.J
+        ws, wn = self._ws.data_ptr(), self._ws.numel()
+        fresh, active, hold = [t.data_ptr() for t in (self._mask_dev[:N], self._mask_dev[N:2 * N],
+                                                      self._mask_dev[2 * N:])]
+        state, counts = self._state.data_ptr(), self._counts_dev.data_ptr()
+
+        def check(rc, fn):
+            if rc != 0:
+                raise eng.GastError('%s: %s' % (fn, L.last_error()))
+
+        x, y, py = self._x, self._y, self._py
+        launches = 0
+        if self.augment:
+            check(lib.gast_tta_prepare(x.data_ptr(), self._x2.data_ptr(), n * K, J, self.F, 0, 0, len(self.kps_left),
+                                       self._kl, self._kr, st), 'gast_tta_prepare')
+            x, y, py = self._x2, self._y2, self._py2
+            launches += 1
+        check(lib.gast_stream_push_device(h.h, state, N, counts, active, K, x.data_ptr(), y.data_ptr(), fresh, hold,
+                                          ws, wn, st), 'gast_stream_push_device')
+        launches += int(lib.gast_last_launch_count(h.h))
+        if self.augment:
+            check(lib.gast_tta_merge(y.data_ptr(), self._y.data_ptr(), n * K, J, len(self.joints_left), self._jl,
+                                     self._jr, st), 'gast_tta_merge')
+            launches += 1
+        if P:
+            check(lib.gast_stream_peek_device(h.h, state, N, counts, active, P, py.data_ptr(), ws, wn, st),
+                  'gast_stream_peek_device')
+            launches += int(lib.gast_last_launch_count(h.h))
+            if self.augment:
+                check(lib.gast_tta_merge(py.data_ptr(), self._py.data_ptr(), n * P, J, len(self.joints_left),
+                                         self._jl, self._jr, st), 'gast_tta_merge')
+                launches += 1
+        return launches
+
+    def _capture(self):
+        """refresh the handle, size the state and the workspace, warm up outside capture, capture one tick"""
+        eng = self.engine
+        h = eng.model_handle(self.model, self.device)
+        lib, N = h.lib, self.copies * self.n
+        cur = torch.cuda.current_stream(self.device)
+        side = torch.cuda.Stream(self.device)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
+            st = side.cuda_stream
+            h.refresh(self.model, st)
+            if self._state is None:
+                if lib.gast_stream_latency(h.h) != self.latency:
+                    raise eng.GastError('gast_stream_latency: %s' % L.last_error())
+                nb = lib.gast_stream_state_bytes(h.h, N)
+                if nb == 0:
+                    raise eng.GastError('gast_stream_state_bytes: %s' % L.last_error())
+                self._state = torch.zeros(int(nb), dtype=torch.uint8, device=self.device)
+            wb = [lib.gast_stream_device_workspace_bytes(h.h, N, k) for k in (self.K, self.P) if k]
+            if min(wb) == 0:
+                raise eng.GastError('gast_stream_device_workspace_bytes: %s' % L.last_error())
+            if self._ws is None or self._ws.numel() < max(wb):
+                self._ws = torch.empty(int(max(wb)), dtype=torch.uint8, device=self.device)
+            # warm-up (module loads, kernel attributes, the handle's lazy set-up): with every stream inactive it
+            # changes no byte of the state and no count
+            self._mask_dev[N:2 * N].zero_()
+            self._tick(h, st)
+        cur.wait_stream(side)
+        self.graph = None
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            launches = self._tick(h, torch.cuda.current_stream(self.device).cuda_stream)
+        self.graph, self._h, self._sig, self._mode, self._launches = graph, h, h.sig, self._mode_now(), launches
+
+    def push(self, frames, streams=None):
+        eng, name = self.engine, type(self).__name__
+        if self.model.training:
+            raise eng.GastError('%s: call .eval() on the model (streaming is inference)' % name)
+        sel = np.arange(self.n, dtype=np.int64) if streams is None else self._select(streams)
+        frames = torch.as_tensor(frames, dtype=torch.float32)
+        assert tuple(frames.shape) == tuple(self._x.shape), frames.shape
+        with torch.cuda.device(self.device):
+            if self.graph is not None:
+                if self._mode_now() != self._mode:
+                    raise eng.GastError('%s: engine.set_precision or engine.set_gemm_core changed since the tick was '
+                                        'captured; construct a new %s' % (name, name))
+                sig = tuple((v.data_ptr(), v._version) for _, v in eng.named_tensors(self.model))
+                if sig != self._sig or self._h.sig != self._sig:
+                    if not self.book.all_restarting():
+                        raise eng.GastError('%s: the model\'s parameters or buffers changed since the tick was '
+                                            'captured (load_state_dict, an optimiser step or a training forward); the '
+                                            'streams\' history was computed with the old weights -- call reset() '
+                                            'before pushing again' % name)
+                    self.graph = None
+            if self.graph is None:
+                self._capture()
+            n, N, K, P = self.n, self.copies * self.n, self.K, self.P
+            fresh, hold, index = self.book.advance_many(K, streams=sel)
+            idx = np.full((n, K), -1, dtype=np.int64)
+            idx[sel] = index
+            mk = self._mask_host.numpy()
+            self._uploaded.synchronize()                       # the previous tick's copy has left the buffer
+            mk[:] = 0
+            mk[:N] = np.tile(np.isin(np.arange(n), sel[fresh]), self.copies)
+            mk[N:2 * N] = np.tile(np.isin(np.arange(n), sel), self.copies)
+            hk = mk[2 * N:].reshape(self.copies, n, K)
+            hk[:, sel] = hold
+            self._mask_dev.copy_(self._mask_host, non_blocking=True)
+            self._uploaded.record()
+            self._x.copy_(frames, non_blocking=True)
+            self.graph.replay()
+        self._advanced(sel, K)
+        self.last_launches = self._launches
+        out = (self._y, torch.from_numpy(idx))
+        if P:
+            pidx = np.full((n, P), -1, dtype=np.int64)
+            pidx[sel] = self.book.peek(P, streams=sel)
+            out += (self._py, torch.from_numpy(pidx))
+        return out
+
+
 def lift_sequences(model_pos, sequences, n_streams=64, chunk=256, augment=False, kps_left=None, kps_right=None,
                    joints_left=None, joints_right=None):
     """Whole-sequence lifting in bounded memory: sequences [(T_i, J, in_features)] -> [(T_i, J, 3) CUDA tensors],

@@ -322,6 +322,37 @@ int gast_stream_push_subset(gast_t* h, void* state, int32_t n_streams, const int
 int gast_stream_peek_subset(gast_t* h, const void* state, int32_t n_streams, const int32_t* streams,
                             const int64_t* steps, int32_t m, int32_t K, float* y, void* workspace,
                             size_t workspace_bytes, void* stream);
+/* gast_stream_push_device / gast_stream_peek_device: the subset entries with the frame counts kept on the device, so
+ *   that a CUDA graph can capture a tick and replay it at every later count.
+ *   counts (n_streams) int64 on the device: what `steps` is for the subset entries, the frames pushed into each stream
+ *   so far (held frames included).  active (n_streams) int32 on the device, or null (every stream active).  x
+ *   (n_streams, K, J, in_features), y (n_streams, K, J, 3), fresh (n_streams) and hold (n_streams, K) are on the
+ *   device, indexed by stream, null masks as for gast_stream_push_chunk.
+ *   A push returns in the rows of the active streams, and leaves in their bytes of `state`, exactly what
+ *   gast_stream_push_subset returns and leaves when it lists the active streams in ascending order at steps counts[s]
+ *   (bit for bit), and adds K to counts[s] of every active stream on the device.  An inactive stream's row of x is not
+ *   read, its bytes of `state` and its count are unchanged, and its rows of y are unspecified.  A peek returns what
+ *   gast_stream_peek_subset returns for the active streams with counts[s] >= 1 (1 <= K <= gast_stream_latency(h), so
+ *   not for a causal handle) and writes nothing to `state` or `counts`.
+ *   Device values cannot make a kernel address memory outside `state`, the workspace or the operands: a count of 0
+ *   makes its stream fresh (its ring is never read), a negative count is taken as 0 (a push then leaves it at K), and
+ *   counts up to 2^62 work.  The calls read no device data on the host, allocate nothing, do not synchronise and copy
+ *   nothing from host memory; every refusal (null handle, state, counts, x or y, n_streams < 1, K < 1, a peek's K
+ *   outside [1, latency], a dense, non-MODEL or unprepared handle, a workspace smaller than
+ *   gast_stream_device_workspace_bytes(h, n_streams, K)) comes before the first launch.  So a call made during stream
+ *   capture either fails at capture time or records a graph that is right at every replay, provided the handle sees
+ *   no gast_bind / gast_prepare in between (new weights: capture again) and gast_set_timing is off while capturing.
+ *   The launch count is that of the chunk or peek call plus one, whatever n_streams, K and the active set.
+ *   These entries mix freely with the subset entries on one state, as long as the host's steps equal the device
+ *   counts.  Test-time augmentation: 2n_streams library streams with counts, active and the masks repeated for both
+ *   halves, as for the subset entries. */
+size_t gast_stream_device_workspace_bytes(gast_t* h, int32_t n_streams, int32_t K);
+int gast_stream_push_device(gast_t* h, void* state, int32_t n_streams, int64_t* counts, const int32_t* active,
+                            int32_t K, const float* x, float* y, const int32_t* fresh, const int32_t* hold,
+                            void* workspace, size_t workspace_bytes, void* stream);
+int gast_stream_peek_device(gast_t* h, const void* state, int32_t n_streams, const int64_t* counts,
+                            const int32_t* active, int32_t K, float* y, void* workspace, size_t workspace_bytes,
+                            void* stream);
 
 /* ---- either side of the forward, on the device (SURVEY.md 8f N1-N3) --------------------------------
  * All pointers are device pointers unless marked (host).  Work is enqueued on `stream`.
