@@ -1188,14 +1188,16 @@ static int timed_reps(cudaStream_t st, int reps, float* ms_out, Launch launch) {
 // ------------------------------------------------------------------------------------------
 // debug / probe entry: out[M,N] = A[M,K] . W[N,K]^T on a chosen GEMM core (test infrastructure
 // for the numerics of the tensor-core path; not used by the forward).  tc_mode: the tensor-core core's precision
-// (0 fp32-grade as inference runs it, three fp16 products on scaled operands; 1 single-pass TF32).
+// (0 fp32-grade as inference runs it, three fp16 products on scaled operands; 1 single-pass TF32; 3 fp32-grade as
+// training runs it, three TF32 products).
 // ------------------------------------------------------------------------------------------
 extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32_t N, int32_t K,
                                int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (M <= 0 || N <= 0 || K <= 0 || N % 4 || K % 4) return fail("gast_debug_gemm: bad shape");
-  if (core < 0 || core > 1 || tc_mode < 0 || tc_mode > 1 || (core == 1 && tc_mode != 0))
-    return fail("gast_debug_gemm: core must be 0 (tensor cores, tc_mode 0 = fp32-grade or 1 = TF32) or 1 (FFMA, tc_mode 0)");
+  if (core < 0 || core > 1 || (tc_mode != 0 && tc_mode != 1 && tc_mode != 3) || (core == 1 && tc_mode != 0))
+    return fail("gast_debug_gemm: core must be 0 (tensor cores, tc_mode 0 = F16X3, 1 = TF32 or 3 = 3xTF32) or 1 (FFMA, "
+                "tc_mode 0)");
   GemmP p;
   gemm_flat(p, M);
   p.nseg = 1; p.seg[0] = seg_flat(A, K, K);
@@ -1204,7 +1206,7 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
   std::vector<void*> owned;
   TcWeights t;
   if (core == 0) {
-    rc = tc_prepare_weights(t, W, N, K, st, &owned, true);
+    rc = tc_prepare_weights(t, W, N, K, st, &owned, tc_mode != 3);   // 3xTF32 runs on training's tf32 copies
     if (rc || !t.ready || !tc_supported(p, EPI_PLAIN, t)) {
       for (void* q : owned) cudaFree(q);
       return fail("gast_debug_gemm: shape not supported by the tensor-core core (rc=%d)", rc);
@@ -1213,7 +1215,7 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
     cudaFuncSetAttribute((const void*)gemm_ffma_kernel<EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   }
   rc = timed_reps(st, reps, ms_out, [&]() -> int {
-    if (core == 0) return tc_launch(st, EPI_PLAIN, p, t, tc_prec(t, tc_mode));
+    if (core == 0) return tc_launch(st, EPI_PLAIN, p, t, tc_prec(t, tc_mode == 1));
     dim3 grid(cdiv(M, 128), cdiv(N, FF_BN));
     gemm_ffma_kernel<EPI_PLAIN><<<grid, FF_THREADS, ffma_smem_bytes(EPI_PLAIN, 1, 128, 1), st>>>(p);
     return (int)cudaGetLastError();

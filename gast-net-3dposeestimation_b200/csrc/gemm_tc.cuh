@@ -30,9 +30,10 @@
 // 32-wide K stages (tc_stages(PREC) slots of B_hi | B_lo | A, B_hi | A in 1xTF32):
 //   producer (warpgroup 0, 40 registers after setmaxnreg): waits for a slot's `empty` mbarrier, then fills it.
 //     B (weights): the hi and lo copies are stored [K/4][N][4] floats ([K/8][N][8] halves in F16X3,
-//                tc_prepare_weights), so one 3D TMA box per operand lands in the no-swizzle K-major core-matrix
+//                tc_prepare_weights), so one TMA box per operand lands in the no-swizzle K-major core-matrix
 //                layout wgmma reads from shared memory (8 rows x 16 B core matrices, 128 B apart along N, 2048 B
-//                apart along K); one elected thread issues the boxes.
+//                apart along K); the box is described as rows of 2 KB (a k-quad or k-octet of the tile's 128 n),
+//                not 16-byte rows, and one elected thread issues the boxes.
 //     A (activations): rows are gathered per frame (dilated / strided taps, residual slices, concatenations), so
 //                they arrive by cp.async (16 B per row and k-quad, zero-filled outside the tile) from all 128
 //                producer threads.  A stage never straddles a tap (Kc % 32 == 0), so segment, tap and column are
@@ -81,7 +82,7 @@ struct TcWeights {
 enum { TC_3XTF32 = 0, TC_1XTF32 = 1, TC_F16X3 = 2 };
 
 #ifndef GAST_TC1_STAGES
-#define GAST_TC1_STAGES 3                             // ring depth of the 1xTF32 form: 4 and 5 measured slower (DESIGN.md §4.1)
+#define GAST_TC1_STAGES 3                             // ring depth of the 1xTF32 form: 4 and 5 measured no faster (DESIGN.md §4.1)
 #endif
 #ifndef GAST_TC16_STAGES
 #define GAST_TC16_STAGES 3                            // ring depth of the F16X3 form: 4 and 5 measured no faster (DESIGN.md §4.1)
@@ -97,8 +98,8 @@ constexpr int TC_ALD16 = TC_KS + 8;                  // the same for F16X3's 64-
 constexpr int TC_B_BYTES = TC_BN * TC_KS * 4;        // one of B_hi / B_lo in a stage
 constexpr int TC_B16_BYTES = TC_BN * TC_KS * 2;      // the same in F16X3
 constexpr int TC_A_BYTES = TC_BM * TC_ALD * 4;
-// A row stride, B copy bytes, B copies per slot, slot size and ring depth of each precision.  3xTF32: a fourth slot
-// measured slower (DESIGN.md §4.1).
+// A row stride, B copy bytes, B copies per slot, slot size and ring depth of each precision.  3xTF32: a fourth 50 KB
+// slot does not fit in TC_SMEM_MAX beside the row table.
 __host__ __device__ constexpr int tc_ald(int prec) { return prec == TC_F16X3 ? TC_ALD16 : TC_ALD; }
 __host__ __device__ constexpr int tc_bbytes(int prec) { return prec == TC_F16X3 ? TC_B16_BYTES : TC_B_BYTES; }
 __host__ __device__ constexpr int tc_nb(int prec) { return prec == TC_1XTF32 ? 1 : 2; }
@@ -155,10 +156,10 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "WAIT_DONE:\n\t"
       "}" ::"r"(bar), "r"(parity) : "memory");
 }
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int x, int y, int z) {
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int x, int y) {
   asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(x), "r"(y), "r"(z) : "memory");
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(x), "r"(y) : "memory");
 }
 // 16 bytes global -> shared, zero-filled when src_bytes == 0
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
@@ -404,8 +405,8 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
       if (tid == 0) {
         mbar_arrive_expect_tx(full, NB * BBYTES);
         const int kq = (kcol + k0) >> KSH;
-        tma_load_3d(sb, &mhi, full, 0, n0, kq);
-        if (NB == 2) tma_load_3d(sb + BBYTES, &mlo, full, 0, n0, kq);
+        tma_load_2d(sb, &mhi, full, 2 * n0, kq);
+        if (NB == 2) tma_load_2d(sb + BBYTES, &mlo, full, 2 * n0, kq);
       }
       const ASeg& sg = p.seg[seg];
       const float* src = sg.base + tap * sg.tap_stride + kin + q * 4;
@@ -578,23 +579,25 @@ inline int tc_prepare_weights(TcWeights& t, const float* W, int N, int K, cudaSt
     t.lo = f16 ? nullptr : (float*)b;
     t.h16 = f16 ? (__half*)b : nullptr;
     t.sw = f16 ? (int*)(t.h16 + 2 * (size_t)N * K) : nullptr;
-    // dims {4 k's, N rows, K/4 k-quads}; box {4, 128, TC_KS/4}: rows past N read as zero
-    cuuint64_t dims[3] = {4, (cuuint64_t)N, (cuuint64_t)(K / 4)};
-    cuuint64_t strides[2] = {16, (cuuint64_t)N * 16};
-    cuuint32_t box[3] = {4, (cuuint32_t)TC_BN, (cuuint32_t)(TC_KS / 4)};
-    cuuint32_t estr[3] = {1, 1, 1};
+    // Each k-quad ([K/4][N][4] floats) or k-octet ([K/8][N][8] halves) row of a copy is N 16-byte pieces, contiguous,
+    // so a copy is described as 2D of 8-byte elements: dims {2N, K/4 or K/8}, box {256, TC_KS/4 or TC_KS/8}.  A box is
+    // then 8 (4) rows of 2 KB, the slot image of 128 n by 32 k, and the TMA engine issues 2 KB rows instead of
+    // 16-byte ones.  Elements past 2N (columns past N of a partial last column tile) read as zero.
+    cuuint64_t strides[1] = {(cuuint64_t)N * 16};
+    cuuint32_t estr[2] = {1, 1};
+    cuuint64_t dims[2] = {2 * (cuuint64_t)N, (cuuint64_t)(K / 4)};
+    cuuint32_t box[2] = {2 * (cuuint32_t)TC_BN, (cuuint32_t)(TC_KS / 4)};
     for (int m = 0; m < (f16 ? 1 : 2); ++m) {
-      CUresult r = enc(m ? &t.map_lo : &t.map_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, m ? t.lo : t.hi, dims, strides, box,
+      CUresult r = enc(m ? &t.map_lo : &t.map_hi, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, m ? t.lo : t.hi, dims, strides, box,
                        estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) { t.hi = nullptr; return -1; }
     }
     if (f16) {
-      // dims {8 k's, N rows, K/8 k-octets}; box {8, 128, TC_KS/8}: the same 16-byte rows as the fp32 copies
-      cuuint64_t d16[3] = {8, (cuuint64_t)N, (cuuint64_t)(K / 8)};
-      cuuint32_t b16[3] = {8, (cuuint32_t)TC_BN, (cuuint32_t)(TC_KS / 8)};
+      cuuint64_t d16[2] = {2 * (cuuint64_t)N, (cuuint64_t)(K / 8)};
+      cuuint32_t b16[2] = {2 * (cuuint32_t)TC_BN, (cuuint32_t)(TC_KS / 8)};
       for (int m = 0; m < 2; ++m) {
-        CUresult r = enc(m ? &t.map_h16lo : &t.map_h16hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, t.h16 + (size_t)m * N * K,
+        CUresult r = enc(m ? &t.map_h16lo : &t.map_h16hi, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, t.h16 + (size_t)m * N * K,
                          d16, strides, b16, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { t.hi = nullptr; return -1; }

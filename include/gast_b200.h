@@ -442,8 +442,9 @@ int gast_adam_step(const int64_t* table, int32_t n_chunks, float* exp_avg, float
                    double lr, double beta1, double beta2, double eps, double weight_decay, int64_t step, void* stream);
 
 /* Test/probe entry (not on the forward path): out[M,N] = A[M,K] . W[N,K]^T on one GEMM core
- * (core 0 = tensor cores, tc_mode 0 = fp32-grade as inference runs it, three scaled fp16 products, or
- * 1 = single-pass TF32; core 1 = FFMA, tc_mode 0).  Runs once, then `reps` timed launches
+ * (core 0 = tensor cores, tc_mode 0 = fp32-grade as inference runs it, three scaled fp16 products (F16X3),
+ * 1 = single-pass TF32, or 3 = fp32-grade as training runs it, three TF32 products (3xTF32); tc_mode 2 is not a
+ * mode and is refused; core 1 = FFMA, tc_mode 0).  Runs once, then `reps` timed launches
  * (CUDA events) whose mean duration is written to *ms_out (host).  Synchronises the stream. */
 int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32_t N, int32_t K,
                     int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream);
