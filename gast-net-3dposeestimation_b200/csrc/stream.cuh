@@ -214,6 +214,36 @@ __global__ void rotate_taps_kernel(float* __restrict__ dst, const float* __restr
   dst[idx] = src[nrow * K + (long long)j * Cw + c];
 }
 
+// ---- moving streams between states (gast_stream_export / gast_stream_import, below) ----
+// A stream's snapshot is its history in time order: [xhist (k0, J, F)][ring_1 (R_1, J, C_1)] ... [ring_{L-1}], each
+// part oldest first.  Part p is R_p rows of rowlen floats; row j of ring i of a stream at count c is its slot
+// (c - R_i + j) mod R_i = (c + j) mod R_i, so the snapshot does not depend on the ring phase and an import at another
+// count lands at that count's phase.  The input history is one row (it is kept in time order already).
+struct MovePart { long long state_off, slot_stride, stream_stride, snap_off; int R, rowlen; };
+struct MovePlan { MovePart part[GAST_MAX_STAGES]; int nparts; long long snap_floats; };
+
+// grid = (rows of one snapshot, listed streams in a grid-stride loop); tab (2m): row b is state stream tab[b] at phase
+// tab[m + b] (its count mod R_max, which every R_i divides).  kImport: snap (m, snap_floats) -> state, else the other
+// way.  Plain float copies: the input history row (k0 J F floats) and the snapshot's part offsets need not be
+// multiples of 4.
+template <bool kImport>
+__global__ void __launch_bounds__(256) stream_move_kernel(float* __restrict__ state, float* __restrict__ snap,
+                                                          const MovePlan p, const int32_t* __restrict__ tab, int m) {
+  int q = 0, j = blockIdx.x;
+  while (j >= p.part[q].R) j -= p.part[q++].R;            // snapshot row -> (part, time position)
+  const MovePart& g = p.part[q];
+  for (int b = blockIdx.y; b < m; b += gridDim.y) {
+    const int slot = q ? (tab[m + b] % g.R + j) % g.R : 0;
+    float* s = state + g.state_off + slot * g.slot_stride + tab[b] * g.stream_stride;
+    float* t = snap + b * p.snap_floats + g.snap_off + (long long)j * g.rowlen;
+#pragma unroll 4
+    for (int e = threadIdx.x; e < g.rowlen; e += blockDim.x) {
+      if (kImport) s[e] = t[e];
+      else t[e] = s[e];
+    }
+  }
+}
+
 }  // namespace gast
 
 struct StreamPlan {
@@ -636,4 +666,79 @@ extern "C" int gast_stream_peek_device(gast_t* h, const void* state, int32_t n_s
   // only read: the table kernel advances no count for a peek, and chunk_forward writes no ring back
   return chunk_call(who, h, const_cast<void*>(state), n_streams, nullptr, nullptr, const_cast<int64_t*>(counts), active,
                     0, n_streams, K, nullptr, y, nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
+// ---- moving streams between states: a gather to and a scatter from their time-ordered snapshots -----------------
+// The parts of a snapshot (stream_move_kernel) over the state layout of stream_plan.
+static MovePlan move_plan(const gast_handle* h, const StreamPlan& sp) {
+  const gast_cfg& c = h->cfg;
+  const int J = c.num_joints, xrow = c.filter_widths[0] * J * c.in_features;
+  MovePlan p{};
+  p.part[0] = MovePart{(long long)sp.xhist_off, 0, xrow, 0, 1, xrow};
+  long long off = xrow;
+  for (size_t i = 0; i < sp.R.size(); ++i) {
+    const int row = J * (c.channels << (i + 1)), R = sp.R[i];
+    p.part[i + 1] = MovePart{(long long)sp.ring_off[i], (long long)sp.n * row, row, off, R, row};
+    off += (long long)R * row;
+  }
+  p.nparts = (int)sp.R.size() + 1;
+  p.snap_floats = off;
+  return p;
+}
+
+extern "C" size_t gast_stream_snapshot_floats(gast_t* h) {
+  StreamPlan sp;
+  if (!h || stream_plan(h, 1, &sp)) return 0;
+  return (size_t)move_plan(h, sp).snap_floats;
+}
+
+extern "C" size_t gast_stream_move_workspace_bytes(gast_t* h, int32_t m) {
+  if (!h || stream_check(h) || m < 1) return 0;
+  Arena a{nullptr, 0, 0, true};
+  a.take((size_t)2 * m);                                   // the (stream, phase) table, 2 int32 per stream
+  return a.off + 256;
+}
+
+// Both directions: the subset entries' checks of streams and counts (counts >= 1), the table to the workspace in one
+// copy, then one stream_move_kernel launch.  Every refusal comes before the first launch.
+static int move_call(const char* who, bool import, gast_handle* h, void* state, int n_streams, const int32_t* streams,
+                     const int64_t* counts, int m, float* snap, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h) return fail("%s: null handle", who);
+  if (!streams || !counts) return fail("%s: null streams or counts", who);
+  if (!state || !snap) return fail("%s: bad arguments", who);
+  StreamPlan sp;
+  if (stream_plan(h, n_streams, &sp)) return 1;
+  std::vector<int32_t> tab;
+  bool lockstep;
+  if (subset_table(sp, streams, counts, m, 1, who, &tab, &lockstep)) return 1;
+  if (call_begin(h, who, gast_stream_move_workspace_bytes(h, m), workspace, workspace_bytes)) return 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const MovePlan p = move_plan(h, sp);
+  int32_t* dtab = reinterpret_cast<int32_t*>(workspace_arena(workspace, workspace_bytes).take((size_t)2 * m));
+  CUDA_OK(cudaMemcpyAsync(dtab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  int rows = 0;
+  for (int q = 0; q < p.nparts; ++q) rows += p.part[q].R;
+  const dim3 grid((unsigned)rows, (unsigned)std::min(m, 65535));
+  float* sbase = reinterpret_cast<float*>(align256(state));
+  if (import) stream_move_kernel<true><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
+  else stream_move_kernel<false><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
+  h->launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gast_stream_export(gast_t* h, const void* state, int32_t n_streams, const int32_t* streams,
+                                  const int64_t* counts, int32_t m, float* out, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  // only read: the export kernel writes the snapshot
+  return move_call("gast_stream_export", false, h, const_cast<void*>(state), n_streams, streams, counts, m, out,
+                   workspace, workspace_bytes, stream);
+}
+
+extern "C" int gast_stream_import(gast_t* h, void* state, int32_t n_streams, const int32_t* streams,
+                                  const int64_t* counts, int32_t m, const float* in, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  // only read: the import kernel reads the snapshot
+  return move_call("gast_stream_import", true, h, state, n_streams, streams, counts, m, const_cast<float*>(in),
+                   workspace, workspace_bytes, stream);
 }

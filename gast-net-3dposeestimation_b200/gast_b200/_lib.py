@@ -25,7 +25,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_stream_latency', 'gast_stream_push_ex', 'gast_stream_chunk_workspace_bytes', 'gast_stream_push_chunk',
            'gast_stream_peek', 'gast_stream_subset_workspace_bytes', 'gast_stream_push_subset', 'gast_stream_peek_subset',
            'gast_stream_device_workspace_bytes', 'gast_stream_push_device', 'gast_stream_peek_device',
-           'gast_chunk_gather', 'gast_keypoints_convert', 'gast_h36m_coco_format', 'gast_revise_kpts',
+           'gast_stream_snapshot_floats', 'gast_stream_move_workspace_bytes', 'gast_stream_export',
+           'gast_stream_import', 'gast_chunk_gather', 'gast_keypoints_convert', 'gast_h36m_coco_format', 'gast_revise_kpts',
            'gast_revise_skes_workspace_bytes', 'gast_revise_skes', 'gast_revise_skes_real_time_workspace_bytes',
            'gast_revise_skes_real_time', 'gast_normalize_screen', 'gast_camera_to_world',
            'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_adam_chunk', 'gast_adam_step',
@@ -143,6 +144,13 @@ def load():
     lib.gast_stream_push_device.restype = C.c_int
     lib.gast_stream_peek_device.argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, vp, vp, C.c_size_t, vp]
     lib.gast_stream_peek_device.restype = C.c_int
+    lib.gast_stream_snapshot_floats.argtypes = [vp]
+    lib.gast_stream_snapshot_floats.restype = C.c_size_t
+    lib.gast_stream_move_workspace_bytes.argtypes = [vp, C.c_int32]
+    lib.gast_stream_move_workspace_bytes.restype = C.c_size_t
+    for fn in ('gast_stream_export', 'gast_stream_import'):
+        getattr(lib, fn).argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, vp, vp, C.c_size_t, vp]
+        getattr(lib, fn).restype = C.c_int
     lib.gast_stream_latency.argtypes = [vp]
     lib.gast_stream_latency.restype = C.c_int32
     ip = C.POINTER(C.c_int32)

@@ -17,7 +17,9 @@ reference does (`tools/inference.py:19-110`).  The poses of a sequence then equa
 `UnchunkedGenerator([seq], pad, causal_shift, augment)` + `tools/inference.evaluate`.  Until then `peek()` returns
 provisional poses of the pending frames, those of the sequence cut at its newest frame, without changing any stream.
 `CausalStream` is the causal,
-un-augmented restriction that returns the pose of the newest frame.
+un-augmented restriction that returns the pose of the newest frame.  `export_streams` / `import_streams` move live
+streams with their history into another pool of the same model (another size, eager or graphed), where they continue
+as if they had never moved (`StreamSnapshot`, C ABI `gast_stream_export` / `gast_stream_import`).
 
 The rings hold activations computed with the weights of the pushes that wrote them.  Any change to the model's
 parameters or buffers (`load_state_dict`, an optimiser step, a training forward, which moves the BatchNorm running
@@ -81,6 +83,17 @@ class SequenceBook(object):
         out = fn(sub)
         self.fresh[s], self.length[s], self.left[s] = sub.fresh, sub.length, sub.left
         return out
+
+    def rows(self, streams):
+        """-> (fresh, length, left) of the listed streams, copies: their sequences, for `put_rows` of another book"""
+        s = self.check_streams(streams)
+        return self.fresh[s].copy(), self.length[s].copy(), self.left[s].copy()
+
+    def put_rows(self, streams, rows):
+        """the listed streams take the sequences `rows` (from `rows`): later calls treat them as the source book
+        treated its streams (a fresh or idle stream stays so, an ending one keeps its pending poses)"""
+        s = self.check_streams(streams)
+        self.fresh[s], self.length[s], self.left[s] = rows
 
     def reset(self, streams=None):
         s = self._sel(streams)
@@ -166,6 +179,27 @@ class SequenceBook(object):
         return book.advance_many(K)[2]
 
 
+class StreamSnapshot(object):
+    """Some streams of a `PoseStream` moved out by `export_streams`, for `import_streams` into a pool of the same
+    model (another n_streams, eager or graphed).
+
+    data (m, copies, floats) float32: per stream its library snapshot (`gast_stream_export`: the input history and
+    every ring in time order), copies = 2 with augment (the stream and its mirrored twin); fresh, length, left (m,):
+    the streams' SequenceBook rows; counts (m,): their frame counts in the source pool.  The rest names what the
+    history belongs to: arch (J, F, channels, filter widths, causal, latency), augment and the symmetry lists, the
+    model object, the parameter signature of the weights that computed the history, and the device.  `to(device)`
+    moves `data` only (e.g. to host memory and back); a snapshot is valid within the process that made it."""
+
+    def __init__(self, data, fresh, length, left, counts, arch, augment, lists, model, sig, device):
+        self.data, self.fresh, self.length, self.left, self.counts = data, fresh, length, left, counts
+        self.arch, self.augment, self.lists, self.model, self.sig, self.device = arch, augment, lists, model, sig, device
+
+    def to(self, device):
+        c = copy.copy(self)
+        c.data = self.data.to(device)
+        return c
+
+
 class PoseStream(object):
     """O(1)-per-frame lifting of `n_streams` concurrent streams with any non-dense model of the drop-in classes
     (`SpatioTemporalModel` or `SpatioTemporalModelOptimized1f`, causal or not: the weights are interchangeable).
@@ -237,6 +271,10 @@ class PoseStream(object):
         streams=None once the counts differ)"""
         if streams is None:
             return np.arange(self.n, dtype=np.int64) if self._delta.any() else None
+        return self._listed(streams)
+
+    def _listed(self, streams):
+        """-> streams as int64 indices; GastError unless they are 1 to n distinct indices in [0, n)"""
         try:
             return self.book.check_streams(streams)
         except ValueError as e:
@@ -422,6 +460,105 @@ class PoseStream(object):
         self.last_launches = launches
         return y, torch.from_numpy(index)
 
+    # ---- moving streams between pools -------------------------------------------------------------------------------
+    def _arch(self):
+        m = self.model
+        return (self.J, self.F, int(m._gast_channels), tuple(int(w) for w in m.filter_widths), self.causal,
+                self.latency)
+
+    def _lists(self):
+        return (self.kps_left, self.kps_right, self.joints_left, self.joints_right) if self.augment else None
+
+    def _move_begin(self):
+        """-> the refreshed handle, with the state allocated; refuses over history computed with other weights"""
+        h = self.engine.model_handle(self.model, self.device)
+        self._begin(h, torch.cuda.current_stream(self.device).cuda_stream)
+        return h
+
+    def _move(self, fn, h, sel, counts, data):
+        """gast_stream_export / _import of data (m, copies, floats) for the streams sel at their counts: library
+        streams [s, s + n] per stream with augment, so that the rows of data are (stream, copy)"""
+        lib = h.lib
+        lib_streams = (sel[:, None] + self.n * np.arange(self.copies)[None, :]).reshape(-1).astype(np.int32)
+        lib_counts = np.repeat(np.asarray(counts, dtype=np.int64), self.copies)
+        mm = lib_streams.size
+        wb = lib.gast_stream_move_workspace_bytes(h.h, mm)
+        if wb == 0:
+            raise self.engine.GastError('gast_stream_move_workspace_bytes: %s' % L.last_error())
+        # not self._ws: a GraphedPoseStream's graph keeps that buffer's address
+        ws = torch.empty(int(wb), dtype=torch.uint8, device=self.device)
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        if getattr(lib, fn)(h.h, self._state.data_ptr(), self.copies * self.n, lib_streams.ctypes.data,
+                            lib_counts.ctypes.data, mm, data.data_ptr(), ws.data_ptr(), ws.numel(), st) != 0:
+            raise self.engine.GastError('%s: %s' % (fn, L.last_error()))
+        self.last_launches = int(lib.gast_last_launch_count(h.h))
+
+    def export_streams(self, streams):
+        """-> StreamSnapshot of the listed streams (distinct indices): their history on the device, their sequence
+        bookkeeping and counts, for `import_streams` of a pool of the same model and architecture (any n_streams,
+        eager or graphed).  Nothing changes in this pool.  Refused (GastError) like a push when the model's parameters
+        or buffers changed since the last push and not every stream is restarting."""
+        sel = self._listed(streams)
+        with torch.cuda.device(self.device):
+            h = self._move_begin()
+            nf = int(h.lib.gast_stream_snapshot_floats(h.h))
+            if nf == 0:
+                raise self.engine.GastError('gast_stream_snapshot_floats: %s' % L.last_error())
+            data = torch.empty((sel.size, self.copies, nf), dtype=torch.float32, device=self.device)
+            # a stream that never pushed is fresh or idle: its rows are never read, any count >= 1 will do
+            self._move('gast_stream_export', h, sel, np.maximum(self.counts[sel], 1), data)
+        return StreamSnapshot(data, *self.book.rows(sel), self.counts[sel].copy(), self._arch(), self.augment,
+                              self._lists(), self.model, h.sig, self.device)
+
+    def import_streams(self, snapshot, streams):
+        """Overwrite the listed streams (distinct indices, one per exported stream, in the snapshot's order) with the
+        exported streams: their history, their sequences (a fresh or idle stream stays so, an ending one keeps its
+        pending poses) and the same poses from then on.  Each takes the count max(step, 1), the phase of this pool's
+        lockstep calls.  The other streams are untouched.  Refused with GastError, changing nothing in either pool: a
+        snapshot of another model object, architecture, `augment` or symmetry lists or device, a change of the
+        model's parameters or buffers since the export (unless every exported stream is restarting), this pool's own
+        weight-change rule, bad or duplicate streams, or a count that differs from the snapshot's."""
+        eng, name = self.engine, type(self).__name__
+        sel = self._listed(streams)
+        if not isinstance(snapshot, StreamSnapshot):
+            raise eng.GastError('%s.import_streams needs a StreamSnapshot from export_streams' % name)
+        s = snapshot
+        if sel.size != s.counts.size:
+            raise eng.GastError('%s.import_streams: %d streams listed for a snapshot of %d' % (name, sel.size,
+                                                                                              s.counts.size))
+        if s.arch != self._arch() or s.augment != self.augment or s.lists != self._lists() or s.device != self.device:
+            raise eng.GastError('%s.import_streams: the snapshot\'s architecture, augment, symmetry lists or device '
+                                'differ from this pool\'s' % name)
+        if s.model is not self.model:
+            raise eng.GastError('%s.import_streams: the snapshot was exported from a pool of another model object'
+                                % name)
+        restarting = bool(np.all(s.fresh | (s.left == 0)))
+        if not restarting and self._model_sig() != s.sig:
+            raise eng.GastError('%s.import_streams: the model\'s parameters or buffers changed since the export; the '
+                                'exported history was computed with the old weights' % name)
+        if tuple(s.data.shape[:2]) != (sel.size, self.copies):
+            raise eng.GastError('%s.import_streams: snapshot data of shape %s' % (name, tuple(s.data.shape)))
+        target = max(self.step, 1)
+        with torch.cuda.device(self.device):
+            h = self._move_begin()
+            if s.data.shape[2] != h.lib.gast_stream_snapshot_floats(h.h):
+                raise eng.GastError('%s.import_streams: snapshot data of shape %s' % (name, tuple(s.data.shape)))
+            data = s.data.to(device=self.device, dtype=torch.float32).contiguous()
+            self._move('gast_stream_import', h, sel, np.full(sel.size, target), data)
+            self._moved_in(sel, target)
+        self._sig = h.sig
+        self.book.put_rows(sel, (s.fresh, s.length, s.left))
+        counts = self.counts
+        counts[sel] = target
+        self.step = int(counts.min())
+        self._delta = counts - self.step
+
+    def _model_sig(self):
+        return tuple((v.data_ptr(), v._version) for _, v in self.engine.named_tensors(self.model))
+
+    def _moved_in(self, sel, count):
+        """device bookkeeping of streams imported at `count` (none here: the counts are the host's)"""
+
 
 class CausalStream(PoseStream):
     """O(1)-per-frame lifting of `n_streams` concurrent streams with a causal model of the drop-in classes
@@ -586,6 +723,35 @@ class GraphedPoseStream(PoseStream):
             launches = self._tick(h, torch.cuda.current_stream(self.device).cuda_stream)
         self.graph, self._h, self._sig, self._mode, self._launches = graph, h, h.sig, self._mode_now(), launches
 
+    def _ready(self):
+        """refuse a tick over another GEMM core or precision, or over history computed with other weights; capture
+        the tick when there is no graph yet, or again after a weight change with every stream restarting"""
+        eng, name = self.engine, type(self).__name__
+        if self.graph is not None:
+            if self._mode_now() != self._mode:
+                raise eng.GastError('%s: engine.set_precision or engine.set_gemm_core changed since the tick was '
+                                    'captured; construct a new %s' % (name, name))
+            sig = self._model_sig()
+            if sig != self._sig or self._h.sig != self._sig:
+                if not self.book.all_restarting():
+                    raise eng.GastError('%s: the model\'s parameters or buffers changed since the tick was '
+                                        'captured (load_state_dict, an optimiser step or a training forward); the '
+                                        'streams\' history was computed with the old weights -- call reset() '
+                                        'before pushing again' % name)
+                self.graph = None
+        if self.graph is None:
+            self._capture()
+
+    def _move_begin(self):
+        self._ready()
+        return self._h
+
+    def _moved_in(self, sel, count):
+        """the device counts of both library halves of the imported streams, ordered before the next replay on the
+        current stream (the graph keeps the state and workspace addresses: no capture again)"""
+        rows = (sel[:, None] + self.n * np.arange(self.copies)[None, :]).reshape(-1)
+        self._counts_dev[torch.from_numpy(rows).to(self.device)] = int(count)
+
     def push(self, frames, streams=None):
         eng, name = self.engine, type(self).__name__
         if self.model.training:
@@ -594,20 +760,7 @@ class GraphedPoseStream(PoseStream):
         frames = torch.as_tensor(frames, dtype=torch.float32)
         assert tuple(frames.shape) == tuple(self._x.shape), frames.shape
         with torch.cuda.device(self.device):
-            if self.graph is not None:
-                if self._mode_now() != self._mode:
-                    raise eng.GastError('%s: engine.set_precision or engine.set_gemm_core changed since the tick was '
-                                        'captured; construct a new %s' % (name, name))
-                sig = tuple((v.data_ptr(), v._version) for _, v in eng.named_tensors(self.model))
-                if sig != self._sig or self._h.sig != self._sig:
-                    if not self.book.all_restarting():
-                        raise eng.GastError('%s: the model\'s parameters or buffers changed since the tick was '
-                                            'captured (load_state_dict, an optimiser step or a training forward); the '
-                                            'streams\' history was computed with the old weights -- call reset() '
-                                            'before pushing again' % name)
-                    self.graph = None
-            if self.graph is None:
-                self._capture()
+            self._ready()
             n, N, K, P = self.n, self.copies * self.n, self.K, self.P
             fresh, hold, index = self.book.advance_many(K, streams=sel)
             idx = np.full((n, K), -1, dtype=np.int64)

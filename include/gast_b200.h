@@ -353,6 +353,33 @@ int gast_stream_push_device(gast_t* h, void* state, int32_t n_streams, int64_t* 
 int gast_stream_peek_device(gast_t* h, const void* state, int32_t n_streams, const int64_t* counts,
                             const int32_t* active, int32_t K, float* y, void* workspace, size_t workspace_bytes,
                             void* stream);
+/* gast_stream_export / gast_stream_import: move streams between states with their history, e.g. into a state of
+ *   another n_streams, or between a state driven by the host counts and one driven by device counts.
+ *   A stream's SNAPSHOT is its history in time order, gast_stream_snapshot_floats(h) floats:
+ *     [input history (k0, J, in_features), oldest first][ring_1 (R_1, J, C_1), oldest first] ... [ring_{L-1}]
+ *   with k0 = filter_widths[0], C_i = channels << i, R_i = filter_widths[i] * (filter_widths[0] * ... *
+ *   filter_widths[i-1]).  Row j of ring i of a stream whose count is c is its slot (c - R_i + j) mod R_i, so a
+ *   snapshot does not depend on the ring phase.
+ *   gast_stream_export writes out (m, snapshot_floats) (device) = the snapshots of streams streams[0..m) at their
+ *   counts counts[0..m); `state` is only read.  gast_stream_import writes snapshot in[i] to stream streams[i] at the
+ *   target count counts[i] (so it may land at any phase, e.g. at the target state's lockstep step) and writes no
+ *   byte of an unlisted stream.  A stream imported at count c' then continues exactly as the exported stream did at
+ *   count c, the same for every later push, peek and subset call at counts c' + k (the chunk path reads the rings in
+ *   time order; a single-frame lockstep push is bitwise the same when c' = c mod R_max, and equal up to float rounding
+ *   otherwise, as the tap-rotated weights differ).  Both need a handle of the architecture that wrote the state
+ *   (gast_stream_state_bytes sizes) and no gast_prepare; the history stays that of the weights of the pushes that
+ *   wrote it (gast_stream_push's weight-change rule).
+ *   streams and counts are host arrays, checked as for gast_stream_push_subset: m in [1, n_streams], streams
+ *   distinct and in [0, n_streams), counts >= 1.  Every refusal comes before the first launch.  The workspace is
+ *   gast_stream_move_workspace_bytes(h, m) bytes (0 for bad arguments).  Each call is one table copy and one kernel
+ *   launch, whatever n_streams, m and the depth of the model.
+ *   Test-time augmentation: a stream is two library streams, s and s + n_streams of the 2n-stream state. */
+size_t gast_stream_snapshot_floats(gast_t* h);
+size_t gast_stream_move_workspace_bytes(gast_t* h, int32_t m);
+int gast_stream_export(gast_t* h, const void* state, int32_t n_streams, const int32_t* streams, const int64_t* counts,
+                       int32_t m, float* out, void* workspace, size_t workspace_bytes, void* stream);
+int gast_stream_import(gast_t* h, void* state, int32_t n_streams, const int32_t* streams, const int64_t* counts,
+                       int32_t m, const float* in, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- either side of the forward, on the device (SURVEY.md 8f N1-N3) --------------------------------
  * All pointers are device pointers unless marked (host).  Work is enqueued on `stream`.
