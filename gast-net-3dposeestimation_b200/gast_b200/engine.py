@@ -82,6 +82,13 @@ def _check(rc, what):
         raise GastError('%s: %s' % (what, L.last_error()))
 
 
+def _check_size(n, what):
+    """-> n, the result of a size entry (`*_bytes`, `*_floats`), as an int; 0 is that entry's refusal"""
+    if n == 0:
+        raise GastError('%s: %s' % (what, L.last_error()))
+    return int(n)
+
+
 def _mask_lists(m):
     idx = m.nonzero()        # row-major order == order of `e` (local_attention.py:25,41)
     rows = (C.c_int32 * len(idx))(*[int(i) for i in idx[:, 0]])
@@ -120,6 +127,12 @@ def named_params(module, buffers=False):
                 if v is not None and k not in mod._non_persistent_buffers_set:
                     out.append((pre + k, v))
     return out
+
+
+def param_sig(module):
+    """the (data_ptr, _version) signature of the module's parameters and buffers (named_tensors): it changes whenever
+    one of them is replaced or written in place"""
+    return tuple((v.data_ptr(), v._version) for _, v in named_tensors(module))
 
 
 class _HandleStore(dict):
@@ -192,12 +205,11 @@ class _Handle(object):
 
     def refresh(self, module, stream):
         """(re)bind + prepare when any parameter/buffer moved or changed."""
-        items = named_tensors(module)
-        sig = tuple((v.data_ptr(), v._version) for _, v in items)
+        sig = param_sig(module)
         self.apply_core(module)
         if sig == self.sig:
             return
-        _bind(self, 'gast_bind', items)
+        _bind(self, 'gast_bind', named_tensors(module))
         _check(self.lib.gast_prepare(self.h, C.c_void_p(stream)), 'gast_prepare')
         self.sig = sig
 
@@ -209,12 +221,10 @@ class _Handle(object):
 
     def forward(self, x, y, B, T, strided_now, stream, target=None, loss=None):
         """gast_forward, or with a target gast_forward_mpjpe, on the handle's grow-only workspace self.ws"""
-        need = self.lib.gast_workspace_bytes(self.h, B, T, strided_now)
-        if need == 0:
-            raise GastError('gast_workspace_bytes: %s' % L.last_error())
+        need = _check_size(self.lib.gast_workspace_bytes(self.h, B, T, strided_now), 'gast_workspace_bytes')
         if self.ws is None or self.ws.numel() < need:
             self.ws = None
-            self.ws = torch.empty(int(need), dtype=torch.uint8, device=self.device)
+            self.ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         tail = (B, T, strided_now, _p(self.ws), self.ws.numel(), C.c_void_p(stream))
         if target is None:
             _check(self.lib.gast_forward(self.h, _p(x), _p(y), *tail), 'gast_forward')
@@ -296,10 +306,9 @@ class _TrainFn(torch.autograd.Function):
         with torch.cuda.device(dev):
             st = _stream(dev)
             handle.bind_only(module)
-            need = lib.gast_train_workspace_bytes(handle.h, B, T, C.c_float(float(module._gast_dropout)))
-            if need == 0:
-                raise GastError('gast_train_workspace_bytes: %s' % L.last_error())
-            ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
+            need = _check_size(lib.gast_train_workspace_bytes(handle.h, B, T, C.c_float(float(module._gast_dropout))),
+                               'gast_train_workspace_bytes')
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
             y = _new_output(module, handle, B, T, 1 if module._gast_strided else 0, dev)
             p = float(module._gast_dropout)
             seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if p > 0 else 0
@@ -392,10 +401,9 @@ class _EvalFn(torch.autograd.Function):
             st = _stream(dev)
             h.refresh(module, st)            # binds the current storage and GEMM-core choice (no work when unchanged)
             lib = h.lib
-            need = lib.gast_eval_backward_workspace_bytes(h.h, B, T, ctx.sn)
-            if need == 0:
-                raise GastError('gast_eval_backward_workspace_bytes: %s' % L.last_error())
-            ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
+            need = _check_size(lib.gast_eval_backward_workspace_bytes(h.h, B, T, ctx.sn),
+                               'gast_eval_backward_workspace_bytes')
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
             dx = torch.empty_like(x) if need_x else None
             views = _bind_grad_views(h, ctx.names, params, False, dev) if need_p else None
             _check(lib.gast_eval_backward(h.h, _p(x), _p(dy), _p(dx), 1 if need_p else 0, B, T, ctx.sn, _p(ws),

@@ -35,8 +35,6 @@ import ctypes as C
 import numpy as np
 import torch
 
-from . import _lib as L
-
 # left/right keypoint and joint lists of the reference's inference helpers (tools/inference.py:14-15) and of
 # reconstruction.py:get_joints_info for 19 joints (reconstruction.py:185 uses the same lists for the keypoints)
 SYMMETRY = {
@@ -280,13 +278,22 @@ class PoseStream(object):
         except ValueError as e:
             raise self.engine.GastError('%s: %s' % (type(self).__name__, e))
 
+    def _set_counts(self, counts):
+        """counts (n,) int64 become the streams' frame counts, with `step` kept at the smallest count"""
+        self.step = int(counts.min())
+        self._delta = counts - self.step
+
     def _advanced(self, sel, K):
-        """the listed streams pushed K frames: counts[sel] += K, with `step` kept at the smallest count"""
-        delta = self._delta.copy()
-        delta[sel] += K
-        low = int(delta.min())
-        self.step += low
-        self._delta = delta - low
+        """the listed streams pushed K frames: counts[sel] += K"""
+        counts = self.counts
+        counts[sel] += K
+        self._set_counts(counts)
+
+    def _lib_streams(self, sel):
+        """-> (copies, m) int64: the library streams of the pool streams sel (m,), the streams themselves and with
+        augment their mirrored twins s + n.  Calls, their masks and the device counts list them copy-major (this
+        array flattened); a snapshot's rows are stream-major (its transpose)."""
+        return np.asarray(sel, dtype=np.int64)[None, :] + self.n * np.arange(self.copies)[:, None]
 
     def reset(self, streams=None):
         """Start new sequences on all (or the listed) streams with the next pushed frame; drop any pending tail."""
@@ -298,9 +305,9 @@ class PoseStream(object):
         self.book.end(streams)
 
     def _upload(self, fresh, hold):
-        """-> device pointers of the fresh (m,) and hold (m, K) masks of a push, repeated for the mirrored half (None
-        where no stream is set).  Every push reuses one buffer [fresh | hold]: the copy into it and the kernels that
-        read it are ordered on the one stream the calls run on."""
+        """-> device pointers of the fresh (m,) and hold (m, K) masks of a push, repeated for the mirrored half in the
+        copy-major order of `_lib_streams` (None where no stream is set).  Every push reuses one buffer [fresh | hold]:
+        the copy into it and the kernels that read it are ordered on the one stream the calls run on."""
         any_f, any_h = bool(fresh.any()), bool(hold.any())
         if not (any_f or any_h):
             return None, None
@@ -315,20 +322,37 @@ class PoseStream(object):
 
     def _begin(self, h, st):
         """refresh the handle, refuse a push over history computed with other weights, allocate the state"""
-        eng, lib = self.engine, h.lib
         h.refresh(self.model, st)
-        if self._sig is not None and h.sig != self._sig and not self.book.all_restarting():
-            raise eng.GastError('%s: the model\'s parameters or buffers changed since the last push '
-                                '(load_state_dict, an optimiser step or a training forward); the streams\' history '
-                                'was computed with the old weights -- call reset() before pushing again'
-                                % type(self).__name__)
+        self._refuse_stale(self._sig, h.sig)
+        self._alloc_state(h)
+
+    def _refuse_stale(self, sig, now):
+        """GastError unless a call may read the history that the weights of parameter signature `sig` computed (None:
+        nothing pushed yet) when the weights are now those of `now`: the same weights, or every stream restarting"""
+        if sig is not None and sig != now and not self.book.all_restarting():
+            raise self.engine.GastError('%s: the model\'s parameters or buffers changed since the streams\' history '
+                                        'was computed (load_state_dict, an optimiser step or a training forward) -- '
+                                        'call reset() before pushing again' % type(self).__name__)
+
+    def _alloc_state(self, h):
+        """allocate the zeroed library state of the copies * n library streams on first use, after checking that the
+        library's latency is the pool's"""
         if self._state is None:
-            if lib.gast_stream_latency(h.h) != self.latency:
-                raise eng.GastError('gast_stream_latency: %s' % L.last_error())
-            nb = lib.gast_stream_state_bytes(h.h, self.copies * self.n)
-            if nb == 0:
-                raise eng.GastError('gast_stream_state_bytes: %s' % L.last_error())
-            self._state = torch.empty(int(nb), dtype=torch.uint8, device=self.device)
+            eng, lib = self.engine, h.lib
+            eng._check(lib.gast_stream_latency(h.h) != self.latency, 'gast_stream_latency')
+            nb = eng._check_size(lib.gast_stream_state_bytes(h.h, self.copies * self.n), 'gast_stream_state_bytes')
+            self._state = torch.zeros(nb, dtype=torch.uint8, device=self.device)
+
+    def _mirror(self, lib, x, x2, rows, st):
+        """x2 (2, rows, J, F) = [x | x mirrored]: the library input of the twins of x (rows, J, F) (gast_tta_prepare)"""
+        self.engine._check(lib.gast_tta_prepare(x.data_ptr(), x2.data_ptr(), rows, self.J, self.F, 0, 0,
+                                                len(self.kps_left), self._kl, self._kr, st), 'gast_tta_prepare')
+
+    def _merge(self, lib, y2, y, rows, st):
+        """y (rows, J, 3) = the mean of the twins' poses y2 (2, rows, J, 3), the mirrored one un-mirrored
+        (gast_tta_merge)"""
+        self.engine._check(lib.gast_tta_merge(y2.data_ptr(), y.data_ptr(), rows, self.J, len(self.joints_left),
+                                              self._jl, self._jr, st), 'gast_tta_merge')
 
     def push(self, frame, streams=None):
         """frame (n_streams, J, in_features): the newest 2D keypoints of every stream (normalised screen
@@ -412,11 +436,10 @@ class PoseStream(object):
                 fn, wb = 'gast_stream_workspace_bytes', lib.gast_stream_workspace_bytes(h.h, mm)
             else:
                 fn, wb = 'gast_stream_subset_workspace_bytes', lib.gast_stream_subset_workspace_bytes(h.h, mm, K)
-            if wb == 0:
-                raise eng.GastError('%s: %s' % (fn, L.last_error()))
+            wb = eng._check_size(wb, fn)
             if self._ws is None or self._ws.numel() < wb:
                 self._ws = None
-                self._ws = torch.empty(int(wb), dtype=torch.uint8, device=self.device)
+                self._ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
             fresh_p = hold_p = None
             if frames is not None:
                 fresh, hold, index = self.book.advance_many(K, valid, streams=sel)
@@ -427,30 +450,24 @@ class PoseStream(object):
                 if frames is not None:
                     # (2, m, K, J, F) = 2m library streams of K frames: [original | mirrored]
                     x = torch.empty((2,) + tuple(frames.shape), dtype=torch.float32, device=self.device)
-                    if lib.gast_tta_prepare(frames.data_ptr(), x.data_ptr(), r * K, self.J, self.F, 0, 0,
-                                            len(self.kps_left), self._kl, self._kr, st) != 0:
-                        raise eng.GastError('gast_tta_prepare: %s' % L.last_error())
+                    self._mirror(lib, frames, x, r * K, st)
                 out = torch.empty((2, r, K, self.J, 3), dtype=torch.float32, device=self.device)
             state = self._state.data_ptr()
             if single:
                 fn, args = 'gast_stream_push_ex', (state, C.c_int64(self.step), x.data_ptr(), out.data_ptr(), mm,
                                                    fresh_p, hold_p)
             else:
-                # library streams [rows | rows + n] with augment, at their counts
-                lib_streams = np.concatenate([rows[keep] + c * self.n for c in range(self.copies)]).astype(np.int32)
+                lib_streams = self._lib_streams(rows[keep]).reshape(-1).astype(np.int32)
                 lib_steps = np.tile(self.counts[rows[keep]], self.copies).astype(np.int64)
                 table = (state, self.copies * self.n, lib_streams.ctypes.data, lib_steps.ctypes.data, mm, K)
                 if frames is None:
                     fn, args = 'gast_stream_peek_subset', table + (out.data_ptr(),)
                 else:
                     fn, args = 'gast_stream_push_subset', table + (x.data_ptr(), out.data_ptr(), fresh_p, hold_p)
-            if getattr(lib, fn)(h.h, *args, self._ws.data_ptr(), self._ws.numel(), st) != 0:
-                raise eng.GastError('%s: %s' % (fn, L.last_error()))
+            eng._check(getattr(lib, fn)(h.h, *args, self._ws.data_ptr(), self._ws.numel(), st), fn)
             launches = int(lib.gast_last_launch_count(h.h))
             if self.augment:
-                if lib.gast_tta_merge(out.data_ptr(), yr.data_ptr(), r * K, self.J, len(self.joints_left), self._jl,
-                                      self._jr, st) != 0:
-                    raise eng.GastError('gast_tta_merge: %s' % L.last_error())
+                self._merge(lib, out, yr, r * K, st)
                 launches += 2
             if r < rows.size:
                 y[torch.from_numpy(np.flatnonzero(keep)).to(self.device)] = yr
@@ -476,21 +493,18 @@ class PoseStream(object):
         return h
 
     def _move(self, fn, h, sel, counts, data):
-        """gast_stream_export / _import of data (m, copies, floats) for the streams sel at their counts: library
-        streams [s, s + n] per stream with augment, so that the rows of data are (stream, copy)"""
-        lib = h.lib
-        lib_streams = (sel[:, None] + self.n * np.arange(self.copies)[None, :]).reshape(-1).astype(np.int32)
+        """gast_stream_export / _import of data (m, copies, floats) for the streams sel at their counts: the library
+        streams listed stream-major, so that the rows of data are (stream, copy)"""
+        eng, lib = self.engine, h.lib
+        lib_streams = self._lib_streams(sel).T.reshape(-1).astype(np.int32)
         lib_counts = np.repeat(np.asarray(counts, dtype=np.int64), self.copies)
         mm = lib_streams.size
-        wb = lib.gast_stream_move_workspace_bytes(h.h, mm)
-        if wb == 0:
-            raise self.engine.GastError('gast_stream_move_workspace_bytes: %s' % L.last_error())
+        wb = eng._check_size(lib.gast_stream_move_workspace_bytes(h.h, mm), 'gast_stream_move_workspace_bytes')
         # not self._ws: a GraphedPoseStream's graph keeps that buffer's address
-        ws = torch.empty(int(wb), dtype=torch.uint8, device=self.device)
+        ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
         st = torch.cuda.current_stream(self.device).cuda_stream
-        if getattr(lib, fn)(h.h, self._state.data_ptr(), self.copies * self.n, lib_streams.ctypes.data,
-                            lib_counts.ctypes.data, mm, data.data_ptr(), ws.data_ptr(), ws.numel(), st) != 0:
-            raise self.engine.GastError('%s: %s' % (fn, L.last_error()))
+        eng._check(getattr(lib, fn)(h.h, self._state.data_ptr(), self.copies * self.n, lib_streams.ctypes.data,
+                                    lib_counts.ctypes.data, mm, data.data_ptr(), ws.data_ptr(), ws.numel(), st), fn)
         self.last_launches = int(lib.gast_last_launch_count(h.h))
 
     def export_streams(self, streams):
@@ -501,9 +515,7 @@ class PoseStream(object):
         sel = self._listed(streams)
         with torch.cuda.device(self.device):
             h = self._move_begin()
-            nf = int(h.lib.gast_stream_snapshot_floats(h.h))
-            if nf == 0:
-                raise self.engine.GastError('gast_stream_snapshot_floats: %s' % L.last_error())
+            nf = self.engine._check_size(h.lib.gast_stream_snapshot_floats(h.h), 'gast_stream_snapshot_floats')
             data = torch.empty((sel.size, self.copies, nf), dtype=torch.float32, device=self.device)
             # a stream that never pushed is fresh or idle: its rows are never read, any count >= 1 will do
             self._move('gast_stream_export', h, sel, np.maximum(self.counts[sel], 1), data)
@@ -533,7 +545,7 @@ class PoseStream(object):
             raise eng.GastError('%s.import_streams: the snapshot was exported from a pool of another model object'
                                 % name)
         restarting = bool(np.all(s.fresh | (s.left == 0)))
-        if not restarting and self._model_sig() != s.sig:
+        if not restarting and eng.param_sig(self.model) != s.sig:
             raise eng.GastError('%s.import_streams: the model\'s parameters or buffers changed since the export; the '
                                 'exported history was computed with the old weights' % name)
         if tuple(s.data.shape[:2]) != (sel.size, self.copies):
@@ -550,11 +562,7 @@ class PoseStream(object):
         self.book.put_rows(sel, (s.fresh, s.length, s.left))
         counts = self.counts
         counts[sel] = target
-        self.step = int(counts.min())
-        self._delta = counts - self.step
-
-    def _model_sig(self):
-        return tuple((v.data_ptr(), v._version) for _, v in self.engine.named_tensors(self.model))
+        self._set_counts(counts)
 
     def _moved_in(self, sel, count):
         """device bookkeeping of streams imported at `count` (none here: the counts are the host's)"""
@@ -655,37 +663,29 @@ class GraphedPoseStream(PoseStream):
     def _tick(self, h, st):
         """enqueue one tick's library calls on stream `st` -> their launch count"""
         eng, lib = self.engine, h.lib
-        n, N, K, P, J = self.n, self.copies * self.n, self.K, self.P, self.J
+        n, N, K, P = self.n, self.copies * self.n, self.K, self.P
         ws, wn = self._ws.data_ptr(), self._ws.numel()
         fresh, active, hold = [t.data_ptr() for t in (self._mask_dev[:N], self._mask_dev[N:2 * N],
                                                       self._mask_dev[2 * N:])]
         state, counts = self._state.data_ptr(), self._counts_dev.data_ptr()
-
-        def check(rc, fn):
-            if rc != 0:
-                raise eng.GastError('%s: %s' % (fn, L.last_error()))
-
         x, y, py = self._x, self._y, self._py
         launches = 0
         if self.augment:
-            check(lib.gast_tta_prepare(x.data_ptr(), self._x2.data_ptr(), n * K, J, self.F, 0, 0, len(self.kps_left),
-                                       self._kl, self._kr, st), 'gast_tta_prepare')
+            self._mirror(lib, x, self._x2, n * K, st)
             x, y, py = self._x2, self._y2, self._py2
             launches += 1
-        check(lib.gast_stream_push_device(h.h, state, N, counts, active, K, x.data_ptr(), y.data_ptr(), fresh, hold,
-                                          ws, wn, st), 'gast_stream_push_device')
+        eng._check(lib.gast_stream_push_device(h.h, state, N, counts, active, K, x.data_ptr(), y.data_ptr(), fresh,
+                                               hold, ws, wn, st), 'gast_stream_push_device')
         launches += int(lib.gast_last_launch_count(h.h))
         if self.augment:
-            check(lib.gast_tta_merge(y.data_ptr(), self._y.data_ptr(), n * K, J, len(self.joints_left), self._jl,
-                                     self._jr, st), 'gast_tta_merge')
+            self._merge(lib, y, self._y, n * K, st)
             launches += 1
         if P:
-            check(lib.gast_stream_peek_device(h.h, state, N, counts, active, P, py.data_ptr(), ws, wn, st),
-                  'gast_stream_peek_device')
+            eng._check(lib.gast_stream_peek_device(h.h, state, N, counts, active, P, py.data_ptr(), ws, wn, st),
+                       'gast_stream_peek_device')
             launches += int(lib.gast_last_launch_count(h.h))
             if self.augment:
-                check(lib.gast_tta_merge(py.data_ptr(), self._py.data_ptr(), n * P, J, len(self.joints_left),
-                                         self._jl, self._jr, st), 'gast_tta_merge')
+                self._merge(lib, py, self._py, n * P, st)
                 launches += 1
         return launches
 
@@ -700,18 +700,11 @@ class GraphedPoseStream(PoseStream):
         with torch.cuda.stream(side):
             st = side.cuda_stream
             h.refresh(self.model, st)
-            if self._state is None:
-                if lib.gast_stream_latency(h.h) != self.latency:
-                    raise eng.GastError('gast_stream_latency: %s' % L.last_error())
-                nb = lib.gast_stream_state_bytes(h.h, N)
-                if nb == 0:
-                    raise eng.GastError('gast_stream_state_bytes: %s' % L.last_error())
-                self._state = torch.zeros(int(nb), dtype=torch.uint8, device=self.device)
-            wb = [lib.gast_stream_device_workspace_bytes(h.h, N, k) for k in (self.K, self.P) if k]
-            if min(wb) == 0:
-                raise eng.GastError('gast_stream_device_workspace_bytes: %s' % L.last_error())
-            if self._ws is None or self._ws.numel() < max(wb):
-                self._ws = torch.empty(int(max(wb)), dtype=torch.uint8, device=self.device)
+            self._alloc_state(h)
+            wb = max(eng._check_size(lib.gast_stream_device_workspace_bytes(h.h, N, k),
+                                     'gast_stream_device_workspace_bytes') for k in (self.K, self.P) if k)
+            if self._ws is None or self._ws.numel() < wb:
+                self._ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
             # warm-up (module loads, kernel attributes, the handle's lazy set-up): with every stream inactive it
             # changes no byte of the state and no count
             self._mask_dev[N:2 * N].zero_()
@@ -731,13 +724,9 @@ class GraphedPoseStream(PoseStream):
             if self._mode_now() != self._mode:
                 raise eng.GastError('%s: engine.set_precision or engine.set_gemm_core changed since the tick was '
                                     'captured; construct a new %s' % (name, name))
-            sig = self._model_sig()
-            if sig != self._sig or self._h.sig != self._sig:
-                if not self.book.all_restarting():
-                    raise eng.GastError('%s: the model\'s parameters or buffers changed since the tick was '
-                                        'captured (load_state_dict, an optimiser step or a training forward); the '
-                                        'streams\' history was computed with the old weights -- call reset() '
-                                        'before pushing again' % name)
+            now = eng.param_sig(self.model)
+            if now != self._sig or self._h.sig != self._sig:   # new weights, or the handle prepared again
+                self._refuse_stale(self._sig, now)
                 self.graph = None
         if self.graph is None:
             self._capture()
@@ -749,7 +738,7 @@ class GraphedPoseStream(PoseStream):
     def _moved_in(self, sel, count):
         """the device counts of both library halves of the imported streams, ordered before the next replay on the
         current stream (the graph keeps the state and workspace addresses: no capture again)"""
-        rows = (sel[:, None] + self.n * np.arange(self.copies)[None, :]).reshape(-1)
+        rows = self._lib_streams(sel).reshape(-1)
         self._counts_dev[torch.from_numpy(rows).to(self.device)] = int(count)
 
     def push(self, frames, streams=None):
@@ -765,13 +754,13 @@ class GraphedPoseStream(PoseStream):
             fresh, hold, index = self.book.advance_many(K, streams=sel)
             idx = np.full((n, K), -1, dtype=np.int64)
             idx[sel] = index
+            ls = self._lib_streams(sel)
             mk = self._mask_host.numpy()
             self._uploaded.synchronize()                       # the previous tick's copy has left the buffer
             mk[:] = 0
-            mk[:N] = np.tile(np.isin(np.arange(n), sel[fresh]), self.copies)
-            mk[N:2 * N] = np.tile(np.isin(np.arange(n), sel), self.copies)
-            hk = mk[2 * N:].reshape(self.copies, n, K)
-            hk[:, sel] = hold
+            mk[ls[:, fresh]] = 1
+            mk[N + ls] = 1
+            mk[2 * N:].reshape(N, K)[ls] = hold
             self._mask_dev.copy_(self._mask_host, non_blocking=True)
             self._uploaded.record()
             self._x.copy_(frames, non_blocking=True)

@@ -69,7 +69,7 @@ def c_call_ms(ps, fn, sel, data, reps=REPS):
     the library call without the Python method's checks and allocations"""
     h = engine.model_handle(ps.model, ps.device)
     lib = h.lib
-    s = (np.asarray(sel)[:, None] + ps.n * np.arange(ps.copies)[None, :]).reshape(-1).astype(np.int32)
+    s = ps._lib_streams(sel).T.reshape(-1).astype(np.int32)
     c = np.full(s.size, max(ps.step, 1), dtype=np.int64)
     ws = torch.empty(int(lib.gast_stream_move_workspace_bytes(h.h, s.size)), dtype=torch.uint8, device=ps.device)
     st = torch.cuda.current_stream().cuda_stream
