@@ -8,6 +8,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -353,9 +354,14 @@ struct Lookup {
   const char* what;
   bool ok = true;
   std::string err;
+  // optional: every key asked for, once each, with the element count asked, in the order of its first lookup
+  std::vector<std::pair<std::string, int64_t>>* asked = nullptr;
   explicit Lookup(gast_handle* h, bool grads = false)
       : m(grads ? h->grads : h->bound), what(grads ? "gradient buffer" : "parameter") {}
+  Lookup(const std::unordered_map<std::string, Binding>& map, const char* what_) : m(map), what(what_) {}
   float* get(const std::string& key, int64_t numel) {
+    if (asked && std::none_of(asked->begin(), asked->end(), [&](const auto& a) { return a.first == key; }))
+      asked->emplace_back(key, numel);
     auto it = m.find(key);
     if (it != m.end() && (numel < 0 || it->second.numel == numel)) return reinterpret_cast<float*>(it->second.ptr);
     if (ok) {
@@ -906,6 +912,36 @@ static int call_begin(gast_handle* h, const char* who, size_t need, void* worksp
   return 0;
 }
 
+// The launches of a MODEL-kind forward on the workspace carved by `a` (the caller has checked its size)
+static int model_forward(gast_handle* h, cudaStream_t st, const float* x, float* y, int B, int T, int strided_now, Arena a,
+                         const float* target, float* loss) {
+  const int J = h->cfg.num_joints;
+  ModelBufs mb; Geometry g;
+  if (plan_model(h, B, T, strided_now, a, &mb, &g)) return 1;
+  // expand (gast_net.py:163-164) + first GraphAttentionBlock
+  long long F = (long long)B * g.T0;
+  if (launch_expand(h, st, x, mb.act[0], F * J, T, g.T0, g.s0)) return 1;
+  if (run_block(h, st, h->blocks[0], mb.act[0], F, mb.bb, mb.act[1])) return 1;
+  int cur = 1;
+  for (int i = 1; i < h->cfg.num_stages; ++i) {
+    StageConsts& s = h->stages[i - 1];
+    const StageGeo& sg = g.stages[i - 1];
+    const int Cw = s.Cw;
+    const long long Fn = (long long)B * sg.Tout;
+    const float* xin = mb.act[cur];
+    const ASeg taps = seg_taps(xin, Cw, Cw, sg.taps, (long long)sg.dil * J * Cw, sg.tapmap);
+    if (run_stage(h, st, s, Fn, taps, s.Wt, &s.tc_t, mb.tmp, xin, sg.resmap, mb.act[cur ^ 1])) return 1;
+    cur ^= 1;
+    if (run_block(h, st, h->blocks[i], mb.act[cur], Fn, mb.bb, mb.act[cur ^ 1])) return 1;
+    cur ^= 1;
+    F = Fn;
+  }
+  // output is already (B, T_out, J, 3)
+  if (launch_shrink(h, st, mb.act[cur], y, F * J, target, loss)) return 1;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 static int forward_impl(gast_t* h, const float* x, float* y, int32_t B, int32_t T, int32_t strided_now,
                         void* workspace, size_t workspace_bytes, void* stream, const float* target, float* loss) {
   if (!h) return fail("gast_forward: null handle");
@@ -932,31 +968,7 @@ static int forward_impl(gast_t* h, const float* x, float* y, int32_t B, int32_t 
     CUDA_OK(cudaGetLastError());
     return 0;
   }
-
-  ModelBufs mb; Geometry g;
-  if (plan_model(h, B, T, strided_now, a, &mb, &g)) return 1;
-  // expand (gast_net.py:163-164) + first GraphAttentionBlock
-  long long F = (long long)B * g.T0;
-  if (launch_expand(h, st, x, mb.act[0], F * J, T, g.T0, g.s0)) return 1;
-  if (run_block(h, st, h->blocks[0], mb.act[0], F, mb.bb, mb.act[1])) return 1;
-  int cur = 1;
-  for (int i = 1; i < h->cfg.num_stages; ++i) {
-    StageConsts& s = h->stages[i - 1];
-    const StageGeo& sg = g.stages[i - 1];
-    const int Cw = s.Cw;
-    const long long Fn = (long long)B * sg.Tout;
-    const float* xin = mb.act[cur];
-    const ASeg taps = seg_taps(xin, Cw, Cw, sg.taps, (long long)sg.dil * J * Cw, sg.tapmap);
-    if (run_stage(h, st, s, Fn, taps, s.Wt, &s.tc_t, mb.tmp, xin, sg.resmap, mb.act[cur ^ 1])) return 1;
-    cur ^= 1;
-    if (run_block(h, st, h->blocks[i], mb.act[cur], Fn, mb.bb, mb.act[cur ^ 1])) return 1;
-    cur ^= 1;
-    F = Fn;
-  }
-  // output is already (B, T_out, J, 3)
-  if (launch_shrink(h, st, mb.act[cur], y, F * J, target, loss)) return 1;
-  CUDA_OK(cudaGetLastError());
-  return 0;
+  return model_forward(h, st, x, y, B, T, strided_now, a, target, loss);
 }
 
 extern "C" int gast_forward(gast_t* h, const float* x, float* y, int32_t B, int32_t T, int32_t strided_now,
@@ -1158,6 +1170,8 @@ extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, fl
   CUDA_OK(cudaGetLastError());
   return 0;
 }
+
+#include "chunked.cuh"
 
 // Timing of the debug entries: `launch` once, then `reps` more times between two events on `st`; waits for the stream
 // and, when all of it succeeded and reps > 0, stores the ms per rep in *ms_out.  Returns 0, the first failing launch's

@@ -27,8 +27,12 @@ struct TCtx {
   bool pgrad;
   int tc_slot = 0;   // next slot of the handle's table of per-GEMM tensor-core operand copies (train_tcw)
   Lookup params, grad_bufs;
-  TCtx(gast_handle* h_, cudaStream_t st_, Arena a_, bool pgrad_)
-      : h(h_), st(st_), a(a_), J(h_->cfg.num_joints), dry(a_.dry), pgrad(pgrad_), params(h_), grad_bufs(h_, true) {}
+  // grads: where the gradient buffers are looked up, the handle's gast_bind_grads bindings unless given (the chunked
+  // eval backward points the passes after its first at its pass-gradient area)
+  TCtx(gast_handle* h_, cudaStream_t st_, Arena a_, bool pgrad_,
+       const std::unordered_map<std::string, Binding>* grads = nullptr)
+      : h(h_), st(st_), a(a_), J(h_->cfg.num_joints), dry(a_.dry), pgrad(pgrad_), params(h_),
+        grad_bufs(grads ? Lookup(*grads, "gradient buffer") : Lookup(h_, true)) {}
   float* fl(size_t n) { return a.take(n); }
   double* dbl(size_t n) { return reinterpret_cast<double*>(a.take(2 * n)); }
   unsigned char* bytes(size_t n) { return reinterpret_cast<unsigned char*>(a.take((n + 3) / 4)); }

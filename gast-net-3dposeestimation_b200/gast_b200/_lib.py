@@ -20,7 +20,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_get_timings', 'gast_set_gemm_core', 'gast_set_precision', 'gast_set_train_precision',
            'gast_last_wgrad_tc_launch_count', 'gast_debug_gemm', 'gast_debug_wgrad', 'gast_bind_grads',
            'gast_train_workspace_bytes', 'gast_forward_train', 'gast_backward', 'gast_backward_input',
-           'gast_eval_backward_workspace_bytes', 'gast_eval_backward', 'gast_set_dropout_state', 'gast_tta_prepare', 'gast_tta_merge',
+           'gast_eval_backward_workspace_bytes', 'gast_eval_backward', 'gast_chunked_workspace_bytes',
+           'gast_forward_chunked', 'gast_eval_backward_chunked', 'gast_set_dropout_state', 'gast_tta_prepare', 'gast_tta_merge',
            'gast_stream_state_bytes', 'gast_stream_workspace_bytes', 'gast_stream_push',
            'gast_stream_latency', 'gast_stream_push_ex', 'gast_stream_chunk_workspace_bytes', 'gast_stream_push_chunk',
            'gast_stream_peek', 'gast_stream_subset_workspace_bytes', 'gast_stream_push_subset', 'gast_stream_peek_subset',
@@ -115,6 +116,13 @@ def load():
     lib.gast_eval_backward_workspace_bytes.restype = C.c_size_t
     lib.gast_eval_backward.argtypes = [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.c_size_t, vp]
     lib.gast_eval_backward.restype = C.c_int
+    lib.gast_chunked_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]
+    lib.gast_chunked_workspace_bytes.restype = C.c_size_t
+    lib.gast_forward_chunked.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.c_size_t, vp]
+    lib.gast_forward_chunked.restype = C.c_int
+    lib.gast_eval_backward_chunked.argtypes = [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp,
+                                               C.c_size_t, vp]
+    lib.gast_eval_backward_chunked.restype = C.c_int
     lib.gast_set_dropout_state.argtypes = [vp, vp]
     lib.gast_set_dropout_state.restype = C.c_int
     lib.gast_stream_state_bytes.argtypes = [vp, C.c_int32]

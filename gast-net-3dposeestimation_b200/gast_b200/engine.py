@@ -503,6 +503,85 @@ def run_model_mpjpe(module, x, target):
     return y, loss
 
 
+def run_model_chunked(module, x, max_frames):
+    """`model(x)` of a whole model in eval() mode in bounded memory: the library covers the (clip, output frame) grid
+    in passes of at most `max_frames` output positions (whole clips, or windows of one clip's output frames with the
+    input frames they read), so the workspace depends on max_frames and the architecture, not on the batch or the
+    recording length.  Under no_grad, or when neither x nor a parameter requires grad, it is the chunked forward,
+    bitwise model(x).  Otherwise the output carries a backward that runs gast_eval_backward_chunked: the gradients of
+    model(x)'s backward up to summation order across passes (the same kernels in the same order when one pass covers
+    the call).  Train mode
+    raises: batch statistics span the whole batch and cannot be chunked."""
+    x = _cuda_f32(x, 'run_model_chunked')
+    if module.training:
+        raise GastError('run_model_chunked: the model is in train mode, whose BatchNorm statistics span the whole '
+                        'batch and cannot be chunked; call .eval()')
+    h = model_handle(module, x.device)
+    strided_now = _strided_now(module, int(x.shape[1]))
+    np_ = named_params(module) if torch.is_grad_enabled() else []
+    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for _, p in np_)):
+        _fp32_only(module, 'run_model_chunked with autograd (requires_grad input or parameters)')
+        y = _ChunkedEvalFn.apply(module, h, x, strided_now, int(max_frames), [k for k, _ in np_], *[p for _, p in np_])
+    else:
+        y = _chunked_forward(module, h, x, strided_now, int(max_frames))
+    module.__dict__['_gast_last_launches'] = h.launches()
+    return y
+
+
+def _chunked_forward(module, h, x, strided_now, max_frames):
+    """gast_forward_chunked of x (B,T,J,F) -> y (B,T_out,J,3) on a workspace of its own"""
+    dev = x.device
+    B, T = int(x.shape[0]), int(x.shape[1])
+    with torch.cuda.device(dev):
+        st = _stream(dev)
+        h.refresh(module, st)
+        y = _new_output(module, h, B, T, strided_now, dev)
+        need = _check_size(h.lib.gast_chunked_workspace_bytes(h.h, B, T, strided_now, max_frames, 0),
+                           'gast_chunked_workspace_bytes')
+        ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        _check(h.lib.gast_forward_chunked(h.h, _p(x), _p(y), B, T, strided_now, max_frames, _p(ws), ws.numel(),
+                                          C.c_void_p(st)), 'gast_forward_chunked')
+    return y
+
+
+class _ChunkedEvalFn(torch.autograd.Function):
+    """_EvalFn in bounded memory: the chunked forward, and a backward (gast_eval_backward_chunked) that recomputes and
+    differentiates pass by pass.  Saves what _EvalFn saves, so an in-place change before the backward raises torch's
+    version error."""
+
+    @staticmethod
+    def forward(ctx, module, handle, x, strided_now, max_frames, names, *params):
+        y = _chunked_forward(module, handle, x, strided_now, max_frames)
+        stats = [v for k, v in named_tensors(module) if k.endswith('.running_mean') or k.endswith('.running_var')]
+        ctx.save_for_backward(x, *params, *stats)
+        ctx.module, ctx.handle, ctx.sn, ctx.max_frames, ctx.names, ctx.n = (module, handle, strided_now, max_frames,
+                                                                            names, len(params))
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        saved = ctx.saved_tensors
+        x, params = saved[0], saved[1:1 + ctx.n]
+        module, h, mf = ctx.module, ctx.handle, ctx.max_frames
+        need_x = ctx.needs_input_grad[2]
+        need_p = any(ctx.needs_input_grad[6:])
+        dev = x.device
+        B, T = int(x.shape[0]), int(x.shape[1])
+        dy = dy.contiguous()
+        with torch.cuda.device(dev):
+            st = _stream(dev)
+            h.refresh(module, st)
+            lib = h.lib
+            need = _check_size(lib.gast_chunked_workspace_bytes(h.h, B, T, ctx.sn, mf, 1),
+                               'gast_chunked_workspace_bytes')
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            dx = torch.empty_like(x) if need_x else None
+            views = _bind_grad_views(h, ctx.names, params, False, dev) if need_p else None
+            _check(lib.gast_eval_backward_chunked(h.h, _p(x), _p(dy), _p(dx), 1 if need_p else 0, B, T, ctx.sn, mf,
+                                                  _p(ws), ws.numel(), C.c_void_p(st)), 'gast_eval_backward_chunked')
+        return (None, None, dx, None, None, None) + (tuple(views) if views is not None else (None,) * ctx.n)
+
+
 def _run_module(module, x, what, kind, cfg, width_out, masks=None, train_ok=False):
     """The forward of a sub-module on its own, channels-last: x (..., J, C) -> (..., J, width_out), all leading rows in
     one library call.  Only a sub-module without BatchNorm or dropout (train_ok) also runs in train mode."""
