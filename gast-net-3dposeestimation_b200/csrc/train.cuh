@@ -277,6 +277,19 @@ static int block_fwd(TCtx& c, TrainState& ts, BlockSave& b, BlockConsts& bc, con
 }
 
 // ---- GraphAttentionBlock, backward: dOut (M x 2C) -> dX (M x C, overwritten) ----------------------------
+// att_mix_bwd_kernel keeps four 4 x J x J tables in dynamic shared memory, 16 J^2 floats: 50,176 B at J = 28 and
+// 65,536 B at J = 32 (gast_create's limit), over the 48 KB a launch gets without opting in.  The opt-in is per device.
+static int att_mix_bwd_optin(const gast_handle* h) {
+  static bool done[64];
+  bool& d = done[h->cfg.device & 63];
+  if (!d) {
+    CUDA_OK(cudaFuncSetAttribute((const void*)att_mix_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)sizeof(float) * 16 * 32 * 32));
+    d = true;
+  }
+  return 0;
+}
+
 static int block_bwd(TCtx& c, const BlockSave& b, BlockConsts& bc, const float* dOut, float* dX) {
   gast_handle* h = c.h;
   const int C = b.C, J = c.J;
@@ -310,8 +323,14 @@ static int block_bwd(TCtx& c, const BlockSave& b, BlockConsts& bc, const float* 
   float* dbg = c.fl(C);
   float* dcab = c.fl(8);
   float* dXg = c.fl((size_t)M * C);
+  if (c.live([&] { return att_mix_bwd_optin(h); })) return 1;
   c.launch(att_mix_bwd_kernel, (unsigned)F, 256, sizeof(float) * 16 * J * J, dY, C, b.G, C, b.AB, bc.Ck, J, 4, C / 4,
            dG, C, dab, dCkp);
+  if (c.live([&] {
+        const cudaError_t e = cudaGetLastError();
+        return e == cudaSuccess ? 0 : fail("att_mix_bwd_kernel launch failed (J=%d): %s", J, cudaGetErrorString(e));
+      }))
+    return 1;
   if (c.pgrad) {
     c.launch(col_sum_det_kernel, cdiv(4 * J * J, 32), 256, 0, dCkp, F, 4 * J * J, dCk);
     c.zero(dsum, sizeof(double) * (C + 8));

@@ -250,6 +250,32 @@ def module_cases():
          meta=dict(kind='block', J=J2, C=16, seed=9, keys=keys_shapes(blk2)))
 
 
+def variant_cases():
+    """Sub-module variants the drop-in modules reach besides the 4-head, 32 -> 32 ones of module_cases: MultiGlobalGraph
+    with 1 and 3 heads (in // inter; 2 heads cannot run in the reference: each head's g conv is then in_channels wide
+    and the concatenation does not fit its view) at J = 17, 19 and 24 (the attention only uses adj's shape), and
+    SemCHGraphConv / SemGraphConv (shared e, bias) with out_features != in_features, including widths that leave a
+    partial 64-channel tile."""
+    for J, C, inter, seed in ((17, 32, 32, 21), (19, 96, 32, 22), (17, 48, 16, 23), (24, 32, 32, 24), (24, 96, 32, 25)):
+        adj = adj_for(J) if J in (17, 19) else torch.eye(J)
+        x = (0.7 * np.random.RandomState(seed).standard_normal((2, 3, J, C))).astype(np.float32)
+        mg = MultiGlobalGraph(adj, C, inter, dropout=0.05)
+        assert mg.num_non_local == C // inter and mg.attentions[0].g_channels == inter
+        synth.randomize_module(mg, seed)
+        mg.eval()
+        save('var_mglobal_%d_c%d_i%d' % (J, C, inter), x=x, y=mg(torch.from_numpy(x)).contiguous().numpy(),
+             meta=dict(kind='mglobal', J=J, C=C, inter=inter, heads=C // inter, seed=seed, keys=keys_shapes(mg)))
+    for J, cin, cout, shared, seed in ((17, 32, 4, False, 31), (17, 48, 36, False, 32), (19, 32, 200, False, 33),
+                                       (19, 48, 64, False, 34), (17, 32, 36, True, 35), (19, 48, 200, True, 36)):
+        con = LocalGraph(adj_for(J), 8, 8).gcn_con.adj[0]
+        x = (0.7 * np.random.RandomState(seed).standard_normal((2, 3, J, cin))).astype(np.float32)
+        mod = SemGraphConv(cin, cout, con, bias=True) if shared else SemCHGraphConv(cin, cout, con)
+        synth.randomize_module(mod, seed)
+        save('var_%s_%d_%dto%d' % ('semgc' if shared else 'semch', J, cin, cout), x=x,
+             y=mod(torch.from_numpy(x)).contiguous().numpy(), mask=(con > 0).numpy(),
+             meta=dict(kind='semgc' if shared else 'semch', J=J, Cin=cin, Cout=cout, seed=seed, keys=keys_shapes(mod)))
+
+
 def _digest(t, idx):
     """compact fingerprint of one tensor: norm, sum, and the entries at `idx` (flat indices)"""
     f = t.detach().reshape(-1).double()
@@ -420,8 +446,11 @@ if __name__ == '__main__':
         tc_cases()
     elif len(sys.argv) > 1 and sys.argv[1] == 'stream':
         stream_cases()
+    elif len(sys.argv) > 1 and sys.argv[1] == 'variants':
+        variant_cases()
     else:
         main()
+        variant_cases()
         tta_cases()
         pipeline_cases()
         train_cases()
