@@ -345,7 +345,8 @@ __global__ void copy2d_kernel(const float* __restrict__ src, int lds, float* __r
 }
 
 // counter-based dropout mask (nn.Dropout semantics: keep with prob 1-p, scale 1/(1-p)); the
-// stream is ours, not torch's -- loss-match tests use p = 0 (SURVEY.md §7 "Dropout parity")
+// stream is ours, not torch's.  tests/dropoutref.py restates it bit for bit, so the tests replay these masks into the
+// fp64 port and the reference and hold training with dropout to the dropout-0 bars (SURVEY.md §7 "Dropout parity")
 // `dseed` (device, may be null): added to the seed, so that a CUDA-graph replay of the step -- whose kernel arguments
 // are frozen -- still draws a fresh mask (dropout_bump_kernel advances it once per forward).
 __global__ void dropout_mask_kernel(unsigned char* __restrict__ keep, long long n, float p, unsigned long long seed,

@@ -38,6 +38,14 @@ def _relu(h, tap, name):
     return F.relu(h)
 
 
+def _dropout(h, drop, training, name):
+    """F.dropout(h, drop, training) for a float `drop`; a callable `drop(name, h) -> h` instead applies a given mask
+    (in training only), name being the prefix of the BatchNorm in front of this dropout"""
+    if callable(drop):
+        return drop(name, h) if training else h
+    return F.dropout(h, drop, training)
+
+
 def semch(x, W, e, mask, bias=None):
     """SemCHGraphConv.forward (model/local_attention.py:35-53)."""
     Cout = W.shape[2]
@@ -63,7 +71,7 @@ def local_graph(x, p, prefix, masks, training=False, stats=None, drop=0.0, tap=N
     o = torch.cat((a, b), dim=1)
     o = _relu(_bn(F.conv2d(o, p[prefix + 'cat_conv.weight']), p, prefix + 'cat_bn.', training, stats), tap,
               prefix + 'cat_bn.')
-    o = F.dropout(o, drop, training)
+    o = _dropout(o, drop, training, prefix + 'cat_bn.')
     return o.permute(0, 2, 3, 1)
 
 
@@ -97,7 +105,7 @@ def multi_global_graph(x, p, prefix, training=False, stats=None, drop=0.0, tap=N
     y = y.permute(0, 2, 1).contiguous().view(B, T, J, C).permute(0, 3, 1, 2)
     y = _relu(_bn(F.conv2d(y, p[prefix + 'cat_conv.weight']), p, prefix + 'cat_bn.', training, stats), tap,
               prefix + 'cat_bn.')
-    y = F.dropout(y, drop, training)
+    y = _dropout(y, drop, training, prefix + 'cat_bn.')
     return y.permute(0, 2, 3, 1)
 
 
@@ -117,7 +125,9 @@ def forward(x, p, masks, filter_widths, causal=False, strided=False, dense=False
     159-177, 236-251).  x: (B,T,J,F) -> (B,T_out,J,3).
     `tap(name, h)`, when given, sees every kink input in forward order without changing anything: each ReLU input
     (name: the prefix of the BatchNorm in front of it) and each head's attention logits before the LeakyReLU (name:
-    the head's prefix, h of shape (BT, J, J))."""
+    the head's prefix, h of shape (BT, J, J)).
+    `drop` is the dropout probability, or a callable `drop(name, h)` that applies the mask of the dropout behind
+    the BatchNorm `name` in training mode (tests/dropoutref.py replays the library's masks this way)."""
     fw = filter_widths
     pad = [fw[0] // 2]
     shift = [(fw[0] // 2) if causal else 0]
@@ -146,7 +156,7 @@ def forward(x, p, masks, filter_widths, causal=False, strided=False, dense=False
                       training, stats), tap, 'layers_bn.%d.' % (2 * i))
         h = _relu(_bn(F.conv2d(h, p['layers_conv.%d.weight' % (2 * i + 1)]), p, 'layers_bn.%d.' % (2 * i + 1),
                       training, stats), tap, 'layers_bn.%d.' % (2 * i + 1))
-        h = res + F.dropout(h, drop, training)
+        h = res + _dropout(h, drop, training, 'layers_bn.%d.' % (2 * i + 1))
         h = graph_attention_block(h, p, 'layers_graph_conv.%d.' % (i + 1), masks, training, stats, drop, tap)
     y = F.conv2d(h, p['shrink.weight'])
     return y.permute(0, 2, 3, 1)

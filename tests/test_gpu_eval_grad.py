@@ -51,13 +51,17 @@ def _model(J, fw, ch, strided, causal=False, dense=False, dropout=0.25, seed=5):
 def test_gradients_vs_reference_fixture(name, core):
     """`loss = mpjpe(model(x), target)` with x.requires_grad_(): y, loss, every parameter gradient (step-0 bars of
     train_fixture.check_step) and dx (the same relative bars).  The train-mode fixture is also differentiated with
-    every parameter frozen (x only)."""
+    every parameter frozen (x only).  A fixture with dropout ran the reference with the masks the library draws
+    right after torch.manual_seed(meta['drop_seed']) (tests/dropoutref.py): each forward here follows that seed."""
     g = load_golden(name)
     meta = g['meta']
     rep = ['== %s core %d' % (name, core)]
     tgt = torch.from_numpy(g['target']).cuda()
     m = grad_module(meta).cuda()
     x = torch.from_numpy(g['x']).cuda().requires_grad_()
+    seed = meta.get('drop_seed')
+    if seed is not None:
+        torch.manual_seed(seed)
     y = m(x)
     loss = _mpjpe(y, tgt)
     loss.backward()
@@ -67,6 +71,8 @@ def test_gradients_vs_reference_fixture(name, core):
     if meta['training']:
         m = grad_module(meta).cuda().requires_grad_(False)
         x = torch.from_numpy(g['x']).cuda().requires_grad_()
+        if seed is not None:
+            torch.manual_seed(seed)
         _mpjpe(m(x), tgt).backward()
         bad += check_dx(g, x.grad.cpu().numpy(), 5e-2, report=rep)
         assert all(p.grad is None for p in m.parameters())

@@ -1,7 +1,8 @@
 """Every gradient tensor of the lifting network on the GPU, per tensor, against fp64 autograd of the torch-CPU port
 at the kink-free test points of tests/kinkfree.py: y, the loss, every parameter gradient, dL/dx, and dL/dx of the
-input-only path (every parameter frozen) in train mode (batch statistics) and eval mode (running statistics), on
-both GEMM cores.  No ReLU or LeakyReLU input lies near its kink there, so fp64 is an exact reference and every
+input-only path (every parameter frozen) in train mode (batch statistics, with and without dropout: the masks are
+the library's own, replayed into the port by tests/dropoutref.py) and eval mode (running statistics), on both GEMM
+cores.  No ReLU or LeakyReLU input lies near its kink there, so fp64 is an exact reference and every
 tensor is held to a rounding-level bar: a fault confined to one small tensor (C_k, concat_project, e, a BatchNorm
 bias, a tail column of a weight gradient, one split of a reduction) fails it."""
 import os
@@ -33,6 +34,7 @@ def _run(case, ref, frozen):
     m.load_state_dict(ref['sd'])
     m = m.cuda().train(case.training).requires_grad_(not frozen)
     x = ref['x'].cuda().requires_grad_()
+    torch.manual_seed(K.DROP_SEED)      # the dropout masks of the reference (kinkfree.drop_masks)
     y = m(x)
     loss = _mpjpe(y, ref['target'].cuda())
     loss.backward()

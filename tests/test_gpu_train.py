@@ -37,9 +37,9 @@ def _masks(J):
     return tuple(torch.from_numpy(a) for a in O.local_masks(O.adj_from_parents(synth.skeleton_parents(J))))
 
 
-def _oracle_step(p, x, target, fw, J, stats):
+def _oracle_step(p, x, target, fw, J, stats, drop=0.0):
     from oracle import gast_torch_ref as TR
-    y = TR.forward(x, p, _masks(J), fw, strided=True, training=True, stats=stats)
+    y = TR.forward(x, p, _masks(J), fw, strided=True, training=True, stats=stats, drop=drop)
     return y, TR.mpjpe(y, target)
 
 
@@ -110,10 +110,13 @@ def test_train_forward_and_gradients(J, fw, ch, B):
     assert not bad, sorted(bad, key=lambda t: -t[1])[:12]
 
 
-def _run_steps(make_opt, nsteps, B=32, seed=9):
+def _run_steps(make_opt, nsteps, B=32, seed=9, drop=0.0):
+    """`nsteps` optimiser steps of the library and of the port; with dropout, step i's forward follows
+    torch.manual_seed(300 + i) and the port replays the masks the library draws there (tests/dropoutref.py)"""
+    import dropoutref as D
     from model.gast_net import SpatioTemporalModelOptimized1f
     J, fw, ch = 17, [3, 3, 3], 128
-    m = SpatioTemporalModelOptimized1f(_adj(J), J, 2, J, fw, dropout=0.0, channels=ch)
+    m = SpatioTemporalModelOptimized1f(_adj(J), J, 2, J, fw, dropout=drop, channels=ch)
     synth.randomize_module(m, seed)
     sd0 = {k: v.clone() for k, v in m.state_dict().items()}
     p = {k: v.clone().requires_grad_(v.dtype.is_floating_point and 'running' not in k) for k, v in sd0.items()}
@@ -124,12 +127,15 @@ def _run_steps(make_opt, nsteps, B=32, seed=9):
     for step in range(nsteps):
         x = torch.from_numpy(synth.synth_input(B, 27, J, 2, seed=100 + step))
         tgt = torch.from_numpy(synth.synth_target(B, J, seed=200 + step))
+        arch = dict(filter_widths=fw, channels=ch, strided=True)
+        masks = D.masks(arch, B, 27, J, drop, D.engine_seed(300 + step)) if drop > 0 else None
         opt_ref.zero_grad()
-        _, loss_ref = _oracle_step(p, x, tgt, fw, J, stats)
+        _, loss_ref = _oracle_step(p, x, tgt, fw, J, stats, D.dropper(masks) if masks else 0.0)
         loss_ref.backward()
         g_ref = {k: v.grad.clone() for k, v in p.items() if v.requires_grad}
         opt_ref.step()
         opt.zero_grad()
+        torch.manual_seed(300 + step)
         y = m(x.cuda())
         loss = torch.mean(torch.norm(y - tgt.cuda(), dim=3))
         loss.backward()
@@ -144,7 +150,12 @@ def test_three_sgd_steps_match_reference_port():
     weights / running statistics must agree afterwards.  SGD(momentum) is used for the multi-step
     check because Adam's first steps are ~lr*sign(g): parameters whose gradient is rounding noise
     move by +-lr at random in ANY two implementations (CPU vs GPU reference included)."""
-    m, p, stats, losses, _ = _run_steps(lambda ps: torch.optim.SGD(ps, lr=1e-2, momentum=0.9), 3)
+    check_three_sgd_steps(0.0)
+
+
+def check_three_sgd_steps(drop):
+    """test_three_sgd_steps_match_reference_port at dropout `drop`"""
+    m, p, stats, losses, _ = _run_steps(lambda ps: torch.optim.SGD(ps, lr=1e-2, momentum=0.9), 3, drop=drop)
     for step, (a, b) in enumerate(losses):
         assert abs(a - b) < 1e-4 * abs(b), (step, a, b)
     sd = m.state_dict()

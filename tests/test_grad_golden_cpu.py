@@ -1,7 +1,8 @@
 """Gradients of the lifting network with respect to its parameters and its 2D input, in eval() mode (BatchNorm on the
 running statistics, Dropout off) and in train() mode: the differentiable torch-CPU port (oracle/gast_torch_ref.py)
-against fixtures of the UNMODIFIED reference (tests/golden/grad_*.npz, make_golden_grad.py).  This pins the
-oracle the GPU tests of tests/test_gpu_eval_grad.py compare against.  CPU only."""
+against fixtures of the UNMODIFIED reference (tests/golden/grad_*.npz, make_golden_grad.py).  A train-mode fixture
+with dropout stores the masks it ran with (the library's own, tests/dropoutref.py); the port applies them too.  This
+pins the oracle the GPU tests of tests/test_gpu_eval_grad.py compare against.  CPU only."""
 import numpy as np
 import pytest
 import torch
@@ -9,6 +10,7 @@ import torch
 from conftest import load_golden, golden_names
 from oracle import gast_oracle as O
 from gast_b200 import synth
+import dropoutref as D
 import train_fixture as TF
 
 
@@ -50,11 +52,12 @@ def test_torch_ref_gradients_match_reference_fixture(name):
          for k, v in m.state_dict().items()}
     masks = tuple(torch.from_numpy(a) for a in O.local_masks(O.adj_from_parents(synth.skeleton_parents(meta['J']))))
     x = torch.from_numpy(g['x']).requires_grad_()
+    drop = D.dropper(D.golden_masks(g)) if meta.get('drop_seed') is not None else 0.0
     threads = torch.get_num_threads()
     torch.set_num_threads(meta['threads'])      # the fixture's CPU summation order (make_golden_grad.py)
     try:
         y = TR.forward(x, p, masks, meta['filter_widths'], causal=meta['causal'], strided=meta['strided'],
-                       training=meta['training'], stats={} if meta['training'] else None)
+                       training=meta['training'], stats={} if meta['training'] else None, drop=drop)
         loss = TR.mpjpe(y, torch.from_numpy(g['target']))
         loss.backward()
     finally:
