@@ -18,8 +18,7 @@
 // inference only (DESIGN.md §4.1).
 //
 // The three forms share everything below except the slot contents (B_lo is not staged in 1xTF32; F16X3 stages
-// fp16 B copies and pads A rows to 40 floats), the ring depth and the wgmmas per 16-K partial (3xTF32 6 m64n128k8,
-// 1xTF32 2, F16X3 3 m64n128k16).
+// fp16 B copies), the ring depth and the wgmmas per 16-K partial (3xTF32 6 m64n128k8, 1xTF32 2, F16X3 3 m64n128k16).
 //
 // Two-level accumulation: the tensor core aligns and truncates its addends, so a long chain of MMAs
 // into one accumulator is biased towards zero by ~0.5 ulp per MMA.  Every 16 K are therefore accumulated in a
@@ -34,12 +33,17 @@
 //                layout wgmma reads from shared memory (8 rows x 16 B core matrices, 128 B apart along N, 2048 B
 //                apart along K); the box is described as rows of 2 KB (a k-quad or k-octet of the tile's 128 n),
 //                not 16-byte rows, and one elected thread issues the boxes.
-//     A (activations): rows are gathered per frame (dilated / strided taps, residual slices, concatenations), so
-//                they arrive by cp.async (16 B per row and k-quad, zero-filled outside the tile) from all 128
-//                producer threads.  A stage never straddles a tap (Kc % 32 == 0), so segment, tap and column are
-//                advanced once per stage.
-//     The slot's `full` mbarrier completes when the TMA bytes (expect_tx) and every producer thread's cp.asyncs
-//     (cp.async.mbarrier.arrive.noinc) have landed: 1 + 128 arrivals.
+//     A (activations): a stage is 128 dense rows of 32 floats in TMA's 128-byte swizzle (chunk c of row r at
+//                c ^ (r & 7)), which keeps the consumers' fragment loads free of bank conflicts.  A segment whose
+//                tile rows are contiguous in its source (tc_seg_tma: identity frame map, no tap offset; the 1x1 layers,
+//                SemCH, the attention GEMMs and the block concatenations) is one TMA box per stage from the same
+//                elected thread, rows past the source's end zero-filled.  Rows gathered per frame (dilated / strided
+//                taps, the streams' ring taps) arrive by cp.async (16 B per row and k-quad, zero-filled outside the
+//                tile) from all 128 producer threads into the same swizzled layout.  A stage never straddles a tap
+//                (Kc % 32 == 0), so segment, tap, column and path are chosen once per stage.
+//     The slot's `full` mbarrier completes when the TMA bytes (expect_tx) and, in a launch with a gathered segment,
+//     every producer thread's cp.asyncs (cp.async.mbarrier.arrive.noinc) or plain arrivals have landed: 1 + 128
+//     arrivals; 1 when every segment is loaded by TMA (the other producer threads then leave at once).
 //   consumers (warpgroups 1 and 2, 232 registers): warpgroup 1 + w owns rows 64w .. 64w+63 and all 128 columns:
 //     wgmma.m64n128k8 tf32 or m64n128k16 f16, A from registers (loaded from the slot and converted there: to tf32,
 //     split into hi / lo in 3xTF32; in F16X3 the four threads of a quad find their rows' max |a| over the stage's
@@ -49,8 +53,11 @@
 //     and added, and the slot is released (its `empty` mbarrier, one arrival per consumer warp, 8 in all).  No
 //     partial stays in flight across the loop's back edge: ptxas then serialises every wgmma of the kernel (C7514).
 //     The two consumers do not synchronise with each other inside the K loop, so one's MMAs fill the other's drain.
-// Tiles (fpt whole frames per 128-row tile) and the fused epilogues (gemm_epilogue, run by the 256 consumer threads)
-// are the FFMA core's, so both cores are interchangeable per launch.
+// Tiles (fpt whole frames per 128-row tile) and the fused epilogues are the FFMA core's, so both cores are
+// interchangeable per launch.  EPI_PLAIN runs on the wgmma fragments (tc_store_plain: bias, ReLU, residual in
+// gemm_epilogue's order) and leaves by four TMA tensor stores from the freed ring; EPI_SEMCH and EPI_GLOBAL mix
+// joints across rows, so their tiles are handed over in the FFMA thread layout to gemm_epilogue, run by the 256
+// consumer threads.
 //
 // One tile per CTA, on a 1D grid in which the column tile is the fast index (tc_launch): the CTAs dispatched together
 // cover a row tile's column tiles side by side, so its A rows come from HBM once and its other column tiles find them
@@ -85,7 +92,7 @@ enum { TC_3XTF32 = 0, TC_1XTF32 = 1, TC_F16X3 = 2 };
 #define GAST_TC1_STAGES 3                             // ring depth of the 1xTF32 form: 4 and 5 measured no faster (DESIGN.md §4.1)
 #endif
 #ifndef GAST_TC16_STAGES
-#define GAST_TC16_STAGES 3                            // ring depth of the F16X3 form: 4 and 5 measured no faster (DESIGN.md §4.1)
+#define GAST_TC16_STAGES 3                            // ring depth of the F16X3 form: 4 measured within noise of 3 (DESIGN.md §4.1)
 #endif
 
 constexpr int TC_BM = 128, TC_BN = 128;
@@ -93,18 +100,16 @@ constexpr int TC_KS = 32;                            // K per ring stage; segmen
 constexpr int TC_KP = 16;                            // K per partial sum, added into the tile sum with RN
 constexpr int TC_THREADS = 384;                      // warpgroup 0 produces, warpgroups 1 and 2 consume
 constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;   // 128 * 40 + 256 * 232 <= 64K registers of the SM
-constexpr int TC_ALD = TC_KS + 4;                    // A stage row stride (floats): conflict-free fragment loads
-constexpr int TC_ALD16 = TC_KS + 8;                  // the same for F16X3's 64-bit k-pair loads
 constexpr int TC_B_BYTES = TC_BN * TC_KS * 4;        // one of B_hi / B_lo in a stage
 constexpr int TC_B16_BYTES = TC_BN * TC_KS * 2;      // the same in F16X3
-constexpr int TC_A_BYTES = TC_BM * TC_ALD * 4;
-// A row stride, B copy bytes, B copies per slot, slot size and ring depth of each precision.  3xTF32: a fourth 50 KB
-// slot does not fit in TC_SMEM_MAX beside the row table.
-__host__ __device__ constexpr int tc_ald(int prec) { return prec == TC_F16X3 ? TC_ALD16 : TC_ALD; }
+// A stage: 128 dense rows of 32 floats (128 B) in TMA's 128-byte swizzle, 16-byte chunk c of row r at chunk
+// c ^ (r & 7) (tc_achunk); 1024-byte aligned in every slot
+constexpr int TC_A_BYTES = TC_BM * TC_KS * 4;
+// B copy bytes, B copies per slot, slot size and ring depth of each precision
 __host__ __device__ constexpr int tc_bbytes(int prec) { return prec == TC_F16X3 ? TC_B16_BYTES : TC_B_BYTES; }
 __host__ __device__ constexpr int tc_nb(int prec) { return prec == TC_1XTF32 ? 1 : 2; }
 __host__ __device__ constexpr int tc_slot(int prec) {                       // B_hi [| B_lo] | A
-  return tc_nb(prec) * tc_bbytes(prec) + TC_BM * tc_ald(prec) * 4;
+  return tc_nb(prec) * tc_bbytes(prec) + TC_A_BYTES;
 }
 __host__ __device__ constexpr int tc_stages(int prec) {
   return prec == TC_1XTF32 ? GAST_TC1_STAGES : prec == TC_F16X3 ? GAST_TC16_STAGES : 3;
@@ -113,8 +118,8 @@ __host__ __device__ constexpr int tc_ring(int prec) { return tc_stages(prec) * t
 constexpr int TC_STG_LD = 136;                       // [row][col] stride of the accumulator hand-over to the epilogue
 constexpr int TC_ROWBASE_BYTES = 3 * 128 * sizeof(long long);
 constexpr int TC_SMEM_MAX = 200 * 1024;
-static_assert(tc_slot(TC_3XTF32) % 1024 == 0 && tc_slot(TC_1XTF32) % 1024 == 0 && tc_slot(TC_F16X3) % 1024 == 0,
-              "ring slots stay 1024-byte aligned");
+static_assert(tc_slot(TC_3XTF32) % 1024 == 0 && tc_slot(TC_1XTF32) % 1024 == 0 && tc_slot(TC_F16X3) % 1024 == 0 &&
+              TC_B16_BYTES % 1024 == 0, "ring slots and their A stages stay 1024-byte aligned");
 static_assert(tc_ring(TC_1XTF32) + 16 * tc_stages(TC_1XTF32) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX &&
               tc_ring(TC_F16X3) + 16 * tc_stages(TC_F16X3) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX,
               "every ring fits the shared memory the core may use");
@@ -161,6 +166,10 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(x), "r"(y) : "memory");
 }
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int x, int y) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(src), "r"(x), "r"(y) : "memory");
+}
 // 16 bytes global -> shared, zero-filled when src_bytes == 0
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
@@ -170,6 +179,22 @@ __device__ __forceinline__ void cp_async_arrive(uint32_t bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// float offset of 16-byte chunk c of row r in a 128-byte-swizzled [rows][32] fp32 stage
+__device__ __forceinline__ int tc_achunk(int r, int c) { return r * TC_KS + ((c ^ (r & 7)) << 2); }
+
+// An A segment whose tile rows are contiguous in its source (identity frame map, one tap or taps that do not move the
+// row): output row r of the tile starting at frame f0 reads source row f0 J + r, so a stage is one TMA box of its
+// 128 rows (tc_launch_prec encodes the map).  Other segments are gathered per row by cp.async.
+__host__ __device__ inline bool tc_seg_tma(const ASeg& s) {
+  return s.tap_stride == 0 && s.map.T_in == s.map.T_out && s.map.t_mul == 1 && s.map.t_off == 0;
+}
+// per A segment taken by tc_seg_tma: fp32 {Kc, F J} at row stride ld, box {32, 128}, 128-byte swizzle; out: the plain
+// epilogue's output, fp32 {N, F J} at row stride ld_out, box {32, fpt J}, 128-byte swizzle
+struct TcActMaps {
+  CUtensorMap seg[3];
+  CUtensorMap out;
+};
 
 // shared-memory matrix descriptor of a no-swizzle K-major operand: core matrices 128 B apart along N (SBO),
 // 2048 B apart along K (LBO)
@@ -224,16 +249,17 @@ __device__ __forceinline__ void tc_partial(float (&d)[64], const uint32_t (&ah)[
   wgmma_commit();
 }
 
-// A fragment rows r0, r0 + 8 of the k8 steps s0, s0 + 1 of a slot's A (row stride TC_ALD), rounded to tf32 (hi) and,
-// in 3xTF32, the rounding error split off as lo
+// A fragment rows r0, r0 + 8 of the k8 steps s0, s0 + 1 of a slot's A (swizzled, tc_achunk), rounded to tf32 (hi)
+// and, in 3xTF32, the rounding error split off as lo.  k = 8 s + t sits in chunk 2 s, k + 4 in chunk 2 s + 1; the
+// warp's eight rows r0 & 7 = 0 .. 7 then spread each load over all 32 banks.
 template <int PREC>
 __device__ __forceinline__ void tc_load_a(const float* A, int r0, int t, int s0, uint32_t (&ah)[2][4],
                                           uint32_t (&al)[2][4]) {
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const int k = 8 * (s0 + i) + t;
-    const float x[4] = {A[r0 * TC_ALD + k], A[(r0 + 8) * TC_ALD + k], A[r0 * TC_ALD + k + 4],
-                        A[(r0 + 8) * TC_ALD + k + 4]};
+    const int c = 2 * (s0 + i);
+    const float x[4] = {A[tc_achunk(r0, c) + t], A[tc_achunk(r0 + 8, c) + t], A[tc_achunk(r0, c + 1) + t],
+                        A[tc_achunk(r0 + 8, c + 1) + t]};
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       ah[i][q] = tf32_bits(x[q]);
@@ -286,19 +312,22 @@ __device__ __forceinline__ void tc_scale_bounds(int sw, int& smin, int& smax) {
   smax = min(127, 126 - sw);
 }
 
-// The F16X3 A fragments of both k16 steps of a slot's A (row stride TC_ALD16): rows r0, r0 + 8 at k pairs
+// The F16X3 A fragments of both k16 steps of a slot's A (swizzled, tc_achunk): rows r0, r0 + 8 at k pairs
 // 16 s + 2t and 16 s + 2t + 8, scaled per row by 2^s_r and split into fp16 hi / lo; u0, u1 = 2^-(s_r + s_W) of the
-// two rows.  The quad's four threads hold a row's 32 values of the stage between them.
+// two rows.  The quad's four threads hold a row's 32 values of the stage between them.  k = 16 s + 2t sits in chunk
+// 4 s + t / 2 at float 2 (t & 1), k + 8 two chunks on; the swizzle spreads a warp's 64-bit loads over all 32 banks
+// in the two wavefronts 256 bytes take.
 __device__ __forceinline__ void tc_load_a16(const float* A, int r0, int t, int sw, int smin, int smax,
                                             uint32_t (&ah)[2][4], uint32_t (&al)[2][4], float& u0, float& u1) {
   float2 x[2][4];
+  const int w = 2 * (t & 1);
 #pragma unroll
   for (int s = 0; s < 2; ++s) {
-    const int k = 16 * s + 2 * t;
-    x[s][0] = *reinterpret_cast<const float2*>(A + r0 * TC_ALD16 + k);
-    x[s][1] = *reinterpret_cast<const float2*>(A + (r0 + 8) * TC_ALD16 + k);
-    x[s][2] = *reinterpret_cast<const float2*>(A + r0 * TC_ALD16 + k + 8);
-    x[s][3] = *reinterpret_cast<const float2*>(A + (r0 + 8) * TC_ALD16 + k + 8);
+    const int c = 4 * s + (t >> 1);
+    x[s][0] = *reinterpret_cast<const float2*>(A + tc_achunk(r0, c) + w);
+    x[s][1] = *reinterpret_cast<const float2*>(A + tc_achunk(r0 + 8, c) + w);
+    x[s][2] = *reinterpret_cast<const float2*>(A + tc_achunk(r0, c + 2) + w);
+    x[s][3] = *reinterpret_cast<const float2*>(A + tc_achunk(r0 + 8, c + 2) + w);
   }
   float m[2] = {0.f, 0.f};
 #pragma unroll
@@ -345,13 +374,63 @@ __device__ __forceinline__ void tc_tile(const GemmP& p, int& rt, int& ctile) {
   ctile = (int)b - rt * col_tiles;
 }
 
-// mlo is not read in 1xTF32, sw (s_W) only in F16X3
+// EPI_PLAIN on the consumers' wgmma fragments (rows r0, r0 + 8; columns 8 i + 2t, + 1 in acc[4 i ..]): bias, ReLU and
+// residual in gemm_epilogue's order, so the bits are the same, then the tile goes through the free ring to TMA as four
+// 128-byte-swizzled column blocks of 32 floats ([128][32] each, 16 KB apart), and one thread stores them with `out`
+// (tile rows f0 J .. f0 J + fpt J - 1 of the box; the map's dims drop rows past F J and columns past N).
+__device__ __forceinline__ void tc_store_plain(const GemmP& p, const float (&acc)[64], unsigned char* ring,
+                                               uint32_t rb, const CUtensorMap& out, int r0, int t, int ct, int f0,
+                                               int vrows, int n0) {
+  const int J = p.J;
+  const float* resrow[2] = {nullptr, nullptr};
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + 8 * h;
+    if (p.res && r < vrows) {
+      const int fr = r / J, j = r - fr * J;
+      resrow[h] = p.res + (map_frame(p.res_map, f0 + fr) * J + j) * (long long)p.res_ld;
+    }
+  }
+  float* S = reinterpret_cast<float*>(ring);
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const int col = 8 * i + 2 * t, n = n0 + col;
+    const bool in = n < p.N;                                            // N % 4 == 0: n + 1 < N too
+    float2 b = make_float2(0.f, 0.f);
+    if (p.bias && in) b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+      if (p.bias) { v0 += b.x; v1 += b.y; }
+      if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      if (resrow[h] && in) {
+        const float2 rr = __ldg(reinterpret_cast<const float2*>(resrow[h] + n));
+        v0 += rr.x; v1 += rr.y;
+      }
+      const int r = r0 + 8 * h;
+      *reinterpret_cast<float2*>(S + (i >> 2) * (TC_BM * TC_KS) + tc_achunk(r, col >> 2 & 7) + (col & 3)) =
+          make_float2(v0, v1);
+    }
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // the writes above, seen by the TMA engine
+  epi_sync();
+  if (ct == 0) {
+    for (int cb = 0; cb < TC_BN / TC_KS && n0 + cb * TC_KS < p.N; ++cb)
+      tma_store_2d(&out, rb + cb * TC_A_BYTES, n0 + cb * TC_KS, f0 * J);
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the ring may go once the engine has read it
+  }
+}
+
+// mlo is not read in 1xTF32, sw (s_W) only in F16X3, am.seg[s] only for the segments tc_seg_tma takes, am.out only in
+// EPI_PLAIN
 template <int EPI, int PREC>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensorMap mhi,
-               const __grid_constant__ CUtensorMap mlo, const int* __restrict__ sw) {
+               const __grid_constant__ CUtensorMap mlo, const __grid_constant__ TcActMaps am,
+               const int* __restrict__ sw) {
   constexpr int STAGES = tc_stages(PREC), SLOT = tc_slot(PREC), NB = tc_nb(PREC);
-  constexpr int BBYTES = tc_bbytes(PREC), ALD = tc_ald(PREC);
+  constexpr int BBYTES = tc_bbytes(PREC);
   constexpr int KSH = PREC == TC_F16X3 ? 3 : 2;                         // log2 of the k's per 16-byte row of a B copy
   extern __shared__ __align__(16) unsigned char smem_raw[];
   long long* rowbase = reinterpret_cast<long long*>(smem_raw);          // [3][128]
@@ -369,10 +448,13 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   const int nf = min(p.fpt, p.F - f0);
   const int vrows = nf * J;
   const int n0 = ctile * TC_BN;
+  int tma_segs = 0;                                                     // bit s: segment s is loaded by TMA
+  for (int s = 0; s < p.nseg; ++s) tma_segs |= tc_seg_tma(p.seg[s]) << s;
+  const bool gather = tma_segs != (1 << p.nseg) - 1;                    // some segment is gathered per row
 
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full0 + 8 * s, 1 + 128);
+      mbar_init(full0 + 8 * s, gather ? 1 + 128 : 1);
       mbar_init(empty0 + 8 * s, 8);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -396,27 +478,35 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   if (warp < 4) {
     // producer: stage c into ring slot c % STAGES once both consumers have released the slot's previous stage
     setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (!gather && tid != 0) return;                                    // the elected thread issues every stage
     const int q = tid & 7, rq = tid >> 3;                               // k-quad q of rows rq + 16 i
+    const uint32_t adst = NB * BBYTES + 4 * tc_achunk(rq, q);           // its slot offset in row rq; rows + 16 i follow
+    const int row0 = f0 * J;                                            // source row of tile row 0 (TMA segments)
     int seg = 0, k0 = 0, kcol = 0, tap = 0, kin = 0;                    // stage start: segment, K in it, W column, tap
     for (int c = 0; c < nstages; ++c) {
       const int slot = c % STAGES;
       if (c >= STAGES) mbar_wait(empty0 + 8 * slot, (c / STAGES - 1) & 1);
       const uint32_t sb = rb + slot * SLOT, full = full0 + 8 * slot;
+      const bool tma_a = (tma_segs >> seg) & 1;
       if (tid == 0) {
-        mbar_arrive_expect_tx(full, NB * BBYTES);
+        mbar_arrive_expect_tx(full, NB * BBYTES + (tma_a ? TC_A_BYTES : 0));
         const int kq = (kcol + k0) >> KSH;
         tma_load_2d(sb, &mhi, full, 2 * n0, kq);
         if (NB == 2) tma_load_2d(sb + BBYTES, &mlo, full, 2 * n0, kq);
+        if (tma_a) tma_load_2d(sb + NB * BBYTES, &am.seg[seg], full, kin, row0);
       }
       const ASeg& sg = p.seg[seg];
-      const float* src = sg.base + tap * sg.tap_stride + kin + q * 4;
+      if (tma_a) {
+        if (gather) mbar_arrive(full);                                  // the barrier counts 128 producer arrivals
+      } else {
+        const float* src = sg.base + tap * sg.tap_stride + kin + q * 4;
 #pragma unroll
-      for (int i = 0; i < TC_BM / 16; ++i) {
-        const int r = rq + 16 * i;
-        const long long off = rowbase[seg * 128 + r];
-        cp_async16(sb + NB * BBYTES + (r * ALD + q * 4) * 4, off >= 0 ? src + off : sg.base, off >= 0 ? 16 : 0);
+        for (int i = 0; i < TC_BM / 16; ++i) {
+          const long long off = rowbase[seg * 128 + rq + 16 * i];
+          cp_async16(sb + adst + i * 16 * 128, off >= 0 ? src + off : sg.base, off >= 0 ? 16 : 0);
+        }
+        cp_async_arrive(full);
       }
-      cp_async_arrive(full);
       k0 += TC_KS;
       kin += TC_KS;
       if (kin == sg.Kc) { kin = 0; ++tap; }
@@ -478,6 +568,10 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   tc_tile(p, rt, ctile);
   const int fe = rt * p.fpt, nfe = min(p.fpt, p.F - fe);
 
+  if constexpr (EPI == EPI_PLAIN) {
+    tc_store_plain(p, acc, ring, rb, am.out, r0, t, ct, fe, nfe * J, ctile * TC_BN);
+    return;
+  }
   // hand the tile over in the FFMA thread layout the shared epilogues expect
   float* S = reinterpret_cast<float*>(ring);   // [128][TC_STG_LD]
 #pragma unroll
@@ -555,6 +649,21 @@ inline tc_encode_fn tc_get_encode() {
       fn = reinterpret_cast<tc_encode_fn>(q);
   }
   return fn;
+}
+
+// fp32 [rows][cols] at row stride ld floats, box {32, box_rows} (128-byte rows), 128-byte swizzle; reads past the
+// dims fill zeros, writes past them are dropped
+inline int tc_encode_rows(CUtensorMap* m, const float* base, int cols, long long rows, int ld, int box_rows) {
+  tc_encode_fn enc = tc_get_encode();
+  if (!enc) return -1;
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+  const cuuint32_t box[2] = {(cuuint32_t)TC_KS, (cuuint32_t)box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : -1;
 }
 
 // W: [N][K] fp32 K-major (device).  Allocates the copies once per shape and form, encodes their TMA maps and splits W
@@ -649,9 +758,16 @@ inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeig
   }
   const CUtensorMap& mhi = PREC == TC_F16X3 ? t.map_h16hi : t.map_hi;
   const CUtensorMap& mlo = PREC == TC_F16X3 ? t.map_h16lo : t.map_lo;
-  if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, t.sw);
-  else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, t.sw);
-  else gemm_tc_kernel<EPI_GLOBAL, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, t.sw);
+  // the activation maps follow the pointers, so they are encoded per launch (graph capture keeps them by value)
+  TcActMaps am{};
+  const long long rows = (long long)p.F * p.J;
+  for (int s = 0; s < p.nseg; ++s)
+    if (tc_seg_tma(p.seg[s]) && tc_encode_rows(&am.seg[s], p.seg[s].base, p.seg[s].Kc, rows, p.seg[s].ld, TC_BM))
+      return -1;
+  if (epi == EPI_PLAIN && tc_encode_rows(&am.out, p.out, p.N, rows, p.ld_out, p.fpt * p.J)) return -1;
+  if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw);
+  else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw);
+  else gemm_tc_kernel<EPI_GLOBAL, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw);
   return (int)cudaGetLastError();
 }
 
