@@ -116,6 +116,11 @@ struct gast_handle {
   int fpt = 0;
   int sm_count = 132;
   float* loss_scratch = nullptr;   // shrink+mpjpe: SHL_MAXBLOCKS double partials | ticket (zero-initialised, reset by the kernel)
+  // test-only GEMM audit (gast_debug_set_gemm_audit): called around every launch_gemm outside graph capture
+  gast_gemm_audit_fn audit_fn = nullptr;
+  void* audit_user = nullptr;
+  long long audit_index = 0;
+  long long audit_skips = 0;
 };
 
 constexpr int GAST_MAX_PENDING_TRAIN = 16;   // training forwards that may wait for their backward per handle
@@ -659,16 +664,42 @@ static void gemm_defaults(GemmP& p, const gast_handle* h, long long F) {
 // F*J "frames" of one joint, so that every tile carries 128 rows instead of floor(128/J)*J (119 for J=17).
 static void gemm_defaults_flat(GemmP& p, const gast_handle* h, long long F) { gemm_flat(p, F * h->cfg.num_joints); }
 
-static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p, const TcWeights* tcw) {
-  if (p.F <= 0) return 0;
-  int Ktot = 0;
-  for (int s = 0; s < p.nseg; ++s) Ktot += p.seg[s].K;
-  if (Ktot != p.ldw) return fail("internal: K mismatch %d vs %d", Ktot, p.ldw);
-  if (p.N % 4 || p.ld_out % 4) return fail("internal: N/ld_out must be multiples of 4");
-  if (h->gemm_core == 0 && tcw && tc_supported(p, epi, *tcw)) {
+// the audit record of a launch (gast_gemm_audit mirrors GemmP); prec < 0: the FFMA core
+static void gemm_audit_record(const gast_handle* h, int epi, const GemmP& p, int prec, gast_gemm_audit* d) {
+  memset(d, 0, sizeof(*d));
+  d->index = h->audit_index;
+  d->epi = epi;
+  d->core = prec < 0 ? 1 : 0;
+  d->tc_form = prec;
+  d->nseg = p.nseg;
+  for (int s = 0; s < p.nseg; ++s) {
+    const ASeg& a = p.seg[s];
+    d->seg[s] = gast_gemm_audit_seg{a.base, a.tap_stride, a.ld, a.K, a.Kc, a.map.T_out, a.map.T_in, a.map.t_mul, a.map.t_off};
+    if (prec >= 0 && tc_seg_tma(a)) d->tma_mask |= 1 << s;
+  }
+  d->W = p.W; d->ldw = p.ldw; d->N = p.N; d->F = p.F; d->J = p.J; d->fpt = p.fpt; d->ld_out = p.ld_out;
+  d->out = p.out; d->bias = p.bias; d->relu = p.relu; d->res = p.res; d->res_ld = p.res_ld;
+  d->res_T_out = p.res_map.T_out; d->res_T_in = p.res_map.T_in; d->res_t_mul = p.res_map.t_mul; d->res_t_off = p.res_map.t_off;
+  d->coef[0] = p.coef[0]; d->coef[1] = p.coef[1]; d->shift = p.shift; d->C = p.C; d->tiles_per_mask = p.tiles_per_mask;
+  for (int m = 0; m < 2; ++m) {
+    memcpy(d->nbr_row_ptr[m], p.nbr[m].row_ptr, sizeof(d->nbr_row_ptr[m]));
+    memcpy(d->nbr_col[m], p.nbr[m].col, sizeof(d->nbr_col[m]));
+  }
+  d->ab = p.ab; d->ck = p.ck; d->bg = p.bg; d->heads = p.heads; d->Cg = p.Cg;
+}
+
+static int gemm_audit_call(gast_handle* h, cudaStream_t st, int phase, const gast_gemm_audit& d) {
+  CUDA_OK(cudaStreamSynchronize(st));
+  if (h->audit_fn(phase, &d, h->audit_user))
+    return fail("GEMM audit rejected launch %lld (epi %d, core %d, form %d, F %d J %d N %d K %d) %s", (long long)d.index,
+                d.epi, d.core, d.tc_form, d.F, d.J, d.N, d.ldw, phase ? "after it ran" : "before it ran");
+  return 0;
+}
+
+static int launch_gemm_core(gast_handle* h, cudaStream_t st, int epi, const GemmP& p, const TcWeights* tcw, int prec) {
+  if (prec >= 0) {
     TimedLaunch tl(h, st, LK_TC_PLAIN + epi);
-    // training's operand copies (train_tcw, the only ones without the fp16 pair) run at the training precision
-    int rc = tc_launch(st, epi, p, *tcw, tc_prec(*tcw, tcw->f16 ? h->precision : h->train_precision));
+    int rc = tc_launch(st, epi, p, *tcw, prec);
     if (rc) return fail("tensor-core gemm launch failed: %s", cudaGetErrorString((cudaError_t)rc));
     h->launches++;
     h->tc_launches++;
@@ -694,6 +725,38 @@ static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p,
   h->launches++;
   return 0;
 }
+
+static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p, const TcWeights* tcw) {
+  if (p.F <= 0) return 0;
+  int Ktot = 0;
+  for (int s = 0; s < p.nseg; ++s) Ktot += p.seg[s].K;
+  if (Ktot != p.ldw) return fail("internal: K mismatch %d vs %d", Ktot, p.ldw);
+  if (p.N % 4 || p.ld_out % 4) return fail("internal: N/ld_out must be multiples of 4");
+  // training's operand copies (train_tcw, the only ones without the fp16 pair) run at the training precision
+  const int prec = (h->gemm_core == 0 && tcw && tc_supported(p, epi, *tcw))
+                       ? tc_prec(*tcw, tcw->f16 ? h->precision : h->train_precision) : -1;
+  if (!h->audit_fn) return launch_gemm_core(h, st, epi, p, tcw, prec);
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CUDA_OK(cudaStreamIsCapturing(st, &cs));
+  if (cs != cudaStreamCaptureStatusNone) {
+    h->audit_skips++;
+    return launch_gemm_core(h, st, epi, p, tcw, prec);
+  }
+  gast_gemm_audit d;
+  gemm_audit_record(h, epi, p, prec, &d);
+  h->audit_index++;
+  if (gemm_audit_call(h, st, 0, d) || launch_gemm_core(h, st, epi, p, tcw, prec)) return 1;
+  return gemm_audit_call(h, st, 1, d);
+}
+
+extern "C" int gast_debug_set_gemm_audit(gast_t* h, gast_gemm_audit_fn fn, void* user) {
+  if (!h) return fail("gast_debug_set_gemm_audit: null handle");
+  h->audit_fn = fn;
+  h->audit_user = user;
+  return 0;
+}
+
+extern "C" int64_t gast_debug_gemm_audit_skips(const gast_t* h) { return h ? h->audit_skips : -1; }
 
 static int launch_rowdot(gast_handle* h, cudaStream_t st, const float* X, int ldx, const BlockConsts& b,
                          float* ab, long long rows) {

@@ -728,6 +728,8 @@ inline int tc_prepare_weights(TcWeights& t, const float* W, int N, int K, cudaSt
 // The shapes the core takes are the same in every precision (each ring is no larger than the bound below).
 inline bool tc_supported(const GemmP& p, int epi, const TcWeights& t) {
   if (!t.ready || t.K != p.ldw || t.N < p.N || p.N % 4) return false;
+  // the plain epilogue's tensor store: the output map needs a 16-byte-aligned base and a row stride of 16-byte units
+  if ((reinterpret_cast<uintptr_t>(p.out) & 15) || p.ld_out % 4) return false;
   for (int s = 0; s < p.nseg; ++s) {
     const ASeg& sg = p.seg[s];
     if (sg.K % TC_KS || sg.Kc % TC_KS || sg.ld % 4 || sg.tap_stride % 4) return false;

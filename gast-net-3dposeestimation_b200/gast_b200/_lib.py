@@ -18,7 +18,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_receptive_field', 'gast_workspace_bytes', 'gast_forward', 'gast_forward_mpjpe',
            'gast_last_launch_count', 'gast_last_tc_launch_count', 'gast_set_timing',
            'gast_get_timings', 'gast_set_gemm_core', 'gast_set_precision', 'gast_set_train_precision',
-           'gast_last_wgrad_tc_launch_count', 'gast_debug_gemm', 'gast_debug_wgrad', 'gast_bind_grads',
+           'gast_last_wgrad_tc_launch_count', 'gast_debug_gemm', 'gast_debug_wgrad', 'gast_debug_set_gemm_audit',
+           'gast_debug_gemm_audit_skips', 'gast_bind_grads',
            'gast_train_workspace_bytes', 'gast_forward_train', 'gast_backward', 'gast_backward_input',
            'gast_eval_backward_workspace_bytes', 'gast_eval_backward', 'gast_chunked_workspace_bytes',
            'gast_forward_chunked', 'gast_eval_backward_chunked', 'gast_set_dropout_state', 'gast_tta_prepare', 'gast_tta_merge',
@@ -47,6 +48,28 @@ class GastCfg(C.Structure):
         ('device', C.c_int32),
     ]
 
+
+class GemmAuditSeg(C.Structure):
+    """gast_gemm_audit_seg: one K-segment of a GEMM launch's A operand"""
+    _fields_ = [('base', C.c_void_p), ('tap_stride', C.c_int64), ('ld', C.c_int32), ('K', C.c_int32),
+                ('Kc', C.c_int32), ('T_out', C.c_int32), ('T_in', C.c_int32), ('t_mul', C.c_int32),
+                ('t_off', C.c_int32)]
+
+
+class GemmAudit(C.Structure):
+    """gast_gemm_audit: what one GEMM launch receives (gast_debug_set_gemm_audit)"""
+    _fields_ = [('index', C.c_int64), ('epi', C.c_int32), ('core', C.c_int32), ('tc_form', C.c_int32),
+                ('tma_mask', C.c_int32), ('nseg', C.c_int32), ('seg', GemmAuditSeg * 3), ('W', C.c_void_p),
+                ('ldw', C.c_int32), ('N', C.c_int32), ('F', C.c_int32), ('J', C.c_int32), ('fpt', C.c_int32),
+                ('ld_out', C.c_int32), ('out', C.c_void_p), ('bias', C.c_void_p), ('relu', C.c_int32),
+                ('res_ld', C.c_int32), ('res', C.c_void_p), ('res_T_out', C.c_int32), ('res_T_in', C.c_int32),
+                ('res_t_mul', C.c_int32), ('res_t_off', C.c_int32), ('coef', C.c_void_p * 2), ('shift', C.c_void_p),
+                ('C', C.c_int32), ('tiles_per_mask', C.c_int32), ('nbr_row_ptr', (C.c_uint8 * 36) * 2),
+                ('nbr_col', (C.c_uint8 * 164) * 2), ('ab', C.c_void_p), ('ck', C.c_void_p), ('bg', C.c_void_p),
+                ('heads', C.c_int32), ('Cg', C.c_int32)]
+
+
+GemmAuditFn = C.CFUNCTYPE(C.c_int32, C.c_int32, C.POINTER(GemmAudit), C.c_void_p)
 
 _lib = None
 
@@ -102,6 +125,10 @@ def load():
     lib.gast_debug_wgrad.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                      C.POINTER(C.c_float), vp]
     lib.gast_debug_wgrad.restype = C.c_int
+    lib.gast_debug_set_gemm_audit.argtypes = [vp, GemmAuditFn, vp]
+    lib.gast_debug_set_gemm_audit.restype = C.c_int
+    lib.gast_debug_gemm_audit_skips.argtypes = [vp]
+    lib.gast_debug_gemm_audit_skips.restype = C.c_int64
     lib.gast_bind_grads.argtypes = [vp, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(vp), C.POINTER(C.c_int64)]
     lib.gast_bind_grads.restype = C.c_int
     lib.gast_train_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32, C.c_float]

@@ -517,6 +517,55 @@ int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32
 int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int32_t M, int32_t N, int32_t K,
                      int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream);
 
+/* Test-only audit of every GEMM launch a handle makes (forward, training, gradients, chunked calls, streams).
+ * A plain-C mirror of the launch's parameters: the rows of A come from up to three K-segments, output row
+ * f J + j of segment s reading source row (map_s(f) J + j) at base_s + row ld_s + tap tap_stride_s + c for column
+ * tap Kc_s + c of the segment, map(f) = (f / T_out) T_in + (f % T_out) t_mul + t_off.  W is [N][ldw] K-major, the
+ * output [F J][ld_out].  epi 0 (plain): relu?(A W^T + bias) + res[(res_map(f) J + j) res_ld]; 1 (SemCH): per 128
+ * columns of W (mask = tile / tiles_per_mask), 64 self and 64 neighbour products mixed over nbr[mask] with coef
+ * [nnz][C] and shift [2][C] into columns mask C + c; 2 (global attention): softmax over joints of
+ * LeakyReLU_0.2(ab[i, 2h] + ab[j, 2h + 1]) + ck[h][i][j] mixing G = A W^T + bg, head h = column / Cg. */
+typedef struct gast_gemm_audit_seg {
+  const float* base;
+  int64_t tap_stride;                    /* floats added per tap */
+  int32_t ld, K, Kc;                     /* row stride, columns (taps * Kc), columns per tap */
+  int32_t T_out, T_in, t_mul, t_off;     /* frame map */
+} gast_gemm_audit_seg;
+
+typedef struct gast_gemm_audit {
+  int64_t index;                         /* running index of the handle's audited launches */
+  int32_t epi;                           /* 0 plain, 1 SemCH, 2 global attention */
+  int32_t core;                          /* the core that runs: 0 tensor cores, 1 FFMA */
+  int32_t tc_form;                       /* tensor cores: 0 3xTF32, 1 1xTF32, 2 F16X3; FFMA: -1 */
+  int32_t tma_mask;                      /* tensor cores: bit s set when segment s is fed by TMA */
+  int32_t nseg;
+  gast_gemm_audit_seg seg[3];
+  const float* W;
+  int32_t ldw, N, F, J, fpt, ld_out;
+  float* out;
+  const float* bias;
+  int32_t relu, res_ld;
+  const float* res;
+  int32_t res_T_out, res_T_in, res_t_mul, res_t_off;
+  const float* coef[2];                  /* SemCH */
+  const float* shift;
+  int32_t C, tiles_per_mask;
+  uint8_t nbr_row_ptr[2][36];            /* neighbours of joint i: nbr_col[m][row_ptr[m][i] .. row_ptr[m][i + 1]) */
+  uint8_t nbr_col[2][164];
+  const float* ab;                       /* global attention */
+  const float* ck;
+  const float* bg;
+  int32_t heads, Cg;
+} gast_gemm_audit;
+
+/* fn(0, d, user) runs just before a launch and fn(1, d, user) just after it, the stream synchronised before each
+ * call, so that fn may read every operand and the output.  A non-zero return fails the call.  fn == NULL turns the
+ * audit off; a launch into a stream under CUDA-graph capture is not audited and is counted instead
+ * (gast_debug_gemm_audit_skips). */
+typedef int (*gast_gemm_audit_fn)(int32_t phase, const gast_gemm_audit* d, void* user);
+int gast_debug_set_gemm_audit(gast_t* h, gast_gemm_audit_fn fn, void* user);
+int64_t gast_debug_gemm_audit_skips(const gast_t* h);
+
 const char* gast_last_error(void);
 const char* gast_version(void);
 

@@ -5,6 +5,7 @@ own frames.
 
 - gast_debug_gemm in each precision with an output buffer longer than M: the rows after M keep their NaN sentinels,
   and the result is within the form's emulation and fp64 bars, bitwise equal between two runs;
+- an output 4, 8 or 12 bytes into a buffer, which the tensor store's map cannot take: refused before any launch;
 - a SpatioTemporalModel at J = 17 (119-row frame tiles, several per GEMM; identity-map layers fed by TMA, the stage
   convolutions gathered per row): the tensor-core forward matches the FFMA core's to the parity bar and is bitwise
   equal between two runs."""
@@ -57,6 +58,23 @@ def test_rows_past_m_untouched(prec, M, N, K):
     rel = lambda ref: float(np.linalg.norm(y - ref) / np.linalg.norm(ref))
     assert rel(emu) < 2e-6, (prec, M, N, K, rel(emu))
     assert rel(exact) < (2e-3 if prec == 'tf32' else 2e-6), (prec, M, N, K, rel(exact))
+
+
+@pytest.mark.parametrize('offset', [4, 8, 12])
+@pytest.mark.parametrize('prec', list(MODES))
+def test_unaligned_output_refused_up_front(prec, offset):
+    """the plain store's tensor map needs a 16-byte-aligned output: the tensor-core core does not take an output 4, 8
+    or 12 bytes into a buffer (tc_supported), so the call is refused before any launch and the buffer is untouched"""
+    lib = _lib.load()
+    M, N, K = 300, 36, 64
+    a = torch.ones((M, K), dtype=torch.float32, device='cuda')
+    w = torch.ones((N, K), dtype=torch.float32, device='cuda')
+    o = torch.full((M * N + 8,), float('nan'), dtype=torch.float32, device='cuda')
+    rc = lib.gast_debug_gemm(a.data_ptr(), w.data_ptr(), o.data_ptr() + offset, M, N, K, 0, MODES[prec], 0, None,
+                             torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    assert rc != 0 and 'not supported by the tensor-core core' in _lib.last_error(), _lib.last_error()
+    assert torch.isnan(o).all()
 
 
 def _adj(J):
