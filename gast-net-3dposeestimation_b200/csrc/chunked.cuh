@@ -1,6 +1,8 @@
-// Chunked eval-mode forward and backward: a call covers its (clip, output frame) grid in passes of at most
-// `max_frames` output positions, so its workspace depends on max_frames and the architecture, not on B or T.
-// Included by gast_api.cu after the eval backward (uses its planning, sizing and the training path of train.cuh).
+// Eval-mode backward and chunked eval-mode forward: a call covers its (clip, output frame) grid in passes of at most
+// `max_frames` output positions, so its workspace depends on max_frames and the architecture, not on B or T; the
+// unchunked eval backward is the one-pass plan (WHOLE_CALL).  A backward pass recomputes the activations from x with a
+// frozen-BatchNorm training forward, then runs the training backward; nothing is held between the inference forward
+// and the backward.  Included by gast_api.cu after train.cuh (uses its planning, sizing and training path).
 //
 // Under frozen BatchNorm every output position depends on its own receptive field only, so a pass is an ordinary
 // call on a slice: whole clips when a clip's output fits a pass, else a window of output frames of one clip and the
@@ -10,6 +12,15 @@
 #pragma once
 
 constexpr int GRAD_ADD_CHUNK = 4096;
+
+// max_frames of the one-pass plan, which no public entry can pass: B * T_out may exceed INT32_MAX
+constexpr long long WHOLE_CALL = LLONG_MAX;
+
+static TrainState eval_state(int strided_now) {
+  TrainState ts;
+  ts.frozen = true; ts.sn = strided_now ? 1 : 0;
+  return ts;
+}
 
 // dst[i] += src[i] over every chunk of a table of 3 int64 per chunk: {dst ptr, src ptr, count <= GRAD_ADD_CHUNK}.
 // One block per chunk, so all parameter gradients of a pass are added in one launch.
@@ -57,10 +68,10 @@ static ChunkPass chunk_pass(const ChunkPlan& pl, int B, int T, long long p) {
   return q;
 }
 
-static int chunk_plan(const gast_handle* h, const char* who, int B, int T, int strided_now, int max_frames,
+static int chunk_plan(const gast_handle* h, const char* who, int B, int T, int strided_now, long long max_frames,
                       ChunkPlan* pl) {
   if (h->cfg.kind != GAST_KIND_MODEL) return fail("%s: only the MODEL kind is chunked", who);
-  if (max_frames < 1) return fail("%s: max_frames must be at least 1 (got %d)", who, max_frames);
+  if (max_frames < 1) return fail("%s: max_frames must be at least 1 (got %lld)", who, max_frames);
   if (B <= 0 || T <= 0) return fail("%s: empty batch (B=%d T=%d)", who, B, T);
   Geometry g;
   if (geometry(h, T, strided_now, &g)) return 1;
@@ -70,11 +81,11 @@ static int chunk_plan(const gast_handle* h, const char* who, int B, int T, int s
   pl->rf = gast_receptive_field(h);
   pl->windows = g.T_out > max_frames;
   if (!pl->windows) {
-    pl->clips = std::min(B, max_frames / g.T_out);
-    pl->passes = (B + pl->clips - 1) / pl->clips;
+    pl->clips = (int)std::min<long long>(B, max_frames / g.T_out);
+    pl->passes = ((long long)B + pl->clips - 1) / pl->clips;
   } else {
-    pl->K = max_frames;
-    pl->wpc = (g.T_out + max_frames - 1) / max_frames;
+    pl->K = (int)max_frames;
+    pl->wpc = (int)((g.T_out + max_frames - 1) / max_frames);
     pl->passes = (long long)B * pl->wpc;
   }
   // a window is an ordinary call whose output is exactly its k frames: check the full and the last one
@@ -92,8 +103,8 @@ static void chunk_full(const ChunkPlan& pl, int T, int* nb, int* Tin) {
   *Tin = pl.windows ? (pl.K - 1) * pl.S + pl.rf : T;
 }
 
-// The backward's own area at the start of the workspace: the chunk table and a pass-gradient buffer per gradient
-// tensor (with parameter gradients), and one window's dL/dx (windows).  The passes' arena follows it.
+// The backward's own area at the start of the workspace, taken by a plan of several passes only: the chunk table and a
+// pass-gradient buffer per gradient tensor (with parameter gradients), and one window's dL/dx (windows).
 struct ChunkArea {
   long long* table = nullptr;
   int n_chunks = 0;
@@ -103,6 +114,7 @@ struct ChunkArea {
 
 static void chunk_area(Arena& a, const std::vector<std::pair<std::string, int64_t>>& asked, const ChunkPlan& pl,
                        int T, int Fin_J, ChunkArea* ca) {
+  if (pl.passes == 1) return;               // no area (a plan with windows has two passes at least)
   ca->n_chunks = 0;
   for (const auto& k : asked) ca->n_chunks += (int)((k.second + GRAD_ADD_CHUNK - 1) / GRAD_ADD_CHUNK);
   ca->table = reinterpret_cast<long long*>(a.take((size_t)6 * ca->n_chunks));
@@ -113,13 +125,13 @@ static void chunk_area(Arena& a, const std::vector<std::pair<std::string, int64_
   if (pl.windows) ca->dxw = a.take((size_t)Tin * Fin_J);
 }
 
-// Workspace of a chunked backward, by the sizing pass of its largest pass; 0 on error.  `asked` receives the gradient
-// buffers that pass looks up, and `dry` its lookups for the caller to refuse on.
+// Workspace of an eval backward, by the sizing pass of its largest pass; 0 on error.  With several passes `asked`
+// receives the gradient buffers that pass looks up; `dry` keeps its lookups for the caller to refuse on.
 static size_t chunked_backward_sizing(gast_handle* h, TCtx& dry, int B, int T, int strided_now, const ChunkPlan& pl,
                                       std::vector<std::pair<std::string, int64_t>>* asked) {
   int nb, Tin;
   chunk_full(pl, T, &nb, &Tin);
-  dry.grad_bufs.asked = asked;
+  if (pl.passes > 1) dry.grad_bufs.asked = asked;
   const size_t pass = train_sizing(dry, nb, Tin, eval_state(strided_now));
   if (pass == 0) return 0;
   Arena a = sizing_arena();
@@ -128,20 +140,28 @@ static size_t chunked_backward_sizing(gast_handle* h, TCtx& dry, int B, int T, i
   return a.off + pass;
 }
 
-extern "C" size_t gast_chunked_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now, int32_t max_frames,
-                                               int32_t with_backward) {
-  if (!h) return 0;
+// The workspace query of an eval backward with parameter gradients, planned with `max_frames`: 0 when refused
+static size_t eval_backward_workspace(gast_handle* h, const char* who, int B, int T, int strided_now,
+                                      long long max_frames) {
   ChunkPlan pl;
-  if (chunk_plan(h, "gast_chunked_workspace_bytes", B, T, strided_now, max_frames, &pl)) return 0;
-  if (!with_backward) {
-    int nb, Tin;
-    chunk_full(pl, T, &nb, &Tin);
-    return gast_workspace_bytes(h, nb, Tin, strided_now);
-  }
-  if (train_check(h, "gast_chunked_workspace_bytes")) return 0;
+  if (!h || train_check(h, who) || chunk_plan(h, who, B, T, strided_now, max_frames, &pl)) return 0;
   TCtx dry(h, nullptr, sizing_arena(), true);
   std::vector<std::pair<std::string, int64_t>> asked;
   return chunked_backward_sizing(h, dry, B, T, strided_now, pl, &asked);
+}
+
+extern "C" size_t gast_eval_backward_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now) {
+  return eval_backward_workspace(h, "gast_eval_backward_workspace_bytes", B, T, strided_now, WHOLE_CALL);
+}
+
+extern "C" size_t gast_chunked_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now, int32_t max_frames,
+                                               int32_t with_backward) {
+  if (with_backward) return eval_backward_workspace(h, "gast_chunked_workspace_bytes", B, T, strided_now, max_frames);
+  ChunkPlan pl;
+  if (!h || chunk_plan(h, "gast_chunked_workspace_bytes", B, T, strided_now, max_frames, &pl)) return 0;
+  int nb, Tin;
+  chunk_full(pl, T, &nb, &Tin);
+  return gast_workspace_bytes(h, nb, Tin, strided_now);
 }
 
 extern "C" int gast_forward_chunked(gast_t* h, const float* x, float* y, int32_t B, int32_t T, int32_t strided_now,
@@ -167,10 +187,9 @@ extern "C" int gast_forward_chunked(gast_t* h, const float* x, float* y, int32_t
   return 0;
 }
 
-extern "C" int gast_eval_backward_chunked(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads,
-                                          int32_t B, int32_t T, int32_t strided_now, int32_t max_frames, void* workspace,
-                                          size_t workspace_bytes, void* stream) {
-  const char* who = "gast_eval_backward_chunked";
+static int eval_backward(gast_handle* h, const char* who, const float* x, const float* dy, float* dx, int param_grads,
+                         int B, int T, int strided_now, long long max_frames, void* workspace, size_t workspace_bytes,
+                         void* stream) {
   if (!h) return fail("%s: null handle", who);
   if (train_check(h, who)) return 1;
   if (!x || !dy) return fail("%s: x and dy must be device pointers", who);
@@ -228,4 +247,17 @@ extern "C" int gast_eval_backward_chunked(gast_t* h, const float* x, const float
   }
   CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads, int32_t B,
+                                  int32_t T, int32_t strided_now, void* workspace, size_t workspace_bytes, void* stream) {
+  return eval_backward(h, "gast_eval_backward", x, dy, dx, param_grads, B, T, strided_now, WHOLE_CALL, workspace,
+                       workspace_bytes, stream);
+}
+
+extern "C" int gast_eval_backward_chunked(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads,
+                                          int32_t B, int32_t T, int32_t strided_now, int32_t max_frames, void* workspace,
+                                          size_t workspace_bytes, void* stream) {
+  return eval_backward(h, "gast_eval_backward_chunked", x, dy, dx, param_grads, B, T, strided_now, max_frames,
+                       workspace, workspace_bytes, stream);
 }

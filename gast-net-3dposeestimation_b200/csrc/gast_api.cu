@@ -1200,40 +1200,6 @@ extern "C" int gast_backward_input(gast_t* h, const float* dy, float* dx, int32_
   return 0;
 }
 
-// ---- eval-mode backward: a frozen-BatchNorm training forward recomputes the activations from x, then the training
-// backward runs on them.  The inference forward stays as it is; nothing is held between forward and backward.
-static TrainState eval_state(int strided_now) {
-  TrainState ts;
-  ts.frozen = true; ts.sn = strided_now ? 1 : 0;
-  return ts;
-}
-
-extern "C" size_t gast_eval_backward_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now) {
-  if (!h || train_check(h, "gast_eval_backward_workspace_bytes")) return 0;
-  TCtx c(h, nullptr, sizing_arena(), true);
-  return train_sizing(c, B, T, eval_state(strided_now));
-}
-
-extern "C" int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, int32_t param_grads, int32_t B,
-                                  int32_t T, int32_t strided_now, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h) return fail("gast_eval_backward: null handle");
-  if (train_check(h, "gast_eval_backward")) return 1;
-  if (B <= 0 || T <= 0) return fail("gast_eval_backward: empty batch (B=%d T=%d)", B, T);
-  if (!x || !dy) return fail("gast_eval_backward: x and dy must be device pointers");
-  if (!dx && !param_grads) return fail("gast_eval_backward: neither dx nor parameter gradients requested");
-  TrainState ts = eval_state(strided_now);
-  TCtx dry(h, nullptr, sizing_arena(), param_grads != 0);
-  const size_t need = train_sizing(dry, B, T, ts);
-  if (need == 0 || dry.refuse(true)) return 1;
-  if (call_begin(h, "gast_eval_backward", need, workspace, workspace_bytes)) return 1;
-  TCtx c(h, reinterpret_cast<cudaStream_t>(stream), workspace_arena(workspace, workspace_bytes), param_grads != 0);
-  if (train_forward(h, c, ts, x, nullptr, B, T)) return 1;
-  c.tc_slot = 1024;
-  if (train_backward(h, c, ts, dy, dx)) return 1;
-  CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
 #include "chunked.cuh"
 
 // Timing of the debug entries: `launch` once, then `reps` more times between two events on `st`; waits for the stream

@@ -373,27 +373,29 @@ def _bind_grad_views(handle, names, params, direct, dev):
 
 class _EvalFn(torch.autograd.Function):
     """Eval-mode forward of the whole model with a backward (model.eval(): BatchNorm on the running statistics, no
-    dropout).  The forward is the inference forward, unchanged.  The backward (gast_eval_backward) recomputes the
-    activations from the saved x with a frozen-BatchNorm training forward, then runs the training backward: nothing is
-    held on the device between the two beyond x.  x, the parameters and the running statistics are saved with
-    save_for_backward, so an in-place change to any of them before the backward raises torch's version error, as
-    it does for the reference module."""
+    dropout), whole (max_frames None) or in passes of at most max_frames output positions.  The forward is the
+    inference forward, unchanged.  The backward (gast_eval_backward, or gast_eval_backward_chunked pass by pass)
+    recomputes the activations from the saved x with a frozen-BatchNorm training forward, then runs the training
+    backward: nothing is held on the device between the two beyond x.  x, the parameters and the running statistics
+    are saved with save_for_backward, so an in-place change to any of them before the backward raises torch's version
+    error, as it does for the reference module."""
 
     @staticmethod
-    def forward(ctx, module, handle, x, strided_now, names, *params):
-        y = _eval_forward(module, handle, x, strided_now)
+    def forward(ctx, module, handle, x, strided_now, max_frames, names, *params):
+        y = _chunked_forward(module, handle, x, strided_now, max_frames)
         stats = [v for k, v in named_tensors(module) if k.endswith('.running_mean') or k.endswith('.running_var')]
         ctx.save_for_backward(x, *params, *stats)
-        ctx.module, ctx.handle, ctx.sn, ctx.names, ctx.n = module, handle, strided_now, names, len(params)
+        ctx.module, ctx.handle, ctx.sn, ctx.max_frames, ctx.names, ctx.n = (module, handle, strided_now, max_frames,
+                                                                            names, len(params))
         return y
 
     @staticmethod
     def backward(ctx, dy):
         saved = ctx.saved_tensors
         x, params = saved[0], saved[1:1 + ctx.n]
-        module, h = ctx.module, ctx.handle
+        module, h, mf = ctx.module, ctx.handle, ctx.max_frames
         need_x = ctx.needs_input_grad[2]
-        need_p = any(ctx.needs_input_grad[5:])
+        need_p = any(ctx.needs_input_grad[6:])
         dev = x.device
         B, T = int(x.shape[0]), int(x.shape[1])
         dy = dy.contiguous()
@@ -401,14 +403,20 @@ class _EvalFn(torch.autograd.Function):
             st = _stream(dev)
             h.refresh(module, st)            # binds the current storage and GEMM-core choice (no work when unchanged)
             lib = h.lib
-            need = _check_size(lib.gast_eval_backward_workspace_bytes(h.h, B, T, ctx.sn),
-                               'gast_eval_backward_workspace_bytes')
+            if mf is None:
+                need = _check_size(lib.gast_eval_backward_workspace_bytes(h.h, B, T, ctx.sn),
+                                   'gast_eval_backward_workspace_bytes')
+                entry, plan = 'gast_eval_backward', ()
+            else:
+                need = _check_size(lib.gast_chunked_workspace_bytes(h.h, B, T, ctx.sn, mf, 1),
+                                   'gast_chunked_workspace_bytes')
+                entry, plan = 'gast_eval_backward_chunked', (mf,)
             ws = torch.empty(need, dtype=torch.uint8, device=dev)
             dx = torch.empty_like(x) if need_x else None
             views = _bind_grad_views(h, ctx.names, params, False, dev) if need_p else None
-            _check(lib.gast_eval_backward(h.h, _p(x), _p(dy), _p(dx), 1 if need_p else 0, B, T, ctx.sn, _p(ws),
-                                          ws.numel(), C.c_void_p(st)), 'gast_eval_backward')
-        return (None, None, dx, None, None) + (tuple(views) if views is not None else (None,) * ctx.n)
+            _check(getattr(lib, entry)(h.h, _p(x), _p(dy), _p(dx), 1 if need_p else 0, B, T, ctx.sn, *plan, _p(ws),
+                                       ws.numel(), C.c_void_p(st)), entry)
+        return (None, None, dx, None, None, None) + (tuple(views) if views is not None else (None,) * ctx.n)
 
 
 def _no_train(module, what):
@@ -450,16 +458,20 @@ def run_model(module, x):
         np_ = named_params(module)
         y = _TrainFn.apply(module, h, x, [k for k, _ in np_], *[p for _, p in np_])
     else:
-        strided_now = _strided_now(module, int(x.shape[1]))
-        np_ = named_params(module) if torch.is_grad_enabled() else []
-        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for _, p in np_)):
-            # the reference's output would carry a grad_fn here: same forward, plus a backward
-            _fp32_only(module, 'SpatioTemporalModel.forward with autograd (requires_grad input or parameters)')
-            y = _EvalFn.apply(module, h, x, strided_now, [k for k, _ in np_], *[p for _, p in np_])
-        else:
-            y = _eval_forward(module, h, x, strided_now)
+        y = _run_eval(module, h, x, None, 'SpatioTemporalModel.forward')
     module.__dict__['_gast_last_launches'] = h.launches()
     return y
+
+
+def _run_eval(module, h, x, max_frames, what):
+    """the eval-mode forward of x, whole (max_frames None) or in passes (_chunked_forward); with a backward (_EvalFn)
+    when autograd is on and x or a parameter requires grad, where the reference's output would carry a grad_fn"""
+    strided_now = _strided_now(module, int(x.shape[1]))
+    np_ = named_params(module) if torch.is_grad_enabled() else []
+    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for _, p in np_)):
+        _fp32_only(module, '%s with autograd (requires_grad input or parameters)' % what)
+        return _EvalFn.apply(module, h, x, strided_now, max_frames, [k for k, _ in np_], *[p for _, p in np_])
+    return _chunked_forward(module, h, x, strided_now, max_frames)
 
 
 def _eval_forward(module, h, x, strided_now, target=None):
@@ -517,19 +529,16 @@ def run_model_chunked(module, x, max_frames):
         raise GastError('run_model_chunked: the model is in train mode, whose BatchNorm statistics span the whole '
                         'batch and cannot be chunked; call .eval()')
     h = model_handle(module, x.device)
-    strided_now = _strided_now(module, int(x.shape[1]))
-    np_ = named_params(module) if torch.is_grad_enabled() else []
-    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for _, p in np_)):
-        _fp32_only(module, 'run_model_chunked with autograd (requires_grad input or parameters)')
-        y = _ChunkedEvalFn.apply(module, h, x, strided_now, int(max_frames), [k for k, _ in np_], *[p for _, p in np_])
-    else:
-        y = _chunked_forward(module, h, x, strided_now, int(max_frames))
+    y = _run_eval(module, h, x, int(max_frames), 'run_model_chunked')
     module.__dict__['_gast_last_launches'] = h.launches()
     return y
 
 
 def _chunked_forward(module, h, x, strided_now, max_frames):
-    """gast_forward_chunked of x (B,T,J,F) -> y (B,T_out,J,3) on a workspace of its own"""
+    """gast_forward_chunked of x (B,T,J,F) -> y (B,T_out,J,3) on a workspace of its own; max_frames None is the whole
+    call, gast_forward on the handle's cached workspace (_eval_forward)"""
+    if max_frames is None:
+        return _eval_forward(module, h, x, strided_now)
     dev = x.device
     B, T = int(x.shape[0]), int(x.shape[1])
     with torch.cuda.device(dev):
@@ -542,44 +551,6 @@ def _chunked_forward(module, h, x, strided_now, max_frames):
         _check(h.lib.gast_forward_chunked(h.h, _p(x), _p(y), B, T, strided_now, max_frames, _p(ws), ws.numel(),
                                           C.c_void_p(st)), 'gast_forward_chunked')
     return y
-
-
-class _ChunkedEvalFn(torch.autograd.Function):
-    """_EvalFn in bounded memory: the chunked forward, and a backward (gast_eval_backward_chunked) that recomputes and
-    differentiates pass by pass.  Saves what _EvalFn saves, so an in-place change before the backward raises torch's
-    version error."""
-
-    @staticmethod
-    def forward(ctx, module, handle, x, strided_now, max_frames, names, *params):
-        y = _chunked_forward(module, handle, x, strided_now, max_frames)
-        stats = [v for k, v in named_tensors(module) if k.endswith('.running_mean') or k.endswith('.running_var')]
-        ctx.save_for_backward(x, *params, *stats)
-        ctx.module, ctx.handle, ctx.sn, ctx.max_frames, ctx.names, ctx.n = (module, handle, strided_now, max_frames,
-                                                                            names, len(params))
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        saved = ctx.saved_tensors
-        x, params = saved[0], saved[1:1 + ctx.n]
-        module, h, mf = ctx.module, ctx.handle, ctx.max_frames
-        need_x = ctx.needs_input_grad[2]
-        need_p = any(ctx.needs_input_grad[6:])
-        dev = x.device
-        B, T = int(x.shape[0]), int(x.shape[1])
-        dy = dy.contiguous()
-        with torch.cuda.device(dev):
-            st = _stream(dev)
-            h.refresh(module, st)
-            lib = h.lib
-            need = _check_size(lib.gast_chunked_workspace_bytes(h.h, B, T, ctx.sn, mf, 1),
-                               'gast_chunked_workspace_bytes')
-            ws = torch.empty(need, dtype=torch.uint8, device=dev)
-            dx = torch.empty_like(x) if need_x else None
-            views = _bind_grad_views(h, ctx.names, params, False, dev) if need_p else None
-            _check(lib.gast_eval_backward_chunked(h.h, _p(x), _p(dy), _p(dx), 1 if need_p else 0, B, T, ctx.sn, mf,
-                                                  _p(ws), ws.numel(), C.c_void_p(st)), 'gast_eval_backward_chunked')
-        return (None, None, dx, None, None, None) + (tuple(views) if views is not None else (None,) * ctx.n)
 
 
 def _run_module(module, x, what, kind, cfg, width_out, masks=None, train_ok=False):

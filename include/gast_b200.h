@@ -217,15 +217,17 @@ int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, in
 
 /* ---- the same in bounded memory: long recordings and large batches (MODEL kind) ------------------------------
  * A chunked call covers the (clip, output frame) grid of gast_forward(h, x, ..., B, T, strided_now) in passes of at
- * most max_frames output positions.  With T_out = gast_out_frames(h, T, strided_now): if T_out <= max_frames a pass
- * covers max_frames / T_out whole clips; otherwise every clip is covered by windows of max_frames output frames (the
- * last may be shorter), and the window of output frames [t0, t0 + K) reads the input frames that map to them,
- * [t0*S, t0*S + (K-1)*S + rf) with rf = gast_receptive_field(h) and S the schedule's output stride (1 dilated or
- * dense, rf strided).  Passes run clip by clip, window by window; every output position falls in exactly one.
+ * most max_frames output positions; gast_eval_backward and its workspace query are the case of one pass.  With
+ * T_out = gast_out_frames(h, T, strided_now): if T_out <= max_frames a pass covers max_frames / T_out whole clips;
+ * otherwise every clip is covered by windows of max_frames output frames (the last may be shorter), and the window
+ * of output frames [t0, t0 + K) reads the input frames that map to them, [t0*S, t0*S + (K-1)*S + rf) with
+ * rf = gast_receptive_field(h) and S the schedule's output stride (1 dilated or dense, rf strided).  Passes run clip
+ * by clip, window by window; every output position falls in exactly one.
  * gast_chunked_workspace_bytes: scratch for gast_forward_chunked (with_backward = 0) or for
  *   gast_eval_backward_chunked with parameter gradients (with_backward != 0; the input-only call needs less); 0 when
  *   the call would be refused.  It needs nothing bound.  For a fixed max_frames it does not depend on T once a clip
- *   needs windows, nor on B once one pass is full.
+ *   needs windows, nor on B once one pass is full (with_backward: once there are two passes, since a single pass is
+ *   gast_eval_backward_workspace_bytes).
  * gast_forward_chunked: y (B,T_out,J,3) is bitwise gast_forward's (a GEMM row does not depend on its tile).
  * gast_eval_backward_chunked: the contract of gast_eval_backward.  Each pass is that call's frozen-BatchNorm
  *   recompute and backward on its slice of x and dy.  Parameter gradients are WRITTEN into the buffers bound with
@@ -233,11 +235,11 @@ int gast_eval_backward(gast_t* h, const float* x, const float* dy, float* dx, in
  *   kernel adds them, in pass order.  dx (may be null) is written: a clip's windows overlap by rf - 1 input frames,
  *   so with windows dx is zeroed first and every window adds its own.  Handle kind, max_frames >= 1, B, T, the
  *   parameter and gradient bindings and the workspace size are checked before the first launch; a refused call
- *   changes no buffer.  With a single pass (max_frames >= B * T_out) the results are gast_eval_backward's, by the
- *   same kernels in the same order; with several they differ from it by summation order only.  Both repeat bit for
- *   bit where gast_eval_backward does: on the strided schedule.  On the dilated and dense schedules the taps of a
- *   temporal conv overlap and their adjoints are added with float atomics, so there either call varies in the last
- *   bits from run to run. */
+ *   changes no buffer.  With a single pass (max_frames >= B * T_out) it is gast_eval_backward: the same workspace
+ *   size, kernels and order; with several passes the results differ from it by summation order only.  Both repeat
+ *   bit for bit where gast_eval_backward does: on the strided schedule.  On the dilated and dense schedules the taps
+ *   of a temporal conv overlap and their adjoints are added with float atomics, so there either call varies in the
+ *   last bits from run to run. */
 size_t gast_chunked_workspace_bytes(gast_t* h, int32_t B, int32_t T, int32_t strided_now, int32_t max_frames,
                                     int32_t with_backward);
 int gast_forward_chunked(gast_t* h, const float* x, float* y, int32_t B, int32_t T, int32_t strided_now,

@@ -2,7 +2,7 @@
 engine.run_model_chunked) on the GPU, on both GEMM cores:
   * the forward is bitwise model(x) (dilated, causal, 19 joints, the 81-frame / 64-channel model, strided with
     T > receptive field);
-  * one pass is bitwise gast_eval_backward, for every parameter gradient and dL/dx;
+  * one pass is bitwise gast_eval_backward, for every parameter gradient and dL/dx, and asks for the same workspace;
   * several passes (windows that do not divide T_out, windows of one frame, whole-clip passes) agree with the
     unchunked call up to summation order, meet the rounding-level bars against the fp64 port at kink-free points
     (tests/kinkfree.py), and repeat bit for bit;
@@ -133,6 +133,20 @@ def test_single_pass_is_bitwise_eval_backward(strided, B, T, core):
         y1, g1 = _run(m, x, dy, mf)
         assert torch.equal(y1, y0)
         _assert_same(g1, g0, exact=strided)
+
+
+@pytest.mark.parametrize('strided,causal,B,T', [(True, False, 3, 81), (False, False, 2, 60), (False, True, 2, 60),
+                                                (False, False, 5, 27)],
+                         ids=['strided', 'dilated', 'causal', 'dilated_rf'])
+def test_single_pass_workspace_is_eval_backward_workspace(strided, causal, B, T):
+    m = _model(17, [3, 3, 3], 32, strided, causal)
+    h = engine.model_handle(m, torch.device('cuda'))
+    sn = engine._strided_now(m, T)
+    T_out = h.lib.gast_out_frames(h.h, T, sn)
+    need = h.lib.gast_eval_backward_workspace_bytes(h.h, B, T, sn)
+    assert T_out > 0 and need > 0
+    for mf in (B * T_out, B * T_out + 7):
+        assert h.lib.gast_chunked_workspace_bytes(h.h, B, T, sn, mf, 1) == need, mf
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -328,7 +342,7 @@ def test_refused_calls_change_no_buffer():
     assert not torch.all(dx == 7.0).item() and all(torch.all(b == 7.0).item() for b in bufs.values())
 
 
-def test_workspace_query_does_not_grow_with_T_or_B():
+def test_workspace_query_stops_growing_with_T_or_B():
     m = _model(17, [3, 3, 3], 32)
     with torch.no_grad():
         m(torch.from_numpy(synth.synth_input(1, 27, 17, 2, seed=1)).cuda())
@@ -338,9 +352,11 @@ def test_workspace_query_does_not_grow_with_T_or_B():
         # windows: one clip needs several passes at any of these T
         sizes = {q(h.h, 1, T, 0, 8, wb) for T in (40, 100, 1000, 100000)} | {q(h.h, 5, 1000, 0, 8, wb)}
         assert len(sizes) == 1 and 0 not in sizes, sizes
-        # whole clips (T == receptive field, strided schedule, one output each): 8 per pass
-        full = {q(h.h, B, 27, 1, 8, wb) for B in (8, 9, 100, 10000)}
-        assert len(full) == 1 and 0 not in full and q(h.h, 4, 27, 1, 8, wb) <= min(full), full
+        # whole clips (T == receptive field, strided schedule, one output each): 8 per pass.  A one-pass backward
+        # takes no pass-gradient area, so its query stops growing at two passes
+        full = {q(h.h, B, 27, 1, 8, wb) for B in ((8,) if wb == 0 else ()) + (9, 16, 100, 10000)}
+        assert len(full) == 1 and 0 not in full, full
+        assert q(h.h, 4, 27, 1, 8, wb) <= q(h.h, 8, 27, 1, 8, wb) <= min(full)
     assert q(h.h, 1, 1000, 0, 8, 0) < q(h.h, 1, 1000, 0, 8, 1)
 
 
