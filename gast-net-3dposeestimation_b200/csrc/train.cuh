@@ -3,8 +3,11 @@
 // batch-statistics BatchNorm with running-stat updates, Dropout, and the full backward down to
 // every parameter of the reference's state_dict.  Included by gast_api.cu (uses its helpers).
 //
-// Everything a backward needs is kept in the caller's workspace (bump allocation, no reuse): the
-// training batch is small (b=128 -> 19,584 / 6,528 / 2,176 rows), so memory is not the constraint.
+// Everything a backward needs is kept in the caller's workspace (bump allocation, no reuse except the one partials
+// area of the column reductions, col_reduce_area): the training batch is small (b=128 -> 19,584 / 6,528 / 2,176 rows),
+// so memory is not the constraint.  No sum depends on the order in which blocks run: the tap adjoints are gathers
+// (seg_adjoint_kernel) and the column sums are finished by their consumer in a fixed order (col_partials, col_total),
+// so every call repeats bit for bit.
 // Dense contractions run on the FFMA GEMM kernel (exact fp32); the frame-mapped operands of the
 // temporal stages are gathered exactly as in inference.  Both schedules train: the strided one of
 // SpatioTemporalModelOptimized1f (main.py:166-170) and the dilated one of SpatioTemporalModel (main.py:171-175).
@@ -26,6 +29,9 @@ struct TCtx {
   // gradient kernel, and no gradient buffer has to be bound
   bool pgrad;
   int tc_slot = 0;   // next slot of the handle's table of per-GEMM tensor-core operand copies (train_tcw)
+  // the partials area of the column reductions (TrainState::red_part), set by train_forward and train_backward; the
+  // reductions and their consumers run in stream order and share it
+  double* red_part = nullptr;
   Lookup params, grad_bufs;
   // grads: where the gradient buffers are looked up, the handle's gast_bind_grads bindings unless given (the chunked
   // eval backward points the passes after its first at its pass-gradient area)
@@ -55,7 +61,33 @@ struct TCtx {
   }
   // f() in the launch pass only: the counted launches of the inference code
   template <class F> int live(F f) { return dry ? 0 : f(); }
+  // grid of a column reduction over M rows and N columns (col_partials); its consumer takes cdiv(N, 32) blocks
+  static dim3 col_grid(long long M, int N) {
+    return dim3(cdiv(N, 32), (unsigned)std::min<long long>(COL_RED_ROWS, (M + 7) / 8));
+  }
 };
+
+// The column reductions' partials area of a training forward of B clips of T frames and of its backward: the widest
+// reduction has max(in_features, the last block's 2 x channels) columns, and none has more rows than init_bn's B*T*J.
+static void col_reduce_area(TCtx& c, TrainState& ts, int B, int T) {
+  const gast_cfg& cf = c.h->cfg;
+  const int N = std::max({cf.in_features, cf.channels << cf.num_stages, 8});
+  const long long R = TCtx::col_grid((long long)B * T * c.J, N).y;
+  ts.red_part = c.dbl((size_t)R * 2 * N);
+  c.red_part = ts.red_part;
+}
+
+// dX = the adjoint of the tap gather `sg` of F output frames (seg_adjoint_kernel): sg.base is dX, its taps are
+// sg.tap_stride / (J * sg.ld) frames apart, src holds the gathered gradient (row stride lds); plus the residual slice
+// of map rmap from rsrc (row stride ldr) when rsrc is given.  Writes every element of dX.
+static void seg_adjoint(TCtx& c, const ASeg& sg, long long F, const float* src, int lds, RowMap rmap = RowMap{1, 1, 1, 0},
+                        const float* rsrc = nullptr, int ldr = 0) {
+  const int taps = sg.K / sg.Kc;
+  const int dil = (int)(sg.tap_stride / ((long long)c.J * sg.ld));
+  const long long F_in = F / sg.map.T_out * sg.map.T_in;
+  c.launch(seg_adjoint_kernel, cdiv(F_in * c.J * sg.Kc, 256), 256, 0, sg.map, taps, dil, sg.Kc, src, lds, rmap, rsrc,
+           ldr, c.J, F_in, const_cast<float*>(sg.base), sg.ld);
+}
 
 // Tensor-core operand copies of one training GEMM's weight matrix (forward: the raw weights, backward: their transposes):
 // the weights change every step, so the hi/lo split runs per call; buffers live in a per-handle table indexed by the
@@ -171,7 +203,6 @@ static int bn_fwd(TCtx& c, BnSave& s, const std::string& prefix, const float* Z,
                   float drop_p, TrainState& ts, const float* res, int ldres, RowMap rmap, float* Y, int ldy) {
   s.prefix = prefix; s.Z = Z; s.ldz = ldz; s.M = M; s.N = N; s.relu = relu; s.frozen = ts.frozen;
   s.mean = c.fl(N); s.invstd = c.fl(N);
-  double* sums = ts.frozen ? nullptr : c.dbl(2 * (size_t)N);
   if (ts.frozen) drop_p = 0.f;   // eval semantics whatever the module's dropout
   unsigned char* keep = nullptr;
   s.kscale = 1.f;
@@ -183,10 +214,9 @@ static int bn_fwd(TCtx& c, BnSave& s, const std::string& prefix, const float* Z,
   if (ts.frozen) {
     c.launch(bn_running_kernel, cdiv(N, 128), 128, 0, rm, rv, N, s.mean, s.invstd);
   } else {
-    c.zero(sums, sizeof(double) * 2 * N);
-    dim3 grid(cdiv(N, 32), (unsigned)std::min<long long>(256, (M + 7) / 8));
-    c.launch(col_stats_kernel, grid, 256, 0, Z, M, N, ldz, sums, sums + N);
-    c.launch(bn_finalize_kernel, cdiv(N, 128), 128, 0, sums, sums + N, M, N, s.mean, s.invstd, rm, rv, 0.1f);
+    const dim3 grid = TCtx::col_grid(M, N);
+    c.launch(col_stats_kernel, grid, 256, 0, Z, M, N, ldz, c.red_part);
+    c.launch(bn_finalize_kernel, grid.x, 256, 0, c.red_part, (int)grid.y, M, N, s.mean, s.invstd, rm, rv, 0.1f);
   }
   if (keep) {
     const unsigned long long seed = ts.seed + 0x51ED270B * (++ts.drop_ctr);
@@ -204,10 +234,10 @@ static int bn_bwd(TCtx& c, const BnSave& s, const float* dY, int lddy, float* dZ
   float* gw = c.grad(s.prefix + "weight", s.N);
   float* gb = c.grad(s.prefix + "bias", s.N);
   if (sums) {
-    c.zero(sums, sizeof(double) * 2 * s.N);
-    dim3 grid(cdiv(s.N, 32), (unsigned)std::min<long long>(256, (s.M + 7) / 8));
-    c.launch(bn_bwd_reduce_kernel, grid, 256, 0, dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma, s.beta, s.relu, s.keep,
-             s.kscale, s.M, s.N, sums, sums + s.N);
+    const dim3 grid = TCtx::col_grid(s.M, s.N);
+    c.launch(bn_bwd_reduce_kernel, grid, 256, 0, dY, lddy, s.Z, s.ldz, s.mean, s.invstd, s.gamma, s.beta, s.relu,
+             s.keep, s.kscale, s.M, s.N, c.red_part);
+    c.launch(col_total_kernel<2>, grid.x, 256, 0, c.red_part, (int)grid.y, s.N, sums, nullptr);
   }
   const double* dg = sums;
   const double* db = sums ? sums + s.N : nullptr;
@@ -319,7 +349,6 @@ static int block_bwd(TCtx& c, const BlockSave& b, BlockConsts& bc, const float* 
   float* dCkp = c.fl((size_t)F * 4 * J * J);     // per-frame contributions, reduced in a fixed order
   float* dWg = c.fl((size_t)C * C);
   float* dU = c.fl((size_t)8 * C);
-  double* dsum = c.dbl((size_t)C + 8);
   float* dbg = c.fl(C);
   float* dcab = c.fl(8);
   float* dXg = c.fl((size_t)M * C);
@@ -333,13 +362,11 @@ static int block_bwd(TCtx& c, const BlockSave& b, BlockConsts& bc, const float* 
     return 1;
   if (c.pgrad) {
     c.launch(col_sum_det_kernel, cdiv(4 * J * J, 32), 256, 0, dCkp, F, 4 * J * J, dCk);
-    c.zero(dsum, sizeof(double) * (C + 8));
-    dim3 g1(cdiv(C, 32), (unsigned)std::min<long long>(256, (M + 7) / 8));
-    c.launch(col_sum_kernel, g1, 256, 0, dG, M, C, C, dsum);
-    dim3 g2(1, (unsigned)std::min<long long>(256, (M + 7) / 8));
-    c.launch(col_sum_kernel, g2, 256, 0, dab, M, 8, 8, dsum + C);
-    c.launch(d2f_kernel, cdiv(C, 128), 128, 0, dsum, dbg, C);
-    c.launch(d2f_kernel, 1, 32, 0, dsum + C, dcab, 8);
+    const dim3 g1 = TCtx::col_grid(M, C), g2 = TCtx::col_grid(M, 8);
+    c.launch(col_sum_kernel, g1, 256, 0, dG, M, C, C, c.red_part);
+    c.launch(col_total_kernel<1>, g1.x, 256, 0, c.red_part, (int)g1.y, C, nullptr, dbg);
+    c.launch(col_sum_kernel, g2, 256, 0, dab, M, 8, 8, c.red_part);
+    c.launch(col_total_kernel<1>, g2.x, 256, 0, c.red_part, (int)g2.y, 8, nullptr, dcab);
   }
   if (dense_tn(c, dG, C, b.X, C, M, C, C, dWg, C)) return 1;
   if (dense_nn(c, dG, C, bc.Wg, C, M, C, C, dXg, C)) return 1;
@@ -426,6 +453,7 @@ static int train_forward(gast_handle* h, TCtx& c, TrainState& ts, const float* x
   ts.We8 = c.fl((size_t)C * KP);
   ts.Z0 = c.fl((size_t)M0 * C);
   ts.act0 = c.fl((size_t)M0 * C);
+  col_reduce_area(c, ts, B, T);
   if (bn_fwd(c, ts.bnin, "init_bn.", x, Fin, Min, Fin, 0, 0.f, ts, nullptr, 0, id, ts.xbn, Fin)) return 1;
   const float* we = c.param("expand_conv.weight", (int64_t)C * Fin * k0);
   float* tmp = c.fl((size_t)C * k0 * Fin);
@@ -477,6 +505,7 @@ static int train_backward(gast_handle* h, TCtx& c, const TrainState& ts, const f
   const int J = c.J, C = cf.channels, L = cf.num_stages, Fin = cf.in_features, k0 = cf.filter_widths[0];
   const int Cl = C << L;
   const Geometry& g = ts.geo;
+  c.red_part = ts.red_part;
   // shrink
   const long long M = (long long)ts.B * g.T_out * J;
   float* dcur = c.fl((size_t)M * Cl);
@@ -498,9 +527,6 @@ static int train_backward(gast_handle* h, TCtx& c, const TrainState& ts, const f
     float* Xcol = c.fl((size_t)Mn * taps * Cw);
     float* dXcol = c.fl((size_t)Mn * taps * Cw);
     float* dWt = c.fl((size_t)Cw * taps * Cw);
-    c.zero(dXin, sizeof(float) * (size_t)Mi * Cw);
-    const ASeg rs = seg_taps(dXin, Cw, Cw, 1, 0, s.g.resmap);
-    c.launch(seg_scatter_add_kernel, cdiv(Mn * Cw, 256), 256, 0, rs, J, Fout, dSout, Cw, 0);
     if (bn_bwd(c, s.bnB, dSout, Cw, dZ2, Cw)) return 1;
     if (conv1x1_bwd(c, "layers_conv." + std::to_string(2 * s.idx + 1) + ".weight", dZ2, s.Hh, Mn, Cw, Cw, dHh)) return 1;
     if (bn_bwd(c, s.bnA, dHh, Cw, dZ1, Cw)) return 1;
@@ -511,8 +537,9 @@ static int train_backward(gast_handle* h, TCtx& c, const TrainState& ts, const f
     float* gw0 = c.grad("layers_conv." + std::to_string(2 * s.idx) + ".weight", (int64_t)Cw * Cw * taps);
     if (gw0)
       c.launch(conv_wgrad_relayout_kernel, cdiv((long long)Cw * Cw * taps, 256), 256, 0, dWt, Cw, Cw, taps, taps * Cw, gw0);
+    // dXin = the residual slice's gradient, then the taps' (one fixed order, every element written once)
     ASeg dsg = sg; dsg.base = dXin;
-    c.launch(seg_scatter_add_kernel, cdiv(Mn * dsg.K, 256), 256, 0, dsg, J, Fout, dXcol, taps * Cw, 0);
+    seg_adjoint(c, dsg, Fout, dXcol, taps * Cw, s.g.resmap, dSout, Cw);
     dcur = dXin;
   }
   // first block
@@ -532,9 +559,8 @@ static int train_backward(gast_handle* h, TCtx& c, const TrainState& ts, const f
   if (dense_nn(c, dZ0, C, ts.We8, KP, M0, C, KP, dAcol, KP)) return 1;
   float* gwe = c.grad("expand_conv.weight", (int64_t)C * Fin * k0);
   if (gwe) c.launch(conv_wgrad_relayout_kernel, cdiv((long long)C * Fin * k0, 256), 256, 0, dWe8, C, Fin, k0, KP, gwe);
-  c.zero(dxbn, sizeof(float) * (size_t)Min * Fin);
   const ASeg sg = seg_taps(dxbn, Fin, Fin, k0, (long long)J * Fin, RowMap{g.T0, ts.T, g.s0, 0});
-  c.launch(seg_scatter_add_kernel, cdiv(M0 * sg.K, 256), 256, 0, sg, J, F0, dAcol, KP, 0);
+  seg_adjoint(c, sg, F0, dAcol, KP);
   // init_bn: dx = dxbn . gamma . invstd (frozen), the batch-statistics adjoint otherwise
   if (bn_bwd(c, ts.bnin, dxbn, Fin, dx ? dx : dxin, Fin)) return 1;
   return 0;

@@ -1,6 +1,6 @@
 // Training-mode kernels of the lifting path (row a12 of SURVEY.md §8): batch-statistics BatchNorm
-// forward/backward, the joint-mixing operators and their adjoints, gather/scatter of the temporal
-// taps, and small reductions.  The training batch of the reference is small (b=128: 19,584 /
+// forward/backward, the joint-mixing operators and their adjoints, the gather of the temporal
+// taps and its adjoint, and small reductions, every one of them in a fixed summation order.  The training batch of the reference is small (b=128: 19,584 /
 // 6,528 / 2,176 rows per stage), so these kernels are written for exactness and simplicity; the
 // dense contractions (Z = A.W^T, dA = dZ.W, dW = dZ^T.A) run on the same GEMM kernels as inference.
 #pragma once
@@ -9,41 +9,107 @@
 namespace gast {
 
 // ----------------------------------------------------------------------------------------------
-// column reductions over rows:  out[n] (+)= sum_m f(...)    (block = 32 columns x 8 row lanes)
+// column reductions over rows: the totals over m of V values f_v(m, n) per column n, in two launches of one stream,
+// each adding in a fixed order, so a call repeats bit for bit (no atomics):
+//   - the reduction kernel, grid = (column groups of 32, R row blocks), block = 32 columns x 8 row lanes: a lane walks
+//     its rows in order, the block adds its 8 lanes in order and stores its V double partials to its own row of the
+//     partials area, part[(row block * V + v) * N + n] (col_partials);
+//   - its consumer, grid = column groups, block = 32 columns x 8 lanes, adds the R rows: lane rl takes the row blocks
+//     rl, rl + 8, ... in order, and the 8 lanes are added in order (col_total): bn_finalize_kernel, or
+//     col_total_kernel.
+// The next reduction of the stream reuses the area after its consumer.  COL_RED_ROWS bounds R.
 // ----------------------------------------------------------------------------------------------
-// sum and sum of squares per column, accumulated in double (BatchNorm batch statistics,
-// nn.BatchNorm2d training mode: gast_net.py:20,58-59,147,149 and the attention modules)
-__global__ void col_stats_kernel(const float* __restrict__ Z, long long M, int N, int ld,
-                                 double* __restrict__ sum, double* __restrict__ sumsq) {
-  const int n = blockIdx.x * 32 + (threadIdx.x & 31);
-  const int rl = threadIdx.x >> 5;                 // 0..7
-  double s = 0.0, q = 0.0;
-  if (n < N) {
-    for (long long m = (long long)blockIdx.y * 8 + rl; m < M; m += (long long)gridDim.y * 8) {
-      double v = (double)Z[m * ld + n];
-      s += v; q += v * v;
-    }
-  }
-  __shared__ double sh[2][8][33];
-  sh[0][rl][threadIdx.x & 31] = s;
-  sh[1][rl][threadIdx.x & 31] = q;
+constexpr int COL_RED_ROWS = 256;
+
+template <int V>
+__device__ __forceinline__ void col_partials(double (&s)[V], int n, int N, double* __restrict__ part) {
+  const int col = threadIdx.x & 31, rl = threadIdx.x >> 5;
+  __shared__ double sh[V][8][33];
+#pragma unroll
+  for (int v = 0; v < V; ++v) sh[v][rl][col] = s[v];
   __syncthreads();
   if (rl == 0 && n < N) {
-    for (int i = 1; i < 8; ++i) { s += sh[0][i][threadIdx.x & 31]; q += sh[1][i][threadIdx.x & 31]; }
-    atomicAdd(sum + n, s);
-    atomicAdd(sumsq + n, q);
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+      for (int i = 1; i < 8; ++i) s[v] += sh[v][i][col];
+      part[((long long)blockIdx.y * V + v) * N + n] = s[v];
+    }
   }
 }
 
-// mean / invstd from the sums; running statistics updated like torch (momentum 0.1, unbiased var)
-__global__ void bn_finalize_kernel(const double* __restrict__ sum, const double* __restrict__ sumsq, long long M,
-                                   int N, float* __restrict__ mean, float* __restrict__ invstd,
-                                   float* __restrict__ running_mean, float* __restrict__ running_var,
-                                   float momentum) {
-  int n = blockIdx.x * blockDim.x + threadIdx.x;
-  if (n >= N) return;
-  double mu = sum[n] / (double)M;
-  double var = sumsq[n] / (double)M - mu * mu;
+// t = the totals of column n over the R row blocks of part; valid in the threads of row lane 0.  A lane loads its row
+// blocks COL_RED_BATCH at a time, so that their round trips overlap, and adds them in order.
+template <int V>
+__device__ __forceinline__ void col_total(const double* __restrict__ part, int R, int n, int N, double (&t)[V]) {
+  constexpr int COL_RED_BATCH = 16;
+  const int col = threadIdx.x & 31, rl = threadIdx.x >> 5;
+  __shared__ double sh[V][8][33];
+#pragma unroll
+  for (int v = 0; v < V; ++v) {
+    t[v] = 0.0;
+    for (int y0 = rl; n < N && y0 < R; y0 += 8 * COL_RED_BATCH) {
+      double p[COL_RED_BATCH];
+#pragma unroll
+      for (int i = 0; i < COL_RED_BATCH; ++i) {
+        const int y = y0 + 8 * i;
+        p[i] = y < R ? __ldg(part + ((long long)y * V + v) * N + n) : 0.0;
+      }
+#pragma unroll
+      for (int i = 0; i < COL_RED_BATCH; ++i)
+        if (y0 + 8 * i < R) t[v] += p[i];
+    }
+    sh[v][rl][col] = t[v];
+  }
+  __syncthreads();
+  if (rl == 0) {
+#pragma unroll
+    for (int v = 0; v < V; ++v)
+      for (int i = 1; i < 8; ++i) t[v] += sh[v][i][col];
+  }
+}
+
+// the totals of a column reduction of V values: sums[v*N + n] in double and/or sumf[v*N + n] in float (either may be
+// null); grid = column groups, 256 threads
+template <int V>
+__global__ void col_total_kernel(const double* __restrict__ part, int R, int N, double* __restrict__ sums,
+                                 float* __restrict__ sumf) {
+  const int n = blockIdx.x * 32 + (threadIdx.x & 31);
+  double t[V];
+  col_total<V>(part, R, n, N, t);
+  if ((threadIdx.x >> 5) != 0 || n >= N) return;
+#pragma unroll
+  for (int v = 0; v < V; ++v) {
+    if (sums) sums[(long long)v * N + n] = t[v];
+    if (sumf) sumf[(long long)v * N + n] = (float)t[v];
+  }
+}
+
+// sum and sum of squares per column, accumulated in double (BatchNorm batch statistics,
+// nn.BatchNorm2d training mode: gast_net.py:20,58-59,147,149 and the attention modules): partials, V = 2
+__global__ void col_stats_kernel(const float* __restrict__ Z, long long M, int N, int ld, double* __restrict__ part) {
+  const int n = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int rl = threadIdx.x >> 5;                 // 0..7
+  double s[2] = {0.0, 0.0};
+  if (n < N) {
+    for (long long m = (long long)blockIdx.y * 8 + rl; m < M; m += (long long)gridDim.y * 8) {
+      double v = (double)Z[m * ld + n];
+      s[0] += v; s[1] += v * v;
+    }
+  }
+  col_partials<2>(s, n, N, part);
+}
+
+// mean / invstd from the sums (the R row blocks of col_stats_kernel's partials); running statistics updated like torch
+// (momentum 0.1, unbiased var).  grid = column groups, 256 threads
+__global__ void bn_finalize_kernel(const double* __restrict__ part, int R, long long M, int N, float* __restrict__ mean,
+                                   float* __restrict__ invstd, float* __restrict__ running_mean,
+                                   float* __restrict__ running_var, float momentum) {
+  const int n = blockIdx.x * 32 + (threadIdx.x & 31);
+  double t[2];
+  col_total<2>(part, R, n, N, t);
+  if ((threadIdx.x >> 5) != 0 || n >= N) return;
+  double mu = t[0] / (double)M;
+  double var = t[1] / (double)M - mu * mu;
   if (var < 0) var = 0;
   mean[n] = (float)mu;
   invstd[n] = (float)(1.0 / sqrt(var + (double)BN_EPS));
@@ -86,14 +152,15 @@ __global__ void bn_apply_kernel(const float* __restrict__ Z, int ldz, const floa
 }
 
 // dgamma[n] = sum_m dYhat*xhat ; dbeta[n] = sum_m dYhat,   dYhat = dY * keep * [bn(Z) > 0 if relu]
+// partials, V = 2 (dgamma, dbeta)
 __global__ void bn_bwd_reduce_kernel(const float* __restrict__ dY, int lddy, const float* __restrict__ Z, int ldz,
                                      const float* __restrict__ mean, const float* __restrict__ invstd,
                                      const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
                                      const unsigned char* __restrict__ keep, float keep_scale, long long M, int N,
-                                     double* __restrict__ dgamma, double* __restrict__ dbeta) {
+                                     double* __restrict__ part) {
   const int n = blockIdx.x * 32 + (threadIdx.x & 31);
   const int rl = threadIdx.x >> 5;
-  double g = 0.0, b = 0.0;
+  double s[2] = {0.0, 0.0};
   if (n < N) {
     const float mu = mean[n], is = invstd[n], ga = gamma[n], be = beta[n];
     for (long long m = (long long)blockIdx.y * 8 + rl; m < M; m += (long long)gridDim.y * 8) {
@@ -101,19 +168,11 @@ __global__ void bn_bwd_reduce_kernel(const float* __restrict__ dY, int lddy, con
       float d = dY[m * lddy + n];
       if (keep) d = keep[m * N + n] ? d * keep_scale : 0.f;
       if (relu && !(xh * ga + be > 0.f)) d = 0.f;
-      g += (double)d * xh;
-      b += (double)d;
+      s[0] += (double)d * xh;
+      s[1] += (double)d;
     }
   }
-  __shared__ double sh[2][8][33];
-  sh[0][rl][threadIdx.x & 31] = g;
-  sh[1][rl][threadIdx.x & 31] = b;
-  __syncthreads();
-  if (rl == 0 && n < N) {
-    for (int i = 1; i < 8; ++i) { g += sh[0][i][threadIdx.x & 31]; b += sh[1][i][threadIdx.x & 31]; }
-    atomicAdd(dgamma + n, g);
-    atomicAdd(dbeta + n, b);
-  }
+  col_partials<2>(s, n, N, part);
 }
 
 // dZ = gamma*invstd*(dYhat - dbeta/M - xhat*dgamma/M); also writes the float parameter grads (when g_gamma / g_beta are
@@ -148,25 +207,14 @@ __global__ void bn_bwd_apply_kernel(const float* __restrict__ dY, int lddy, cons
   }
 }
 
-// out[n] = sum_m X[m][n]   (bias gradients)
-__global__ void col_sum_kernel(const float* __restrict__ X, long long M, int N, int ld, double* __restrict__ out) {
+// sum_m X[m][n]   (bias gradients): partials, V = 1
+__global__ void col_sum_kernel(const float* __restrict__ X, long long M, int N, int ld, double* __restrict__ part) {
   const int n = blockIdx.x * 32 + (threadIdx.x & 31);
   const int rl = threadIdx.x >> 5;
-  double s = 0.0;
+  double s[1] = {0.0};
   if (n < N)
-    for (long long m = (long long)blockIdx.y * 8 + rl; m < M; m += (long long)gridDim.y * 8) s += (double)X[m * ld + n];
-  __shared__ double sh[8][33];
-  sh[rl][threadIdx.x & 31] = s;
-  __syncthreads();
-  if (rl == 0 && n < N) {
-    for (int i = 1; i < 8; ++i) s += sh[i][threadIdx.x & 31];
-    atomicAdd(out + n, s);
-  }
-}
-
-__global__ void d2f_kernel(const double* __restrict__ in, float* __restrict__ out, int n) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = (float)in[i];
+    for (long long m = (long long)blockIdx.y * 8 + rl; m < M; m += (long long)gridDim.y * 8) s[0] += (double)X[m * ld + n];
+  col_partials<1>(s, n, N, part);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -313,18 +361,39 @@ __global__ void seg_gather_kernel(ASeg sg, int J, long long F, float* __restrict
   dst[m * ldd + coff + k] = sg.base[(map_frame(sg.map, f) * J + j) * (long long)sg.ld + tap * sg.tap_stride + c];
 }
 
-// Adjoint of the gather:  grad_seg(m, k) += src[m][coff + k]   (atomic: taps / residuals may overlap)
-__global__ void seg_scatter_add_kernel(ASeg sg, int J, long long F, const float* __restrict__ src, int lds, int coff) {
-  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long M = F * J;
-  if (idx >= M * sg.K) return;
-  long long m = idx / sg.K;
-  int k = (int)(idx - m * sg.K);
-  long long f = m / J;
-  int j = (int)(m - f * J);
-  int tap = k / sg.Kc, c = k - tap * sg.Kc;
-  float* dstp = const_cast<float*>(sg.base) + (map_frame(sg.map, f) * J + j) * (long long)sg.ld + tap * sg.tap_stride + c;
-  atomicAdd(dstp, src[m * lds + coff + k]);
+// Adjoint of seg_gather_kernel, computed from the input side: one thread per element of dX, which it writes once (no
+// atomics, no zero-fill).  The gather reads input frame b*T_in + t*t_mul + t_off + k*dil for output frame t of clip b
+// and tap k (map = the gather's RowMap, dil in frames), so
+//   dX[b*T_in + u][j][c] = rsrc[b*T_out + r][j][c]                      (r*rmap.t_mul + rmap.t_off == u; rsrc optional)
+//                        + sum over k = 0 .. taps-1, ascending, of src[b*T_out + t][j][k*Kc + c]
+//                                                                    (t*map.t_mul + map.t_off + k*dil == u)
+// over the t, r in [0, T_out) that exist; frames that no output reads get 0.  rsrc is the residual slice of a temporal
+// stage (one tap, its own map, the same T_out and T_in).  Rows of dX, src and rsrc are J joints apart; row strides
+// ldx, lds and ldr.
+__global__ void seg_adjoint_kernel(RowMap map, int taps, int dil, int Kc, const float* __restrict__ src, int lds,
+                                   RowMap rmap, const float* __restrict__ rsrc, int ldr, int J, long long F_in,
+                                   float* __restrict__ dX, int ldx) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= F_in * J * Kc) return;
+  const long long row = idx / Kc;
+  const int c = (int)(idx - row * Kc);
+  const long long fr = row / J;
+  const int j = (int)(row - fr * J);
+  const long long b = fr / map.T_in;
+  const int u = (int)(fr - b * map.T_in);
+  const long long out0 = b * map.T_out;    // first output frame of clip b
+  float s = 0.f;
+  if (rsrc) {
+    const int v = u - rmap.t_off;
+    if (v >= 0 && v % rmap.t_mul == 0 && v / rmap.t_mul < rmap.T_out)
+      s += rsrc[((out0 + v / rmap.t_mul) * J + j) * ldr + c];
+  }
+  for (int k = 0; k < taps; ++k) {
+    const int v = u - map.t_off - k * dil;
+    if (v >= 0 && v % map.t_mul == 0 && v / map.t_mul < map.T_out)
+      s += src[((out0 + v / map.t_mul) * J + j) * lds + k * Kc + c];
+  }
+  dX[row * ldx + c] = s;
 }
 
 // y[i] += x[i]

@@ -58,6 +58,9 @@ struct TrainState {
   std::vector<BlockSave> blocks;
   std::vector<StageSave> stages;
   const float* last = nullptr;   // input of shrink
+  // partials area of every column reduction of the forward and its backward (col_partials), in the forward's part of
+  // the workspace
+  double* red_part = nullptr;
   float drop_p = 0.f; unsigned long long seed = 0; unsigned long long drop_ctr = 0;
   size_t arena_off = 0;          // workspace used by the forward (backward temporaries go after it)
   size_t workspace_bytes = 0;    // what the forward checked: its own sizing pass plus a backward with parameter gradients,
