@@ -178,10 +178,13 @@ extern "C" int gast_forward_chunked(gast_t* h, const float* x, float* y, int32_t
   if (call_begin(h, "gast_forward_chunked", need, workspace, workspace_bytes)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long xrow = (long long)h->cfg.num_joints * h->cfg.in_features, yrow = (long long)h->cfg.num_joints * 3;
+  const size_t es = h->act_dtype == GAST_F16 ? sizeof(__half) : sizeof(float);   // bytes per element of x and y
   for (long long p = 0; p < pl.passes; ++p) {
     const ChunkPass q = chunk_pass(pl, B, T, p);
-    if (model_forward(h, st, x + ((long long)q.b0 * T + q.f0) * xrow, y + ((long long)q.b0 * pl.T_out + q.t0) * yrow,
-                      q.nb, q.Tin, strided_now, workspace_arena(workspace, workspace_bytes), nullptr, nullptr))
+    const char* xp = reinterpret_cast<const char*>(x) + ((long long)q.b0 * T + q.f0) * xrow * es;
+    char* yp = reinterpret_cast<char*>(y) + ((long long)q.b0 * pl.T_out + q.t0) * yrow * es;
+    if (model_forward(h, st, reinterpret_cast<const float*>(xp), reinterpret_cast<float*>(yp), q.nb, q.Tin, strided_now,
+                      workspace_arena(workspace, workspace_bytes), nullptr, nullptr))
       return 1;
   }
   return 0;

@@ -103,6 +103,7 @@ struct gast_handle {
   int gemm_core = 0;                 // 0 auto (tensor cores where possible), 1 force FFMA
   int precision = 0;                 // 0 fp32-grade (3xFP16 on scaled operands in inference, 3xTF32 in training),
                                      // 1 single-pass TF32 (inference only)
+  int act_dtype = GAST_F32;          // activation type of the model forward (gast_set_activation_dtype)
   int train_precision = 0;           // training and every gradient: 0 fp32-grade, 1 single-pass TF32 (forward and
                                      // input-gradient GEMMs) with the TF32 weight-gradient kernel (wgrad_tc.cuh)
   int wgrad_tc_launches = 0;         // weight gradients of the last training call that ran on wgrad_tc_kernel
@@ -127,6 +128,14 @@ constexpr int GAST_MAX_PENDING_TRAIN = 16;   // training forwards that may wait 
 
 enum { LK_EXPAND = 0, LK_GEMM_PLAIN = 1, LK_GEMM_SEMCH = 2, LK_GEMM_GLOBAL = 3, LK_ROWDOT = 4, LK_SHRINK = 5,
        LK_TC_PLAIN = 6, LK_TC_SEMCH = 7, LK_TC_GLOBAL = 8, LK_GLOBAL_MIX = 9 };
+
+// The refusal of every entry that half does not run: training, every backward, the streams, the mpjpe forward
+static int half_check(const gast_handle* h, const char* who) {
+  if (h->act_dtype == GAST_F16)
+    return fail("%s: the handle's activation type is fp16 (gast_set_activation_dtype), which runs the eval-mode forward "
+                "and the chunked forward only; set GAST_F32 to train, differentiate, stream or take the mpjpe", who);
+  return 0;
+}
 
 struct TimedLaunch {   // RAII: event pair around one launch when timing is on
   gast_handle* h; cudaStream_t st; bool on;
@@ -306,6 +315,9 @@ extern "C" int gast_bind(gast_t* h, int32_t n, const char* const* keys, void* co
 extern "C" int gast_set_gemm_core(gast_t* h, int32_t core) {
   if (!h) return fail("null handle");
   if (core != 0 && core != 1) return fail("gast_set_gemm_core: core must be 0 (auto) or 1 (ffma)");
+  if (core == 1 && h->act_dtype == GAST_F16)
+    return fail("gast_set_gemm_core: the activation type is fp16 (gast_set_activation_dtype), which runs on the "
+                "tensor-core core only");
   h->gemm_core = core;
   return 0;
 }
@@ -313,7 +325,30 @@ extern "C" int gast_set_gemm_core(gast_t* h, int32_t core) {
 extern "C" int gast_set_precision(gast_t* h, int32_t mode) {
   if (!h) return fail("null handle");
   if (mode != 0 && mode != 1) return fail("gast_set_precision: mode must be 0 (fp32-grade) or 1 (tf32), got %d", mode);
+  if (mode == 1 && h->act_dtype == GAST_F16)
+    return fail("gast_set_precision: the activation type is fp16 (gast_set_activation_dtype), which has its own "
+                "arithmetic; TF32 needs GAST_F32");
   h->precision = mode;
+  return 0;
+}
+
+extern "C" int gast_set_activation_dtype(gast_t* h, int32_t dtype) {
+  if (!h) return fail("null handle");
+  if (dtype != GAST_F32 && dtype != GAST_F16)
+    return fail("gast_set_activation_dtype: dtype must be GAST_F32 (0) or GAST_F16 (1), got %d", dtype);
+  if (dtype == GAST_F16) {
+    if (h->cfg.kind != GAST_KIND_MODEL)
+      return fail("gast_set_activation_dtype: fp16 runs the whole model (MODEL kind) only, not a sub-module");
+    if (h->precision != 0) return fail("gast_set_activation_dtype: fp16 needs gast_set_precision(h, 0), not TF32");
+    if (h->cfg.num_joints > MIX_JMAX)   // the attention then needs the fused GLOBAL epilogue, not offered in half
+      return fail("gast_set_activation_dtype: fp16 takes at most %d joints (got %d)", MIX_JMAX, h->cfg.num_joints);
+    if (h->cfg.channels % TC_KS)   // every GEMM width is a multiple of channels; the half form takes multiples of 32
+      return fail("gast_set_activation_dtype: fp16 needs channels that are a multiple of %d (got %d): there is no FFMA "
+                  "core in half", TC_KS, h->cfg.channels);
+    if (h->gemm_core != 0) return fail("gast_set_activation_dtype: fp16 runs on the tensor-core core only "
+                                       "(gast_set_gemm_core(h, 0))");
+  }
+  h->act_dtype = dtype;
   return 0;
 }
 
@@ -610,8 +645,11 @@ extern "C" int32_t gast_out_frames(const gast_t* h, int32_t T, int32_t strided_n
 // workspace carve-up ------------------------------------------------------------------
 struct Arena {
   char* base; size_t size; size_t off = 0; bool dry;
-  float* take(size_t nfloats) {
-    size_t bytes = (nfloats * sizeof(float) + 255) & ~(size_t)255;
+  size_t esize = sizeof(float);   // bytes per element of take(): 2 for the activations of a half forward (plan_model)
+  float* take(size_t n) { return take_bytes(n * esize); }
+  float* take32(size_t nfloats) { return take_bytes(nfloats * sizeof(float)); }
+  float* take_bytes(size_t b) {
+    size_t bytes = (b + 255) & ~(size_t)255;
     float* p = dry ? nullptr : reinterpret_cast<float*>(base + off);
     off += bytes;
     return p;
@@ -733,8 +771,14 @@ static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p,
   if (Ktot != p.ldw) return fail("internal: K mismatch %d vs %d", Ktot, p.ldw);
   if (p.N % 4 || p.ld_out % 4) return fail("internal: N/ld_out must be multiples of 4");
   // training's operand copies (train_tcw, the only ones without the fp16 pair) run at the training precision
-  const int prec = (h->gemm_core == 0 && tcw && tc_supported(p, epi, *tcw))
-                       ? tc_prec(*tcw, tcw->f16 ? h->precision : h->train_precision) : -1;
+  int prec = (h->gemm_core == 0 && tcw && tc_supported(p, epi, *tcw))
+                 ? tc_prec(*tcw, tcw->f16 ? h->precision : h->train_precision) : -1;
+  if (h->act_dtype == GAST_F16) {   // fp16 operands: the half form or nothing (there is no FFMA core in half)
+    if (!tcw || !tc_supported_h(p, epi, *tcw))
+      return fail("fp16 forward: a GEMM (N %d, K %d, epilogue %d) is not taken by the tensor-core core (widths must be "
+                  "multiples of 32)", p.N, p.ldw, epi);
+    prec = TC_F16;
+  }
   if (!h->audit_fn) return launch_gemm_core(h, st, epi, p, tcw, prec);
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   CUDA_OK(cudaStreamIsCapturing(st, &cs));
@@ -764,6 +808,16 @@ static int launch_rowdot(gast_handle* h, cudaStream_t st, const float* X, int ld
   const int Q = 2 * b.heads;
   unsigned blocks = cdiv(rows * 32, 256);
   TimedLaunch tl(h, st, LK_ROWDOT);
+  if (h->act_dtype == GAST_F16) {   // X holds fp16; the row dots stay fp32 (they feed the softmax)
+    const __half* Xh = reinterpret_cast<const __half*>(X);
+    if (Q == 8 && (size_t)8 * b.C * sizeof(float) <= 48 * 1024) {
+      unsigned g = (unsigned)std::min<long long>((rows * 32 + 255) / 256, (long long)h->sm_count * 8);
+      rowdot8_kernel<<<g, 256, sizeof(float) * 8 * b.C, st>>>(Xh, ldx, b.U, b.cab, ab, rows, b.C);
+    } else if (Q == 8) rowdot_kernel<8><<<blocks, 256, 0, st>>>(Xh, ldx, b.U, b.cab, ab, rows, b.C);
+    else return fail("internal: fp16 forward with heads=%d", b.heads);
+    h->launches++;
+    return 0;
+  }
   if (Q == 8 && b.C % 4 == 0 && (size_t)8 * b.C * sizeof(float) <= 48 * 1024) {
     unsigned g = (unsigned)std::min<long long>((rows * 32 + 255) / 256, (long long)h->sm_count * 8);
     rowdot8_kernel<<<g, 256, sizeof(float) * 8 * b.C, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
@@ -820,7 +874,13 @@ static int run_global(gast_handle* h, cudaStream_t st, BlockConsts& b, const flo
     const size_t smem = sizeof(float) * (size_t)fpb * b.heads * J * MIX_JP;
     {
       TimedLaunch tl(h, st, LK_GLOBAL_MIX);
-      global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(out_G, Ng, w.AB, b.Ck, w.Y, Ng, F, J, b.heads, b.Cg, fpb);
+      if (h->act_dtype == GAST_F16)
+        global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(reinterpret_cast<const __half*>(out_G), Ng, w.AB,
+                                                                   b.Ck, reinterpret_cast<__half*>(w.Y), Ng, F, J,
+                                                                   b.heads, b.Cg, fpb);
+      else
+        global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(out_G, Ng, w.AB, b.Ck, w.Y, Ng, F, J, b.heads, b.Cg,
+                                                                   fpb);
       h->launches++;
     }
     CUDA_OK(cudaGetLastError());
@@ -866,6 +926,18 @@ static int launch_expand(gast_handle* h, cudaStream_t st, const float* x, float*
   if (k0 * Fin > EXP_MAXKF) return fail("expand: filter_width*in_features > %d unsupported", EXP_MAXKF);
   TimedLaunch tl(h, st, LK_EXPAND);
   const dim3 grid(cdiv(rows, EXS_ROWS), cdiv(c.channels, EXS_CHUNK));
+  if (h->act_dtype == GAST_F16) {
+    const __half* xh = reinterpret_cast<const __half*>(x);
+    __half* oh = reinterpret_cast<__half*>(out);
+    if (k0 * Fin <= 6)
+      expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(xh, h->We, h->be, oh, rows, c.num_joints, T, T0, stride, k0,
+                                                           Fin, c.channels);
+    else
+      expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(xh, h->We, h->be, oh, rows, c.num_joints, T, T0,
+                                                                   stride, k0, Fin, c.channels);
+    h->launches++;
+    return 0;
+  }
   if (k0 * Fin <= 6)
     expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, out, rows, c.num_joints, T, T0, stride, k0,
                                                          Fin, c.channels);
@@ -908,6 +980,10 @@ static int launch_shrink(gast_handle* h, cudaStream_t st, const float* X, float*
     const unsigned nb = (unsigned)std::min<long long>(SHL_MAXBLOCKS, (rows + 7) / 8);
     TimedLaunch tl(h, st, LK_SHRINK);
     shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(X, Cl, ws, y, rows, Cl, target, partial, ticket, loss);
+  } else if (h->act_dtype == GAST_F16) {
+    TimedLaunch tl(h, st, LK_SHRINK);
+    shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws,
+                                                        reinterpret_cast<__half*>(y), rows, Cl);
   } else {
     TimedLaunch tl(h, st, LK_SHRINK);
     shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(X, Cl, ws, y, rows, Cl);
@@ -916,6 +992,8 @@ static int launch_shrink(gast_handle* h, cudaStream_t st, const float* X, float*
   return 0;
 }
 
+// In a half forward (gast_set_activation_dtype) every buffer but bb.AB holds fp16: the pointers are typed float and
+// the launches reinterpret them.
 struct ModelBufs {
   float* act[2];
   float* tmp;
@@ -924,6 +1002,7 @@ struct ModelBufs {
 
 static int plan_model(const gast_handle* h, int B, int T, int strided_now, Arena& a, ModelBufs* mb, Geometry* g) {
   if (geometry(h, T, strided_now, g)) return 1;
+  a.esize = h->act_dtype == GAST_F16 ? sizeof(__half) : sizeof(float);
   const int J = h->cfg.num_joints, C = h->cfg.channels, L = h->cfg.num_stages;
   // max over layers
   size_t act = 0, tmp = 0, xy = 0, l = 0, ab = 0;
@@ -941,7 +1020,7 @@ static int plan_model(const gast_handle* h, int B, int T, int strided_now, Arena
   }
   mb->act[0] = a.take(act); mb->act[1] = a.take(act);
   mb->tmp = a.take(tmp);
-  mb->bb.XY = a.take(xy); mb->bb.L = a.take(l); mb->bb.AB = a.take(ab); mb->bb.Y = a.take(l); mb->bb.Gl = a.take(l);
+  mb->bb.XY = a.take(xy); mb->bb.L = a.take(l); mb->bb.AB = a.take32(ab); mb->bb.Y = a.take(l); mb->bb.Gl = a.take(l);
   return 0;
 }
 
@@ -1047,6 +1126,7 @@ extern "C" int gast_forward_mpjpe(gast_t* h, const float* x, const float* target
   if (!h) return fail("gast_forward_mpjpe: null handle");
   if (h->cfg.kind != GAST_KIND_MODEL) return fail("gast_forward_mpjpe: only the MODEL kind has a shrink layer");
   if (!target || !loss) return fail("gast_forward_mpjpe: target and loss must be device pointers");
+  if (half_check(h, "gast_forward_mpjpe")) return 1;
   return forward_impl(h, x, y, B, T, strided_now, workspace, workspace_bytes, stream, target, loss);
 }
 
@@ -1104,6 +1184,7 @@ extern "C" int gast_bind_grads(gast_t* h, int32_t n, const char* const* keys, vo
 // The inference precision alone does not reach training: a handle at inference TF32 trains and differentiates only
 // once the training precision is TF32 too (gast_set_train_precision), and nothing falls back silently
 static int precision_check(gast_handle* h, const char* what) {
+  if (half_check(h, what)) return 1;
   if (h->precision != 0 && h->train_precision == 0)
     return fail("%s: reduced precision is inference-only; call gast_set_precision(h, 0) before training or "
                 "differentiating (precision is %d)", what, h->precision);
@@ -1232,15 +1313,16 @@ static int timed_reps(cudaStream_t st, int reps, float* ms_out, Launch launch) {
 // debug / probe entry: out[M,N] = A[M,K] . W[N,K]^T on a chosen GEMM core (test infrastructure
 // for the numerics of the tensor-core path; not used by the forward).  tc_mode: the tensor-core core's precision
 // (0 fp32-grade as inference runs it, three fp16 products on scaled operands; 1 single-pass TF32; 3 fp32-grade as
-// training runs it, three TF32 products).
+// training runs it, three TF32 products; 16 the half form, on fp16 A and out).
 // ------------------------------------------------------------------------------------------
 extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32_t N, int32_t K,
                                int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (M <= 0 || N <= 0 || K <= 0 || N % 4 || K % 4) return fail("gast_debug_gemm: bad shape");
-  if (core < 0 || core > 1 || (tc_mode != 0 && tc_mode != 1 && tc_mode != 3) || (core == 1 && tc_mode != 0))
-    return fail("gast_debug_gemm: core must be 0 (tensor cores, tc_mode 0 = F16X3, 1 = TF32 or 3 = 3xTF32) or 1 (FFMA, "
-                "tc_mode 0)");
+  if (core < 0 || core > 1 || (tc_mode != 0 && tc_mode != 1 && tc_mode != 3 && tc_mode != 16) ||
+      (core == 1 && tc_mode != 0))
+    return fail("gast_debug_gemm: core must be 0 (tensor cores, tc_mode 0 = F16X3, 1 = TF32, 3 = 3xTF32 or 16 = the "
+                "half form) or 1 (FFMA, tc_mode 0)");
   GemmP p;
   gemm_flat(p, M);
   p.nseg = 1; p.seg[0] = seg_flat(A, K, K);
@@ -1250,7 +1332,7 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
   TcWeights t;
   if (core == 0) {
     rc = tc_prepare_weights(t, W, N, K, st, &owned, tc_mode != 3);   // 3xTF32 runs on training's tf32 copies
-    if (rc || !t.ready || !tc_supported(p, EPI_PLAIN, t)) {
+    if (rc || !t.ready || !(tc_mode == 16 ? tc_supported_h(p, EPI_PLAIN, t) : tc_supported(p, EPI_PLAIN, t))) {
       for (void* q : owned) cudaFree(q);
       return fail("gast_debug_gemm: shape not supported by the tensor-core core (rc=%d)", rc);
     }
@@ -1258,7 +1340,7 @@ extern "C" int gast_debug_gemm(const float* A, const float* W, float* out, int32
     cudaFuncSetAttribute((const void*)gemm_ffma_kernel<EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   }
   rc = timed_reps(st, reps, ms_out, [&]() -> int {
-    if (core == 0) return tc_launch(st, EPI_PLAIN, p, t, tc_prec(t, tc_mode == 1));
+    if (core == 0) return tc_launch(st, EPI_PLAIN, p, t, tc_mode == 16 ? TC_F16 : tc_prec(t, tc_mode == 1));
     dim3 grid(cdiv(M, 128), cdiv(N, FF_BN));
     gemm_ffma_kernel<EPI_PLAIN><<<grid, FF_THREADS, ffma_smem_bytes(EPI_PLAIN, 1, 128, 1), st>>>(p);
     return (int)cudaGetLastError();

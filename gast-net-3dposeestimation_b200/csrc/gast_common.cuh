@@ -1,5 +1,6 @@
 // Shared device-side types of libgast_b200 (sm_90a).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -70,6 +71,28 @@ struct GemmP {
 
 __device__ __forceinline__ float4 ldg4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));
+}
+
+// Element access of the HBM-side kernels, which are templated on the activation type (float, or __half under
+// gast_set_activation_dtype(h, GAST_F16)): loads widen to fp32 and stores round to nearest, arithmetic stays fp32.
+__device__ __forceinline__ float ld1(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ld1(const __half* p) { return __half2float(__ldg(p)); }
+__device__ __forceinline__ float4 ld4(const float* p) { return ldg4(p); }
+__device__ __forceinline__ float4 ld4(const __half* p) {   // 4 halves, 8-byte aligned
+  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ void st1(float* p, float v) { *p = v; }
+__device__ __forceinline__ void st1(__half* p, float v) { *p = __float2half_rn(v); }
+__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+__device__ __forceinline__ void st4(__half* p, float4 v) {
+  const __half2 a = __floats2half2_rn(v.x, v.y), b = __floats2half2_rn(v.z, v.w);
+  uint2 u;
+  u.x = *reinterpret_cast<const uint32_t*>(&a);
+  u.y = *reinterpret_cast<const uint32_t*>(&b);
+  *reinterpret_cast<uint2*>(p) = u;
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

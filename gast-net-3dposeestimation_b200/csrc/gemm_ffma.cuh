@@ -47,7 +47,8 @@ __device__ __forceinline__ void epi_sync() { asm volatile("bar.sync 1, 256;" :::
 // thread tid (of 256) owns rows {ty*4+i, 64+ty*4+i} (i<4) and cols {tx*4+j, 64+tx*4+j} (j<4), ty = tid/16,
 // tx = tid%16.  `smem` is free scratch of at least ffma_smem_bytes() - 3*128*8 bytes; callers synchronise before.
 // The tile is frames f0 .. f0 + nf - 1 (vrows rows) x columns n0 .. n0 + 127, column tile `ctile` (n0 = 128 ctile).
-template <int EPI>
+// OT: the element type of out and res (float; __half in the tensor-core core's half form, gemm_tc_h_kernel).
+template <int EPI, typename OT = float>
 __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)[8][8], float* smem, int tid,
                                               int f0, int nf, int vrows, int n0, int ctile) {
   const int J = p.J;
@@ -59,10 +60,10 @@ __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)
       if (r >= vrows) continue;
       int fr = r / J, j = r - fr * J;
       long long orow = ((long long)(f0 + fr) * J + j);
-      const float* resrow = nullptr;
+      const OT* resrow = nullptr;
       if (p.res) {
         long long fin = map_frame(p.res_map, f0 + fr);
-        resrow = p.res + (fin * J + j) * (long long)p.res_ld;
+        resrow = reinterpret_cast<const OT*>(p.res) + (fin * J + j) * (long long)p.res_ld;
       }
 #pragma unroll
       for (int g = 0; g < 2; ++g) {
@@ -78,10 +79,10 @@ __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)
           for (int q = 0; q < 4; ++q) v[q] = fmaxf(v[q], 0.f);
         }
         if (resrow) {
-          float4 rr = ldg4(resrow + n);
+          float4 rr = ld4(resrow + n);
           v[0] += rr.x; v[1] += rr.y; v[2] += rr.z; v[3] += rr.w;
         }
-        *reinterpret_cast<float4*>(p.out + orow * p.ld_out + n) = make_float4(v[0], v[1], v[2], v[3]);
+        st4(reinterpret_cast<OT*>(p.out) + orow * p.ld_out + n, make_float4(v[0], v[1], v[2], v[3]));
       }
     }
   } else if (EPI == EPI_SEMCH) {
@@ -119,7 +120,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)
         }
         if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
         long long orow = ((long long)(f0 + fr) * J + ji);
-        *reinterpret_cast<float4*>(p.out + orow * p.ld_out + mask * p.C + c0) = make_float4(v0, v1, v2, v3);
+        st4(reinterpret_cast<OT*>(p.out) + orow * p.ld_out + mask * p.C + c0, make_float4(v0, v1, v2, v3));
       }
     }
   } else {  // EPI_GLOBAL
@@ -199,7 +200,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmP& p, const float (&acc)
         }
       }
       long long orow = ((long long)(f0 + fr) * J + ji);
-      *reinterpret_cast<float4*>(p.out + orow * p.ld_out + n) = make_float4(v[0], v[1], v[2], v[3]);
+      st4(reinterpret_cast<OT*>(p.out) + orow * p.ld_out + n, make_float4(v[0], v[1], v[2], v[3]));
     }
   }
 }

@@ -85,8 +85,8 @@ struct TcWeights {
 };
 
 // precision of the core: TC_3XTF32 and TC_F16X3 are gast_set_precision's mode 0 (training and inference), TC_1XTF32
-// its mode 1
-enum { TC_3XTF32 = 0, TC_1XTF32 = 1, TC_F16X3 = 2 };
+// its mode 1; TC_F16 is the half form (fp16 activations, gemm_tc_h_kernel)
+enum { TC_3XTF32 = 0, TC_1XTF32 = 1, TC_F16X3 = 2, TC_F16 = 3 };
 
 #ifndef GAST_TC1_STAGES
 #define GAST_TC1_STAGES 3                             // ring depth of the 1xTF32 form: 4 and 5 measured no faster (DESIGN.md §4.1)
@@ -595,6 +595,246 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   gemm_epilogue<EPI>(p, out, reinterpret_cast<float*>(ring), ct, fe, nfe, nfe * J, ctile * TC_BN, ctile);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// TC_F16, the half form (gast_set_activation_dtype(h, GAST_F16)): A and the output are fp16 in memory, so a MAC is one
+// fp16 product,  D = 2^-s_W (A . fp16(W 2^s_W)),  with fp32 accumulation.  B is the F16X3 hi copy unchanged; the weight
+// scale is applied once, to the finished tile, before the epilogue (a power of two: no rounding).  Both operands are
+// read by wgmma from shared memory through descriptors (m64n128k16, SS form), in one layout: the no-swizzle K-major
+// core-matrix layout of the B copies, [K/8][rows][8] halves (8 rows x 16 B core matrices, 128 B apart along the rows,
+// 2048 B apart along K), so tc_bdesc describes A as well.  A stage is 128 rows x 32 K = 8 KB:
+//   identity segments (tc_seg_tma): one 3D TMA box {8 halves, 128 rows, 4 k-octets} of a map with dims
+//     {8, rows, Kc / 8} and strides {ld, 8} halves (tc_encode_a16), which lands in exactly that layout;
+//   gathered segments: cp.async of 16 B = one row's k-octet, zero-filled outside the tile.
+// K is chained in the accumulator: the tensor core's truncation bias (~0.5 ulp of fp32 per k16 MMA) stays far below
+// the 2^-11 rounding of the fp16 operands (K = 1536 is 96 MMAs), so the two-level partial sums of the fp32-grade forms
+// buy nothing here.  Tiles, ring protocol, producer and epilogues are gemm_tc_kernel's; the epilogues read the residual
+// and write the output as fp16 (tc_store_plain_h's TMA store of two [128][64]-half column blocks; SemCH through
+// gemm_epilogue<EPI_SEMCH, __half>).  There is no EPI_GLOBAL form: a half model's attention mix is its own kernel
+// (global_mix_kernel, J <= MIX_JMAX, which gast_set_activation_dtype requires).
+#ifndef GAST_TCH_STAGES
+#define GAST_TCH_STAGES 6
+#endif
+constexpr int TCH_STAGES = GAST_TCH_STAGES;
+constexpr int TC_H_A_BYTES = TC_BM * TC_KS * 2;
+constexpr int TC_H_SLOT = TC_B16_BYTES + TC_H_A_BYTES;
+constexpr int TC_H_RING = TCH_STAGES * TC_H_SLOT;
+static_assert(TC_H_SLOT % 1024 == 0 && TC_H_RING >= 2 * TC_BM * 64 * 2,
+              "slots stay 1024-byte aligned, and the ring holds the plain epilogue's fp16 tile");
+
+__host__ __device__ inline size_t tch_smem_bytes(int epi, int J, int fpt, int hpt) {
+  size_t m = (size_t)TC_H_RING + 16 * TCH_STAGES;
+  const size_t stg = (size_t)TC_BM * TC_STG_LD * 4;
+  const size_t e = ffma_smem_bytes(epi, J, fpt, hpt) - TC_ROWBASE_BYTES;
+  if (stg > m) m = stg;
+  if (e > m) m = e;
+  return TC_ROWBASE_BYTES + 1024 + m;
+}
+
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int x, int y, int z) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(x), "r"(y), "r"(z) : "memory");
+}
+
+// d (+)= A . B, m64n128k16, fp16 operands both K-major in shared memory, fp32 accumulate; scale_d == 0 overwrites d
+__device__ __forceinline__ void wgmma_f16ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+
+// EPI_PLAIN of the half form: tc_store_plain's order (bias, ReLU, residual read as fp16), each value rounded once to
+// fp16, staged in the free ring as two 128-byte-swizzled [128][64]-half column blocks (16 KB apart) and stored with
+// `out` (fp16 {N, F J}, box {64, fpt J}).
+__device__ __forceinline__ void tc_store_plain_h(const GemmP& p, const float (&acc)[64], unsigned char* ring,
+                                                 uint32_t rb, const CUtensorMap& out, int r0, int t, int ct, int f0,
+                                                 int vrows, int n0) {
+  const int J = p.J;
+  const __half* resrow[2] = {nullptr, nullptr};
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + 8 * h;
+    if (p.res && r < vrows) {
+      const int fr = r / J, j = r - fr * J;
+      resrow[h] = reinterpret_cast<const __half*>(p.res) + (map_frame(p.res_map, f0 + fr) * J + j) * (long long)p.res_ld;
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const int col = 8 * i + 2 * t, n = n0 + col;
+    const bool in = n < p.N;                                            // N % 4 == 0: n + 1 < N too
+    float2 b = make_float2(0.f, 0.f);
+    if (p.bias && in) b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+      if (p.bias) { v0 += b.x; v1 += b.y; }
+      if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      if (resrow[h] && in) {
+        const float2 rr = __half22float2(__ldg(reinterpret_cast<const __half2*>(resrow[h] + n)));
+        v0 += rr.x; v1 += rr.y;
+      }
+      const int r = r0 + 8 * h;
+      *reinterpret_cast<__half2*>(ring + (col >> 6) * (TC_BM * 128) + r * 128 + ((((col >> 3) & 7) ^ (r & 7)) << 4) +
+                                  (col & 7) * 2) = __floats2half2_rn(v0, v1);
+    }
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // the writes above, seen by the TMA engine
+  epi_sync();
+  if (ct == 0) {
+    for (int cb = 0; cb < 2 && n0 + cb * 64 < p.N; ++cb) tma_store_2d(&out, rb + cb * TC_BM * 128, n0 + cb * 64, f0 * J);
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+  }
+}
+
+// The half form of gemm_tc_kernel: p's segment bases, out and res point to __half; lds, tap strides and residual
+// strides count halves.  mb: the F16X3 hi copy's map; am.seg[s] (tc_encode_a16) for the segments tc_seg_tma takes,
+// am.out (fp16, tc_encode_rows16) in EPI_PLAIN.
+template <int EPI>   // EPI_PLAIN or EPI_SEMCH
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_h_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensorMap mb,
+                 const __grid_constant__ TcActMaps am, const int* __restrict__ sw) {
+  constexpr int STAGES = TCH_STAGES, SLOT = TC_H_SLOT;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  long long* rowbase = reinterpret_cast<long long*>(smem_raw);          // [3][128]
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t rb = (raw + TC_ROWBASE_BYTES + 1023) & ~1023u;        // ring base (shared address)
+  unsigned char* ring = smem_raw + (rb - raw);
+  const uint32_t full0 = rb + TC_H_RING;
+  const uint32_t empty0 = full0 + 8 * STAGES;
+
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int J = p.J;
+  int rt, ctile;
+  tc_tile(p, rt, ctile);
+  const int f0 = rt * p.fpt;
+  const int nf = min(p.fpt, p.F - f0);
+  const int vrows = nf * J;
+  const int n0 = ctile * TC_BN;
+  int tma_segs = 0;
+  for (int s = 0; s < p.nseg; ++s) tma_segs |= tc_seg_tma(p.seg[s]) << s;
+  const bool gather = tma_segs != (1 << p.nseg) - 1;
+
+  if (tid == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full0 + 8 * s, gather ? 1 + 128 : 1);
+      mbar_init(empty0 + 8 * s, 8);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  for (int i = tid; i < p.nseg * 128; i += TC_THREADS) {
+    int s = i >> 7, r = i & 127;
+    long long off = -1;
+    if (r < vrows) {
+      int fr = r / J, j = r - fr * J;
+      long long fin = map_frame(p.seg[s].map, f0 + fr);
+      off = (fin * J + j) * (long long)p.seg[s].ld;
+    }
+    rowbase[s * 128 + r] = off;
+  }
+  __syncthreads();
+
+  int nstages = 0;
+  for (int s = 0; s < p.nseg; ++s) nstages += p.seg[s].K / TC_KS;
+
+  if (warp < 4) {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (!gather && tid != 0) return;
+    const int q = tid & 3, rq = tid >> 2;                               // k-octet q of rows rq + 32 i
+    const uint32_t adst = TC_B16_BYTES + q * 2048 + rq * 16;
+    const int row0 = f0 * J;
+    int seg = 0, k0 = 0, kcol = 0, tap = 0, kin = 0;
+    for (int c = 0; c < nstages; ++c) {
+      const int slot = c % STAGES;
+      if (c >= STAGES) mbar_wait(empty0 + 8 * slot, (c / STAGES - 1) & 1);
+      const uint32_t sb = rb + slot * SLOT, full = full0 + 8 * slot;
+      const bool tma_a = (tma_segs >> seg) & 1;
+      if (tid == 0) {
+        mbar_arrive_expect_tx(full, TC_B16_BYTES + (tma_a ? TC_H_A_BYTES : 0));
+        tma_load_2d(sb, &mb, full, 2 * n0, (kcol + k0) >> 3);
+        if (tma_a) tma_load_3d(sb + TC_B16_BYTES, &am.seg[seg], full, 0, row0, kin >> 3);
+      }
+      const ASeg& sg = p.seg[seg];
+      if (tma_a) {
+        if (gather) mbar_arrive(full);
+      } else {
+        const __half* base = reinterpret_cast<const __half*>(sg.base);
+        const __half* src = base + tap * sg.tap_stride + kin + q * 8;
+#pragma unroll
+        for (int i = 0; i < TC_BM / 32; ++i) {
+          const long long off = rowbase[seg * 128 + rq + 32 * i];
+          cp_async16(sb + adst + i * 32 * 16, off >= 0 ? src + off : base, off >= 0 ? 16 : 0);
+        }
+        cp_async_arrive(full);
+      }
+      k0 += TC_KS;
+      kin += TC_KS;
+      if (kin == sg.Kc) { kin = 0; ++tap; }
+      if (k0 == sg.K) { kcol += sg.K; k0 = 0; tap = 0; ++seg; }
+    }
+    cp_async_wait_all();
+    return;
+  }
+
+  // consumers: warpgroup 1 + w multiplies rows 64 w .. 64 w + 63 (1024 B into each octet plane of the A stage)
+  setmaxnreg_inc<TC_CONSUMER_REGS>();
+  const int ct = tid - 128;
+  const int wg = ct >> 7, wq = (ct >> 5) & 3;
+  const int g = lane >> 2, t = lane & 3;
+  const int r0 = wg * 64 + wq * 16 + g;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int c = 0; c < nstages; ++c) {
+    const int slot = c % STAGES;
+    mbar_wait(full0 + 8 * slot, (c / STAGES) & 1);
+    const uint32_t sb = rb + slot * SLOT, sa = sb + TC_B16_BYTES + wg * 1024;
+    tile_fence(acc);
+    wgmma_fence();
+    wgmma_f16ss(acc, tc_bdesc(sa), tc_bdesc(sb), c > 0);
+    wgmma_f16ss(acc, tc_bdesc(sa + 4096), tc_bdesc(sb + 4096), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    tile_fence(acc);
+    if (lane == 0) mbar_arrive(empty0 + 8 * slot);
+  }
+  const float u = exp2i(-*sw);                                          // 2^-s_W
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] *= u;
+  epi_sync();
+  tc_tile(p, rt, ctile);
+  const int fe = rt * p.fpt, nfe = min(p.fpt, p.F - fe);
+
+  if constexpr (EPI == EPI_PLAIN) {
+    tc_store_plain_h(p, acc, ring, rb, am.out, r0, t, ct, fe, nfe * J, ctile * TC_BN);
+    return;
+  }
+  float* S = reinterpret_cast<float*>(ring);   // [128][TC_STG_LD]
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const int col = 8 * i + 2 * t;
+    *reinterpret_cast<float2*>(S + r0 * TC_STG_LD + col) = make_float2(acc[4 * i], acc[4 * i + 1]);
+    *reinterpret_cast<float2*>(S + (r0 + 8) * TC_STG_LD + col) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+  }
+  epi_sync();
+  const int ty = ct >> 4, tx = ct & 15;
+  float out[8][8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int r = (i < 4) ? (ty * 4 + i) : (64 + ty * 4 + i - 4);
+    const float4 a = *reinterpret_cast<const float4*>(S + r * TC_STG_LD + tx * 4);
+    const float4 b = *reinterpret_cast<const float4*>(S + r * TC_STG_LD + 64 + tx * 4);
+    out[i][0] = a.x; out[i][1] = a.y; out[i][2] = a.z; out[i][3] = a.w;
+    out[i][4] = b.x; out[i][5] = b.y; out[i][6] = b.z; out[i][7] = b.w;
+  }
+  epi_sync();
+  gemm_epilogue<EPI, __half>(p, out, reinterpret_cast<float*>(ring), ct, fe, nfe, nfe * J, ctile * TC_BN, ctile);
+}
+
 // W [N][K] -> hi / lo in the TMA-friendly layout [K/4][N][4] (both TF32 forms read hi = tf32(W)); lo may be null
 __global__ void tc_split_kernel(const float* __restrict__ w, float* __restrict__ hi, float* __restrict__ lo, int N, int K) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -662,6 +902,37 @@ inline int tc_encode_rows(CUtensorMap* m, const float* base, int cols, long long
   const cuuint32_t estr[2] = {1, 1};
   const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : -1;
+}
+
+// fp16 [rows][cols] at row stride ld halves, box {64, box_rows} (128-byte rows), 128-byte swizzle: the half form's
+// plain-epilogue output
+inline int tc_encode_rows16(CUtensorMap* m, const void* base, int cols, long long rows, int ld, int box_rows) {
+  tc_encode_fn enc = tc_get_encode();
+  if (!enc) return -1;
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  const cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : -1;
+}
+
+// An fp16 A segment [rows][Kc] at row stride ld halves as the half form's stages read it: dims {8, rows, Kc / 8},
+// strides {ld, 8} halves, box {8, 128, 4}, no swizzle, so a box lands as [4 k-octets][128 rows][8 halves]; rows past
+// the end read as zeros
+inline int tc_encode_a16(CUtensorMap* m, const void* base, int Kc, long long rows, int ld) {
+  tc_encode_fn enc = tc_get_encode();
+  if (!enc) return -1;
+  const cuuint64_t dims[3] = {8, (cuuint64_t)rows, (cuuint64_t)(Kc / 8)};
+  const cuuint64_t strides[2] = {(cuuint64_t)ld * 2, 16};
+  const cuuint32_t box[3] = {8, (cuuint32_t)TC_BM, (cuuint32_t)(TC_KS / 8)};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : -1;
 }
@@ -742,6 +1013,45 @@ inline bool tc_supported(const GemmP& p, int epi, const TcWeights& t) {
   return true;
 }
 
+// The shapes the half form takes: fp16 copies, and every fp16 operand 16-byte aligned with 16-byte row strides
+inline bool tc_supported_h(const GemmP& p, int epi, const TcWeights& t) {
+  if (!t.ready || !t.f16 || t.K != p.ldw || t.N < p.N || p.N % 4) return false;
+  if ((reinterpret_cast<uintptr_t>(p.out) & 15) || p.ld_out % 8) return false;
+  if (p.res && (p.res_ld % 2 || (reinterpret_cast<uintptr_t>(p.res) & 3))) return false;
+  for (int s = 0; s < p.nseg; ++s) {
+    const ASeg& sg = p.seg[s];
+    if (sg.K % TC_KS || sg.Kc % TC_KS || sg.ld % 8 || sg.tap_stride % 8) return false;
+    if (reinterpret_cast<uintptr_t>(sg.base) & 15) return false;
+  }
+  const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
+  return tch_smem_bytes(epi, p.J, p.fpt, hpt) <= TC_SMEM_MAX;
+}
+
+inline int tc_launch_h(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t) {
+  if (!t.f16 || epi == EPI_GLOBAL) return -1;
+  const dim3 grid((unsigned)(((p.F + p.fpt - 1) / p.fpt) * ((p.N + TC_BN - 1) / TC_BN)));
+  const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
+  const size_t smem = tch_smem_bytes(epi, p.J, p.fpt, hpt);
+  static bool attr_set[64][3];
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (!attr_set[dev & 63][epi]) {
+    const void* fn = epi == EPI_PLAIN ? (const void*)gemm_tc_h_kernel<EPI_PLAIN>
+                                      : (const void*)gemm_tc_h_kernel<EPI_SEMCH>;
+    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX);
+    if (e != cudaSuccess) return (int)e;
+    attr_set[dev & 63][epi] = true;
+  }
+  TcActMaps am{};
+  const long long rows = (long long)p.F * p.J;
+  for (int s = 0; s < p.nseg; ++s)
+    if (tc_seg_tma(p.seg[s]) && tc_encode_a16(&am.seg[s], p.seg[s].base, p.seg[s].Kc, rows, p.seg[s].ld)) return -1;
+  if (epi == EPI_PLAIN && tc_encode_rows16(&am.out, p.out, p.N, rows, p.ld_out, p.fpt * p.J)) return -1;
+  if (epi == EPI_PLAIN) gemm_tc_h_kernel<EPI_PLAIN><<<grid, TC_THREADS, smem, st>>>(p, t.map_h16hi, am, t.sw);
+  else gemm_tc_h_kernel<EPI_SEMCH><<<grid, TC_THREADS, smem, st>>>(p, t.map_h16hi, am, t.sw);
+  return (int)cudaGetLastError();
+}
+
 template <int PREC>
 inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t) {
   const dim3 grid((unsigned)(((p.F + p.fpt - 1) / p.fpt) * ((p.N + TC_BN - 1) / TC_BN)));
@@ -774,8 +1084,9 @@ inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeig
 }
 
 // One CTA per tile, tile = row tile * column tiles + column tile (the column tile fastest, see gemm_tc_kernel).
-// prec: TC_3XTF32 (needs t.f16 false), TC_1XTF32 or TC_F16X3 (needs t.f16).
+// prec: TC_3XTF32 (needs t.f16 false), TC_1XTF32, TC_F16X3 or TC_F16 (both need t.f16).
 inline int tc_launch(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t, int prec) {
+  if (prec == TC_F16) return tc_launch_h(st, epi, p, t);
   if (prec == TC_1XTF32) return tc_launch_prec<TC_1XTF32>(st, epi, p, t);
   if (prec == TC_F16X3) return t.f16 ? tc_launch_prec<TC_F16X3>(st, epi, p, t) : -1;
   return t.f16 ? -1 : tc_launch_prec<TC_3XTF32>(st, epi, p, t);

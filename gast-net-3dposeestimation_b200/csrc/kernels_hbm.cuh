@@ -25,10 +25,11 @@ constexpr int EXS_ROWS = 128;
 constexpr int EXS_THREADS = 256;
 constexpr int EXS_CHUNK = 4 * EXS_THREADS;               // channels per block: 4 per thread
 constexpr int EXP_MAXKF = 10;   // taps * in_features supported by the register path (3*2 = 6; 5*2 = 10)
-template <int KFT>   // register-resident K = taps * in_features rounded up: 6 (3 taps x 2) or EXP_MAXKF
+// Act: the activation type of x and out (float, or __half in a half forward)
+template <int KFT, typename Act>   // register-resident K = taps * in_features rounded up: 6 (3 taps x 2) or EXP_MAXKF
 __global__ void __launch_bounds__(EXS_THREADS)
-expand_rows_kernel(const float* __restrict__ x, const float* __restrict__ We, const float* __restrict__ be,
-                   float* __restrict__ out, long long rows, int J, int T, int T0, int stride, int taps, int Fin, int C) {
+expand_rows_kernel(const Act* __restrict__ x, const float* __restrict__ We, const float* __restrict__ be,
+                   Act* __restrict__ out, long long rows, int J, int T, int T0, int stride, int taps, int Fin, int C) {
   constexpr int KP = (KFT + 3) & ~3;                      // padded row of staged inputs (float4 reads)
   __shared__ __align__(16) float xs[EXS_ROWS * KP];
   const int tid = threadIdx.x;
@@ -43,7 +44,7 @@ expand_rows_kernel(const float* __restrict__ x, const float* __restrict__ We, co
       const int f = row / J, j = row - f * J;
       const int b = f / T0, t = f - b * T0;
       const int kk = k / Fin, i = k - kk * Fin;
-      v = __ldg(x + (((long long)b * T + (long long)t * stride + kk) * J + j) * Fin + i);
+      v = ld1(x + (((long long)b * T + (long long)t * stride + kk) * J + j) * Fin + i);
     }
     xs[e] = v;
   }
@@ -62,7 +63,7 @@ expand_rows_kernel(const float* __restrict__ x, const float* __restrict__ We, co
   const float4 b4 = ldg4(be + c);
   __syncthreads();
   if (rsub >= rpp) return;                                // (256 % cq != 0: the surplus threads have no row)
-  float* op = out + (r0 + rsub) * C + c;
+  Act* op = out + (r0 + rsub) * C + c;
   const long long ostep = (long long)rpp * C;
 #pragma unroll 4
   for (int rr = rsub; rr < nrows; rr += rpp, op += ostep) {
@@ -78,7 +79,7 @@ expand_rows_kernel(const float* __restrict__ x, const float* __restrict__ We, co
       v0 = fmaf(w[0][k], xv[k], v0); v1 = fmaf(w[1][k], xv[k], v1);
       v2 = fmaf(w[2][k], xv[k], v2); v3 = fmaf(w[3][k], xv[k], v3);
     }
-    *reinterpret_cast<float4*>(op) = make_float4(fmaxf(v0, 0.f), fmaxf(v1, 0.f), fmaxf(v2, 0.f), fmaxf(v3, 0.f));
+    st4(op, make_float4(fmaxf(v0, 0.f), fmaxf(v1, 0.f), fmaxf(v2, 0.f), fmaxf(v3, 0.f)));
   }
 }
 

@@ -10,19 +10,19 @@ namespace gast {
 // The theta/phi 1x1 convs followed by the concat-project conv (global_attention.py:60-72)
 // collapse to these 2 dot products per head: f[i,j] = a_i + b_j.
 // ---------------------------------------------------------------------------------------
-template <int Q>
-__global__ void rowdot_kernel(const float* __restrict__ X, int ldx, const float* __restrict__ U,
+template <int Q, typename T>
+__global__ void rowdot_kernel(const T* __restrict__ X, int ldx, const float* __restrict__ U,
                               const float* __restrict__ cab, float* __restrict__ ab,
                               long long rows, int K) {
   long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
   if (row >= rows) return;
-  const float* xr = X + row * ldx;
+  const T* xr = X + row * ldx;
   float acc[Q];
 #pragma unroll
   for (int q = 0; q < Q; ++q) acc[q] = 0.f;
   for (int k = lane * 4; k < K; k += 128) {
-    float4 xv = ldg4(xr + k);
+    float4 xv = ld4(xr + k);
 #pragma unroll
     for (int q = 0; q < Q; ++q) {
       float4 u = ldg4(U + (long long)q * K + k);
@@ -39,7 +39,8 @@ __global__ void rowdot_kernel(const float* __restrict__ X, int ldx, const float*
 
 // Q = 8 (4 heads) version: U staged in shared memory, a warp walks rows with a grid stride, and the
 // 8 partial sums are reduced with a halving butterfly (9 shuffles instead of 40).
-__global__ void rowdot8_kernel(const float* __restrict__ X, int ldx, const float* __restrict__ U,
+template <typename T>
+__global__ void rowdot8_kernel(const T* __restrict__ X, int ldx, const float* __restrict__ U,
                                const float* __restrict__ cab, float* __restrict__ ab, long long rows, int K) {
   extern __shared__ __align__(16) float us[];          // [8][K]
   for (int i = threadIdx.x * 4; i < 8 * K; i += blockDim.x * 4)
@@ -55,14 +56,14 @@ __global__ void rowdot8_kernel(const float* __restrict__ X, int ldx, const float
   for (long long row0 = warp; row0 < rows; row0 += 2 * nwarps) {
     const long long row1 = row0 + nwarps;
     const bool has1 = row1 < rows;
-    const float* xr0 = X + row0 * ldx;
-    const float* xr1 = X + (has1 ? row1 : row0) * ldx;
+    const T* xr0 = X + row0 * ldx;
+    const T* xr1 = X + (has1 ? row1 : row0) * ldx;
     float va[8], vb[8];
 #pragma unroll
     for (int q = 0; q < 8; ++q) { va[q] = 0.f; vb[q] = 0.f; }
     for (int k = lane * 4; k < K; k += 128) {
-      const float4 xa = ldg4(xr0 + k);
-      const float4 xb = ldg4(xr1 + k);
+      const float4 xa = ld4(xr0 + k);
+      const float4 xb = ld4(xr1 + k);
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
         const float4 u = *reinterpret_cast<const float4*>(us + q * K + k);
@@ -98,22 +99,23 @@ __global__ void rowdot8_kernel(const float* __restrict__ X, int ldx, const float
 }
 
 // shrink (gast_net.py:60,99): y[row][o] = X[row,:] . Ws[o,:], o < 3.   Warp per row.
-__global__ void shrink_kernel(const float* __restrict__ X, int ldx, const float* __restrict__ Ws,
-                              float* __restrict__ y, long long rows, int K) {
+template <typename T>
+__global__ void shrink_kernel(const T* __restrict__ X, int ldx, const float* __restrict__ Ws,
+                              T* __restrict__ y, long long rows, int K) {
   long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
   if (row >= rows) return;
-  const float* xr = X + row * ldx;
+  const T* xr = X + row * ldx;
   float a0 = 0.f, a1 = 0.f, a2 = 0.f;
   for (int k = lane * 4; k < K; k += 128) {
-    float4 xv = ldg4(xr + k);
+    float4 xv = ld4(xr + k);
     float4 w0 = ldg4(Ws + k), w1 = ldg4(Ws + K + k), w2 = ldg4(Ws + 2 * K + k);
     a0 = fmaf(xv.x, w0.x, fmaf(xv.y, w0.y, fmaf(xv.z, w0.z, fmaf(xv.w, w0.w, a0))));
     a1 = fmaf(xv.x, w1.x, fmaf(xv.y, w1.y, fmaf(xv.z, w1.z, fmaf(xv.w, w1.w, a1))));
     a2 = fmaf(xv.x, w2.x, fmaf(xv.y, w2.y, fmaf(xv.z, w2.z, fmaf(xv.w, w2.w, a2))));
   }
   a0 = warp_sum(a0); a1 = warp_sum(a1); a2 = warp_sum(a2);
-  if (lane == 0) { y[row * 3 + 0] = a0; y[row * 3 + 1] = a1; y[row * 3 + 2] = a2; }
+  if (lane == 0) { st1(y + row * 3, a0); st1(y + row * 3 + 1, a1); st1(y + row * 3 + 2, a2); }
 }
 
 // ---------------------------------------------------------------------------------------
@@ -170,9 +172,10 @@ constexpr int MIX_JMAX = 20;
 constexpr int MIX_JP = 20;        // padded row length of an attention row in shared memory (float4 reads)
 
 // 17 float4 of g in registers per thread: 116 registers, 16 warps per SM.
+template <typename T>
 __global__ void __launch_bounds__(MIX_THREADS, 1)
-global_mix_kernel(const float* __restrict__ G, int ldg, const float* __restrict__ ab, const float* __restrict__ ck,
-                  float* __restrict__ Y, int ldy, long long F, int J, int heads, int Cg, int fpb) {
+global_mix_kernel(const T* __restrict__ G, int ldg, const float* __restrict__ ab, const float* __restrict__ ck,
+                  T* __restrict__ Y, int ldy, long long F, int J, int heads, int Cg, int fpb) {
   extern __shared__ __align__(16) float att_s[];            // [fpb][heads][J][MIX_JP]
   const int tid = threadIdx.x;
   const int H2 = 2 * heads;
@@ -218,12 +221,12 @@ global_mix_kernel(const float* __restrict__ G, int ldg, const float* __restrict_
     if (f >= F) continue;
     const int h = c / Cg;
     float4 g[MIX_JMAX];
-    const float* gp = G + (f * J) * (long long)ldg + c;
+    const T* gp = G + (f * J) * (long long)ldg + c;
 #pragma unroll
     for (int j = 0; j < MIX_JMAX; ++j)
-      if (j < J) g[j] = ldg4(gp + (long long)j * ldg);
+      if (j < J) g[j] = ld4(gp + (long long)j * ldg);
     const float* arow = att_s + (size_t)((fs * heads + h) * J) * MIX_JP;
-    float* yp = Y + (f * J) * (long long)ldy + c;
+    T* yp = Y + (f * J) * (long long)ldy + c;
     for (int i = 0; i < J; ++i) {
       float a[MIX_JMAX];
 #pragma unroll
@@ -238,7 +241,7 @@ global_mix_kernel(const float* __restrict__ G, int ldg, const float* __restrict_
           o.x = fmaf(a[j], g[j].x, o.x); o.y = fmaf(a[j], g[j].y, o.y);
           o.z = fmaf(a[j], g[j].z, o.z); o.w = fmaf(a[j], g[j].w, o.w);
         }
-      *reinterpret_cast<float4*>(yp + (long long)i * ldy) = o;
+      st4(yp + (long long)i * ldy, o);
     }
   }
 }

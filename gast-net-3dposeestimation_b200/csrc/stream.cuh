@@ -255,6 +255,7 @@ struct StreamPlan {
 
 static int stream_check(const gast_handle* h) {
   if (h->cfg.kind != GAST_KIND_MODEL) return fail("streaming is implemented for the MODEL kind only");
+  if (half_check(h, "streaming")) return 1;
   if (h->cfg.dense) return fail("the dense ablation has no streaming form");
   // checked before a push touches the stream state (launch_expand checks it again for the forward)
   if (h->cfg.filter_widths[0] * h->cfg.in_features > EXP_MAXKF)

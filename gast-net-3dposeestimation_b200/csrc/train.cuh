@@ -495,7 +495,7 @@ static int train_forward(gast_handle* h, TCtx& c, TrainState& ts, const float* x
   const int Cl = C << L;
   const long long M = (long long)B * g.T_out * J;
   const float* ws = c.param("shrink.weight", (int64_t)3 * Cl);
-  if (y) c.launch(shrink_kernel, cdiv(M * 32, 256), 256, 0, cur, Cl, ws, y, M, Cl);
+  if (y) c.launch(shrink_kernel<float>, cdiv(M * 32, 256), 256, 0, cur, Cl, ws, y, M, Cl);
   return 0;
 }
 

@@ -18,6 +18,7 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_receptive_field', 'gast_workspace_bytes', 'gast_forward', 'gast_forward_mpjpe',
            'gast_last_launch_count', 'gast_last_tc_launch_count', 'gast_set_timing',
            'gast_get_timings', 'gast_set_gemm_core', 'gast_set_precision', 'gast_set_train_precision',
+           'gast_set_activation_dtype',
            'gast_last_wgrad_tc_launch_count', 'gast_debug_gemm', 'gast_debug_wgrad', 'gast_debug_set_gemm_audit',
            'gast_debug_gemm_audit_skips', 'gast_bind_grads',
            'gast_train_workspace_bytes', 'gast_forward_train', 'gast_backward', 'gast_backward_input',
@@ -115,6 +116,8 @@ def load():
     lib.gast_set_gemm_core.restype = C.c_int
     lib.gast_set_precision.argtypes = [vp, C.c_int32]
     lib.gast_set_precision.restype = C.c_int
+    lib.gast_set_activation_dtype.argtypes = [vp, C.c_int32]
+    lib.gast_set_activation_dtype.restype = C.c_int
     lib.gast_set_train_precision.argtypes = [vp, C.c_int32]
     lib.gast_set_train_precision.restype = C.c_int
     lib.gast_last_wgrad_tc_launch_count.argtypes = [vp]

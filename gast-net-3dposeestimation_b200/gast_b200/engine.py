@@ -77,6 +77,29 @@ def _fp32_only(module, what):
                         "engine.set_precision(model, 'fp32') to train or differentiate it" % what)
 
 
+_HALF_ONLY = ('the model is half precision (model.half()), which runs inference only: the eval-mode forward under '
+              'torch.no_grad() / torch.inference_mode() (model(x), run_model_chunked); call model.float() for %s')
+
+
+def model_dtype(module, what):
+    """torch.float32 or torch.float16, the floating dtype of all of the module's parameters and buffers: a model
+    runs in half once model.half() made every one of them fp16.  A mix of dtypes, or any other, raises, as a torch
+    module of mixed dtypes does."""
+    dts = {v.dtype for _, v in named_tensors(module) if v.is_floating_point()}
+    if not dts or dts == {torch.float32}:
+        return torch.float32
+    if dts == {torch.float16}:
+        return torch.float16
+    raise GastError("%s: the module's parameters and buffers must all be float32 or all float16 (model.float() / "
+                    "model.half()), got %s" % (what, ', '.join(sorted(str(d) for d in dts))))
+
+
+def refuse_half(module, what, instead):
+    """raise when `module` is a half model: `what` runs in float32 only"""
+    if any(v.dtype == torch.float16 for _, v in named_tensors(module)):
+        raise GastError('%s: %s' % (what, _HALF_ONLY % instead))
+
+
 def _check(rc, what):
     if rc != 0:
         raise GastError('%s: %s' % (what, L.last_error()))
@@ -179,6 +202,8 @@ class _Handle(object):
         self.core = None
         self.precision = 0
         self.train_precision = 0
+        self.act_dtype = 0               # gast_set_activation_dtype: 1 (GAST_F16) for a half model
+        self.f32 = None                  # a half model's float32 copies of its tensors, bound in their place
 
     def __del__(self):
         try:
@@ -190,7 +215,12 @@ class _Handle(object):
 
     def apply_core(self, module):
         """hand the set_gemm_core() choice and the module's set_precision() and set_training_precision() to the
-        library handle (every forward, training or eval, and every stream push)"""
+        library handle (every forward, training or eval, and every stream push), and for a whole model its activation
+        type: fp16 for a half model.  Half goes off first and on last, as the library refuses TF32 and the FFMA core in
+        half."""
+        act = 1 if self.kind == L.KIND_MODEL and model_dtype(module, 'forward') == torch.float16 else 0
+        if act == 0 and self.act_dtype != 0:
+            self._set_act(0)
         if _FORCE_CORE['core'] != self.core:
             _check(self.lib.gast_set_gemm_core(self.h, _FORCE_CORE['core']), 'gast_set_gemm_core')
             self.core = _FORCE_CORE['core']
@@ -202,6 +232,12 @@ class _Handle(object):
         if tprec != self.train_precision:
             _check(self.lib.gast_set_train_precision(self.h, tprec), 'gast_set_train_precision')
             self.train_precision = tprec
+        if act != self.act_dtype:
+            self._set_act(act)
+
+    def _set_act(self, act):
+        _check(self.lib.gast_set_activation_dtype(self.h, act), 'gast_set_activation_dtype')
+        self.act_dtype = act
 
     def refresh(self, module, stream):
         """(re)bind + prepare when any parameter/buffer moved or changed."""
@@ -209,7 +245,10 @@ class _Handle(object):
         self.apply_core(module)
         if sig == self.sig:
             return
-        _bind(self, 'gast_bind', named_tensors(module))
+        items = named_tensors(module)
+        # a half model: the library folds float32 parameters, so float32 copies are bound (kept until the next change)
+        self.f32 = [(k, v.float() if v.dtype == torch.float16 else v) for k, v in items] if self.act_dtype else None
+        _bind(self, 'gast_bind', self.f32 or items)
         _check(self.lib.gast_prepare(self.h, C.c_void_p(stream)), 'gast_prepare')
         self.sig = sig
 
@@ -252,6 +291,9 @@ def _bind(handle, entry, items):
                             % (k, v.device, handle.device))
         if not v.is_contiguous():
             raise GastError('parameter %r is not contiguous' % k)
+        if v.is_floating_point() and v.dtype != torch.float32:
+            raise GastError('parameter %r is %s: the library binds float32 tensors (a whole model in half precision binds '
+                            'float32 copies; call .float() on a sub-module)' % (k, v.dtype))
         keys[i] = k.encode()
         ptrs[i] = v.data_ptr()
         numel[i] = v.numel()
@@ -269,6 +311,17 @@ def _cuda_f32(x, what):
         raise GastError('%s: input must be a CUDA tensor -- this implementation has no CPU path' % what)
     if x.dtype != torch.float32:
         raise GastError('%s: input must be float32 (got %s)' % (what, x.dtype))
+    return x.contiguous()
+
+
+def _cuda_input(x, dtype, what):
+    """x as a contiguous CUDA tensor of the model's dtype (float32, or float16 for a half model); anything else raises"""
+    if dtype == torch.float32:
+        return _cuda_f32(x, what)
+    if not isinstance(x, torch.Tensor) or not x.is_cuda:
+        raise GastError('%s: input must be a CUDA tensor -- this implementation has no CPU path' % what)
+    if x.dtype != dtype:
+        raise GastError('%s: the model is %s, the input %s (convert one of them)' % (what, dtype, x.dtype))
     return x.contiguous()
 
 
@@ -449,9 +502,10 @@ def _strided_now(module, T):
 
 def run_model(module, x):
     """SpatioTemporalModelBase.forward (gast_net.py:84-104) on the CUDA library."""
-    x = _cuda_f32(x, 'SpatioTemporalModel.forward')
+    x = _cuda_input(x, model_dtype(module, 'SpatioTemporalModel.forward'), 'SpatioTemporalModel.forward')
     h = model_handle(module, x.device)
     if module.training:
+        refuse_half(module, 'SpatioTemporalModel.forward in train mode', 'training')
         _fp32_only(module, 'SpatioTemporalModel.forward in train mode')
         # both of the reference's training models: Optimized1f (main.py:166-170) and, with
         # --disable-optimizations / stride > 1, the dilated SpatioTemporalModel (main.py:171-175)
@@ -469,6 +523,7 @@ def _run_eval(module, h, x, max_frames, what):
     strided_now = _strided_now(module, int(x.shape[1]))
     np_ = named_params(module) if torch.is_grad_enabled() else []
     if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for _, p in np_)):
+        refuse_half(module, '%s with autograd (requires_grad input or parameters)' % what, 'gradients')
         _fp32_only(module, '%s with autograd (requires_grad input or parameters)' % what)
         return _EvalFn.apply(module, h, x, strided_now, max_frames, [k for k, _ in np_], *[p for _, p in np_])
     return _chunked_forward(module, h, x, strided_now, max_frames)
@@ -482,7 +537,7 @@ def _eval_forward(module, h, x, strided_now, target=None):
     with torch.cuda.device(dev):
         st = _stream(dev)
         h.refresh(module, st)
-        y = _new_output(module, h, B, T, strided_now, dev)
+        y = _new_output(module, h, B, T, strided_now, dev, x.dtype)
         if target is None:
             h.forward(x, y, B, T, strided_now, st)
             return y
@@ -494,18 +549,19 @@ def _eval_forward(module, h, x, strided_now, target=None):
     return y, loss
 
 
-def _new_output(module, h, B, T, strided_now, dev):
-    """an empty (B, T_out, J, 3) model output for an input of T frames on the schedule `strided_now`"""
+def _new_output(module, h, B, T, strided_now, dev, dtype=torch.float32):
+    """an empty (B, T_out, J, 3) model output of `dtype` for an input of T frames on the schedule `strided_now`"""
     T_out = h.lib.gast_out_frames(h.h, T, strided_now)
     if T_out <= 0:
         raise GastError('forward: %s' % L.last_error())
-    return torch.empty((B, T_out, module.num_joints_in, 3), dtype=torch.float32, device=dev)
+    return torch.empty((B, T_out, module.num_joints_in, 3), dtype=dtype, device=dev)
 
 
 def run_model_mpjpe(module, x, target):
     """`predicted = model(x); error = mpjpe(predicted, target)` (main.py:270-300, common/loss.py:5-11) as ONE library
     call: the loss is taken in the shrink kernel's epilogue.  Eval mode; returns (predicted, loss) with loss a 0-d
     CUDA tensor.  (The training loss goes through gast_b200.pipeline.mpjpe, which also produces the gradient.)"""
+    refuse_half(module, 'run_model_mpjpe', 'the fused mpjpe')
     x = _cuda_f32(x, 'run_model_mpjpe')
     target = _cuda_f32(target, 'run_model_mpjpe (target)')
     _no_train(module, 'run_model_mpjpe')
@@ -524,7 +580,7 @@ def run_model_chunked(module, x, max_frames):
     model(x)'s backward up to summation order across passes (the same kernels in the same order when one pass covers
     the call).  Train mode
     raises: batch statistics span the whole batch and cannot be chunked."""
-    x = _cuda_f32(x, 'run_model_chunked')
+    x = _cuda_input(x, model_dtype(module, 'run_model_chunked'), 'run_model_chunked')
     if module.training:
         raise GastError('run_model_chunked: the model is in train mode, whose BatchNorm statistics span the whole '
                         'batch and cannot be chunked; call .eval()')
@@ -544,7 +600,7 @@ def _chunked_forward(module, h, x, strided_now, max_frames):
     with torch.cuda.device(dev):
         st = _stream(dev)
         h.refresh(module, st)
-        y = _new_output(module, h, B, T, strided_now, dev)
+        y = _new_output(module, h, B, T, strided_now, dev, x.dtype)
         need = _check_size(h.lib.gast_chunked_workspace_bytes(h.h, B, T, strided_now, max_frames, 0),
                            'gast_chunked_workspace_bytes')
         ws = torch.empty(need, dtype=torch.uint8, device=dev)
@@ -556,6 +612,7 @@ def _chunked_forward(module, h, x, strided_now, max_frames):
 def _run_module(module, x, what, kind, cfg, width_out, masks=None, train_ok=False):
     """The forward of a sub-module on its own, channels-last: x (..., J, C) -> (..., J, width_out), all leading rows in
     one library call.  Only a sub-module without BatchNorm or dropout (train_ok) also runs in train mode."""
+    refuse_half(module, what, 'a sub-module on its own (only the whole model runs in half)')
     x = _cuda_f32(x, what)
     if not train_ok:
         _no_train(module, what)
@@ -647,7 +704,8 @@ def profile_forward(module, x, reps=5):
     ng = sum(v for k, v in n_launch.items() if fam(k))
     tc = int(lib.gast_last_tc_launch_count(h.h))
     # fp32 grade: three fp16 products on scaled operands, as precise as 3xTF32 (gemm_tc.cuh)
-    tc_name = 'wgmma-1xtf32' if get_precision(module) == 'tf32' else 'wgmma-3xtf32-grade-3xfp16'
+    tc_name = ('wgmma-fp16' if model_dtype(module, 'profile_forward') == torch.float16
+               else 'wgmma-1xtf32' if get_precision(module) == 'tf32' else 'wgmma-3xtf32-grade-3xfp16')
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     with torch.no_grad():
         e0.record()

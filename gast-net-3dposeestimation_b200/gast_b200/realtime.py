@@ -222,6 +222,7 @@ class PoseStream(object):
             raise engine.GastError('%s needs a model of the drop-in classes (model/gast_net.py)' % name)
         if getattr(model_pos, '_gast_dense', False):
             raise engine.GastError('%s: the dense ablation has no streaming form' % name)
+        engine.refuse_half(model_pos, name, 'streaming')
         if device is None:
             device = next(model_pos.parameters()).device
         self.device = torch.device(device)
@@ -783,6 +784,7 @@ def lift_sequences(model_pos, sequences, n_streams=64, chunk=256, augment=False,
     `PoseStream` and pushed `chunk` frames at a time; a stream starts its next sequence at the first chunk after the
     last pose of its previous one.  The library's scratch memory depends on (n_streams, chunk), not on T_i."""
     from . import engine
+    engine.refuse_half(model_pos, 'lift_sequences', 'streaming')
     dev = next(model_pos.parameters()).device
     seqs = [torch.as_tensor(s, dtype=torch.float32).to(dev) for s in sequences]
     J, F = int(model_pos.num_joints_in), int(model_pos.in_features)

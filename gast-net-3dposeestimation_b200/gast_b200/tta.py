@@ -10,7 +10,7 @@ import ctypes as C
 import torch
 
 from . import _lib as L
-from .engine import GastError, _check, _cuda_f32, _ilist, _stream
+from .engine import GastError, _check, _cuda_f32, _ilist, _stream, refuse_half
 
 
 def tta_prepare(seq, pad, causal_shift, kps_left, kps_right):
@@ -44,6 +44,7 @@ def tta_merge(pred, joints_left, joints_right):
 
 def evaluate_sequence(model_pos, keypoints, kps_left, kps_right, joints_left, joints_right, causal=False):
     """keypoints (T,J,2) (numpy or tensor, normalised screen coordinates) -> (T,J,3) CUDA tensor."""
+    refuse_half(model_pos, 'tta.evaluate_sequence', 'test-time augmentation')
     dev = next(model_pos.parameters()).device
     seq = torch.as_tensor(keypoints, dtype=torch.float32).to(dev)
     pad = (model_pos.receptive_field() - 1) // 2

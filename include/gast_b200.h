@@ -144,6 +144,26 @@ int gast_set_gemm_core(gast_t* h, int32_t core);
  * gast_prepare, costs nothing and does not invalidate stream `state`. */
 int gast_set_precision(gast_t* h, int32_t mode);
 
+/* Activation type of the model forward (MODEL kind only):
+ *   GAST_F32 (default): every activation, x and y are float32.
+ *   GAST_F16: gast_forward, gast_forward_chunked, gast_workspace_bytes and gast_chunked_workspace_bytes(.., 0) take
+ *       __half x and y, and every activation in the workspace is fp16 (the attention row dots stay fp32).  The
+ *       parameters are still bound as float32 and folded exactly as before.  Every GEMM runs the tensor-core core's
+ *       half form: one fp16 product per multiply-add on fp16(W 2^s_W) (the fp32-grade form's weight copy), fp32
+ *       accumulation, the weight scale and the fused epilogues applied in fp32, each stored value rounded once to fp16
+ *       (DESIGN.md §4.1).  Expand, row dots, the attention mix and shrink read and write fp16 and compute in fp32.
+ *       A GEMM the tensor-core core does not take (widths that are not multiples of 32) fails the forward: there is no
+ *       FFMA core in half.  Inference only: while it is set, gast_forward_mpjpe, gast_forward_train, gast_backward,
+ *       gast_backward_input, gast_eval_backward(_chunked), gast_chunked_workspace_bytes(.., 1), the training and
+ *       eval-backward workspace queries and every gast_stream_* entry fail, as do gast_set_gemm_core(h, 1) and
+ *       gast_set_precision(h, 1) (TF32 and half are separate modes: neither picks the other).  Setting GAST_F16 fails
+ *       on a sub-module kind, a TF32 handle, one forced onto the FFMA core, channels that are not a multiple of 32
+ *       (the widths the half form takes) or more than 20 joints (the attention mix then needs the fused epilogue,
+ *       which has no half form), before anything is launched.
+ * bf16 is not offered (8 significant bits are about a centimetre on these poses).  Needs no gast_prepare. */
+enum { GAST_F32 = 0, GAST_F16 = 1 };
+int gast_set_activation_dtype(gast_t* h, int32_t dtype);
+
 /* Arithmetic of training and of every gradient: gast_forward_train, gast_backward, gast_backward_input and
  * gast_eval_backward (its recompute of the activations included):
  *   0 = fp32-grade (default): 3xTF32 tensor-core GEMMs, weight gradients in exact fp32 (FFMA).
@@ -503,8 +523,9 @@ int gast_adam_step(const int64_t* table, int32_t n_chunks, float* exp_avg, float
 
 /* Test/probe entry (not on the forward path): out[M,N] = A[M,K] . W[N,K]^T on one GEMM core
  * (core 0 = tensor cores, tc_mode 0 = fp32-grade as inference runs it, three scaled fp16 products (F16X3),
- * 1 = single-pass TF32, or 3 = fp32-grade as training runs it, three TF32 products (3xTF32); tc_mode 2 is not a
- * mode and is refused; core 1 = FFMA, tc_mode 0).  Runs once, then `reps` timed launches
+ * 1 = single-pass TF32, 3 = fp32-grade as training runs it, three TF32 products (3xTF32), or 16 = the half form of
+ * gast_set_activation_dtype(h, GAST_F16): A and out hold __half values, W float32; every other tc_mode is refused;
+ * core 1 = FFMA, tc_mode 0).  Runs once, then `reps` timed launches
  * (CUDA events) whose mean duration is written to *ms_out (host).  Synchronises the stream. */
 int gast_debug_gemm(const float* A, const float* W, float* out, int32_t M, int32_t N, int32_t K,
                     int32_t core, int32_t tc_mode, int32_t reps, float* ms_out, void* stream);
@@ -538,7 +559,7 @@ typedef struct gast_gemm_audit {
   int64_t index;                         /* running index of the handle's audited launches */
   int32_t epi;                           /* 0 plain, 1 SemCH, 2 global attention */
   int32_t core;                          /* the core that runs: 0 tensor cores, 1 FFMA */
-  int32_t tc_form;                       /* tensor cores: 0 3xTF32, 1 1xTF32, 2 F16X3; FFMA: -1 */
+  int32_t tc_form;                       /* tensor cores: 0 3xTF32, 1 1xTF32, 2 F16X3, 3 half (A, out, res fp16); FFMA: -1 */
   int32_t tma_mask;                      /* tensor cores: bit s set when segment s is fed by TMA */
   int32_t nseg;
   gast_gemm_audit_seg seg[3];

@@ -1,16 +1,19 @@
-"""GPU: the single-pass TF32 precision (engine.set_precision(model, 'tf32')) against the default fp32-grade one, in
-one process: the card's name, power limit and SM clock, then
-  * the headline workload (4096 clips x 27 frames x 17 joints, 27-frame/128ch model) in fp32 and TF32, alternated
-    three times each;
+"""GPU: the single-pass TF32 precision (engine.set_precision(model, 'tf32')) and the half model (model.half(), fp16
+weights, inputs and activations) against the default fp32-grade one, in one process: the card's name, power limit and
+SM clock, then
+  * the headline workload (4096 clips x 27 frames x 17 joints, 27-frame/128ch model) in fp32, TF32 and fp16,
+    alternated three times each;
   * the 81-frame/64ch and 19-joint workloads;
-  * per-GEMM device times of the headline forward in both modes (gast_set_timing);
-  * PoseStream with 1024 streams: single pushes and push_frames at K = 64;
-  * the distance between fp32 and TF32 poses: max |dy| / max |y| and the mean joint distance.
+  * per-GEMM device times of the headline forward in every mode (gast_set_timing);
+  * PoseStream with 1024 streams (fp32 and TF32; half does not stream): single pushes and push_frames at K = 64;
+  * the distance of the TF32 and fp16 poses from the fp32-grade ones: max |dy| / max |y| and the mean joint distance
+    (the half model's input is the fp32 input rounded to fp16, its weights the fp32 model's rounded to fp16).
 CUDA events after a warm-up; one JSON line per measurement.
 
     python tools/precision_bench.py [--headline-only] [--steps K]
 """
 import argparse
+import copy
 import ctypes as C
 import json
 import os
@@ -55,21 +58,37 @@ def clips_per_s(m, x, steps):
     return x.shape[0] / ms * 1e3, ms
 
 
+MODES = ('fp32', 'tf32', 'fp16')
+
+
+def in_mode(m, mh, x, xh, mode):
+    """(model, input) of a mode: the fp32 model at set_precision(mode), or its half copy mh with the fp16 input"""
+    if mode == 'fp16':
+        return mh, xh
+    engine.set_precision(m, mode)
+    return m, x
+
+
 def emit(d):
     print(json.dumps(d), flush=True)
 
 
-def accuracy(m, x):
+def accuracy(m, mh, x, xh):
+    """per reduced mode, its poses' distance from the fp32-grade poses"""
+    out = {}
     with torch.no_grad():
         engine.set_precision(m, 'fp32')
         y32 = m(x).double()
         engine.set_precision(m, 'tf32')
         yt = m(x).double()
+        yh = mh(xh).double()
     engine.set_precision(m, 'fp32')
-    d = yt - y32
-    return {'max_abs_dy': float(d.abs().max()), 'max_abs_y': float(y32.abs().max()),
-            'max_dy_over_max_y': float(d.abs().max() / y32.abs().max()),
-            'mean_joint_distance': float(d.norm(dim=-1).mean())}
+    for mode, y in (('tf32', yt), ('fp16', yh)):
+        d = y - y32
+        out[mode] = {'max_abs_dy': float(d.abs().max()), 'max_abs_y': float(y32.abs().max()),
+                     'max_dy_over_max_y': float(d.abs().max() / y32.abs().max()),
+                     'mean_joint_distance': float(d.norm(dim=-1).mean())}
+    return out
 
 
 def per_gemm(m, x, J, ch, fw, reps=5):
@@ -108,34 +127,39 @@ def main():
     emit({'card': card(), 'library': os.environ.get('GAST_B200_LIB', 'in-tree')})
     J, fw, ch = 17, [3, 3, 3], 128
     m = model(J, fw, ch)
+    mh = copy.deepcopy(m).half()
     x = torch.from_numpy(synth.synth_input(4096, 27, J, 2, seed=5)).cuda()
+    xh = x.half()
     for rnd in range(3):
-        for prec in ('fp32', 'tf32'):
-            engine.set_precision(m, prec)
-            cps, ms = clips_per_s(m, x, args.steps)
+        for prec in MODES:
+            mm, xx = in_mode(m, mh, x, xh, prec)
+            cps, ms = clips_per_s(mm, xx, args.steps)
             emit({'workload': 'headline 4096x27x17, 27-frame/128ch', 'round': rnd, 'precision': prec,
                   'clips_per_s': round(cps), 'ms_per_step': round(ms, 3)})
-    emit(dict(workload='headline accuracy (synthetic weights)', **accuracy(m, x)))
+    emit(dict(workload='headline accuracy (synthetic weights)', **accuracy(m, mh, x, xh)))
     if args.headline_only:
         return
-    for prec in ('fp32', 'tf32'):
-        engine.set_precision(m, prec)
-        rows = per_gemm(m, x, J, ch, fw)
+    for prec in MODES:
+        mm, xx = in_mode(m, mh, x, xh, prec)
+        rows = per_gemm(mm, xx, J, ch, fw)
         emit({'per_gemm_ms': prec, 'total_ms': round(sum(r[-1] for r in rows), 3),
               'gemms': [[r[0], r[1], r[2], r[3], round(r[4], 4)] for r in rows]})
     engine.set_precision(m, 'fp32')
+    del mh, xh
     for name, (Jw, fww, chw, T, B) in (('81-frame/64ch 17-joint', (17, [3, 3, 3, 3], 64, 81, 2048)),
                                        ('27-frame/128ch 19-joint', (19, [3, 3, 3], 128, 27, 8192))):
         mw = model(Jw, fww, chw)
+        mwh = copy.deepcopy(mw).half()
         xw = torch.from_numpy(synth.synth_input(B, T, Jw, 2, seed=5)).cuda()
+        xwh = xw.half()
         for rnd in range(2):
-            for prec in ('fp32', 'tf32'):
-                engine.set_precision(mw, prec)
-                cps, ms = clips_per_s(mw, xw, args.steps)
+            for prec in MODES:
+                mm, xx = in_mode(mw, mwh, xw, xwh, prec)
+                cps, ms = clips_per_s(mm, xx, args.steps)
                 emit({'workload': '%s, %d clips' % (name, B), 'round': rnd, 'precision': prec,
                       'clips_per_s': round(cps), 'ms_per_step': round(ms, 3)})
-        emit(dict(workload='%s accuracy (synthetic weights)' % name, **accuracy(mw, xw)))
-        del mw, xw
+        emit(dict(workload='%s accuracy (synthetic weights)' % name, **accuracy(mw, mwh, xw, xwh)))
+        del mw, mwh, xw, xwh
     n = 1024
     frames = torch.from_numpy(synth.synth_input(n, 64, J, 2, seed=9)).cuda()
     for prec in ('fp32', 'tf32', 'fp32', 'tf32'):
