@@ -102,7 +102,8 @@ struct gast_handle {
   int tc_launches = 0;
   int gemm_core = 0;                 // 0 auto (tensor cores where possible), 1 force FFMA
   int precision = 0;                 // 0 fp32-grade (3xFP16 on scaled operands in inference, 3xTF32 in training),
-                                     // 1 single-pass TF32 (inference only)
+                                     // 1 single-pass TF32 (inference only), 16 fp16 (inference only: the half form's
+                                     // arithmetic and fp16 activations behind float32 x and y, act_f16)
   int act_dtype = GAST_F32;          // activation type of the model forward (gast_set_activation_dtype)
   int train_precision = 0;           // training and every gradient: 0 fp32-grade, 1 single-pass TF32 (forward and
                                      // input-gradient GEMMs) with the TF32 weight-gradient kernel (wgrad_tc.cuh)
@@ -128,6 +129,13 @@ constexpr int GAST_MAX_PENDING_TRAIN = 16;   // training forwards that may wait 
 
 enum { LK_EXPAND = 0, LK_GEMM_PLAIN = 1, LK_GEMM_SEMCH = 2, LK_GEMM_GLOBAL = 3, LK_ROWDOT = 4, LK_SHRINK = 5,
        LK_TC_PLAIN = 6, LK_TC_SEMCH = 7, LK_TC_GLOBAL = 8, LK_GLOBAL_MIX = 9 };
+
+// Whether the activations of an inference forward or stream call are fp16: in a half model (act_dtype, which also makes
+// x and y fp16) and at the fp16 precision (x, y and the streams' input history stay float32).  Training and every
+// gradient keep fp32 activations at any inference precision: they run only where precision_check lets them.
+static bool act_f16(const gast_handle* h) { return h->act_dtype == GAST_F16 || h->precision == 16; }
+
+static size_t act_esize(const gast_handle* h) { return act_f16(h) ? sizeof(__half) : sizeof(float); }
 
 // The refusal of every entry that half does not run: training, every backward, the streams, the mpjpe forward
 static int half_check(const gast_handle* h, const char* who) {
@@ -318,16 +326,34 @@ extern "C" int gast_set_gemm_core(gast_t* h, int32_t core) {
   if (core == 1 && h->act_dtype == GAST_F16)
     return fail("gast_set_gemm_core: the activation type is fp16 (gast_set_activation_dtype), which runs on the "
                 "tensor-core core only");
+  if (core == 1 && h->precision == 16)
+    return fail("gast_set_gemm_core: the precision is fp16 (gast_set_precision(h, 16)), which runs on the tensor-core "
+                "core only");
   h->gemm_core = core;
   return 0;
 }
 
 extern "C" int gast_set_precision(gast_t* h, int32_t mode) {
   if (!h) return fail("null handle");
-  if (mode != 0 && mode != 1) return fail("gast_set_precision: mode must be 0 (fp32-grade) or 1 (tf32), got %d", mode);
+  if (mode != 0 && mode != 1 && mode != 16)
+    return fail("gast_set_precision: mode must be 0 (fp32-grade), 1 (tf32) or 16 (fp16), got %d", mode);
   if (mode == 1 && h->act_dtype == GAST_F16)
     return fail("gast_set_precision: the activation type is fp16 (gast_set_activation_dtype), which has its own "
                 "arithmetic; TF32 needs GAST_F32");
+  if (mode == 16) {   // the half form's arithmetic: its limits (gast_set_activation_dtype) apply
+    if (h->act_dtype == GAST_F16)
+      return fail("gast_set_precision: fp16 precision is for float32 models; the activation type is already fp16 "
+                  "(gast_set_activation_dtype), which has its own fp16 arithmetic");
+    if (h->cfg.kind != GAST_KIND_MODEL)
+      return fail("gast_set_precision: fp16 precision runs the whole model (MODEL kind) only, not a sub-module");
+    if (h->gemm_core != 0)
+      return fail("gast_set_precision: fp16 precision runs on the tensor-core core only (gast_set_gemm_core(h, 0))");
+    if (h->cfg.channels % TC_KS)
+      return fail("gast_set_precision: fp16 precision needs channels that are a multiple of %d (got %d): there is no "
+                  "FFMA core in fp16", TC_KS, h->cfg.channels);
+    if (h->cfg.num_joints > MIX_JMAX)
+      return fail("gast_set_precision: fp16 precision takes at most %d joints (got %d)", MIX_JMAX, h->cfg.num_joints);
+  }
   h->precision = mode;
   return 0;
 }
@@ -339,7 +365,9 @@ extern "C" int gast_set_activation_dtype(gast_t* h, int32_t dtype) {
   if (dtype == GAST_F16) {
     if (h->cfg.kind != GAST_KIND_MODEL)
       return fail("gast_set_activation_dtype: fp16 runs the whole model (MODEL kind) only, not a sub-module");
-    if (h->precision != 0) return fail("gast_set_activation_dtype: fp16 needs gast_set_precision(h, 0), not TF32");
+    if (h->precision != 0)
+      return fail("gast_set_activation_dtype: fp16 needs gast_set_precision(h, 0), not TF32 or the fp16 precision "
+                  "(precision is %d)", h->precision);
     if (h->cfg.num_joints > MIX_JMAX)   // the attention then needs the fused GLOBAL epilogue, not offered in half
       return fail("gast_set_activation_dtype: fp16 takes at most %d joints (got %d)", MIX_JMAX, h->cfg.num_joints);
     if (h->cfg.channels % TC_KS)   // every GEMM width is a multiple of channels; the half form takes multiples of 32
@@ -773,7 +801,9 @@ static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p,
   // training's operand copies (train_tcw, the only ones without the fp16 pair) run at the training precision
   int prec = (h->gemm_core == 0 && tcw && tc_supported(p, epi, *tcw))
                  ? tc_prec(*tcw, tcw->f16 ? h->precision : h->train_precision) : -1;
-  if (h->act_dtype == GAST_F16) {   // fp16 operands: the half form or nothing (there is no FFMA core in half)
+  // fp16 operands: the half form or nothing (there is no FFMA core in half).  Training's operand copies (null, or
+  // without the fp16 pair) read fp32 activations at every inference precision.
+  if (h->act_dtype == GAST_F16 || (h->precision == 16 && tcw && tcw->f16)) {
     if (!tcw || !tc_supported_h(p, epi, *tcw))
       return fail("fp16 forward: a GEMM (N %d, K %d, epilogue %d) is not taken by the tensor-core core (widths must be "
                   "multiples of 32)", p.N, p.ldw, epi);
@@ -802,13 +832,14 @@ extern "C" int gast_debug_set_gemm_audit(gast_t* h, gast_gemm_audit_fn fn, void*
 
 extern "C" int64_t gast_debug_gemm_audit_skips(const gast_t* h) { return h ? h->audit_skips : -1; }
 
+// xf16: X holds fp16 (act_f16 in inference; training passes false)
 static int launch_rowdot(gast_handle* h, cudaStream_t st, const float* X, int ldx, const BlockConsts& b,
-                         float* ab, long long rows) {
+                         float* ab, long long rows, bool xf16) {
   if (rows <= 0) return 0;
   const int Q = 2 * b.heads;
   unsigned blocks = cdiv(rows * 32, 256);
   TimedLaunch tl(h, st, LK_ROWDOT);
-  if (h->act_dtype == GAST_F16) {   // X holds fp16; the row dots stay fp32 (they feed the softmax)
+  if (xf16) {   // X holds fp16; the row dots stay fp32 (they feed the softmax)
     const __half* Xh = reinterpret_cast<const __half*>(X);
     if (Q == 8 && (size_t)8 * b.C * sizeof(float) <= 48 * 1024) {
       unsigned g = (unsigned)std::min<long long>((rows * 32 + 255) / 256, (long long)h->sm_count * 8);
@@ -857,7 +888,7 @@ static int run_local(gast_handle* h, cudaStream_t st, BlockConsts& b, const floa
 static int run_global(gast_handle* h, cudaStream_t st, BlockConsts& b, const float* X, long long F,
                       const BlockBufs& w, float* out_G, int kind) {
   const int C = b.C, J = h->cfg.num_joints, Ng = b.heads * b.Cg;
-  if (launch_rowdot(h, st, X, C, b, w.AB, F * J)) return 1;
+  if (launch_rowdot(h, st, X, C, b, w.AB, F * J, act_f16(h))) return 1;
   GemmP p;
   // tensor-core core, block / MultiGlobalGraph: plain `g` GEMM (flat 128-row tiles) into out_G as scratch, then the
   // attention mix as its own full-occupancy kernel into Y.  Measured faster than the mix fused into the GEMM
@@ -874,7 +905,7 @@ static int run_global(gast_handle* h, cudaStream_t st, BlockConsts& b, const flo
     const size_t smem = sizeof(float) * (size_t)fpb * b.heads * J * MIX_JP;
     {
       TimedLaunch tl(h, st, LK_GLOBAL_MIX);
-      if (h->act_dtype == GAST_F16)
+      if (act_f16(h))
         global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(reinterpret_cast<const __half*>(out_G), Ng, w.AB,
                                                                    b.Ck, reinterpret_cast<__half*>(w.Y), Ng, F, J,
                                                                    b.heads, b.Cg, fpb);
@@ -926,6 +957,17 @@ static int launch_expand(gast_handle* h, cudaStream_t st, const float* x, float*
   if (k0 * Fin > EXP_MAXKF) return fail("expand: filter_width*in_features > %d unsupported", EXP_MAXKF);
   TimedLaunch tl(h, st, LK_EXPAND);
   const dim3 grid(cdiv(rows, EXS_ROWS), cdiv(c.channels, EXS_CHUNK));
+  if (h->act_dtype == GAST_F32 && act_f16(h)) {   // the fp16 precision: float32 x, fp16 out
+    __half* oh = reinterpret_cast<__half*>(out);
+    if (k0 * Fin <= 6)
+      expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, oh, rows, c.num_joints, T, T0, stride, k0,
+                                                           Fin, c.channels);
+    else
+      expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, oh, rows, c.num_joints, T, T0,
+                                                                   stride, k0, Fin, c.channels);
+    h->launches++;
+    return 0;
+  }
   if (h->act_dtype == GAST_F16) {
     const __half* xh = reinterpret_cast<const __half*>(x);
     __half* oh = reinterpret_cast<__half*>(out);
@@ -979,7 +1021,14 @@ static int launch_shrink(gast_handle* h, cudaStream_t st, const float* X, float*
     unsigned* ticket = reinterpret_cast<unsigned*>(h->loss_scratch + 2 * SHL_MAXBLOCKS);
     const unsigned nb = (unsigned)std::min<long long>(SHL_MAXBLOCKS, (rows + 7) / 8);
     TimedLaunch tl(h, st, LK_SHRINK);
-    shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(X, Cl, ws, y, rows, Cl, target, partial, ticket, loss);
+    if (act_f16(h))   // the fp16 precision (a half model refuses the mpjpe forward): fp16 X, float32 y
+      shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws, y, rows, Cl, target, partial,
+                                              ticket, loss);
+    else
+      shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(X, Cl, ws, y, rows, Cl, target, partial, ticket, loss);
+  } else if (h->act_dtype == GAST_F32 && act_f16(h)) {
+    TimedLaunch tl(h, st, LK_SHRINK);
+    shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws, y, rows, Cl);
   } else if (h->act_dtype == GAST_F16) {
     TimedLaunch tl(h, st, LK_SHRINK);
     shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws,
@@ -992,8 +1041,8 @@ static int launch_shrink(gast_handle* h, cudaStream_t st, const float* X, float*
   return 0;
 }
 
-// In a half forward (gast_set_activation_dtype) every buffer but bb.AB holds fp16: the pointers are typed float and
-// the launches reinterpret them.
+// In a half forward (gast_set_activation_dtype) and at the fp16 precision (act_f16) every buffer but bb.AB holds fp16:
+// the pointers are typed float and the launches reinterpret them.
 struct ModelBufs {
   float* act[2];
   float* tmp;
@@ -1002,7 +1051,7 @@ struct ModelBufs {
 
 static int plan_model(const gast_handle* h, int B, int T, int strided_now, Arena& a, ModelBufs* mb, Geometry* g) {
   if (geometry(h, T, strided_now, g)) return 1;
-  a.esize = h->act_dtype == GAST_F16 ? sizeof(__half) : sizeof(float);
+  a.esize = act_esize(h);
   const int J = h->cfg.num_joints, C = h->cfg.channels, L = h->cfg.num_stages;
   // max over layers
   size_t act = 0, tmp = 0, xy = 0, l = 0, ab = 0;

@@ -25,11 +25,11 @@ constexpr int EXS_ROWS = 128;
 constexpr int EXS_THREADS = 256;
 constexpr int EXS_CHUNK = 4 * EXS_THREADS;               // channels per block: 4 per thread
 constexpr int EXP_MAXKF = 10;   // taps * in_features supported by the register path (3*2 = 6; 5*2 = 10)
-// Act: the activation type of x and out (float, or __half in a half forward)
-template <int KFT, typename Act>   // register-resident K = taps * in_features rounded up: 6 (3 taps x 2) or EXP_MAXKF
+// In, Out: the types of x and out (float, or __half: both in a half forward, out only at the fp16 precision)
+template <int KFT, typename In, typename Out>   // register-resident K = taps * in_features rounded up: 6 or EXP_MAXKF
 __global__ void __launch_bounds__(EXS_THREADS)
-expand_rows_kernel(const Act* __restrict__ x, const float* __restrict__ We, const float* __restrict__ be,
-                   Act* __restrict__ out, long long rows, int J, int T, int T0, int stride, int taps, int Fin, int C) {
+expand_rows_kernel(const In* __restrict__ x, const float* __restrict__ We, const float* __restrict__ be,
+                   Out* __restrict__ out, long long rows, int J, int T, int T0, int stride, int taps, int Fin, int C) {
   constexpr int KP = (KFT + 3) & ~3;                      // padded row of staged inputs (float4 reads)
   __shared__ __align__(16) float xs[EXS_ROWS * KP];
   const int tid = threadIdx.x;
@@ -63,7 +63,7 @@ expand_rows_kernel(const Act* __restrict__ x, const float* __restrict__ We, cons
   const float4 b4 = ldg4(be + c);
   __syncthreads();
   if (rsub >= rpp) return;                                // (256 % cq != 0: the surplus threads have no row)
-  Act* op = out + (r0 + rsub) * C + c;
+  Out* op = out + (r0 + rsub) * C + c;
   const long long ostep = (long long)rpp * C;
 #pragma unroll 4
   for (int rr = rsub; rr < nrows; rr += rpp, op += ostep) {
@@ -88,20 +88,22 @@ expand_rows_kernel(const Act* __restrict__ x, const float* __restrict__ We, cons
 // of an output joint also takes ||y - target|| of it.  Partial sums are double (like mpjpe_kernel); the last block to
 // finish (atomic ticket) adds the block partials in index order, so the loss does not depend on the scheduling, and
 // resets the ticket for the next call (CUDA-graph replay safe).  y is written as by shrink_kernel (same FMA order).
+// X: float, or __half at the fp16 precision (y, target and the loss stay float).
 // ---------------------------------------------------------------------------------------
 constexpr int SHL_MAXBLOCKS = 1024;
+template <typename T>
 __global__ void __launch_bounds__(256)
-shrink_mpjpe_kernel(const float* __restrict__ X, int ldx, const float* __restrict__ Ws, float* __restrict__ y,
+shrink_mpjpe_kernel(const T* __restrict__ X, int ldx, const float* __restrict__ Ws, float* __restrict__ y,
                     long long rows, int K, const float* __restrict__ target, double* __restrict__ partial,
                     unsigned* __restrict__ ticket, float* __restrict__ loss) {
   const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
   const long long nw = (long long)gridDim.x * 8;
   double acc = 0.0;
   for (long long row = (long long)blockIdx.x * 8 + wrp; row < rows; row += nw) {
-    const float* xr = X + row * ldx;
+    const T* xr = X + row * ldx;
     float a0 = 0.f, a1 = 0.f, a2 = 0.f;
     for (int k = lane * 4; k < K; k += 128) {
-      float4 xv = ldg4(xr + k);
+      float4 xv = ld4(xr + k);
       float4 w0 = ldg4(Ws + k), w1 = ldg4(Ws + K + k), w2 = ldg4(Ws + 2 * K + k);
       a0 = fmaf(xv.x, w0.x, fmaf(xv.y, w0.y, fmaf(xv.z, w0.z, fmaf(xv.w, w0.w, a0))));
       a1 = fmaf(xv.x, w1.x, fmaf(xv.y, w1.y, fmaf(xv.z, w1.z, fmaf(xv.w, w1.w, a1))));

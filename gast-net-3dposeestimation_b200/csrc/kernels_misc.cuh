@@ -98,10 +98,11 @@ __global__ void rowdot8_kernel(const T* __restrict__ X, int ldx, const float* __
   }
 }
 
-// shrink (gast_net.py:60,99): y[row][o] = X[row,:] . Ws[o,:], o < 3.   Warp per row.
-template <typename T>
+// shrink (gast_net.py:60,99): y[row][o] = X[row,:] . Ws[o,:], o < 3.   Warp per row.  T, Y: the types of X and y
+// (float, or __half: both in a half forward, X only at the fp16 precision)
+template <typename T, typename Y>
 __global__ void shrink_kernel(const T* __restrict__ X, int ldx, const float* __restrict__ Ws,
-                              T* __restrict__ y, long long rows, int K) {
+                              Y* __restrict__ y, long long rows, int K) {
   long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
   if (row >= rows) return;

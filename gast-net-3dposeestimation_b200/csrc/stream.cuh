@@ -56,19 +56,19 @@ __global__ void stream_xpush_kernel(float* __restrict__ xhist, const float* __re
   }
 }
 
-// ring (R, n, rowlen): for every fresh stream copy its row block of slot `src` to every other slot.
-// grid = (n, chunks of the row block); a block whose stream is not fresh exits at once.
-__global__ void stream_fill_fresh_kernel(float* __restrict__ ring, int R, int src, int n, long long rowlen,
+// ring (R, n, row16 16-byte vectors): for every fresh stream copy its row block of slot `src` to every other slot.
+// grid = (n, chunks of the row block); a block whose stream is not fresh exits at once.  The rows are measured in
+// bytes, so the kernel moves fp32 and fp16 rings alike.
+__global__ void stream_fill_fresh_kernel(uint4* __restrict__ ring, int R, int src, int n, long long row16,
                                          const int32_t* __restrict__ fresh) {
   const int b = blockIdx.x;
   if (!fresh[b]) return;
-  const long long slot_stride = (long long)n * rowlen;
-  const float4* s = reinterpret_cast<const float4*>(ring + (long long)src * slot_stride + (long long)b * rowlen);
-  const long long n4 = rowlen >> 2;
-  for (long long i = (long long)blockIdx.y * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.y * blockDim.x) {
-    const float4 v = s[i];
+  const long long slot_stride = (long long)n * row16;
+  const uint4* s = ring + (long long)src * slot_stride + (long long)b * row16;
+  for (long long i = (long long)blockIdx.y * blockDim.x + threadIdx.x; i < row16; i += (long long)gridDim.y * blockDim.x) {
+    const uint4 v = s[i];
     for (int r = 0; r < R; ++r)
-      if (r != src) reinterpret_cast<float4*>(ring + (long long)r * slot_stride + (long long)b * rowlen)[i] = v;
+      if (r != src) ring[(long long)r * slot_stride + (long long)b * row16 + i] = v;
   }
 }
 
@@ -129,21 +129,22 @@ stream_chunk_xin_kernel(float* __restrict__ xhist, const float* __restrict__ x, 
 // (step - H + p) mod R, the tail (p >= H) from the previous block's K outputs tail (m, K, rowlen).  A fresh stream's head
 // is copies of its tail position 0 (its history is constant, as stream_fill_fresh_kernel makes it).  The ring holds n
 // streams per slot.  tab null: m = n, row b is stream b and hs = step mod R for all; else row b is state stream tab[b]
-// at its own phase tab[m + b] (its step mod R_max, which R divides) and hs is unused.
-__global__ void stream_chunk_gather_kernel(float4* __restrict__ G, const float4* __restrict__ ring,
-                                           const float4* __restrict__ tail, const int32_t* __restrict__ fresh, int m,
-                                           int n, int R, int hs, int H, int K, long long row4,
+// at its own phase tab[m + b] (its step mod R_max, which R divides) and hs is unused.  Rows are row16 16-byte vectors
+// (J channels of the stage in fp32 or fp16).
+__global__ void stream_chunk_gather_kernel(uint4* __restrict__ G, const uint4* __restrict__ ring,
+                                           const uint4* __restrict__ tail, const int32_t* __restrict__ fresh, int m,
+                                           int n, int R, int hs, int H, int K, long long row16,
                                            const int32_t* __restrict__ tab) {
-  const long long total = (long long)m * (H + K) * row4;
+  const long long total = (long long)m * (H + K) * row16;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const long long q = i % row4, f = i / row4;
+    const long long q = i % row16, f = i / row16;
     const int b = (int)(f / (H + K)), p = (int)(f - (long long)b * (H + K));
-    float4 v;
-    if (p >= H) v = tail[((long long)b * K + (p - H)) * row4 + q];
-    else if (fresh && fresh[b]) v = tail[(long long)b * K * row4 + q];
+    uint4 v;
+    if (p >= H) v = tail[((long long)b * K + (p - H)) * row16 + q];
+    else if (fresh && fresh[b]) v = tail[(long long)b * K * row16 + q];
     else {
       const int sb = tab ? tab[b] : b, h = tab ? tab[m + b] % R : hs;
-      v = ring[((long long)((h - H + p + R) % R) * n + sb) * row4 + q];
+      v = ring[((long long)((h - H + p + R) % R) * n + sb) * row16 + q];
     }
     G[i] = v;
   }
@@ -154,20 +155,20 @@ __global__ void stream_chunk_gather_kernel(float4* __restrict__ G, const float4*
 // ek = (step + K - 1) mod R.  Launched after stream_chunk_gather_kernel, which reads slots this kernel overwrites.
 // Grid over the R*m rows (slot, listed stream); tab as in stream_chunk_gather_kernel (null: m = n, ek for all; else
 // ek = (tab[m + b] + K - 1) mod R per stream and slot p of stream tab[b] is written).  act (m) or null (all active):
-// nothing is written for a row with act[b] == 0.
-__global__ void stream_chunk_ring_kernel(float4* __restrict__ ring, const float4* __restrict__ G,
+// nothing is written for a row with act[b] == 0.  Rows are row16 16-byte vectors, as in stream_chunk_gather_kernel.
+__global__ void stream_chunk_ring_kernel(uint4* __restrict__ ring, const uint4* __restrict__ G,
                                          const int32_t* __restrict__ fresh, int m, int n, int R, int ek, int H, int K,
-                                         long long row4, const int32_t* __restrict__ tab,
+                                         long long row16, const int32_t* __restrict__ tab,
                                          const int32_t* __restrict__ act) {
-  const long long total = (long long)R * m * row4;
+  const long long total = (long long)R * m * row16;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const long long q = i % row4, f = i / row4;
+    const long long q = i % row16, f = i / row16;
     const int p = (int)(f / m), b = (int)(f - (long long)p * m);
     if (act && !act[b]) continue;
     const int e = tab ? (int)(((long long)tab[m + b] + K - 1) % R) : ek;
     const int k = K - 1 - (e - p + R) % R;                // chunk position of time t
     if (k < 0 && !(fresh && fresh[b])) continue;
-    ring[tab ? ((long long)p * n + tab[b]) * row4 + q : i] = G[((long long)b * (H + K) + H + max(k, 0)) * row4 + q];
+    ring[tab ? ((long long)p * n + tab[b]) * row16 + q : i] = G[((long long)b * (H + K) + H + max(k, 0)) * row16 + q];
   }
 }
 
@@ -224,33 +225,44 @@ struct MovePlan { MovePart part[GAST_MAX_STAGES]; int nparts; long long snap_flo
 
 // grid = (rows of one snapshot, listed streams in a grid-stride loop); tab (2m): row b is state stream tab[b] at phase
 // tab[m + b] (its count mod R_max, which every R_i divides).  kImport: snap (m, snap_floats) -> state, else the other
-// way.  Plain float copies: the input history row (k0 J F floats) and the snapshot's part offsets need not be
-// multiples of 4.
-template <bool kImport>
-__global__ void __launch_bounds__(256) stream_move_kernel(float* __restrict__ state, float* __restrict__ snap,
+// way.  Plain element copies: the input history row (k0 J F floats) and the snapshot's part offsets need not be
+// multiples of 4.  Ring: the element type of the rings (parts q >= 1; float, or __half at the fp16 precision, which an
+// export widens exactly and an import rounds to nearest); the input history (part 0) is float in every state.  The
+// part offsets into the state are bytes, the strides elements of the part's type.
+template <typename E>
+__device__ __forceinline__ void move_row(E* __restrict__ s, float* __restrict__ t, int rowlen, bool import) {
+#pragma unroll 4
+  for (int e = threadIdx.x; e < rowlen; e += blockDim.x) {
+    if (import) st1(s + e, t[e]);
+    else t[e] = ld1(s + e);
+  }
+}
+
+template <bool kImport, typename Ring>
+__global__ void __launch_bounds__(256) stream_move_kernel(char* __restrict__ state, float* __restrict__ snap,
                                                           const MovePlan p, const int32_t* __restrict__ tab, int m) {
   int q = 0, j = blockIdx.x;
   while (j >= p.part[q].R) j -= p.part[q++].R;            // snapshot row -> (part, time position)
   const MovePart& g = p.part[q];
   for (int b = blockIdx.y; b < m; b += gridDim.y) {
     const int slot = q ? (tab[m + b] % g.R + j) % g.R : 0;
-    float* s = state + g.state_off + slot * g.slot_stride + tab[b] * g.stream_stride;
+    const long long e0 = slot * g.slot_stride + tab[b] * g.stream_stride;
     float* t = snap + b * p.snap_floats + g.snap_off + (long long)j * g.rowlen;
-#pragma unroll 4
-    for (int e = threadIdx.x; e < g.rowlen; e += blockDim.x) {
-      if (kImport) s[e] = t[e];
-      else t[e] = s[e];
-    }
+    if (q) move_row(reinterpret_cast<Ring*>(state + g.state_off) + e0, t, g.rowlen, kImport);
+    else move_row(reinterpret_cast<float*>(state + g.state_off) + e0, t, g.rowlen, kImport);
   }
 }
 
 }  // namespace gast
 
+// The state of n streams: the float32 input history, then one ring per temporal stage in the activation type (fp16 at
+// the fp16 precision, act_esize), each part 256-byte aligned.
 struct StreamPlan {
   int n = 0;
   std::vector<int> dil, R;              // per stage (index i-1): dilation d_i, ring slots R_i = w_i d_i
-  std::vector<size_t> ring_off;         // float offsets into the state
-  size_t xhist_off = 0, state_floats = 0;
+  std::vector<size_t> ring_off;         // byte offsets into the state
+  size_t xhist_off = 0, state_bytes = 0;
+  size_t esize = sizeof(float);         // bytes per ring element
 };
 
 static int stream_check(const gast_handle* h) {
@@ -269,18 +281,19 @@ static int stream_plan(const gast_handle* h, int n, StreamPlan* sp) {
   const gast_cfg& c = h->cfg;
   const int J = c.num_joints, L = c.num_stages;
   sp->n = n;
+  sp->esize = act_esize(h);
   size_t off = 0;
-  auto take = [&](size_t nf) { size_t o = off; off += (nf + 63) & ~(size_t)63; return o; };
-  sp->xhist_off = take((size_t)n * c.filter_widths[0] * J * c.in_features);
+  auto take = [&](size_t nb) { size_t o = off; off += (nb + 255) & ~(size_t)255; return o; };
+  sp->xhist_off = take((size_t)n * c.filter_widths[0] * J * c.in_features * sizeof(float));
   int d = c.filter_widths[0];
   for (int i = 1; i < L; ++i) {
     const int fw = c.filter_widths[i], Cw = c.channels << i;
     sp->dil.push_back(d);
     sp->R.push_back(fw * d);
-    sp->ring_off.push_back(take((size_t)fw * d * n * J * Cw));
+    sp->ring_off.push_back(take((size_t)fw * d * n * J * Cw * sp->esize));
     d *= fw;
   }
-  sp->state_floats = off;
+  sp->state_bytes = off;
   return 0;
 }
 
@@ -288,20 +301,22 @@ extern "C" size_t gast_stream_state_bytes(gast_t* h, int32_t n_streams) {
   if (!h) return 0;
   StreamPlan sp;
   if (stream_plan(h, n_streams, &sp)) return 0;
-  return sp.state_floats * sizeof(float) + 256;
+  return sp.state_bytes + 256;
 }
 
+// every buffer but bb.AB holds activations (fp16 at the fp16 precision, act_esize)
 struct StreamBufs { float *E, *tmp, *act, *fin; BlockBufs bb; };
 
 static void stream_bufs(const gast_handle* h, int n, Arena& a, StreamBufs* sb) {
   const int J = h->cfg.num_joints, C = h->cfg.channels, L = h->cfg.num_stages;
   const size_t rows = (size_t)n * J;
   const int Cmax = C << (L - 1);                 // widest block input
+  a.esize = act_esize(h);
   sb->E = a.take(rows * C);
   sb->tmp = a.take(rows * Cmax);
   sb->act = a.take(rows * Cmax);
   sb->fin = a.take(rows * 2 * Cmax);
-  sb->bb.XY = a.take(rows * 2 * Cmax); sb->bb.L = a.take(rows * Cmax); sb->bb.AB = a.take(rows * 8);
+  sb->bb.XY = a.take(rows * 2 * Cmax); sb->bb.L = a.take(rows * Cmax); sb->bb.AB = a.take32(rows * 8);
   sb->bb.Y = a.take(rows * Cmax); sb->bb.Gl = a.take(rows * Cmax);
 }
 
@@ -355,31 +370,33 @@ extern "C" int gast_stream_push_ex(gast_t* h, void* state, int64_t step, const f
   if (!h->stream_ready && stream_prepare(h, st)) return 1;
   const gast_cfg& c = h->cfg;
   const int n = n_streams, J = c.num_joints, C = c.channels, L = c.num_stages, k0 = c.filter_widths[0], Fin = c.in_features;
-  float* sbase = reinterpret_cast<float*>(align256(state));
+  char* sbase = align256(state);
   Arena a = workspace_arena(workspace, workspace_bytes);
   StreamBufs sb;
   stream_bufs(h, n, a, &sb);
   const long long rows = (long long)n * J;
+  const size_t es = sp.esize;
   // input history + expand (gast_net.py:163-164) on the last k0 frames
-  float* xhist = sbase + sp.xhist_off;
+  float* xhist = reinterpret_cast<float*>(sbase + sp.xhist_off);
   stream_xpush_kernel<<<cdiv((long long)n * J * Fin, 256), 256, 0, st>>>(xhist, x, fresh, hold, n, k0, J * Fin);
   h->launches++;
   if (launch_expand(h, st, xhist, sb.E, rows, k0, 1, 1)) return 1;
   auto slot_ptr = [&](int i /*stage 1..L-1*/) {
     const int R = sp.R[i - 1], Cw = C << i;
-    return sbase + sp.ring_off[i - 1] + (size_t)(step % R) * n * J * Cw;
+    return reinterpret_cast<float*>(sbase + sp.ring_off[i - 1] + (size_t)(step % R) * n * J * Cw * es);
   };
   float* bout = (L > 1) ? slot_ptr(1) : sb.fin;
   if (run_block(h, st, h->blocks[0], sb.E, n, sb.bb, bout)) return 1;
   for (int i = 1; i < L; ++i) {
     StageConsts& s = h->stages[i - 1];
     const int Cw = s.Cw, fw = c.filter_widths[i], d = sp.dil[i - 1], R = sp.R[i - 1];
-    float* ring = sbase + sp.ring_off[i - 1];
+    char* ring = sbase + sp.ring_off[i - 1];
     const int hs = (int)(step % R);
-    const long long slot_floats = (long long)n * J * Cw;
+    const long long slot_elems = (long long)n * J * Cw, slot_bytes = slot_elems * (long long)es;
     if (fresh) {
-      dim3 g((unsigned)n, (unsigned)std::max<long long>(1, std::min<long long>(8, (long long)J * Cw / 4 / 256)));
-      stream_fill_fresh_kernel<<<g, 256, 0, st>>>(ring, R, hs, n, (long long)J * Cw, fresh);
+      const long long row16 = (long long)J * Cw * (long long)es / 16;
+      dim3 g((unsigned)n, (unsigned)std::max<long long>(1, std::min<long long>(8, row16 / 256)));
+      stream_fill_fresh_kernel<<<g, 256, 0, st>>>(reinterpret_cast<uint4*>(ring), R, hs, n, row16, fresh);
       h->launches++;
     }
     // taps = slots p0 + k d with the weights rotated to slot order; residual = the newest slot (causal_shift = pad)
@@ -387,8 +404,11 @@ extern "C" int gast_stream_push_ex(gast_t* h, void* state, int64_t step, const f
     const int p0 = hs % d, r = hs / d;
     const int rs = c.causal ? hs : (hs + R - (fw / 2) * d) % R;
     const RowMap same{n, n, 1, 0};
-    const ASeg taps = seg_taps(ring + (long long)p0 * slot_floats, Cw, Cw, fw, (long long)d * slot_floats, same);
-    if (run_stage(h, st, s, n, taps, s.Wrot[r], &s.tc_rot[r], sb.tmp, ring + (long long)rs * slot_floats, same, sb.act))
+    // the base pointers in bytes, the tap stride in elements (floats or halves, as the GEMM reads them)
+    const ASeg taps = seg_taps(reinterpret_cast<const float*>(ring + (long long)p0 * slot_bytes), Cw, Cw, fw,
+                               (long long)d * slot_elems, same);
+    if (run_stage(h, st, s, n, taps, s.Wrot[r], &s.tc_rot[r], sb.tmp,
+                  reinterpret_cast<const float*>(ring + (long long)rs * slot_bytes), same, sb.act))
       return 1;
     bout = (i < L - 1) ? slot_ptr(i + 1) : sb.fin;
     if (run_block(h, st, h->blocks[i], sb.act, n, sb.bb, bout)) return 1;
@@ -429,10 +449,11 @@ static int chunk_bufs(const gast_handle* h, const StreamPlan& sp, int m, int K, 
   size_t g = 0;
   for (int i = 1; i < c.num_stages; ++i)
     g = std::max(g, (size_t)m * ((c.filter_widths[i] - 1) * sp.dil[i - 1] + K) * J * (c.channels << i));
-  cb->xin = a.take((size_t)m * (k0 - 1 + K) * J * c.in_features);
+  a.esize = act_esize(h);                                  // G holds activations, xin float32 input frames
+  cb->xin = a.take32((size_t)m * (k0 - 1 + K) * J * c.in_features);
   cb->G = a.take(g);
   stream_bufs(h, m * K, a, &cb->sb);
-  cb->tab = table ? reinterpret_cast<int32_t*>(a.take((size_t)table * m)) : nullptr;
+  cb->tab = table ? reinterpret_cast<int32_t*>(a.take32((size_t)table * m)) : nullptr;
   return 0;
 }
 
@@ -454,7 +475,7 @@ extern "C" size_t gast_stream_chunk_workspace_bytes(gast_t* h, int32_t n_streams
 // history (ring write-back when write_rings), shrink into y (m, K, J, 3).  tab null: all m = sp.n streams at `step`;
 // else the device table of a subset call (stream_chunk_gather_kernel): m listed streams, each at its own phase.  act
 // (m) or null: the write-back skips the rows with act[b] == 0.
-static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, float* sbase, int64_t step, int m,
+static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, char* sbase, int64_t step, int m,
                          int K, const int32_t* fresh, bool write_rings, const ChunkBufs& cb, float* y,
                          const int32_t* tab, const int32_t* act) {
   const gast_cfg& c = h->cfg;
@@ -468,18 +489,19 @@ static int chunk_forward(gast_handle* h, cudaStream_t st, const StreamPlan& sp, 
     const StageConsts& s = h->stages[i - 1];
     const int Cw = s.Cw, fw = c.filter_widths[i], d = sp.dil[i - 1], R = sp.R[i - 1], H = (fw - 1) * d;
     if (s.taps != fw) return fail("streaming: stage %d has %d taps, expected %d", i - 1, s.taps, fw);
-    if ((J * Cw) % 4) return fail("streaming chunk: J*channels of stage %d is not a multiple of 4", i);
-    float* ring = sbase + sp.ring_off[i - 1];
-    const long long row4 = (long long)J * Cw / 4;
-    const long long g4 = (long long)m * (H + K) * row4, r4 = (long long)R * m * row4;
-    stream_chunk_gather_kernel<<<(unsigned)std::min<long long>(cdiv(g4, 256), grid_cap), 256, 0, st>>>(
-        reinterpret_cast<float4*>(cb.G), reinterpret_cast<const float4*>(ring),
-        reinterpret_cast<const float4*>(sb.fin), fresh, m, n, R, (int)(step % R), H, K, row4, tab);
+    const long long row_bytes = (long long)J * Cw * (long long)sp.esize;
+    if (row_bytes % 16) return fail("streaming chunk: a row of stage %d (J*channels) is not a multiple of 16 bytes", i);
+    char* ring = sbase + sp.ring_off[i - 1];
+    const long long row16 = row_bytes / 16;
+    const long long g16 = (long long)m * (H + K) * row16, r16 = (long long)R * m * row16;
+    stream_chunk_gather_kernel<<<(unsigned)std::min<long long>(cdiv(g16, 256), grid_cap), 256, 0, st>>>(
+        reinterpret_cast<uint4*>(cb.G), reinterpret_cast<const uint4*>(ring), reinterpret_cast<const uint4*>(sb.fin),
+        fresh, m, n, R, (int)(step % R), H, K, row16, tab);
     h->launches++;
     if (write_rings) {
-      stream_chunk_ring_kernel<<<(unsigned)std::min<long long>(cdiv(r4, 256), grid_cap), 256, 0, st>>>(
-          reinterpret_cast<float4*>(ring), reinterpret_cast<const float4*>(cb.G), fresh, m, n, R,
-          (int)((step + K - 1) % R), H, K, row4, tab, act);
+      stream_chunk_ring_kernel<<<(unsigned)std::min<long long>(cdiv(r16, 256), grid_cap), 256, 0, st>>>(
+          reinterpret_cast<uint4*>(ring), reinterpret_cast<const uint4*>(cb.G), fresh, m, n, R,
+          (int)((step + K - 1) % R), H, K, row16, tab, act);
       h->launches++;
     }
     // output frame (b, t) = time step+t: taps at G positions t, t+d, ..., t+H; residual at the newest tap (causal)
@@ -567,7 +589,7 @@ static int chunk_call(const char* who, gast_handle* h, void* state, int n_stream
   if (call_begin(h, who, need, workspace, workspace_bytes)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int J = h->cfg.num_joints, k0 = h->cfg.filter_widths[0], JF = J * h->cfg.in_features;
-  float* sbase = reinterpret_cast<float*>(align256(state));
+  char* sbase = align256(state);
   Arena a = workspace_arena(workspace, workspace_bytes);
   ChunkBufs cb;
   chunk_bufs(h, sp, m, K, table, who, a, &cb);                   // sized above: cannot fail
@@ -586,10 +608,10 @@ static int chunk_call(const char* who, gast_handle* h, void* state, int n_stream
   if (peek) {
     const long long xe = (long long)m * (k0 - 1 + K) * JF;
     stream_peek_xin_kernel<<<(unsigned)std::min<long long>(cdiv(xe, 256), (long long)h->sm_count * 16), 256, 0, st>>>(
-        sbase + sp.xhist_off, cb.xin, m, k0, K, JF, dtab);
+        reinterpret_cast<const float*>(sbase + sp.xhist_off), cb.xin, m, k0, K, JF, dtab);
   } else {
-    stream_chunk_xin_kernel<<<m, CHUNK_XIN_THREADS, 0, st>>>(sbase + sp.xhist_off, x, cb.xin, fresh, hold, k0, K, JF,
-                                                             dtab, active);
+    stream_chunk_xin_kernel<<<m, CHUNK_XIN_THREADS, 0, st>>>(reinterpret_cast<float*>(sbase + sp.xhist_off), x, cb.xin,
+                                                             fresh, hold, k0, K, JF, dtab, active);
   }
   h->launches++;
   return chunk_forward(h, st, sp, sbase, step, m, K, fresh, !peek, cb, y, dtab, active);
@@ -670,7 +692,8 @@ extern "C" int gast_stream_peek_device(gast_t* h, const void* state, int32_t n_s
 }
 
 // ---- moving streams between states: a gather to and a scatter from their time-ordered snapshots -----------------
-// The parts of a snapshot (stream_move_kernel) over the state layout of stream_plan.
+// The parts of a snapshot (stream_move_kernel) over the state layout of stream_plan: byte offsets into the state,
+// element strides.
 static MovePlan move_plan(const gast_handle* h, const StreamPlan& sp) {
   const gast_cfg& c = h->cfg;
   const int J = c.num_joints, xrow = c.filter_widths[0] * J * c.in_features;
@@ -720,9 +743,14 @@ static int move_call(const char* who, bool import, gast_handle* h, void* state, 
   int rows = 0;
   for (int q = 0; q < p.nparts; ++q) rows += p.part[q].R;
   const dim3 grid((unsigned)rows, (unsigned)std::min(m, 65535));
-  float* sbase = reinterpret_cast<float*>(align256(state));
-  if (import) stream_move_kernel<true><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
-  else stream_move_kernel<false><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
+  char* sbase = align256(state);
+  if (sp.esize == sizeof(__half)) {
+    if (import) stream_move_kernel<true, __half><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
+    else stream_move_kernel<false, __half><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
+  } else {
+    if (import) stream_move_kernel<true, float><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
+    else stream_move_kernel<false, float><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
+  }
   h->launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -27,25 +27,33 @@ class GastError(RuntimeError):
     pass
 
 
-_PRECISIONS = {'fp32': 0, 'tf32': 1}
+_PRECISIONS = {'fp32': 0, 'tf32': 1, 'fp16': 16}     # set_precision -> gast_set_precision's mode
+_TRAIN_PRECISIONS = {'fp32': 0, 'tf32': 1}          # set_training_precision -> gast_set_train_precision's mode
 
 
 def set_precision(module, mode):
     """Arithmetic of the tensor-core GEMMs of `module` and all of its sub-modules, like torch's `allow_tf32`:
     'fp32' (default) is fp32-grade (3xTF32, the reference's numbers to ~1e-7 relative); 'tf32' is one TF32 product
-    per multiply-add with fp32 accumulation, faster and about 1e-3 relative off (DESIGN.md §4.1).  'tf32' is for
-    inference: forward under no_grad, run_model_mpjpe, the streams, lift_sequences, tta.evaluate_sequence; a
-    train-mode forward or one that builds an autograd graph raises.  The setting lives in each module's __dict__
-    (DataParallel replicas and deepcopies keep it, state_dict does not).  Returns the module."""
+    per multiply-add with fp32 accumulation, faster and about 1e-3 relative off (DESIGN.md §4.1); 'fp16' is the
+    arithmetic of a half model behind float32 input, parameters and poses: every activation stored in fp16, one fp16
+    product per multiply-add with fp32 accumulation, fastest and about 2e-3 of max |y| off (DESIGN.md §4.1, "The fp16
+    precision").  'tf32' and 'fp16' are for inference: forward under no_grad, run_model_chunked, run_model_mpjpe, the
+    streams, lift_sequences, tta.evaluate_sequence; a train-mode forward or one that builds an autograd graph raises
+    unless the training precision is 'tf32' (set_training_precision).  'fp16' runs whole float32 models with channels
+    that are multiples of 32 on the tensor-core core; a half model (model.half()) raises at 'fp16' (it has its own
+    fp16 arithmetic), as does a sub-module called on its own.  The streams keep their history in fp16 at 'fp16', so
+    a PoseStream pool with history refuses a switch between 'fp16' and the other two (DESIGN.md §4.1).  The setting
+    lives in each module's __dict__ (DataParallel replicas and deepcopies keep it, state_dict does not).  Returns the
+    module."""
     if mode not in _PRECISIONS:
-        raise GastError("set_precision: mode must be 'fp32' or 'tf32' (got %r)" % (mode,))
+        raise GastError("set_precision: mode must be 'fp32', 'tf32' or 'fp16' (got %r)" % (mode,))
     for m in module.modules():
         m.__dict__['_gast_precision'] = mode
     return module
 
 
 def get_precision(module):
-    """'fp32' or 'tf32' (set_precision)"""
+    """'fp32', 'tf32' or 'fp16' (set_precision)"""
     return module.__dict__.get('_gast_precision', 'fp32')
 
 
@@ -59,7 +67,7 @@ def set_training_precision(module, mode):
     inference forward, at the inference precision (set_precision); its backward recomputes the activations at this
     precision.  Stored in each module's __dict__ like set_precision (DataParallel replicas and deepcopies keep it,
     state_dict does not).  Returns the module."""
-    if mode not in _PRECISIONS:
+    if mode not in _TRAIN_PRECISIONS:
         raise GastError("set_training_precision: mode must be 'fp32' or 'tf32' (got %r)" % (mode,))
     for m in module.modules():
         m.__dict__['_gast_train_precision'] = mode
@@ -72,9 +80,11 @@ def get_training_precision(module):
 
 
 def _fp32_only(module, what):
-    if get_precision(module) != 'fp32' and get_training_precision(module) == 'fp32':
-        raise GastError("%s: the model is set to TF32, which is inference-only; call "
-                        "engine.set_precision(model, 'fp32') to train or differentiate it" % what)
+    prec = get_precision(module)
+    if prec != 'fp32' and get_training_precision(module) == 'fp32':
+        raise GastError("%s: the model is set to %s, which is inference-only; call "
+                        "engine.set_precision(model, 'fp32') to train or differentiate it"
+                        % (what, 'TF32' if prec == 'tf32' else 'the fp16 precision'))
 
 
 _HALF_ONLY = ('the model is half precision (model.half()), which runs inference only: the eval-mode forward under '
@@ -216,24 +226,34 @@ class _Handle(object):
     def apply_core(self, module):
         """hand the set_gemm_core() choice and the module's set_precision() and set_training_precision() to the
         library handle (every forward, training or eval, and every stream push), and for a whole model its activation
-        type: fp16 for a half model.  Half goes off first and on last, as the library refuses TF32 and the FFMA core in
-        half."""
+        type: fp16 for a half model.  Half and the fp16 precision go off first and on last, as the library refuses
+        TF32, the fp16 precision and the FFMA core in half, and half and the FFMA core at the fp16 precision.  A half
+        model at 'fp16' raises here, before anything is set or launched."""
         act = 1 if self.kind == L.KIND_MODEL and model_dtype(module, 'forward') == torch.float16 else 0
+        prec = _PRECISIONS[get_precision(module)]
+        if act and prec == _PRECISIONS['fp16']:
+            raise GastError("the model is half precision (model.half()), which has its own fp16 arithmetic; the fp16 "
+                            "precision is for float32 models: call engine.set_precision(model, 'fp32') (or "
+                            "model.float())")
         if act == 0 and self.act_dtype != 0:
             self._set_act(0)
+        if self.precision == _PRECISIONS['fp16'] and prec != self.precision:
+            self._set_precision(prec)
         if _FORCE_CORE['core'] != self.core:
             _check(self.lib.gast_set_gemm_core(self.h, _FORCE_CORE['core']), 'gast_set_gemm_core')
             self.core = _FORCE_CORE['core']
-        prec = _PRECISIONS[get_precision(module)]
         if prec != self.precision:
-            _check(self.lib.gast_set_precision(self.h, prec), 'gast_set_precision')
-            self.precision = prec
-        tprec = _PRECISIONS[get_training_precision(module)]
+            self._set_precision(prec)
+        tprec = _TRAIN_PRECISIONS[get_training_precision(module)]
         if tprec != self.train_precision:
             _check(self.lib.gast_set_train_precision(self.h, tprec), 'gast_set_train_precision')
             self.train_precision = tprec
         if act != self.act_dtype:
             self._set_act(act)
+
+    def _set_precision(self, prec):
+        _check(self.lib.gast_set_precision(self.h, prec), 'gast_set_precision')
+        self.precision = prec
 
     def _set_act(self, act):
         _check(self.lib.gast_set_activation_dtype(self.h, act), 'gast_set_activation_dtype')
@@ -704,7 +724,7 @@ def profile_forward(module, x, reps=5):
     ng = sum(v for k, v in n_launch.items() if fam(k))
     tc = int(lib.gast_last_tc_launch_count(h.h))
     # fp32 grade: three fp16 products on scaled operands, as precise as 3xTF32 (gemm_tc.cuh)
-    tc_name = ('wgmma-fp16' if model_dtype(module, 'profile_forward') == torch.float16
+    tc_name = ('wgmma-fp16' if model_dtype(module, 'profile_forward') == torch.float16 or get_precision(module) == 'fp16'
                else 'wgmma-1xtf32' if get_precision(module) == 'tf32' else 'wgmma-3xtf32-grade-3xfp16')
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     with torch.no_grad():

@@ -25,7 +25,11 @@ The rings hold activations computed with the weights of the pushes that wrote th
 parameters or buffers (`load_state_dict`, an optimiser step, a training forward, which moves the BatchNorm running
 statistics) therefore invalidates the history of every stream: the next push raises `GastError` unless `reset()`
 (every stream) was called after the change.  Switching the GEMM core (`engine.set_gemm_core`) or the precision
-(`engine.set_precision`, which the streams follow like every forward) changes no weight and keeps the streams.
+between 'fp32' and 'tf32' (`engine.set_precision`, which the streams follow like every forward) changes no weight and
+keeps the streams.  At 'fp16' the library keeps the rings in fp16 (half the bytes of history per stream), so a pool
+records the ring type its state was allocated at: a switch to or from 'fp16' reallocates the state when every stream
+is restarting and otherwise raises `GastError`.  A live pool changes precision by `export_streams` at the old
+precision and `import_streams` into a new pool at the new one (snapshots are float32 at every precision).
 
 `WindowStream` is the generic form for any callable network: a device ring of the last `rf` input frames and one
 window forward per pushed frame (what the reference does; used for non-GAST callables and as the cross-check).
@@ -257,6 +261,7 @@ class PoseStream(object):
         self._delta = np.zeros(self.n, dtype=np.int64)   # counts - step (>= 0; all 0 while the streams are in step)
         self._sig = None                 # the handle's parameter signature at the last push
         self._state = None
+        self._ring = None                # ring storage of the state: 'fp16' at the fp16 precision, else 'fp32'
         self._ws = None                  # library workspace of the largest call so far
         self._masks = None               # device [fresh | hold] masks of the largest push so far
 
@@ -337,12 +342,22 @@ class PoseStream(object):
 
     def _alloc_state(self, h):
         """allocate the zeroed library state of the copies * n library streams on first use, after checking that the
-        library's latency is the pool's"""
+        library's latency is the pool's; allocate it again at a precision with another ring storage type when every
+        stream is restarting, else refuse (the history is stored in the old type)"""
+        eng, lib = self.engine, h.lib
+        ring = 'fp16' if eng.get_precision(self.model) == 'fp16' else 'fp32'
+        if self._state is not None and ring != self._ring:
+            if not self.book.all_restarting():
+                raise eng.GastError("%s: the streams' history is stored in %s, the model is now set to precision %r, "
+                                    "which keeps it in %s; set the precision back, or move the live streams with "
+                                    "export_streams and import_streams into a pool used at the new precision"
+                                    % (type(self).__name__, self._ring, eng.get_precision(self.model), ring))
+            self._state = None
         if self._state is None:
-            eng, lib = self.engine, h.lib
             eng._check(lib.gast_stream_latency(h.h) != self.latency, 'gast_stream_latency')
             nb = eng._check_size(lib.gast_stream_state_bytes(h.h, self.copies * self.n), 'gast_stream_state_bytes')
             self._state = torch.zeros(nb, dtype=torch.uint8, device=self.device)
+            self._ring = ring
 
     def _mirror(self, lib, x, x2, rows, st):
         """x2 (2, rows, J, F) = [x | x mirrored]: the library input of the twins of x (rows, J, F) (gast_tta_prepare)"""

@@ -127,7 +127,8 @@ int32_t gast_get_timings(gast_t* h, int32_t max_n, float* ms, int32_t* kinds);
 
 /* GEMM core selection for A/B checks on the GPU: 0 = auto (tensor cores where the shape
  * allows; fp32-grade or single-pass TF32 as gast_set_precision says), 1 = force the FP32 FFMA core (fp32 in either
- * precision).  Not a fallback switch: both are CUDA paths. */
+ * precision; refused at the fp16 precision and in half, which run on the tensor cores only).  Not a fallback switch:
+ * both are CUDA paths. */
 int gast_set_gemm_core(gast_t* h, int32_t core);
 
 /* Arithmetic of the GEMMs the tensor-core core runs, for every handle kind and for gast_forward,
@@ -139,9 +140,21 @@ int gast_set_gemm_core(gast_t* h, int32_t core);
  *       rounded to 10 mantissa bits (round to nearest, ties away), so outputs move by ~1e-3 relative
  *       (DESIGN.md §4.1).  Inference only: gast_forward_train, gast_backward(_input), gast_eval_backward and their
  *       workspace queries fail while it is set, unless the training precision is TF32 too (gast_set_train_precision).
+ *   16 = fp16 (GAST_PRECISION_F16), MODEL kind only: the arithmetic and activation storage of the half form
+ *       (gast_set_activation_dtype(h, GAST_F16)) behind float32 x, y and parameters.  Every activation in the
+ *       workspace is fp16 (the attention row dots stay fp32); every GEMM is one fp16 product per multiply-add on
+ *       fp16(W 2^s_W) with fp32 accumulation; expand reads float32 x and writes fp16, shrink reads fp16 and writes
+ *       float32 y (and the mpjpe of gast_forward_mpjpe).  Each computes in fp32 and rounds once.  Outputs move by
+ *       ~2e-3 of max |y| (DESIGN.md §4.1).  The stream rings are fp16 (the input history stays float32), so
+ *       gast_stream_state_bytes depends on it and a state must be used at the precision it was sized at;
+ *       gast_stream_export / _import convert (snapshots stay float32), which is how streams change precision.
+ *       Inference only, like 1.  Setting it fails, before anything is launched, on a half handle (GAST_F16, which
+ *       has its own fp16 arithmetic), a sub-module kind, a handle forced onto the FFMA core, channels that are not a
+ *       multiple of 32 or more than 20 joints: the half form's own limits.
  * Any other value fails.  Everything else (expand, row-dots, the attention mix, shrink, GEMMs the tensor-core core
- * does not take, every GEMM under gast_set_gemm_core(h, 1)) stays fp32.  Like a core switch it needs no
- * gast_prepare, costs nothing and does not invalidate stream `state`. */
+ * does not take, every GEMM under gast_set_gemm_core(h, 1)) stays fp32 at 0 and 1.  Like a core switch it needs no
+ * gast_prepare and costs nothing; between 0 and 1 it does not invalidate stream `state`. */
+enum { GAST_PRECISION_F16 = 16 };
 int gast_set_precision(gast_t* h, int32_t mode);
 
 /* Activation type of the model forward (MODEL kind only):
@@ -157,7 +170,7 @@ int gast_set_precision(gast_t* h, int32_t mode);
  *       gast_backward_input, gast_eval_backward(_chunked), gast_chunked_workspace_bytes(.., 1), the training and
  *       eval-backward workspace queries and every gast_stream_* entry fail, as do gast_set_gemm_core(h, 1) and
  *       gast_set_precision(h, 1) (TF32 and half are separate modes: neither picks the other).  Setting GAST_F16 fails
- *       on a sub-module kind, a TF32 handle, one forced onto the FFMA core, channels that are not a multiple of 32
+ *       on a sub-module kind, a TF32 or fp16-precision handle, one forced onto the FFMA core, channels that are not a multiple of 32
  *       (the widths the half form takes) or more than 20 joints (the attention mix then needs the fused epilogue,
  *       which has no half form), before anything is launched.
  * bf16 is not offered (8 significant bits are about a centimetre on these poses).  Needs no gast_prepare. */
@@ -287,8 +300,9 @@ int gast_set_dropout_state(gast_t* h, void* dev_u64);
  *   The rings hold layer inputs computed with the weights of the pushes that wrote them.  A gast_prepare (after
  *   new weights or BatchNorm statistics were bound) therefore invalidates `state`: unless the next push marks
  *   every stream fresh, it mixes old and new weights for up to receptive_field - 1 pushes.  Nothing checks this
- *   here; gast_b200.realtime.CausalStream refuses such a push.  gast_set_gemm_core and gast_set_precision do not
- *   invalidate `state`. */
+ *   here; gast_b200.realtime.CausalStream refuses such a push.  gast_set_gemm_core and gast_set_precision between 0
+ *   and 1 do not invalidate `state`.  At the fp16 precision the rings are fp16 and the state is smaller: a state
+ *   sized at one ring type must not be pushed at the other (gast_stream_export / _import move streams across). */
 size_t gast_stream_state_bytes(gast_t* h, int32_t n_streams);
 size_t gast_stream_workspace_bytes(gast_t* h, int32_t n_streams);
 int gast_stream_push(gast_t* h, void* state, int64_t step, const float* x, float* y, int32_t n_streams,
@@ -412,7 +426,9 @@ int gast_stream_peek_device(gast_t* h, const void* state, int32_t n_streams, con
  *     [input history (k0, J, in_features), oldest first][ring_1 (R_1, J, C_1), oldest first] ... [ring_{L-1}]
  *   with k0 = filter_widths[0], C_i = channels << i, R_i = filter_widths[i] * (filter_widths[0] * ... *
  *   filter_widths[i-1]).  Row j of ring i of a stream whose count is c is its slot (c - R_i + j) mod R_i, so a
- *   snapshot does not depend on the ring phase.
+ *   snapshot does not depend on the ring phase.  Snapshots are float32 at every precision: an export from fp16 rings
+ *   (gast_set_precision(h, 16)) widens them exactly, an import into fp16 rings rounds to nearest, so streams move
+ *   between states of either precision.
  *   gast_stream_export writes out (m, snapshot_floats) (device) = the snapshots of streams streams[0..m) at their
  *   counts counts[0..m); `state` is only read.  gast_stream_import writes snapshot in[i] to stream streams[i] at the
  *   target count counts[i] (so it may land at any phase, e.g. at the target state's lockstep step) and writes no
