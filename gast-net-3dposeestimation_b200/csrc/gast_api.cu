@@ -79,6 +79,14 @@ struct StageConsts {
   std::vector<TcWeights> tc_rot;
 };
 
+template <typename Rec>
+struct AuditHook {   // one test-only launch audit of a handle: its callback, running index and captured-launch count
+  int (*fn)(int32_t phase, const Rec* d, void* user) = nullptr;
+  void* user = nullptr;
+  long long index = 0;
+  long long skips = 0;
+};
+
 struct gast_handle {
   gast_cfg cfg;
   std::vector<int32_t> sym_r, sym_c, con_r, con_c;
@@ -118,11 +126,10 @@ struct gast_handle {
   int fpt = 0;
   int sm_count = 132;
   float* loss_scratch = nullptr;   // shrink+mpjpe: SHL_MAXBLOCKS double partials | ticket (zero-initialised, reset by the kernel)
-  // test-only GEMM audit (gast_debug_set_gemm_audit): called around every launch_gemm outside graph capture
-  gast_gemm_audit_fn audit_fn = nullptr;
-  void* audit_user = nullptr;
-  long long audit_index = 0;
-  long long audit_skips = 0;
+  // test-only launch audits (gast_debug_set_gemm_audit, gast_debug_set_kernel_audit): called around every launch_gemm,
+  // and every expand, row-dot, attention-mix and shrink launch, outside graph capture
+  AuditHook<gast_gemm_audit> gemm_audit;
+  AuditHook<gast_kernel_audit> kernel_audit;
 };
 
 constexpr int GAST_MAX_PENDING_TRAIN = 16;   // training forwards that may wait for their backward per handle
@@ -730,10 +737,55 @@ static void gemm_defaults(GemmP& p, const gast_handle* h, long long F) {
 // F*J "frames" of one joint, so that every tile carries 128 rows instead of floor(128/J)*J (119 for J=17).
 static void gemm_defaults_flat(GemmP& p, const gast_handle* h, long long F) { gemm_flat(p, F * h->cfg.num_joints); }
 
+static void audit_describe(const gast_gemm_audit& d, char* s, size_t n) {
+  snprintf(s, n, "GEMM audit rejected launch %lld (epi %d, core %d, form %d, F %d J %d N %d K %d)", (long long)d.index,
+           d.epi, d.core, d.tc_form, d.F, d.J, d.N, d.ldw);
+}
+
+static void audit_describe(const gast_kernel_audit& d, char* s, size_t n) {
+  static const char* const kinds[] = {"expand", "rowdot", "mix", "shrink", "shrink_mpjpe"};
+  snprintf(s, n, "kernel audit rejected launch %lld (%s, variant %d, rows %lld K %d)", (long long)d.index,
+           kinds[d.kind], d.variant, (long long)d.rows, d.K);
+}
+
+// The host side of both test-only audits: launch() as it is when the hook is off, and, counted as a skip, under CUDA-graph
+// capture (a callback cannot read a captured launch's operands); otherwise fill(d) writes the record and the hook's
+// callback sees it just before and just after the launch, the stream synchronised each time.
+template <typename Rec, typename Fill, typename Launch>
+static int audited_launch(cudaStream_t st, AuditHook<Rec>& a, Fill fill, Launch launch) {
+  if (!a.fn) return launch();
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CUDA_OK(cudaStreamIsCapturing(st, &cs));
+  if (cs != cudaStreamCaptureStatusNone) {
+    a.skips++;
+    return launch();
+  }
+  Rec d;
+  memset(&d, 0, sizeof(d));
+  fill(d);
+  d.index = a.index++;
+  for (int phase = 0; phase < 2; ++phase) {
+    if (phase && launch()) return 1;
+    CUDA_OK(cudaStreamSynchronize(st));
+    if (a.fn(phase, &d, a.user)) {
+      char s[256];
+      audit_describe(d, s, sizeof(s));
+      return fail("%s %s", s, phase ? "after it ran" : "before it ran");
+    }
+  }
+  return 0;
+}
+
+template <typename Fill, typename Launch>
+static int kernel_audited(gast_handle* h, cudaStream_t st, Fill fill, Launch launch) {
+  return audited_launch(st, h->kernel_audit, [&](gast_kernel_audit& d) {
+    d.gemm_index = h->gemm_audit.index;
+    fill(d);
+  }, launch);
+}
+
 // the audit record of a launch (gast_gemm_audit mirrors GemmP); prec < 0: the FFMA core
-static void gemm_audit_record(const gast_handle* h, int epi, const GemmP& p, int prec, gast_gemm_audit* d) {
-  memset(d, 0, sizeof(*d));
-  d->index = h->audit_index;
+static void gemm_audit_record(int epi, const GemmP& p, int prec, gast_gemm_audit* d) {
   d->epi = epi;
   d->core = prec < 0 ? 1 : 0;
   d->tc_form = prec;
@@ -752,14 +804,6 @@ static void gemm_audit_record(const gast_handle* h, int epi, const GemmP& p, int
     memcpy(d->nbr_col[m], p.nbr[m].col, sizeof(d->nbr_col[m]));
   }
   d->ab = p.ab; d->ck = p.ck; d->bg = p.bg; d->heads = p.heads; d->Cg = p.Cg;
-}
-
-static int gemm_audit_call(gast_handle* h, cudaStream_t st, int phase, const gast_gemm_audit& d) {
-  CUDA_OK(cudaStreamSynchronize(st));
-  if (h->audit_fn(phase, &d, h->audit_user))
-    return fail("GEMM audit rejected launch %lld (epi %d, core %d, form %d, F %d J %d N %d K %d) %s", (long long)d.index,
-                d.epi, d.core, d.tc_form, d.F, d.J, d.N, d.ldw, phase ? "after it ran" : "before it ran");
-  return 0;
 }
 
 static int launch_gemm_core(gast_handle* h, cudaStream_t st, int epi, const GemmP& p, const TcWeights* tcw, int prec) {
@@ -809,28 +853,29 @@ static int launch_gemm(gast_handle* h, cudaStream_t st, int epi, const GemmP& p,
                   "multiples of 32)", p.N, p.ldw, epi);
     prec = TC_F16;
   }
-  if (!h->audit_fn) return launch_gemm_core(h, st, epi, p, tcw, prec);
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  CUDA_OK(cudaStreamIsCapturing(st, &cs));
-  if (cs != cudaStreamCaptureStatusNone) {
-    h->audit_skips++;
-    return launch_gemm_core(h, st, epi, p, tcw, prec);
-  }
-  gast_gemm_audit d;
-  gemm_audit_record(h, epi, p, prec, &d);
-  h->audit_index++;
-  if (gemm_audit_call(h, st, 0, d) || launch_gemm_core(h, st, epi, p, tcw, prec)) return 1;
-  return gemm_audit_call(h, st, 1, d);
+  return audited_launch(st, h->gemm_audit, [&](gast_gemm_audit& d) { gemm_audit_record(epi, p, prec, &d); },
+                        [&] { return launch_gemm_core(h, st, epi, p, tcw, prec); });
 }
 
 extern "C" int gast_debug_set_gemm_audit(gast_t* h, gast_gemm_audit_fn fn, void* user) {
   if (!h) return fail("gast_debug_set_gemm_audit: null handle");
-  h->audit_fn = fn;
-  h->audit_user = user;
+  h->gemm_audit.fn = fn;
+  h->gemm_audit.user = user;
   return 0;
 }
 
-extern "C" int64_t gast_debug_gemm_audit_skips(const gast_t* h) { return h ? h->audit_skips : -1; }
+extern "C" int64_t gast_debug_gemm_audit_skips(const gast_t* h) { return h ? h->gemm_audit.skips : -1; }
+
+extern "C" int gast_debug_set_kernel_audit(gast_t* h, gast_kernel_audit_fn fn, void* user) {
+  if (!h) return fail("gast_debug_set_kernel_audit: null handle");
+  h->kernel_audit.fn = fn;
+  h->kernel_audit.user = user;
+  return 0;
+}
+
+extern "C" int64_t gast_debug_kernel_audit_skips(const gast_t* h) { return h ? h->kernel_audit.skips : -1; }
+
+enum { KA_EXPAND = 0, KA_ROWDOT = 1, KA_MIX = 2, KA_SHRINK = 3, KA_SHRINK_MPJPE = 4 };
 
 // xf16: X holds fp16 (act_f16 in inference; training passes false)
 static int launch_rowdot(gast_handle* h, cudaStream_t st, const float* X, int ldx, const BlockConsts& b,
@@ -838,27 +883,36 @@ static int launch_rowdot(gast_handle* h, cudaStream_t st, const float* X, int ld
   if (rows <= 0) return 0;
   const int Q = 2 * b.heads;
   unsigned blocks = cdiv(rows * 32, 256);
-  TimedLaunch tl(h, st, LK_ROWDOT);
-  if (xf16) {   // X holds fp16; the row dots stay fp32 (they feed the softmax)
-    const __half* Xh = reinterpret_cast<const __half*>(X);
-    if (Q == 8 && (size_t)8 * b.C * sizeof(float) <= 48 * 1024) {
+  // rowdot8_kernel stages U in 48 KB of shared memory; its float32 form also reads X in float4 of 4 channels
+  const bool r8 = Q == 8 && (size_t)8 * b.C * sizeof(float) <= 48 * 1024 && (xf16 || b.C % 4 == 0);
+  auto fill = [&](gast_kernel_audit& d) {
+    d.kind = KA_ROWDOT; d.variant = r8 ? 0 : Q; d.block = (int)(&b - h->blocks.data());
+    d.in_type = xf16; d.x = X; d.U = b.U; d.cab = b.cab; d.ab = ab; d.rows = rows; d.K = b.C; d.ld = ldx;
+    d.heads = b.heads;
+  };
+  return kernel_audited(h, st, fill, [&] {
+    TimedLaunch tl(h, st, LK_ROWDOT);
+    if (xf16) {   // X holds fp16; the row dots stay fp32 (they feed the softmax)
+      const __half* Xh = reinterpret_cast<const __half*>(X);
+      if (r8) {
+        unsigned g = (unsigned)std::min<long long>((rows * 32 + 255) / 256, (long long)h->sm_count * 8);
+        rowdot8_kernel<<<g, 256, sizeof(float) * 8 * b.C, st>>>(Xh, ldx, b.U, b.cab, ab, rows, b.C);
+      } else if (Q == 8) rowdot_kernel<8><<<blocks, 256, 0, st>>>(Xh, ldx, b.U, b.cab, ab, rows, b.C);
+      else return fail("internal: fp16 forward with heads=%d", b.heads);
+      h->launches++;
+      return 0;
+    }
+    if (r8) {
       unsigned g = (unsigned)std::min<long long>((rows * 32 + 255) / 256, (long long)h->sm_count * 8);
-      rowdot8_kernel<<<g, 256, sizeof(float) * 8 * b.C, st>>>(Xh, ldx, b.U, b.cab, ab, rows, b.C);
-    } else if (Q == 8) rowdot_kernel<8><<<blocks, 256, 0, st>>>(Xh, ldx, b.U, b.cab, ab, rows, b.C);
-    else return fail("internal: fp16 forward with heads=%d", b.heads);
+      rowdot8_kernel<<<g, 256, sizeof(float) * 8 * b.C, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
+    } else if (Q == 8) rowdot_kernel<8><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
+    else if (Q == 6) rowdot_kernel<6><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
+    else if (Q == 4) rowdot_kernel<4><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
+    else if (Q == 2) rowdot_kernel<2><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
+    else return fail("internal: heads=%d", b.heads);
     h->launches++;
     return 0;
-  }
-  if (Q == 8 && b.C % 4 == 0 && (size_t)8 * b.C * sizeof(float) <= 48 * 1024) {
-    unsigned g = (unsigned)std::min<long long>((rows * 32 + 255) / 256, (long long)h->sm_count * 8);
-    rowdot8_kernel<<<g, 256, sizeof(float) * 8 * b.C, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
-  } else if (Q == 8) rowdot_kernel<8><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
-  else if (Q == 6) rowdot_kernel<6><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
-  else if (Q == 4) rowdot_kernel<4><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
-  else if (Q == 2) rowdot_kernel<2><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
-  else return fail("internal: heads=%d", b.heads);
-  h->launches++;
-  return 0;
+  });
 }
 
 // SemCH (both masks) -> XY ; then local cat conv -> L          (local_attention.py:130-151)
@@ -903,17 +957,24 @@ static int run_global(gast_handle* h, cudaStream_t st, BlockConsts& b, const flo
     int fpb = GV >= MIX_THREADS ? 1 : MIX_THREADS / GV;
     fpb = std::max(1, std::min(fpb, (int)(40 * 1024 / (sizeof(float) * b.heads * J * MIX_JP))));   // attention rows fit 40 KB
     const size_t smem = sizeof(float) * (size_t)fpb * b.heads * J * MIX_JP;
-    {
-      TimedLaunch tl(h, st, LK_GLOBAL_MIX);
-      if (act_f16(h))
-        global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(reinterpret_cast<const __half*>(out_G), Ng, w.AB,
-                                                                   b.Ck, reinterpret_cast<__half*>(w.Y), Ng, F, J,
-                                                                   b.heads, b.Cg, fpb);
-      else
-        global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(out_G, Ng, w.AB, b.Ck, w.Y, Ng, F, J, b.heads, b.Cg,
-                                                                   fpb);
-      h->launches++;
-    }
+    auto fill = [&](gast_kernel_audit& d) {
+      d.kind = KA_MIX; d.fpb = fpb; d.block = (int)(&b - h->blocks.data());
+      d.in_type = d.out_type = act_f16(h); d.x = out_G; d.ab = w.AB; d.Ck = b.Ck; d.out = w.Y;
+      d.rows = F; d.K = Ng; d.ld = Ng; d.J = J; d.heads = b.heads; d.Cg = b.Cg;
+    };
+    if (kernel_audited(h, st, fill, [&] {
+          TimedLaunch tl(h, st, LK_GLOBAL_MIX);
+          if (act_f16(h))
+            global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(reinterpret_cast<const __half*>(out_G), Ng,
+                                                                       w.AB, b.Ck, reinterpret_cast<__half*>(w.Y), Ng,
+                                                                       F, J, b.heads, b.Cg, fpb);
+          else
+            global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(out_G, Ng, w.AB, b.Ck, w.Y, Ng, F, J, b.heads,
+                                                                       b.Cg, fpb);
+          h->launches++;
+          return 0;
+        }))
+      return 1;
     CUDA_OK(cudaGetLastError());
     gemm_defaults_flat(p, h, F);
     p.nseg = 1; p.seg[0] = seg_flat(w.Y, C, C);
@@ -955,39 +1016,47 @@ static int launch_expand(gast_handle* h, cudaStream_t st, const float* x, float*
   const int k0 = c.filter_widths[0], Fin = c.in_features;
   if (rows >= 0x7fffffffLL) return fail("expand: more than 2^31 positions in one call");
   if (k0 * Fin > EXP_MAXKF) return fail("expand: filter_width*in_features > %d unsupported", EXP_MAXKF);
-  TimedLaunch tl(h, st, LK_EXPAND);
-  const dim3 grid(cdiv(rows, EXS_ROWS), cdiv(c.channels, EXS_CHUNK));
-  if (h->act_dtype == GAST_F32 && act_f16(h)) {   // the fp16 precision: float32 x, fp16 out
-    __half* oh = reinterpret_cast<__half*>(out);
+  auto fill = [&](gast_kernel_audit& d) {
+    d.kind = KA_EXPAND; d.variant = k0 * Fin <= 6 ? 6 : EXP_MAXKF;
+    d.in_type = h->act_dtype == GAST_F16; d.out_type = act_f16(h); d.x = x; d.We = h->We; d.be = h->be; d.out = out;
+    d.rows = rows; d.K = c.channels; d.ld = c.channels; d.J = c.num_joints; d.T = T; d.T0 = T0; d.stride = stride;
+    d.taps = k0; d.Fin = Fin;
+  };
+  return kernel_audited(h, st, fill, [&] {
+    TimedLaunch tl(h, st, LK_EXPAND);
+    const dim3 grid(cdiv(rows, EXS_ROWS), cdiv(c.channels, EXS_CHUNK));
+    if (h->act_dtype == GAST_F32 && act_f16(h)) {   // the fp16 precision: float32 x, fp16 out
+      __half* oh = reinterpret_cast<__half*>(out);
+      if (k0 * Fin <= 6)
+        expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, oh, rows, c.num_joints, T, T0, stride, k0,
+                                                             Fin, c.channels);
+      else
+        expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, oh, rows, c.num_joints, T, T0,
+                                                                     stride, k0, Fin, c.channels);
+      h->launches++;
+      return 0;
+    }
+    if (h->act_dtype == GAST_F16) {
+      const __half* xh = reinterpret_cast<const __half*>(x);
+      __half* oh = reinterpret_cast<__half*>(out);
+      if (k0 * Fin <= 6)
+        expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(xh, h->We, h->be, oh, rows, c.num_joints, T, T0, stride,
+                                                             k0, Fin, c.channels);
+      else
+        expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(xh, h->We, h->be, oh, rows, c.num_joints, T, T0,
+                                                                     stride, k0, Fin, c.channels);
+      h->launches++;
+      return 0;
+    }
     if (k0 * Fin <= 6)
-      expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, oh, rows, c.num_joints, T, T0, stride, k0,
+      expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, out, rows, c.num_joints, T, T0, stride, k0,
                                                            Fin, c.channels);
     else
-      expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, oh, rows, c.num_joints, T, T0,
+      expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, out, rows, c.num_joints, T, T0,
                                                                    stride, k0, Fin, c.channels);
     h->launches++;
     return 0;
-  }
-  if (h->act_dtype == GAST_F16) {
-    const __half* xh = reinterpret_cast<const __half*>(x);
-    __half* oh = reinterpret_cast<__half*>(out);
-    if (k0 * Fin <= 6)
-      expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(xh, h->We, h->be, oh, rows, c.num_joints, T, T0, stride, k0,
-                                                           Fin, c.channels);
-    else
-      expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(xh, h->We, h->be, oh, rows, c.num_joints, T, T0,
-                                                                   stride, k0, Fin, c.channels);
-    h->launches++;
-    return 0;
-  }
-  if (k0 * Fin <= 6)
-    expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, out, rows, c.num_joints, T, T0, stride, k0,
-                                                         Fin, c.channels);
-  else
-    expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, out, rows, c.num_joints, T, T0, stride,
-                                                                 k0, Fin, c.channels);
-  h->launches++;
-  return 0;
+  });
 }
 
 // temporal stage on F frames: conv over the taps of `taps` + BN + ReLU into tmp, then 1x1 conv + BN + ReLU (+Dropout =
@@ -1014,31 +1083,35 @@ static int launch_shrink(gast_handle* h, cudaStream_t st, const float* X, float*
   const int Cl = h->cfg.channels << h->cfg.num_stages;
   const float* ws = Lk.get("shrink.weight", (int64_t)3 * Cl);
   if (!Lk.ok) return 1;
-  if (target) {
-    static_assert(SHL_MAXBLOCKS == 1024, "loss_scratch is sized for 1024 block partials");
-    if (!h->loss_scratch) return fail("gast_forward_mpjpe: handle has no loss scratch");
-    double* partial = reinterpret_cast<double*>(h->loss_scratch);
-    unsigned* ticket = reinterpret_cast<unsigned*>(h->loss_scratch + 2 * SHL_MAXBLOCKS);
-    const unsigned nb = (unsigned)std::min<long long>(SHL_MAXBLOCKS, (rows + 7) / 8);
+  static_assert(SHL_MAXBLOCKS == 1024, "loss_scratch is sized for 1024 block partials");
+  if (target && !h->loss_scratch) return fail("gast_forward_mpjpe: handle has no loss scratch");
+  auto fill = [&](gast_kernel_audit& d) {
+    d.kind = target ? KA_SHRINK_MPJPE : KA_SHRINK;
+    d.in_type = act_f16(h); d.out_type = h->act_dtype == GAST_F16; d.x = X; d.Ws = ws; d.target = target;
+    d.loss = loss; d.out = y; d.rows = rows; d.K = Cl; d.ld = Cl;
+  };
+  return kernel_audited(h, st, fill, [&] {
     TimedLaunch tl(h, st, LK_SHRINK);
-    if (act_f16(h))   // the fp16 precision (a half model refuses the mpjpe forward): fp16 X, float32 y
-      shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws, y, rows, Cl, target, partial,
-                                              ticket, loss);
-    else
-      shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(X, Cl, ws, y, rows, Cl, target, partial, ticket, loss);
-  } else if (h->act_dtype == GAST_F32 && act_f16(h)) {
-    TimedLaunch tl(h, st, LK_SHRINK);
-    shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws, y, rows, Cl);
-  } else if (h->act_dtype == GAST_F16) {
-    TimedLaunch tl(h, st, LK_SHRINK);
-    shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws,
-                                                        reinterpret_cast<__half*>(y), rows, Cl);
-  } else {
-    TimedLaunch tl(h, st, LK_SHRINK);
-    shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(X, Cl, ws, y, rows, Cl);
-  }
-  h->launches++;
-  return 0;
+    if (target) {
+      double* partial = reinterpret_cast<double*>(h->loss_scratch);
+      unsigned* ticket = reinterpret_cast<unsigned*>(h->loss_scratch + 2 * SHL_MAXBLOCKS);
+      const unsigned nb = (unsigned)std::min<long long>(SHL_MAXBLOCKS, (rows + 7) / 8);
+      if (act_f16(h))   // the fp16 precision (a half model refuses the mpjpe forward): fp16 X, float32 y
+        shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws, y, rows, Cl, target,
+                                                partial, ticket, loss);
+      else
+        shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(X, Cl, ws, y, rows, Cl, target, partial, ticket, loss);
+    } else if (h->act_dtype == GAST_F32 && act_f16(h)) {
+      shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws, y, rows, Cl);
+    } else if (h->act_dtype == GAST_F16) {
+      shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws,
+                                                          reinterpret_cast<__half*>(y), rows, Cl);
+    } else {
+      shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(X, Cl, ws, y, rows, Cl);
+    }
+    h->launches++;
+    return 0;
+  });
 }
 
 // In a half forward (gast_set_activation_dtype) and at the fp16 precision (act_f16) every buffer but bb.AB holds fp16:

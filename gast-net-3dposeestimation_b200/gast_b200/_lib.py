@@ -20,7 +20,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_get_timings', 'gast_set_gemm_core', 'gast_set_precision', 'gast_set_train_precision',
            'gast_set_activation_dtype',
            'gast_last_wgrad_tc_launch_count', 'gast_debug_gemm', 'gast_debug_wgrad', 'gast_debug_set_gemm_audit',
-           'gast_debug_gemm_audit_skips', 'gast_bind_grads',
+           'gast_debug_gemm_audit_skips', 'gast_debug_set_kernel_audit', 'gast_debug_kernel_audit_skips',
+           'gast_bind_grads',
            'gast_train_workspace_bytes', 'gast_forward_train', 'gast_backward', 'gast_backward_input',
            'gast_eval_backward_workspace_bytes', 'gast_eval_backward', 'gast_chunked_workspace_bytes',
            'gast_forward_chunked', 'gast_eval_backward_chunked', 'gast_set_dropout_state', 'gast_tta_prepare', 'gast_tta_merge',
@@ -71,6 +72,21 @@ class GemmAudit(C.Structure):
 
 
 GemmAuditFn = C.CFUNCTYPE(C.c_int32, C.c_int32, C.POINTER(GemmAudit), C.c_void_p)
+
+
+class KernelAudit(C.Structure):
+    """gast_kernel_audit: what one expand, row-dot, attention-mix or shrink launch receives
+    (gast_debug_set_kernel_audit)"""
+    _fields_ = [('index', C.c_int64), ('gemm_index', C.c_int64), ('kind', C.c_int32), ('variant', C.c_int32),
+                ('fpb', C.c_int32), ('block', C.c_int32), ('in_type', C.c_int32), ('out_type', C.c_int32),
+                ('x', C.c_void_p), ('We', C.c_void_p), ('be', C.c_void_p), ('U', C.c_void_p), ('cab', C.c_void_p),
+                ('ab', C.c_void_p), ('Ck', C.c_void_p), ('Ws', C.c_void_p), ('target', C.c_void_p),
+                ('loss', C.c_void_p), ('out', C.c_void_p), ('rows', C.c_int64), ('K', C.c_int32), ('ld', C.c_int32),
+                ('J', C.c_int32), ('T', C.c_int32), ('T0', C.c_int32), ('stride', C.c_int32), ('taps', C.c_int32),
+                ('Fin', C.c_int32), ('heads', C.c_int32), ('Cg', C.c_int32)]
+
+
+KernelAuditFn = C.CFUNCTYPE(C.c_int32, C.c_int32, C.POINTER(KernelAudit), C.c_void_p)
 
 _lib = None
 
@@ -132,6 +148,10 @@ def load():
     lib.gast_debug_set_gemm_audit.restype = C.c_int
     lib.gast_debug_gemm_audit_skips.argtypes = [vp]
     lib.gast_debug_gemm_audit_skips.restype = C.c_int64
+    lib.gast_debug_set_kernel_audit.argtypes = [vp, KernelAuditFn, vp]
+    lib.gast_debug_set_kernel_audit.restype = C.c_int
+    lib.gast_debug_kernel_audit_skips.argtypes = [vp]
+    lib.gast_debug_kernel_audit_skips.restype = C.c_int64
     lib.gast_bind_grads.argtypes = [vp, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(vp), C.POINTER(C.c_int64)]
     lib.gast_bind_grads.restype = C.c_int
     lib.gast_train_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32, C.c_float]

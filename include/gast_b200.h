@@ -605,6 +605,41 @@ typedef int (*gast_gemm_audit_fn)(int32_t phase, const gast_gemm_audit* d, void*
 int gast_debug_set_gemm_audit(gast_t* h, gast_gemm_audit_fn fn, void* user);
 int64_t gast_debug_gemm_audit_skips(const gast_t* h);
 
+/* Test-only audit of the other kernels of the inference forward and the streams, on the GEMM audit's terms: every
+ * launch of the expand, the theta/phi row dots (the training forward's too), the attention mix kernel and the shrink.
+ *   expand (kind 0):  out[r][c] = relu(be[c] + sum_{kk < taps, i < Fin} We[kk Fin + i][c] x[((b T + t stride + kk) J + j)
+ *                     Fin + i]) for rows r = (b T0 + t) J + j < rows, c < C = K (ld = C); variant = KFT (6 or 10).
+ *   rowdot (1):       ab[r][q] = X[r ld + k] U[q][k] + cab[q], q < Q = 2 heads, k < K; variant 0 = rowdot8_kernel,
+ *                     else Q of rowdot_kernel<Q>; block = the handle's graph-attention block.
+ *   mix (2):          Y[(f J + i) ld + n] = sum_j att_{n / Cg}[f, i, j] G[(f J + j) ld + n], n < heads Cg, f < F, with
+ *                     att_h = softmax_j(LeakyReLU_0.2(ab[f J + i][2h] + ab[f J + j][2h + 1])) + Ck[h][i][j]; fpb frames
+ *                     per CTA; block as for rowdot.
+ *   shrink (3):       out[r][o] = X[r ld + k] Ws[o][k], o < 3, k < K.
+ *   shrink_mpjpe (4): shrink into out, and *loss = mean_r ||out[r] - target[r]||.
+ * in_type / out_type: 0 float32, 1 fp16 (the rowdot's ab and shrink_mpjpe's out, target and loss are float32).
+ * gemm_index: the number of GEMM launches the GEMM audit had checked before this one. */
+typedef struct gast_kernel_audit {
+  int64_t index;                         /* running index of the handle's audited kernel launches */
+  int64_t gemm_index;
+  int32_t kind;                          /* 0 expand, 1 rowdot, 2 mix, 3 shrink, 4 shrink_mpjpe */
+  int32_t variant, fpb, block;
+  int32_t in_type, out_type;
+  const void* x;                         /* x (expand), X (rowdot, shrink) or G (mix) */
+  const float* We; const float* be;      /* expand */
+  const float* U; const float* cab;      /* rowdot */
+  float* ab;                             /* rowdot: written; mix: read */
+  const float* Ck;                       /* mix */
+  const float* Ws; const float* target;  /* shrink */
+  float* loss;
+  void* out;                             /* out (expand, shrink) or Y (mix) */
+  int64_t rows;                          /* rows (expand, rowdot, shrink) or frames F (mix) */
+  int32_t K, ld, J, T, T0, stride, taps, Fin, heads, Cg;
+} gast_kernel_audit;
+
+typedef int (*gast_kernel_audit_fn)(int32_t phase, const gast_kernel_audit* d, void* user);
+int gast_debug_set_kernel_audit(gast_t* h, gast_kernel_audit_fn fn, void* user);
+int64_t gast_debug_kernel_audit_skips(const gast_t* h);
+
 const char* gast_last_error(void);
 const char* gast_version(void);
 
