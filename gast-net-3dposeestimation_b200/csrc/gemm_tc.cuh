@@ -55,13 +55,22 @@
 //     The two consumers do not synchronise with each other inside the K loop, so one's MMAs fill the other's drain.
 // Tiles (fpt whole frames per 128-row tile) and the fused epilogues are the FFMA core's, so both cores are
 // interchangeable per launch.  EPI_PLAIN runs on the wgmma fragments (tc_store_plain: bias, ReLU, residual in
-// gemm_epilogue's order) and leaves by four TMA tensor stores from the freed ring; EPI_SEMCH and EPI_GLOBAL mix
-// joints across rows, so their tiles are handed over in the FFMA thread layout to gemm_epilogue, run by the 256
-// consumer threads.
+// gemm_epilogue's order) and leaves by four TMA tensor stores from a 64 KB staging buffer of its own; EPI_SEMCH and
+// EPI_GLOBAL mix joints across rows, so their tiles are handed over in the FFMA thread layout to gemm_epilogue, run by
+// the 256 consumer threads, with the ring as scratch.
 //
-// One tile per CTA, on a 1D grid in which the column tile is the fast index (tc_launch): the CTAs dispatched together
-// cover a row tile's column tiles side by side, so its A rows come from HBM once and its other column tiles find them
-// in L2.  (Every layer's A is larger than the L2; with the row tile fast, A was read from HBM once per column tile.)
+// Tiles are numbered on a 1D order in which the column tile is the fast index: the CTAs running together cover a row
+// tile's column tiles side by side, so its A rows come from HBM once and its other column tiles find them in L2.
+// (Every layer's A is larger than the L2; with the row tile fast, A was read from HBM once per column tile.)
+//   EPI_PLAIN is persistent (tc_persistent): min(tiles, SMs) CTAs, CTA i takes tiles i, i + grid, i + 2 grid, ...
+//     The ring's stage counter c and the mbarrier phases run on across tiles (stage c of the CTA's run uses slot
+//     c % STAGES; `full` is waited on parity (c / STAGES) & 1, `empty` before refilling on (c / STAGES - 1) & 1), and
+//     the producer rebuilds its row table (`rowbase`, under named barrier 3 over its 128 threads) at each tile, so it
+//     fills the next tile's first stages while the consumers finish the current one.  The consumers write a finished
+//     tile into the staging buffer, meet at one named barrier, and one of them issues the tensor stores; it waits for
+//     the TMA engine to have read them only before the next tile is written there (and before it exits), so the
+//     consumers go on to the next tile's K loop while the stores drain.
+//   EPI_SEMCH and EPI_GLOBAL use the ring as their epilogue's scratch, so they run one tile per CTA (grid = tiles).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -117,15 +126,23 @@ __host__ __device__ constexpr int tc_stages(int prec) {
 __host__ __device__ constexpr int tc_ring(int prec) { return tc_stages(prec) * tc_slot(prec); }
 constexpr int TC_STG_LD = 136;                       // [row][col] stride of the accumulator hand-over to the epilogue
 constexpr int TC_ROWBASE_BYTES = 3 * 128 * sizeof(long long);
-constexpr int TC_SMEM_MAX = 200 * 1024;
+constexpr int TC_SMEM_MAX = 200 * 1024;              // the half form's bound
+constexpr int TC_SMEM_OPTIN = 227 * 1024;            // the SM's opt-in shared memory per block: gemm_tc_kernel's bound
+constexpr int TC_TILE_BYTES = TC_BM * TC_BN * 4;     // EPI_PLAIN's staging buffer: one fp32 tile
+// EPI_PLAIN runs a persistent tile loop; EPI_SEMCH and EPI_GLOBAL, whose epilogues take the ring as scratch, one tile
+// per CTA
+__host__ __device__ constexpr bool tc_persistent(int epi) { return epi == EPI_PLAIN; }
 static_assert(tc_slot(TC_3XTF32) % 1024 == 0 && tc_slot(TC_1XTF32) % 1024 == 0 && tc_slot(TC_F16X3) % 1024 == 0 &&
               TC_B16_BYTES % 1024 == 0, "ring slots and their A stages stay 1024-byte aligned");
 static_assert(tc_ring(TC_1XTF32) + 16 * tc_stages(TC_1XTF32) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX &&
               tc_ring(TC_F16X3) + 16 * tc_stages(TC_F16X3) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX,
               "every ring fits the shared memory the core may use");
 
+// rowbase | ring (1024-byte aligned) | EPI_PLAIN: staging buffer | a full and an empty mbarrier per slot
 __host__ __device__ inline size_t tc_smem_bytes(int prec, int epi, int J, int fpt, int hpt) {
-  size_t m = (size_t)tc_ring(prec) + 16 * tc_stages(prec);   // + a full and an empty mbarrier per slot
+  if (tc_persistent(epi))
+    return TC_ROWBASE_BYTES + 1024 + (size_t)tc_ring(prec) + TC_TILE_BYTES + 16 * tc_stages(prec);
+  size_t m = (size_t)tc_ring(prec) + 16 * tc_stages(prec);
   const size_t stg = (size_t)TC_BM * TC_STG_LD * 4;
   const size_t e = ffma_smem_bytes(epi, J, fpt, hpt) - TC_ROWBASE_BYTES;
   if (stg > m) m = stg;
@@ -375,11 +392,13 @@ __device__ __forceinline__ void tc_tile(const GemmP& p, int& rt, int& ctile) {
 }
 
 // EPI_PLAIN on the consumers' wgmma fragments (rows r0, r0 + 8; columns 8 i + 2t, + 1 in acc[4 i ..]): bias, ReLU and
-// residual in gemm_epilogue's order, so the bits are the same, then the tile goes through the free ring to TMA as four
-// 128-byte-swizzled column blocks of 32 floats ([128][32] each, 16 KB apart), and one thread stores them with `out`
-// (tile rows f0 J .. f0 J + fpt J - 1 of the box; the map's dims drop rows past F J and columns past N).
-__device__ __forceinline__ void tc_store_plain(const GemmP& p, const float (&acc)[64], unsigned char* ring,
-                                               uint32_t rb, const CUtensorMap& out, int r0, int t, int ct, int f0,
+// residual in gemm_epilogue's order, so the bits are the same, then the tile goes through the staging buffer (`stage`,
+// shared address sb) to TMA as four 128-byte-swizzled column blocks of 32 floats ([128][32] each, 16 KB apart), and
+// consumer thread 0 stores them with `out` (tile rows f0 J .. f0 J + fpt J - 1 of the box; the map's dims drop rows
+// past F J and columns past N).  The buffer must be free (the previous stores read) when this is called; the stores
+// are committed as one bulk group, not waited for.
+__device__ __forceinline__ void tc_store_plain(const GemmP& p, const float (&acc)[64], unsigned char* stage,
+                                               uint32_t sb, const CUtensorMap& out, int r0, int t, int ct, int f0,
                                                int vrows, int n0) {
   const int J = p.J;
   const float* resrow[2] = {nullptr, nullptr};
@@ -391,7 +410,7 @@ __device__ __forceinline__ void tc_store_plain(const GemmP& p, const float (&acc
       resrow[h] = p.res + (map_frame(p.res_map, f0 + fr) * J + j) * (long long)p.res_ld;
     }
   }
-  float* S = reinterpret_cast<float*>(ring);
+  float* S = reinterpret_cast<float*>(stage);
 #pragma unroll
   for (int i = 0; i < 16; ++i) {
     const int col = 8 * i + 2 * t, n = n0 + col;
@@ -416,10 +435,29 @@ __device__ __forceinline__ void tc_store_plain(const GemmP& p, const float (&acc
   epi_sync();
   if (ct == 0) {
     for (int cb = 0; cb < TC_BN / TC_KS && n0 + cb * TC_KS < p.N; ++cb)
-      tma_store_2d(&out, rb + cb * TC_A_BYTES, n0 + cb * TC_KS, f0 * J);
+      tma_store_2d(&out, sb + cb * TC_A_BYTES, n0 + cb * TC_KS, f0 * J);
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the ring may go once the engine has read it
   }
+}
+
+// consumer thread 0: wait until the TMA engine has read every tensor store it issued from the staging buffer
+__device__ __forceinline__ void tc_stores_read(int ct) {
+  if (ct == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+}
+
+// Whether this CTA has a tile after its tile u (tile blockIdx.x + u gridDim.x), and that tile's row and column tile.
+// %ctaid and %nctaid are read with volatile moves, so that the consumers recompute the tile after their K loop instead
+// of keeping it in registers through it.
+__device__ __forceinline__ bool tc_tile_at(const GemmP& p, int u, int& rt, int& ctile) {
+  uint32_t b, g;
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(b));
+  asm volatile("mov.u32 %0, %%nctaid.x;" : "=r"(g));
+  const int col_tiles = (p.N + TC_BN - 1) / TC_BN;
+  const long long tile = b + (long long)u * g;
+  if (tile >= (long long)((p.F + p.fpt - 1) / p.fpt) * col_tiles) return false;
+  rt = (int)(tile / col_tiles);
+  ctile = (int)(tile - (long long)rt * col_tiles);
+  return true;
 }
 
 // mlo is not read in 1xTF32, sw (s_W) only in F16X3, am.seg[s] only for the segments tc_seg_tma takes, am.out only in
@@ -432,22 +470,18 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   constexpr int STAGES = tc_stages(PREC), SLOT = tc_slot(PREC), NB = tc_nb(PREC);
   constexpr int BBYTES = tc_bbytes(PREC);
   constexpr int KSH = PREC == TC_F16X3 ? 3 : 2;                         // log2 of the k's per 16-byte row of a B copy
+  constexpr int STG = tc_persistent(EPI) ? TC_TILE_BYTES : 0;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   long long* rowbase = reinterpret_cast<long long*>(smem_raw);          // [3][128]
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t rb = (raw + TC_ROWBASE_BYTES + 1023) & ~1023u;        // ring base (shared address)
   unsigned char* ring = smem_raw + (rb - raw);
-  const uint32_t full0 = rb + tc_ring(PREC);                            // per ring slot: stage landed
+  const uint32_t stg = rb + tc_ring(PREC);                              // EPI_PLAIN: staging buffer
+  const uint32_t full0 = stg + STG;                                     // per ring slot: stage landed
   const uint32_t empty0 = full0 + 8 * STAGES;                           // per ring slot: both consumers done with it
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int J = p.J;
-  int rt, ctile;
-  tc_tile(p, rt, ctile);
-  const int f0 = rt * p.fpt;
-  const int nf = min(p.fpt, p.F - f0);
-  const int vrows = nf * J;
-  const int n0 = ctile * TC_BN;
   int tma_segs = 0;                                                     // bit s: segment s is loaded by TMA
   for (int s = 0; s < p.nseg; ++s) tma_segs |= tc_seg_tma(p.seg[s]) << s;
   const bool gather = tma_segs != (1 << p.nseg) - 1;                    // some segment is gathered per row
@@ -460,57 +494,69 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  for (int i = tid; i < p.nseg * 128; i += TC_THREADS) {
-    int s = i >> 7, r = i & 127;
-    long long off = -1;
-    if (r < vrows) {
-      int fr = r / J, j = r - fr * J;
-      long long fin = map_frame(p.seg[s].map, f0 + fr);
-      off = (fin * J + j) * (long long)p.seg[s].ld;
-    }
-    rowbase[s * 128 + r] = off;
-  }
   __syncthreads();
 
   int nstages = 0;
   for (int s = 0; s < p.nseg; ++s) nstages += p.seg[s].K / TC_KS;
 
   if (warp < 4) {
-    // producer: stage c into ring slot c % STAGES once both consumers have released the slot's previous stage
+    // producer: stage c of the CTA's run into ring slot c % STAGES once both consumers have released the slot's
+    // previous stage
     setmaxnreg_dec<TC_PRODUCER_REGS>();
     if (!gather && tid != 0) return;                                    // the elected thread issues every stage
     const int q = tid & 7, rq = tid >> 3;                               // k-quad q of rows rq + 16 i
     const uint32_t adst = NB * BBYTES + 4 * tc_achunk(rq, q);           // its slot offset in row rq; rows + 16 i follow
-    const int row0 = f0 * J;                                            // source row of tile row 0 (TMA segments)
-    int seg = 0, k0 = 0, kcol = 0, tap = 0, kin = 0;                    // stage start: segment, K in it, W column, tap
-    for (int c = 0; c < nstages; ++c) {
-      const int slot = c % STAGES;
-      if (c >= STAGES) mbar_wait(empty0 + 8 * slot, (c / STAGES - 1) & 1);
-      const uint32_t sb = rb + slot * SLOT, full = full0 + 8 * slot;
-      const bool tma_a = (tma_segs >> seg) & 1;
-      if (tid == 0) {
-        mbar_arrive_expect_tx(full, NB * BBYTES + (tma_a ? TC_A_BYTES : 0));
-        const int kq = (kcol + k0) >> KSH;
-        tma_load_2d(sb, &mhi, full, 2 * n0, kq);
-        if (NB == 2) tma_load_2d(sb + BBYTES, &mlo, full, 2 * n0, kq);
-        if (tma_a) tma_load_2d(sb + NB * BBYTES, &am.seg[seg], full, kin, row0);
-      }
-      const ASeg& sg = p.seg[seg];
-      if (tma_a) {
-        if (gather) mbar_arrive(full);                                  // the barrier counts 128 producer arrivals
-      } else {
-        const float* src = sg.base + tap * sg.tap_stride + kin + q * 4;
-#pragma unroll
-        for (int i = 0; i < TC_BM / 16; ++i) {
-          const long long off = rowbase[seg * 128 + rq + 16 * i];
-          cp_async16(sb + adst + i * 16 * 128, off >= 0 ? src + off : sg.base, off >= 0 ? 16 : 0);
+    const int col_tiles = (p.N + TC_BN - 1) / TC_BN;
+    const int tiles = ((p.F + p.fpt - 1) / p.fpt) * col_tiles;
+    int c = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+      const int rt = tile / col_tiles;
+      const int f0 = rt * p.fpt, n0 = (tile - rt * col_tiles) * TC_BN;
+      if (gather) {                                                     // the tile's row table, for the gathered rows
+        const int vrows = min(p.fpt, p.F - f0) * J;
+        asm volatile("bar.sync 3, 128;" ::: "memory");                  // every thread has issued the last tile
+        for (int i = tid; i < p.nseg * 128; i += 128) {
+          const int s = i >> 7, r = i & 127;
+          long long off = -1;
+          if (r < vrows) {
+            const int fr = r / J, j = r - fr * J;
+            off = (map_frame(p.seg[s].map, f0 + fr) * J + j) * (long long)p.seg[s].ld;
+          }
+          rowbase[i] = off;
         }
-        cp_async_arrive(full);
+        asm volatile("bar.sync 3, 128;" ::: "memory");
       }
-      k0 += TC_KS;
-      kin += TC_KS;
-      if (kin == sg.Kc) { kin = 0; ++tap; }
-      if (k0 == sg.K) { kcol += sg.K; k0 = 0; tap = 0; ++seg; }
+      const int row0 = f0 * J;                                          // source row of tile row 0 (TMA segments)
+      int seg = 0, k0 = 0, kcol = 0, tap = 0, kin = 0;                  // stage start: segment, K in it, W column, tap
+      for (int k = 0; k < nstages; ++k, ++c) {
+        const int slot = c % STAGES;
+        if (c >= STAGES) mbar_wait(empty0 + 8 * slot, (c / STAGES - 1) & 1);
+        const uint32_t sb = rb + slot * SLOT, full = full0 + 8 * slot;
+        const bool tma_a = (tma_segs >> seg) & 1;
+        if (tid == 0) {
+          mbar_arrive_expect_tx(full, NB * BBYTES + (tma_a ? TC_A_BYTES : 0));
+          const int kq = (kcol + k0) >> KSH;
+          tma_load_2d(sb, &mhi, full, 2 * n0, kq);
+          if (NB == 2) tma_load_2d(sb + BBYTES, &mlo, full, 2 * n0, kq);
+          if (tma_a) tma_load_2d(sb + NB * BBYTES, &am.seg[seg], full, kin, row0);
+        }
+        const ASeg& sg = p.seg[seg];
+        if (tma_a) {
+          if (gather) mbar_arrive(full);                                // the barrier counts 128 producer arrivals
+        } else {
+          const float* src = sg.base + tap * sg.tap_stride + kin + q * 4;
+#pragma unroll
+          for (int i = 0; i < TC_BM / 16; ++i) {
+            const long long off = rowbase[seg * 128 + rq + 16 * i];
+            cp_async16(sb + adst + i * 16 * 128, off >= 0 ? src + off : sg.base, off >= 0 ? 16 : 0);
+          }
+          cp_async_arrive(full);
+        }
+        k0 += TC_KS;
+        kin += TC_KS;
+        if (kin == sg.Kc) { kin = 0; ++tap; }
+        if (k0 == sg.K) { kcol += sg.K; k0 = 0; tap = 0; ++seg; }
+      }
     }
     cp_async_wait_all();
     return;
@@ -522,77 +568,94 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   const int wg = ct >> 7, wq = (ct >> 5) & 3;
   const int g = lane >> 2, t = lane & 3;
   const int r0 = wg * 64 + wq * 16 + g;                                 // fragment rows r0 and r0 + 8
-  float acc[64], part0[64], part1[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-
+  int s_w = 0, smin = 0, smax = 0;                                      // F16X3: s_W and s_r's range
   if constexpr (PREC == TC_F16X3) {
-    const int s_w = *sw;
-    int smin, smax;
+    s_w = *sw;
     tc_scale_bounds(s_w, smin, smax);
-    for (int c = 0; c < nstages; ++c) {
-      const int slot = c % STAGES;
-      mbar_wait(full0 + 8 * slot, (c / STAGES) & 1);
-      const uint32_t sb = rb + slot * SLOT;
-      const float* A = reinterpret_cast<const float*>(ring + slot * SLOT + NB * BBYTES);
-      uint32_t ah[2][4], al[2][4];
-      float u0, u1;
-      tc_load_a16(A, r0, t, s_w, smin, smax, ah, al, u0, u1);   // one scale per row and stage
-      tc_partial16(part0, ah[0], al[0], sb, 0);
-      tc_partial16(part1, ah[1], al[1], sb, 1);
-      wgmma_wait<1>();
-      tc_add_scaled(acc, part0, u0, u1);
-      wgmma_wait<0>();
-      tc_add_scaled(acc, part1, u0, u1);
-      if (lane == 0) mbar_arrive(empty0 + 8 * slot);
-    }
-  } else {
-    for (int c = 0; c < nstages; ++c) {
-      const int slot = c % STAGES;
-      mbar_wait(full0 + 8 * slot, (c / STAGES) & 1);
-      const uint32_t sb = rb + slot * SLOT;
-      const float* A = reinterpret_cast<const float*>(ring + slot * SLOT + NB * TC_B_BYTES);
-      uint32_t ah[2][4], al[2][4];
-      tc_load_a<PREC>(A, r0, t, 0, ah, al);
-      tc_partial<PREC>(part0, ah, al, sb, 0);
-      tc_load_a<PREC>(A, r0, t, 2, ah, al);
-      tc_partial<PREC>(part1, ah, al, sb, 2);
-      wgmma_wait<1>();                            // the first partial has retired ...
-      tc_add(acc, part0);                         // ... and is summed while the second runs
-      wgmma_wait<0>();
-      tc_add(acc, part1);
-      if (lane == 0) mbar_arrive(empty0 + 8 * slot);
-    }
   }
-  epi_sync();                                   // both consumers are done with the ring
-  tc_tile(p, rt, ctile);
-  const int fe = rt * p.fpt, nfe = min(p.fpt, p.F - fe);
+  // The stage counter c is the only tile state carried through the K loop: the CTA's tile u is c / nstages - 1 after
+  // it, and the tile itself is read again from the grid position (tc_tile_at).
+  int c = 0;
+  for (;;) {
+    float acc[64], part0[64], part1[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    const int cend = c + nstages;
 
-  if constexpr (EPI == EPI_PLAIN) {
-    tc_store_plain(p, acc, ring, rb, am.out, r0, t, ct, fe, nfe * J, ctile * TC_BN);
-    return;
-  }
-  // hand the tile over in the FFMA thread layout the shared epilogues expect
-  float* S = reinterpret_cast<float*>(ring);   // [128][TC_STG_LD]
+    if constexpr (PREC == TC_F16X3) {
+      for (; c < cend; ++c) {
+        const int slot = c % STAGES;
+        mbar_wait(full0 + 8 * slot, (c / STAGES) & 1);
+        const uint32_t sb = rb + slot * SLOT;
+        const float* A = reinterpret_cast<const float*>(ring + slot * SLOT + NB * BBYTES);
+        uint32_t ah[2][4], al[2][4];
+        float u0, u1;
+        tc_load_a16(A, r0, t, s_w, smin, smax, ah, al, u0, u1);   // one scale per row and stage
+        tc_partial16(part0, ah[0], al[0], sb, 0);
+        tc_partial16(part1, ah[1], al[1], sb, 1);
+        wgmma_wait<1>();
+        tc_add_scaled(acc, part0, u0, u1);
+        wgmma_wait<0>();
+        tc_add_scaled(acc, part1, u0, u1);
+        if (lane == 0) mbar_arrive(empty0 + 8 * slot);
+      }
+    } else {
+      for (; c < cend; ++c) {
+        const int slot = c % STAGES;
+        mbar_wait(full0 + 8 * slot, (c / STAGES) & 1);
+        const uint32_t sb = rb + slot * SLOT;
+        const float* A = reinterpret_cast<const float*>(ring + slot * SLOT + NB * TC_B_BYTES);
+        uint32_t ah[2][4], al[2][4];
+        tc_load_a<PREC>(A, r0, t, 0, ah, al);
+        tc_partial<PREC>(part0, ah, al, sb, 0);
+        tc_load_a<PREC>(A, r0, t, 2, ah, al);
+        tc_partial<PREC>(part1, ah, al, sb, 2);
+        wgmma_wait<1>();                            // the first partial has retired ...
+        tc_add(acc, part0);                         // ... and is summed while the second runs
+        wgmma_wait<0>();
+        tc_add(acc, part1);
+        if (lane == 0) mbar_arrive(empty0 + 8 * slot);
+      }
+    }
+    int rt, ctile;
+    const int u = c / nstages - 1;
+    tc_tile_at(p, u, rt, ctile);
+    const int fe = rt * p.fpt, nfe = min(p.fpt, p.F - fe);
+
+    if constexpr (EPI == EPI_PLAIN) {
+      tc_stores_read(ct);                       // the staging buffer is free once the last tile's stores are read
+      epi_sync();
+      tc_store_plain(p, acc, ring + tc_ring(PREC), stg, am.out, r0, t, ct, fe, nfe * J, ctile * TC_BN);
+      if (!tc_tile_at(p, u + 1, rt, ctile)) {
+        tc_stores_read(ct);                     // the staging buffer stays until the engine has read it
+        return;
+      }
+    } else {
+      epi_sync();                               // both consumers are done with the ring
+      // hand the tile over in the FFMA thread layout the shared epilogues expect
+      float* S = reinterpret_cast<float*>(ring);   // [128][TC_STG_LD]
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    const int col = 8 * i + 2 * t;
-    *reinterpret_cast<float2*>(S + r0 * TC_STG_LD + col) = make_float2(acc[4 * i], acc[4 * i + 1]);
-    *reinterpret_cast<float2*>(S + (r0 + 8) * TC_STG_LD + col) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
-  }
-  epi_sync();
-  const int ty = ct >> 4, tx = ct & 15;
-  float out[8][8];
+      for (int i = 0; i < 16; ++i) {
+        const int col = 8 * i + 2 * t;
+        *reinterpret_cast<float2*>(S + r0 * TC_STG_LD + col) = make_float2(acc[4 * i], acc[4 * i + 1]);
+        *reinterpret_cast<float2*>(S + (r0 + 8) * TC_STG_LD + col) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+      }
+      epi_sync();
+      const int ty = ct >> 4, tx = ct & 15;
+      float out[8][8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int r = (i < 4) ? (ty * 4 + i) : (64 + ty * 4 + i - 4);
-    const float4 u = *reinterpret_cast<const float4*>(S + r * TC_STG_LD + tx * 4);
-    const float4 v = *reinterpret_cast<const float4*>(S + r * TC_STG_LD + 64 + tx * 4);
-    out[i][0] = u.x; out[i][1] = u.y; out[i][2] = u.z; out[i][3] = u.w;
-    out[i][4] = v.x; out[i][5] = v.y; out[i][6] = v.z; out[i][7] = v.w;
+      for (int i = 0; i < 8; ++i) {
+        const int r = (i < 4) ? (ty * 4 + i) : (64 + ty * 4 + i - 4);
+        const float4 a = *reinterpret_cast<const float4*>(S + r * TC_STG_LD + tx * 4);
+        const float4 b = *reinterpret_cast<const float4*>(S + r * TC_STG_LD + 64 + tx * 4);
+        out[i][0] = a.x; out[i][1] = a.y; out[i][2] = a.z; out[i][3] = a.w;
+        out[i][4] = b.x; out[i][5] = b.y; out[i][6] = b.z; out[i][7] = b.w;
+      }
+      epi_sync();
+      gemm_epilogue<EPI>(p, out, reinterpret_cast<float*>(ring), ct, fe, nfe, nfe * J, ctile * TC_BN, ctile);
+      return;                                   // one tile per CTA (tc_persistent)
+    }
   }
-  epi_sync();
-  gemm_epilogue<EPI>(p, out, reinterpret_cast<float*>(ring), ct, fe, nfe, nfe * J, ctile * TC_BN, ctile);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -607,8 +670,8 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
 //   gathered segments: cp.async of 16 B = one row's k-octet, zero-filled outside the tile.
 // K is chained in the accumulator: the tensor core's truncation bias (~0.5 ulp of fp32 per k16 MMA) stays far below
 // the 2^-11 rounding of the fp16 operands (K = 1536 is 96 MMAs), so the two-level partial sums of the fp32-grade forms
-// buy nothing here.  Tiles, ring protocol, producer and epilogues are gemm_tc_kernel's; the epilogues read the residual
-// and write the output as fp16 (tc_store_plain_h's TMA store of two [128][64]-half column blocks; SemCH through
+// buy nothing here.  It runs one tile per CTA; tiles, ring protocol and producer are gemm_tc_kernel's; the epilogues
+// read the residual and write the output as fp16 (tc_store_plain_h's TMA store of two [128][64]-half column blocks; SemCH through
 // gemm_epilogue<EPI_SEMCH, __half>).  There is no EPI_GLOBAL form: a half model's attention mix is its own kernel
 // (global_mix_kernel, J <= MIX_JMAX, which gast_set_activation_dtype requires).
 #ifndef GAST_TCH_STAGES
@@ -1007,9 +1070,9 @@ inline bool tc_supported(const GemmP& p, int epi, const TcWeights& t) {
     if (reinterpret_cast<uintptr_t>(sg.base) & 15) return false;
   }
   const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
-  if (tc_smem_bytes(TC_3XTF32, epi, p.J, p.fpt, hpt) > TC_SMEM_MAX) return false;
-  if (tc_smem_bytes(TC_1XTF32, epi, p.J, p.fpt, hpt) > TC_SMEM_MAX) return false;
-  if (tc_smem_bytes(TC_F16X3, epi, p.J, p.fpt, hpt) > TC_SMEM_MAX) return false;
+  if (tc_smem_bytes(TC_3XTF32, epi, p.J, p.fpt, hpt) > TC_SMEM_OPTIN) return false;
+  if (tc_smem_bytes(TC_1XTF32, epi, p.J, p.fpt, hpt) > TC_SMEM_OPTIN) return false;
+  if (tc_smem_bytes(TC_F16X3, epi, p.J, p.fpt, hpt) > TC_SMEM_OPTIN) return false;
   return true;
 }
 
@@ -1054,20 +1117,25 @@ inline int tc_launch_h(cudaStream_t st, int epi, const GemmP& p, const TcWeights
 
 template <int PREC>
 inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t) {
-  const dim3 grid((unsigned)(((p.F + p.fpt - 1) / p.fpt) * ((p.N + TC_BN - 1) / TC_BN)));
+  const int tiles = ((p.F + p.fpt - 1) / p.fpt) * ((p.N + TC_BN - 1) / TC_BN);
   const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
   const size_t smem = tc_smem_bytes(PREC, epi, p.J, p.fpt, hpt);
   static bool attr_set[64][3];              // the shared-memory opt-in is per device
+  static int sms[64];
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr_set[dev & 63][epi]) {
     const void* fn = epi == EPI_PLAIN ? (const void*)gemm_tc_kernel<EPI_PLAIN, PREC>
                    : epi == EPI_SEMCH ? (const void*)gemm_tc_kernel<EPI_SEMCH, PREC>
                                       : (const void*)gemm_tc_kernel<EPI_GLOBAL, PREC>;
-    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX);
+    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_OPTIN);
+    if (e != cudaSuccess) return (int)e;
+    e = cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev);
     if (e != cudaSuccess) return (int)e;
     attr_set[dev & 63][epi] = true;
   }
+  // the persistent form takes one CTA per SM at most, the others one per tile
+  const dim3 grid((unsigned)(tc_persistent(epi) && tiles > sms[dev & 63] ? sms[dev & 63] : tiles));
   const CUtensorMap& mhi = PREC == TC_F16X3 ? t.map_h16hi : t.map_hi;
   const CUtensorMap& mlo = PREC == TC_F16X3 ? t.map_h16lo : t.map_lo;
   // the activation maps follow the pointers, so they are encoded per launch (graph capture keeps them by value)
@@ -1083,7 +1151,7 @@ inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeig
   return (int)cudaGetLastError();
 }
 
-// One CTA per tile, tile = row tile * column tiles + column tile (the column tile fastest, see gemm_tc_kernel).
+// Tiles in the order tile = row tile * column tiles + column tile (the column tile fastest, see gemm_tc_kernel).
 // prec: TC_3XTF32 (needs t.f16 false), TC_1XTF32, TC_F16X3 or TC_F16 (both need t.f16).
 inline int tc_launch(cudaStream_t st, int epi, const GemmP& p, const TcWeights& t, int prec) {
   if (prec == TC_F16) return tc_launch_h(st, epi, p, t);
