@@ -54,23 +54,24 @@
 //     partial stays in flight across the loop's back edge: ptxas then serialises every wgmma of the kernel (C7514).
 //     The two consumers do not synchronise with each other inside the K loop, so one's MMAs fill the other's drain.
 // Tiles (fpt whole frames per 128-row tile) and the fused epilogues are the FFMA core's, so both cores are
-// interchangeable per launch.  EPI_PLAIN runs on the wgmma fragments (tc_store_plain: bias, ReLU, residual in
-// gemm_epilogue's order) and leaves by four TMA tensor stores from a 64 KB staging buffer of its own; EPI_SEMCH and
-// EPI_GLOBAL mix joints across rows, so their tiles are handed over in the FFMA thread layout to gemm_epilogue, run by
-// the 256 consumer threads, with the ring as scratch.
+// interchangeable per launch.  EPI_PLAIN and EPI_SEMCH run on the wgmma fragments, in gemm_epilogue's order, and leave
+// by TMA tensor stores from a 64 KB staging buffer of their own: tc_store_plain (bias, ReLU, residual) stores four
+// 32-column blocks; tc_store_semch stages the neighbour half of the tile in two of the blocks, mixes each row's
+// neighbours into the other two and stores those.  EPI_GLOBAL's attention mix is handed over in the FFMA thread layout
+// to gemm_epilogue, run by the 256 consumer threads, with the ring as scratch.
 //
 // Tiles are numbered on a 1D order in which the column tile is the fast index: the CTAs running together cover a row
 // tile's column tiles side by side, so its A rows come from HBM once and its other column tiles find them in L2.
 // (Every layer's A is larger than the L2; with the row tile fast, A was read from HBM once per column tile.)
-//   EPI_PLAIN is persistent (tc_persistent): min(tiles, SMs) CTAs, CTA i takes tiles i, i + grid, i + 2 grid, ...
+//   EPI_PLAIN and EPI_SEMCH are persistent (tc_persistent): min(tiles, SMs) CTAs, CTA i takes tiles i, i + grid, ...
 //     The ring's stage counter c and the mbarrier phases run on across tiles (stage c of the CTA's run uses slot
 //     c % STAGES; `full` is waited on parity (c / STAGES) & 1, `empty` before refilling on (c / STAGES - 1) & 1), and
 //     the producer rebuilds its row table (`rowbase`, under named barrier 3 over its 128 threads) at each tile, so it
 //     fills the next tile's first stages while the consumers finish the current one.  The consumers write a finished
-//     tile into the staging buffer, meet at one named barrier, and one of them issues the tensor stores; it waits for
-//     the TMA engine to have read them only before the next tile is written there (and before it exits), so the
-//     consumers go on to the next tile's K loop while the stores drain.
-//   EPI_SEMCH and EPI_GLOBAL use the ring as their epilogue's scratch, so they run one tile per CTA (grid = tiles).
+//     tile into the staging buffer, meet at a named barrier (SemCH: two), and one of them issues the tensor stores; it
+//     waits for the TMA engine to have read them only before the next tile is written there (and before it exits), so
+//     the consumers go on to the next tile's K loop while the stores drain.
+//   EPI_GLOBAL uses the ring as its epilogue's scratch, so it runs one tile per CTA (grid = tiles).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -128,17 +129,17 @@ constexpr int TC_STG_LD = 136;                       // [row][col] stride of the
 constexpr int TC_ROWBASE_BYTES = 3 * 128 * sizeof(long long);
 constexpr int TC_SMEM_MAX = 200 * 1024;              // the half form's bound
 constexpr int TC_SMEM_OPTIN = 227 * 1024;            // the SM's opt-in shared memory per block: gemm_tc_kernel's bound
-constexpr int TC_TILE_BYTES = TC_BM * TC_BN * 4;     // EPI_PLAIN's staging buffer: one fp32 tile
-// EPI_PLAIN runs a persistent tile loop; EPI_SEMCH and EPI_GLOBAL, whose epilogues take the ring as scratch, one tile
-// per CTA
-__host__ __device__ constexpr bool tc_persistent(int epi) { return epi == EPI_PLAIN; }
+constexpr int TC_TILE_BYTES = TC_BM * TC_BN * 4;     // the persistent forms' staging buffer: one fp32 tile
+// EPI_PLAIN and EPI_SEMCH run a persistent tile loop with a staging buffer of their own; EPI_GLOBAL, whose epilogue
+// takes the ring as scratch, one tile per CTA
+__host__ __device__ constexpr bool tc_persistent(int epi) { return epi == EPI_PLAIN || epi == EPI_SEMCH; }
 static_assert(tc_slot(TC_3XTF32) % 1024 == 0 && tc_slot(TC_1XTF32) % 1024 == 0 && tc_slot(TC_F16X3) % 1024 == 0 &&
               TC_B16_BYTES % 1024 == 0, "ring slots and their A stages stay 1024-byte aligned");
 static_assert(tc_ring(TC_1XTF32) + 16 * tc_stages(TC_1XTF32) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX &&
               tc_ring(TC_F16X3) + 16 * tc_stages(TC_F16X3) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX,
               "every ring fits the shared memory the core may use");
 
-// rowbase | ring (1024-byte aligned) | EPI_PLAIN: staging buffer | a full and an empty mbarrier per slot
+// rowbase | ring (1024-byte aligned) | persistent forms: staging buffer | a full and an empty mbarrier per slot
 __host__ __device__ inline size_t tc_smem_bytes(int prec, int epi, int J, int fpt, int hpt) {
   if (tc_persistent(epi))
     return TC_ROWBASE_BYTES + 1024 + (size_t)tc_ring(prec) + TC_TILE_BYTES + 16 * tc_stages(prec);
@@ -187,6 +188,10 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t sr
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(map), "r"(src), "r"(x), "r"(y) : "memory");
 }
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int x, int y, int z) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(map), "r"(src), "r"(x), "r"(y), "r"(z) : "memory");
+}
 // 16 bytes global -> shared, zero-filled when src_bytes == 0
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
@@ -207,7 +212,8 @@ __host__ __device__ inline bool tc_seg_tma(const ASeg& s) {
   return s.tap_stride == 0 && s.map.T_in == s.map.T_out && s.map.t_mul == 1 && s.map.t_off == 0;
 }
 // per A segment taken by tc_seg_tma: fp32 {Kc, F J} at row stride ld, box {32, 128}, 128-byte swizzle; out: the plain
-// epilogue's output, fp32 {N, F J} at row stride ld_out, box {32, fpt J}, 128-byte swizzle
+// epilogue's output, fp32 {N, F J} at row stride ld_out, box {32, fpt J}, or the SemCH epilogue's (tc_encode_semch),
+// 128-byte swizzle
 struct TcActMaps {
   CUtensorMap seg[3];
   CUtensorMap out;
@@ -440,6 +446,84 @@ __device__ __forceinline__ void tc_store_plain(const GemmP& p, const float (&acc
   }
 }
 
+// EPI_SEMCH on the consumers' wgmma fragments.  The tile is 64 channels of one mask: columns 0 .. 63 hold the self
+// products X.W0, columns 64 .. 127 the neighbour products H = X.W1 (gemm_epilogue).  The staging buffer (`stage`,
+// shared address sb) holds four 128-byte-swizzled [128][32] float blocks (tc_achunk): blocks 0 and 1 take H, blocks 2
+// and 3 the output O.  Every thread writes its H columns (acc[4 i ..], i >= 8), and after a barrier mixes its rows r0,
+// r0 + 8 below vrows in its channel pairs c = chan0 + 8 i + 2t, + 1 (i < 8):  v = shift, then
+// v = fmaf(coef[z][c], h_jj[c], v) over the row's neighbours z in row_ptr order, the self term from its own fragment
+// and the others from H at their row of the same frame, then ReLU.  That is gemm_epilogue's order, so the bits are the
+// same.  Consumer thread 0 then stores each 32-channel O block whose first channel is below C with `out`
+// (tc_encode_semch: channels {C, masks, F J}, which drops channels past C of each mask and rows past F J).  The buffer
+// must be free (the previous stores read) when this is called; the stores are committed as one bulk group, not waited
+// for.
+__device__ __forceinline__ void tc_store_semch(const GemmP& p, const float (&acc)[64], unsigned char* stage,
+                                               uint32_t sb, const CUtensorMap& out, int r0, int t, int ct, int ctile,
+                                               int f0, int vrows) {
+  const int J = p.J, C = p.C;
+  float* S = reinterpret_cast<float*>(stage);
+#pragma unroll
+  for (int i = 8; i < 16; ++i) {
+    const int col = 8 * i + 2 * t - 64;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(S + (col >> 5) * (TC_BM * TC_KS) + tc_achunk(r0 + 8 * h, col >> 2 & 7) + (col & 3)) =
+          make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+  }
+  epi_sync();
+  const int mask = ctile / p.tiles_per_mask;
+  const int chan0 = (ctile - mask * p.tiles_per_mask) * 64;
+  const NbrTable& nb = p.nbr[mask];
+  const float* coef = p.coef[mask] + chan0 + 2 * t;
+  float2 sh[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    sh[i] = make_float2(0.f, 0.f);
+    if (p.shift && chan0 + 8 * i + 2 * t < C)                           // C % 4 == 0: c + 1 < C too
+      sh[i] = __ldg(reinterpret_cast<const float2*>(p.shift + mask * C + chan0 + 8 * i + 2 * t));
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + 8 * h;
+    if (r >= vrows) continue;
+    const int fr = r / J, ji = r - fr * J;
+    float2 v[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v[i] = sh[i];
+    const int zend = nb.row_ptr[ji + 1];
+    for (int z = nb.row_ptr[ji]; z < zend; ++z) {
+      const int jj = nb.col[z];
+      const float* cz = coef + (long long)z * C;
+      const int hr = fr * J + jj;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int col = 8 * i + 2 * t;
+        float2 cf = make_float2(0.f, 0.f);
+        if (chan0 + col < C) cf = __ldg(reinterpret_cast<const float2*>(cz + 8 * i));
+        float2 hv;
+        if (jj == ji) hv = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+        else hv = *reinterpret_cast<const float2*>(S + (i >> 2) * (TC_BM * TC_KS) + tc_achunk(hr, col >> 2 & 7) +
+                                                   (col & 3));
+        v[i].x = fmaf(cf.x, hv.x, v[i].x);
+        v[i].y = fmaf(cf.y, hv.y, v[i].y);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int col = 8 * i + 2 * t;
+      if (p.relu) { v[i].x = fmaxf(v[i].x, 0.f); v[i].y = fmaxf(v[i].y, 0.f); }
+      *reinterpret_cast<float2*>(S + (2 + (i >> 2)) * (TC_BM * TC_KS) + tc_achunk(r, col >> 2 & 7) + (col & 3)) = v[i];
+    }
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // the writes above, seen by the TMA engine
+  epi_sync();
+  if (ct == 0) {
+    for (int cb = 0; cb < 2 && chan0 + cb * TC_KS < C; ++cb)
+      tma_store_3d(&out, sb + (2 + cb) * TC_A_BYTES, chan0 + cb * TC_KS, mask, f0 * J);
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+  }
+}
+
 // consumer thread 0: wait until the TMA engine has read every tensor store it issued from the staging buffer
 __device__ __forceinline__ void tc_stores_read(int ct) {
   if (ct == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
@@ -461,7 +545,7 @@ __device__ __forceinline__ bool tc_tile_at(const GemmP& p, int u, int& rt, int& 
 }
 
 // mlo is not read in 1xTF32, sw (s_W) only in F16X3, am.seg[s] only for the segments tc_seg_tma takes, am.out only in
-// EPI_PLAIN
+// EPI_PLAIN and EPI_SEMCH
 template <int EPI, int PREC>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensorMap mhi,
@@ -476,7 +560,7 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t rb = (raw + TC_ROWBASE_BYTES + 1023) & ~1023u;        // ring base (shared address)
   unsigned char* ring = smem_raw + (rb - raw);
-  const uint32_t stg = rb + tc_ring(PREC);                              // EPI_PLAIN: staging buffer
+  const uint32_t stg = rb + tc_ring(PREC);                              // persistent forms: staging buffer
   const uint32_t full0 = stg + STG;                                     // per ring slot: stage landed
   const uint32_t empty0 = full0 + 8 * STAGES;                           // per ring slot: both consumers done with it
 
@@ -630,9 +714,16 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
         tc_stores_read(ct);                     // the staging buffer stays until the engine has read it
         return;
       }
+    } else if constexpr (EPI == EPI_SEMCH) {
+      tc_stores_read(ct);                       // as EPI_PLAIN; tc_store_semch's first barrier follows
+      tc_store_semch(p, acc, ring + tc_ring(PREC), stg, am.out, r0, t, ct, ctile, fe, nfe * J);
+      if (!tc_tile_at(p, u + 1, rt, ctile)) {
+        tc_stores_read(ct);
+        return;
+      }
     } else {
       epi_sync();                               // both consumers are done with the ring
-      // hand the tile over in the FFMA thread layout the shared epilogues expect
+      // hand the tile over in the FFMA thread layout gemm_epilogue<EPI_GLOBAL> expects
       float* S = reinterpret_cast<float*>(ring);   // [128][TC_STG_LD]
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
@@ -969,6 +1060,22 @@ inline int tc_encode_rows(CUtensorMap* m, const float* base, int cols, long long
   return r == CUDA_SUCCESS ? 0 : -1;
 }
 
+// The SemCH epilogue's output: fp32 [rows][masks][C] at row stride ld floats (mask m's channels at column m C), as 3D
+// {C, masks, rows}, box {32, 1, box_rows}, 128-byte swizzle, so a block's channels past C of its mask are dropped
+// rather than written into the next mask's columns (C % 4 == 0 and ld % 4 == 0 keep the strides in 16-byte units)
+inline int tc_encode_semch(CUtensorMap* m, const float* base, int C, int masks, long long rows, int ld, int box_rows) {
+  tc_encode_fn enc = tc_get_encode();
+  if (!enc) return -1;
+  const cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)masks, (cuuint64_t)rows};
+  const cuuint64_t strides[2] = {(cuuint64_t)C * 4, (cuuint64_t)ld * 4};
+  const cuuint32_t box[3] = {(cuuint32_t)TC_KS, 1, (cuuint32_t)box_rows};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : -1;
+}
+
 // fp16 [rows][cols] at row stride ld halves, box {64, box_rows} (128-byte rows), 128-byte swizzle: the half form's
 // plain-epilogue output
 inline int tc_encode_rows16(CUtensorMap* m, const void* base, int cols, long long rows, int ld, int box_rows) {
@@ -1062,8 +1169,10 @@ inline int tc_prepare_weights(TcWeights& t, const float* W, int N, int K, cudaSt
 // The shapes the core takes are the same in every precision (each ring is no larger than the bound below).
 inline bool tc_supported(const GemmP& p, int epi, const TcWeights& t) {
   if (!t.ready || t.K != p.ldw || t.N < p.N || p.N % 4) return false;
-  // the plain epilogue's tensor store: the output map needs a 16-byte-aligned base and a row stride of 16-byte units
+  // the plain and SemCH epilogues' tensor stores: the output map needs a 16-byte-aligned base and strides of 16-byte
+  // units (SemCH's mask stride is C floats)
   if ((reinterpret_cast<uintptr_t>(p.out) & 15) || p.ld_out % 4) return false;
+  if (epi == EPI_SEMCH && (p.C % 4 || p.tiles_per_mask <= 0 || p.N % (TC_BN * p.tiles_per_mask))) return false;
   for (int s = 0; s < p.nseg; ++s) {
     const ASeg& sg = p.seg[s];
     if (sg.K % TC_KS || sg.Kc % TC_KS || sg.ld % 4 || sg.tap_stride % 4) return false;
@@ -1145,6 +1254,9 @@ inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeig
     if (tc_seg_tma(p.seg[s]) && tc_encode_rows(&am.seg[s], p.seg[s].base, p.seg[s].Kc, rows, p.seg[s].ld, TC_BM))
       return -1;
   if (epi == EPI_PLAIN && tc_encode_rows(&am.out, p.out, p.N, rows, p.ld_out, p.fpt * p.J)) return -1;
+  if (epi == EPI_SEMCH && tc_encode_semch(&am.out, p.out, p.C, p.N / (TC_BN * p.tiles_per_mask), rows, p.ld_out,
+                                          p.fpt * p.J))
+    return -1;
   if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw);
   else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw);
   else gemm_tc_kernel<EPI_GLOBAL, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw);
