@@ -793,7 +793,7 @@ static void gemm_audit_record(int epi, const GemmP& p, int prec, gast_gemm_audit
   for (int s = 0; s < p.nseg; ++s) {
     const ASeg& a = p.seg[s];
     d->seg[s] = gast_gemm_audit_seg{a.base, a.tap_stride, a.ld, a.K, a.Kc, a.map.T_out, a.map.T_in, a.map.t_mul, a.map.t_off};
-    if (prec >= 0 && tc_seg_tma(a)) d->tma_mask |= 1 << s;
+    if (prec >= 0 && (prec == TC_F16 ? tc_seg_tma_h(a) : tc_seg_tma(a))) d->tma_mask |= 1 << s;
   }
   d->W = p.W; d->ldw = p.ldw; d->N = p.N; d->F = p.F; d->J = p.J; d->fpt = p.fpt; d->ld_out = p.ld_out;
   d->out = p.out; d->bias = p.bias; d->relu = p.relu; d->res = p.res; d->res_ld = p.res_ld;

@@ -35,12 +35,15 @@
 //                not 16-byte rows, and one elected thread issues the boxes.
 //     A (activations): a stage is 128 dense rows of 32 floats in TMA's 128-byte swizzle (chunk c of row r at
 //                c ^ (r & 7)), which keeps the consumers' fragment loads free of bank conflicts.  A segment whose
-//                tile rows are contiguous in its source (tc_seg_tma: identity frame map, no tap offset; the 1x1 layers,
-//                SemCH, the attention GEMMs and the block concatenations) is one TMA box per stage from the same
-//                elected thread, rows past the source's end zero-filled.  Rows gathered per frame (dilated / strided
-//                taps, the streams' ring taps) arrive by cp.async (16 B per row and k-quad, zero-filled outside the
-//                tile) from all 128 producer threads into the same swizzled layout.  A stage never straddles a tap
-//                (Kc % 32 == 0), so segment, tap, column and path are chosen once per stage.
+//                frame map is affine over the launch (tc_seg_tma: source frame t_mul f + t_off, tap k tap_stride
+//                floats on; the 1x1 layers, SemCH, the attention GEMMs, the block concatenations, the strided stage
+//                convolutions and a stream's ring taps) is one 4D TMA box {32, J, 1, fpt} per stage from the same
+//                elected thread (tc_encode_taps): the tile's fpt J rows land densely from the slot's A, frames past F
+//                zero-filled, slot rows past fpt J left as they were (they belong to no stored output row).  Rows
+//                gathered per frame (the dilated schedule across clips, the streams' chunk calls) arrive by cp.async
+//                (16 B per row and k-quad, zero-filled outside the tile) from all 128 producer threads into the same
+//                swizzled layout.  A stage never straddles a tap (Kc % 32 == 0), so segment, tap, column and path are
+//                chosen once per stage.
 //     The slot's `full` mbarrier completes when the TMA bytes (expect_tx) and, in a launch with a gathered segment,
 //     every producer thread's cp.asyncs (cp.async.mbarrier.arrive.noinc) or plain arrivals have landed: 1 + 128
 //     arrivals; 1 when every segment is loaded by TMA (the other producer threads then leave at once).
@@ -56,7 +59,10 @@
 // Tiles (fpt whole frames per 128-row tile) and the fused epilogues are the FFMA core's, so both cores are
 // interchangeable per launch.  EPI_PLAIN and EPI_SEMCH run on the wgmma fragments, in gemm_epilogue's order, and leave
 // by TMA tensor stores from a 64 KB staging buffer of their own: tc_store_plain (bias, ReLU, residual) stores four
-// 32-column blocks; tc_store_semch stages the neighbour half of the tile in two of the blocks, mixes each row's
+// 32-column blocks.  An affine residual map (tc_res_tma: the stage 1x1 layers, a stream's residual slot) has the
+// tile's residual loaded into that buffer by TMA during the K loop (tc_load_res: consumer thread 0 after the tile's
+// third stage, on an mbarrier of its own), so the epilogue reads it from shared memory at the positions it then
+// overwrites instead of from HBM after the K loop; tc_store_semch stages the neighbour half of the tile in two of the blocks, mixes each row's
 // neighbours into the other two and stores those.  EPI_GLOBAL's attention mix is handed over in the FFMA thread layout
 // to gemm_epilogue, run by the 256 consumer threads, with the ring as scratch.
 //
@@ -139,10 +145,11 @@ static_assert(tc_ring(TC_1XTF32) + 16 * tc_stages(TC_1XTF32) + TC_ROWBASE_BYTES 
               tc_ring(TC_F16X3) + 16 * tc_stages(TC_F16X3) + TC_ROWBASE_BYTES + 1024 <= TC_SMEM_MAX,
               "every ring fits the shared memory the core may use");
 
-// rowbase | ring (1024-byte aligned) | persistent forms: staging buffer | a full and an empty mbarrier per slot
+// rowbase | ring (1024-byte aligned) | persistent forms: staging buffer | a full and an empty mbarrier per slot |
+// persistent forms: the residual's mbarrier
 __host__ __device__ inline size_t tc_smem_bytes(int prec, int epi, int J, int fpt, int hpt) {
   if (tc_persistent(epi))
-    return TC_ROWBASE_BYTES + 1024 + (size_t)tc_ring(prec) + TC_TILE_BYTES + 16 * tc_stages(prec);
+    return TC_ROWBASE_BYTES + 1024 + (size_t)tc_ring(prec) + TC_TILE_BYTES + 16 * tc_stages(prec) + 8;
   size_t m = (size_t)tc_ring(prec) + 16 * tc_stages(prec);
   const size_t stg = (size_t)TC_BM * TC_STG_LD * 4;
   const size_t e = ffma_smem_bytes(epi, J, fpt, hpt) - TC_ROWBASE_BYTES;
@@ -184,6 +191,12 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(x), "r"(y) : "memory");
 }
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int x, int y, int z,
+                                            int w) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
+}
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int x, int y) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(map), "r"(src), "r"(x), "r"(y) : "memory");
@@ -205,15 +218,33 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 // float offset of 16-byte chunk c of row r in a 128-byte-swizzled [rows][32] fp32 stage
 __device__ __forceinline__ int tc_achunk(int r, int c) { return r * TC_KS + ((c ^ (r & 7)) << 2); }
 
-// An A segment whose tile rows are contiguous in its source (identity frame map, one tap or taps that do not move the
-// row): output row r of the tile starting at frame f0 reads source row f0 J + r, so a stage is one TMA box of its
-// 128 rows (tc_launch_prec encodes the map).  Other segments are gathered per row by cp.async.
+// An A segment whose frame map is affine over the whole launch: T_in == t_mul T_out, so map_frame(f) = t_mul f + t_off
+// across clip boundaries, and tap k of output frame f, joint j, reads source row (t_mul f + t_off) J + j plus k
+// tap_stride floats.  Its stages are TMA boxes of a 4D map (tc_encode_taps): identity segments (the 1x1 layers, SemCH,
+// the attention GEMMs, the block concatenations), the strided stage convolutions and the taps of a stream's ring.
+// Other segments (the dilated schedule across clips, the streams' chunk calls) are gathered per row by cp.async.
+// tc_supported has already required Kc % 32 == 0 and tap strides of 16-byte multiples.
+__host__ __device__ inline bool tc_map_affine(const RowMap& m) {
+  return m.t_mul >= 1 && m.t_off >= 0 && m.T_in == m.t_mul * m.T_out;
+}
 __host__ __device__ inline bool tc_seg_tma(const ASeg& s) {
+  return tc_map_affine(s.map) && (s.K == s.Kc || s.tap_stride > 0);
+}
+// The plain epilogue's residual by TMA (EPI_PLAIN): an affine residual map over a 16-byte-aligned residual with rows of
+// 16-byte multiples.  Each tile's residual columns are then loaded into the staging buffer during the K loop
+// (tc_load_res) instead of being read by __ldg after it.
+__host__ __device__ inline bool tc_res_tma(const GemmP& p) {
+  return p.res && tc_map_affine(p.res_map) && !(reinterpret_cast<uintptr_t>(p.res) & 15) && p.res_ld % 4 == 0;
+}
+// The half form's TMA segments: tile rows contiguous in the source (identity frame map, one tap), output row r of the
+// tile starting at frame f0 at source row f0 J + r (tc_encode_a16)
+__host__ __device__ inline bool tc_seg_tma_h(const ASeg& s) {
   return s.tap_stride == 0 && s.map.T_in == s.map.T_out && s.map.t_mul == 1 && s.map.t_off == 0;
 }
-// per A segment taken by tc_seg_tma: fp32 {Kc, F J} at row stride ld, box {32, 128}, 128-byte swizzle; out: the plain
-// epilogue's output, fp32 {N, F J} at row stride ld_out, box {32, fpt J}, or the SemCH epilogue's (tc_encode_semch),
-// 128-byte swizzle
+// per A segment taken by tc_seg_tma: tc_encode_taps (tc_encode_a16 in the half form); out: the plain epilogue's
+// output, fp32 {N, F J} at row stride ld_out, box {32, fpt J}, or the SemCH epilogue's (tc_encode_semch), 128-byte
+// swizzle.  (gemm_tc_kernel's plain epilogue takes the residual's map, when tc_res_tma takes it, as a parameter of
+// its own: tc_encode_taps of {N columns, one tap, res_map}.)
 struct TcActMaps {
   CUtensorMap seg[3];
   CUtensorMap out;
@@ -401,17 +432,18 @@ __device__ __forceinline__ void tc_tile(const GemmP& p, int& rt, int& ctile) {
 // residual in gemm_epilogue's order, so the bits are the same, then the tile goes through the staging buffer (`stage`,
 // shared address sb) to TMA as four 128-byte-swizzled column blocks of 32 floats ([128][32] each, 16 KB apart), and
 // consumer thread 0 stores them with `out` (tile rows f0 J .. f0 J + fpt J - 1 of the box; the map's dims drop rows
-// past F J and columns past N).  The buffer must be free (the previous stores read) when this is called; the stores
-// are committed as one bulk group, not waited for.
+// past F J and columns past N).  res_stg: the residual is already in the buffer (tc_load_res, landed), each value at
+// the position its output takes, and is read from there; otherwise it is read by __ldg.  The buffer must otherwise be
+// free (the previous stores read) when this is called; the stores are committed as one bulk group, not waited for.
 __device__ __forceinline__ void tc_store_plain(const GemmP& p, const float (&acc)[64], unsigned char* stage,
                                                uint32_t sb, const CUtensorMap& out, int r0, int t, int ct, int f0,
-                                               int vrows, int n0) {
+                                               int vrows, int n0, bool res_stg) {
   const int J = p.J;
   const float* resrow[2] = {nullptr, nullptr};
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = r0 + 8 * h;
-    if (p.res && r < vrows) {
+    if (p.res && !res_stg && r < vrows) {
       const int fr = r / J, j = r - fr * J;
       resrow[h] = p.res + (map_frame(p.res_map, f0 + fr) * J + j) * (long long)p.res_ld;
     }
@@ -428,13 +460,16 @@ __device__ __forceinline__ void tc_store_plain(const GemmP& p, const float (&acc
       float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
       if (p.bias) { v0 += b.x; v1 += b.y; }
       if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      const int r = r0 + 8 * h;
+      float2* o = reinterpret_cast<float2*>(S + (i >> 2) * (TC_BM * TC_KS) + tc_achunk(r, col >> 2 & 7) + (col & 3));
       if (resrow[h] && in) {
         const float2 rr = __ldg(reinterpret_cast<const float2*>(resrow[h] + n));
         v0 += rr.x; v1 += rr.y;
+      } else if (res_stg) {                                             // the residual tc_load_res staged here
+        const float2 rr = *o;
+        v0 += rr.x; v1 += rr.y;
       }
-      const int r = r0 + 8 * h;
-      *reinterpret_cast<float2*>(S + (i >> 2) * (TC_BM * TC_KS) + tc_achunk(r, col >> 2 & 7) + (col & 3)) =
-          make_float2(v0, v1);
+      *o = make_float2(v0, v1);
     }
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // the writes above, seen by the TMA engine
@@ -544,17 +579,35 @@ __device__ __forceinline__ bool tc_tile_at(const GemmP& p, int u, int& rt, int& 
   return true;
 }
 
+// Consumer thread 0, in the K loop of the CTA's tile u: once the TMA engine has read the previous tile's stores from
+// the staging buffer (at `stg`), load the tile's residual rows into it, one box of `map` per 32-column block below N,
+// on the mbarrier `bar` (completed once per tile; tc_store_plain waits on parity u & 1).  Each block lands in the
+// swizzled [128][32] layout tc_store_plain writes the output in, so every consumer thread finds its residual values
+// at the positions it then overwrites.
+__device__ __forceinline__ void tc_load_res(const GemmP& p, const CUtensorMap& map, uint32_t stg, uint32_t bar, int u) {
+  int rt, ctile;
+  tc_tile_at(p, u, rt, ctile);
+  const int n0 = ctile * TC_BN, f0 = rt * p.fpt;
+  const int nb = min(TC_BN / TC_KS, (p.N - n0 + TC_KS - 1) / TC_KS);
+  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+  mbar_arrive_expect_tx(bar, nb * TC_KS * 4 * p.J * p.fpt);
+  for (int cb = 0; cb < nb; ++cb) tma_load_4d(stg + cb * TC_A_BYTES, &map, bar, n0 + cb * TC_KS, 0, 0, f0);
+}
+
 // mlo is not read in 1xTF32, sw (s_W) only in F16X3, am.seg[s] only for the segments tc_seg_tma takes, am.out only in
-// EPI_PLAIN and EPI_SEMCH
+// EPI_PLAIN and EPI_SEMCH, mres only in EPI_PLAIN when tc_res_tma takes the residual
 template <int EPI, int PREC>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensorMap mhi,
                const __grid_constant__ CUtensorMap mlo, const __grid_constant__ TcActMaps am,
-               const int* __restrict__ sw) {
+               const int* __restrict__ sw, const __grid_constant__ CUtensorMap mres) {
   constexpr int STAGES = tc_stages(PREC), SLOT = tc_slot(PREC), NB = tc_nb(PREC);
   constexpr int BBYTES = tc_bbytes(PREC);
   constexpr int KSH = PREC == TC_F16X3 ? 3 : 2;                         // log2 of the k's per 16-byte row of a B copy
   constexpr int STG = tc_persistent(EPI) ? TC_TILE_BYTES : 0;
+  // the plain epilogue's residual by TMA (tc_load_res), in the inference forms; 3xTF32 (training and the gradients)
+  // keeps its K loop as it was and reads the residual by __ldg
+  constexpr bool RES_TMA = EPI == EPI_PLAIN && PREC != TC_3XTF32;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   long long* rowbase = reinterpret_cast<long long*>(smem_raw);          // [3][128]
   const uint32_t raw = smem_u32(smem_raw);
@@ -563,18 +616,21 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
   const uint32_t stg = rb + tc_ring(PREC);                              // persistent forms: staging buffer
   const uint32_t full0 = stg + STG;                                     // per ring slot: stage landed
   const uint32_t empty0 = full0 + 8 * STAGES;                           // per ring slot: both consumers done with it
+  const uint32_t resbar = empty0 + 8 * STAGES;                          // EPI_PLAIN: the tile's residual landed
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int J = p.J;
   int tma_segs = 0;                                                     // bit s: segment s is loaded by TMA
   for (int s = 0; s < p.nseg; ++s) tma_segs |= tc_seg_tma(p.seg[s]) << s;
   const bool gather = tma_segs != (1 << p.nseg) - 1;                    // some segment is gathered per row
+  const uint32_t abytes = TC_KS * 4 * J * p.fpt;                        // a TMA segment's stage: the tile's fpt J rows
 
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full0 + 8 * s, gather ? 1 + 128 : 1);
       mbar_init(empty0 + 8 * s, 8);
     }
+    if (RES_TMA) mbar_init(resbar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
@@ -610,7 +666,6 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
         }
         asm volatile("bar.sync 3, 128;" ::: "memory");
       }
-      const int row0 = f0 * J;                                          // source row of tile row 0 (TMA segments)
       int seg = 0, k0 = 0, kcol = 0, tap = 0, kin = 0;                  // stage start: segment, K in it, W column, tap
       for (int k = 0; k < nstages; ++k, ++c) {
         const int slot = c % STAGES;
@@ -618,11 +673,11 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
         const uint32_t sb = rb + slot * SLOT, full = full0 + 8 * slot;
         const bool tma_a = (tma_segs >> seg) & 1;
         if (tid == 0) {
-          mbar_arrive_expect_tx(full, NB * BBYTES + (tma_a ? TC_A_BYTES : 0));
+          mbar_arrive_expect_tx(full, NB * BBYTES + (tma_a ? abytes : 0));
           const int kq = (kcol + k0) >> KSH;
           tma_load_2d(sb, &mhi, full, 2 * n0, kq);
           if (NB == 2) tma_load_2d(sb + BBYTES, &mlo, full, 2 * n0, kq);
-          if (tma_a) tma_load_2d(sb + NB * BBYTES, &am.seg[seg], full, kin, row0);
+          if (tma_a) tma_load_4d(sb + NB * BBYTES, &am.seg[seg], full, kin, 0, tap, f0);
         }
         const ASeg& sg = p.seg[seg];
         if (tma_a) {
@@ -665,6 +720,8 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     const int cend = c + nstages;
+    // EPI_PLAIN with tc_res_tma: consumer thread 0 loads the tile's residual after the tile's third stage (its last,
+    // if it has fewer), when the last tile's stores have long been read and most of the K loop is left to hide it
 
     if constexpr (PREC == TC_F16X3) {
       for (; c < cend; ++c) {
@@ -682,6 +739,8 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
         wgmma_wait<0>();
         tc_add_scaled(acc, part1, u0, u1);
         if (lane == 0) mbar_arrive(empty0 + 8 * slot);
+        if (RES_TMA && ct == 0 && c + nstages - cend == min(2, nstages - 1) && tc_res_tma(p))
+          tc_load_res(p, mres, stg, resbar, c / nstages);
       }
     } else {
       for (; c < cend; ++c) {
@@ -699,6 +758,8 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
         wgmma_wait<0>();
         tc_add(acc, part1);
         if (lane == 0) mbar_arrive(empty0 + 8 * slot);
+        if (RES_TMA && ct == 0 && c + nstages - cend == min(2, nstages - 1) && tc_res_tma(p))
+          tc_load_res(p, mres, stg, resbar, c / nstages);
       }
     }
     int rt, ctile;
@@ -709,7 +770,9 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
     if constexpr (EPI == EPI_PLAIN) {
       tc_stores_read(ct);                       // the staging buffer is free once the last tile's stores are read
       epi_sync();
-      tc_store_plain(p, acc, ring + tc_ring(PREC), stg, am.out, r0, t, ct, fe, nfe * J, ctile * TC_BN);
+      const bool res_stg = RES_TMA && tc_res_tma(p);
+      if (res_stg) mbar_wait(resbar, u & 1);   // the tile's residual, loaded into the buffer by tc_load_res
+      tc_store_plain(p, acc, ring + tc_ring(PREC), stg, am.out, r0, t, ct, fe, nfe * J, ctile * TC_BN, res_stg);
       if (!tc_tile_at(p, u + 1, rt, ctile)) {
         tc_stores_read(ct);                     // the staging buffer stays until the engine has read it
         return;
@@ -756,7 +819,7 @@ gemm_tc_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtensor
 // read by wgmma from shared memory through descriptors (m64n128k16, SS form), in one layout: the no-swizzle K-major
 // core-matrix layout of the B copies, [K/8][rows][8] halves (8 rows x 16 B core matrices, 128 B apart along the rows,
 // 2048 B apart along K), so tc_bdesc describes A as well.  A stage is 128 rows x 32 K = 8 KB:
-//   identity segments (tc_seg_tma): one 3D TMA box {8 halves, 128 rows, 4 k-octets} of a map with dims
+//   identity segments (tc_seg_tma_h): one 3D TMA box {8 halves, 128 rows, 4 k-octets} of a map with dims
 //     {8, rows, Kc / 8} and strides {ld, 8} halves (tc_encode_a16), which lands in exactly that layout;
 //   gathered segments: cp.async of 16 B = one row's k-octet, zero-filled outside the tile.
 // K is chained in the accumulator: the tensor core's truncation bias (~0.5 ulp of fp32 per k16 MMA) stays far below
@@ -845,7 +908,7 @@ __device__ __forceinline__ void tc_store_plain_h(const GemmP& p, const float (&a
 }
 
 // The half form of gemm_tc_kernel: p's segment bases, out and res point to __half; lds, tap strides and residual
-// strides count halves.  mb: the F16X3 hi copy's map; am.seg[s] (tc_encode_a16) for the segments tc_seg_tma takes,
+// strides count halves.  mb: the F16X3 hi copy's map; am.seg[s] (tc_encode_a16) for the segments tc_seg_tma_h takes,
 // am.out (fp16, tc_encode_rows16) in EPI_PLAIN.
 template <int EPI>   // EPI_PLAIN or EPI_SEMCH
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -869,7 +932,7 @@ gemm_tc_h_kernel(const __grid_constant__ GemmP p, const __grid_constant__ CUtens
   const int vrows = nf * J;
   const int n0 = ctile * TC_BN;
   int tma_segs = 0;
-  for (int s = 0; s < p.nseg; ++s) tma_segs |= tc_seg_tma(p.seg[s]) << s;
+  for (int s = 0; s < p.nseg; ++s) tma_segs |= tc_seg_tma_h(p.seg[s]) << s;
   const bool gather = tma_segs != (1 << p.nseg) - 1;
 
   if (tid == 0) {
@@ -1060,6 +1123,28 @@ inline int tc_encode_rows(CUtensorMap* m, const float* base, int cols, long long
   return r == CUDA_SUCCESS ? 0 : -1;
 }
 
+// An A segment taken by tc_seg_tma as the stages of F output frames of J joints read it: fp32 dims {Kc, J, taps, F}
+// with byte strides {ld, tap_stride, t_mul J ld} x 4 from base + t_off J ld, box {32, J, 1, fpt}, 128-byte swizzle.
+// The box at (kin, 0, tap, f0) is the tile's fpt J rows of one stage, dense from the slot's 1024-byte-aligned A in the
+// swizzle tc_achunk reads (chunk c of slot row r at c ^ (r & 7)); frames past F read as zeros, and slot rows past fpt J,
+// which belong to no stored output row, keep what they held.  One tap: the tap stride is never used, and is given as
+// a frame's J ld so that the strides stay nested.
+inline int tc_encode_taps(CUtensorMap* m, const ASeg& s, int F, int J, int fpt) {
+  tc_encode_fn enc = tc_get_encode();
+  if (!enc) return -1;
+  const int taps = s.K / s.Kc;
+  const cuuint64_t row = (cuuint64_t)s.ld * 4, frame = (cuuint64_t)J * row;
+  const cuuint64_t dims[4] = {(cuuint64_t)s.Kc, (cuuint64_t)J, (cuuint64_t)taps, (cuuint64_t)F};
+  const cuuint64_t strides[3] = {row, taps > 1 ? (cuuint64_t)s.tap_stride * 4 : frame, (cuuint64_t)s.map.t_mul * frame};
+  const cuuint32_t box[4] = {(cuuint32_t)TC_KS, (cuuint32_t)J, 1, (cuuint32_t)fpt};
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  const float* base = s.base + (long long)s.map.t_off * J * s.ld;
+  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : -1;
+}
+
 // The SemCH epilogue's output: fp32 [rows][masks][C] at row stride ld floats (mask m's channels at column m C), as 3D
 // {C, masks, rows}, box {32, 1, box_rows}, 128-byte swizzle, so a block's channels past C of its mask are dropped
 // rather than written into the next mask's columns (C % 4 == 0 and ld % 4 == 0 keep the strides in 16-byte units)
@@ -1217,7 +1302,7 @@ inline int tc_launch_h(cudaStream_t st, int epi, const GemmP& p, const TcWeights
   TcActMaps am{};
   const long long rows = (long long)p.F * p.J;
   for (int s = 0; s < p.nseg; ++s)
-    if (tc_seg_tma(p.seg[s]) && tc_encode_a16(&am.seg[s], p.seg[s].base, p.seg[s].Kc, rows, p.seg[s].ld)) return -1;
+    if (tc_seg_tma_h(p.seg[s]) && tc_encode_a16(&am.seg[s], p.seg[s].base, p.seg[s].Kc, rows, p.seg[s].ld)) return -1;
   if (epi == EPI_PLAIN && tc_encode_rows16(&am.out, p.out, p.N, rows, p.ld_out, p.fpt * p.J)) return -1;
   if (epi == EPI_PLAIN) gemm_tc_h_kernel<EPI_PLAIN><<<grid, TC_THREADS, smem, st>>>(p, t.map_h16hi, am, t.sw);
   else gemm_tc_h_kernel<EPI_SEMCH><<<grid, TC_THREADS, smem, st>>>(p, t.map_h16hi, am, t.sw);
@@ -1251,15 +1336,20 @@ inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeig
   TcActMaps am{};
   const long long rows = (long long)p.F * p.J;
   for (int s = 0; s < p.nseg; ++s)
-    if (tc_seg_tma(p.seg[s]) && tc_encode_rows(&am.seg[s], p.seg[s].base, p.seg[s].Kc, rows, p.seg[s].ld, TC_BM))
-      return -1;
+    if (tc_seg_tma(p.seg[s]) && tc_encode_taps(&am.seg[s], p.seg[s], p.F, p.J, p.fpt)) return -1;
   if (epi == EPI_PLAIN && tc_encode_rows(&am.out, p.out, p.N, rows, p.ld_out, p.fpt * p.J)) return -1;
+  CUtensorMap mres{};
+  if (epi == EPI_PLAIN && tc_res_tma(p)) {
+    ASeg r;                                  // the residual as a one-tap segment of N columns at its frame map
+    r.base = p.res; r.ld = p.res_ld; r.K = r.Kc = p.N; r.tap_stride = 0; r.map = p.res_map;
+    if (tc_encode_taps(&mres, r, p.F, p.J, p.fpt)) return -1;
+  }
   if (epi == EPI_SEMCH && tc_encode_semch(&am.out, p.out, p.C, p.N / (TC_BN * p.tiles_per_mask), rows, p.ld_out,
                                           p.fpt * p.J))
     return -1;
-  if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw);
-  else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw);
-  else gemm_tc_kernel<EPI_GLOBAL, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw);
+  if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw, mres);
+  else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw, mres);
+  else gemm_tc_kernel<EPI_GLOBAL, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw, mres);
   return (int)cudaGetLastError();
 }
 
