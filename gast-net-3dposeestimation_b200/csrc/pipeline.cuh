@@ -450,15 +450,17 @@ __device__ inline void jacobi_eig3(double a[3][3], double v[3][3]) {   // a symm
   }
 }
 
-__global__ void p_mpjpe_kernel(const float* __restrict__ pred, const float* __restrict__ tgt, float* __restrict__ err,
-                               int N, int J) {
-  const int frame = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
-  const int lane = threadIdx.x & 31;
-  if (frame >= N) return;
+// One frame per warp, lane j < J on joint j: returns on every lane the sum over the joints of the distance after the
+// alignment of the prediction to the target.  zero_root reads target joint 0 as 0.
+__device__ __forceinline__ double procrustes_dist_sum(const float* __restrict__ pred, const float* __restrict__ tgt,
+                                                      long long frame, int J, int lane, bool zero_root) {
   const bool on = lane < J;
   double X[3] = {0, 0, 0}, Y[3] = {0, 0, 0};
   if (on)
-    for (int c = 0; c < 3; ++c) { X[c] = tgt[((long long)frame * J + lane) * 3 + c]; Y[c] = pred[((long long)frame * J + lane) * 3 + c]; }
+    for (int c = 0; c < 3; ++c) {
+      X[c] = (zero_root && lane == 0) ? 0.0 : tgt[(frame * J + lane) * 3 + c];
+      Y[c] = pred[(frame * J + lane) * 3 + c];
+    }
   double muX[3], muY[3];
   for (int c = 0; c < 3; ++c) { muX[c] = warp_sum_d(X[c]) / J; muY[c] = warp_sum_d(Y[c]) / J; }
   double X0[3], Y0[3], nx = 0, ny = 0;
@@ -536,8 +538,80 @@ __global__ void p_mpjpe_kernel(const float* __restrict__ pred, const float* __re
     }
     e = sqrt(d2);
   }
-  e = warp_sum_d(e);
+  return warp_sum_d(e);
+}
+
+__global__ void p_mpjpe_kernel(const float* __restrict__ pred, const float* __restrict__ tgt, float* __restrict__ err,
+                               int N, int J) {
+  const int frame = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
+  if (frame >= N) return;
+  const double e = procrustes_dist_sum(pred, tgt, frame, J, lane, false);
   if (lane == 0) err[frame] = (float)(e / J);
+}
+
+// ------------------------------------------------------------------------------------------
+// Scoring a test set (main.py:299-353 evaluate, common/loss.py:56-90 euclidean_losses / pck / auc): per segment of
+// frames one row of doubles  [frames, sum_f mpjpe_f, sum_f p_mpjpe_f, sum_f dist_fj (J), count(dist < thr_k) (n_thr)].
+// A segment is cut into slices of METRIC_SLICE frames at fixed offsets from its first frame.  One CTA reduces a slice
+// (warp w takes frames w, w + METRIC_WARPS, ...; fp64 sums in that order, warps added in order); one CTA per segment
+// then adds its slices in order.  A row depends on its own segment's frames only, and no float atomics are used.
+// dist = sqrt((dx*dx + dy*dy) + dz*dz) rounded at every step, the order of torch's CPU diff.pow(2).sum(-1).sqrt().
+// ------------------------------------------------------------------------------------------
+constexpr int METRIC_SLICE = 64, METRIC_WARPS = 8, METRIC_MAX_THR = 64;
+
+__global__ void __launch_bounds__(METRIC_WARPS * 32)
+pose_metrics_slice_kernel(const float* __restrict__ pred, const float* __restrict__ tgt,
+                          const long long* __restrict__ slices, const float* __restrict__ thr, int n_thr, int J,
+                          int zero_root, int procrustes, float* __restrict__ dist_out, double* __restrict__ part) {
+  __shared__ double sh[METRIC_WARPS][3 + 32 + METRIC_MAX_THR];
+  __shared__ float sthr[METRIC_MAX_THR];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = 3 + J + n_thr;
+  for (int k = threadIdx.x; k < n_thr; k += blockDim.x) sthr[k] = thr[k];
+  __syncthreads();
+  const long long f0 = slices[2 * blockIdx.x], nf = slices[2 * blockIdx.x + 1];
+  const bool on = lane < J;
+  double s_mpjpe = 0.0, s_pm = 0.0, s_joint = 0.0;
+  int cnt[METRIC_MAX_THR / 32] = {0, 0};                  // lane holds the counts of thresholds lane, lane + 32
+  for (long long i = warp; i < nf; i += METRIC_WARPS) {
+    const long long f = f0 + i;
+    float d = 0.f;
+    if (on) {
+      const long long o = (f * J + lane) * 3;
+      float p[3], t[3];
+      for (int c = 0; c < 3; ++c) { p[c] = pred[o + c]; t[c] = (zero_root && lane == 0) ? 0.f : tgt[o + c]; }
+      const float dx = __fsub_rn(p[0], t[0]), dy = __fsub_rn(p[1], t[1]), dz = __fsub_rn(p[2], t[2]);
+      d = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+      if (dist_out) dist_out[f * J + lane] = d;
+    }
+    s_joint += d;
+    s_mpjpe += warp_sum_d(d) / J;
+    if (procrustes) s_pm += (double)(float)(procrustes_dist_sum(pred, tgt, f, J, lane, zero_root) / J);   // gast_p_mpjpe's value
+    for (int k = 0; k < n_thr; ++k) {
+      const unsigned b = __ballot_sync(0xffffffffu, on && d < sthr[k]);
+      if (lane == (k & 31)) cnt[k >> 5] += __popc(b);
+    }
+  }
+  if (lane == 0) { sh[warp][1] = s_mpjpe; sh[warp][2] = s_pm; }
+  if (on) sh[warp][3 + lane] = s_joint;
+  for (int k = lane; k < n_thr; k += 32) sh[warp][3 + J + k] = (double)cnt[k >> 5];
+  __syncthreads();
+  for (int c = threadIdx.x; c < W; c += blockDim.x) {
+    double v = 0.0;
+    if (c == 0) v = (double)nf;
+    else for (int w = 0; w < METRIC_WARPS; ++w) v += sh[w][c];
+    part[(long long)blockIdx.x * W + c] = v;
+  }
+}
+
+__global__ void pose_metrics_sum_kernel(const double* __restrict__ part, const long long* __restrict__ segs, int W,
+                                        double* __restrict__ rows) {
+  const long long s0 = segs[2 * blockIdx.x], ns = segs[2 * blockIdx.x + 1];
+  for (int c = threadIdx.x; c < W; c += blockDim.x) {
+    double v = 0.0;
+    for (long long k = 0; k < ns; ++k) v += part[(s0 + k) * W + c];
+    rows[(long long)blockIdx.x * W + c] = v;
+  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -760,6 +834,70 @@ extern "C" int gast_revise_skes_real_time(const float* pred, const float* kpts, 
   float* part = reinterpret_cast<float*>(workspace);
   revise_rt_kernel<<<nb, PREP_BLOCK, 0, st>>>(pred, kpts, out, M, D, cx, cy, r, part);
   zmin_subtract_kernel<<<nb, PREP_BLOCK, 0, st>>>(out, (long long)M * 17, part, nb);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" size_t gast_pose_metrics_workspace_bytes(int32_t S, int32_t J, int32_t n_thr, int64_t N) {
+  if (S <= 0 || J < 1 || J > 32 || n_thr < 0 || n_thr > METRIC_MAX_THR || N < 0) {
+    fail("gast_pose_metrics_workspace_bytes: bad arguments (S = %d >= 1, 1 <= J = %d <= 32, 0 <= n_thr = %d <= %d, N = %lld >= 0)",
+         S, J, n_thr, METRIC_MAX_THR, (long long)N);
+    return 0;
+  }
+  // sum_s ceil(T_s / METRIC_SLICE) <= S + N / METRIC_SLICE slices
+  const size_t slices = (size_t)S + (size_t)(N / METRIC_SLICE);
+  return align256(sizeof(int64_t) * 2 * (slices + S) + sizeof(float) * n_thr) + sizeof(double) * slices * (3 + J + n_thr);
+}
+
+extern "C" int gast_pose_metrics(const float* pred, const float* target, int64_t N, int32_t J, const int64_t* seg_start,
+                                 int32_t S, const float* thresholds, int32_t n_thr, int32_t zero_root, int32_t procrustes,
+                                 double* rows, float* dist, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!seg_start || !rows || !workspace || S <= 0 || N < 0 || (N > 0 && (!pred || !target)) || J < 1 || J > 32)
+    return fail("gast_pose_metrics: bad arguments (1 <= J <= 32, S >= 1)");
+  if (procrustes && J < 3) return fail("gast_pose_metrics: Procrustes alignment needs J >= 3, got %d", J);
+  if (n_thr < 0 || n_thr > METRIC_MAX_THR || (n_thr > 0 && !thresholds))
+    return fail("gast_pose_metrics: %d thresholds (at most %d)", n_thr, METRIC_MAX_THR);
+  for (int k = 0; k < n_thr; ++k)
+    if (thresholds[k] != thresholds[k]) return fail("gast_pose_metrics: threshold %d is NaN", k);
+  if (seg_start[0] != 0 || seg_start[S] != N)
+    return fail("gast_pose_metrics: segment offsets must run from 0 to N = %lld, got %lld .. %lld", (long long)N,
+                (long long)seg_start[0], (long long)seg_start[S]);
+  long long nsl = 0;
+  for (int s = 0; s < S; ++s) {
+    if (seg_start[s + 1] < seg_start[s])
+      return fail("gast_pose_metrics: segment offsets not sorted at %d (%lld > %lld)", s, (long long)seg_start[s],
+                  (long long)seg_start[s + 1]);
+    nsl += cdiv(seg_start[s + 1] - seg_start[s], METRIC_SLICE);
+  }
+  const size_t need = gast_pose_metrics_workspace_bytes(S, J, n_thr, N);
+  if (workspace_bytes < need) return fail("gast_pose_metrics: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+  // one upload: the slices' (first frame, frames), the segments' (first slice, slices), the thresholds
+  std::vector<long long> tab(2 * (nsl + S));
+  long long z = 0;
+  for (int s = 0; s < S; ++s) {
+    tab[2 * (nsl + s)] = z;
+    for (long long f = seg_start[s]; f < seg_start[s + 1]; f += METRIC_SLICE, ++z) {
+      tab[2 * z] = f;
+      tab[2 * z + 1] = std::min<long long>(METRIC_SLICE, seg_start[s + 1] - f);
+    }
+    tab[2 * (nsl + s) + 1] = z - tab[2 * (nsl + s)];
+  }
+  const size_t tab_bytes = sizeof(long long) * tab.size();
+  std::vector<char> host(tab_bytes + sizeof(float) * n_thr);
+  memcpy(host.data(), tab.data(), tab_bytes);
+  if (n_thr > 0) memcpy(host.data() + tab_bytes, thresholds, sizeof(float) * n_thr);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  char* ws = reinterpret_cast<char*>(workspace);
+  const long long* dslices = reinterpret_cast<const long long*>(ws);
+  const float* dthr = reinterpret_cast<const float*>(ws + tab_bytes);
+  const size_t slices_max = (size_t)S + (size_t)(N / METRIC_SLICE);
+  double* part = reinterpret_cast<double*>(ws + align256(sizeof(int64_t) * 2 * (slices_max + S) + sizeof(float) * n_thr));
+  CUDA_OK(cudaMemcpyAsync(ws, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+  const int W = 3 + J + n_thr;
+  if (nsl > 0)
+    pose_metrics_slice_kernel<<<(unsigned)nsl, METRIC_WARPS * 32, 0, st>>>(pred, target, dslices, dthr, n_thr, J,
+                                                                          zero_root ? 1 : 0, procrustes ? 1 : 0, dist, part);
+  pose_metrics_sum_kernel<<<S, 128, 0, st>>>(part, dslices + 2 * nsl, W, rows);
   CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -33,7 +33,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_stream_import', 'gast_chunk_gather', 'gast_keypoints_convert', 'gast_h36m_coco_format', 'gast_revise_kpts',
            'gast_revise_skes_workspace_bytes', 'gast_revise_skes', 'gast_revise_skes_real_time_workspace_bytes',
            'gast_revise_skes_real_time', 'gast_normalize_screen', 'gast_camera_to_world',
-           'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_adam_chunk', 'gast_adam_step',
+           'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_pose_metrics_workspace_bytes',
+           'gast_pose_metrics', 'gast_adam_chunk', 'gast_adam_step',
            'gast_last_error', 'gast_version']
 
 
@@ -246,6 +247,11 @@ def load():
     lib.gast_mpjpe.restype = C.c_int
     lib.gast_p_mpjpe.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, vp]
     lib.gast_p_mpjpe.restype = C.c_int
+    lib.gast_pose_metrics_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int64]
+    lib.gast_pose_metrics_workspace_bytes.restype = C.c_size_t
+    lib.gast_pose_metrics.argtypes = [vp, vp, C.c_int64, C.c_int32, C.POINTER(C.c_int64), C.c_int32, fp, C.c_int32,
+                                      C.c_int32, C.c_int32, vp, vp, vp, C.c_size_t, vp]
+    lib.gast_pose_metrics.restype = C.c_int
     lib.gast_adam_chunk.argtypes = []
     lib.gast_adam_chunk.restype = C.c_int32
     lib.gast_adam_step.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,

@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .engine import GastError, _check, _cuda_f32, _ilist, _p, _stream
+from .engine import GastError, _check, _check_size, _cuda_f32, _ilist, _p, _stream
 
 KPT_COCO_H36M, KPT_MPII_H36M, KPT_COCO_H36M_TOE = 0, 1, 2
 
@@ -256,6 +256,35 @@ def p_mpjpe_per_frame(predicted, target):
     with torch.cuda.device(p.device):
         _check(L.load().gast_p_mpjpe(_p(p), _p(t), N, J, _p(out), C.c_void_p(_stream(p.device))), 'gast_p_mpjpe')
     return out
+
+
+def pose_metrics(predicted, target, seg_start, thresholds=(), zero_root=False, procrustes=True, distances=False):
+    """Score rows per segment (gast_pose_metrics; main.py:299-353, common/loss.py:56-90).  predicted, target (N,J,3)
+    CUDA float32; seg_start the S+1 host frame offsets of the segments, 0 .. N; thresholds host floats (compared in
+    float32, as torch compares a float32 tensor with a Python float).  Returns the (S, 3+J+n_thr) float64 CUDA tensor
+    [frames, sum_f mpjpe_f, sum_f p_mpjpe_f (0 without procrustes), sum_f dist_fj (J), count(dist < thr_k) (n_thr)],
+    and with distances=True also the (N,J) float32 joint distances.  zero_root reads target joint 0 as 0 without
+    writing the target.  Every argument is checked before the first launch."""
+    p = _cuda_f32(predicted, 'pose_metrics')
+    t = _cuda_f32(target, 'pose_metrics')
+    if p.shape != t.shape or p.dim() != 3 or p.shape[-1] != 3 or p.device != t.device:
+        raise GastError('pose_metrics: predicted and target (N,J,3) on one device expected, got %s and %s'
+                        % (tuple(p.shape), tuple(t.shape)))
+    seg = np.ascontiguousarray(np.asarray(seg_start, dtype=np.int64).reshape(-1))
+    thr = np.ascontiguousarray(np.asarray(thresholds, dtype=np.float32).reshape(-1))
+    N, J, S = int(p.shape[0]), int(p.shape[1]), int(seg.size) - 1
+    dev = p.device
+    lib = L.load()
+    wb = _check_size(lib.gast_pose_metrics_workspace_bytes(S, J, int(thr.size), N), 'pose_metrics')
+    rows = torch.empty((S, 3 + J + int(thr.size)), dtype=torch.float64, device=dev)
+    dist = torch.empty((N, J), dtype=torch.float32, device=dev) if distances else None
+    with torch.cuda.device(dev):
+        ws = _prep_ws(dev, wb)
+        _check(lib.gast_pose_metrics(_p(p), _p(t), N, J, seg.ctypes.data_as(C.POINTER(C.c_int64)), S,
+                                     thr.ctypes.data_as(C.POINTER(C.c_float)), int(thr.size), 1 if zero_root else 0,
+                                     1 if procrustes else 0, _p(rows), _p(dist), _p(ws), ws.numel(),
+                                     C.c_void_p(_stream(dev))), 'gast_pose_metrics')
+    return (rows, dist) if distances else rows
 
 
 class FusedAdam(object):

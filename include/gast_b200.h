@@ -530,6 +530,22 @@ int gast_mpjpe(const float* pred, const float* target, int64_t n_points, int32_t
  * (Procrustes) alignment of pred[n] (J,3) to target[n]; the reference's scalar is the mean of per_frame. */
 int gast_p_mpjpe(const float* pred, const float* target, int32_t N, int32_t J, float* per_frame, void* stream);
 
+/* Scores of a test set, per segment (main.py:299-353 evaluate; common/loss.py:56-90 euclidean_losses, pck, auc).
+ * pred, target (N,J,3) float32 on the device, 1 <= J <= 32 (>= 3 with procrustes).  seg_start (S+1) host int64:
+ * 0 = seg_start[0] <= ... <= seg_start[S] = N; segment s is frames seg_start[s] .. seg_start[s+1]-1.  thresholds:
+ * n_thr (<= 64) host float32, none NaN.  rows (S, 3+J+n_thr) float64 on the device receives per segment
+ *   [frames, sum_f mpjpe_f, sum_f p_mpjpe_f, sum_f dist_fj for j < J, count(dist_fj < thresholds[k]) for k < n_thr]
+ * with dist = sqrt((dx*dx + dy*dy) + dz*dz) in float32, every step rounded (torch's CPU order), mpjpe_f the mean of a
+ * frame's dist in double, and p_mpjpe_f gast_p_mpjpe's value of the frame (0 with procrustes = 0).  zero_root reads
+ * target joint 0 as 0 (main.py:327) without writing it.  dist (N,J) float32 on the device, or null, receives every
+ * dist.  The sums run in float64 in a fixed order: a segment's row depends only on its own frames, so it is the same
+ * bits whatever other segments the call holds.  workspace: gast_pose_metrics_workspace_bytes(S, J, n_thr, N) bytes
+ * on the device.  Every argument is checked on the host before the first launch. */
+size_t gast_pose_metrics_workspace_bytes(int32_t S, int32_t J, int32_t n_thr, int64_t N);
+int gast_pose_metrics(const float* pred, const float* target, int64_t N, int32_t J, const int64_t* seg_start, int32_t S,
+                      const float* thresholds, int32_t n_thr, int32_t zero_root, int32_t procrustes, double* rows,
+                      float* dist, void* workspace, size_t workspace_bytes, void* stream);
+
 /* optim.Adam(amsgrad=True) (trainval.py:78,162-164) for every parameter in one launch.  table (n_chunks,4)
  * int64 on the device: {param pointer, grad pointer, offset into the flat state buffers, count <=
  * gast_adam_chunk()}.  max_exp_avg_sq null = plain Adam.  step = 1 for the first update. */
