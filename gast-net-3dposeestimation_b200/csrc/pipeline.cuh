@@ -18,9 +18,9 @@ namespace gast {
 //   when flip (feature 0 negated, left/right keypoints swapped); batch_3d likewise without padding;
 //   batch_cam[b] = cameras[seq] with entries 2 and 7 negated when flip (:139-144).
 // ------------------------------------------------------------------------------------------
-__global__ void chunk_gather_kernel(const float* __restrict__ poses, const long long* __restrict__ seq_start,
-                                    const int* __restrict__ pairs, float* __restrict__ out, int B, int Tc, int J, int F,
-                                    int lead, JointPerm perm) {
+__device__ __forceinline__ void chunk_gather_at(const float* __restrict__ poses, const long long* __restrict__ seq_start,
+                                                const int* __restrict__ pairs, float* __restrict__ out, int B, int Tc,
+                                                int J, int F, int lead, const JointPerm& perm) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long n = (long long)B * Tc * J * F;
   if (idx >= n) return;
@@ -37,14 +37,48 @@ __global__ void chunk_gather_kernel(const float* __restrict__ poses, const long 
   out[idx] = (flip && c == 0) ? -v : v;
 }
 
-__global__ void chunk_cam_kernel(const float* __restrict__ cams, const int* __restrict__ pairs, float* __restrict__ out,
-                                 int B, int ncam) {
+__device__ __forceinline__ void chunk_cam_at(const float* __restrict__ cams, const int* __restrict__ pairs,
+                                             float* __restrict__ out, int B, int ncam) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= B * ncam) return;
   const int b = idx / ncam, k = idx - b * ncam;
   float v = cams[(long long)pairs[4 * b] * ncam + k];
   if (pairs[4 * b + 3] && (k == 2 || k == 7)) v = -v;
   out[idx] = v;
+}
+
+__global__ void chunk_gather_kernel(const float* __restrict__ poses, const long long* __restrict__ seq_start,
+                                    const int* __restrict__ pairs, float* __restrict__ out, int B, int Tc, int J, int F,
+                                    int lead, JointPerm perm) {
+  chunk_gather_at(poses, seq_start, pairs, out, B, Tc, J, F, lead, perm);
+}
+
+__global__ void chunk_cam_kernel(const float* __restrict__ cams, const int* __restrict__ pairs, float* __restrict__ out,
+                                 int B, int ncam) {
+  chunk_cam_at(cams, pairs, out, B, ncam);
+}
+
+// The same batch read from an epoch's whole pair table at the epoch's batch counter *batch (device): rows
+// *batch * stride .. + B - 1.  Nothing is written when those rows are not all in the table.
+__device__ __forceinline__ const int* batch_pairs(const int* pairs, long long n_pairs, int stride, const long long* batch,
+                                                  int B) {
+  const long long r0 = *batch * stride;
+  return (r0 < 0 || r0 + B > n_pairs) ? nullptr : pairs + 4 * r0;
+}
+
+__global__ void chunk_gather_indexed_kernel(const float* __restrict__ poses, const long long* __restrict__ seq_start,
+                                            const int* __restrict__ pairs, long long n_pairs, int stride,
+                                            const long long* __restrict__ batch, float* __restrict__ out, int B, int Tc,
+                                            int J, int F, int lead, JointPerm perm) {
+  const int* pb = batch_pairs(pairs, n_pairs, stride, batch, B);
+  if (pb) chunk_gather_at(poses, seq_start, pb, out, B, Tc, J, F, lead, perm);
+}
+
+__global__ void chunk_cam_indexed_kernel(const float* __restrict__ cams, const int* __restrict__ pairs, long long n_pairs,
+                                         int stride, const long long* __restrict__ batch, float* __restrict__ out, int B,
+                                         int ncam) {
+  const int* pb = batch_pairs(pairs, n_pairs, stride, batch, B);
+  if (pb) chunk_cam_at(cams, pb, out, B, ncam);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -621,9 +655,10 @@ __global__ void pose_metrics_sum_kernel(const double* __restrict__ part, const l
 // ------------------------------------------------------------------------------------------
 constexpr int ADAM_CHUNK = 4096;
 
-__global__ void adam_multi_kernel(const long long* __restrict__ table, float* __restrict__ exp_avg,
-                                  float* __restrict__ exp_avg_sq, float* __restrict__ max_sq, float one_m_b1, float b2,
-                                  float one_m_b2, float step_size, float bc2_sqrt, float eps, float wd) {
+__device__ __forceinline__ void adam_chunk_update(const long long* __restrict__ table, float* __restrict__ exp_avg,
+                                                  float* __restrict__ exp_avg_sq, float* __restrict__ max_sq,
+                                                  float one_m_b1, float b2, float one_m_b2, float step_size,
+                                                  float bc2_sqrt, float eps, float wd) {
   const long long* e = table + 4LL * blockIdx.x;
   float* p = reinterpret_cast<float*>(e[0]);
   const float* g = reinterpret_cast<const float*>(e[1]);
@@ -644,6 +679,80 @@ __global__ void adam_multi_kernel(const long long* __restrict__ table, float* __
   }
 }
 
+__global__ void adam_multi_kernel(const long long* __restrict__ table, float* __restrict__ exp_avg,
+                                  float* __restrict__ exp_avg_sq, float* __restrict__ max_sq, float one_m_b1, float b2,
+                                  float one_m_b2, float step_size, float bc2_sqrt, float eps, float wd) {
+  adam_chunk_update(table, exp_avg, exp_avg_sq, max_sq, one_m_b1, b2, one_m_b2, step_size, bc2_sqrt, eps, wd);
+}
+
+// The step of batch *batch of an epoch: coef[2 b] = lr / bc1 and coef[2 b + 1] = sqrt(bc2) of that step, as
+// gast_adam_step rounds them (adam_coefs).  No update when b is outside the table.
+__global__ void adam_multi_indexed_kernel(const long long* __restrict__ table, float* __restrict__ exp_avg,
+                                          float* __restrict__ exp_avg_sq, float* __restrict__ max_sq, float one_m_b1,
+                                          float b2, float one_m_b2, const float* __restrict__ coef, long long n_steps,
+                                          const long long* __restrict__ batch, float eps, float wd) {
+  const long long b = *batch;
+  if (b < 0 || b >= n_steps) return;
+  adam_chunk_update(table, exp_avg, exp_avg_sq, max_sq, one_m_b1, b2, one_m_b2, coef[2 * b], coef[2 * b + 1], eps, wd);
+}
+
+// The last launch of an epoch step: losses[b] = *loss, *sum += weight * *loss in double (main.train's
+// `epoch_loss_3d_train += B * T * loss.item()`, in batch order), then the batch counter moves on.
+__global__ void epoch_loss_accumulate_kernel(const float* __restrict__ loss, long long weight, double* __restrict__ sum,
+                                             float* __restrict__ losses, long long n_steps, long long* __restrict__ batch) {
+  const long long b = *batch;
+  const float l = *loss;
+  if (b >= 0 && b < n_steps) losses[b] = l;
+  *sum += (double)weight * (double)l;
+  *batch = b + 1;
+}
+
+// gast_adam_step's host arithmetic for one step: lr / bc1 and sqrt(bc2), in double, rounded to float
+static inline void adam_coefs(double lr, double beta1, double beta2, long long step, float* step_size, float* bc2_sqrt) {
+  const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
+  *step_size = (float)(lr / bc1);
+  *bc2_sqrt = (float)sqrt(bc2);
+}
+
+}  // namespace gast
+
+namespace gast {
+// gast_chunk_gather and, with a batch counter, gast_chunk_gather_indexed: the batch's pairs are pairs[0 .. B-1], or the
+// rows *batch * stride .. of the epoch's n_pairs-row table
+static int chunk_gather_launch(const char* what, const float* poses_2d, const float* poses_3d, const float* cameras,
+                               const int64_t* seq_start, int32_t n_seq, const int32_t* pairs, long long n_pairs,
+                               int32_t stride, const int64_t* batch, int32_t B, int32_t chunk, int32_t pad,
+                               int32_t causal_shift, int32_t J2, int32_t F2, int32_t J3, int32_t ncam, int32_t n_sym2,
+                               const int32_t* kps_left, const int32_t* kps_right, int32_t n_sym3,
+                               const int32_t* joints_left, const int32_t* joints_right, float* batch_2d,
+                               float* batch_3d, float* batch_cam, void* stream) {
+  if (!poses_2d || !seq_start || !pairs || !batch_2d || B <= 0 || chunk <= 0 || pad < 0 || n_seq <= 0 || J2 <= 0 || F2 <= 0)
+    return fail("%s: bad arguments", what);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  JointPerm p2, p3;
+  if (make_perm(J2, n_sym2, kps_left, kps_right, &p2)) return 1;
+  const bool want3 = poses_3d && batch_3d;
+  if (want3 && make_perm(J3, n_sym3, joints_left, joints_right, &p3)) return 1;
+  const long long* ss = reinterpret_cast<const long long*>(seq_start);
+  const long long* bp = reinterpret_cast<const long long*>(batch);
+  const int Tc = chunk + 2 * pad;
+  const long long n2 = (long long)B * Tc * J2 * F2, n3 = (long long)B * chunk * J3 * 3, nc = (long long)B * ncam;
+  if (!bp) {
+    chunk_gather_kernel<<<cdiv(n2, 256), 256, 0, st>>>(poses_2d, ss, pairs, batch_2d, B, Tc, J2, F2, pad + causal_shift, p2);
+    if (want3) chunk_gather_kernel<<<cdiv(n3, 256), 256, 0, st>>>(poses_3d, ss, pairs, batch_3d, B, chunk, J3, 3, 0, p3);
+    if (cameras && batch_cam && ncam > 0) chunk_cam_kernel<<<cdiv(nc, 256), 256, 0, st>>>(cameras, pairs, batch_cam, B, ncam);
+  } else {
+    chunk_gather_indexed_kernel<<<cdiv(n2, 256), 256, 0, st>>>(poses_2d, ss, pairs, n_pairs, stride, bp, batch_2d, B, Tc,
+                                                               J2, F2, pad + causal_shift, p2);
+    if (want3)
+      chunk_gather_indexed_kernel<<<cdiv(n3, 256), 256, 0, st>>>(poses_3d, ss, pairs, n_pairs, stride, bp, batch_3d, B,
+                                                                 chunk, J3, 3, 0, p3);
+    if (cameras && batch_cam && ncam > 0)
+      chunk_cam_indexed_kernel<<<cdiv(nc, 256), 256, 0, st>>>(cameras, pairs, n_pairs, stride, bp, batch_cam, B, ncam);
+  }
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
 }  // namespace gast
 
 extern "C" int gast_chunk_gather(const float* poses_2d, const float* poses_3d, const float* cameras,
@@ -652,25 +761,24 @@ extern "C" int gast_chunk_gather(const float* poses_2d, const float* poses_3d, c
                                  int32_t ncam, int32_t n_sym2, const int32_t* kps_left, const int32_t* kps_right,
                                  int32_t n_sym3, const int32_t* joints_left, const int32_t* joints_right,
                                  float* batch_2d, float* batch_3d, float* batch_cam, void* stream) {
-  if (!poses_2d || !seq_start || !pairs || !batch_2d || B <= 0 || chunk <= 0 || pad < 0 || n_seq <= 0 || J2 <= 0 || F2 <= 0)
-    return fail("gast_chunk_gather: bad arguments");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  JointPerm p2, p3;
-  if (make_perm(J2, n_sym2, kps_left, kps_right, &p2)) return 1;
-  const int Tc = chunk + 2 * pad;
-  const long long n2 = (long long)B * Tc * J2 * F2;
-  chunk_gather_kernel<<<cdiv(n2, 256), 256, 0, st>>>(poses_2d, reinterpret_cast<const long long*>(seq_start), pairs,
-                                                     batch_2d, B, Tc, J2, F2, pad + causal_shift, p2);
-  if (poses_3d && batch_3d) {
-    if (make_perm(J3, n_sym3, joints_left, joints_right, &p3)) return 1;
-    const long long n3 = (long long)B * chunk * J3 * 3;
-    chunk_gather_kernel<<<cdiv(n3, 256), 256, 0, st>>>(poses_3d, reinterpret_cast<const long long*>(seq_start), pairs,
-                                                       batch_3d, B, chunk, J3, 3, 0, p3);
-  }
-  if (cameras && batch_cam && ncam > 0)
-    chunk_cam_kernel<<<cdiv((long long)B * ncam, 256), 256, 0, st>>>(cameras, pairs, batch_cam, B, ncam);
-  CUDA_OK(cudaGetLastError());
-  return 0;
+  return chunk_gather_launch("gast_chunk_gather", poses_2d, poses_3d, cameras, seq_start, n_seq, pairs, B, B, nullptr, B,
+                             chunk, pad, causal_shift, J2, F2, J3, ncam, n_sym2, kps_left, kps_right, n_sym3, joints_left,
+                             joints_right, batch_2d, batch_3d, batch_cam, stream);
+}
+
+extern "C" int gast_chunk_gather_indexed(const float* poses_2d, const float* poses_3d, const float* cameras,
+                                         const int64_t* seq_start, int32_t n_seq, const int32_t* pairs, int64_t n_pairs,
+                                         int32_t batch_stride, const int64_t* batch, int32_t B, int32_t chunk,
+                                         int32_t pad, int32_t causal_shift, int32_t J2, int32_t F2, int32_t J3,
+                                         int32_t ncam, int32_t n_sym2, const int32_t* kps_left, const int32_t* kps_right,
+                                         int32_t n_sym3, const int32_t* joints_left, const int32_t* joints_right,
+                                         float* batch_2d, float* batch_3d, float* batch_cam, void* stream) {
+  if (!batch || n_pairs <= 0 || batch_stride < B)
+    return fail("gast_chunk_gather_indexed: bad arguments (batch counter, n_pairs = %lld > 0, batch_stride = %d >= B = %d)",
+                (long long)n_pairs, batch_stride, B);
+  return chunk_gather_launch("gast_chunk_gather_indexed", poses_2d, poses_3d, cameras, seq_start, n_seq, pairs, n_pairs,
+                             batch_stride, batch, B, chunk, pad, causal_shift, J2, F2, J3, ncam, n_sym2, kps_left,
+                             kps_right, n_sym3, joints_left, joints_right, batch_2d, batch_3d, batch_cam, stream);
 }
 
 extern "C" int gast_keypoints_convert(const float* kpts, float* out, int32_t* valid, int32_t T, int32_t J_in, int32_t mode,
@@ -729,10 +837,40 @@ extern "C" int gast_adam_step(const int64_t* table, int32_t n_chunks, float* exp
                               double lr, double beta1, double beta2, double eps, double weight_decay, int64_t step,
                               void* stream) {
   if (!table || !exp_avg || !exp_avg_sq || n_chunks <= 0 || step < 1) return fail("gast_adam_step: bad arguments");
-  const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
+  float step_size, bc2_sqrt;
+  adam_coefs(lr, beta1, beta2, step, &step_size, &bc2_sqrt);
   adam_multi_kernel<<<n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const long long*>(table), exp_avg, exp_avg_sq, max_exp_avg_sq, (float)(1.0 - beta1), (float)beta2,
-      (float)(1.0 - beta2), (float)(lr / bc1), (float)sqrt(bc2), (float)eps, (float)weight_decay);
+      (float)(1.0 - beta2), step_size, bc2_sqrt, (float)eps, (float)weight_decay);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gast_adam_step_table(double lr, double beta1, double beta2, int64_t first_step, int32_t n_steps,
+                                    float* coef) {
+  if (!coef || n_steps <= 0 || first_step < 1) return fail("gast_adam_step_table: bad arguments");
+  for (int32_t i = 0; i < n_steps; ++i) adam_coefs(lr, beta1, beta2, first_step + i, &coef[2 * i], &coef[2 * i + 1]);
+  return 0;
+}
+
+extern "C" int gast_adam_step_indexed(const int64_t* table, int32_t n_chunks, float* exp_avg, float* exp_avg_sq,
+                                      float* max_exp_avg_sq, double beta1, double beta2, double eps, double weight_decay,
+                                      const float* coef, int64_t n_steps, const int64_t* batch, void* stream) {
+  if (!table || !exp_avg || !exp_avg_sq || !coef || !batch || n_chunks <= 0 || n_steps <= 0)
+    return fail("gast_adam_step_indexed: bad arguments");
+  adam_multi_indexed_kernel<<<n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const long long*>(table), exp_avg, exp_avg_sq, max_exp_avg_sq, (float)(1.0 - beta1), (float)beta2,
+      (float)(1.0 - beta2), coef, n_steps, reinterpret_cast<const long long*>(batch), (float)eps, (float)weight_decay);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gast_epoch_loss_accumulate(const float* loss, int64_t weight, double* sum, float* losses, int64_t n_steps,
+                                          int64_t* batch, void* stream) {
+  if (!loss || !sum || !losses || !batch || weight <= 0 || n_steps <= 0)
+    return fail("gast_epoch_loss_accumulate: bad arguments");
+  epoch_loss_accumulate_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      loss, weight, sum, losses, n_steps, reinterpret_cast<long long*>(batch));
   CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -34,7 +34,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_revise_skes_workspace_bytes', 'gast_revise_skes', 'gast_revise_skes_real_time_workspace_bytes',
            'gast_revise_skes_real_time', 'gast_normalize_screen', 'gast_camera_to_world',
            'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_pose_metrics_workspace_bytes',
-           'gast_pose_metrics', 'gast_adam_chunk', 'gast_adam_step',
+           'gast_pose_metrics', 'gast_adam_chunk', 'gast_adam_step', 'gast_chunk_gather_indexed',
+           'gast_adam_step_table', 'gast_adam_step_indexed', 'gast_epoch_loss_accumulate',
            'gast_last_error', 'gast_version']
 
 
@@ -257,6 +258,17 @@ def load():
     lib.gast_adam_step.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,
                                    C.c_double, C.c_int64, vp]
     lib.gast_adam_step.restype = C.c_int
+    lib.gast_chunk_gather_indexed.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int64, C.c_int32, vp, C.c_int32,
+                                              C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                              C.c_int32, C.c_int32, ip, ip, C.c_int32, ip, ip, vp, vp, vp, vp]
+    lib.gast_chunk_gather_indexed.restype = C.c_int
+    lib.gast_adam_step_table.argtypes = [C.c_double, C.c_double, C.c_double, C.c_int64, C.c_int32, vp]
+    lib.gast_adam_step_table.restype = C.c_int
+    lib.gast_adam_step_indexed.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,
+                                           vp, C.c_int64, vp, vp]
+    lib.gast_adam_step_indexed.restype = C.c_int
+    lib.gast_epoch_loss_accumulate.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, vp, vp]
+    lib.gast_epoch_loss_accumulate.restype = C.c_int
     lib.gast_last_error.argtypes = []
     lib.gast_last_error.restype = C.c_char_p
     lib.gast_version.argtypes = []

@@ -68,6 +68,38 @@ def chunk_gather(seqs, pairs, chunk_length, pad, causal_shift=0, kps_left=None, 
     return bc, b3, b2
 
 
+def chunk_gather_indexed(seqs, pairs, batch, B, batch_stride, chunk_length, pad, causal_shift=0, kps_left=None,
+                         kps_right=None, joints_left=None, joints_right=None):
+    """chunk_gather of pairs[b*batch_stride : b*batch_stride + B], b the CUDA int64 batch counter `batch` (read on the
+    device, so one CUDA graph serves every batch of an epoch).  pairs: the epoch's (n_pairs,4) CUDA int32 table.
+    Same results, bit for bit; nothing is written when those rows are not all in the table."""
+    dev = seqs.poses_2d.device
+    if pairs.dtype != torch.int32 or pairs.dim() != 2 or pairs.shape[1] != 4 or not pairs.is_contiguous() \
+            or batch.dtype != torch.int64 or pairs.device != dev or batch.device != dev:
+        raise GastError('chunk_gather_indexed: pairs (n,4) contiguous int32 and an int64 batch counter on %s expected' % dev)
+    J2, F2 = int(seqs.poses_2d.shape[1]), int(seqs.poses_2d.shape[2])
+    b2 = torch.empty((B, chunk_length + 2 * pad, J2, F2), dtype=torch.float32, device=dev)
+    b3, J3 = None, 0
+    if seqs.poses_3d is not None:
+        J3 = int(seqs.poses_3d.shape[1])
+        b3 = torch.empty((B, chunk_length, J3, 3), dtype=torch.float32, device=dev)
+    bc, ncam = None, 0
+    if seqs.cameras is not None:
+        ncam = int(seqs.cameras.shape[1])
+        bc = torch.empty((B, ncam), dtype=torch.float32, device=dev)
+    kl, n2 = _ilist(kps_left)
+    kr, _ = _ilist(kps_right)
+    jl, n3 = _ilist(joints_left)
+    jr, _ = _ilist(joints_right)
+    with torch.cuda.device(dev):
+        _check(L.load().gast_chunk_gather_indexed(_p(seqs.poses_2d), _p(seqs.poses_3d), _p(seqs.cameras),
+                                                  _p(seqs.seq_start), seqs.n_seq, _p(pairs), int(pairs.shape[0]),
+                                                  int(batch_stride), _p(batch), int(B), int(chunk_length), int(pad),
+                                                  int(causal_shift), J2, F2, J3, ncam, n2, kl, kr, n3, jl, jr, _p(b2),
+                                                  _p(b3), _p(bc), C.c_void_p(_stream(dev))), 'gast_chunk_gather_indexed')
+    return bc, b3, b2
+
+
 # ------------------------------------------------------------------------------------------------
 # N3: keypoint formats, screen normalisation, camera -> world
 # ------------------------------------------------------------------------------------------------
@@ -287,6 +319,28 @@ def pose_metrics(predicted, target, seg_start, thresholds=(), zero_root=False, p
     return (rows, dist) if distances else rows
 
 
+def adam_step_table(lr, betas, first_step, n_steps):
+    """(n_steps,2) float32 numpy: {lr / bc1, sqrt(bc2)} of steps first_step .. first_step + n_steps - 1, rounded as
+    gast_adam_step rounds them (gast_adam_step_table), for FusedAdam.step_indexed."""
+    out = np.empty((int(n_steps), 2), dtype=np.float32)
+    _check(L.load().gast_adam_step_table(float(lr), float(betas[0]), float(betas[1]), int(first_step), int(n_steps),
+                                         out.ctypes.data_as(C.c_void_p)), 'gast_adam_step_table')
+    return out
+
+
+def epoch_loss_accumulate(loss, weight, loss_sum, losses, batch):
+    """The last launch of an epoch step: losses[b] = loss, loss_sum += weight * loss in fp64, b += 1 (b the CUDA int64
+    batch counter `batch`).  loss 0-d float32, loss_sum 0-d float64, losses (n_steps,) float32, all on one device."""
+    dev = loss.device
+    if loss.dtype != torch.float32 or loss_sum.dtype != torch.float64 or losses.dtype != torch.float32 \
+            or batch.dtype != torch.int64 or {loss_sum.device, losses.device, batch.device} != {dev} or not loss.is_cuda:
+        raise GastError('epoch_loss_accumulate: float32 loss, float64 sum, float32 losses and an int64 batch counter '
+                        'on one CUDA device expected')
+    with torch.cuda.device(dev):
+        _check(L.load().gast_epoch_loss_accumulate(_p(loss), int(weight), _p(loss_sum), _p(losses), losses.numel(),
+                                                   _p(batch), C.c_void_p(_stream(dev))), 'gast_epoch_loss_accumulate')
+
+
 class FusedAdam(object):
     """optim.Adam(params, lr, amsgrad=True) (trainval.py:78) as ONE kernel launch per step over every
     parameter (the stock optimiser issues ~10 elementwise launches per tensor, ~2000 per step here).
@@ -344,6 +398,28 @@ class FusedAdam(object):
                                            self.step_count, C.c_void_p(_stream(dev))), 'gast_adam_step')
         # the kernel writes the parameters through raw pointers: bump their version counters so that everything
         # keyed on (data_ptr, _version) -- the engine's folded eval-mode constants -- sees the update
+        torch.autograd.graph.increment_version(self.params)
+
+    def step_indexed(self, coef, batch):
+        """step() at step step_count + 1 + b without a host argument that changes per step: b the CUDA int64 batch
+        counter `batch`, coef the (n_steps,2) CUDA float32 adam_step_table of the steps from step_count + 1 at the
+        current lr.  Bit for bit step()'s update; no update when b >= n_steps.  step_count is the caller's to
+        advance (EpochTrainer adds an epoch's steps at its end)."""
+        if any(p.grad is None for p in self.params):
+            raise GastError('FusedAdam.step_indexed: every parameter needs a gradient')
+        dev = self.params[0].device
+        if coef.dtype != torch.float32 or coef.dim() != 2 or coef.shape[1] != 2 or not coef.is_contiguous() \
+                or batch.dtype != torch.int64 or coef.device != dev or batch.device != dev:
+            raise GastError('FusedAdam.step_indexed: coef (n,2) contiguous float32 and an int64 batch counter on %s '
+                            'expected' % dev)
+        self._build_table()
+        g = self.param_groups[0]
+        with torch.cuda.device(dev):
+            _check(L.load().gast_adam_step_indexed(_p(self._table), int(self._table.shape[0]), _p(self.exp_avg),
+                                                   _p(self.exp_avg_sq), _p(self.max_exp_avg_sq), float(g['betas'][0]),
+                                                   float(g['betas'][1]), float(g['eps']), float(g['weight_decay']),
+                                                   _p(coef), int(coef.shape[0]), _p(batch), C.c_void_p(_stream(dev))),
+                   'gast_adam_step_indexed')
         torch.autograd.graph.increment_version(self.params)
 
     def state_dict(self):

@@ -553,6 +553,39 @@ int32_t gast_adam_chunk(void);
 int gast_adam_step(const int64_t* table, int32_t n_chunks, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
                    double lr, double beta1, double beta2, double eps, double weight_decay, int64_t step, void* stream);
 
+/* ---- whole training epochs on the device (gast_b200.training.EpochTrainer) --------------------------------------
+ * A training step that one CUDA graph captures once and replays for every batch of an epoch reads which batch it is
+ * from a device int64 batch counter *batch (b below) that the epoch keeps: 0 at the start of the epoch, advanced by
+ * gast_epoch_loss_accumulate, the last launch of a step.  None of the three reads device data on the host,
+ * allocates or synchronises.
+ *
+ * gast_chunk_gather_indexed: gast_chunk_gather's arguments, with pairs the whole epoch's (n_pairs,4) int32 pair
+ *   table; writes exactly what gast_chunk_gather writes for pairs[b*batch_stride .. b*batch_stride + B - 1], bit for
+ *   bit (batch_stride >= B: the full batch size, so that a shorter last batch is served with its own B).  Writes
+ *   nothing when those rows are not all in the table. */
+int gast_chunk_gather_indexed(const float* poses_2d, const float* poses_3d, const float* cameras, const int64_t* seq_start,
+                              int32_t n_seq, const int32_t* pairs, int64_t n_pairs, int32_t batch_stride,
+                              const int64_t* batch, int32_t B, int32_t chunk, int32_t pad, int32_t causal_shift,
+                              int32_t J2, int32_t F2, int32_t J3, int32_t ncam, int32_t n_sym2, const int32_t* kps_left,
+                              const int32_t* kps_right, int32_t n_sym3, const int32_t* joints_left,
+                              const int32_t* joints_right, float* batch_2d, float* batch_3d, float* batch_cam,
+                              void* stream);
+
+/* gast_adam_step_table: coef (2*n_steps) (host) receives, for steps first_step .. first_step + n_steps - 1,
+ *   {lr / bc1, sqrt(bc2)} computed and rounded to float exactly as gast_adam_step computes them (in double, C pow).
+ * gast_adam_step_indexed: gast_adam_step at step first_step + b, with coef (2*n_steps) that table on the device:
+ *   bit for bit the same update.  No update when b >= n_steps. */
+int gast_adam_step_table(double lr, double beta1, double beta2, int64_t first_step, int32_t n_steps, float* coef);
+int gast_adam_step_indexed(const int64_t* table, int32_t n_chunks, float* exp_avg, float* exp_avg_sq,
+                           float* max_exp_avg_sq, double beta1, double beta2, double eps, double weight_decay,
+                           const float* coef, int64_t n_steps, const int64_t* batch, void* stream);
+
+/* gast_epoch_loss_accumulate: losses[b] = *loss (when b < n_steps), *sum += (double)weight * (double)*loss (fp64),
+ *   then *batch = b + 1.  With weight = B * T_out of the step, *sum / (sum of the weights) is main.train's epoch
+ *   loss (main.py:231,242) bit for bit. */
+int gast_epoch_loss_accumulate(const float* loss, int64_t weight, double* sum, float* losses, int64_t n_steps,
+                               int64_t* batch, void* stream);
+
 /* Test/probe entry (not on the forward path): out[M,N] = A[M,K] . W[N,K]^T on one GEMM core
  * (core 0 = tensor cores, tc_mode 0 = fp32-grade as inference runs it, three scaled fp16 products (F16X3),
  * 1 = single-pass TF32, 3 = fp32-grade as training runs it, three TF32 products (3xTF32), or 16 = the half form of
