@@ -142,6 +142,7 @@ __device__ __forceinline__ void coco_to_h36m_frame(const float* kp, int ld, floa
 // mode 0: coco_h36m            kp (T,17,2)  -> out (T,17,2)
 // mode 1: mpii_h36m            kp (T,16,2)  -> out (T,17,2)   (:51-59)
 // mode 2: coco_h36m_toe_format kp (T,Jin>=22,2) -> out (T,19,2)   (:62-78)
+// mode 3: HumanEva's COCO -> 15 joints (main.py:80-95) kp (T,17,2) -> out (T,15,2)
 __global__ void kpt_convert_kernel(const float* __restrict__ kp, float* __restrict__ out, int* __restrict__ valid,
                                    int T, int Jin, int mode) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -160,6 +161,16 @@ __global__ void kpt_convert_kernel(const float* __restrict__ kp, float* __restri
 #pragma unroll
     for (int c = 0; c < 2; ++c)
       o[7 * 2 + c] = __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(k[2 * 2 + c], k[3 * 2 + c]), k[12 * 2 + c]), k[13 * 2 + c]), 4.f);
+  } else if (mode == 3) {
+    Jo = 15;
+    const int coco_of[13] = {5, 7, 9, 6, 8, 10, 11, 13, 15, 12, 14, 16, 0};   // kps_15[2 ..] = kps[coco_of]
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      o[c] = __fdiv_rn(__fadd_rn(k[11 * 2 + c], k[12 * 2 + c]), 2.f);
+      o[2 + c] = __fdiv_rn(__fadd_rn(k[5 * 2 + c], k[6 * 2 + c]), 2.f);
+#pragma unroll
+      for (int i = 0; i < 13; ++i) o[(i + 2) * 2 + c] = k[coco_of[i] * 2 + c];
+    }
   } else {
     Jo = 19;
     float h[34];
@@ -405,6 +416,135 @@ __global__ void cam_to_world_kernel(const float* __restrict__ x, float* __restri
   out[3 * i] = vx + 2.f * (q0 * ux + wx) + t0;
   out[3 * i + 1] = vy + 2.f * (q0 * uy + wy) + t1;
   out[3 * i + 2] = vz + 2.f * (q0 * uz + wz) + t2;
+}
+
+// ------------------------------------------------------------------------------------------
+// Dataset preparation (main.py:24-104 load_data, data/prepare_data_h36m.py:113-121) as segmented launches: output
+// segment s takes rows dst[s] .. dst[s+1]-1 from source rows src[s] .. with its own camera, so one launch covers every
+// (sequence, camera) of a dataset.  The tables are device-resident; a row whose source falls outside the input is
+// not written.  float32 in torch's CPU / numpy's order of operations, no contraction: bit-identical to the reference.
+// ------------------------------------------------------------------------------------------
+// the segment of output row i: the last s < S with dst[s] <= i (dst ascending from dst[0] = 0)
+__device__ __forceinline__ int seg_of(const long long* __restrict__ dst, int S, long long i) {
+  int lo = 0, hi = S - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (dst[mid] <= i) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// a1*b2 - a2*b1 as torch's CPU cross product rounds it: fma(a1, b2, -(a2*b1))
+__device__ __forceinline__ float cross_term(float a1, float b2, float a2, float b1) {
+  return __fmaf_rn(a1, b2, -__fmul_rn(a2, b1));
+}
+
+// world_to_camera (camera.py:22-24) of point p: qort(qinverse(R), p - t) (quaternion.py:4-35), qt = {R[4], t[3]}
+__device__ __forceinline__ void world_to_camera_point(const float* __restrict__ p, const float* __restrict__ qt, float* o) {
+  const float v[3] = {__fsub_rn(p[0], qt[4]), __fsub_rn(p[1], qt[5]), __fsub_rn(p[2], qt[6])};
+  const float q[3] = {-qt[1], -qt[2], -qt[3]};
+  float u[3], w[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) u[c] = cross_term(q[(c + 1) % 3], v[(c + 2) % 3], q[(c + 2) % 3], v[(c + 1) % 3]);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) w[c] = cross_term(q[(c + 1) % 3], u[(c + 2) % 3], q[(c + 2) % 3], u[(c + 1) % 3]);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) o[c] = __fadd_rn(v[c], __fmul_rn(2.f, __fadd_rn(__fmul_rn(qt[0], u[c]), w[c])));
+}
+
+// one thread per output point (frame, joint) of frames of J points; qt (S,7).  root_relative: pos[:, 1:] -= pos[:, :1]
+// (main.py:33), joint 0 recomputed by each thread of the frame.
+__global__ void world_to_camera_kernel(const float* __restrict__ x, long long n_src, int J, const long long* __restrict__ src,
+                                       const long long* __restrict__ dst, const float* __restrict__ qt, int S,
+                                       long long n_out, int root_relative, float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_out * J) return;
+  const long long f = i / J;
+  const int j = (int)(i - f * J);
+  const int s = seg_of(dst, S, f);
+  const long long fs = src[s] + (f - dst[s]);
+  if (fs < 0 || fs >= n_src) return;
+  float o[3];
+  world_to_camera_point(x + (fs * J + j) * 3, qt + 7 * s, o);
+  if (root_relative && j > 0) {
+    float r[3];
+    world_to_camera_point(x + fs * J * 3, qt + 7 * s, r);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = __fsub_rn(o[c], r[c]);
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) out[i * 3 + c] = o[c];
+}
+
+// project_to_2d (camera.py:31-62), one thread per point; segment s (points seg[s] .. seg[s+1]-1) has the intrinsics
+// k = intr[9 s ..] = {f[2], c[2], radial[3], tangential[2]}.  Sums in torch's order: r2 = x*x + y*y,
+// radial = 1 + ((k0*r2 + k1*r2^2) + k2*r2^3) with r2^3 = (r2*r2)*r2.
+__global__ void project_to_2d_kernel(const float* __restrict__ x, long long n, const long long* __restrict__ seg,
+                                     const float* __restrict__ intr, int S, float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float* k = intr + 9 * seg_of(seg, S, i);
+  const float z = x[3 * i + 2];
+  const float xx = __fdiv_rn(x[3 * i], z), yy = __fdiv_rn(x[3 * i + 1], z);
+  const float r2 = __fadd_rn(__fmul_rn(xx, xx), __fmul_rn(yy, yy));
+  const float r4 = __fmul_rn(r2, r2), r6 = __fmul_rn(r4, r2);
+  const float radial = __fadd_rn(1.f, __fadd_rn(__fadd_rn(__fmul_rn(k[4], r2), __fmul_rn(k[5], r4)), __fmul_rn(k[6], r6)));
+  const float tan = __fadd_rn(__fmul_rn(k[7], xx), __fmul_rn(k[8], yy));
+  const float rt = __fadd_rn(radial, tan);
+  const float u = __fadd_rn(__fmul_rn(xx, rt), __fmul_rn(k[7], r2));
+  const float v = __fadd_rn(__fmul_rn(yy, rt), __fmul_rn(k[8], r2));
+  out[2 * i] = __fadd_rn(__fmul_rn(k[0], u), k[2]);
+  out[2 * i + 1] = __fadd_rn(__fmul_rn(k[1], v), k[3]);
+}
+
+// dL/dX of project_to_2d_kernel's map given dL/d out, in double (one rounding, at the store).  With s = radial + tan,
+// A = gu x + gv y (gu = g0 f0, gv = g1 f1) and g_r2 = A dradial/dr2 + gu p0 + gv p1:
+// dL/dx = gu s + A p0 + 2 x g_r2, dL/dy = gv s + A p1 + 2 y g_r2, then through x = X/Z, y = Y/Z.
+__global__ void project_to_2d_backward_kernel(const float* __restrict__ x, long long n, const long long* __restrict__ seg,
+                                              const float* __restrict__ intr, int S, const float* __restrict__ g,
+                                              float* __restrict__ gx) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float* k = intr + 9 * seg_of(seg, S, i);
+  const double z = x[3 * i + 2], xx = x[3 * i] / z, yy = x[3 * i + 1] / z;
+  const double k0 = k[4], k1 = k[5], k2 = k[6], p0 = k[7], p1 = k[8];
+  const double r2 = xx * xx + yy * yy;
+  const double s = 1.0 + k0 * r2 + k1 * r2 * r2 + k2 * r2 * r2 * r2 + p0 * xx + p1 * yy;
+  const double dradial = k0 + 2.0 * k1 * r2 + 3.0 * k2 * r2 * r2;
+  const double gu = (double)g[2 * i] * (double)k[0], gv = (double)g[2 * i + 1] * (double)k[1];
+  const double A = gu * xx + gv * yy;
+  const double gr2 = A * dradial + gu * p0 + gv * p1;
+  const double dx = gu * s + A * p0 + 2.0 * xx * gr2, dy = gv * s + A * p1 + 2.0 * yy * gr2;
+  gx[3 * i] = (float)(dx / z);
+  gx[3 * i + 1] = (float)(dy / z);
+  gx[3 * i + 2] = (float)(-(dx * xx + dy * yy) / z);
+}
+
+// normalize_screen_coordinates per segment (main.py:97,101): frames of P points of F floats, channels 0 and 1
+// normalised with the segment's wh = {w, h/w} (double) as screen_norm_kernel does, the others copied.  from_image first
+// takes the point through image_coordinates and float32, the ground-truth round trip of prepare_data_h36m.py:119 and
+// main.py:101.
+__global__ void screen_norm_seg_kernel(const float* __restrict__ x, long long n_src, int P, int F,
+                                       const long long* __restrict__ src, const long long* __restrict__ dst,
+                                       const double* __restrict__ wh, int S, long long n_out, int from_image,
+                                       float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long per_frame = (long long)P * F;
+  if (i >= n_out * per_frame) return;
+  const long long f = i / per_frame;
+  const long long r = i - f * per_frame;
+  const int s = seg_of(dst, S, f);
+  const long long fs = src[s] + (f - dst[s]);
+  if (fs < 0 || fs >= n_src) return;
+  float v = x[fs * per_frame + r];
+  const int c = (int)(r % F);
+  if (c < 2) {
+    const double wd = wh[2 * s], off = c ? wh[2 * s + 1] : 1.0;
+    if (from_image) v = (float)(((double)v + off) * wd / 2.0);
+    v = (float)((double)__fmul_rn(__fdiv_rn(v, (float)wd), 2.f) - off);
+  }
+  out[i] = v;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -784,7 +924,8 @@ extern "C" int gast_chunk_gather_indexed(const float* poses_2d, const float* pos
 extern "C" int gast_keypoints_convert(const float* kpts, float* out, int32_t* valid, int32_t T, int32_t J_in, int32_t mode,
                                       void* stream) {
   if (!kpts || !out || T <= 0) return fail("gast_keypoints_convert: bad arguments");
-  if ((mode == 0 && J_in != 17) || (mode == 1 && J_in != 16) || (mode == 2 && J_in < 22) || mode < 0 || mode > 2)
+  if ((mode == 0 && J_in != 17) || (mode == 1 && J_in != 16) || (mode == 2 && J_in < 22) || (mode == 3 && J_in != 17) ||
+      mode < 0 || mode > 3)
     return fail("gast_keypoints_convert: mode %d does not take %d joints", mode, J_in);
   kpt_convert_kernel<<<cdiv(T, 128), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(kpts, out, valid, T, J_in, mode);
   CUDA_OK(cudaGetLastError());
@@ -806,6 +947,53 @@ extern "C" int gast_camera_to_world(const float* x, float* out, int64_t n_points
   if (!x || !out || !q || n_points <= 0) return fail("gast_camera_to_world: bad arguments");
   cam_to_world_kernel<<<cdiv(n_points, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       x, out, n_points, q[0], q[1], q[2], q[3], t ? t[0] : 0.f, t ? t[1] : 0.f, t ? t[2] : 0.f);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gast_world_to_camera(const float* x, int64_t n_src_frames, int32_t J, const int64_t* src_start,
+                                    const int64_t* dst_start, const float* qt, int32_t S, int64_t n_out_frames,
+                                    int32_t root_relative, float* out, void* stream) {
+  if (!x || !src_start || !dst_start || !qt || !out || n_src_frames <= 0 || J <= 0 || S <= 0 || n_out_frames <= 0)
+    return fail("gast_world_to_camera: bad arguments");
+  const long long n = (long long)n_out_frames * J;
+  world_to_camera_kernel<<<cdiv(n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      x, n_src_frames, J, reinterpret_cast<const long long*>(src_start), reinterpret_cast<const long long*>(dst_start), qt,
+      S, n_out_frames, root_relative ? 1 : 0, out);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gast_project_to_2d(const float* x, int64_t n_points, const int64_t* seg_start, const float* intrinsics,
+                                  int32_t S, float* out, void* stream) {
+  if (!x || !seg_start || !intrinsics || !out || n_points <= 0 || S <= 0) return fail("gast_project_to_2d: bad arguments");
+  project_to_2d_kernel<<<cdiv(n_points, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      x, n_points, reinterpret_cast<const long long*>(seg_start), intrinsics, S, out);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gast_project_to_2d_backward(const float* x, int64_t n_points, const int64_t* seg_start,
+                                           const float* intrinsics, int32_t S, const float* grad_out, float* grad_x,
+                                           void* stream) {
+  if (!x || !seg_start || !intrinsics || !grad_out || !grad_x || n_points <= 0 || S <= 0)
+    return fail("gast_project_to_2d_backward: bad arguments");
+  project_to_2d_backward_kernel<<<cdiv(n_points, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      x, n_points, reinterpret_cast<const long long*>(seg_start), intrinsics, S, grad_out, grad_x);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gast_normalize_screen_segments(const float* x, int64_t n_src_frames, int32_t P, int32_t F,
+                                              const int64_t* src_start, const int64_t* dst_start, const double* wh,
+                                              int32_t S, int64_t n_out_frames, int32_t from_image, float* out,
+                                              void* stream) {
+  if (!x || !src_start || !dst_start || !wh || !out || n_src_frames <= 0 || P <= 0 || F < 2 || S <= 0 || n_out_frames <= 0)
+    return fail("gast_normalize_screen_segments: bad arguments (F >= 2)");
+  const long long n = (long long)n_out_frames * P * F;
+  screen_norm_seg_kernel<<<cdiv(n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      x, n_src_frames, P, F, reinterpret_cast<const long long*>(src_start), reinterpret_cast<const long long*>(dst_start),
+      wh, S, n_out_frames, from_image ? 1 : 0, out);
   CUDA_OK(cudaGetLastError());
   return 0;
 }

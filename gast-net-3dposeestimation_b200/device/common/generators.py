@@ -8,7 +8,8 @@ protocol, but the sequences live concatenated in HBM (gast_b200.pipeline.DeviceS
 is one gather kernel (edge padding, horizontal flip, left/right swap: csrc/pipeline.cuh) that yields CUDA
 float32 tensors -- the reference fills float64 numpy buffers chunk by chunk in a Python loop and the
 training loop then casts and uploads them (main.py:219-223).  `UnchunkedGenerator` (generators.py:160-235)
-yields one padded (and, with augment, mirrored) sequence at a time, also as CUDA tensors.
+yields one padded (and, with augment, mirrored) sequence at a time, also as CUDA tensors.  Both take the
+sequences as numpy arrays or as CUDA tensors (gast_b200.dataset's fetch), the latter without a host round trip.
 """
 from itertools import zip_longest
 
@@ -116,6 +117,8 @@ class UnchunkedGenerator(object):
         self.augment = augment
 
     def _dev(self, a):
+        if isinstance(a, torch.Tensor) and a.is_cuda:                 # fetched on the device: no host round trip
+            return a.to(device=self.device, dtype=torch.float32).contiguous()
         return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float32)).to(self.device)
 
     def next_epoch(self):

@@ -32,7 +32,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_stream_snapshot_floats', 'gast_stream_move_workspace_bytes', 'gast_stream_export',
            'gast_stream_import', 'gast_chunk_gather', 'gast_keypoints_convert', 'gast_h36m_coco_format', 'gast_revise_kpts',
            'gast_revise_skes_workspace_bytes', 'gast_revise_skes', 'gast_revise_skes_real_time_workspace_bytes',
-           'gast_revise_skes_real_time', 'gast_normalize_screen', 'gast_camera_to_world',
+           'gast_revise_skes_real_time', 'gast_normalize_screen', 'gast_camera_to_world', 'gast_world_to_camera',
+           'gast_project_to_2d', 'gast_project_to_2d_backward', 'gast_normalize_screen_segments',
            'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_pose_metrics_workspace_bytes',
            'gast_pose_metrics', 'gast_adam_chunk', 'gast_adam_step', 'gast_chunk_gather_indexed',
            'gast_adam_step_table', 'gast_adam_step_indexed', 'gast_epoch_loss_accumulate',
@@ -242,6 +243,15 @@ def load():
     lib.gast_normalize_screen.restype = C.c_int
     lib.gast_camera_to_world.argtypes = [vp, vp, C.c_int64, fp, fp, vp]
     lib.gast_camera_to_world.restype = C.c_int
+    lib.gast_world_to_camera.argtypes = [vp, C.c_int64, C.c_int32, vp, vp, vp, C.c_int32, C.c_int64, C.c_int32, vp, vp]
+    lib.gast_world_to_camera.restype = C.c_int
+    lib.gast_project_to_2d.argtypes = [vp, C.c_int64, vp, vp, C.c_int32, vp, vp]
+    lib.gast_project_to_2d.restype = C.c_int
+    lib.gast_project_to_2d_backward.argtypes = [vp, C.c_int64, vp, vp, C.c_int32, vp, vp, vp]
+    lib.gast_project_to_2d_backward.restype = C.c_int
+    lib.gast_normalize_screen_segments.argtypes = [vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32, C.c_int64,
+                                                   C.c_int32, vp, vp]
+    lib.gast_normalize_screen_segments.restype = C.c_int
     lib.gast_mpjpe_workspace_bytes.argtypes = []
     lib.gast_mpjpe_workspace_bytes.restype = C.c_size_t
     lib.gast_mpjpe.argtypes = [vp, vp, C.c_int64, C.c_int32, vp, vp, C.c_float, vp, vp]

@@ -12,7 +12,7 @@ import torch
 from . import _lib as L
 from .engine import GastError, _check, _check_size, _cuda_f32, _ilist, _p, _stream
 
-KPT_COCO_H36M, KPT_MPII_H36M, KPT_COCO_H36M_TOE = 0, 1, 2
+KPT_COCO_H36M, KPT_MPII_H36M, KPT_COCO_H36M_TOE, KPT_COCO_HUMANEVA = 0, 1, 2, 3
 
 
 # ------------------------------------------------------------------------------------------------
@@ -21,21 +21,30 @@ KPT_COCO_H36M, KPT_MPII_H36M, KPT_COCO_H36M_TOE = 0, 1, 2
 class DeviceSequences(object):
     """All videos of a dataset split concatenated along time in HBM: poses_2d (sum T,J2,F2), poses_3d
     (sum T,J3,3), cameras (n,ncam) and the prefix frame offsets -- what ChunkedGenerator indexes into
-    (generators.py:64-66) once per batch on the host."""
+    (generators.py:64-66) once per batch on the host.  Lists of CUDA tensors (views included, as
+    gast_b200.dataset's fetch returns them) are concatenated on the device."""
 
     def __init__(self, poses_2d, poses_3d=None, cameras=None, device='cuda'):
         lens = [int(p.shape[0]) for p in poses_2d]
         self.n_seq = len(lens)
         self.lengths = lens
         self.seq_start = torch.tensor(np.concatenate([[0], np.cumsum(lens)]), dtype=torch.int64, device=device)
-        self.poses_2d = torch.as_tensor(np.concatenate([np.asarray(p, dtype=np.float32) for p in poses_2d], 0)).to(device)
+        self.poses_2d = _joined(poses_2d, torch.cat, np.concatenate, device)
         self.poses_3d = None
         if poses_3d is not None:
             assert [int(p.shape[0]) for p in poses_3d] == lens
-            self.poses_3d = torch.as_tensor(np.concatenate([np.asarray(p, dtype=np.float32) for p in poses_3d], 0)).to(device)
+            self.poses_3d = _joined(poses_3d, torch.cat, np.concatenate, device)
         self.cameras = None
         if cameras is not None:
-            self.cameras = torch.as_tensor(np.stack([np.asarray(c, dtype=np.float32) for c in cameras], 0)).to(device)
+            self.cameras = _joined(cameras, torch.stack, np.stack, device)
+
+
+def _joined(arrays, join_t, join_np, device):
+    """the arrays joined along a new or the first axis as one float32 tensor on `device`: CUDA tensors on the device,
+    anything else on the host and uploaded once"""
+    if all(isinstance(a, torch.Tensor) and a.is_cuda for a in arrays):
+        return join_t([a.to(device=device, dtype=torch.float32) for a in arrays], 0)
+    return torch.as_tensor(join_np([np.asarray(a, dtype=np.float32) for a in arrays], 0)).to(device)
 
 
 def chunk_gather(seqs, pairs, chunk_length, pad, causal_shift=0, kps_left=None, kps_right=None, joints_left=None,
@@ -104,12 +113,13 @@ def chunk_gather_indexed(seqs, pairs, batch, B, batch_stride, chunk_length, pad,
 # N3: keypoint formats, screen normalisation, camera -> world
 # ------------------------------------------------------------------------------------------------
 def keypoints_convert(kpts, mode):
-    """tools/mpii_coco_h36m.py: (T,J_in,2) -> ((T,17|19,2), valid mask (T,) int32)."""
+    """tools/mpii_coco_h36m.py, and HumanEva's COCO -> 15 joints (main.py:80-95): (T,J_in,2) -> ((T,17|19|15,2), valid
+    mask (T,) int32)."""
     k = _cuda_f32(kpts, 'keypoints_convert')
     if k.dim() != 3 or k.shape[-1] != 2:
         raise GastError('keypoints_convert: (T,J,2) expected')
     T, Jin = int(k.shape[0]), int(k.shape[1])
-    Jo = 19 if mode == KPT_COCO_H36M_TOE else 17
+    Jo = {KPT_COCO_H36M_TOE: 19, KPT_COCO_HUMANEVA: 15}.get(mode, 17)
     out = torch.empty((T, Jo, 2), dtype=torch.float32, device=k.device)
     valid = torch.empty((T,), dtype=torch.int32, device=k.device)
     with torch.cuda.device(k.device):
@@ -140,6 +150,97 @@ def camera_to_world(x, R, t=0):
     with torch.cuda.device(x.device):
         _check(L.load().gast_camera_to_world(_p(x), _p(out), x.numel() // 3, q, tt, C.c_void_p(_stream(x.device))),
                'gast_camera_to_world')
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# Dataset preparation (main.py:24-104, data/prepare_data_h36m.py:113-121): segmented launches.  Output segment s holds
+# rows dst_start[s] .. dst_start[s+1]-1 taken from source rows src_start[s] ..; the tables are CUDA tensors (int64
+# offsets, float32 / float64 parameters), so a launch reads nothing from the host.
+# ------------------------------------------------------------------------------------------------
+def _table(t, dtype, shape, dev, what):
+    if not isinstance(t, torch.Tensor) or t.dtype != dtype or tuple(t.shape) != tuple(shape) or t.device != dev \
+            or not t.is_contiguous():
+        raise GastError('%s: a contiguous %s table %s on %s expected, got %s' % (
+            what, dtype, tuple(shape), dev, (t.dtype, tuple(t.shape), t.device) if isinstance(t, torch.Tensor) else type(t)))
+    return t
+
+
+def world_to_camera_segments(x, src_start, dst_start, qt, n_out, root_relative=False):
+    """world_to_camera (camera.py:22-24) of frames x (n_src,J,3) -> (n_out,J,3): segment s from its own source frames
+    with qt[s] = {orientation[4], translation[3]}; root_relative also does main.py:33 (pos[:, 1:] -= pos[:, :1])."""
+    x = _cuda_f32(x, 'world_to_camera')
+    if x.dim() != 3 or x.shape[-1] != 3:
+        raise GastError('world_to_camera: frames (n,J,3) expected, got %s' % (tuple(x.shape),))
+    S, dev = int(qt.shape[0]) if isinstance(qt, torch.Tensor) else 0, x.device
+    _table(qt, torch.float32, (S, 7), dev, 'world_to_camera')
+    _table(src_start, torch.int64, (S,), dev, 'world_to_camera')
+    _table(dst_start, torch.int64, (S + 1,), dev, 'world_to_camera')
+    out = torch.empty((int(n_out), int(x.shape[1]), 3), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _check(L.load().gast_world_to_camera(_p(x), int(x.shape[0]), int(x.shape[1]), _p(src_start), _p(dst_start), _p(qt),
+                                             S, int(n_out), 1 if root_relative else 0, _p(out), C.c_void_p(_stream(dev))),
+               'gast_world_to_camera')
+    return out
+
+
+def world_to_camera(x, R, t):
+    """camera.py:22-24 with one rotation R (4,) and translation t (3,) for every point of x (...,3); R and t may be
+    host arrays or tensors on any device"""
+    x = _cuda_f32(x, 'world_to_camera')
+    assert x.shape[-1] == 3
+    dev = x.device
+    qt = torch.cat([torch.as_tensor(R, dtype=torch.float32).reshape(4).to(dev),
+                    torch.as_tensor(t, dtype=torch.float32).reshape(3).to(dev)]).reshape(1, 7)
+    n = x.numel() // 3
+    offs = torch.tensor([0, 0, n], dtype=torch.int64, device=dev)           # src_start = {0}, dst_start = {0, n}
+    return world_to_camera_segments(x.reshape(n, 1, 3), offs[:1], offs[1:], qt, n).reshape(x.shape)
+
+
+def project_to_2d_segments(x, seg_start, intrinsics, grad_out=None):
+    """project_to_2d (camera.py:31-62) of the points x (...,3) -> (...,2); the points seg_start[s] .. seg_start[s+1]-1
+    (in points) use intrinsics[s] (9,).  With grad_out (...,2) returns dL/dx (...,3) instead."""
+    x = _cuda_f32(x, 'project_to_2d')
+    if x.shape[-1] != 3:
+        raise GastError('project_to_2d: points (...,3) expected, got %s' % (tuple(x.shape),))
+    dev, n = x.device, x.numel() // 3
+    S = int(intrinsics.shape[0]) if isinstance(intrinsics, torch.Tensor) else 0
+    _table(intrinsics, torch.float32, (S, 9), dev, 'project_to_2d')
+    _table(seg_start, torch.int64, (S + 1,), dev, 'project_to_2d')
+    lib = L.load()
+    with torch.cuda.device(dev):
+        if grad_out is None:
+            out = torch.empty(tuple(x.shape[:-1]) + (2,), dtype=torch.float32, device=dev)
+            _check(lib.gast_project_to_2d(_p(x), n, _p(seg_start), _p(intrinsics), S, _p(out), C.c_void_p(_stream(dev))),
+                   'gast_project_to_2d')
+        else:
+            g = _cuda_f32(grad_out, 'project_to_2d backward')
+            if tuple(g.shape) != tuple(x.shape[:-1]) + (2,):
+                raise GastError('project_to_2d backward: grad (...,2) of the points expected, got %s' % (tuple(g.shape),))
+            out = torch.empty_like(x)
+            _check(lib.gast_project_to_2d_backward(_p(x), n, _p(seg_start), _p(intrinsics), S, _p(g), _p(out),
+                                                   C.c_void_p(_stream(dev))), 'gast_project_to_2d_backward')
+    return out
+
+
+def normalize_screen_segments(x, src_start, dst_start, wh, n_out, from_image=False):
+    """normalize_screen_coordinates (camera.py:8-12) of frames x (n_src,P,F>=2) -> (n_out,P,F): channels 0 and 1 with
+    segment s's wh[s] = {w, h/w} (float64), the others copied.  from_image first takes the points through
+    image_coordinates and float32 (the ground-truth keypoints' round trip)."""
+    x = _cuda_f32(x, 'normalize_screen_segments')
+    if x.dim() != 3 or x.shape[-1] < 2:
+        raise GastError('normalize_screen_segments: frames (n,P,F>=2) expected, got %s' % (tuple(x.shape),))
+    S = int(wh.shape[0]) if isinstance(wh, torch.Tensor) else 0
+    dev = x.device
+    _table(wh, torch.float64, (S, 2), dev, 'normalize_screen_segments')
+    _table(src_start, torch.int64, (S,), dev, 'normalize_screen_segments')
+    _table(dst_start, torch.int64, (S + 1,), dev, 'normalize_screen_segments')
+    P, F = int(x.shape[1]), int(x.shape[2])
+    out = torch.empty((int(n_out), P, F), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _check(L.load().gast_normalize_screen_segments(_p(x), int(x.shape[0]), P, F, _p(src_start), _p(dst_start), _p(wh),
+                                                       S, int(n_out), 1 if from_image else 0, _p(out),
+                                                       C.c_void_p(_stream(dev))), 'gast_normalize_screen_segments')
     return out
 
 

@@ -466,7 +466,8 @@ int gast_chunk_gather(const float* poses_2d, const float* poses_3d, const float*
                       float* batch_2d, float* batch_3d, float* batch_cam, void* stream);
 
 /* tools/mpii_coco_h36m.py: mode 0 = coco_h36m (T,17,2)->(T,17,2) (:20-48), 1 = mpii_h36m (T,16,2)->(T,17,2)
- * (:51-59), 2 = coco_h36m_toe_format (T,J_in>=22,2)->(T,19,2) (:62-78).  valid (T) int32, may be null:
+ * (:51-59), 2 = coco_h36m_toe_format (T,J_in>=22,2)->(T,19,2) (:62-78), 3 = HumanEva's COCO -> 15 joints
+ * (T,17,2)->(T,15,2) (main.py:80-95).  valid (T) int32, may be null:
  * 1 where the frame's coordinate sum is non-zero (the mask the reference takes np.where of). */
 int gast_keypoints_convert(const float* kpts, float* out, int32_t* valid, int32_t T, int32_t J_in, int32_t mode,
                            void* stream);
@@ -518,6 +519,33 @@ int gast_normalize_screen(const float* x, float* out, int64_t n_points, float w,
 /* common/camera.py:27-28 camera_to_world with one rotation for all points: qort(q, x) + t
  * (common/quaternion.py:4-18).  q[4], t[3] (host; t may be null = 0). */
 int gast_camera_to_world(const float* x, float* out, int64_t n_points, const float* q, const float* t, void* stream);
+
+/* Dataset preparation (main.py:24-104 load_data, data/prepare_data_h36m.py:113-121) as segmented launches, bit-identical
+ * to the reference for float32 input.  Output segment s (s < S) holds rows dst_start[s] .. dst_start[s+1]-1, taken from
+ * source rows src_start[s] ..; dst_start (S+1, ascending from 0) and src_start (S) are int64 device arrays, as are the
+ * per-segment parameter tables.  An output row whose source row lies outside the input is left unwritten.
+ *
+ * gast_world_to_camera: world_to_camera (camera.py:22-24) of frames of J points x (n_src_frames,J,3) -> out
+ *   (n_out_frames,J,3); qt (S,7) float = {orientation[4], translation[3]} per segment.  root_relative subtracts each
+ *   frame's joint 0 from its joints 1.. (main.py:33).  torch's CPU cross product rounds each component as
+ *   fma(a1, b2, -(a2*b1)); the kernel does the same.
+ * gast_project_to_2d: project_to_2d (camera.py:31-62) of n_points camera-space points x (n,3) -> out (n,2); here the
+ *   segments count points (seg_start, S+1) and intrinsics (S,9) = {f[2], c[2], k[3], p[2]} per segment.
+ * gast_project_to_2d_backward: grad_x (n,3) = dL/dx given grad_out (n,2) = dL/dout, evaluated in double.
+ * gast_normalize_screen_segments: normalize_screen_coordinates (camera.py:8-12) of frames of P points of F >= 2 floats,
+ *   x (n_src_frames,P,F) -> out (n_out_frames,P,F): channels 0 and 1 with wh (S,2) double = {w, h/w} per segment,
+ *   the others copied.  from_image = 1 takes each point through image_coordinates (camera.py:15-19) and float32
+ *   first: the ground-truth keypoints' round trip. */
+int gast_world_to_camera(const float* x, int64_t n_src_frames, int32_t J, const int64_t* src_start,
+                         const int64_t* dst_start, const float* qt, int32_t S, int64_t n_out_frames, int32_t root_relative,
+                         float* out, void* stream);
+int gast_project_to_2d(const float* x, int64_t n_points, const int64_t* seg_start, const float* intrinsics, int32_t S,
+                       float* out, void* stream);
+int gast_project_to_2d_backward(const float* x, int64_t n_points, const int64_t* seg_start, const float* intrinsics,
+                                int32_t S, const float* grad_out, float* grad_x, void* stream);
+int gast_normalize_screen_segments(const float* x, int64_t n_src_frames, int32_t P, int32_t F, const int64_t* src_start,
+                                   const int64_t* dst_start, const double* wh, int32_t S, int64_t n_out_frames,
+                                   int32_t from_image, float* out, void* stream);
 
 /* common/loss.py:5-11 mpjpe: *loss = mean_i ||pred_i - target_i|| over n_points rows of D (<= 4) coordinates;
  * when dpred is not null it receives grad_scale * d loss / d pred (the backward of the same pass).
