@@ -1508,3 +1508,8 @@ extern "C" int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int3
 // callers / data formats either side of the forward (SURVEY.md §8f N1-N3)
 // ------------------------------------------------------------------------------------------
 #include "pipeline.cuh"
+
+// ------------------------------------------------------------------------------------------
+// the reconstruction's animation frames (DESIGN.md §8.5)
+// ------------------------------------------------------------------------------------------
+#include "render.cuh"

@@ -35,7 +35,8 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_revise_skes_real_time', 'gast_normalize_screen', 'gast_camera_to_world', 'gast_world_to_camera',
            'gast_project_to_2d', 'gast_project_to_2d_backward', 'gast_normalize_screen_segments',
            'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_pose_metrics_workspace_bytes',
-           'gast_pose_metrics', 'gast_adam_chunk', 'gast_adam_step', 'gast_chunk_gather_indexed',
+           'gast_pose_metrics', 'gast_render_geometry', 'gast_render_frames', 'gast_downsample_frames',
+           'gast_adam_chunk', 'gast_adam_step', 'gast_chunk_gather_indexed',
            'gast_adam_step_table', 'gast_adam_step_indexed', 'gast_epoch_loss_accumulate',
            'gast_last_error', 'gast_version']
 
@@ -263,6 +264,16 @@ def load():
     lib.gast_pose_metrics.argtypes = [vp, vp, C.c_int64, C.c_int32, C.POINTER(C.c_int64), C.c_int32, fp, C.c_int32,
                                       C.c_int32, C.c_int32, vp, vp, vp, C.c_size_t, vp]
     lib.gast_pose_metrics.restype = C.c_int
+    lib.gast_render_geometry.argtypes = [C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float,
+                                         C.c_float, C.c_int32, fp]
+    lib.gast_render_geometry.restype = C.c_int
+    lib.gast_render_frames.argtypes = [vp, C.c_int64, C.c_int32, C.c_int32, vp, C.c_int32, C.c_int64, vp, C.c_int64,
+                                       C.c_int32, C.c_int32, ip, C.POINTER(C.c_uint8), ip, C.c_int32, C.c_int32,
+                                       C.c_int32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32,
+                                       C.c_int64, C.c_int32, vp, vp]
+    lib.gast_render_frames.restype = C.c_int
+    lib.gast_downsample_frames.argtypes = [vp, C.c_int64, C.c_int64, C.c_int32, C.c_int32, vp, vp]
+    lib.gast_downsample_frames.restype = C.c_int
     lib.gast_adam_chunk.argtypes = []
     lib.gast_adam_chunk.restype = C.c_int32
     lib.gast_adam_step.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,

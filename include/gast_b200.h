@@ -574,6 +574,38 @@ int gast_pose_metrics(const float* pred, const float* target, int64_t N, int32_t
                       const float* thresholds, int32_t n_thr, int32_t zero_root, int32_t procrustes, double* rows,
                       float* dist, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Animation frames of the reconstruction (tools/vis_h36m.py:58-249 and tools/visualization.py:84-227
+ * render_animation), rasterised.  Frame f < F of out (F, S, S*(1+P), 3) uint8 on the device is source frame f0+f:
+ * the input panel (S x S) and then P = (flags & GAST_RENDER_SHARED_PANEL ? 1 : n_pose) 3D panels.
+ *   keypoints (n_kp_frames, M, J, 2) float32 in image pixels; poses (n_pose, n_pose_frames, J, 3) float32 world
+ *   coordinates; video (n_video_frames, Hin, Win, 3) uint8 or null (a black Hin x Win image); all on the device.
+ *   parents (J), colors (J, 3) RGB of the bone ending at each joint, right (n_right): host arrays.  J <= 32,
+ *   M*J <= 256, n_pose <= 8 (shared: n_pose*J <= 256).  Bones j = 1 .. n_bones-1 with parents[j] >= 0 are drawn.
+ *   flags: GAST_RENDER_SHARED_PANEL draws every pose in one panel with x, y limits +-radius (else +-radius/2; z in
+ *   [0, radius]); GAST_RENDER_FOLLOW_ROOT centres each panel's x, y limits on its pose's joint 0 at every frame
+ *   (visualization.py:166-167); GAST_RENDER_BONES_2D draws the 2D bones (pink) under the joint discs.
+ *   View: elevation elev and azimuth azim in degrees, eye distance dist in units of the axis box (ax.dist).
+ * Each pixel is written by one thread, with no atomics: the bytes repeat from call to call, and a frame's bytes do not
+ * depend on f0 and F.  Formulas in DESIGN.md §8.5.
+ * gast_render_geometry: the call's geometry as float32 geo[20] on the host: [0..11] the 3D panels' rows
+ *   (sx, sy, dz) = M (x, y, z, 1), [12..14] the input image's scale and offsets (ox, oy), [15..18] the coverage
+ *   edges of the 3D bones, the 2D bones, the disc fill and the disc edge, [19] S/2.
+ * gast_downsample_frames: downsample_tensor (vis_h36m.py:53-55) of x (n_in_frames, frame_elems) -> out
+ *   (n_in_frames / factor, frame_elems) on the device; dtype 0 = float32 (numpy's float32 mean), 1 = uint8 (numpy's
+ *   mean then astype('uint8')). */
+#define GAST_RENDER_SHARED_PANEL 1
+#define GAST_RENDER_FOLLOW_ROOT 2
+#define GAST_RENDER_BONES_2D 4
+int gast_render_geometry(int32_t S, float dpi, int32_t Hin, int32_t Win, float elev, float azim, float radius,
+                         float dist, int32_t shared, float* geo);
+int gast_render_frames(const float* keypoints, int64_t n_kp_frames, int32_t M, int32_t J, const float* poses,
+                       int32_t n_pose, int64_t n_pose_frames, const uint8_t* video, int64_t n_video_frames, int32_t Hin,
+                       int32_t Win, const int32_t* parents, const uint8_t* colors, const int32_t* right, int32_t n_right,
+                       int32_t n_bones, int32_t S, float dpi, float elev, float azim, float radius, float dist,
+                       int32_t flags, int64_t f0, int32_t F, uint8_t* out, void* stream);
+int gast_downsample_frames(const void* x, int64_t n_in_frames, int64_t frame_elems, int32_t factor, int32_t dtype,
+                           void* out, void* stream);
+
 /* optim.Adam(amsgrad=True) (trainval.py:78,162-164) for every parameter in one launch.  table (n_chunks,4)
  * int64 on the device: {param pointer, grad pointer, offset into the flat state buffers, count <=
  * gast_adam_chunk()}.  max_exp_avg_sq null = plain Adam.  step = 1 for the first update. */
