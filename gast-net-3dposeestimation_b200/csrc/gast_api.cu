@@ -1513,3 +1513,8 @@ extern "C" int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int3
 // the reconstruction's animation frames (DESIGN.md §8.5)
 // ------------------------------------------------------------------------------------------
 #include "render.cuh"
+
+// ------------------------------------------------------------------------------------------
+// the 2D pose net's person crops and heatmap decode (DESIGN.md §8.6)
+// ------------------------------------------------------------------------------------------
+#include "keypoints2d.cuh"

@@ -606,6 +606,28 @@ int gast_render_frames(const float* keypoints, int64_t n_kp_frames, int32_t M, i
 int gast_downsample_frames(const void* x, int64_t n_in_frames, int64_t frame_elems, int32_t factor, int32_t dtype,
                            void* out, void* stream);
 
+/* The 2D pose net's input crops and its heatmap decode (lib/pose/hrnet/pose_estimation/gen_kpts.py:234-256).
+ * gast_person_crops: PreProcess (lib/pose/hrnet/lib/utils/utilitys.py:140-170) of n boxes.  Record r crops frame
+ *   frame_index[r] of frames (n_frames, H, W, 3) uint8 (BGR as cv2 reads it; RGB with GAST_CROP_RGB_INPUT) by the
+ *   forward 2x3 matrix forward_mats[6r..6r+5] (what cv2.warpAffine receives) into out (n, 3, out_h, out_w) float32:
+ *   cv2.warpAffine(frame, M, (out_w, out_h), flags=INTER_LINEAR) with a constant 0 border, ToTensor and
+ *   Normalize(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225]) bit for bit, the statistics applied to the BGR
+ *   planes in order.  Planes in the frame's BGR order, or with GAST_CROP_NET_ORDER in the order the net receives
+ *   (inputs[:, [2, 1, 0]]).  A frame index outside [0, n_frames) crops a black frame.  Frame and crop sides <= 32767.
+ * gast_heatmap_decode: get_final_preds (lib/pose/hrnet/lib/utils/inference.py:21-82) of heatmaps (n, J, hh, hw)
+ *   float32 with the inverse (heatmap -> frame) 2x3 matrices inverse_mats (n, 6) double: preds (n, J, 2) and maxvals
+ *   (n, J, 1) float32, bit for bit; post_process 1 = TEST.POST_PROCESS (the quarter-pixel shift).  J <= 32, sides <=
+ *   256.
+ * Device pointers, the caller's stream, no allocation or synchronisation; calls repeat bit for bit and a record's
+ * result does not depend on the others.  Formulas in DESIGN.md §8.6. */
+#define GAST_CROP_RGB_INPUT 1
+#define GAST_CROP_NET_ORDER 2
+int gast_person_crops(const uint8_t* frames, int64_t n_frames, int32_t H, int32_t W, const int32_t* frame_index,
+                      const double* forward_mats, int32_t n, int32_t out_w, int32_t out_h, int32_t flags, float* out,
+                      void* stream);
+int gast_heatmap_decode(const float* heatmaps, const double* inverse_mats, int32_t n, int32_t J, int32_t hh,
+                        int32_t hw, int32_t post_process, float* preds, float* maxvals, void* stream);
+
 /* optim.Adam(amsgrad=True) (trainval.py:78,162-164) for every parameter in one launch.  table (n_chunks,4)
  * int64 on the device: {param pointer, grad pointer, offset into the flat state buffers, count <=
  * gast_adam_chunk()}.  max_exp_avg_sq null = plain Adam.  step = 1 for the first update. */
