@@ -1518,3 +1518,8 @@ extern "C" int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int3
 // the 2D pose net's person crops and heatmap decode (DESIGN.md §8.6)
 // ------------------------------------------------------------------------------------------
 #include "keypoints2d.cuh"
+
+// ------------------------------------------------------------------------------------------
+// the person detector's letterbox and post-processing (DESIGN.md §8.7)
+// ------------------------------------------------------------------------------------------
+#include "detect.cuh"

@@ -36,7 +36,7 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_project_to_2d', 'gast_project_to_2d_backward', 'gast_normalize_screen_segments',
            'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_pose_metrics_workspace_bytes',
            'gast_pose_metrics', 'gast_render_geometry', 'gast_render_frames', 'gast_downsample_frames',
-           'gast_person_crops', 'gast_heatmap_decode',
+           'gast_person_crops', 'gast_heatmap_decode', 'gast_letterbox', 'gast_person_detections',
            'gast_adam_chunk', 'gast_adam_step', 'gast_chunk_gather_indexed',
            'gast_adam_step_table', 'gast_adam_step_indexed', 'gast_epoch_loss_accumulate',
            'gast_last_error', 'gast_version']
@@ -280,6 +280,12 @@ def load():
     lib.gast_person_crops.restype = C.c_int
     lib.gast_heatmap_decode.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp]
     lib.gast_heatmap_decode.restype = C.c_int
+    lib.gast_letterbox.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                   vp, vp]
+    lib.gast_letterbox.restype = C.c_int
+    lib.gast_person_detections.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.c_float, C.c_float,
+                                           C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp]
+    lib.gast_person_detections.restype = C.c_int
     lib.gast_adam_chunk.argtypes = []
     lib.gast_adam_chunk.restype = C.c_int32
     lib.gast_adam_step.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,

@@ -628,6 +628,31 @@ int gast_person_crops(const uint8_t* frames, int64_t n_frames, int32_t H, int32_
 int gast_heatmap_decode(const float* heatmaps, const double* inverse_mats, int32_t n, int32_t J, int32_t hh,
                         int32_t hw, int32_t post_process, float* preds, float* maxvals, void* stream);
 
+/* The person detector's input and output handling (lib/detector/yolov3/human_detector.py:106-157).
+ * gast_letterbox: preprocess.prep_image (lib/detector/yolov3/preprocess.py:9-38) of n frames (n, H, W, 3) uint8 (BGR
+ *   as cv2 reads them; RGB with GAST_LETTERBOX_RGB_INPUT) into out (n, 3, D, D) float32 RGB planes: cv2.resize(
+ *   INTER_CUBIC) to new_w x new_h (OpenCV's own path, not IPP's), pasted at ((D - new_w) / 2, (D - new_h) / 2) into a
+ *   canvas of 128, each value u8 / 255 correctly rounded.  new_w = int(W * min(D / W, D / H)) as the reference's double
+ *   expression gives it, new_h likewise, 1 .. D.  Sides <= 32767; D a multiple of 32 above 32.
+ * gast_person_detections: write_results(pred, confidence, 80, nms=True, nms_conf=nms_thresh, det_hm=True)
+ *   (lib/detector/yolov3/util.py:107-225) of each frame's predictions (n, N, 85) float32 (Darknet.forward's output),
+ *   N = 3 * sum((D / s)^2, s = 32, 16, 8), then yolo_human_det's rescale to frame_sizes (n, 2) int32 (W, H), clamp to
+ *   the frame and round(v, 2): boxes (n, max_det, 4), scores (n, max_det) (the objectness) in the reference's order,
+ *   zero past the count; counts (n) the number of survivors, which may exceed max_det.  GAST_DETECT_RAW leaves the
+ *   boxes as write_results' corners in the D x D input.  Optional: max_conf (n, max_det) write_results' class score
+ *   column; persons (n) the rows that reach its person filter (its early return when 0).  Objectness ties keep the
+ *   lower prediction index first.  N * 9 bytes of shared memory (D <= 640).
+ * Device pointers, the caller's stream, no allocation or synchronisation; calls repeat bit for bit and a frame's
+ * result does not depend on the others.  Formulas in DESIGN.md §8.7. */
+#define GAST_LETTERBOX_RGB_INPUT 1
+#define GAST_DETECT_RAW 1
+int gast_letterbox(const uint8_t* frames, int32_t n, int32_t H, int32_t W, int32_t D, int32_t new_w, int32_t new_h,
+                   int32_t flags, float* out, void* stream);
+int gast_person_detections(const float* predictions, int32_t n, int32_t N, int32_t attrs, int32_t D,
+                           const int32_t* frame_sizes, float confidence, float nms_thresh, int32_t max_det,
+                           int32_t flags, float* boxes, float* scores, int32_t* counts, float* max_conf,
+                           int32_t* persons, void* stream);
+
 /* optim.Adam(amsgrad=True) (trainval.py:78,162-164) for every parameter in one launch.  table (n_chunks,4)
  * int64 on the device: {param pointer, grad pointer, offset into the flat state buffers, count <=
  * gast_adam_chunk()}.  max_exp_avg_sq null = plain Adam.  step = 1 for the first update. */
