@@ -125,7 +125,6 @@ struct gast_handle {
   size_t ev_used = 0;
   int fpt = 0;
   int sm_count = 132;
-  float* loss_scratch = nullptr;   // shrink+mpjpe: SHL_MAXBLOCKS double partials | ticket (zero-initialised, reset by the kernel)
   // test-only launch audits (gast_debug_set_gemm_audit, gast_debug_set_kernel_audit): called around every launch_gemm,
   // and every expand, row-dot, attention-mix and shrink launch, outside graph capture
   AuditHook<gast_gemm_audit> gemm_audit;
@@ -296,7 +295,6 @@ extern "C" int gast_create(gast_t** out, const gast_cfg* cfg) {
       nd *= fw;
     }
     rc |= dalloc(h, &h->We, (size_t)C * cfg->filter_widths[0] * cfg->in_features) | dalloc(h, &h->be, C);
-    rc |= dalloc(h, &h->loss_scratch, 2 * 1024 + 4);   // shrink+mpjpe partials and ticket (SHL_MAXBLOCKS doubles + 1 word)
   } else {
     h->blocks.resize(1);
     const int C = cfg->channels;
@@ -1076,15 +1074,17 @@ static int run_stage(gast_handle* h, cudaStream_t st, const StageConsts& s, long
   return launch_gemm(h, st, EPI_PLAIN, p, &s.tc_1);
 }
 
-// shrink (gast_net.py:99): X (rows, C << L) -> y (rows, 3); with a target also the mpjpe of y into *loss
+// shrink (gast_net.py:99): X (rows, C << L) -> y (rows, 3); with a target also the mpjpe of y into *loss, its block
+// partials and ticket in `scratch` (LOSS_SCRATCH_FLOATS of the call's workspace, ModelBufs::loss)
 static int launch_shrink(gast_handle* h, cudaStream_t st, const float* X, float* y, long long rows, const float* target,
-                         float* loss) {
+                         float* loss, float* scratch = nullptr) {
   Lookup Lk{h};
   const int Cl = h->cfg.channels << h->cfg.num_stages;
   const float* ws = Lk.get("shrink.weight", (int64_t)3 * Cl);
   if (!Lk.ok) return 1;
-  static_assert(SHL_MAXBLOCKS == 1024, "loss_scratch is sized for 1024 block partials");
-  if (target && !h->loss_scratch) return fail("gast_forward_mpjpe: handle has no loss scratch");
+  if (target && !scratch) return fail("gast_forward_mpjpe: no loss scratch in the workspace");
+  // a fresh workspace is not zeroed: clear the ticket on the call's stream (a captured graph replays this memset too)
+  if (target) CUDA_OK(cudaMemsetAsync(scratch + 2 * SHL_MAXBLOCKS, 0, sizeof(unsigned), st));
   auto fill = [&](gast_kernel_audit& d) {
     d.kind = target ? KA_SHRINK_MPJPE : KA_SHRINK;
     d.in_type = act_f16(h); d.out_type = h->act_dtype == GAST_F16; d.x = X; d.Ws = ws; d.target = target;
@@ -1093,8 +1093,8 @@ static int launch_shrink(gast_handle* h, cudaStream_t st, const float* X, float*
   return kernel_audited(h, st, fill, [&] {
     TimedLaunch tl(h, st, LK_SHRINK);
     if (target) {
-      double* partial = reinterpret_cast<double*>(h->loss_scratch);
-      unsigned* ticket = reinterpret_cast<unsigned*>(h->loss_scratch + 2 * SHL_MAXBLOCKS);
+      double* partial = reinterpret_cast<double*>(scratch);
+      unsigned* ticket = reinterpret_cast<unsigned*>(scratch + 2 * SHL_MAXBLOCKS);
       const unsigned nb = (unsigned)std::min<long long>(SHL_MAXBLOCKS, (rows + 7) / 8);
       if (act_f16(h))   // the fp16 precision (a half model refuses the mpjpe forward): fp16 X, float32 y
         shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws, y, rows, Cl, target,
@@ -1120,7 +1120,11 @@ struct ModelBufs {
   float* act[2];
   float* tmp;
   BlockBufs bb;
+  float* loss;   // gast_forward_mpjpe's SHL_MAXBLOCKS double partials and ticket: in the workspace, so that calls on
+                 // distinct workspaces never share them
 };
+
+constexpr size_t LOSS_SCRATCH_FLOATS = 2 * SHL_MAXBLOCKS + 4;
 
 static int plan_model(const gast_handle* h, int B, int T, int strided_now, Arena& a, ModelBufs* mb, Geometry* g) {
   if (geometry(h, T, strided_now, g)) return 1;
@@ -1143,6 +1147,7 @@ static int plan_model(const gast_handle* h, int B, int T, int strided_now, Arena
   mb->act[0] = a.take(act); mb->act[1] = a.take(act);
   mb->tmp = a.take(tmp);
   mb->bb.XY = a.take(xy); mb->bb.L = a.take(l); mb->bb.AB = a.take32(ab); mb->bb.Y = a.take(l); mb->bb.Gl = a.take(l);
+  mb->loss = a.take32(LOSS_SCRATCH_FLOATS);
   return 0;
 }
 
@@ -1201,7 +1206,7 @@ static int model_forward(gast_handle* h, cudaStream_t st, const float* x, float*
     F = Fn;
   }
   // output is already (B, T_out, J, 3)
-  if (launch_shrink(h, st, mb.act[cur], y, F * J, target, loss)) return 1;
+  if (launch_shrink(h, st, mb.act[cur], y, F * J, target, loss, mb.loss)) return 1;
   CUDA_OK(cudaGetLastError());
   return 0;
 }

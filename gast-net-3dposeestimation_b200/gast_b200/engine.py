@@ -4,7 +4,9 @@ For each module instance (and device) the engine keeps one C handle.  The handle
 the module's own parameter/buffer storage (`gast_bind`, no copies), so optimiser steps and
 `load_state_dict` are seen; derived constants are refreshed (`gast_prepare`) whenever a
 tensor's (data_ptr, _version) signature changes.  torch provides device memory (outputs and
-a cached workspace from the caching allocator) and the current CUDA stream -- plumbing only.
+each call's workspace from the caching allocator) and the current CUDA stream -- plumbing only.  Every call orders all of
+its work on the current stream and keeps no device buffer after it returns, so calls on several streams and inside a
+user's CUDA graph capture behave as torch's own ops do.
 
 No fallback: CPU tensors, a missing library or an unsupported mode raise.
 """
@@ -208,7 +210,6 @@ class _Handle(object):
         self.h = C.c_void_p()
         _check(lib.gast_create(C.byref(self.h), C.byref(cfg)), 'gast_create')
         self.sig = None
-        self.ws = None
         self.core = None
         self.precision = 0
         self.train_precision = 0
@@ -279,12 +280,13 @@ class _Handle(object):
         self.sig = None
 
     def forward(self, x, y, B, T, strided_now, stream, target=None, loss=None):
-        """gast_forward, or with a target gast_forward_mpjpe, on the handle's grow-only workspace self.ws"""
+        """gast_forward, or with a target gast_forward_mpjpe, on a workspace of the call's own from the caching
+        allocator, as the chunked forward, the backward and training take theirs.  It is freed to the current stream
+        `stream` when the call returns, and the allocator hands it only to later work of that stream (or keeps it in
+        the private pool of a graph being captured), so no call in flight on another stream or in a graph shares it."""
         need = _check_size(self.lib.gast_workspace_bytes(self.h, B, T, strided_now), 'gast_workspace_bytes')
-        if self.ws is None or self.ws.numel() < need:
-            self.ws = None
-            self.ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-        tail = (B, T, strided_now, _p(self.ws), self.ws.numel(), C.c_void_p(stream))
+        ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        tail = (B, T, strided_now, _p(ws), ws.numel(), C.c_void_p(stream))
         if target is None:
             _check(self.lib.gast_forward(self.h, _p(x), _p(y), *tail), 'gast_forward')
         else:
@@ -612,7 +614,7 @@ def run_model_chunked(module, x, max_frames):
 
 def _chunked_forward(module, h, x, strided_now, max_frames):
     """gast_forward_chunked of x (B,T,J,F) -> y (B,T_out,J,3) on a workspace of its own; max_frames None is the whole
-    call, gast_forward on the handle's cached workspace (_eval_forward)"""
+    call, gast_forward (_eval_forward)"""
     if max_frames is None:
         return _eval_forward(module, h, x, strided_now)
     dev = x.device
@@ -732,7 +734,9 @@ def profile_forward(module, x, reps=5):
         run_model(module, x)
         e1.record()
     torch.cuda.synchronize(dev)
+    B, T = int(x.shape[0]), int(x.shape[1])
+    ws_bytes = int(lib.gast_workspace_bytes(h.h, B, T, _strided_now(module, T)))   # one forward's workspace
     return {'per_kernel_ms': per, 'launches': n_launch, 'gemm_ms_per_step': gemm, 'gemm_launches': ng,
-            'step_ms': e0.elapsed_time(e1), 'workspace_bytes': int(h.ws.numel()) if h.ws is not None else 0,
+            'step_ms': e0.elapsed_time(e1), 'workspace_bytes': ws_bytes,
             'gemm_core': ('%s x%d + ffma x%d + attention-mix x%d'
                           % (tc_name, tc, ng - tc - n_launch.get('global_mix', 0), n_launch.get('global_mix', 0))) if tc else 'ffma-fp32'}

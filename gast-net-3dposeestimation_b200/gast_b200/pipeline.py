@@ -247,16 +247,11 @@ def normalize_screen_segments(x, src_start, dst_start, wh, n_out, from_image=Fal
 # ------------------------------------------------------------------------------------------------
 # The video demo's keypoint repair and placement of the lifted persons (tools/preprocess.py)
 # ------------------------------------------------------------------------------------------------
-_PREP_WS = {}
-
-
 def _prep_ws(dev, nbytes):
-    """scratch for the placement minima, grown on demand and kept per device"""
-    ws = _PREP_WS.get(dev)
-    if ws is None or ws.numel() < nbytes:
-        ws = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
-        _PREP_WS[dev] = ws
-    return ws
+    """the call's own scratch (placement minima, metric partials) from the caching allocator, freed to the current
+    stream when the call returns: a scratch kept across calls would be shared by calls in flight on two streams and
+    freed under a call still queued on another stream or captured in a CUDA graph"""
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
 
 
 def h36m_coco_format(kpts, scores):
@@ -339,15 +334,9 @@ def revise_skes_real_time(pred, kpts, width):
 # ------------------------------------------------------------------------------------------------
 # N2: losses and the optimiser step
 # ------------------------------------------------------------------------------------------------
-_WS = {}
-
-
 def _mpjpe_ws(dev):
-    ws = _WS.get(dev)
-    if ws is None:
-        ws = torch.empty(int(L.load().gast_mpjpe_workspace_bytes()), dtype=torch.uint8, device=dev)
-        _WS[dev] = ws
-    return ws
+    """the call's own block partials (see _prep_ws)"""
+    return torch.empty(int(L.load().gast_mpjpe_workspace_bytes()), dtype=torch.uint8, device=dev)
 
 
 class _MpjpeFn(torch.autograd.Function):
