@@ -1528,3 +1528,8 @@ extern "C" int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int3
 // the person detector's letterbox and post-processing (DESIGN.md §8.7)
 // ------------------------------------------------------------------------------------------
 #include "detect.cuh"
+
+// ------------------------------------------------------------------------------------------
+// the SORT tracker between the detector and the 2D pose net (DESIGN.md §8.8)
+// ------------------------------------------------------------------------------------------
+#include "track.cuh"

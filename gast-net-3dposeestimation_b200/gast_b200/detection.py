@@ -5,7 +5,7 @@ for any number of frames in one launch; `person_boxes` is write_results(det_hm=T
 clamp and round(v, 2) for any number of frames in one launch.  Both take numpy arrays or CUDA tensors, return CUDA
 tensors and do not wait for the device.  `video_boxes` is the front half of gen_video_kpts on a chunk of decoded
 frames: one letterbox launch, one call to the caller's Darknet, one post-processing launch, one copy to the host, then
-the caller's tracker frame by frame.  The kernels are csrc/detect.cuh; every formula is in DESIGN.md §8.7.
+the caller's tracker frame by frame (or, with a tracking.DeviceSort, one tracking launch before the copy).  The kernels are csrc/detect.cuh; every formula is in DESIGN.md §8.7.
 
 The letterbox equals OpenCV's own INTER_CUBIC resize bit for bit; cv2 builds that route the resize through IPP differ
 from it by at most one grey level in a few percent of the bytes.  Exact objectness ties, which the reference's sort
@@ -151,7 +151,9 @@ def video_boxes(frames, det_net, tracker, inp_dim=416, confidence=0.7, nms_thres
     det_net(batch, True) is the caller's Darknet: (T, 3, D, D) float32 letterboxed frames on the device to (T, N, 85)
     predictions on the device.  One letterbox launch, one net call, one post-processing launch and one copy of the
     boxes and counts to the host; then tracker.update(bboxs) (the reference's Sort) for each frame in order with
-    yolo_human_det's (n, 4) float32 boxes, skipping frames without a box or whose boxes are all zero.
+    yolo_human_det's (n, 4) float32 boxes, skipping frames without a box or whose boxes are all zero.  A
+    gast_b200.tracking.DeviceSort tracker runs on the device instead, in one launch after the post-processing, and
+    the chunk's one copy is of its tracks.
 
     Returns the T per-frame tracker outputs, None for a skipped frame: what video_keypoints takes as boxes.  Raises
     GastError if a frame has more than max_det boxes."""
@@ -169,6 +171,10 @@ def video_boxes(frames, det_net, tracker, inp_dim=416, confidence=0.7, nms_thres
         raise GastError('detection: the detector must return (%d, %d, %d) predictions on the device'
                         % (T, num_predictions(D), ATTRS))
     boxes, _, counts = person_boxes(pred, (W, H), D, confidence, nms_thresh, max_det)
+    from .tracking import DeviceSort, host_tracks
+    if isinstance(tracker, DeviceSort):
+        # the tracker on the device too: the chunk's one copy is of the tracks
+        return host_tracks(*tracker.update_chunk(boxes, counts, skip_empty=True))
     # one copy: the boxes and the counts' bits side by side
     packed = torch.cat([boxes.view(T, -1), counts.view(torch.float32).view(T, 1)], 1).cpu().numpy()
     counts = packed[:, -1].copy().view(np.int32)

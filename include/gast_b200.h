@@ -653,6 +653,41 @@ int gast_person_detections(const float* predictions, int32_t n, int32_t N, int32
                            int32_t flags, float* boxes, float* scores, int32_t* counts, float* max_conf,
                            int32_t* persons, void* stream);
 
+/* SORT (lib/track/sort.py, called at lib/pose/hrnet/pose_estimation/gen_kpts.py:143,213,306) for S sequences (videos
+ * or cameras) at once, K frames per call, one CTA per sequence with its frames in order.
+ * gast_sort_state_bytes: the state of S sequences of at most `capacity` trackers (1 .. 4096); 0 on refusal.  Each
+ *   sequence's state starts with eight int64 words: frame_count, next id, trackers, status, max_age, min_hits,
+ *   capacity and a tag; the ordered tracker list and each tracker's fp64 x[7], P[7x7], id, time_since_update, hits,
+ *   hit_streak and age follow.
+ * gast_sort_init: Sort(max_age, min_hits) in every sequence; the first tracker of sequence s gets id first_ids[s]
+ *   (device int64 (S), or null for 0), as KalmanBoxTracker.count would have it.
+ * gast_sort_update: Sort.update for frame t of sequence s with the detections boxes[s, t, :counts[s, t]] ((S, K,
+ *   max_det, 4) float32, person_boxes' layout; counts (S, K) int32).  out_rows (S, K, capacity, 5) float64 gets the
+ *   reference's return value, [x1, y1, x2, y2, id + 1] in its order (the tracker list reversed, filtered by
+ *   time_since_update < 1 and (hit_streak >= min_hits or frame_count <= min_hits)); rows past out_counts[s, t] are
+ *   not written.  GAST_SORT_SKIP_EMPTY skips a frame whose count is 0 or whose boxes are all zero, as gen_video_kpts
+ *   does: no update, frame_count stays, out_counts -1.  status (S) int32 gets the sequence's status word: nonzero
+ *   makes its outputs from that frame on invalid (out_counts 0) and is never cleared: GAST_SORT_ST_COUNT a count
+ *   above max_det (or below 0), GAST_SORT_ST_CAPACITY a tracker list beyond capacity, GAST_SORT_ST_IOU an IoU the
+ *   reference refuses (a zero denominator, or NaN: linear_sum_assignment raises), GAST_SORT_ST_INF a predicted box
+ *   with an infinite, non-NaN coordinate (the reference's trks and trackers go out of step), GAST_SORT_ST_STATE a
+ *   state not initialised for this capacity.  The state lives in shared memory for the launch: the capacity and
+ *   max_det must fit 227 KB (about 490 bytes per tracker), else the call is refused before any launch.
+ * Device pointers, the caller's stream, no allocation, synchronisation or host read, so an update can be captured in
+ * a graph; no atomics, calls repeat bit for bit.  Formulas in DESIGN.md §8.8. */
+#define GAST_SORT_SKIP_EMPTY 1
+#define GAST_SORT_ST_COUNT 1
+#define GAST_SORT_ST_CAPACITY 2
+#define GAST_SORT_ST_IOU 4
+#define GAST_SORT_ST_INF 8
+#define GAST_SORT_ST_STATE 16
+size_t gast_sort_state_bytes(int32_t S, int32_t capacity);
+int gast_sort_init(void* state, int32_t S, int32_t capacity, int32_t max_age, int32_t min_hits,
+                   const int64_t* first_ids, void* stream);
+int gast_sort_update(void* state, int32_t S, int32_t capacity, int32_t K, const float* boxes, const int32_t* counts,
+                     int32_t max_det, int32_t flags, double* out_rows, int32_t* out_counts, int32_t* status,
+                     void* stream);
+
 /* optim.Adam(amsgrad=True) (trainval.py:78,162-164) for every parameter in one launch.  table (n_chunks,4)
  * int64 on the device: {param pointer, grad pointer, offset into the flat state buffers, count <=
  * gast_adam_chunk()}.  max_exp_avg_sq null = plain Adam.  step = 1 for the first update. */
