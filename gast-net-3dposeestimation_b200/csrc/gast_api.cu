@@ -1533,3 +1533,8 @@ extern "C" int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int3
 // the SORT tracker between the detector and the 2D pose net (DESIGN.md §8.8)
 // ------------------------------------------------------------------------------------------
 #include "track.cuh"
+
+// ------------------------------------------------------------------------------------------
+// SORT's tracks to the 2D pose net's crop records (DESIGN.md §8.9)
+// ------------------------------------------------------------------------------------------
+#include "records.cuh"

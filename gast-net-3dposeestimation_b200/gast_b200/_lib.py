@@ -37,7 +37,7 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_pose_metrics_workspace_bytes',
            'gast_pose_metrics', 'gast_render_geometry', 'gast_render_frames', 'gast_downsample_frames',
            'gast_person_crops', 'gast_heatmap_decode', 'gast_letterbox', 'gast_person_detections',
-           'gast_sort_state_bytes', 'gast_sort_init', 'gast_sort_update',
+           'gast_sort_state_bytes', 'gast_sort_init', 'gast_sort_update', 'gast_track_records', 'gast_record_inverse',
            'gast_adam_chunk', 'gast_adam_step', 'gast_chunk_gather_indexed',
            'gast_adam_step_table', 'gast_adam_step_indexed', 'gast_epoch_loss_accumulate',
            'gast_last_error', 'gast_version']
@@ -293,6 +293,11 @@ def load():
     lib.gast_sort_init.restype = C.c_int
     lib.gast_sort_update.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
     lib.gast_sort_update.restype = C.c_int
+    lib.gast_track_records.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp, vp]
+    lib.gast_track_records.restype = C.c_int
+    lib.gast_record_inverse.argtypes = [vp, C.c_int32, vp, C.c_int32, C.c_int32, vp, vp]
+    lib.gast_record_inverse.restype = C.c_int
     lib.gast_adam_chunk.argtypes = []
     lib.gast_adam_chunk.restype = C.c_int32
     lib.gast_adam_step.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,

@@ -144,7 +144,7 @@ def person_boxes(predictions, frame_sizes, inp_dim=416, confidence=0.7, nms_thre
 
 
 def video_boxes(frames, det_net, tracker, inp_dim=416, confidence=0.7, nms_thresh=0.4, max_det=MAX_DET,
-                rgb_input=False):
+                rgb_input=False, on_device=False):
     """The front half of gen_video_kpts (gen_kpts.py:199-227) on a chunk of decoded frames (T, H, W, 3) uint8 (BGR
     as cv2 reads them, RGB with rgb_input), numpy or CUDA.
 
@@ -156,12 +156,19 @@ def video_boxes(frames, det_net, tracker, inp_dim=416, confidence=0.7, nms_thres
     the chunk's one copy is of its tracks.
 
     Returns the T per-frame tracker outputs, None for a skipped frame: what video_keypoints takes as boxes.  Raises
-    GastError if a frame has more than max_det boxes."""
+    GastError if a frame has more than max_det boxes.  With a DeviceSort and on_device=True nothing is copied: it
+    returns update_chunk's (rows, counts, status) on the device, which video_keypoints also takes as boxes, so the
+    chain to the keypoints makes no per-box host work."""
+    from .tracking import DeviceSort, host_tracks
+    if on_device and not isinstance(tracker, DeviceSort):
+        raise GastError('detection: on_device=True needs a tracking.DeviceSort tracker')
     shape = tuple(frames.shape)
     if len(shape) != 4 or shape[-1] != 3:
         raise GastError('detection: frames (T, H, W, 3) expected, got %s' % (shape,))
     T, H, W = int(shape[0]), int(shape[1]), int(shape[2])
     if T == 0:
+        if on_device:
+            return tracker.update_chunk(np.zeros((0, max_det, 4), np.float32), np.zeros(0, np.int32))
         return []
     D = check_inp_dim(inp_dim)
     batch = letterbox(frames, D, rgb_input=rgb_input)
@@ -171,10 +178,10 @@ def video_boxes(frames, det_net, tracker, inp_dim=416, confidence=0.7, nms_thres
         raise GastError('detection: the detector must return (%d, %d, %d) predictions on the device'
                         % (T, num_predictions(D), ATTRS))
     boxes, _, counts = person_boxes(pred, (W, H), D, confidence, nms_thresh, max_det)
-    from .tracking import DeviceSort, host_tracks
     if isinstance(tracker, DeviceSort):
-        # the tracker on the device too: the chunk's one copy is of the tracks
-        return host_tracks(*tracker.update_chunk(boxes, counts, skip_empty=True))
+        # the tracker on the device too: the chunk's one copy is of the tracks, or none with on_device
+        tracks = tracker.update_chunk(boxes, counts, skip_empty=True)
+        return tracks if on_device else host_tracks(*tracks)
     # one copy: the boxes and the counts' bits side by side
     packed = torch.cat([boxes.view(T, -1), counts.view(torch.float32).view(T, 1)], 1).cpu().numpy()
     counts = packed[:, -1].copy().view(np.int32)

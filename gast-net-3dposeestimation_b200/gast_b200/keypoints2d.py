@@ -6,8 +6,13 @@ number of boxes of any number of frames in one launch; `decode_heatmaps` is get_
 tensors and do not wait for the device.  `video_keypoints` is the back half of gen_video_kpts(gen_output=True) on a
 chunk of decoded frames.  The kernels are csrc/keypoints2d.cuh; every formula is in DESIGN.md §8.6.
 
-The box geometry (box_to_center_scale, get_affine_transform) stays on the host, because the boxes come from the
-tracker on the host; it follows the reference's float32 / float64 steps.  The matrices themselves come from
+`track_records` and `record_inverse` compute the box geometry on the device from DeviceSort.update_chunk's tracks:
+select_tracks, round(v, 2), box_to_center_scale and get_affine_transform with OpenCV's own 6 x 6 LU restated in its
+order, equal to the host functions with cv2 bit for bit (csrc/records.cuh, DESIGN.md §8.9).  `video_keypoints` takes
+those tracks directly, and then makes one synchronisation per chunk: the copy of the record count and status.
+
+For per-frame track lists the box geometry (box_to_center_scale, get_affine_transform) runs on the host, as do the
+drop-ins; it follows the reference's float32 / float64 steps.  The matrices themselves come from
 cv2.getAffineTransform when cv2 is importable, which makes the crops and keypoints equal to the reference's bit for
 bit.  Without cv2 a closed form in double gives matrices within a few ulps of OpenCV's; a crop warped with them can
 then differ from the reference's in a few pixels by one grey level, where the fixed-point warp rounds an exact half.
@@ -16,6 +21,7 @@ Refused before any launch (GastError): a box whose width and height are both non
 singular), a non-finite box or matrix, a frame side above 32767 (OpenCV keeps source coordinates as int16), a crop
 side above 32767, heatmaps of more than 32 joints or with a side above 256, non-float32 heatmaps, a frame index out of
 range, and in `video_keypoints` a frame with between 2 and num_person - 1 tracks (the reference's reshape raises).
+With DeviceSort's tracks these are found on the device and raised at the call's one copy, with the same messages.
 """
 import ctypes as C
 
@@ -257,10 +263,12 @@ def video_keypoints(frames, boxes, pose_net, num_person, image_size=IMAGE_SIZE, 
     with the crop and the decode on the device.
 
     frames (T, H, W, 3) uint8 (BGR as cv2 reads them, RGB with rgb_input), numpy or CUDA; boxes: T per-frame tracker
-    outputs (k, 5) or (k, 4) in frame pixels, or None / empty where nothing was detected; pose_net: a callable
+    outputs (k, 5) or (k, 4) in frame pixels, or None / empty where nothing was detected, or the (rows, counts,
+    status) triple tracking.DeviceSort.update_chunk returns for one sequence of T frames; pose_net: a callable
     mapping the crops (n, 3, h, w) float32 on the device, planes in the net's order, to heatmaps (n, 17, hh, hw)
     float32 on the device (HRNet w48_384x288: 96 x 72).  Every box of the chunk is cropped in one launch, the net runs
-    once, and the decode is one launch.
+    once, and the decode is one launch.  With the triple the boxes' geometry is one launch too (track_records), and
+    the call's one synchronisation is the copy of its record count and status to the host.
 
     Returns keypoints (num_person, T', 17, 2) and scores (num_person, T', 17) float32 on the device, T' the frames with
     at least one track; a slot without a track stays zero.  Feeds device.tools.preprocess.h36m_coco_format."""
@@ -271,6 +279,18 @@ def video_keypoints(frames, boxes, pose_net, num_person, image_size=IMAGE_SIZE, 
     if len(shape) != 4 or shape[-1] != 3:
         raise GastError('keypoints2d: frames (T, H, W, 3) expected, got %s' % (shape,))
     T, H, W = int(shape[0]), int(shape[1]), int(shape[2])
+    if _is_track_triple(boxes):
+        rows, counts, status = boxes
+        if rows.dim() != 3 or int(rows.shape[0]) != T:
+            raise GastError('keypoints2d: %d frames but tracks %s (one sequence of (T, capacity, 5) rows expected)'
+                            % (T, tuple(rows.shape)))
+        rec = track_records(rows, counts, status, num_person, (W, H), image_size)
+        summary = rec.summary.cpu().numpy()                  # the call's one synchronisation
+        _raise_records_error(summary, rows, counts, num_person, (W, H))
+        n, t_out = int(summary[0, 0]), int(summary[0, 1])
+        dev = frames.device if isinstance(frames, torch.Tensor) and frames.is_cuda else _device(None)
+        return _keypoints(frames, dev, n, t_out, num_person, rec.frame[:n], rec.forward[:n], rec.slot[:n],
+                          lambda size: record_inverse(rec, size)[:n], pose_net, image_size, post_process, rgb_input)
     if len(boxes) != T:
         raise GastError('keypoints2d: %d frames but %d box lists' % (T, len(boxes)))
     frame_idx, slots, centers, scales, fwd = [], [], [], [], []
@@ -287,24 +307,144 @@ def video_keypoints(frames, boxes, pose_net, num_person, image_size=IMAGE_SIZE, 
             scales.append(s)
             fwd.append(affine_pair(c, s, image_size)[0])
         t_out += 1
+    n = len(frame_idx)
     dev = frames.device if isinstance(frames, torch.Tensor) and frames.is_cuda else _device(None)
+    return _keypoints(frames, dev, n, t_out, num_person, frame_idx, np.stack(fwd) if n else None,
+                      np.asarray(slots, dtype=np.int64),
+                      lambda size: np.stack([inverse_matrix(c, s, size) for c, s in zip(centers, scales)]),
+                      pose_net, image_size, post_process, rgb_input)
+
+
+def _keypoints(frames, dev, n, t_out, num_person, frame_idx, fwd, slots, inverse, pose_net, image_size, post_process,
+               rgb_input):
+    """video_keypoints' crop, net, decode and scatter of n records into t_out frames; inverse((hw, hh)) gives the
+    records' inverse matrices once the net's heatmap size is known"""
     J = 17
     kpts = torch.zeros((t_out * num_person, J, 2), dtype=torch.float32, device=dev)
     scores = torch.zeros((t_out * num_person, J), dtype=torch.float32, device=dev)
-    if frame_idx:
-        crops = crop_persons(frames, frame_idx, np.stack(fwd), image_size, rgb_input=rgb_input, net_order=True)
+    if n:
+        crops = crop_persons(frames, frame_idx, fwd, image_size, rgb_input=rgb_input, net_order=True)
         with torch.no_grad():
             heat = pose_net(crops)
         if not isinstance(heat, torch.Tensor) or not heat.is_cuda or heat.dim() != 4 or \
-                int(heat.shape[0]) != len(frame_idx) or int(heat.shape[1]) != J:
+                int(heat.shape[0]) != n or int(heat.shape[1]) != J:
             raise GastError('keypoints2d: the pose net must return (%d, %d, hh, hw) heatmaps on the device'
-                            % (len(frame_idx), J))
+                            % (n, J))
         hh, hw = int(heat.shape[2]), int(heat.shape[3])
-        inv = np.stack([inverse_matrix(c, s, (hw, hh)) for c, s in zip(centers, scales)])
-        preds, maxvals = decode_heatmaps(heat, inv, post_process)
-        slot = _on_device(np.asarray(slots, dtype=np.int64), torch.int64, dev, 'slots')
+        preds, maxvals = decode_heatmaps(heat, inverse((hw, hh)), post_process)
+        slot = _on_device(slots, torch.int64, dev, 'slots')
         kpts.index_copy_(0, slot, preds)
         scores.index_copy_(0, slot, maxvals.view(-1, J))
     kpts = kpts.view(t_out, num_person, J, 2).transpose(0, 1).contiguous()
     scores = scores.view(t_out, num_person, J).transpose(0, 1).contiguous()
     return kpts, scores
+
+
+# ------------------------------------------------------------------------------------------------
+# SORT's tracks to crop records on the device
+# ------------------------------------------------------------------------------------------------
+REC_TRACKS, REC_NONFINITE, REC_EMPTY, REC_MATRIX = 0x100, 0x200, 0x400, 0x800    # GAST_REC_ST_*
+SORT_BITS = 0xff                                                                 # SORT's own word
+
+
+class TrackRecords:
+    """track_records' outputs on the device, with room for S * K * num_person records; those past `total` are not
+    written.  frame (N,) int32: s * K + t; slot (N,) int64: t' * num_person + p, t' the frame's rank among the
+    sequence's kept frames; forward (N, 2, 3) float64: the frame -> crop matrix cv2.warpAffine receives;
+    center_scale (N, 4) float32 (center and scale are its views); summary (S, 4) int32: each sequence's records, kept
+    frames, status word and first offending frame (-1 for none); total (1,) int32: all sequences' records."""
+
+    def __init__(self, frame, slot, forward, center_scale, summary, total):
+        self.frame, self.slot, self.forward, self.center_scale = frame, slot, forward, center_scale
+        self.summary, self.total = summary, total
+
+    @property
+    def center(self):
+        return self.center_scale[:, :2]
+
+    @property
+    def scale(self):
+        return self.center_scale[:, 2:]
+
+
+def _is_track_triple(boxes):
+    return isinstance(boxes, tuple) and len(boxes) == 3 and all(isinstance(b, torch.Tensor) and b.is_cuda
+                                                                 for b in boxes)
+
+
+def track_records(rows, counts, status, num_person, frame_size, image_size=IMAGE_SIZE):
+    """The crop records of every box gen_video_kpts keeps (select_tracks, then center_scale and affine_pair's forward
+    matrix, bit for bit) from DeviceSort.update_chunk's outputs: rows (K, capacity, 5) / (S, K, capacity, 5) float64,
+    counts (K,) / (S, K) int32 and status (S,) int32, for frames of frame_size (W, H) and crops of image_size (w, h).
+    One launch; returns a TrackRecords of CUDA tensors without waiting for the device."""
+    if not all(isinstance(x, torch.Tensor) and x.is_cuda for x in (rows, counts, status)):
+        raise GastError('keypoints2d: rows, counts and status must be CUDA tensors (DeviceSort.update_chunk\'s)')
+    if rows.dtype != torch.float64 or counts.dtype != torch.int32 or status.dtype != torch.int32:
+        raise GastError('keypoints2d: float64 rows and int32 counts and status expected, got %s, %s, %s'
+                        % (rows.dtype, counts.dtype, status.dtype))
+    R = rows[None] if rows.dim() == 3 else rows
+    N = counts[None] if counts.dim() == 1 else counts
+    if R.dim() != 4 or R.shape[-1] != 5 or tuple(N.shape) != tuple(R.shape[:2]) or tuple(status.shape) != (R.shape[0],):
+        raise GastError('keypoints2d: rows %s, counts %s and status %s do not match'
+                        % (tuple(rows.shape), tuple(counts.shape), tuple(status.shape)))
+    S, K, cap = int(R.shape[0]), int(R.shape[1]), int(R.shape[2])
+    num_person = int(num_person)
+    if num_person < 1:
+        raise GastError('keypoints2d: num_person must be >= 1')
+    W, H = int(frame_size[0]), int(frame_size[1])
+    w, h = int(image_size[0]), int(image_size[1])
+    if not (0 < W <= MAX_SIDE and 0 < H <= MAX_SIDE and 0 < w <= MAX_SIDE and 0 < h <= MAX_SIDE):
+        raise GastError('keypoints2d: a %d x %d frame or a %d x %d crop (each side 1 .. %d)' % (W, H, w, h, MAX_SIDE))
+    dev = rows.device
+    n = S * K * num_person
+    frame = torch.empty(n, dtype=torch.int32, device=dev)
+    slot = torch.empty(n, dtype=torch.int64, device=dev)
+    forward = torch.empty((n, 2, 3), dtype=torch.float64, device=dev)
+    cs = torch.empty((n, 4), dtype=torch.float32, device=dev)
+    summary = torch.empty((S, 4), dtype=torch.int32, device=dev)
+    total = torch.zeros(1, dtype=torch.int32, device=dev)
+    R, N, st = R.contiguous(), N.to(device=dev).contiguous(), status.to(device=dev).contiguous()
+    with torch.cuda.device(dev):
+        _check(L.load().gast_track_records(_p(R), _p(N), _p(st), S, K, cap, num_person, W, H, w, h, _p(frame), _p(slot),
+                                           _p(forward), _p(cs), _p(summary), _p(total), C.c_void_p(_stream(dev))),
+               'gast_track_records')
+    return TrackRecords(frame, slot, forward, cs, summary, total)
+
+
+def record_inverse(records, heatmap_size):
+    """get_affine_transform(center, scale, 0, heatmap_size, inv=1) of every record: (N, 2, 3) float64 on the device,
+    inverse_matrix's bits; rows past records.total are not written.  One launch, no synchronisation."""
+    hw, hh = int(heatmap_size[0]), int(heatmap_size[1])
+    if not (0 < hw <= MAX_SIDE and 0 < hh <= MAX_SIDE):
+        raise GastError('keypoints2d: a %d x %d heatmap (each side 1 .. %d)' % (hw, hh, MAX_SIDE))
+    cs = records.center_scale
+    dev = cs.device
+    n = int(cs.shape[0])
+    out = torch.empty((n, 2, 3), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _check(L.load().gast_record_inverse(_p(cs), n, _p(records.total), hw, hh, _p(out), C.c_void_p(_stream(dev))),
+               'gast_record_inverse')
+    return out
+
+
+def _raise_records_error(summary, rows, counts, num_person, frame_size):
+    """GastError with the host path's message for the first sequence whose status word is set: tracking's message
+    for SORT's bits; for a frame's bits, select_tracks' or center_scale's own, from one copy of that frame's tracks"""
+    bad = np.flatnonzero(summary[:, 2])
+    if not bad.size:
+        return
+    s = int(bad[0])
+    word, t = int(summary[s, 2]), int(summary[s, 3])
+    if word & SORT_BITS:
+        from .tracking import status_message
+        raise GastError('tracking: sequence %d: %s' % (s, status_message(word & SORT_BITS)))
+    if t >= 0:
+        R = rows[None] if rows.dim() == 3 else rows
+        N = counts[None] if counts.dim() == 1 else counts
+        k = int(N[s, t])
+        track = R[s, t, :max(0, min(k, int(R.shape[2])))].cpu().numpy()
+        sel = select_tracks(track, num_person)
+        for box in sel[:num_person] if sel is not None else ():
+            center_scale(box, frame_size[1], frame_size[0])
+        raise GastError('keypoints2d: sequence %d frame %d: %d tracks (capacity %d)' % (s, t, k, int(R.shape[2])))
+    raise GastError('keypoints2d: forward matrices are not finite')

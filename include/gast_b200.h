@@ -688,6 +688,42 @@ int gast_sort_update(void* state, int32_t S, int32_t capacity, int32_t K, const 
                      int32_t max_det, int32_t flags, double* out_rows, int32_t* out_counts, int32_t* status,
                      void* stream);
 
+/* SORT's tracks to the 2D pose net's crop records (lib/pose/hrnet/pose_estimation/gen_kpts.py:214-256), so that no
+ * per-box host work lies between the tracker and the pose net.
+ * gast_track_records: reads gast_sort_update's outputs of S sequences x K frames as they are (rows (S, K, capacity,
+ *   5) float64, only rows [0, counts[s, t]) read; counts (S, K) int32, -1 a skipped frame; status (S) int32) and
+ *   applies gen_video_kpts' record rule to every frame: k <= 0 tracks drop the frame, k = 1 keeps the one row,
+ *   k >= num_person keeps the last num_person rows reversed (select_tracks).  Each kept box is rounded as
+ *   round(v, 2), goes through box_to_center_scale with the frame's (H, W) in the model-size slots (PreProcess's call)
+ *   and get_affine_transform to the out_w x out_h crop, with the reference's float32 / float64 steps, and the matrix
+ *   is cv2.getAffineTransform's (OpenCV's 6 x 6 LU, unfused double; a pivot below 100 * DBL_EPSILON gives a zero
+ *   matrix), bit for bit.  Record r, contiguous in (s, t, p) order over all sequences, gets frame_index[r] = s * K +
+ *   t, slots[r] = t' * num_person + p (t' the frame's rank among the sequence's kept frames), forward_mats[6r..6r+5]
+ *   and center_scale[4r..4r+3] = (center x, center y, scale x, scale y) float32.  The arrays must hold S * K *
+ *   num_person records; those past the total are not written.  summary (S, 4) int32: the sequence's records, its kept
+ *   frames, its status word and the first frame (t) that set a GAST_REC_ST_TRACKS, GAST_REC_ST_NONFINITE or
+ *   GAST_REC_ST_EMPTY bit (-1 for none).  The status word is SORT's word (its low bits) or'ed with:
+ *   GAST_REC_ST_TRACKS a frame with 2 .. num_person - 1 tracks (the reference's reshape raises) or a count outside
+ *   -1 .. capacity, GAST_REC_ST_NONFINITE a kept box with a non-finite coordinate, GAST_REC_ST_EMPTY a kept box with
+ *   a non-positive width and height (its triangle is singular), GAST_REC_ST_MATRIX a non-finite forward matrix.
+ *   total (1) int32: all sequences' records.  Sides <= 32767; S * K * num_person < 2^31.
+ * gast_record_inverse: get_affine_transform(center, scale, 0, (hw, hh), inv=1) of the first min(n, *total) records'
+ *   center_scale (n, 4) float32 (total: a device int32, or null for n): inverse_mats (n, 6) float64, the heatmap ->
+ *   frame matrices get_final_preds applies, with the same triangles and LU, bit for bit.
+ * Device pointers, the caller's stream, no allocation, synchronisation or host read, so both can be captured in a
+ * graph; no atomics, calls repeat bit for bit and a sequence's records do not depend on the other sequences' rows.
+ * Formulas in DESIGN.md §8.9. */
+#define GAST_REC_ST_TRACKS 0x100
+#define GAST_REC_ST_NONFINITE 0x200
+#define GAST_REC_ST_EMPTY 0x400
+#define GAST_REC_ST_MATRIX 0x800
+int gast_track_records(const double* rows, const int32_t* counts, const int32_t* status, int32_t S, int32_t K,
+                       int32_t capacity, int32_t num_person, int32_t W, int32_t H, int32_t out_w, int32_t out_h,
+                       int32_t* frame_index, int64_t* slots, double* forward_mats, float* center_scale,
+                       int32_t* summary, int32_t* total, void* stream);
+int gast_record_inverse(const float* center_scale, int32_t n, const int32_t* total, int32_t hw, int32_t hh,
+                        double* inverse_mats, void* stream);
+
 /* optim.Adam(amsgrad=True) (trainval.py:78,162-164) for every parameter in one launch.  table (n_chunks,4)
  * int64 on the device: {param pointer, grad pointer, offset into the flat state buffers, count <=
  * gast_adam_chunk()}.  max_exp_avg_sq null = plain Adam.  step = 1 for the first update. */
