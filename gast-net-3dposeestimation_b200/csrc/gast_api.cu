@@ -1538,3 +1538,4 @@ extern "C" int gast_debug_wgrad(const float* dZ, const float* A, float* dW, int3
 // SORT's tracks to the 2D pose net's crop records (DESIGN.md §8.9)
 // ------------------------------------------------------------------------------------------
 #include "records.cuh"
+#include "live.cuh"

@@ -198,6 +198,25 @@ __global__ void kpt_convert_kernel(const float* __restrict__ kp, float* __restri
 constexpr int PREP_BLOCK = 256;
 __device__ __forceinline__ float np_minf(float a, float b) { return (isnan(a) || a < b) ? a : b; }   // np.amin: NaN wins
 
+// h36m_coco_format's keep test of one frame's 17 COCO keypoints (preprocess.py:60): some coordinate is non-zero
+__device__ __forceinline__ bool coco_any_nonzero(const float* k) {
+  bool any = false;
+  for (int c = 0; c < 34; ++c) any |= (k[c] != 0.f);
+  return any;
+}
+
+// h36m_coco_format's scores (preprocess.py:65-69): one frame's 17 COCO scores s -> H36M scores n
+__device__ __forceinline__ void coco_scores_to_h36m(const float* s, float (&n)[17]) {
+  const int h36m_coco_order[13] = {9, 11, 14, 12, 15, 13, 16, 4, 1, 5, 2, 6, 3};
+  const int coco_order[13] = {0, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16};
+#pragma unroll
+  for (int q = 0; q < 13; ++q) n[h36m_coco_order[q]] = s[coco_order[q]];
+  n[0] = __fdiv_rn(__fadd_rn(s[11], s[12]), 2.f);
+  n[8] = __fdiv_rn(__fadd_rn(s[5], s[6]), 2.f);
+  n[7] = __fdiv_rn(__fadd_rn(n[0], n[8]), 2.f);
+  n[10] = __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(s[1], s[2]), s[3]), s[4]), 4.f);
+}
+
 // h36m_coco_format (preprocess.py:47-75): one thread per (person, frame).  Keypoints and valid mask as
 // kpt_convert_kernel mode 0; the scores remapped (:65-69); keep[p] = 1 once any coordinate of person p is non-zero
 // (keep is zeroed by the caller; every writer stores the same value).
@@ -207,44 +226,24 @@ __global__ void h36m_coco_format_kernel(const float* __restrict__ kp, const floa
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)P * T) return;
   const float* k = kp + i * 34;
-  bool any = false;
-  for (int c = 0; c < 34; ++c) any |= (k[c] != 0.f);
-  if (any) keep[i / T] = 1;
+  if (coco_any_nonzero(k)) keep[i / T] = 1;
   float o[34];
   coco_to_h36m_frame(k, 2, o);
   float* op = out + i * 34;
   for (int c = 0; c < 34; ++c) op[c] = o[c];
   valid[i] = (np_pairwise_sum(o, 34) != 0.f) ? 1 : 0;
-  const float* s = sc + i * 17;
   float n[17];
-  const int h36m_coco_order[13] = {9, 11, 14, 12, 15, 13, 16, 4, 1, 5, 2, 6, 3};
-  const int coco_order[13] = {0, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16};
-#pragma unroll
-  for (int q = 0; q < 13; ++q) n[h36m_coco_order[q]] = s[coco_order[q]];
-  n[0] = __fdiv_rn(__fadd_rn(s[11], s[12]), 2.f);
-  n[8] = __fdiv_rn(__fadd_rn(s[5], s[6]), 2.f);
-  n[7] = __fdiv_rn(__fadd_rn(n[0], n[8]), 2.f);
-  n[10] = __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(s[1], s[2]), s[3]), s[4]), 4.f);
+  coco_scores_to_h36m(sc + i * 17, n);
   float* so = sout + i * 17;
 #pragma unroll
   for (int q = 0; q < 17; ++q) so[q] = n[q];
 }
 
-// revise_kpts (preprocess.py:78-112): one thread per (person, frame).  Zero outside the valid frames; at a valid
-// frame the pose, with the low-confidence limb joints replaced by the first matching case of :94-109 (every right-hand
-// side read before the assignment, as numpy's fancy indexing does).  low joints: score < float32(0.3).
-__global__ void revise_kpts_kernel(const float* __restrict__ kp, const float* __restrict__ sc, const int* __restrict__ mask,
-                                   float* __restrict__ out, long long PT, int J) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= PT) return;
-  const float2* k = reinterpret_cast<const float2*>(kp) + i * J;
-  float2* o = reinterpret_cast<float2*>(out) + i * J;
-  if (!mask[i]) {
-    for (int j = 0; j < J; ++j) o[j] = make_float2(0.f, 0.f);
-    return;
-  }
+// revise_kpts at one valid frame (preprocess.py:94-109): o = the pose k of J joints, with the low-confidence limb
+// joints replaced by the first matching case (every right-hand side read before the assignment, as numpy's fancy
+// indexing does).  low joints: score s < float32(0.3).
+__device__ __forceinline__ void revise_kpts_frame(const float2* k, const float* s, float2* o, int J) {
   for (int j = 0; j < J; ++j) o[j] = k[j];
-  const float* s = sc + i * J;
   const int low = (s[2] < 0.3f ? 1 : 0) | (s[3] < 0.3f ? 2 : 0) | (s[5] < 0.3f ? 4 : 0) | (s[6] < 0.3f ? 8 : 0);
   const float2 k1 = k[1], k2 = k[2], k4 = k[4], k5 = k[5];
   switch (low) {
@@ -256,6 +255,21 @@ __global__ void revise_kpts_kernel(const float* __restrict__ kp, const float* __
     case 8: o[6] = k5; break;                                     // 6 <- 5
     default: break;                                               // any other combination: unchanged
   }
+}
+
+// revise_kpts (preprocess.py:78-112): one thread per (person, frame).  Zero outside the valid frames; at a valid
+// frame revise_kpts_frame.
+__global__ void revise_kpts_kernel(const float* __restrict__ kp, const float* __restrict__ sc, const int* __restrict__ mask,
+                                   float* __restrict__ out, long long PT, int J) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= PT) return;
+  const float2* k = reinterpret_cast<const float2*>(kp) + i * J;
+  float2* o = reinterpret_cast<float2*>(out) + i * J;
+  if (!mask[i]) {
+    for (int j = 0; j < J; ++j) o[j] = make_float2(0.f, 0.f);
+    return;
+  }
+  revise_kpts_frame(k, sc + i * J, o, J);
 }
 
 // mean over joints [1, 4, 11, 14] of (a - b) (b may be null = 0), channel c of rows with D floats per joint:
@@ -365,6 +379,14 @@ __global__ void zmin_subtract_kernel(float* __restrict__ x, long long n, const f
     x[3 * i + 2] = __fsub_rn(x[3 * i + 2], zmin);
 }
 
+// revise_skes_real_time's placement of one joint (:167-168): p (3 floats) moved by the limb mean of the person's 2D
+// keypoints a (17 joints of D floats): x -= (m_x - cx) / r, y += (m_y - cy) / r
+__device__ __forceinline__ void rt_place(const float* p, const float* a, int D, float cx, float cy, float r, float& x,
+                                         float& y) {
+  x = __fsub_rn(p[0], __fdiv_rn(__fsub_rn(limb_mean(a, nullptr, D, 0), cx), r));
+  y = __fadd_rn(p[1], __fdiv_rn(__fsub_rn(limb_mean(a, nullptr, D, 1), cy), r));
+}
+
 // revise_skes_real_time (:158-172), one thread per (person, joint): x -= (m_x - cx) / r, y += (m_y - cy) / r with m the
 // limb mean of the person's 2D keypoints (J = 17, D floats per keypoint), and the per-block minimum of z
 __global__ void revise_rt_kernel(const float* __restrict__ pred, const float* __restrict__ kp, float* __restrict__ out, int M,
@@ -373,8 +395,8 @@ __global__ void revise_rt_kernel(const float* __restrict__ pred, const float* __
   float z = INFINITY;
   if (i < M * 17) {
     const float* a = kp + (long long)(i / 17) * 17 * D;
-    const float x = __fsub_rn(pred[3 * i], __fdiv_rn(__fsub_rn(limb_mean(a, nullptr, D, 0), cx), r));
-    const float y = __fadd_rn(pred[3 * i + 1], __fdiv_rn(__fsub_rn(limb_mean(a, nullptr, D, 1), cy), r));
+    float x, y;
+    rt_place(pred + 3 * i, a, D, cx, cy, r, x, y);
     z = pred[3 * i + 2];
     out[3 * i] = x; out[3 * i + 1] = y; out[3 * i + 2] = z;
   }
@@ -391,14 +413,17 @@ __global__ void revise_rt_kernel(const float* __restrict__ pred, const float* __
 // normalize_screen_coordinates (common/camera.py:8-12): X/w*2 - [1, h/w].  numpy evaluates X/w*2 in
 // float32 and the subtraction of the Python-float list in float64; the result is rounded to float32
 // here (callers cast it: reconstruction.py:143, main.py:46).   image_coordinates (:15-19) is the inverse.
+__device__ __forceinline__ float screen_norm(float x, float w, double c) {
+  return (float)((double)__fmul_rn(__fdiv_rn(x, w), 2.f) - c);
+}
+
 __global__ void screen_norm_kernel(const float* __restrict__ x, float* __restrict__ out, long long n, float w, double hw,
                                    int inverse) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n) return;
   const double c = (idx & 1) ? hw : 1.0;
   if (!inverse) {
-    const float s = __fmul_rn(__fdiv_rn(x[idx], w), 2.f);
-    out[idx] = (float)((double)s - c);
+    out[idx] = screen_norm(x[idx], w, c);
   } else {
     out[idx] = (float)(((double)x[idx] + c) * (double)w / 2.0);
   }
@@ -1141,6 +1166,16 @@ extern "C" int gast_revise_skes(const float* pred, const int64_t* frames, const 
   return 0;
 }
 
+namespace gast {
+// preprocess.py:159,167-168 under NumPy 2's promotion: the Python-float constants are rounded to float32 and every
+// operation is float32
+static void rt_constants(double width, float& cx, float& cy, float& r) {
+  cx = (float)(3.0 * width / 5.0);
+  cy = (float)(width / 5.0);
+  r = (float)(500.0 * (width / 1920.0));
+}
+}  // namespace gast
+
 extern "C" size_t gast_revise_skes_real_time_workspace_bytes(int32_t M) {
   return M > 0 ? sizeof(float) * cdiv((long long)M * 17, PREP_BLOCK) : 0;
 }
@@ -1152,9 +1187,8 @@ extern "C" int gast_revise_skes_real_time(const float* pred, const float* kpts, 
   if (workspace_bytes < gast_revise_skes_real_time_workspace_bytes(M))
     return fail("gast_revise_skes_real_time: workspace of %zu bytes, %zu needed", workspace_bytes,
                 gast_revise_skes_real_time_workspace_bytes(M));
-  // preprocess.py:159,167-168 under NumPy 2's promotion: the Python-float constants are rounded to float32 and every
-  // operation is float32
-  const float cx = (float)(3.0 * width / 5.0), cy = (float)(width / 5.0), r = (float)(500.0 * (width / 1920.0));
+  float cx, cy, r;
+  rt_constants(width, cx, cy, r);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int nb = (int)cdiv((long long)M * 17, PREP_BLOCK);
   float* part = reinterpret_cast<float*>(workspace);

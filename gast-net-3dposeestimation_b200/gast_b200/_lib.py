@@ -38,6 +38,7 @@ SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out
            'gast_pose_metrics', 'gast_render_geometry', 'gast_render_frames', 'gast_downsample_frames',
            'gast_person_crops', 'gast_heatmap_decode', 'gast_letterbox', 'gast_person_detections',
            'gast_sort_state_bytes', 'gast_sort_init', 'gast_sort_update', 'gast_track_records', 'gast_record_inverse',
+           'gast_live_slots', 'gast_live_inputs', 'gast_live_place',
            'gast_adam_chunk', 'gast_adam_step', 'gast_chunk_gather_indexed',
            'gast_adam_step_table', 'gast_adam_step_indexed', 'gast_epoch_loss_accumulate',
            'gast_last_error', 'gast_version']
@@ -298,6 +299,15 @@ def load():
     lib.gast_track_records.restype = C.c_int
     lib.gast_record_inverse.argtypes = [vp, C.c_int32, vp, C.c_int32, C.c_int32, vp, vp]
     lib.gast_record_inverse.restype = C.c_int
+    # the live tick (DESIGN.md §8.10)
+    lib.gast_live_slots.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                    C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp, vp]
+    lib.gast_live_slots.restype = C.c_int
+    lib.gast_live_inputs.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp,
+                                     vp, vp]
+    lib.gast_live_inputs.restype = C.c_int
+    lib.gast_live_place.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_double, vp, vp]
+    lib.gast_live_place.restype = C.c_int
     lib.gast_adam_chunk.argtypes = []
     lib.gast_adam_chunk.restype = C.c_int32
     lib.gast_adam_step.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,

@@ -724,6 +724,43 @@ int gast_track_records(const double* rows, const int32_t* counts, const int32_t*
 int gast_record_inverse(const float* center_scale, int32_t n, const int32_t* total, int32_t hw, int32_t hh,
                         double* inverse_mats, void* stream);
 
+/* The live tick (gen_img_kpts, lib/pose/hrnet/pose_estimation/gen_kpts.py:115-175, into the causal real-time streams
+ * and revise_skes_real_time) for C cameras of P = num_person slots each, one frame per camera and tick; slot p of
+ * camera c is row c * P + p.  A slot is bound to a SORT id: it keeps that id's stream across ticks.
+ * gast_live_slots: reads gast_sort_update's outputs of C sequences x 1 frame as they are (rows (C, capacity, 5),
+ *   counts (C), sort_status (C)) and selects a frame's tracks as gen_img_kpts does (k <= 0: none, k = 1: row 0,
+ *   k >= P: rows k-1 .. k-P; 2 <= k < P: none and GAST_REC_ST_TRACKS), without round(v, 2).  The slot book (3, C, P)
+ *   int64 holds per slot its id (the row's fifth column, -1 none), the last tick it was selected (-1 never) and
+ *   whether its stream must restart; initialise it to (-1, -1, 1).  A selected id that holds a slot keeps it; the
+ *   other selected ids, in selection order, take the free slots in ascending order, then the slots not selected this
+ *   tick with the oldest last tick (the lowest slot on a tie), and mark them to restart.  Per slot: slot_active (C * P)
+ *   int32, and the box's geometry as gast_track_records computes it: center_scale (C * P, 4) float32, forward_mats
+ *   (C * P, 6) float64 to the out_w x out_h crop and, when hw, hh > 0, inverse_mats (C * P, 6) float64 from the hw x hh
+ *   heatmap (hw = hh = 0: inverse_mats is not written).  A slot is inactive, and its center, scale and forward matrix
+ *   zero, when it holds no selected id, or its box is not finite or empty or its forward matrix not finite (the bit is
+ *   set).  status (C, 16) int64 per camera: [0] the sticky status word (SORT's word or'ed with the GAST_REC_ST_* bits),
+ *   [1] the ticks so far (the tick counter: initialise to 0), [2 + b] the tick that first set bit b < 12 (-1 none).
+ *   1 <= num_person <= 32.
+ * gast_live_inputs: the n = C * P slots' decoded COCO keypoints preds (n, 17, 2) and maxvals (n, 17) ->
+ *   gast_h36m_coco_format's H36M keypoints, scores, keep and valid of the one frame, gast_revise_kpts' repair: kpts
+ *   (n, 17, 2) and scores (n, 17); x (n, 17, 2) normalize_screen_coordinates(kpts, w = W, h = H).  active (n) uint8
+ *   = slot_active and keep and valid; an inactive slot's kpts, scores and x are zero.  The stream pool's device masks
+ *   fresh_mask and active_mask (copies * n int32, copies = 2 with test-time augmentation: slot s and its twin s + n)
+ *   get active and (active and restart); book_fresh (n) int64 (the book's third plane) is cleared for the active slots.
+ * gast_live_place: revise_skes_real_time(world[active slots of camera c], kpts[same], width) for every camera: world
+ *   (n, 17, 3) camera_to_world's poses, kpts (n, 17, 2), active (n) uint8 -> out (n, 17, 3), inactive slots zero.
+ * Device pointers, the caller's stream, no allocation, synchronisation or host read, so a tick can be captured in a
+ * graph; no atomics, calls repeat bit for bit.  Formulas in DESIGN.md §8.10. */
+int gast_live_slots(const double* rows, const int32_t* counts, const int32_t* sort_status, int32_t C, int32_t capacity,
+                    int32_t num_person, int32_t W, int32_t H, int32_t out_w, int32_t out_h, int32_t hw, int32_t hh,
+                    int64_t* book, int64_t* status, int32_t* slot_active, double* forward_mats, double* inverse_mats,
+                    float* center_scale, void* stream);
+int gast_live_inputs(const float* preds, const float* maxvals, const int32_t* slot_active, int32_t n, int32_t W,
+                     int32_t H, int32_t copies, int64_t* book_fresh, float* kpts, float* scores, float* x,
+                     int32_t* fresh_mask, int32_t* active_mask, uint8_t* active, void* stream);
+int gast_live_place(const float* world, const float* kpts, const uint8_t* active, int32_t C, int32_t num_person,
+                    double width, float* out, void* stream);
+
 /* optim.Adam(amsgrad=True) (trainval.py:78,162-164) for every parameter in one launch.  table (n_chunks,4)
  * int64 on the device: {param pointer, grad pointer, offset into the flat state buffers, count <=
  * gast_adam_chunk()}.  max_exp_avg_sq null = plain Adam.  step = 1 for the first update. */
