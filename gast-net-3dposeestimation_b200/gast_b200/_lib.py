@@ -1,47 +1,64 @@
 """ctypes binding of csrc/libgast_b200.so (C ABI: include/gast_b200.h).
 
+The header is the one statement of the ABI: every entry's argument and return types are read from its prototype
+when this module is imported, so there is no second copy to keep in step with it.  A parameter or return type
+outside the fixed map below raises RuntimeError here, before any call.
+
 There is no fallback: if the shared library is missing or fails to load, importing the
 engine raises with the build command.
 """
 import ctypes as C
 import os
+import re
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('GAST_B200_LIB') or os.path.join(os.path.dirname(_HERE), 'csrc', 'libgast_b200.so')
 # (GAST_B200_LIB: alternative build of the same library, used only for A/B experiments)
+HEADER = os.path.join(os.path.dirname(os.path.dirname(_HERE)), 'include', 'gast_b200.h')
 
 GAST_MAX_STAGES = 8
 KIND_MODEL, KIND_BLOCK, KIND_LOCAL, KIND_MGLOBAL, KIND_SEMCH, KIND_GLOBAL_HEAD = range(6)
 
-# every symbol include/gast_b200.h declares
-SYMBOLS = ['gast_create', 'gast_destroy', 'gast_bind', 'gast_prepare', 'gast_out_frames',
-           'gast_receptive_field', 'gast_workspace_bytes', 'gast_forward', 'gast_forward_mpjpe',
-           'gast_last_launch_count', 'gast_last_tc_launch_count', 'gast_set_timing',
-           'gast_get_timings', 'gast_set_gemm_core', 'gast_set_precision', 'gast_set_train_precision',
-           'gast_set_activation_dtype',
-           'gast_last_wgrad_tc_launch_count', 'gast_debug_gemm', 'gast_debug_wgrad', 'gast_debug_set_gemm_audit',
-           'gast_debug_gemm_audit_skips', 'gast_debug_set_kernel_audit', 'gast_debug_kernel_audit_skips',
-           'gast_bind_grads',
-           'gast_train_workspace_bytes', 'gast_forward_train', 'gast_backward', 'gast_backward_input',
-           'gast_eval_backward_workspace_bytes', 'gast_eval_backward', 'gast_chunked_workspace_bytes',
-           'gast_forward_chunked', 'gast_eval_backward_chunked', 'gast_set_dropout_state', 'gast_tta_prepare', 'gast_tta_merge',
-           'gast_stream_state_bytes', 'gast_stream_workspace_bytes', 'gast_stream_push',
-           'gast_stream_latency', 'gast_stream_push_ex', 'gast_stream_chunk_workspace_bytes', 'gast_stream_push_chunk',
-           'gast_stream_peek', 'gast_stream_subset_workspace_bytes', 'gast_stream_push_subset', 'gast_stream_peek_subset',
-           'gast_stream_device_workspace_bytes', 'gast_stream_push_device', 'gast_stream_peek_device',
-           'gast_stream_snapshot_floats', 'gast_stream_move_workspace_bytes', 'gast_stream_export',
-           'gast_stream_import', 'gast_chunk_gather', 'gast_keypoints_convert', 'gast_h36m_coco_format', 'gast_revise_kpts',
-           'gast_revise_skes_workspace_bytes', 'gast_revise_skes', 'gast_revise_skes_real_time_workspace_bytes',
-           'gast_revise_skes_real_time', 'gast_normalize_screen', 'gast_camera_to_world', 'gast_world_to_camera',
-           'gast_project_to_2d', 'gast_project_to_2d_backward', 'gast_normalize_screen_segments',
-           'gast_mpjpe_workspace_bytes', 'gast_mpjpe', 'gast_p_mpjpe', 'gast_pose_metrics_workspace_bytes',
-           'gast_pose_metrics', 'gast_render_geometry', 'gast_render_frames', 'gast_downsample_frames',
-           'gast_person_crops', 'gast_heatmap_decode', 'gast_letterbox', 'gast_person_detections',
-           'gast_sort_state_bytes', 'gast_sort_init', 'gast_sort_update', 'gast_track_records', 'gast_record_inverse',
-           'gast_live_slots', 'gast_live_inputs', 'gast_live_place',
-           'gast_adam_chunk', 'gast_adam_step', 'gast_chunk_gather_indexed',
-           'gast_adam_step_table', 'gast_adam_step_indexed', 'gast_epoch_loss_accumulate',
-           'gast_last_error', 'gast_version']
+# the C scalar types of the ABI; every pointer (function-pointer typedefs included) is bound as c_void_p
+_SCALARS = {'int32_t': C.c_int32, 'int': C.c_int, 'int64_t': C.c_int64, 'uint64_t': C.c_uint64, 'size_t': C.c_size_t,
+            'float': C.c_float, 'double': C.c_double}
+_RETURNS = dict(_SCALARS, **{'void': None, 'const char*': C.c_char_p})
+_PROTOTYPE = re.compile(r'(?P<ret>[\w\s*]+?)\s*\b(?P<name>gast_\w+)\s*\((?P<params>[^()]*)\)')
+_PARAM = re.compile(r'(?:const\s+)?(?P<type>\w+)(?P<ptr>(?:\s*\*\s*(?:const\b)?)*)\s*\w*')
+
+
+def prototypes(text):
+    """-> [(name, restype, argtypes)] of every gast_* function the C header `text` declares, in its order.
+    RuntimeError names the entry and the type when a parameter or return type has no binding."""
+    text = re.sub(r'/\*.*?\*/|//[^\n]*', ' ', text, flags=re.S)
+    text = re.sub(r'^\s*#[^\n]*', '', text, flags=re.M)
+    fn_pointers = set(re.findall(r'typedef[^;{}]*\(\s*\*\s*(\w+)\s*\)', text))
+    out = []
+    for stmt in re.split(r'[;{}]', text):
+        m = _PROTOTYPE.fullmatch(stmt.strip())
+        if m is None:
+            continue
+        name = m.group('name')
+        ret = ' '.join(m.group('ret').replace('*', ' * ').split()).replace(' *', '*')
+        if ret not in _RETURNS:
+            raise RuntimeError('gast_b200: %s returns %r, which has no ctypes binding' % (name, ret))
+        params = [p.strip() for p in m.group('params').split(',')]
+        argtypes = []
+        for p in ([] if params == ['void'] else params):
+            a = _PARAM.fullmatch(p)
+            if a is not None and (a.group('ptr') or a.group('type') in fn_pointers):
+                argtypes.append(C.c_void_p)
+            elif a is not None and a.group('type') in _SCALARS:
+                argtypes.append(_SCALARS[a.group('type')])
+            else:
+                raise RuntimeError('gast_b200: %s takes %r, which has no ctypes binding' % (name, p))
+        out.append((name, _RETURNS[ret], argtypes))
+    return out
+
+
+with open(HEADER) as _f:
+    _PROTOTYPES = prototypes(_f.read())
+SYMBOLS = [name for name, _, _ in _PROTOTYPES]          # every entry the header declares, in its order
 
 
 class GastCfg(C.Structure):
@@ -108,226 +125,9 @@ def load():
             'gast_b200: %s not found. Build it with `python __graft_entry__.py build` '
             '(or gast-net-3dposeestimation_b200/csrc/build.sh). There is no fallback path.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    vp = C.c_void_p
-    lib.gast_create.argtypes = [C.POINTER(vp), C.POINTER(GastCfg)]
-    lib.gast_create.restype = C.c_int
-    lib.gast_destroy.argtypes = [vp]
-    lib.gast_destroy.restype = None
-    lib.gast_bind.argtypes = [vp, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(vp), C.POINTER(C.c_int64)]
-    lib.gast_bind.restype = C.c_int
-    lib.gast_prepare.argtypes = [vp, vp]
-    lib.gast_prepare.restype = C.c_int
-    lib.gast_out_frames.argtypes = [vp, C.c_int32, C.c_int32]
-    lib.gast_out_frames.restype = C.c_int32
-    lib.gast_receptive_field.argtypes = [vp]
-    lib.gast_receptive_field.restype = C.c_int32
-    lib.gast_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32]
-    lib.gast_workspace_bytes.restype = C.c_size_t
-    lib.gast_forward.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, C.c_size_t, vp]
-    lib.gast_forward.restype = C.c_int
-    lib.gast_forward_mpjpe.argtypes = [vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, C.c_size_t, vp]
-    lib.gast_forward_mpjpe.restype = C.c_int
-    lib.gast_last_launch_count.argtypes = [vp]
-    lib.gast_last_launch_count.restype = C.c_int32
-    lib.gast_last_tc_launch_count.argtypes = [vp]
-    lib.gast_last_tc_launch_count.restype = C.c_int32
-    lib.gast_set_timing.argtypes = [vp, C.c_int32]
-    lib.gast_set_timing.restype = C.c_int
-    lib.gast_get_timings.argtypes = [vp, C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int32)]
-    lib.gast_get_timings.restype = C.c_int32
-    lib.gast_set_gemm_core.argtypes = [vp, C.c_int32]
-    lib.gast_set_gemm_core.restype = C.c_int
-    lib.gast_set_precision.argtypes = [vp, C.c_int32]
-    lib.gast_set_precision.restype = C.c_int
-    lib.gast_set_activation_dtype.argtypes = [vp, C.c_int32]
-    lib.gast_set_activation_dtype.restype = C.c_int
-    lib.gast_set_train_precision.argtypes = [vp, C.c_int32]
-    lib.gast_set_train_precision.restype = C.c_int
-    lib.gast_last_wgrad_tc_launch_count.argtypes = [vp]
-    lib.gast_last_wgrad_tc_launch_count.restype = C.c_int32
-    lib.gast_debug_gemm.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                    C.POINTER(C.c_float), vp]
-    lib.gast_debug_gemm.restype = C.c_int
-    lib.gast_debug_wgrad.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                     C.POINTER(C.c_float), vp]
-    lib.gast_debug_wgrad.restype = C.c_int
-    lib.gast_debug_set_gemm_audit.argtypes = [vp, GemmAuditFn, vp]
-    lib.gast_debug_set_gemm_audit.restype = C.c_int
-    lib.gast_debug_gemm_audit_skips.argtypes = [vp]
-    lib.gast_debug_gemm_audit_skips.restype = C.c_int64
-    lib.gast_debug_set_kernel_audit.argtypes = [vp, KernelAuditFn, vp]
-    lib.gast_debug_set_kernel_audit.restype = C.c_int
-    lib.gast_debug_kernel_audit_skips.argtypes = [vp]
-    lib.gast_debug_kernel_audit_skips.restype = C.c_int64
-    lib.gast_bind_grads.argtypes = [vp, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(vp), C.POINTER(C.c_int64)]
-    lib.gast_bind_grads.restype = C.c_int
-    lib.gast_train_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32, C.c_float]
-    lib.gast_train_workspace_bytes.restype = C.c_size_t
-    lib.gast_forward_train.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_float, C.c_uint64, vp, C.c_size_t, vp]
-    lib.gast_forward_train.restype = C.c_int
-    lib.gast_backward.argtypes = [vp, vp, vp, C.c_size_t, vp]
-    lib.gast_backward.restype = C.c_int
-    lib.gast_backward_input.argtypes = [vp, vp, vp, C.c_int32, vp, C.c_size_t, vp]
-    lib.gast_backward_input.restype = C.c_int
-    lib.gast_eval_backward_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32]
-    lib.gast_eval_backward_workspace_bytes.restype = C.c_size_t
-    lib.gast_eval_backward.argtypes = [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.c_size_t, vp]
-    lib.gast_eval_backward.restype = C.c_int
-    lib.gast_chunked_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]
-    lib.gast_chunked_workspace_bytes.restype = C.c_size_t
-    lib.gast_forward_chunked.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.c_size_t, vp]
-    lib.gast_forward_chunked.restype = C.c_int
-    lib.gast_eval_backward_chunked.argtypes = [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp,
-                                               C.c_size_t, vp]
-    lib.gast_eval_backward_chunked.restype = C.c_int
-    lib.gast_set_dropout_state.argtypes = [vp, vp]
-    lib.gast_set_dropout_state.restype = C.c_int
-    lib.gast_stream_state_bytes.argtypes = [vp, C.c_int32]
-    lib.gast_stream_state_bytes.restype = C.c_size_t
-    lib.gast_stream_workspace_bytes.argtypes = [vp, C.c_int32]
-    lib.gast_stream_workspace_bytes.restype = C.c_size_t
-    lib.gast_stream_push.argtypes = [vp, vp, C.c_int64, vp, vp, C.c_int32, vp, vp, C.c_size_t, vp]
-    lib.gast_stream_push.restype = C.c_int
-    lib.gast_stream_push_ex.argtypes = [vp, vp, C.c_int64, vp, vp, C.c_int32, vp, vp, vp, C.c_size_t, vp]
-    lib.gast_stream_push_ex.restype = C.c_int
-    lib.gast_stream_chunk_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32]
-    lib.gast_stream_chunk_workspace_bytes.restype = C.c_size_t
-    lib.gast_stream_push_chunk.argtypes = [vp, vp, C.c_int64, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, C.c_size_t, vp]
-    lib.gast_stream_push_chunk.restype = C.c_int
-    lib.gast_stream_peek.argtypes = [vp, vp, C.c_int64, vp, C.c_int32, C.c_int32, vp, C.c_size_t, vp]
-    lib.gast_stream_peek.restype = C.c_int
-    lib.gast_stream_subset_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32]
-    lib.gast_stream_subset_workspace_bytes.restype = C.c_size_t
-    lib.gast_stream_push_subset.argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp,
-                                            C.c_size_t, vp]
-    lib.gast_stream_push_subset.restype = C.c_int
-    lib.gast_stream_peek_subset.argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, C.c_int32, vp, vp, C.c_size_t, vp]
-    lib.gast_stream_peek_subset.restype = C.c_int
-    lib.gast_stream_device_workspace_bytes.argtypes = [vp, C.c_int32, C.c_int32]
-    lib.gast_stream_device_workspace_bytes.restype = C.c_size_t
-    lib.gast_stream_push_device.argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, vp, vp, vp, vp, vp, C.c_size_t, vp]
-    lib.gast_stream_push_device.restype = C.c_int
-    lib.gast_stream_peek_device.argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, vp, vp, C.c_size_t, vp]
-    lib.gast_stream_peek_device.restype = C.c_int
-    lib.gast_stream_snapshot_floats.argtypes = [vp]
-    lib.gast_stream_snapshot_floats.restype = C.c_size_t
-    lib.gast_stream_move_workspace_bytes.argtypes = [vp, C.c_int32]
-    lib.gast_stream_move_workspace_bytes.restype = C.c_size_t
-    for fn in ('gast_stream_export', 'gast_stream_import'):
-        getattr(lib, fn).argtypes = [vp, vp, C.c_int32, vp, vp, C.c_int32, vp, vp, C.c_size_t, vp]
-        getattr(lib, fn).restype = C.c_int
-    lib.gast_stream_latency.argtypes = [vp]
-    lib.gast_stream_latency.restype = C.c_int32
-    ip = C.POINTER(C.c_int32)
-    lib.gast_tta_prepare.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, ip, ip, vp]
-    lib.gast_tta_prepare.restype = C.c_int
-    lib.gast_tta_merge.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, ip, ip, vp]
-    lib.gast_tta_merge.restype = C.c_int
-    fp = C.POINTER(C.c_float)
-    lib.gast_chunk_gather.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                      C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, ip, ip, C.c_int32, ip, ip,
-                                      vp, vp, vp, vp]
-    lib.gast_chunk_gather.restype = C.c_int
-    lib.gast_keypoints_convert.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp]
-    lib.gast_keypoints_convert.restype = C.c_int
-    lib.gast_h36m_coco_format.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp]
-    lib.gast_h36m_coco_format.restype = C.c_int
-    lib.gast_revise_kpts.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp]
-    lib.gast_revise_kpts.restype = C.c_int
-    lib.gast_revise_skes_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
-    lib.gast_revise_skes_workspace_bytes.restype = C.c_size_t
-    lib.gast_revise_skes.argtypes = [vp, vp, C.POINTER(C.c_int64), C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp,
-                                     C.c_size_t, vp]
-    lib.gast_revise_skes.restype = C.c_int
-    lib.gast_revise_skes_real_time_workspace_bytes.argtypes = [C.c_int32]
-    lib.gast_revise_skes_real_time_workspace_bytes.restype = C.c_size_t
-    lib.gast_revise_skes_real_time.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, vp, vp, C.c_size_t, vp]
-    lib.gast_revise_skes_real_time.restype = C.c_int
-    lib.gast_normalize_screen.argtypes = [vp, vp, C.c_int64, C.c_float, C.c_float, C.c_int32, vp]
-    lib.gast_normalize_screen.restype = C.c_int
-    lib.gast_camera_to_world.argtypes = [vp, vp, C.c_int64, fp, fp, vp]
-    lib.gast_camera_to_world.restype = C.c_int
-    lib.gast_world_to_camera.argtypes = [vp, C.c_int64, C.c_int32, vp, vp, vp, C.c_int32, C.c_int64, C.c_int32, vp, vp]
-    lib.gast_world_to_camera.restype = C.c_int
-    lib.gast_project_to_2d.argtypes = [vp, C.c_int64, vp, vp, C.c_int32, vp, vp]
-    lib.gast_project_to_2d.restype = C.c_int
-    lib.gast_project_to_2d_backward.argtypes = [vp, C.c_int64, vp, vp, C.c_int32, vp, vp, vp]
-    lib.gast_project_to_2d_backward.restype = C.c_int
-    lib.gast_normalize_screen_segments.argtypes = [vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32, C.c_int64,
-                                                   C.c_int32, vp, vp]
-    lib.gast_normalize_screen_segments.restype = C.c_int
-    lib.gast_mpjpe_workspace_bytes.argtypes = []
-    lib.gast_mpjpe_workspace_bytes.restype = C.c_size_t
-    lib.gast_mpjpe.argtypes = [vp, vp, C.c_int64, C.c_int32, vp, vp, C.c_float, vp, vp]
-    lib.gast_mpjpe.restype = C.c_int
-    lib.gast_p_mpjpe.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, vp]
-    lib.gast_p_mpjpe.restype = C.c_int
-    lib.gast_pose_metrics_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int64]
-    lib.gast_pose_metrics_workspace_bytes.restype = C.c_size_t
-    lib.gast_pose_metrics.argtypes = [vp, vp, C.c_int64, C.c_int32, C.POINTER(C.c_int64), C.c_int32, fp, C.c_int32,
-                                      C.c_int32, C.c_int32, vp, vp, vp, C.c_size_t, vp]
-    lib.gast_pose_metrics.restype = C.c_int
-    lib.gast_render_geometry.argtypes = [C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float,
-                                         C.c_float, C.c_int32, fp]
-    lib.gast_render_geometry.restype = C.c_int
-    lib.gast_render_frames.argtypes = [vp, C.c_int64, C.c_int32, C.c_int32, vp, C.c_int32, C.c_int64, vp, C.c_int64,
-                                       C.c_int32, C.c_int32, ip, C.POINTER(C.c_uint8), ip, C.c_int32, C.c_int32,
-                                       C.c_int32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32,
-                                       C.c_int64, C.c_int32, vp, vp]
-    lib.gast_render_frames.restype = C.c_int
-    lib.gast_downsample_frames.argtypes = [vp, C.c_int64, C.c_int64, C.c_int32, C.c_int32, vp, vp]
-    lib.gast_downsample_frames.restype = C.c_int
-    lib.gast_person_crops.argtypes = [vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, C.c_int32, C.c_int32, C.c_int32,
-                                      C.c_int32, vp, vp]
-    lib.gast_person_crops.restype = C.c_int
-    lib.gast_heatmap_decode.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp]
-    lib.gast_heatmap_decode.restype = C.c_int
-    lib.gast_letterbox.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                   vp, vp]
-    lib.gast_letterbox.restype = C.c_int
-    lib.gast_person_detections.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.c_float, C.c_float,
-                                           C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp]
-    lib.gast_person_detections.restype = C.c_int
-    lib.gast_sort_state_bytes.argtypes = [C.c_int32, C.c_int32]
-    lib.gast_sort_state_bytes.restype = C.c_size_t
-    lib.gast_sort_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp]
-    lib.gast_sort_init.restype = C.c_int
-    lib.gast_sort_update.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
-    lib.gast_sort_update.restype = C.c_int
-    lib.gast_track_records.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                       C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp, vp]
-    lib.gast_track_records.restype = C.c_int
-    lib.gast_record_inverse.argtypes = [vp, C.c_int32, vp, C.c_int32, C.c_int32, vp, vp]
-    lib.gast_record_inverse.restype = C.c_int
-    # the live tick (DESIGN.md §8.10)
-    lib.gast_live_slots.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                    C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp, vp]
-    lib.gast_live_slots.restype = C.c_int
-    lib.gast_live_inputs.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp,
-                                     vp, vp]
-    lib.gast_live_inputs.restype = C.c_int
-    lib.gast_live_place.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_double, vp, vp]
-    lib.gast_live_place.restype = C.c_int
-    lib.gast_adam_chunk.argtypes = []
-    lib.gast_adam_chunk.restype = C.c_int32
-    lib.gast_adam_step.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,
-                                   C.c_double, C.c_int64, vp]
-    lib.gast_adam_step.restype = C.c_int
-    lib.gast_chunk_gather_indexed.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int64, C.c_int32, vp, C.c_int32,
-                                              C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                              C.c_int32, C.c_int32, ip, ip, C.c_int32, ip, ip, vp, vp, vp, vp]
-    lib.gast_chunk_gather_indexed.restype = C.c_int
-    lib.gast_adam_step_table.argtypes = [C.c_double, C.c_double, C.c_double, C.c_int64, C.c_int32, vp]
-    lib.gast_adam_step_table.restype = C.c_int
-    lib.gast_adam_step_indexed.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_double, C.c_double, C.c_double, C.c_double,
-                                           vp, C.c_int64, vp, vp]
-    lib.gast_adam_step_indexed.restype = C.c_int
-    lib.gast_epoch_loss_accumulate.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, vp, vp]
-    lib.gast_epoch_loss_accumulate.restype = C.c_int
-    lib.gast_last_error.argtypes = []
-    lib.gast_last_error.restype = C.c_char_p
-    lib.gast_version.argtypes = []
-    lib.gast_version.restype = C.c_char_p
+    for name, restype, argtypes in _PROTOTYPES:
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 

@@ -16,13 +16,10 @@ multiple of 32 above 32 or whose predictions do not fit one CTA's shared memory 
 not 3 * sum((inp_dim / s)^2) for s = 32, 16, 8 or whose last dimension is not 85, non-float32 predictions, and frame
 sizes that do not match the predictions.
 """
-import ctypes as C
-
 import numpy as np
 import torch
 
-from . import _lib as L
-from .engine import GastError, _check, _p, _stream
+from .engine import GastError, _launch, _p
 from .keypoints2d import _device, _on_device
 
 MAX_SIDE = 32767
@@ -78,9 +75,7 @@ def letterbox(frames, inp_dim=416, rgb_input=False):
     out = torch.empty((F, 3, D, D), dtype=torch.float32, device=dev)
     if F:
         fr = _on_device(frames, torch.uint8, dev, 'frames')
-        with torch.cuda.device(dev):
-            _check(L.load().gast_letterbox(_p(fr), F, H, W, D, nw, nh, RGB_INPUT if rgb_input else 0, _p(out),
-                                           C.c_void_p(_stream(dev))), 'gast_letterbox')
+        _launch(dev, 'gast_letterbox', _p(fr), F, H, W, D, nw, nh, RGB_INPUT if rgb_input else 0, _p(out))
     return out
 
 
@@ -133,11 +128,9 @@ def person_boxes(predictions, frame_sizes, inp_dim=416, confidence=0.7, nms_thre
     persons = torch.empty(F, dtype=torch.int32, device=dev) if extras else None
     if F:
         pred = _on_device(predictions, torch.float32, dev, 'predictions')
-        with torch.cuda.device(dev):
-            _check(L.load().gast_person_detections(
-                _p(pred), F, N, ATTRS, D, _p(sizes), float(np.float32(confidence)), float(np.float32(nms_thresh)), K,
-                RAW if raw else 0, _p(boxes), _p(scores), _p(counts), _p(mconf), _p(persons),
-                C.c_void_p(_stream(dev))), 'gast_person_detections')
+        _launch(dev, 'gast_person_detections', _p(pred), F, N, ATTRS, D, _p(sizes), float(np.float32(confidence)),
+                float(np.float32(nms_thresh)), K, RAW if raw else 0, _p(boxes), _p(scores), _p(counts), _p(mconf),
+                _p(persons))
     if extras:
         return boxes, scores, counts, mconf, persons
     return boxes, scores, counts

@@ -113,8 +113,20 @@ def refuse_half(module, what, instead):
 
 
 def _check(rc, what):
+    """GastError with the library's message unless rc, the result of a status entry, is 0"""
     if rc != 0:
         raise GastError('%s: %s' % (what, L.last_error()))
+
+
+def _call(entry, *args):
+    """call the library's status entry `entry` (0 on success); GastError with its message otherwise"""
+    _check(getattr(L.load(), entry)(*args), entry)
+
+
+def _launch(dev, entry, *args):
+    """_call on CUDA device `dev`, torch's current stream of `dev` appended as the entry's last argument"""
+    with torch.cuda.device(dev):
+        _call(entry, *args, _stream(dev))
 
 
 def _check_size(n, what):
@@ -208,7 +220,7 @@ class _Handle(object):
             cfg.con_rows, cfg.con_cols, cfg.con_nnz = r, c, n
             keep += [r, c]
         self.h = C.c_void_p()
-        _check(lib.gast_create(C.byref(self.h), C.byref(cfg)), 'gast_create')
+        _call('gast_create', C.byref(self.h), C.byref(cfg))
         self.sig = None
         self.core = None
         self.precision = 0
@@ -241,23 +253,23 @@ class _Handle(object):
         if self.precision == _PRECISIONS['fp16'] and prec != self.precision:
             self._set_precision(prec)
         if _FORCE_CORE['core'] != self.core:
-            _check(self.lib.gast_set_gemm_core(self.h, _FORCE_CORE['core']), 'gast_set_gemm_core')
+            _call('gast_set_gemm_core', self.h, _FORCE_CORE['core'])
             self.core = _FORCE_CORE['core']
         if prec != self.precision:
             self._set_precision(prec)
         tprec = _TRAIN_PRECISIONS[get_training_precision(module)]
         if tprec != self.train_precision:
-            _check(self.lib.gast_set_train_precision(self.h, tprec), 'gast_set_train_precision')
+            _call('gast_set_train_precision', self.h, tprec)
             self.train_precision = tprec
         if act != self.act_dtype:
             self._set_act(act)
 
     def _set_precision(self, prec):
-        _check(self.lib.gast_set_precision(self.h, prec), 'gast_set_precision')
+        _call('gast_set_precision', self.h, prec)
         self.precision = prec
 
     def _set_act(self, act):
-        _check(self.lib.gast_set_activation_dtype(self.h, act), 'gast_set_activation_dtype')
+        _call('gast_set_activation_dtype', self.h, act)
         self.act_dtype = act
 
     def refresh(self, module, stream):
@@ -270,7 +282,7 @@ class _Handle(object):
         # a half model: the library folds float32 parameters, so float32 copies are bound (kept until the next change)
         self.f32 = [(k, v.float() if v.dtype == torch.float16 else v) for k, v in items] if self.act_dtype else None
         _bind(self, 'gast_bind', self.f32 or items)
-        _check(self.lib.gast_prepare(self.h, C.c_void_p(stream)), 'gast_prepare')
+        _call('gast_prepare', self.h, C.c_void_p(stream))
         self.sig = sig
 
     def bind_only(self, module):
@@ -288,10 +300,9 @@ class _Handle(object):
         ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         tail = (B, T, strided_now, _p(ws), ws.numel(), C.c_void_p(stream))
         if target is None:
-            _check(self.lib.gast_forward(self.h, _p(x), _p(y), *tail), 'gast_forward')
+            _call('gast_forward', self.h, _p(x), _p(y), *tail)
         else:
-            _check(self.lib.gast_forward_mpjpe(self.h, _p(x), _p(target), _p(y), _p(loss), *tail),
-                   'gast_forward_mpjpe')
+            _call('gast_forward_mpjpe', self.h, _p(x), _p(target), _p(y), _p(loss), *tail)
 
     def launches(self):
         return int(self.lib.gast_last_launch_count(self.h))
@@ -319,7 +330,7 @@ def _bind(handle, entry, items):
         keys[i] = k.encode()
         ptrs[i] = v.data_ptr()
         numel[i] = v.numel()
-    _check(getattr(handle.lib, entry)(handle.h, n, keys, ptrs, numel), entry)
+    _call(entry, handle.h, n, keys, ptrs, numel)
 
 
 def _p(t):
@@ -389,9 +400,9 @@ class _TrainFn(torch.autograd.Function):
             seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if p > 0 else 0
             # device-side dropout counter (set by a graph-capturing trainer): keeps the masks fresh across replays
             ds = module.__dict__.get('_gast_dropout_state')
-            _check(lib.gast_set_dropout_state(handle.h, _p(ds)), 'gast_set_dropout_state')
-            _check(lib.gast_forward_train(handle.h, _p(x), _p(y), B, T, C.c_float(p), C.c_uint64(seed), _p(ws),
-                                          ws.numel(), C.c_void_p(st)), 'gast_forward_train')
+            _call('gast_set_dropout_state', handle.h, _p(ds))
+            _call('gast_forward_train', handle.h, _p(x), _p(y), B, T, C.c_float(p), C.c_uint64(seed), _p(ws),
+                  ws.numel(), C.c_void_p(st))
         # BatchNorm bookkeeping that torch does in Python: num_batches_tracked (this also bumps the
         # buffers' versions, so the eval-mode constants are refreshed on the next eval forward)
         with torch.no_grad():
@@ -408,7 +419,6 @@ class _TrainFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         handle, ws, names, params = ctx.handle, ctx.ws, ctx.names, ctx.params
-        lib = handle.lib
         n = len(params)
         need_x = ctx.needs_input_grad[2]
         need_p = any(ctx.needs_input_grad[4:])
@@ -423,10 +433,9 @@ class _TrainFn(torch.autograd.Function):
         dx = torch.empty_like(ctx.x) if need_x else None
         with torch.cuda.device(ctx.dev):
             views = _bind_grad_views(handle, names, params, direct, ctx.dev) if need_p else None
-            # no parameter needs a gradient (all frozen, only x is differentiated): the library skips every
-            # weight-gradient kernel
-            _check(lib.gast_backward_input(handle.h, _p(dy), _p(dx), 1 if need_p else 0, _p(ws), ws.numel(),
-                                           C.c_void_p(_stream(ctx.dev))), 'gast_backward')
+        # no parameter needs a gradient (all frozen, only x is differentiated): the library skips every
+        # weight-gradient kernel
+        _launch(ctx.dev, 'gast_backward_input', handle.h, _p(dy), _p(dx), 1 if need_p else 0, _p(ws), ws.numel())
         ctx.ws = None
         ctx.x = None
         if direct or views is None:
@@ -489,8 +498,8 @@ class _EvalFn(torch.autograd.Function):
             ws = torch.empty(need, dtype=torch.uint8, device=dev)
             dx = torch.empty_like(x) if need_x else None
             views = _bind_grad_views(h, ctx.names, params, False, dev) if need_p else None
-            _check(getattr(lib, entry)(h.h, _p(x), _p(dy), _p(dx), 1 if need_p else 0, B, T, ctx.sn, *plan, _p(ws),
-                                       ws.numel(), C.c_void_p(st)), entry)
+            _call(entry, h.h, _p(x), _p(dy), _p(dx), 1 if need_p else 0, B, T, ctx.sn, *plan, _p(ws), ws.numel(),
+                  C.c_void_p(st))
         return (None, None, dx, None, None, None) + (tuple(views) if views is not None else (None,) * ctx.n)
 
 
@@ -626,8 +635,8 @@ def _chunked_forward(module, h, x, strided_now, max_frames):
         need = _check_size(h.lib.gast_chunked_workspace_bytes(h.h, B, T, strided_now, max_frames, 0),
                            'gast_chunked_workspace_bytes')
         ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        _check(h.lib.gast_forward_chunked(h.h, _p(x), _p(y), B, T, strided_now, max_frames, _p(ws), ws.numel(),
-                                          C.c_void_p(st)), 'gast_forward_chunked')
+        _call('gast_forward_chunked', h.h, _p(x), _p(y), B, T, strided_now, max_frames, _p(ws), ws.numel(),
+              C.c_void_p(st))
     return y
 
 
@@ -699,7 +708,7 @@ def profile_forward(module, x, reps=5):
         run_model(module, x)
     h = module.__dict__['_gast_handles'][(dev.type, dev.index)]
     lib = h.lib
-    _check(lib.gast_set_timing(h.h, 1), 'gast_set_timing')
+    _call('gast_set_timing', h.h, 1)
     acc = {}
     n_launch = {}
     try:

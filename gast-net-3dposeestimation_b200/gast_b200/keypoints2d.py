@@ -23,13 +23,10 @@ side above 32767, heatmaps of more than 32 joints or with a side above 256, non-
 range, and in `video_keypoints` a frame with between 2 and num_person - 1 tracks (the reference's reshape raises).
 With DeviceSort's tracks these are found on the device and raised at the call's one copy, with the same messages.
 """
-import ctypes as C
-
 import numpy as np
 import torch
 
-from . import _lib as L
-from .engine import GastError, _check, _p, _stream
+from .engine import GastError, _launch, _p
 
 IMAGE_SIZE = (288, 384)          # w48_384x288: MODEL.IMAGE_SIZE (w, h)
 PIXEL_STD = 200
@@ -192,9 +189,7 @@ def crop_persons(frames, frame_index, forward_mats, size=IMAGE_SIZE, rgb_input=F
     if n and F:
         fr = _on_device(frames, torch.uint8, dev, 'frames')
         flags = (RGB_INPUT if rgb_input else 0) | (NET_ORDER if net_order else 0)
-        with torch.cuda.device(dev):
-            _check(L.load().gast_person_crops(_p(fr), F, H, W, _p(idx), _p(mats), n, w, h, flags, _p(out),
-                                              C.c_void_p(_stream(dev))), 'gast_person_crops')
+        _launch(dev, 'gast_person_crops', _p(fr), F, H, W, _p(idx), _p(mats), n, w, h, flags, _p(out))
     return out
 
 
@@ -227,9 +222,8 @@ def decode_heatmaps(heatmaps, inverse_mats, post_process=True):
     maxvals = torch.empty((n, J, 1), dtype=torch.float32, device=dev)
     if n:
         hm = _on_device(heatmaps, torch.float32, dev, 'heatmaps')
-        with torch.cuda.device(dev):
-            _check(L.load().gast_heatmap_decode(_p(hm), _p(mats), n, J, hh, hw, 1 if post_process else 0, _p(preds),
-                                                _p(maxvals), C.c_void_p(_stream(dev))), 'gast_heatmap_decode')
+        _launch(dev, 'gast_heatmap_decode', _p(hm), _p(mats), n, J, hh, hw, 1 if post_process else 0, _p(preds),
+                _p(maxvals))
     return preds, maxvals
 
 
@@ -404,10 +398,8 @@ def track_records(rows, counts, status, num_person, frame_size, image_size=IMAGE
     summary = torch.empty((S, 4), dtype=torch.int32, device=dev)
     total = torch.zeros(1, dtype=torch.int32, device=dev)
     R, N, st = R.contiguous(), N.to(device=dev).contiguous(), status.to(device=dev).contiguous()
-    with torch.cuda.device(dev):
-        _check(L.load().gast_track_records(_p(R), _p(N), _p(st), S, K, cap, num_person, W, H, w, h, _p(frame), _p(slot),
-                                           _p(forward), _p(cs), _p(summary), _p(total), C.c_void_p(_stream(dev))),
-               'gast_track_records')
+    _launch(dev, 'gast_track_records', _p(R), _p(N), _p(st), S, K, cap, num_person, W, H, w, h, _p(frame), _p(slot),
+            _p(forward), _p(cs), _p(summary), _p(total))
     return TrackRecords(frame, slot, forward, cs, summary, total)
 
 
@@ -421,9 +413,7 @@ def record_inverse(records, heatmap_size):
     dev = cs.device
     n = int(cs.shape[0])
     out = torch.empty((n, 2, 3), dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        _check(L.load().gast_record_inverse(_p(cs), n, _p(records.total), hw, hh, _p(out), C.c_void_p(_stream(dev))),
-               'gast_record_inverse')
+    _launch(dev, 'gast_record_inverse', _p(cs), n, _p(records.total), hw, hh, _p(out))
     return out
 
 

@@ -28,10 +28,9 @@ import ctypes as C
 import numpy as np
 import torch
 
-from . import _lib as L
 from . import detection as Dt
 from . import keypoints2d as K
-from .engine import GastError, _check, _p
+from .engine import GastError, _call, _p
 from .realtime import GraphedPoseStream
 from .tracking import SKIP_EMPTY, DeviceSort, status_message
 
@@ -185,42 +184,36 @@ class LiveTick(GraphedPoseStream):
     # ---- the tick -----------------------------------------------------------------------------------------------
     def _run(self, h, st):
         """enqueue one tick after the frame copy on stream `st` -> the library's launch count (the nets excluded)"""
-        lib, C_, n, P = h.lib, self.C, self.n, self.persons
+        C_, n, P = self.C, self.n, self.persons
         s = C.c_void_p(st)
         w, hh_ = K.IMAGE_SIZE
         hw, hh = self._hm
-        _check(lib.gast_letterbox(_p(self.frames), C_, self.H, self.W, self.D, self._nw, self._nh,
-                                  Dt.RGB_INPUT if self.rgb_input else 0, _p(self._batch), s), 'gast_letterbox')
+        _call('gast_letterbox', _p(self.frames), C_, self.H, self.W, self.D, self._nw, self._nh,
+              Dt.RGB_INPUT if self.rgb_input else 0, _p(self._batch), s)
         with torch.no_grad():
             pred = self._det()
-        _check(lib.gast_person_detections(_p(pred), C_, int(pred.shape[1]), Dt.ATTRS, self.D, _p(self._sizes),
-                                          self.confidence, self.nms_thresh, self.max_det, 0, _p(self._boxes),
-                                          _p(self._box_scores), _p(self._counts), None, None, s),
-               'gast_person_detections')
-        _check(lib.gast_sort_update(_p(self.sort.state), C_, self.capacity, 1, _p(self._boxes), _p(self._counts),
-                                    self.max_det, SKIP_EMPTY, _p(self._rows), _p(self._track_counts),
-                                    _p(self._sort_status), s), 'gast_sort_update')
-        _check(lib.gast_live_slots(_p(self._rows), _p(self._track_counts), _p(self._sort_status), C_, self.capacity, P,
-                                   self.W, self.H, w, hh_, hw, hh, _p(self._book), _p(self._status),
-                                   _p(self._slot_active), _p(self._fwd), _p(self._inv), _p(self._cs), s),
-               'gast_live_slots')
+        _call('gast_person_detections', _p(pred), C_, int(pred.shape[1]), Dt.ATTRS, self.D, _p(self._sizes),
+              self.confidence, self.nms_thresh, self.max_det, 0, _p(self._boxes), _p(self._box_scores),
+              _p(self._counts), None, None, s)
+        _call('gast_sort_update', _p(self.sort.state), C_, self.capacity, 1, _p(self._boxes), _p(self._counts),
+              self.max_det, SKIP_EMPTY, _p(self._rows), _p(self._track_counts), _p(self._sort_status), s)
+        _call('gast_live_slots', _p(self._rows), _p(self._track_counts), _p(self._sort_status), C_, self.capacity, P,
+              self.W, self.H, w, hh_, hw, hh, _p(self._book), _p(self._status), _p(self._slot_active), _p(self._fwd),
+              _p(self._inv), _p(self._cs), s)
         flags = (K.RGB_INPUT if self.rgb_input else 0) | K.NET_ORDER
-        _check(lib.gast_person_crops(_p(self.frames), C_, self.H, self.W, _p(self._frame_index), _p(self._fwd), n, w,
-                                     hh_, flags, _p(self._crops), s), 'gast_person_crops')
+        _call('gast_person_crops', _p(self.frames), C_, self.H, self.W, _p(self._frame_index), _p(self._fwd), n, w, hh_,
+              flags, _p(self._crops), s)
         with torch.no_grad():
             heat = self._pose()
-        _check(lib.gast_heatmap_decode(_p(heat), _p(self._inv), n, 17, hh, hw, 1, _p(self._preds), _p(self._maxvals),
-                                       s), 'gast_heatmap_decode')
+        _call('gast_heatmap_decode', _p(heat), _p(self._inv), n, 17, hh, hw, 1, _p(self._preds), _p(self._maxvals), s)
         N = self.copies * n
-        _check(lib.gast_live_inputs(_p(self._preds), _p(self._maxvals), _p(self._slot_active), n, self.W, self.H,
-                                    self.copies, _p(self._book[2]), _p(self._kpts), _p(self._scores), _p(self._x),
-                                    _p(self._mask_dev[:N]), _p(self._mask_dev[N:2 * N]), _p(self._active), s),
-               'gast_live_inputs')
+        _call('gast_live_inputs', _p(self._preds), _p(self._maxvals), _p(self._slot_active), n, self.W, self.H,
+              self.copies, _p(self._book[2]), _p(self._kpts), _p(self._scores), _p(self._x), _p(self._mask_dev[:N]),
+              _p(self._mask_dev[N:2 * N]), _p(self._active), s)
         launches = 9 + self._tick(h, st)
-        _check(lib.gast_camera_to_world(_p(self._y), _p(self._world), n * 17, self._q, self._t, s),
-               'gast_camera_to_world')
-        _check(lib.gast_live_place(_p(self._world), _p(self._kpts), _p(self._active), C_, P, float(self.W),
-                                   _p(self._poses), s), 'gast_live_place')
+        _call('gast_camera_to_world', _p(self._y), _p(self._world), n * 17, self._q, self._t, s)
+        _call('gast_live_place', _p(self._world), _p(self._kpts), _p(self._active), C_, P, float(self.W),
+              _p(self._poses), s)
         return launches
 
     def _eager(self, h, st):
@@ -301,14 +294,13 @@ class LiveTick(GraphedPoseStream):
         if cams.size and (cams.min() < 0 or cams.max() >= self.C or np.unique(cams).size != cams.size):
             raise GastError('LiveTick.reset: cameras must be distinct indices in [0, %d) (got %s)'
                             % (self.C, cams.tolist()))
-        srt, lib = self.sort, L.load()
+        srt = self.sort
         with torch.cuda.device(self.device):
             st = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
             next_ids = srt.header()[:, 1].clone()
             for c in cams.tolist():
-                _check(lib.gast_sort_init(C.c_void_p(srt.state.data_ptr() + c * srt.state_bytes), 1, self.capacity,
-                                          srt.max_age, srt.min_hits, C.c_void_p(next_ids[c:].data_ptr()), st),
-                       'gast_sort_init')
+                _call('gast_sort_init', C.c_void_p(srt.state.data_ptr() + c * srt.state_bytes), 1, self.capacity,
+                      srt.max_age, srt.min_hits, C.c_void_p(next_ids[c:].data_ptr()), st)
                 rows = slice(c * self.persons, (c + 1) * self.persons)
                 for plane, v in enumerate(BOOK_INIT):
                     self._book[plane, rows].fill_(v)

@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .engine import GastError, _check, _check_size, _cuda_f32, _ilist, _p, _stream
+from .engine import GastError, _call, _check_size, _cuda_f32, _ilist, _launch, _p
 
 KPT_COCO_H36M, KPT_MPII_H36M, KPT_COCO_H36M_TOE, KPT_COCO_HUMANEVA = 0, 1, 2, 3
 
@@ -69,11 +69,9 @@ def chunk_gather(seqs, pairs, chunk_length, pad, causal_shift=0, kps_left=None, 
     kr, _ = _ilist(kps_right)
     jl, n3 = _ilist(joints_left)
     jr, _ = _ilist(joints_right)
-    with torch.cuda.device(dev):
-        _check(L.load().gast_chunk_gather(_p(seqs.poses_2d), _p(seqs.poses_3d), _p(seqs.cameras), _p(seqs.seq_start),
-                                          seqs.n_seq, _p(pr), B, int(chunk_length), int(pad), int(causal_shift), J2, F2,
-                                          J3, ncam, n2, kl, kr, n3, jl, jr, _p(b2), _p(b3), _p(bc),
-                                          C.c_void_p(_stream(dev))), 'gast_chunk_gather')
+    _launch(dev, 'gast_chunk_gather', _p(seqs.poses_2d), _p(seqs.poses_3d), _p(seqs.cameras), _p(seqs.seq_start),
+            seqs.n_seq, _p(pr), B, int(chunk_length), int(pad), int(causal_shift), J2, F2, J3, ncam, n2, kl, kr, n3, jl,
+            jr, _p(b2), _p(b3), _p(bc))
     return bc, b3, b2
 
 
@@ -100,12 +98,10 @@ def chunk_gather_indexed(seqs, pairs, batch, B, batch_stride, chunk_length, pad,
     kr, _ = _ilist(kps_right)
     jl, n3 = _ilist(joints_left)
     jr, _ = _ilist(joints_right)
-    with torch.cuda.device(dev):
-        _check(L.load().gast_chunk_gather_indexed(_p(seqs.poses_2d), _p(seqs.poses_3d), _p(seqs.cameras),
-                                                  _p(seqs.seq_start), seqs.n_seq, _p(pairs), int(pairs.shape[0]),
-                                                  int(batch_stride), _p(batch), int(B), int(chunk_length), int(pad),
-                                                  int(causal_shift), J2, F2, J3, ncam, n2, kl, kr, n3, jl, jr, _p(b2),
-                                                  _p(b3), _p(bc), C.c_void_p(_stream(dev))), 'gast_chunk_gather_indexed')
+    _launch(dev, 'gast_chunk_gather_indexed', _p(seqs.poses_2d), _p(seqs.poses_3d), _p(seqs.cameras),
+            _p(seqs.seq_start), seqs.n_seq, _p(pairs), int(pairs.shape[0]), int(batch_stride), _p(batch), int(B),
+            int(chunk_length), int(pad), int(causal_shift), J2, F2, J3, ncam, n2, kl, kr, n3, jl, jr, _p(b2), _p(b3),
+            _p(bc))
     return bc, b3, b2
 
 
@@ -122,9 +118,7 @@ def keypoints_convert(kpts, mode):
     Jo = {KPT_COCO_H36M_TOE: 19, KPT_COCO_HUMANEVA: 15}.get(mode, 17)
     out = torch.empty((T, Jo, 2), dtype=torch.float32, device=k.device)
     valid = torch.empty((T,), dtype=torch.int32, device=k.device)
-    with torch.cuda.device(k.device):
-        _check(L.load().gast_keypoints_convert(_p(k), _p(out), _p(valid), T, Jin, int(mode), C.c_void_p(_stream(k.device))),
-               'gast_keypoints_convert')
+    _launch(k.device, 'gast_keypoints_convert', _p(k), _p(out), _p(valid), T, Jin, int(mode))
     return out, valid
 
 
@@ -133,9 +127,7 @@ def normalize_screen(x, w, h, inverse=False):
     x = _cuda_f32(x, 'normalize_screen')
     assert x.shape[-1] == 2
     out = torch.empty_like(x)
-    with torch.cuda.device(x.device):
-        _check(L.load().gast_normalize_screen(_p(x), _p(out), x.numel() // 2, float(w), float(h), 1 if inverse else 0,
-                                              C.c_void_p(_stream(x.device))), 'gast_normalize_screen')
+    _launch(x.device, 'gast_normalize_screen', _p(x), _p(out), x.numel() // 2, float(w), float(h), 1 if inverse else 0)
     return out
 
 
@@ -147,9 +139,7 @@ def camera_to_world(x, R, t=0):
     tv = np.broadcast_to(np.asarray(t, dtype=np.float32), (3,))
     tt = (C.c_float * 3)(*[float(v) for v in tv])
     out = torch.empty_like(x)
-    with torch.cuda.device(x.device):
-        _check(L.load().gast_camera_to_world(_p(x), _p(out), x.numel() // 3, q, tt, C.c_void_p(_stream(x.device))),
-               'gast_camera_to_world')
+    _launch(x.device, 'gast_camera_to_world', _p(x), _p(out), x.numel() // 3, q, tt)
     return out
 
 
@@ -177,10 +167,8 @@ def world_to_camera_segments(x, src_start, dst_start, qt, n_out, root_relative=F
     _table(src_start, torch.int64, (S,), dev, 'world_to_camera')
     _table(dst_start, torch.int64, (S + 1,), dev, 'world_to_camera')
     out = torch.empty((int(n_out), int(x.shape[1]), 3), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        _check(L.load().gast_world_to_camera(_p(x), int(x.shape[0]), int(x.shape[1]), _p(src_start), _p(dst_start), _p(qt),
-                                             S, int(n_out), 1 if root_relative else 0, _p(out), C.c_void_p(_stream(dev))),
-               'gast_world_to_camera')
+    _launch(dev, 'gast_world_to_camera', _p(x), int(x.shape[0]), int(x.shape[1]), _p(src_start), _p(dst_start), _p(qt),
+            S, int(n_out), 1 if root_relative else 0, _p(out))
     return out
 
 
@@ -207,19 +195,15 @@ def project_to_2d_segments(x, seg_start, intrinsics, grad_out=None):
     S = int(intrinsics.shape[0]) if isinstance(intrinsics, torch.Tensor) else 0
     _table(intrinsics, torch.float32, (S, 9), dev, 'project_to_2d')
     _table(seg_start, torch.int64, (S + 1,), dev, 'project_to_2d')
-    lib = L.load()
-    with torch.cuda.device(dev):
-        if grad_out is None:
-            out = torch.empty(tuple(x.shape[:-1]) + (2,), dtype=torch.float32, device=dev)
-            _check(lib.gast_project_to_2d(_p(x), n, _p(seg_start), _p(intrinsics), S, _p(out), C.c_void_p(_stream(dev))),
-                   'gast_project_to_2d')
-        else:
-            g = _cuda_f32(grad_out, 'project_to_2d backward')
-            if tuple(g.shape) != tuple(x.shape[:-1]) + (2,):
-                raise GastError('project_to_2d backward: grad (...,2) of the points expected, got %s' % (tuple(g.shape),))
-            out = torch.empty_like(x)
-            _check(lib.gast_project_to_2d_backward(_p(x), n, _p(seg_start), _p(intrinsics), S, _p(g), _p(out),
-                                                   C.c_void_p(_stream(dev))), 'gast_project_to_2d_backward')
+    if grad_out is None:
+        out = torch.empty(tuple(x.shape[:-1]) + (2,), dtype=torch.float32, device=dev)
+        _launch(dev, 'gast_project_to_2d', _p(x), n, _p(seg_start), _p(intrinsics), S, _p(out))
+    else:
+        g = _cuda_f32(grad_out, 'project_to_2d backward')
+        if tuple(g.shape) != tuple(x.shape[:-1]) + (2,):
+            raise GastError('project_to_2d backward: grad (...,2) of the points expected, got %s' % (tuple(g.shape),))
+        out = torch.empty_like(x)
+        _launch(dev, 'gast_project_to_2d_backward', _p(x), n, _p(seg_start), _p(intrinsics), S, _p(g), _p(out))
     return out
 
 
@@ -237,10 +221,8 @@ def normalize_screen_segments(x, src_start, dst_start, wh, n_out, from_image=Fal
     _table(dst_start, torch.int64, (S + 1,), dev, 'normalize_screen_segments')
     P, F = int(x.shape[1]), int(x.shape[2])
     out = torch.empty((int(n_out), P, F), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        _check(L.load().gast_normalize_screen_segments(_p(x), int(x.shape[0]), P, F, _p(src_start), _p(dst_start), _p(wh),
-                                                       S, int(n_out), 1 if from_image else 0, _p(out),
-                                                       C.c_void_p(_stream(dev))), 'gast_normalize_screen_segments')
+    _launch(dev, 'gast_normalize_screen_segments', _p(x), int(x.shape[0]), P, F, _p(src_start), _p(dst_start), _p(wh),
+            S, int(n_out), 1 if from_image else 0, _p(out))
     return out
 
 
@@ -268,9 +250,7 @@ def h36m_coco_format(kpts, scores):
     sout = torch.empty_like(s)
     valid = torch.empty((P, T), dtype=torch.int32, device=dev)
     keep = torch.empty((P,), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        _check(L.load().gast_h36m_coco_format(_p(k), _p(s), P, T, _p(out), _p(sout), _p(valid), _p(keep),
-                                              C.c_void_p(_stream(dev))), 'gast_h36m_coco_format')
+    _launch(dev, 'gast_h36m_coco_format', _p(k), _p(s), P, T, _p(out), _p(sout), _p(valid), _p(keep))
     return out, sout, valid, keep
 
 
@@ -283,9 +263,7 @@ def revise_kpts(kpts, scores, valid):
     v = valid.to(torch.int32).contiguous()
     P, T, J = (int(d) for d in k.shape[:3])
     out = torch.empty_like(k)
-    with torch.cuda.device(k.device):
-        _check(L.load().gast_revise_kpts(_p(k), _p(s), _p(v), P, T, J, _p(out), C.c_void_p(_stream(k.device))),
-               'gast_revise_kpts')
+    _launch(k.device, 'gast_revise_kpts', _p(k), _p(s), _p(v), P, T, J, _p(out))
     return out
 
 
@@ -303,12 +281,9 @@ def revise_skes(pred, frames, offsets, kpts):
     P, T, J, D = (int(d) for d in k.shape)
     dev = k.device
     out = torch.empty((P, T, J, 3), dtype=torch.float32, device=dev)
-    lib = L.load()
-    wb = int(lib.gast_revise_skes_workspace_bytes(P, T))
-    with torch.cuda.device(dev):
-        ws = _prep_ws(dev, wb)
-        _check(lib.gast_revise_skes(_p(pr), _p(fr), off.ctypes.data_as(C.POINTER(C.c_int64)), P, T, J, D, _p(k), _p(out),
-                                    _p(ws), ws.numel(), C.c_void_p(_stream(dev))), 'gast_revise_skes')
+    ws = _prep_ws(dev, L.load().gast_revise_skes_workspace_bytes(P, T))
+    _launch(dev, 'gast_revise_skes', _p(pr), _p(fr), off.ctypes.data_as(C.POINTER(C.c_int64)), P, T, J, D, _p(k),
+            _p(out), _p(ws), ws.numel())
     return out
 
 
@@ -322,12 +297,8 @@ def revise_skes_real_time(pred, kpts, width):
     M, J, D = int(pr.shape[0]), int(pr.shape[1]), int(k.shape[2])
     dev = pr.device
     out = torch.empty_like(pr)
-    lib = L.load()
-    wb = int(lib.gast_revise_skes_real_time_workspace_bytes(M))
-    with torch.cuda.device(dev):
-        ws = _prep_ws(dev, wb)
-        _check(lib.gast_revise_skes_real_time(_p(pr), _p(k), M, J, D, float(width), _p(out), _p(ws), ws.numel(),
-                                              C.c_void_p(_stream(dev))), 'gast_revise_skes_real_time')
+    ws = _prep_ws(dev, L.load().gast_revise_skes_real_time_workspace_bytes(M))
+    _launch(dev, 'gast_revise_skes_real_time', _p(pr), _p(k), M, J, D, float(width), _p(out), _p(ws), ws.numel())
     return out
 
 
@@ -350,9 +321,7 @@ class _MpjpeFn(torch.autograd.Function):
         loss = torch.empty((), dtype=torch.float32, device=p.device)
         need = predicted.requires_grad
         dp = torch.empty_like(p) if need else None
-        with torch.cuda.device(p.device):
-            _check(L.load().gast_mpjpe(_p(p), _p(t), p.numel() // D, D, _p(loss), _p(dp), 1.0, _p(_mpjpe_ws(p.device)),
-                                       C.c_void_p(_stream(p.device))), 'gast_mpjpe')
+        _launch(p.device, 'gast_mpjpe', _p(p), _p(t), p.numel() // D, D, _p(loss), _p(dp), 1.0, _p(_mpjpe_ws(p.device)))
         if need:
             ctx.save_for_backward(dp)
         return loss
@@ -375,8 +344,7 @@ def p_mpjpe_per_frame(predicted, target):
     assert p.shape == t.shape and p.dim() == 3 and p.shape[-1] == 3
     N, J = int(p.shape[0]), int(p.shape[1])
     out = torch.empty((N,), dtype=torch.float32, device=p.device)
-    with torch.cuda.device(p.device):
-        _check(L.load().gast_p_mpjpe(_p(p), _p(t), N, J, _p(out), C.c_void_p(_stream(p.device))), 'gast_p_mpjpe')
+    _launch(p.device, 'gast_p_mpjpe', _p(p), _p(t), N, J, _p(out))
     return out
 
 
@@ -396,16 +364,13 @@ def pose_metrics(predicted, target, seg_start, thresholds=(), zero_root=False, p
     thr = np.ascontiguousarray(np.asarray(thresholds, dtype=np.float32).reshape(-1))
     N, J, S = int(p.shape[0]), int(p.shape[1]), int(seg.size) - 1
     dev = p.device
-    lib = L.load()
-    wb = _check_size(lib.gast_pose_metrics_workspace_bytes(S, J, int(thr.size), N), 'pose_metrics')
+    wb = _check_size(L.load().gast_pose_metrics_workspace_bytes(S, J, int(thr.size), N), 'pose_metrics')
     rows = torch.empty((S, 3 + J + int(thr.size)), dtype=torch.float64, device=dev)
     dist = torch.empty((N, J), dtype=torch.float32, device=dev) if distances else None
-    with torch.cuda.device(dev):
-        ws = _prep_ws(dev, wb)
-        _check(lib.gast_pose_metrics(_p(p), _p(t), N, J, seg.ctypes.data_as(C.POINTER(C.c_int64)), S,
-                                     thr.ctypes.data_as(C.POINTER(C.c_float)), int(thr.size), 1 if zero_root else 0,
-                                     1 if procrustes else 0, _p(rows), _p(dist), _p(ws), ws.numel(),
-                                     C.c_void_p(_stream(dev))), 'gast_pose_metrics')
+    ws = _prep_ws(dev, wb)
+    _launch(dev, 'gast_pose_metrics', _p(p), _p(t), N, J, seg.ctypes.data_as(C.POINTER(C.c_int64)), S,
+            thr.ctypes.data_as(C.POINTER(C.c_float)), int(thr.size), 1 if zero_root else 0, 1 if procrustes else 0,
+            _p(rows), _p(dist), _p(ws), ws.numel())
     return (rows, dist) if distances else rows
 
 
@@ -413,8 +378,8 @@ def adam_step_table(lr, betas, first_step, n_steps):
     """(n_steps,2) float32 numpy: {lr / bc1, sqrt(bc2)} of steps first_step .. first_step + n_steps - 1, rounded as
     gast_adam_step rounds them (gast_adam_step_table), for FusedAdam.step_indexed."""
     out = np.empty((int(n_steps), 2), dtype=np.float32)
-    _check(L.load().gast_adam_step_table(float(lr), float(betas[0]), float(betas[1]), int(first_step), int(n_steps),
-                                         out.ctypes.data_as(C.c_void_p)), 'gast_adam_step_table')
+    _call('gast_adam_step_table', float(lr), float(betas[0]), float(betas[1]), int(first_step), int(n_steps),
+          out.ctypes.data_as(C.c_void_p))
     return out
 
 
@@ -426,9 +391,8 @@ def epoch_loss_accumulate(loss, weight, loss_sum, losses, batch):
             or batch.dtype != torch.int64 or {loss_sum.device, losses.device, batch.device} != {dev} or not loss.is_cuda:
         raise GastError('epoch_loss_accumulate: float32 loss, float64 sum, float32 losses and an int64 batch counter '
                         'on one CUDA device expected')
-    with torch.cuda.device(dev):
-        _check(L.load().gast_epoch_loss_accumulate(_p(loss), int(weight), _p(loss_sum), _p(losses), losses.numel(),
-                                                   _p(batch), C.c_void_p(_stream(dev))), 'gast_epoch_loss_accumulate')
+    _launch(dev, 'gast_epoch_loss_accumulate', _p(loss), int(weight), _p(loss_sum), _p(losses), losses.numel(),
+            _p(batch))
 
 
 class FusedAdam(object):
@@ -481,11 +445,9 @@ class FusedAdam(object):
         g = self.param_groups[0]
         self.step_count += 1
         dev = self.params[0].device
-        with torch.cuda.device(dev):
-            _check(L.load().gast_adam_step(_p(self._table), int(self._table.shape[0]), _p(self.exp_avg), _p(self.exp_avg_sq),
-                                           _p(self.max_exp_avg_sq), float(g['lr']), float(g['betas'][0]),
-                                           float(g['betas'][1]), float(g['eps']), float(g['weight_decay']),
-                                           self.step_count, C.c_void_p(_stream(dev))), 'gast_adam_step')
+        _launch(dev, 'gast_adam_step', _p(self._table), int(self._table.shape[0]), _p(self.exp_avg),
+                _p(self.exp_avg_sq), _p(self.max_exp_avg_sq), float(g['lr']), float(g['betas'][0]),
+                float(g['betas'][1]), float(g['eps']), float(g['weight_decay']), self.step_count)
         # the kernel writes the parameters through raw pointers: bump their version counters so that everything
         # keyed on (data_ptr, _version) -- the engine's folded eval-mode constants -- sees the update
         torch.autograd.graph.increment_version(self.params)
@@ -504,12 +466,9 @@ class FusedAdam(object):
                             'expected' % dev)
         self._build_table()
         g = self.param_groups[0]
-        with torch.cuda.device(dev):
-            _check(L.load().gast_adam_step_indexed(_p(self._table), int(self._table.shape[0]), _p(self.exp_avg),
-                                                   _p(self.exp_avg_sq), _p(self.max_exp_avg_sq), float(g['betas'][0]),
-                                                   float(g['betas'][1]), float(g['eps']), float(g['weight_decay']),
-                                                   _p(coef), int(coef.shape[0]), _p(batch), C.c_void_p(_stream(dev))),
-                   'gast_adam_step_indexed')
+        _launch(dev, 'gast_adam_step_indexed', _p(self._table), int(self._table.shape[0]), _p(self.exp_avg),
+                _p(self.exp_avg_sq), _p(self.max_exp_avg_sq), float(g['betas'][0]), float(g['betas'][1]),
+                float(g['eps']), float(g['weight_decay']), _p(coef), int(coef.shape[0]), _p(batch))
         torch.autograd.graph.increment_version(self.params)
 
     def state_dict(self):

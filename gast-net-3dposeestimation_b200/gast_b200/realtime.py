@@ -354,21 +354,24 @@ class PoseStream(object):
                                     % (type(self).__name__, self._ring, eng.get_precision(self.model), ring))
             self._state = None
         if self._state is None:
-            eng._check(lib.gast_stream_latency(h.h) != self.latency, 'gast_stream_latency')
+            latency = lib.gast_stream_latency(h.h)
+            if latency != self.latency:
+                raise eng.GastError('%s: gast_stream_latency gives this model a latency of %d pushes (-1: it cannot '
+                                    'stream), the pool expects %d' % (type(self).__name__, latency, self.latency))
             nb = eng._check_size(lib.gast_stream_state_bytes(h.h, self.copies * self.n), 'gast_stream_state_bytes')
             self._state = torch.zeros(nb, dtype=torch.uint8, device=self.device)
             self._ring = ring
 
-    def _mirror(self, lib, x, x2, rows, st):
+    def _mirror(self, x, x2, rows, st):
         """x2 (2, rows, J, F) = [x | x mirrored]: the library input of the twins of x (rows, J, F) (gast_tta_prepare)"""
-        self.engine._check(lib.gast_tta_prepare(x.data_ptr(), x2.data_ptr(), rows, self.J, self.F, 0, 0,
-                                                len(self.kps_left), self._kl, self._kr, st), 'gast_tta_prepare')
+        self.engine._call('gast_tta_prepare', x.data_ptr(), x2.data_ptr(), rows, self.J, self.F, 0, 0,
+                          len(self.kps_left), self._kl, self._kr, st)
 
-    def _merge(self, lib, y2, y, rows, st):
+    def _merge(self, y2, y, rows, st):
         """y (rows, J, 3) = the mean of the twins' poses y2 (2, rows, J, 3), the mirrored one un-mirrored
         (gast_tta_merge)"""
-        self.engine._check(lib.gast_tta_merge(y2.data_ptr(), y.data_ptr(), rows, self.J, len(self.joints_left),
-                                              self._jl, self._jr, st), 'gast_tta_merge')
+        self.engine._call('gast_tta_merge', y2.data_ptr(), y.data_ptr(), rows, self.J, len(self.joints_left), self._jl,
+                          self._jr, st)
 
     def push(self, frame, streams=None):
         """frame (n_streams, J, in_features): the newest 2D keypoints of every stream (normalised screen
@@ -466,7 +469,7 @@ class PoseStream(object):
                 if frames is not None:
                     # (2, m, K, J, F) = 2m library streams of K frames: [original | mirrored]
                     x = torch.empty((2,) + tuple(frames.shape), dtype=torch.float32, device=self.device)
-                    self._mirror(lib, frames, x, r * K, st)
+                    self._mirror(frames, x, r * K, st)
                 out = torch.empty((2, r, K, self.J, 3), dtype=torch.float32, device=self.device)
             state = self._state.data_ptr()
             if single:
@@ -480,10 +483,10 @@ class PoseStream(object):
                     fn, args = 'gast_stream_peek_subset', table + (out.data_ptr(),)
                 else:
                     fn, args = 'gast_stream_push_subset', table + (x.data_ptr(), out.data_ptr(), fresh_p, hold_p)
-            eng._check(getattr(lib, fn)(h.h, *args, self._ws.data_ptr(), self._ws.numel(), st), fn)
+            eng._call(fn, h.h, *args, self._ws.data_ptr(), self._ws.numel(), st)
             launches = int(lib.gast_last_launch_count(h.h))
             if self.augment:
-                self._merge(lib, out, yr, r * K, st)
+                self._merge(out, yr, r * K, st)
                 launches += 2
             if r < rows.size:
                 y[torch.from_numpy(np.flatnonzero(keep)).to(self.device)] = yr
@@ -519,8 +522,8 @@ class PoseStream(object):
         # not self._ws: a GraphedPoseStream's graph keeps that buffer's address
         ws = torch.empty(wb, dtype=torch.uint8, device=self.device)
         st = torch.cuda.current_stream(self.device).cuda_stream
-        eng._check(getattr(lib, fn)(h.h, self._state.data_ptr(), self.copies * self.n, lib_streams.ctypes.data,
-                                    lib_counts.ctypes.data, mm, data.data_ptr(), ws.data_ptr(), ws.numel(), st), fn)
+        eng._call(fn, h.h, self._state.data_ptr(), self.copies * self.n, lib_streams.ctypes.data,
+                  lib_counts.ctypes.data, mm, data.data_ptr(), ws.data_ptr(), ws.numel(), st)
         self.last_launches = int(lib.gast_last_launch_count(h.h))
 
     def export_streams(self, streams):
@@ -687,21 +690,20 @@ class GraphedPoseStream(PoseStream):
         x, y, py = self._x, self._y, self._py
         launches = 0
         if self.augment:
-            self._mirror(lib, x, self._x2, n * K, st)
+            self._mirror(x, self._x2, n * K, st)
             x, y, py = self._x2, self._y2, self._py2
             launches += 1
-        eng._check(lib.gast_stream_push_device(h.h, state, N, counts, active, K, x.data_ptr(), y.data_ptr(), fresh,
-                                               hold, ws, wn, st), 'gast_stream_push_device')
+        eng._call('gast_stream_push_device', h.h, state, N, counts, active, K, x.data_ptr(), y.data_ptr(), fresh, hold,
+                  ws, wn, st)
         launches += int(lib.gast_last_launch_count(h.h))
         if self.augment:
-            self._merge(lib, y, self._y, n * K, st)
+            self._merge(y, self._y, n * K, st)
             launches += 1
         if P:
-            eng._check(lib.gast_stream_peek_device(h.h, state, N, counts, active, P, py.data_ptr(), ws, wn, st),
-                       'gast_stream_peek_device')
+            eng._call('gast_stream_peek_device', h.h, state, N, counts, active, P, py.data_ptr(), ws, wn, st)
             launches += int(lib.gast_last_launch_count(h.h))
             if self.augment:
-                self._merge(lib, py, self._py, n * P, st)
+                self._merge(py, self._py, n * P, st)
                 launches += 1
         return launches
 

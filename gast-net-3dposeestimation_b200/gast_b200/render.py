@@ -17,8 +17,7 @@ import subprocess
 import numpy as np
 import torch
 
-from . import _lib as L
-from .engine import GastError, _check, _p, _stream
+from .engine import GastError, _call, _launch, _p
 
 ELEV = 15.0             # view_init(elev=15.)
 RADIUS = 1.7            # the axis limits' radius
@@ -56,8 +55,8 @@ def geometry(S, dpi, Hin, Win, azim, shared=False, elev=ELEV, radius=RADIUS, dis
     """the library's float32 geometry of a call (gast_render_geometry): the 3D rows, the image fit, the coverage
     edges and S/2 -- what tests/renderref.py restates the kernel with"""
     geo = (C.c_float * 20)()
-    _check(L.load().gast_render_geometry(int(S), float(dpi), int(Hin), int(Win), float(elev), float(azim), float(radius),
-                                         float(dist), 1 if shared else 0, geo), 'gast_render_geometry')
+    _call('gast_render_geometry', int(S), float(dpi), int(Hin), int(Win), float(elev), float(azim), float(radius),
+          float(dist), 1 if shared else 0, geo)
     return np.array(geo[:], dtype=np.float32)
 
 
@@ -98,9 +97,8 @@ def downsample_frames(x, factor):
     for s in x.shape[1:]:
         row *= int(s)
     if n and row:
-        with torch.cuda.device(x.device):
-            _check(L.load().gast_downsample_frames(_p(x), int(x.shape[0]), row, factor, 0 if x.dtype == torch.float32 else 1,
-                                                   _p(out), C.c_void_p(_stream(x.device))), 'gast_downsample_frames')
+        _launch(x.device, 'gast_downsample_frames', _p(x), int(x.shape[0]), row, factor,
+                0 if x.dtype == torch.float32 else 1, _p(out))
     return out
 
 
@@ -232,13 +230,11 @@ class Scene(object):
             out = out.view(-1)[:int(np.prod(shape))].view(shape)
         if f1 > f0:
             v = self.video
-            with torch.cuda.device(self.device):
-                _check(L.load().gast_render_frames(
-                    _p(self.keypoints), int(self.keypoints.shape[0]), self.M, self.J, _p(self.poses),
-                    int(self.poses.shape[0]), int(self.poses.shape[1]), _p(v), int(v.shape[0]) if v is not None else 0,
-                    self.Hin, self.Win, self._parents, self._colors, self._right, self._n_right, self.n_bones, self.S,
-                    self.dpi, ELEV, self.azim, RADIUS, DIST, self.flags, f0, f1 - f0, _p(out),
-                    C.c_void_p(_stream(self.device))), 'gast_render_frames')
+            _launch(self.device, 'gast_render_frames', _p(self.keypoints), int(self.keypoints.shape[0]), self.M, self.J,
+                    _p(self.poses), int(self.poses.shape[0]), int(self.poses.shape[1]), _p(v),
+                    int(v.shape[0]) if v is not None else 0, self.Hin, self.Win, self._parents, self._colors,
+                    self._right, self._n_right, self.n_bones, self.S, self.dpi, ELEV, self.azim, RADIUS, DIST,
+                    self.flags, f0, f1 - f0, _p(out))
         return out
 
 

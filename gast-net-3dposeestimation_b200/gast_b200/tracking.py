@@ -12,13 +12,11 @@ with the Kalman gain cannot follow OpenBLAS's order).  Where the reference raise
 denominator) or goes out of step (an infinite predicted box), and where a count or the tracker list does not fit,
 the sequence's status word is set and host_tracks raises GastError.
 """
-import ctypes as C
-
 import numpy as np
 import torch
 
 from . import _lib as L
-from .engine import GastError, _check, _p, _stream
+from .engine import GastError, _launch, _p
 from .keypoints2d import _device, _on_device
 
 SKIP_EMPTY = 1                   # GAST_SORT_SKIP_EMPTY
@@ -50,9 +48,8 @@ class DeviceSort:
         self.state = torch.empty(int(n), dtype=torch.uint8, device=self.device)
         ids = np.broadcast_to(np.asarray(first_id, np.int64), (self.S,))
         first = _on_device(ids, torch.int64, self.device, 'first_id')
-        with torch.cuda.device(self.device):
-            _check(lib.gast_sort_init(_p(self.state), self.S, self.capacity, self.max_age, self.min_hits, _p(first),
-                                      C.c_void_p(_stream(self.device))), 'gast_sort_init')
+        _launch(self.device, 'gast_sort_init', _p(self.state), self.S, self.capacity, self.max_age, self.min_hits,
+                _p(first))
 
     def header(self):
         """(S, 8) int64 view of each sequence's header words on the device (index 1: the next id)"""
@@ -89,10 +86,8 @@ class DeviceSort:
         rows = torch.empty((S, K, self.capacity, 5), dtype=torch.float64, device=dev)
         out_counts = torch.empty((S, K), dtype=torch.int32, device=dev)
         status = torch.empty(S, dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            _check(L.load().gast_sort_update(_p(self.state), S, self.capacity, K, _p(b), _p(n), M,
-                                             SKIP_EMPTY if skip_empty else 0, _p(rows), _p(out_counts), _p(status),
-                                             C.c_void_p(_stream(dev))), 'gast_sort_update')
+        _launch(dev, 'gast_sort_update', _p(self.state), S, self.capacity, K, _p(b), _p(n), M,
+                SKIP_EMPTY if skip_empty else 0, _p(rows), _p(out_counts), _p(status))
         if single:
             return rows[0], out_counts[0], status
         return rows, out_counts, status

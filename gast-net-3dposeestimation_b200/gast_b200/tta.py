@@ -9,8 +9,7 @@ instead of numpy on the host (common/generators.py:210-233) and torch indexing (
 import ctypes as C
 import torch
 
-from . import _lib as L
-from .engine import GastError, _check, _cuda_f32, _ilist, _stream, refuse_half
+from .engine import GastError, _cuda_f32, _ilist, _launch, refuse_half
 
 
 def tta_prepare(seq, pad, causal_shift, kps_left, kps_right):
@@ -20,10 +19,8 @@ def tta_prepare(seq, pad, causal_shift, kps_left, kps_right):
     out = torch.empty((2, T + 2 * pad, J, F), dtype=torch.float32, device=seq.device)
     kl, n = _ilist(kps_left)
     kr, _ = _ilist(kps_right)
-    with torch.cuda.device(seq.device):
-        _check(L.load().gast_tta_prepare(C.c_void_p(seq.data_ptr()), C.c_void_p(out.data_ptr()), T, J, F, int(pad),
-                                         int(causal_shift), n, kl, kr, C.c_void_p(_stream(seq.device))),
-               'gast_tta_prepare')
+    _launch(seq.device, 'gast_tta_prepare', C.c_void_p(seq.data_ptr()), C.c_void_p(out.data_ptr()), T, J, F, int(pad),
+            int(causal_shift), n, kl, kr)
     return out
 
 
@@ -36,9 +33,7 @@ def tta_merge(pred, joints_left, joints_right):
     out = torch.empty((T, J, 3), dtype=torch.float32, device=pred.device)
     jl, n = _ilist(joints_left)
     jr, _ = _ilist(joints_right)
-    with torch.cuda.device(pred.device):
-        _check(L.load().gast_tta_merge(C.c_void_p(pred.data_ptr()), C.c_void_p(out.data_ptr()), T, J, n, jl, jr,
-                                       C.c_void_p(_stream(pred.device))), 'gast_tta_merge')
+    _launch(pred.device, 'gast_tta_merge', C.c_void_p(pred.data_ptr()), C.c_void_p(out.data_ptr()), T, J, n, jl, jr)
     return out
 
 

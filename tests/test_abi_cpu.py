@@ -1,6 +1,8 @@
 """CPU checks of the boundary: the C-ABI library loads and exports every symbol that
-include/gast_b200.h declares; the drop-in modules keep the reference's API surface; and the
+include/gast_b200.h declares, the header declares every extern "C" definition under csrc/, and the
+ctypes bindings are those its prototypes state; the drop-in modules keep the reference's API surface; and the
 product path refuses to run without a GPU (no fallback)."""
+import ctypes as C
 import os
 import re
 import pytest
@@ -15,15 +17,57 @@ def _adj(J):
     return adj_mx_from_skeleton(Skeleton(synth.skeleton_parents(J), [], []))
 
 
+def _uncommented(path):
+    return re.sub(r'/\*.*?\*/|//[^\n]*', '', open(path).read(), flags=re.S)
+
+
 def test_library_exports_every_declared_symbol():
-    hdr = open(os.path.join(REPO, 'include', 'gast_b200.h')).read()
-    hdr = re.sub(r'/\*.*?\*/', '', hdr, flags=re.S)
+    hdr = _uncommented(os.path.join(REPO, 'include', 'gast_b200.h'))
     declared = set(re.findall(r'\b(gast_[a-z_0-9]+)\s*\(', hdr))
     assert declared == set(_lib.SYMBOLS), declared ^ set(_lib.SYMBOLS)
     lib = _lib.load()
     for s in declared:
         assert getattr(lib, s) is not None
     assert b'sm_90a' in lib.gast_version()
+
+
+def test_header_declares_every_extern_c_definition():
+    csrc = os.path.join(REPO, 'gast-net-3dposeestimation_b200', 'csrc')
+    defined = []
+    for f in sorted(os.listdir(csrc)):
+        if f.endswith(('.cu', '.cuh')):
+            defined += re.findall(r'extern\s+"C"\s+[\w\s*]*?\b(gast_\w+)\s*\(', _uncommented(os.path.join(csrc, f)))
+    assert defined and len(defined) == len(set(defined)) and len(_lib.SYMBOLS) == len(set(_lib.SYMBOLS))
+    assert set(defined) == set(_lib.SYMBOLS), set(defined) ^ set(_lib.SYMBOLS)
+
+
+def test_bindings_derived_from_the_header():
+    lib = _lib.load()
+    train = lib.gast_forward_train.argtypes
+    assert len(train) == 10 and train[6] is C.c_uint64 and train[5] is C.c_float and train[0] is C.c_void_p
+    assert lib.gast_last_error.restype is C.c_char_p and lib.gast_version.restype is C.c_char_p
+    assert lib.gast_destroy.restype is None
+    assert lib.gast_adam_chunk.argtypes == [] and lib.gast_adam_chunk.restype is C.c_int32
+    assert lib.gast_debug_set_gemm_audit.argtypes == [C.c_void_p] * 3            # a callback typedef is a pointer
+    assert lib.gast_bind.argtypes == [C.c_void_p, C.c_int32] + [C.c_void_p] * 3
+    assert lib.gast_workspace_bytes.restype is C.c_size_t
+
+
+def test_prototype_parser():
+    hdr = '''#define X 1
+    typedef int (*gast_cb_fn)(int32_t phase, void* user);   /* a comment: int gast_ghost(int); */
+    typedef struct gast_s { const float* p; int32_t n; } gast_s;
+    int gast_a(const gast_s* const* s, int64_t n, double w, gast_cb_fn fn, uint64_t seed);
+    size_t gast_b(void);
+    void gast_c(float x, int k, size_t n);
+    const char* gast_d(void);'''
+    assert _lib.prototypes(hdr) == [
+        ('gast_a', C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_uint64]),
+        ('gast_b', C.c_size_t, []), ('gast_c', None, [C.c_float, C.c_int, C.c_size_t]), ('gast_d', C.c_char_p, [])]
+    for bad in ('int gast_e(unsigned n);', 'int gast_e(long long n);', 'int gast_e(float q[4]);',
+                'int gast_e(enum gast_kind k);', 'void* gast_e(void);', 'uint8_t gast_e(void);'):
+        with pytest.raises(RuntimeError, match='gast_e'):
+            _lib.prototypes(hdr + '\n' + bad)
 
 
 def test_star_import_namespace_and_state_dict_keys():
