@@ -178,7 +178,7 @@ extern "C" int gast_forward_chunked(gast_t* h, const float* x, float* y, int32_t
   if (call_begin(h, "gast_forward_chunked", need, workspace, workspace_bytes)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long xrow = (long long)h->cfg.num_joints * h->cfg.in_features, yrow = (long long)h->cfg.num_joints * 3;
-  const size_t es = h->act_dtype == GAST_F16 ? sizeof(__half) : sizeof(float);   // bytes per element of x and y
+  const size_t es = with_types(h, [](auto io, auto) { return sizeof(typename decltype(io)::type); });   // of x and y
   for (long long p = 0; p < pl.passes; ++p) {
     const ChunkPass q = chunk_pass(pl, B, T, p);
     const char* xp = reinterpret_cast<const char*>(x) + ((long long)q.b0 * T + q.f0) * xrow * es;

@@ -10,6 +10,7 @@
 #include <string.h>
 #include <algorithm>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -111,7 +112,7 @@ struct gast_handle {
   int gemm_core = 0;                 // 0 auto (tensor cores where possible), 1 force FFMA
   int precision = 0;                 // 0 fp32-grade (3xFP16 on scaled operands in inference, 3xTF32 in training),
                                      // 1 single-pass TF32 (inference only), 16 fp16 (inference only: the half form's
-                                     // arithmetic and fp16 activations behind float32 x and y, act_f16)
+                                     // arithmetic and fp16 activations behind float32 x and y, with_types)
   int act_dtype = GAST_F32;          // activation type of the model forward (gast_set_activation_dtype)
   int train_precision = 0;           // training and every gradient: 0 fp32-grade, 1 single-pass TF32 (forward and
                                      // input-gradient GEMMs) with the TF32 weight-gradient kernel (wgrad_tc.cuh)
@@ -136,12 +137,27 @@ constexpr int GAST_MAX_PENDING_TRAIN = 16;   // training forwards that may wait 
 enum { LK_EXPAND = 0, LK_GEMM_PLAIN = 1, LK_GEMM_SEMCH = 2, LK_GEMM_GLOBAL = 3, LK_ROWDOT = 4, LK_SHRINK = 5,
        LK_TC_PLAIN = 6, LK_TC_SEMCH = 7, LK_TC_GLOBAL = 8, LK_GLOBAL_MIX = 9 };
 
-// Whether the activations of an inference forward or stream call are fp16: in a half model (act_dtype, which also makes
-// x and y fp16) and at the fp16 precision (x, y and the streams' input history stay float32).  Training and every
-// gradient keep fp32 activations at any inference precision: they run only where precision_check lets them.
-static bool act_f16(const gast_handle* h) { return h->act_dtype == GAST_F16 || h->precision == 16; }
+template <typename T>
+struct Elem { using type = T; };   // an element type as a value, for with_types' callback
 
-static size_t act_esize(const gast_handle* h) { return act_f16(h) ? sizeof(__half) : sizeof(float); }
+template <typename T>
+constexpr int32_t elem_dtype = std::is_same<T, __half>::value ? GAST_F16 : GAST_F32;   // the audit records' type code
+
+// The element types of an inference forward or stream call, and the only reading of act_dtype and precision that picks
+// them: f(Elem<Io>(), Elem<Act>()) with Io the type of the model's x and y and Act that of the activations between
+// layers.  A half model (act_dtype) has both fp16; the fp16 precision has fp16 activations behind float32 x and y (and
+// the streams' input history); else both are float32.  Training and every gradient keep fp32 activations at any
+// inference precision (they run only where precision_check lets them) and do not call this.
+template <typename F>
+static auto with_types(const gast_handle* h, F f) {
+  if (h->act_dtype == GAST_F16) return f(Elem<__half>(), Elem<__half>());
+  if (h->precision == 16) return f(Elem<float>(), Elem<__half>());
+  return f(Elem<float>(), Elem<float>());
+}
+
+static size_t act_esize(const gast_handle* h) {
+  return with_types(h, [](auto, auto act) { return sizeof(typename decltype(act)::type); });
+}
 
 // The refusal of every entry that half does not run: training, every backward, the streams, the mpjpe forward
 static int half_check(const gast_handle* h, const char* who) {
@@ -774,12 +790,18 @@ static int audited_launch(cudaStream_t st, AuditHook<Rec>& a, Fill fill, Launch 
   return 0;
 }
 
+// One expand, row-dot, attention-mix or shrink launch: audited, timed as `kind` (LK_*) and counted unless launch() refuses
 template <typename Fill, typename Launch>
-static int kernel_audited(gast_handle* h, cudaStream_t st, Fill fill, Launch launch) {
+static int kernel_audited(gast_handle* h, cudaStream_t st, int kind, Fill fill, Launch launch) {
   return audited_launch(st, h->kernel_audit, [&](gast_kernel_audit& d) {
     d.gemm_index = h->gemm_audit.index;
     fill(d);
-  }, launch);
+  }, [&] {
+    TimedLaunch tl(h, st, kind);
+    if (launch()) return 1;
+    h->launches++;
+    return 0;
+  });
 }
 
 // the audit record of a launch (gast_gemm_audit mirrors GemmP); prec < 0: the FFMA core
@@ -818,18 +840,14 @@ static int launch_gemm_core(gast_handle* h, cudaStream_t st, int epi, const Gemm
   int hpt = 1;
   if (epi == EPI_GLOBAL) hpt = p.heads < 4 ? p.heads : 4;
   size_t smem = ffma_smem_bytes(epi, p.J, p.fpt, hpt);
+  const auto kernel = with_epi(epi, [](auto e) { return gemm_ffma_kernel<decltype(e)::value>; });
   static bool attr_set_dev[64][3];          // the opt-in is per device (one handle per device in one process)
   bool& attr_done = attr_set_dev[h->cfg.device & 63][epi];
   if (!attr_done) {
-    const void* fn = epi == EPI_PLAIN ? (const void*)gemm_ffma_kernel<EPI_PLAIN>
-                   : epi == EPI_SEMCH ? (const void*)gemm_ffma_kernel<EPI_SEMCH>
-                                      : (const void*)gemm_ffma_kernel<EPI_GLOBAL>;
-    CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    CUDA_OK(cudaFuncSetAttribute((const void*)kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     attr_done = true;
   }
-  if (epi == EPI_PLAIN) gemm_ffma_kernel<EPI_PLAIN><<<grid, FF_THREADS, smem, st>>>(p);
-  else if (epi == EPI_SEMCH) gemm_ffma_kernel<EPI_SEMCH><<<grid, FF_THREADS, smem, st>>>(p);
-  else gemm_ffma_kernel<EPI_GLOBAL><<<grid, FF_THREADS, smem, st>>>(p);
+  kernel<<<grid, FF_THREADS, smem, st>>>(p);
   h->launches++;
   return 0;
 }
@@ -875,40 +893,32 @@ extern "C" int64_t gast_debug_kernel_audit_skips(const gast_t* h) { return h ? h
 
 enum { KA_EXPAND = 0, KA_ROWDOT = 1, KA_MIX = 2, KA_SHRINK = 3, KA_SHRINK_MPJPE = 4 };
 
-// xf16: X holds fp16 (act_f16 in inference; training passes false)
-static int launch_rowdot(gast_handle* h, cudaStream_t st, const float* X, int ldx, const BlockConsts& b,
-                         float* ab, long long rows, bool xf16) {
+// Act: the element type of X (with_types' Act; training passes float).  The row dots stay fp32 (they feed the softmax).
+template <typename Act>
+static int launch_rowdot(gast_handle* h, cudaStream_t st, Elem<Act>, const float* X, int ldx, const BlockConsts& b,
+                         float* ab, long long rows) {
   if (rows <= 0) return 0;
+  constexpr bool f16 = std::is_same<Act, __half>::value;
   const int Q = 2 * b.heads;
   unsigned blocks = cdiv(rows * 32, 256);
   // rowdot8_kernel stages U in 48 KB of shared memory; its float32 form also reads X in float4 of 4 channels
-  const bool r8 = Q == 8 && (size_t)8 * b.C * sizeof(float) <= 48 * 1024 && (xf16 || b.C % 4 == 0);
+  const bool r8 = Q == 8 && (size_t)8 * b.C * sizeof(float) <= 48 * 1024 && (f16 || b.C % 4 == 0);
   auto fill = [&](gast_kernel_audit& d) {
     d.kind = KA_ROWDOT; d.variant = r8 ? 0 : Q; d.block = (int)(&b - h->blocks.data());
-    d.in_type = xf16; d.x = X; d.U = b.U; d.cab = b.cab; d.ab = ab; d.rows = rows; d.K = b.C; d.ld = ldx;
+    d.in_type = elem_dtype<Act>; d.x = X; d.U = b.U; d.cab = b.cab; d.ab = ab; d.rows = rows; d.K = b.C; d.ld = ldx;
     d.heads = b.heads;
   };
-  return kernel_audited(h, st, fill, [&] {
-    TimedLaunch tl(h, st, LK_ROWDOT);
-    if (xf16) {   // X holds fp16; the row dots stay fp32 (they feed the softmax)
-      const __half* Xh = reinterpret_cast<const __half*>(X);
-      if (r8) {
-        unsigned g = (unsigned)std::min<long long>((rows * 32 + 255) / 256, (long long)h->sm_count * 8);
-        rowdot8_kernel<<<g, 256, sizeof(float) * 8 * b.C, st>>>(Xh, ldx, b.U, b.cab, ab, rows, b.C);
-      } else if (Q == 8) rowdot_kernel<8><<<blocks, 256, 0, st>>>(Xh, ldx, b.U, b.cab, ab, rows, b.C);
-      else return fail("internal: fp16 forward with heads=%d", b.heads);
-      h->launches++;
-      return 0;
-    }
+  return kernel_audited(h, st, LK_ROWDOT, fill, [&] {
+    const Act* x = reinterpret_cast<const Act*>(X);
     if (r8) {
       unsigned g = (unsigned)std::min<long long>((rows * 32 + 255) / 256, (long long)h->sm_count * 8);
-      rowdot8_kernel<<<g, 256, sizeof(float) * 8 * b.C, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
-    } else if (Q == 8) rowdot_kernel<8><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
-    else if (Q == 6) rowdot_kernel<6><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
-    else if (Q == 4) rowdot_kernel<4><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
-    else if (Q == 2) rowdot_kernel<2><<<blocks, 256, 0, st>>>(X, ldx, b.U, b.cab, ab, rows, b.C);
+      rowdot8_kernel<<<g, 256, sizeof(float) * 8 * b.C, st>>>(x, ldx, b.U, b.cab, ab, rows, b.C);
+    } else if (Q == 8) rowdot_kernel<8><<<blocks, 256, 0, st>>>(x, ldx, b.U, b.cab, ab, rows, b.C);
+    else if constexpr (f16) return fail("internal: fp16 forward with heads=%d", b.heads);   // no fp16 form below
+    else if (Q == 6) rowdot_kernel<6><<<blocks, 256, 0, st>>>(x, ldx, b.U, b.cab, ab, rows, b.C);
+    else if (Q == 4) rowdot_kernel<4><<<blocks, 256, 0, st>>>(x, ldx, b.U, b.cab, ab, rows, b.C);
+    else if (Q == 2) rowdot_kernel<2><<<blocks, 256, 0, st>>>(x, ldx, b.U, b.cab, ab, rows, b.C);
     else return fail("internal: heads=%d", b.heads);
-    h->launches++;
     return 0;
   });
 }
@@ -940,7 +950,7 @@ static int run_local(gast_handle* h, cudaStream_t st, BlockConsts& b, const floa
 static int run_global(gast_handle* h, cudaStream_t st, BlockConsts& b, const float* X, long long F,
                       const BlockBufs& w, float* out_G, int kind) {
   const int C = b.C, J = h->cfg.num_joints, Ng = b.heads * b.Cg;
-  if (launch_rowdot(h, st, X, C, b, w.AB, F * J, act_f16(h))) return 1;
+  if (with_types(h, [&](auto, auto act) { return launch_rowdot(h, st, act, X, C, b, w.AB, F * J); })) return 1;
   GemmP p;
   // tensor-core core, block / MultiGlobalGraph: plain `g` GEMM (flat 128-row tiles) into out_G as scratch, then the
   // attention mix as its own full-occupancy kernel into Y.  Measured faster than the mix fused into the GEMM
@@ -955,22 +965,19 @@ static int run_global(gast_handle* h, cudaStream_t st, BlockConsts& b, const flo
     int fpb = GV >= MIX_THREADS ? 1 : MIX_THREADS / GV;
     fpb = std::max(1, std::min(fpb, (int)(40 * 1024 / (sizeof(float) * b.heads * J * MIX_JP))));   // attention rows fit 40 KB
     const size_t smem = sizeof(float) * (size_t)fpb * b.heads * J * MIX_JP;
-    auto fill = [&](gast_kernel_audit& d) {
-      d.kind = KA_MIX; d.fpb = fpb; d.block = (int)(&b - h->blocks.data());
-      d.in_type = d.out_type = act_f16(h); d.x = out_G; d.ab = w.AB; d.Ck = b.Ck; d.out = w.Y;
-      d.rows = F; d.K = Ng; d.ld = Ng; d.J = J; d.heads = b.heads; d.Cg = b.Cg;
-    };
-    if (kernel_audited(h, st, fill, [&] {
-          TimedLaunch tl(h, st, LK_GLOBAL_MIX);
-          if (act_f16(h))
-            global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(reinterpret_cast<const __half*>(out_G), Ng,
-                                                                       w.AB, b.Ck, reinterpret_cast<__half*>(w.Y), Ng,
-                                                                       F, J, b.heads, b.Cg, fpb);
-          else
-            global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(out_G, Ng, w.AB, b.Ck, w.Y, Ng, F, J, b.heads,
-                                                                       b.Cg, fpb);
-          h->launches++;
-          return 0;
+    if (with_types(h, [&](auto, auto act) {
+          using Act = typename decltype(act)::type;
+          auto fill = [&](gast_kernel_audit& d) {
+            d.kind = KA_MIX; d.fpb = fpb; d.block = (int)(&b - h->blocks.data());
+            d.in_type = d.out_type = elem_dtype<Act>; d.x = out_G; d.ab = w.AB; d.Ck = b.Ck; d.out = w.Y;
+            d.rows = F; d.K = Ng; d.ld = Ng; d.J = J; d.heads = b.heads; d.Cg = b.Cg;
+          };
+          return kernel_audited(h, st, LK_GLOBAL_MIX, fill, [&] {
+            global_mix_kernel<<<cdiv(F, fpb), MIX_THREADS, smem, st>>>(reinterpret_cast<const Act*>(out_G), Ng, w.AB,
+                                                                       b.Ck, reinterpret_cast<Act*>(w.Y), Ng, F, J,
+                                                                       b.heads, b.Cg, fpb);
+            return 0;
+          });
         }))
       return 1;
     CUDA_OK(cudaGetLastError());
@@ -1014,46 +1021,22 @@ static int launch_expand(gast_handle* h, cudaStream_t st, const float* x, float*
   const int k0 = c.filter_widths[0], Fin = c.in_features;
   if (rows >= 0x7fffffffLL) return fail("expand: more than 2^31 positions in one call");
   if (k0 * Fin > EXP_MAXKF) return fail("expand: filter_width*in_features > %d unsupported", EXP_MAXKF);
-  auto fill = [&](gast_kernel_audit& d) {
-    d.kind = KA_EXPAND; d.variant = k0 * Fin <= 6 ? 6 : EXP_MAXKF;
-    d.in_type = h->act_dtype == GAST_F16; d.out_type = act_f16(h); d.x = x; d.We = h->We; d.be = h->be; d.out = out;
-    d.rows = rows; d.K = c.channels; d.ld = c.channels; d.J = c.num_joints; d.T = T; d.T0 = T0; d.stride = stride;
-    d.taps = k0; d.Fin = Fin;
-  };
-  return kernel_audited(h, st, fill, [&] {
-    TimedLaunch tl(h, st, LK_EXPAND);
-    const dim3 grid(cdiv(rows, EXS_ROWS), cdiv(c.channels, EXS_CHUNK));
-    if (h->act_dtype == GAST_F32 && act_f16(h)) {   // the fp16 precision: float32 x, fp16 out
-      __half* oh = reinterpret_cast<__half*>(out);
-      if (k0 * Fin <= 6)
-        expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, oh, rows, c.num_joints, T, T0, stride, k0,
-                                                             Fin, c.channels);
-      else
-        expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, oh, rows, c.num_joints, T, T0,
-                                                                     stride, k0, Fin, c.channels);
-      h->launches++;
+  return with_types(h, [&](auto io, auto act) {
+    using Io = typename decltype(io)::type;
+    using Act = typename decltype(act)::type;
+    auto fill = [&](gast_kernel_audit& d) {
+      d.kind = KA_EXPAND; d.variant = k0 * Fin <= 6 ? 6 : EXP_MAXKF;
+      d.in_type = elem_dtype<Io>; d.out_type = elem_dtype<Act>; d.x = x; d.We = h->We; d.be = h->be; d.out = out;
+      d.rows = rows; d.K = c.channels; d.ld = c.channels; d.J = c.num_joints; d.T = T; d.T0 = T0; d.stride = stride;
+      d.taps = k0; d.Fin = Fin;
+    };
+    return kernel_audited(h, st, LK_EXPAND, fill, [&] {
+      const dim3 grid(cdiv(rows, EXS_ROWS), cdiv(c.channels, EXS_CHUNK));
+      const auto kernel = k0 * Fin <= 6 ? expand_rows_kernel<6, Io, Act> : expand_rows_kernel<EXP_MAXKF, Io, Act>;
+      kernel<<<grid, EXS_THREADS, 0, st>>>(reinterpret_cast<const Io*>(x), h->We, h->be, reinterpret_cast<Act*>(out),
+                                           rows, c.num_joints, T, T0, stride, k0, Fin, c.channels);
       return 0;
-    }
-    if (h->act_dtype == GAST_F16) {
-      const __half* xh = reinterpret_cast<const __half*>(x);
-      __half* oh = reinterpret_cast<__half*>(out);
-      if (k0 * Fin <= 6)
-        expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(xh, h->We, h->be, oh, rows, c.num_joints, T, T0, stride,
-                                                             k0, Fin, c.channels);
-      else
-        expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(xh, h->We, h->be, oh, rows, c.num_joints, T, T0,
-                                                                     stride, k0, Fin, c.channels);
-      h->launches++;
-      return 0;
-    }
-    if (k0 * Fin <= 6)
-      expand_rows_kernel<6><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, out, rows, c.num_joints, T, T0, stride, k0,
-                                                           Fin, c.channels);
-    else
-      expand_rows_kernel<EXP_MAXKF><<<grid, EXS_THREADS, 0, st>>>(x, h->We, h->be, out, rows, c.num_joints, T, T0,
-                                                                   stride, k0, Fin, c.channels);
-    h->launches++;
-    return 0;
+    });
   });
 }
 
@@ -1085,36 +1068,30 @@ static int launch_shrink(gast_handle* h, cudaStream_t st, const float* X, float*
   if (target && !scratch) return fail("gast_forward_mpjpe: no loss scratch in the workspace");
   // a fresh workspace is not zeroed: clear the ticket on the call's stream (a captured graph replays this memset too)
   if (target) CUDA_OK(cudaMemsetAsync(scratch + 2 * SHL_MAXBLOCKS, 0, sizeof(unsigned), st));
-  auto fill = [&](gast_kernel_audit& d) {
-    d.kind = target ? KA_SHRINK_MPJPE : KA_SHRINK;
-    d.in_type = act_f16(h); d.out_type = h->act_dtype == GAST_F16; d.x = X; d.Ws = ws; d.target = target;
-    d.loss = loss; d.out = y; d.rows = rows; d.K = Cl; d.ld = Cl;
-  };
-  return kernel_audited(h, st, fill, [&] {
-    TimedLaunch tl(h, st, LK_SHRINK);
-    if (target) {
-      double* partial = reinterpret_cast<double*>(scratch);
-      unsigned* ticket = reinterpret_cast<unsigned*>(scratch + 2 * SHL_MAXBLOCKS);
-      const unsigned nb = (unsigned)std::min<long long>(SHL_MAXBLOCKS, (rows + 7) / 8);
-      if (act_f16(h))   // the fp16 precision (a half model refuses the mpjpe forward): fp16 X, float32 y
-        shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws, y, rows, Cl, target,
-                                                partial, ticket, loss);
-      else
-        shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(X, Cl, ws, y, rows, Cl, target, partial, ticket, loss);
-    } else if (h->act_dtype == GAST_F32 && act_f16(h)) {
-      shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws, y, rows, Cl);
-    } else if (h->act_dtype == GAST_F16) {
-      shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(X), Cl, ws,
-                                                          reinterpret_cast<__half*>(y), rows, Cl);
-    } else {
-      shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(X, Cl, ws, y, rows, Cl);
-    }
-    h->launches++;
-    return 0;
+  return with_types(h, [&](auto io, auto act) {
+    using Io = typename decltype(io)::type;
+    using Act = typename decltype(act)::type;
+    auto fill = [&](gast_kernel_audit& d) {
+      d.kind = target ? KA_SHRINK_MPJPE : KA_SHRINK;
+      d.in_type = elem_dtype<Act>; d.out_type = elem_dtype<Io>; d.x = X; d.Ws = ws; d.target = target;
+      d.loss = loss; d.out = y; d.rows = rows; d.K = Cl; d.ld = Cl;
+    };
+    return kernel_audited(h, st, LK_SHRINK, fill, [&] {
+      const Act* x = reinterpret_cast<const Act*>(X);
+      if (target) {   // y, target and the loss are float32 (a half model refuses the mpjpe forward)
+        double* partial = reinterpret_cast<double*>(scratch);
+        unsigned* ticket = reinterpret_cast<unsigned*>(scratch + 2 * SHL_MAXBLOCKS);
+        const unsigned nb = (unsigned)std::min<long long>(SHL_MAXBLOCKS, (rows + 7) / 8);
+        shrink_mpjpe_kernel<<<nb, 256, 0, st>>>(x, Cl, ws, y, rows, Cl, target, partial, ticket, loss);
+      } else {
+        shrink_kernel<<<cdiv(rows * 32, 256), 256, 0, st>>>(x, Cl, ws, reinterpret_cast<Io*>(y), rows, Cl);
+      }
+      return 0;
+    });
   });
 }
 
-// In a half forward (gast_set_activation_dtype) and at the fp16 precision (act_f16) every buffer but bb.AB holds fp16:
+// In a half forward (gast_set_activation_dtype) and at the fp16 precision (with_types) every buffer but bb.AB holds fp16:
 // the pointers are typed float and the launches reinterpret them.
 struct ModelBufs {
   float* act[2];

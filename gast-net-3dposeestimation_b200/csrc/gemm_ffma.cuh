@@ -12,6 +12,7 @@
 // This is the exact-fp32 core: used for shapes the tensor-core core does not take (K % 32 != 0,
 // tiny widths) and as the on-GPU cross-check of the tensor-core path.
 #pragma once
+#include <type_traits>
 #include "gast_common.cuh"
 
 namespace gast {
@@ -23,6 +24,14 @@ constexpr int FF_THREADS = 256;
 constexpr int FF_LDS = FF_BM + 4;  // smem leading dim (floats), keeps float4 alignment
 
 enum { EPI_PLAIN = 0, EPI_SEMCH = 1, EPI_GLOBAL = 2 };
+
+// f(std::integral_constant<int, EPI_*>()) for the runtime epilogue epi, so that a launch picks its kernel template once
+template <typename F>
+inline auto with_epi(int epi, F f) {
+  if (epi == EPI_PLAIN) return f(std::integral_constant<int, EPI_PLAIN>());
+  if (epi == EPI_SEMCH) return f(std::integral_constant<int, EPI_SEMCH>());
+  return f(std::integral_constant<int, EPI_GLOBAL>());
+}
 
 // dynamic smem (floats): main loop tiles, reused by the epilogues
 //   main loop : 2 * BK * LDS (A) + 2 * BK * LDS (B)

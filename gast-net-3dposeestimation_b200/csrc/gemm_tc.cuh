@@ -1289,13 +1289,12 @@ inline int tc_launch_h(cudaStream_t st, int epi, const GemmP& p, const TcWeights
   const dim3 grid((unsigned)(((p.F + p.fpt - 1) / p.fpt) * ((p.N + TC_BN - 1) / TC_BN)));
   const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
   const size_t smem = tch_smem_bytes(epi, p.J, p.fpt, hpt);
+  const auto kernel = epi == EPI_PLAIN ? gemm_tc_h_kernel<EPI_PLAIN> : gemm_tc_h_kernel<EPI_SEMCH>;
   static bool attr_set[64][3];
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr_set[dev & 63][epi]) {
-    const void* fn = epi == EPI_PLAIN ? (const void*)gemm_tc_h_kernel<EPI_PLAIN>
-                                      : (const void*)gemm_tc_h_kernel<EPI_SEMCH>;
-    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX);
+    cudaError_t e = cudaFuncSetAttribute((const void*)kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX);
     if (e != cudaSuccess) return (int)e;
     attr_set[dev & 63][epi] = true;
   }
@@ -1304,8 +1303,7 @@ inline int tc_launch_h(cudaStream_t st, int epi, const GemmP& p, const TcWeights
   for (int s = 0; s < p.nseg; ++s)
     if (tc_seg_tma_h(p.seg[s]) && tc_encode_a16(&am.seg[s], p.seg[s].base, p.seg[s].Kc, rows, p.seg[s].ld)) return -1;
   if (epi == EPI_PLAIN && tc_encode_rows16(&am.out, p.out, p.N, rows, p.ld_out, p.fpt * p.J)) return -1;
-  if (epi == EPI_PLAIN) gemm_tc_h_kernel<EPI_PLAIN><<<grid, TC_THREADS, smem, st>>>(p, t.map_h16hi, am, t.sw);
-  else gemm_tc_h_kernel<EPI_SEMCH><<<grid, TC_THREADS, smem, st>>>(p, t.map_h16hi, am, t.sw);
+  kernel<<<grid, TC_THREADS, smem, st>>>(p, t.map_h16hi, am, t.sw);
   return (int)cudaGetLastError();
 }
 
@@ -1314,15 +1312,13 @@ inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeig
   const int tiles = ((p.F + p.fpt - 1) / p.fpt) * ((p.N + TC_BN - 1) / TC_BN);
   const int hpt = epi == EPI_GLOBAL ? (p.heads < 4 ? p.heads : 4) : 1;
   const size_t smem = tc_smem_bytes(PREC, epi, p.J, p.fpt, hpt);
+  const auto kernel = with_epi(epi, [](auto e) { return gemm_tc_kernel<decltype(e)::value, PREC>; });
   static bool attr_set[64][3];              // the shared-memory opt-in is per device
   static int sms[64];
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr_set[dev & 63][epi]) {
-    const void* fn = epi == EPI_PLAIN ? (const void*)gemm_tc_kernel<EPI_PLAIN, PREC>
-                   : epi == EPI_SEMCH ? (const void*)gemm_tc_kernel<EPI_SEMCH, PREC>
-                                      : (const void*)gemm_tc_kernel<EPI_GLOBAL, PREC>;
-    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_OPTIN);
+    cudaError_t e = cudaFuncSetAttribute((const void*)kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_OPTIN);
     if (e != cudaSuccess) return (int)e;
     e = cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev);
     if (e != cudaSuccess) return (int)e;
@@ -1347,9 +1343,7 @@ inline int tc_launch_prec(cudaStream_t st, int epi, const GemmP& p, const TcWeig
   if (epi == EPI_SEMCH && tc_encode_semch(&am.out, p.out, p.C, p.N / (TC_BN * p.tiles_per_mask), rows, p.ld_out,
                                           p.fpt * p.J))
     return -1;
-  if (epi == EPI_PLAIN) gemm_tc_kernel<EPI_PLAIN, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw, mres);
-  else if (epi == EPI_SEMCH) gemm_tc_kernel<EPI_SEMCH, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw, mres);
-  else gemm_tc_kernel<EPI_GLOBAL, PREC><<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw, mres);
+  kernel<<<grid, TC_THREADS, smem, st>>>(p, mhi, mlo, am, t.sw, mres);
   return (int)cudaGetLastError();
 }
 

@@ -743,14 +743,11 @@ static int move_call(const char* who, bool import, gast_handle* h, void* state, 
   int rows = 0;
   for (int q = 0; q < p.nparts; ++q) rows += p.part[q].R;
   const dim3 grid((unsigned)rows, (unsigned)std::min(m, 65535));
-  char* sbase = align256(state);
-  if (sp.esize == sizeof(__half)) {
-    if (import) stream_move_kernel<true, __half><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
-    else stream_move_kernel<false, __half><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
-  } else {
-    if (import) stream_move_kernel<true, float><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
-    else stream_move_kernel<false, float><<<grid, 256, 0, st>>>(sbase, snap, p, dtab, m);
-  }
+  with_types(h, [&](auto, auto act) {   // the rings hold activations
+    using Ring = typename decltype(act)::type;
+    const auto kernel = import ? stream_move_kernel<true, Ring> : stream_move_kernel<false, Ring>;
+    kernel<<<grid, 256, 0, st>>>(align256(state), snap, p, dtab, m);
+  });
   h->launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

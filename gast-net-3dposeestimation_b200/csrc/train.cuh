@@ -294,7 +294,7 @@ static int block_fwd(TCtx& c, TrainState& ts, BlockSave& b, BlockConsts& bc, con
   global_params(h, c.params, bc, gp, GAST_KIND_MGLOBAL, &gpar);
   if (c.live([&] { return prepare_global(h, c.st, bc, gpar, GAST_KIND_MGLOBAL); })) return 1;
   if (dense_nt(c, X, C, bc.Wg, M, C, C, b.G, C, bc.bg)) return 1;
-  if (c.live([&] { return launch_rowdot(h, c.st, X, C, bc, b.AB, M, false); })) return 1;
+  if (c.live([&] { return launch_rowdot(h, c.st, Elem<float>(), X, C, bc, b.AB, M); })) return 1;
   c.launch(att_mix_fwd_kernel, (unsigned)F, 256, sizeof(float) * 4 * J * J, b.G, C, b.AB, bc.Ck, J, 4, C / 4, b.Y, C);
   if (dense_nt(c, b.Y, C, c.param(gp + "cat_conv.weight", (int64_t)C * C), M, C, C, b.Zgc, C)) return 1;
   if (bn_fwd(c, b.bngc, gp + "cat_bn.", b.Zgc, C, M, C, 1, ts.drop_p, ts, nullptr, 0, id, b.Gl, C)) return 1;
