@@ -761,6 +761,52 @@ int gast_live_inputs(const float* preds, const float* maxvals, const int32_t* sl
 int gast_live_place(const float* world, const float* kpts, const uint8_t* active, int32_t C, int32_t num_person,
                     double width, float* out, void* stream);
 
+/* The delayed live tick of the non-causal models (latency = (receptive_field - 1) / 2 >= 1): each slot's stream holds
+ * one person's sequence, the frames where the slot was active joined across the ticks where it was not (gen_pose over
+ * valid_frames), and a push returns the pose of the frame the slot pushed latency pushes earlier.  seq (4, C * P)
+ * int64 per slot: the SORT id of its current sequence (-1 none), the tick of its last push (-1 never), the frames of
+ * the sequence (0: none pending) and the length of the sequence that ended this tick (0: none); initialise it to
+ * (-1, -1, 0, 0).  The ring per slot holds the repaired keypoints ring_kpts (C * P, latency + 1, 17, 2) float32 and the
+ * camera tick ring_ticks (C * P, latency + 1) int64 of its last latency + 1 frames; frame f of a sequence (from 0) is at
+ * ring position f mod (latency + 1).
+ * gast_live_delayed_inputs: gast_live_inputs' outputs (with C, num_person for n = C * P and the whole slot book (3, C,
+ *   P)), and each slot's sequence at this tick (status[c, 1] - 1, after gast_live_slots): a slot's sequence ends when
+ *   it pushes with the restart flag set, or, with max_gap >= 0, when it has not pushed for more than max_gap ticks; in
+ *   both cases only with frames pending.  A gap end sets the restart flag, so the next push starts a new sequence
+ *   (max_gap = -1: never).  tail_mask (copies * n) int32 marks the ending slots for both halves; seq[3] gets their
+ *   lengths and tail_ids (n) int64 their sequences' ids (-1 elsewhere).  A push updates seq[0..2].
+ * gast_live_delayed_end: every slot of a camera with cameras[c] != 0 (cameras (C) uint8 on the device) that has frames
+ *   pending ends its sequence: tail_mask, seq[3] and tail_ids as above; the others get no tail.  seq[2] is left to the
+ *   caller's reset.
+ * gast_live_delayed_place: one CTA per camera, three groups placed as revise_skes_real_time places them, each pose with
+ *   the repaired keypoints of its own frame (the ring's; this tick's kpts (n, 17, 2) for the newest frame):
+ *   - final: world (n, 17, 3) the pushed poses; poses (n, 17, 3) and frame (n) int64 the camera tick of the frame they
+ *     belong to, for each slot that pushed (active (n) uint8) with at least latency + 1 frames; z rebased over those
+ *     slots of the camera;
+ *   - provisional (lookahead L in [0, latency), -1 none): world_now (n, now_rows = latency - L, 17, 3) a peek's poses,
+ *     row now_rows - 1 of every pushed slot with at least L + 1 frames, the frame L behind its newest; now and now_frame
+ *     as poses and frame;
+ *   - tail: world_tail (n, latency, 17, 3) a latency-row peek of the ending slots' streams before the push; row k of a
+ *     slot is frame seq[3] - latency + k of its ended sequence when that is >= 0; tail (n, latency, 17, 3) and
+ *     tail_frame (n, latency), each row placed on its own (z rebased over its 17 joints).
+ *   Unused rows are zero and their frames -1.  Then the ring takes this tick's kpts and tick at the pushed slots' newest
+ *   positions, after every read of it.  active null (after gast_live_delayed_end): only the tails are written, and
+ *   world, world_now, kpts, poses, frame, now and now_frame are not read.
+ * Device pointers, the caller's stream, no allocation, synchronisation or host read; no atomics, calls repeat bit for
+ * bit.  Formulas in DESIGN.md §8.11. */
+int gast_live_delayed_inputs(const float* preds, const float* maxvals, const int32_t* slot_active, int32_t C,
+                             int32_t num_person, int32_t W, int32_t H, int32_t copies, int32_t max_gap,
+                             const int64_t* status, int64_t* book, int64_t* seq, float* kpts, float* scores, float* x,
+                             int32_t* fresh_mask, int32_t* active_mask, int32_t* tail_mask, uint8_t* active,
+                             int64_t* tail_ids, void* stream);
+int gast_live_delayed_end(const uint8_t* cameras, int32_t C, int32_t num_person, int32_t copies, int64_t* seq,
+                          int32_t* tail_mask, int64_t* tail_ids, void* stream);
+int gast_live_delayed_place(const float* world, const float* world_tail, const float* world_now, int32_t now_rows,
+                            const float* kpts, const uint8_t* active, const int64_t* seq, const int64_t* status,
+                            int32_t C, int32_t num_person, int32_t latency, int32_t lookahead, double width,
+                            float* ring_kpts, int64_t* ring_ticks, float* poses, int64_t* frame, float* now,
+                            int64_t* now_frame, float* tail, int64_t* tail_frame, void* stream);
+
 /* optim.Adam(amsgrad=True) (trainval.py:78,162-164) for every parameter in one launch.  table (n_chunks,4)
  * int64 on the device: {param pointer, grad pointer, offset into the flat state buffers, count <=
  * gast_adam_chunk()}.  max_exp_avg_sq null = plain Adam.  step = 1 for the first update. */
